@@ -2,12 +2,15 @@
 """bench.py -- images/sec of the CRNN forward + CTC loss hot path (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c3|c2|c2tf32|c2shape|c1shape] [--impl ours|reference]
+                    [--dump-outputs DIR]
 
 One "step" = conv stack -> BiLSTM -> logits -> CTC loss (+gradient, as warp-ctc's forward op computes it)
--> mean + L2, over one synthetic batch.  Default workload = BASELINE.json configs[2] (1xB200 bf16 tcgen05 path,
+-> mean + L2, over one synthetic batch.  Default workload = BASELINE.json configs[2] (1xH100 bf16 wgmma path,
 batch 1024, 32x256): the configuration the north-star targets are quoted on; under torchrun every rank runs the
 same per-GPU batch (weak scaling, batch-sharded, no data-path collective for the forward).
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  --dump-outputs DIR writes what the last timed step computed (logits, per-line CTC costs, the
+CTC gradient w.r.t. the logits, the total loss) as DIR/<name>.npy; the inputs are seeded, so two builds can be compared output
+for output.
 """
 import argparse
 import json
@@ -24,9 +27,9 @@ sys.path.insert(0, ROOT)
 
 WORKLOADS = {
     # name: (per-GPU batch, padded width, description)
-    "c3": (1024, 256, "BASELINE configs[2]: bf16 tcgen05 conv+LSTM path, batch 1024, 32x256, fwd+CTC"),
+    "c3": (1024, 256, "BASELINE configs[2]: bf16 wgmma conv+LSTM path, batch 1024, 32x256, fwd+CTC"),
     "c2": (256, 160, "BASELINE configs[1]: fp32-class CRNN fwd+CTC-loss (split-bf16 operands x3, f32 accumulate/elementwise), batch 256, 32x160"),
-    "c2tf32": (256, 160, "BASELINE configs[1]: fp32 CRNN fwd+CTC-loss on tcgen05 kind::tf32 operands (f32 accumulate/elementwise), batch 256, 32x160"),
+    "c2tf32": (256, 160, "BASELINE configs[1]: fp32 CRNN fwd+CTC-loss on tf32 wgmma operands (f32 accumulate/elementwise), batch 256, 32x160"),
     "c2shape": (256, 160, "BASELINE configs[1] shapes (batch 256, 32x160) on the bf16 path"),
     "c1shape": (32, 100, "BASELINE configs[0] shapes (batch 32, 32x100)"),
 }
@@ -38,11 +41,12 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], bf16_burst=d["bf16_tflops"], bf16_sustained=d["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, bf16_burst=1590.0, bf16_sustained=1400.0, src="fallback")
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- an upper bound, not a measured rate
+    return dict(hbm=3350.0, bf16_burst=989.0, bf16_sustained=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -193,10 +197,12 @@ def main():
     ap.add_argument("--no-sync-bn", action="store_true", help="N>1: per-replica BatchNorm statistics (round-1 behaviour)")
     ap.add_argument("--no-peer-memory", action="store_true", help="N>1: exchange the BN sums through NCCL instead of peer memory")
     ap.add_argument("--overlap", action="store_true", help="N>1: all-reduce merged gradient buckets on a side stream during the backward "
-                                                           "(default: one all-reduce after it; measured faster, profiles/r2_scaling.md)")
+                                                           "(default: one all-reduce after it)")
     ap.add_argument("--sync-bn-forward", action="store_true", help="N>1: global-batch BN also in the forward-only metric (default: replicas)")
     ap.add_argument("--bucket-mb", type=float, default=8.0, help="N>1: merge announced gradient ranges until this many MB are ready")
     ap.add_argument("--sm-reserve", type=int, default=8, help="N>1 with overlap: SMs the persistent backward kernels leave to the collectives")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's logits, costs, CTC gradient and loss as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -295,6 +301,12 @@ def main():
     sync_all()
     ms_total = e0.elapsed_time(e1)
     loss_val = float(loss.item())
+    if args.dump_outputs and rank == 0:
+        # what a caller of the timed path receives from its last step; [T, N, 64] f32 x 2 is 33 MB at c3, under the 64 MB cap
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in (("logits", logits), ("costs", costs), ("grad", grad)):
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), arr.detach().float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "loss.npy"), np.asarray([loss_val], dtype=np.float64))
     nst = model.lib.crnn_profile_num_stages()
     buf = (np.zeros((K, nst), dtype=np.float32))
     nf = c_int()
@@ -461,23 +473,16 @@ def main():
         dom = max((n for n in stage_names if n in flops and n != "conv1_pool1" and n != "lstm_recurrence"),
                   key=lambda n: stages[n]["ms"])
         ach = flops[dom] / (max(stages[dom]["ms"], 1e-9) * 1e-3) / 1e12
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")
-        if os.path.exists(tp) and args.workload == "c3":
-            traffic = json.load(open(tp))["kernels"].get(dom, {}).get("traffic_bytes")
         roofline = {"kernel": f"gemm_kernel<{dom}>", "bound": "tensor", "achieved": round(ach, 1), "peak": peaks["bf16_sustained"],
-                    "unit": "TFLOP/s", "frac": round(ach / peaks["bf16_sustained"], 3), "traffic": traffic,
-                    "traffic_note": "DRAM read+write bytes of one launch from the committed ncu --set full capture (profiles/r2_ncu_traffic.json); "
-                                    "algorithmic bytes of conv4_2 = 268 MB in + 4.7 MB weights + 268 MB out",
-                    "peak_source": f"MEASURED_PEAKS.json bf16_tflops_sustained ({peaks['src']}); kernel timed inside a long step",
+                    "unit": "TFLOP/s", "frac": round(ach / peaks["bf16_sustained"], 3), "traffic": None,
+                    "traffic_note": "algorithmic bytes of conv4_2 = 268 MB in + 4.7 MB weights + 268 MB out",
+                    "peak_source": f"bf16 sustained peak ({peaks['src']}); kernel timed inside a long step",
                     "whole_step_tflops": round(N * GFLOP_PER_IMG(W) / ms_step, 1),
-                    # the same achieved figure against the BURST cuBLAS number of the same file (a frac above 1 against the sustained
-                    # one means: this kernel, inside the step, runs faster than cuBLAS does in a 4 s back-to-back loop on this box)
                     "peak_burst": peaks["bf16_burst"], "frac_of_burst": round(ach / peaks["bf16_burst"], 3)}
         line = {
             "metric": "text-line images/sec (fwd+CTC loss)", "value": round(value, 1), "unit": "images/s", "n_gpus": world,
             "steps": K, "warmup": Wm, "ms_per_step": round(ms_step, 4), "higher_is_better": True, "scaling": "weak",
-            "vs_baseline": None, "dtype": {"f32": "f32 (bf16x3 split operands, f32 accumulate)", "tf32": "tf32 (kind::tf32 operands, f32 accumulate)"}.get(cdt, "bf16"),
+            "vs_baseline": None, "dtype": {"f32": "f32 (bf16x3 split operands, f32 accumulate)", "tf32": "tf32 (tf32 operands, f32 accumulate)"}.get(cdt, "bf16"),
             "data": "synthetic",
             "config": {"workload": desc, "batch_per_gpu": N, "global_batch": N * world, "width": W, "T": T,
                        "parallelism": (f"dp{world}: batch sharded over ranks; BatchNorm over the GLOBAL batch -- 2 exchanges of 8 KB per forward, "
@@ -485,7 +490,7 @@ def main():
                                        if (dp is not None and args.sync_bn_forward and not args.no_sync_bn)
                                        else f"dp{world}: independent replicas for forward + CTC (each BatchNorm over its own batch of {N}); "
                                             f"the train_step entry shards ONE global batch (global-batch BN, gradient all-reduce)"),
-                       "l2": f"rotating {nrot} distinct input batches ({nrot * N * W * 32 * 4 / 1e6:.0f} MB > 126 MB L2); "
+                       "l2": f"rotating {nrot} distinct input batches ({nrot * N * W * 32 * 4 / 1e6:.0f} MB > 50 MB L2); "
                              f"per-step activation traffic ~2.5 GB"},
             "loss": round(loss_val, 5),
             "e2e": {"value": round(e2e_value, 1), "unit": "images/s", "h2d_bytes_per_step": h2d_b,
@@ -498,25 +503,25 @@ def main():
                     "loss": float(e2e_loss),
                     "variants": {
                         "feeder_copy_inside_own_step": {"value": round(world * N / (ms_feed_instep / Ke / 1e3), 1),
-                                                        "what": "same feeder without the device prefetch: the chunked H2D copy overlaps only its own step's conv front end (the r2 mid-round e2e)"},
+                                                        "what": "same feeder without the device prefetch: the chunked H2D copy overlaps only its own step's conv front end"},
                         "fresh_pageable_array_every_step": {"value": round(world * N / (ms_fresh / Ke / 1e3), 1), "path": fresh_path,
                                                             "what": "np.array(...) built per step as reference train.py:119-125 does; staged through pinned memory"},
                         "refed_host_buffers": {"value": round(world * N / (ms_refed / Ke / 1e3), 1),
                                                "what": "round-1 e2e: the same host buffers re-fed (page-locked in place on re-sighting)"}}},
-            "gpu_launches": K * 16,      # per step: conv1, 8 tcgen05 GEMMs, 2x(bn finalize + apply), persistent LSTM, CTC, loss
+            "gpu_launches": K * 16,      # per step: conv1, 8 wgmma GEMMs, 2x(bn finalize + apply), persistent LSTM, CTC, loss
             "roofline": roofline, "stages": stages, "clocks": clocks,
         }
         if f32_path:
             # no per-stage events on this path: the whole step against the tensor peak of a 3-product contraction
             wt = N * GFLOP_PER_IMG(W) / ms_step
             div = 2.0 if cdt == "tf32" else 3.0
-            line["roofline"] = {"kernel": ("whole step (gemm_kernel kind::tf32 + f32 elementwise passes + per-step LSTM launches)" if cdt == "tf32" else
+            line["roofline"] = {"kernel": ("whole step (gemm_kernel tf32 + f32 elementwise passes + per-step LSTM launches)" if cdt == "tf32" else
                                            "whole step (gemm_kernel x3 products + f32 elementwise passes + per-step LSTM launches)"), "bound": "tensor",
                                 "achieved": round(wt, 1), "peak": round(peaks["bf16_sustained"] / div, 1), "unit": "TFLOP/s",
                                 "frac": round(wt / (peaks["bf16_sustained"] / div), 3), "traffic": None,
-                                "peak_source": ("MEASURED_PEAKS.json bf16_tflops_sustained / 2 (kind::tf32 issues at half the kind::f16 rate; no tf32 figure is measured)"
+                                "peak_source": (f"bf16 sustained peak ({peaks['src']}) / 2 (tf32 issues at half the bf16 rate; no tf32 figure is measured)"
                                                 if cdt == "tf32" else
-                                                "MEASURED_PEAKS.json bf16_tflops_sustained / 3 (each fp32-class product is three bf16 MMAs); "
+                                                f"bf16 sustained peak ({peaks['src']}) / 3 (each fp32-class product is three bf16 MMAs); "
                                                 "achieved counts the ALGORITHMIC flops once")}
             line.pop("stages", None)
             line["gpu_launches"] = K * (1 + 2 * 6 + 4 + 2 + 2 * T + 4)
@@ -540,8 +545,7 @@ def main():
             line["cpu_baseline"]["host_cpus"] = os.cpu_count()
             line["cpu_baseline"]["threads_note"] = "cores = torch threads that ran fastest on this host (ladder 8/16/32/64/all); host_cpus = os.cpu_count()"
             # BASELINE metric, second half ("CTC-loss delta vs ref"): a FRESH inference-mode model with the reference initialisers
-            # (VERDICT r1 weak #1: the round-1 figure was taken on a model that had already run 13 Adam steps) against the fp64
-            # oracle on the same seeded 32x256 samples, three seeds.
+            # (not one that has already taken optimizer steps) against the fp64 oracle on the same seeded 32x256 samples, three seeds.
             try:
                 line["ctc_loss_delta"] = ctc_loss_delta(engine, synthetic, torch, dev, W, sn, compute_dtype=cdt)
             except Exception as e:      # never lose the bench line over the side statistic

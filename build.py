@@ -1,4 +1,4 @@
-"""In-tree build of libcrnnctc.so (sm_100a only; nvcc cross-compiles without a GPU)."""
+"""In-tree build of libcrnnctc.so (sm_90a only; nvcc cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -7,7 +7,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(ROOT, "lstm_ctc_ocr_b200", "csrc")
 OUT = os.path.join(ROOT, "lstm_ctc_ocr_b200", "libcrnnctc.so")
 SOURCES = ["ctc.cu", "kernels.cu", "model.cu", "backward_kernels.cu", "backward.cu", "forward_x3.cu", "peer.cu", "beam.cpp"]
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-I/usr/local/cuda/include"]
 
 
@@ -37,7 +37,7 @@ def build(force=False, verbose=False):
             sys.stderr.write(out)
         if p.returncode != 0:
             raise RuntimeError(f"nvcc failed on {src}")
-    cmd = [nvcc, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
+    cmd = [nvcc, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
     subprocess.check_call(cmd)
     return OUT
 

@@ -1,5 +1,5 @@
 /*
- * crnn_ctc.h -- C ABI of libcrnnctc.so: the B200 (sm_100a) CRNN+CTC hot path that stands
+ * crnn_ctc.h -- C ABI of libcrnnctc.so: the H100 (sm_90a) CRNN+CTC hot path that stands
  * behind the model/solver API of ilovin/lstm_ctc_ocr.
  *
  * The reference has no C ABI of its own (it is pure Python on TensorFlow 1.0.1 + the
@@ -28,7 +28,7 @@ enum crnn_status {
   CRNN_INVALID_VALUE = 1,     /* bad shape / length / null pointer */
   CRNN_CUDA_ERROR = 2,        /* a CUDA runtime/driver call failed; see crnn_last_error() */
   CRNN_NOT_BOUND = 3,         /* model used before crnn_model_bind() */
-  CRNN_UNSUPPORTED = 4,       /* shape outside what the sm_100a kernels implement */
+  CRNN_UNSUPPORTED = 4,       /* shape outside what the sm_90a kernels implement */
   CRNN_WORKSPACE_TOO_SMALL = 5
 };
 
@@ -91,12 +91,12 @@ typedef struct crnn_config {
   int   num_hid;        /* cfg.TRAIN.NUM_HID = 512    (lib/lstm/config.py:48) */
   float bn_eps;         /* 1e-3  tf.contrib.layers.batch_norm default */
   float weight_decay;   /* cfg.TRAIN.WEIGHT_DECAY (lstm/lstm.yml:13 -> 1e-5) */
-  int   compute_dtype;  /* 1 = bf16 operands / f32 accumulate (tcgen05 kind::f16): the throughput path, forward + backward.
-                         * 2 = f32-class: every operand split into bf16 hi + bf16 lo, three tcgen05 products per term, f32
+  int   compute_dtype;  /* 1 = bf16 operands / f32 accumulate (wgmma bf16): the throughput path, forward + backward.
+                         * 2 = f32-class: every operand split into bf16 hi + bf16 lo, three bf16 products per term, f32
                          *     accumulate and f32 elementwise math (the reference computes in fp32, LSTM_train.py:10);
                          *     forward + CTC only (BASELINE configs[1])
-                         * 3 = tf32: the same forward-only orchestration on tcgen05 kind::tf32 operands (f32 tensors, rounded to
-                         *     nearest tf32 where produced; 10-bit mantissa, one pass over K at half the kind::f16 rate) */
+                         * 3 = tf32: the same forward-only orchestration on tf32 wgmma operands (f32 tensors, rounded to
+                         *     nearest tf32 where produced; 10-bit mantissa, one pass over K at half the bf16 rate) */
 } crnn_config;
 
 int     crnn_model_create(const crnn_config* cfg, crnn_model** out);

@@ -1,7 +1,7 @@
 // Backward pass + optimizer orchestration: what tf.gradients / clip_by_global_norm / AdamOptimizer.apply_gradients do in
-// the reference's train_op (lib/lstm/train.py:73-83), as hand-written sm_100a kernels.
-//   data gradients   : K-major tcgen05 GEMMs (csrc/gemm.cuh) with transformed weights
-//   weight gradients : MN-major "TN" tcgen05 GEMMs with split-K f32 reduction (csrc/gemm_tn.cuh)
+// the reference's train_op (lib/lstm/train.py:73-83), as hand-written sm_90a kernels.
+//   data gradients   : K-major wgmma GEMMs (csrc/gemm.cuh) with transformed weights
+//   weight gradients : MN-major "TN" wgmma GEMMs with split-K f32 reduction (csrc/gemm_tn.cuh)
 //   BPTT             : persistent cluster kernel (csrc/lstm_bwd.cuh)
 //   BN / pool / ReLU / bias / conv1 / clip+Adam : HBM-bound kernels (csrc/backward_kernels.cu)
 #include <cmath>
@@ -38,11 +38,6 @@ extern "C" int crnn_model_set_training(crnn_model* m, int flag) {
     CRNN_TRY(make_tmap_2d(&m->tD_x, m->Bxb, 512, 2048, 2048, 256));
     CRNN_TRY(make_tmap_2d(&m->tD_h, m->Bhb, 512, 1024, 1024, 32));
     CRNN_TRY(make_tmap_2d(&m->tD_h256, m->Bhb, 512, 1024, 1024, 256));
-    CRNN_TRY(make_tmap_2d(&m->tDh_c42, m->Bd_c42, 512, 4608, 4608, 128));
-    CRNN_TRY(make_tmap_2d(&m->tDh_c41, m->Bd_c41, 256, 4608, 4608, 128));
-    CRNN_TRY(make_tmap_2d(&m->tDh_c32, m->Bd_c32, 256, 2304, 2304, 128));
-    CRNN_TRY(make_tmap_2d(&m->tDh_c5, m->Bd_c5, 1024, 1024, 1024, 128));
-    CRNN_TRY(make_tmap_2d(&m->tDh_x, m->Bxb, 512, 2048, 2048, 128));
     m->dirty_bwd = true;
   }
   m->training = flag != 0;
@@ -165,8 +160,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
     {  // dW_x (rows 0..511 of both [768,1024] matrices) = a5^T dz
       gemm_tn::Params p = tn_plain(512, 2048, R, G(fw + "/weights"), 1024);
       p.num_n_tiles = 8; p.lstm_cols = 1; p.dir_stride = dW;
-      if (m->use_2cta) { p.num_m_tiles = 2; CRNN_TRY((launch_gemm_tn2<gemm_tn::TN_PLAIN, 6>(pl.tT_a5, pl.tT_dz, p, sms, st))); }
-      else CRNN_TRY((launch_gemm_tn<256, gemm_tn::TN_PLAIN, 4>(pl.tT_a5, pl.tT_dz, p, sms, st)));
+      CRNN_TRY((launch_gemm_tn<256, gemm_tn::TN_PLAIN, 4>(pl.tT_a5, pl.tT_dz, p, sms, st)));
     }
     {  // dW_h forward direction: previous step = frame t-1
       gemm_tn::Params p = tn_plain(256, 1024, R, G(fw + "/weights"), 1024);
@@ -188,8 +182,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
       memset(&p, 0, sizeof(p));
       p.M = (int)R; p.num_m_tiles = (p.M + 127) / 128; p.num_n_tiles = 2; p.num_k_blocks = 32; p.kb_per_shift = 32;
       p.Nc = 512; p.out = pl.d_a5; p.ldo = 512;
-      if (m->use_2cta) CRNN_TRY((launch_gemm2<gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 6>(pl.tG_dz, m->tDh_x, p, sms, st)));
-      else CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tG_dz, m->tD_x, p, sms, st)));
+      CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tG_dz, m->tD_x, p, sms, st)));
     }
   }
   BMARK();
@@ -198,8 +191,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
   for (int r = 0; r < 2; ++r) {
     gemm_tn::Params p = tn_plain(1024, 512, R, G("conv5/weights") + (size_t)r * 1024 * 512, 512);
     p.num_n_tiles = 2; p.a_row_shift = r;
-    if (m->use_2cta) { p.num_m_tiles = 4; CRNN_TRY((launch_gemm_tn2<gemm_tn::TN_PLAIN, 6>(pl.tT_a4b, pl.tT_da5, p, sms, st))); }
-    else CRNN_TRY((launch_gemm_tn<256, gemm_tn::TN_PLAIN, 4>(pl.tT_a4b, pl.tT_da5, p, sms, st)));
+    CRNN_TRY((launch_gemm_tn<256, gemm_tn::TN_PLAIN, 4>(pl.tT_a4b, pl.tT_da5, p, sms, st)));
   }
   notify("conv5/weights", "logits/bidirectional_rnn/fw/lstm_cell/weights");
   {
@@ -207,8 +199,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
     memset(&p, 0, sizeof(p));
     p.M = (int)R; p.num_m_tiles = (p.M + 127) / 128; p.num_n_tiles = 4; p.num_k_blocks = 16; p.kb_per_shift = 8; p.row_shift_mul = -1;
     p.Nc = 1024; p.out = pl.d_a4b; p.ldo = 1024;
-    if (m->use_2cta) CRNN_TRY((launch_gemm2<gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 6>(pl.tG_da5, m->tDh_c5, p, sms, st)));
-    else CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tG_da5, m->tD_c5, p, sms, st)));
+    CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tG_da5, m->tD_c5, p, sms, st)));
   }
   BMARK();
   // ------------------------------------------------------------------ conv4_2: pool3 + ReLU + batch-stat BN backward
@@ -230,8 +221,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
   {
     gemm_tn::Params p = tn_conv(N, H2, 4, 512, 512, G("conv4_2/weights"), pl.wm4);
     p.num_n_tiles = 2;
-    if (m->use_2cta) { p.num_m_tiles = 2; CRNN_TRY((launch_gemm_tn2<gemm_tn::TN_CONV, 6>(pl.tW_a4a, pl.tW_p4b, p, sms, st))); }
-    else CRNN_TRY((launch_gemm_tn<256, gemm_tn::TN_CONV, 4>(pl.tW_a4a, pl.tW_p4b, p, sms, st)));
+    CRNN_TRY((launch_gemm_tn<256, gemm_tn::TN_CONV, 4>(pl.tW_a4a, pl.tW_p4b, p, sms, st)));
   }
   notify("conv4_2/weights", "conv5/weights");
   BMARK();
@@ -241,11 +231,9 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
     gemm::Params p = conv_params(N, H2, 4, 512, 512, 256, nullptr, pl.d_pre4a, pl.mg4);
     p.mask = pl.a4a_pre; p.bnp = pl.bn; p.stats = sums41;
     if (m->bn_red_fused) {
-      if (m->use_2cta) CRNN_TRY((launch_gemm2<gemm::A_CONV3, gemm::EPI_CONV_STORE_BNRED, 6>(pl.tG_p4b, m->tDh_c42, p, sms, st)));
-      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE_BNRED, 4>(pl.tG_p4b, m->tD_c42, p, sms, st)));
+      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE_BNRED, 4>(pl.tG_p4b, m->tD_c42, p, sms, st)));
     } else {
-      if (m->use_2cta) CRNN_TRY((launch_gemm2<gemm::A_CONV3, gemm::EPI_CONV_STORE, 6>(pl.tG_p4b, m->tDh_c42, p, sms, st)));
-      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE, 4>(pl.tG_p4b, m->tD_c42, p, sms, st)));
+      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE, 4>(pl.tG_p4b, m->tD_c42, p, sms, st)));
     }
   }
   BMARK();
@@ -259,15 +247,13 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
   {
     gemm_tn::Params p = tn_conv(N, H2, 4, 256, 512, G("conv4_1/weights"), pl.wm4);
     p.num_n_tiles = 2;
-    if (m->use_2cta) { p.num_m_tiles = 1; CRNN_TRY((launch_gemm_tn2<gemm_tn::TN_CONV, 6>(pl.tW_a3p, pl.tW_p4a, p, sms, st))); }
-    else CRNN_TRY((launch_gemm_tn<256, gemm_tn::TN_CONV, 4>(pl.tW_a3p, pl.tW_p4a, p, sms, st)));
+    CRNN_TRY((launch_gemm_tn<256, gemm_tn::TN_CONV, 4>(pl.tW_a3p, pl.tW_p4a, p, sms, st)));
   }
   notify("conv4_1/weights", "conv4_2/weights");
   BMARK();
   {
     gemm::Params p = conv_params(N, H2, 4, 512, 256, 256, nullptr, pl.d_a3p, pl.mg4);
-    if (m->use_2cta) CRNN_TRY((launch_gemm2<gemm::A_CONV3, gemm::EPI_CONV_STORE, 6>(pl.tG_p4a, m->tDh_c41, p, sms, st)));
-    else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE, 4>(pl.tG_p4a, m->tD_c41, p, sms, st)));
+    CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE, 4>(pl.tG_p4a, m->tD_c41, p, sms, st)));
   }
   BMARK();
   // ------------------------------------------------------------------ conv3_2: 1x2 pool + ReLU backward
@@ -278,8 +264,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
   {
     gemm_tn::Params p = tn_conv(N, H2, 8, 256, 256, G("conv3_2/weights"), pl.wm3);
     p.num_n_tiles = 1;
-    if (m->use_2cta) { p.num_m_tiles = 1; CRNN_TRY((launch_gemm_tn2<gemm_tn::TN_CONV, 6>(pl.tW_a3, pl.tW_p32, p, sms, st))); }
-    else CRNN_TRY((launch_gemm_tn<256, gemm_tn::TN_CONV, 4>(pl.tW_a3, pl.tW_p32, p, sms, st)));
+    CRNN_TRY((launch_gemm_tn<256, gemm_tn::TN_CONV, 4>(pl.tW_a3, pl.tW_p32, p, sms, st)));
   }
   notify("conv3_2/weights", "conv4_1/weights");
   BMARK();
@@ -288,11 +273,9 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
     gemm::Params p = conv_params(N, H2, 8, 256, 256, 256, nullptr, pl.d_pre31, pl.mg3);
     p.mask = pl.a3;
     if (m->relu_mask_fused) {
-      if (m->use_2cta) CRNN_TRY((launch_gemm2<gemm::A_CONV3, gemm::EPI_CONV_STORE_MASK, 6>(pl.tG_p32, m->tDh_c32, p, sms, st)));
-      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE_MASK, 4>(pl.tG_p32, m->tD_c32, p, sms, st)));
+      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE_MASK, 4>(pl.tG_p32, m->tD_c32, p, sms, st)));
     } else {
-      if (m->use_2cta) CRNN_TRY((launch_gemm2<gemm::A_CONV3, gemm::EPI_CONV_STORE, 6>(pl.tG_p32, m->tDh_c32, p, sms, st)));
-      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE, 4>(pl.tG_p32, m->tD_c32, p, sms, st)));
+      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE, 4>(pl.tG_p32, m->tD_c32, p, sms, st)));
     }
   }
   BMARK();
@@ -323,9 +306,9 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
   CRNN_TRY(launch_colsum_masked_bf16(pl.d_a2, pl.a2, (long long)N * H2 * 8, 128, G("conv2/biases"), st));
   BMARK();
   if (m->conv2_wgrad_swap) {
-    // operands swapped (r2): A = d(pre-activation) [positions x 128 co] on the M side, B = a1 with FOUR tap-shifted 64-channel boxes
+    // operands swapped: A = d(pre-activation) [positions x 128 co] on the M side, B = a1 with FOUR tap-shifted 64-channel boxes
     // per 256-column N tile (columns = (tap, ci)); 3 N tiles cover the 9 taps.  N = 256 runs the MMA at full rate where the
-    // Cout = 128 N tile of the straight formulation halves it (0.66 ms for 309 GFLOP).
+    // Cout = 128 N tile of the straight formulation halves it.
     gemm_tn::Params p = tn_conv(N, H1, 16, 64, 128, G("conv2/weights"), pl.wm2);
     p.tap_pack_n = 1; p.num_taps = 1; p.num_m_tiles = 1; p.num_n_tiles = 3; p.M = 128; p.N = 9 * 64; p.ldo = 128; p.tap_stride = 0;
     CRNN_TRY((launch_gemm_tn<256, gemm_tn::TN_CONV, 4>(pl.tW_p2, pl.tW_a1, p, sms, st)));
@@ -396,7 +379,7 @@ extern "C" int crnn_last_grad_norm(crnn_model* m, float grad_mul, float* out, cr
 extern "C" int crnn_test_gemm_tn_bf16(const void* A, const void* B, float* D, int M, int Ncols, int K, int block_n,
                                       int k_splits, crnn_stream_t stream) {
   if (!A || !B || !D || M <= 0 || Ncols <= 0 || K <= 0 || (M % 8) || (Ncols % 8)) return crnn_fail(CRNN_INVALID_VALUE, "test_gemm_tn: bad args");
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   CUtensorMap ta, tb;

@@ -109,8 +109,8 @@ __global__ void __launch_bounds__(256) colsum_bf16_kernel(const __nv_bfloat16* _
   }
 }
 
-// ---- BatchNorm (+ReLU, + optional 1x2 max-pool) backward, pass 1 (sums only -- r2: the routed gradient dy is NOT written here
-// any more; pass 2 re-derives it from the same two inputs, which saves one 268 MB write + one 268 MB read per BN layer):
+// ---- BatchNorm (+ReLU, + optional 1x2 max-pool) backward, pass 1 (sums only -- the routed gradient dy is NOT written here;
+// pass 2 re-derives it from the same two inputs, which saves one 268 MB write + one 268 MB read per BN layer):
 //   dy = routed upstream gradient at the pre-BN resolution, masked by ReLU;  sums[c] += dy, sums[C + c] += dy * xhat
 // POOL = true (conv4_2 / pool3): dout is [P, Wp/2.., C] pooled; x_pre is [P*2 positions..]; the max is re-derived from
 // the saved pre-BN tensor (first position wins ties).  POOL = false (conv4_1): dout has the same shape as x_pre.
@@ -128,8 +128,8 @@ __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const uint4* __restr
     sc[i] = bn[c + i]; sh[i] = bn[C + c + i]; mu[i] = bn[2 * C + c + i]; is[i] = bn[3 * C + c + i];
     s1[i] = 0.f; s2[i] = 0.f;
   }
-  // software-pipelined: the next position's 16-byte loads are in flight while this one is reduced (r2 ncu: 45 % of DRAM peak at
-  // 30 % occupancy with one batch of loads per iteration -- latency-bound)
+  // software-pipelined: the next position's 16-byte loads are in flight while this one is reduced (with one batch of loads
+  // per iteration the pass is latency-bound at this occupancy)
   const size_t pstep = (size_t)gridDim.x * rows_per_block;
   size_t pos = (size_t)blockIdx.x * rows_per_block + threadIdx.x / vpc;
   uint4 qg = make_uint4(0u, 0u, 0u, 0u), qx0 = qg, qx1 = qg;
@@ -327,7 +327,7 @@ __global__ void __launch_bounds__(256) conv1_wgrad_kernel(const __nv_bfloat16* _
   const int cg = lane & 7;
   const int slot = warp * 4 + (lane >> 3);
   // accumulators as f32x2 pairs of adjacent channels: the 288 FMAs per pooled position issue as 144 FFMA2 (the 3-register scalar
-  // FFMA issues every other cycle per scheduler on sm_100 -- the same ceiling the SIMT forward conv1 hit; r2 ncu: issue-bound at 46 %)
+  // FFMA issues every other cycle per scheduler -- the same ceiling the SIMT forward conv1 hits)
   uint64_t acc2[9][4];
   float accb[8];
 #pragma unroll
@@ -545,12 +545,21 @@ __global__ void __launch_bounds__(256) clip_adam_kernel(float* __restrict__ para
 // ------------------------------------------------------------------------------------------------ launchers
 #define LAUNCH_CHECK() CUDA_TRY(cudaGetLastError()); return CRNN_OK
 
+// SM count of the current device: the grid-stride kernels below launch a few CTAs per SM
+static int device_sms() {
+  static int cached[64] = {0};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
+  if (cached[dev] <= 0) cudaDeviceGetAttribute(&cached[dev], cudaDevAttrMultiProcessorCount, dev);
+  return cached[dev] > 0 ? cached[dev] : 1;
+}
+
 int launch_dlogits_rows(const float* dlogits, __nv_bfloat16* rows, float* dbias, int T, int N, int H, cudaStream_t st) {
-  dlogits_rows_kernel<<<592, 256, 0, st>>>(dlogits, rows, dbias, T, N, H);
+  dlogits_rows_kernel<<<4 * device_sms(), 256, 0, st>>>(dlogits, rows, dbias, T, N, H);
   LAUNCH_CHECK();
 }
 int launch_colsum_bf16(const __nv_bfloat16* src, long long R, int C, float* out, int perm_upc, long long dir_stride, cudaStream_t st) {
-  dim3 grid(296, (C + 255) / 256);
+  dim3 grid(2 * device_sms(), (C + 255) / 256);
   colsum_bf16_kernel<<<grid, 256, 0, st>>>(src, nullptr, R, C, 0, out, perm_upc, dir_stride);
   LAUNCH_CHECK();
 }
@@ -560,14 +569,14 @@ int launch_colsum_masked_bf16(const __nv_bfloat16* src, const __nv_bfloat16* mas
   int Cv = C, Cmod = 0;
   long long Rv = R;
   if (C < 256 && 256 % C == 0 && R % (256 / C) == 0) { Cv = 256; Cmod = C; Rv = R / (256 / C); }
-  dim3 grid(296, (Cv + 255) / 256);
+  dim3 grid(2 * device_sms(), (Cv + 255) / 256);
   colsum_bf16_kernel<<<grid, 256, 0, st>>>(src, mask, Rv, Cv, Cmod, out, 0, 0);
   LAUNCH_CHECK();
 }
 int launch_bn_bwd_reduce(bool pool, const __nv_bfloat16* dout, const __nv_bfloat16* x_pre, const float* bn, double* sums,
                          size_t out_positions, int C, cudaStream_t st) {
-  if (pool) bn_bwd_reduce_kernel<true><<<592, 256, 0, st>>>((const uint4*)dout, (const uint4*)x_pre, nullptr, bn, sums, out_positions, C);
-  else bn_bwd_reduce_kernel<false><<<592, 256, 0, st>>>((const uint4*)dout, (const uint4*)x_pre, nullptr, bn, sums, out_positions, C);
+  if (pool) bn_bwd_reduce_kernel<true><<<4 * device_sms(), 256, 0, st>>>((const uint4*)dout, (const uint4*)x_pre, nullptr, bn, sums, out_positions, C);
+  else bn_bwd_reduce_kernel<false><<<4 * device_sms(), 256, 0, st>>>((const uint4*)dout, (const uint4*)x_pre, nullptr, bn, sums, out_positions, C);
   LAUNCH_CHECK();
 }
 // dx = BN/ReLU(/pool) backward of dout; out_positions = positions of dout (pooled positions when pool); dx may alias dout when !pool
@@ -597,32 +606,32 @@ int launch_unpool_relu_bwd(int win, const __nv_bfloat16* dpool, const __nv_bfloa
 int launch_conv1_wgrad(const __nv_bfloat16* d_a1, const __nv_bfloat16* a1, const uint8_t* am1, const float* data, float* dW, float* db,
                        int N, int W, cudaStream_t st) {
   const int tiles = N * (((W >> 1) + C1W_ROWS - 1) / C1W_ROWS);
-  conv1_wgrad_kernel<<<tiles < 296 ? tiles : 296, 256, 0, st>>>(d_a1, a1, am1, data, dW, db, N, W);
+  conv1_wgrad_kernel<<<tiles < 2 * device_sms() ? tiles : 2 * device_sms(), 256, 0, st>>>(d_a1, a1, am1, data, dW, db, N, W);
   LAUNCH_CHECK();
 }
 int launch_dgrad_weight(const float* w, __nv_bfloat16* bd, int Cin, int Cout, cudaStream_t st) {
-  dgrad_weight_kernel<<<592, 256, 0, st>>>(w, bd, Cin, Cout);
+  dgrad_weight_kernel<<<4 * device_sms(), 256, 0, st>>>(w, bd, Cin, Cout);
   LAUNCH_CHECK();
 }
 int launch_conv5_dgrad_weight(const float* w, __nv_bfloat16* bd, cudaStream_t st) {
-  conv5_dgrad_weight_kernel<<<592, 256, 0, st>>>(w, bd);
+  conv5_dgrad_weight_kernel<<<4 * device_sms(), 256, 0, st>>>(w, bd);
   LAUNCH_CHECK();
 }
 int launch_lstm_bwd_weight(const float* w_fw, const float* w_bw, __nv_bfloat16* bxb, __nv_bfloat16* bhb, int upc, cudaStream_t st) {
-  lstm_bwd_weight_kernel<<<592, 256, 0, st>>>(w_fw, w_bw, bxb, bhb, upc);
+  lstm_bwd_weight_kernel<<<4 * device_sms(), 256, 0, st>>>(w_fw, w_bw, bxb, bhb, upc);
   LAUNCH_CHECK();
 }
 int launch_cast_bf16(const float* src, __nv_bfloat16* dst, size_t n, cudaStream_t st) {
-  cast_bf16_kernel<<<148, 256, 0, st>>>(src, dst, n);
+  cast_bf16_kernel<<<device_sms(), 256, 0, st>>>(src, dst, n);
   LAUNCH_CHECK();
 }
 int launch_grad_finish(float* grads, const float* params, const WdSegs& segs, float wd, long long total, double* sumsq, cudaStream_t st) {
   CUDA_TRY(cudaMemsetAsync(sumsq, 0, sizeof(double), st));
-  grad_finish_kernel<<<592, 256, 0, st>>>(grads, params, segs, wd, total, sumsq);
+  grad_finish_kernel<<<4 * device_sms(), 256, 0, st>>>(grads, params, segs, wd, total, sumsq);
   LAUNCH_CHECK();
 }
 int launch_clip_adam(float* params, const float* grads, float* m, float* v, const double* sumsq, float grad_mul, float clip, float lr_t,
                      float b1, float b2, float eps, long long total, cudaStream_t st) {
-  clip_adam_kernel<<<592, 256, 0, st>>>(params, grads, m, v, sumsq, grad_mul, clip, lr_t, b1, b2, eps, total);
+  clip_adam_kernel<<<4 * device_sms(), 256, 0, st>>>(params, grads, m, v, sumsq, grad_mul, clip, lr_t, b1, b2, eps, total);
   LAUNCH_CHECK();
 }

@@ -25,8 +25,7 @@ int crnn_fail(int status, const char* fmt, ...);   // records crnn_last_error(),
 
 // ---- saved LSTM state (training): written by the forward recurrence kernels, read by the BPTT kernels.  Both access it with
 // lane = sample row of a 128-row batch tile, so the layout keeps the 128 rows of a tile adjacent: a warp's 32 lanes store / load
-// 32 consecutive 16-byte vectors (one 512-byte segment) instead of 32 sectors that are T*2 KB apart (r2: the un-coalesced saves
-// doubled the training-mode recurrence, 0.41 -> 0.82 ms).
+// 32 consecutive 16-byte vectors (one 512-byte segment) instead of 32 sectors that are T*2 KB apart.
 //   gates [dir*tiles + tile][step][gate i,j,f,o][unit/8 = 32 chunks][row 128][8 bf16]      (post-activation gate values)
 //   csave [dir*tiles + tile][step][unit/4 = 64 chunks][row 128][4 f32]                      (cell state after the step)
 constexpr size_t LSTM_GCHUNK_STRIDE = 128 * 8;                 // elements between unit chunks of 8

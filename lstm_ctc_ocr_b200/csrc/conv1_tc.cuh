@@ -1,11 +1,11 @@
 // conv1 (3x3 SAME, 1 -> 64, bias, ReLU) + pool1 (2x2/2) on the tensor cores.   lib/networks/LSTM_train.py:24-25
 //
 // The SIMT kernel (kernels.cu) sits on the FP32 FMA ceiling of the chip (288 FMAs per pooled output vector; FFMA2 packs
-// them into 144 instructions but not into fewer pipe cycles): 0.25 ms for 9.7 GFLOP.  As a GEMM the layer is tiny
+// them into 144 instructions but not into fewer pipe cycles).  As a GEMM the layer is tiny
 // (K = 9) -- what costs is moving 8.4 M positions x 64 channels through an epilogue -- so the operands are arranged for the
 // cheapest epilogue:
 //
-//   D[128 x 256] = A[128 x 64] * B[256 x 64]^T        (bf16 in, f32 accumulate in TMEM, four K = 16 tcgen05.mma per tile)
+//   D[128 x 256] = A[128 x 64] * B[256 x 64]^T        (bf16 in, f32 accumulate, four K = 16 wgmma per warpgroup and tile)
 //     A = [ W' 0 ; 0 W' ] rows 0..63  : the 64 filters against K columns 0..31
 //                         rows 64..127: the same filters against K columns 32..63
 //     B row j             K 0..31  = the 3x3 patch of position j of image rows h0..h0+7   (j = hl*32 + w)
@@ -16,24 +16,24 @@
 // f32 fidelity on a bf16 pipe: pixels and taps are split x = xh + xl, w = wh + wl (bf16 high part + bf16 remainder) and the 32
 // K columns of a patch hold  [xh (9) 0 | xl (9) 0 | xh (9) 0 | 0 0]  against  [wh 0 | wh 0 | wl 0 | 0 0]  (10 columns per part, so
 // every bf16x2 word is one F2FP of two neighbouring taps):  xh*wh + xl*wh + xh*wl reproduces the
-// f32 product to ~2^-17 (the dropped xl*wl term), so the layer keeps the numerics of the f32 SIMT kernel it replaces
-// (measured against the fp64 oracle: 2.5e-3 of max |out| either way, all of it the bf16 rounding of the OUTPUT; plain bf16
-// operands would have been 4.3e-3).
+// f32 product to ~2^-17 (the dropped xl*wl term), so the layer keeps the numerics of the f32 SIMT kernel it replaces: what is
+// left of the error is the bf16 rounding of the OUTPUT.
 //
 // Both operands are written by threads (im2col in shared memory, no TMA): no-swizzle K-major layout
-// [K-chunk of 8][row][16 B] (8-row x 16-B core matrices; LBO = rows*16, SBO = 128).  Roles (448 threads): warp 0 idle after
-// setup, warp 1 MMA issuer, warps 2..9 epilogue (TMEM lane quadrant x column half), warps 10..13 im2col builders
-// (double-buffered B tile and input stage, so the build of tile i+1 overlaps the MMA + epilogue of tile i).
+// [K-chunk of 8][row][16 B] (8-row x 16-B core matrices; LBO = rows*16, SBO = 128).  Roles (384 threads): warps 0..3 im2col
+// builders (double-buffered B tile and input stage, so the build of tile i+1 overlaps the MMA + epilogue of tile i), warps
+// 4..11 = two MMA warpgroups (accumulator rows 0..63 / 64..127) and the epilogue (row quadrant x column half) reading the
+// accumulators staged in shared memory.
 #pragma once
 #include <cuda.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace conv1tc {
 
-constexpr int NUM_THREADS = 448;
-constexpr int NUM_EPI_WARPS = 8;
-constexpr int BUILD_WARP0 = 10, BUILD_THREADS = 128;
+constexpr int NUM_THREADS = 384;
+constexpr int BUILD_WARP0 = 0, BUILD_THREADS = 128;
 constexpr int KCH = 8;                           // K-chunks of 8 bf16: 4 per row set
 constexpr int A_BYTES = KCH * 128 * 16;          // [8 K-chunks][128 rows][16 B]
 constexpr int B_BYTES = KCH * 256 * 16;          // [8 K-chunks][256 rows][16 B]
@@ -41,7 +41,8 @@ constexpr int IN_ROWS = 18, IN_STRIDE = 36;      // staged input: image rows h0-
 constexpr int IN_BYTES = IN_ROWS * IN_STRIDE * 4;
 constexpr int OFF_B = A_BYTES;
 constexpr int OFF_IN = OFF_B + 2 * B_BYTES;
-constexpr int OFF_BAR = OFF_IN + 2 * IN_BYTES;
+constexpr int OFF_ACC = (OFF_IN + 2 * IN_BYTES + 15) / 16 * 16;   // staged accumulators [128][256] f32
+constexpr int OFF_BAR = OFF_ACC + 128 * 256 * 4;
 constexpr int SMEM_BYTES = OFF_BAR + 128 + 1024;
 
 // K column k (0..31) of a patch: part = k / 10 (x: hi, lo, hi | w: hi, hi, lo), tap = k % 10; tap 9 and k >= 30 are zero padding
@@ -59,7 +60,6 @@ struct Params {
 
 template <bool TRAIN>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const Params p) {
-  constexpr uint32_t IDESC = ptx::make_idesc_bf16(128, 256);
   extern __shared__ uint8_t smem_raw[];
   // aligned by OFFSET (not by casting through an integer): the pointers stay in the shared address space -> LDS/STS, not LD/ST
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -68,9 +68,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const Params p
   float* s_in = reinterpret_cast<float*>(smem + OFF_IN);
   uint64_t* b_full = reinterpret_cast<uint64_t*>(smem + OFF_BAR);   // [2]
   uint64_t* b_empty = b_full + 2;
-  uint64_t* tmem_full = b_empty + 2;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  float* acc_tile = reinterpret_cast<float*>(smem + OFF_ACC);
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_tiles = p.N * p.tiles_per_img;
@@ -78,15 +76,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const Params p
   if (warp_idx == 0 && lane == 0) {
     for (int s = 0; s < 2; ++s) {
       ptx::mbar_init(&b_full[s], BUILD_THREADS);
-      ptx::mbar_init(&b_empty[s], 1);
-      ptx::mbar_init(&tmem_full[s], 1);
-      ptx::mbar_init(&tmem_empty[s], NUM_EPI_WARPS);
+      ptx::mbar_init(&b_empty[s], 2);          // one arrive per MMA warpgroup
     }
     ptx::fence_barrier_init();
-  }
-  if (warp_idx == 1) {
-    ptx::tmem_alloc(tmem_ptr, 512);
-    ptx::tmem_relinquish();
   }
   // A = [W' 0; 0 W']: entry (chunk, row) = 16 B = 8 bf16 of K
   for (int e = threadIdx.x; e < KCH * 128; e += NUM_THREADS) {
@@ -110,37 +102,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const Params p
         make_uint4(hw[0] | (hw[1] << 16), hw[2] | (hw[3] << 16), hw[4] | (hw[5] << 16), hw[6] | (hw[7] << 16));
   }
   ptx::fence_proxy_async_smem();
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp_idx == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      int it = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        const int st = it & 1;
-        const uint32_t ph = (it >> 1) & 1;
-        ptx::mbar_wait(&tmem_empty[st], ph ^ 1);
-        ptx::mbar_wait(&b_full[st], ph);
-        ptx::tc_fence_after();
-        const uint32_t a_base = ptx::smem_u32(smem_a), b_base = ptx::smem_u32(smem_b + st * B_BYTES);
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          ptx::mma_f16_ss(tmem_base + st * 256, ptx::make_desc_k_nosw(a_base + k * 2 * 2048, 2048, 128),
-                          ptx::make_desc_k_nosw(b_base + k * 2 * 4096, 4096, 128), IDESC, k != 0);
-        ptx::tc_commit(&b_empty[st]);
-        ptx::tc_commit(&tmem_full[st]);
-      }
-    }
-    __syncwarp();
-  } else if (warp_idx >= BUILD_WARP0) {
+  if (warp_idx < BUILD_WARP0 + 4) {
     // ===================== im2col builders =====================
     const int bt = threadIdx.x - BUILD_WARP0 * 32;          // 0..127
     // staged input of a tile: image rows h0-1 .. h0+16 (zero outside the image) = 144 float4; thread bt owns entries bt and
     // bt+128.  The loads of tile i+1 are issued BEFORE tile i is built and land in shared memory after it, so their
-    // L2/HBM latency is off the per-tile critical path (one tile is only ~600 builder cycles).
+    // L2/HBM latency is off the per-tile critical path (a tile is a short piece of builder work).
     auto fetch = [&](int tile, float4 (&v)[2]) {
       const int n = tile / p.tiles_per_img;
       const int h0 = (tile - n * p.tiles_per_img) * 16;
@@ -210,10 +179,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const Params p
       ptx::mbar_arrive(&b_full[st]);
       if (nxt < num_tiles) stash(s_in + (st ^ 1) * (IN_ROWS * IN_STRIDE), pre);
     }
-  } else if (warp_idx >= 2) {
-    // ===================== epilogue: lane = (row set, channel), columns = positions =====================
+  } else {
+    // ===================== MMA (rows wgi*64 ..) + epilogue: row = (row set, channel), columns = positions =====================
+    const int wgi = (warp_idx >> 2) - 1;
+    const bool arriver = (warp_idx & 3) == 0 && lane == 0;
     const int q = warp_idx & 3;
-    const int half = (warp_idx - 2) >> 2;                    // columns half*128 ..: image rows half*4 .. half*4+3 of the set
+    const int half = (warp_idx - 4) >> 2;                    // columns half*128 ..: image rows half*4 .. half*4+3 of the set
     const int set = q >> 1;
     const int c = (q & 1) * 32 + lane;
     const float bias = __ldg(p.bias + c), nbias = -bias;
@@ -223,15 +194,29 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const Params p
       const int st = it & 1;
       const int n = tile / p.tiles_per_img;
       const int h0 = (tile - n * p.tiles_per_img) * 16;
-      ptx::mbar_wait(&tmem_full[st], (it >> 1) & 1);
-      ptx::tc_fence_after();
-      const uint32_t tbase = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + st * 256 + half * 128;
+      ptx::mbar_wait(&b_full[st], (it >> 1) & 1);
+      {
+        float d[128];
+        const uint32_t a_base = ptx::smem_u32(smem_a) + wgi * 64 * 16, b_base = ptx::smem_u32(smem_b + st * B_BYTES);
+        wg::fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wg::mma_bf16<256>(d, ptx::make_desc_k_nosw(a_base + k * 2 * 2048, 2048, 128), ptx::make_desc_k_nosw(b_base + k * 2 * 4096, 4096, 128),
+                            k != 0);
+        wg::commit();
+        wg::wait<0>();
+        wg::fence_operand(d);
+        if (arriver) ptx::mbar_arrive(&b_empty[st]);
+        ptx::bar_sync(1, 256);                               // the previous tile's epilogue reads are done
+        ptx::acc_store<256, 256>(acc_tile, d, wgi * 64);
+        ptx::bar_sync(1, 256);
+      }
+      const int c0 = half * 128, arow = q * 32 + lane;
 #pragma unroll 1
       for (int pr = 0; pr < 2; ++pr) {
         uint32_t v0[32], v1[32];
-        ptx::tmem_ld_32x32b_x32(tbase + pr * 64, v0);        // image row h   (32 columns)
-        ptx::tmem_ld_32x32b_x32(tbase + pr * 64 + 32, v1);   // image row h+1
-        ptx::tmem_ld_wait();
+        ptx::acc_ld<256, 32>(acc_tile, arow, c0 + pr * 64, v0);        // image row h   (32 columns)
+        ptx::acc_ld<256, 32>(acc_tile, arow, c0 + pr * 64 + 32, v1);   // image row h+1
         const int h = h0 + set * 8 + half * 4 + 2 * pr;
         if (h < p.W) {                                        // W is even: both rows of a window are inside or outside together
           const size_t off = (((size_t)n * Hp + (h >> 1)) * 16) * 64 + c;
@@ -241,10 +226,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const Params p
             const float x10 = __uint_as_float(v1[2 * pw]), x11 = __uint_as_float(v1[2 * pw + 1]);
             if (!TRAIN) {
               // relu(max4 + b) == max(max4, -b) + b exactly (the same FADD on the same operand, or (-b) + b = 0): two 3-input
-              // maxima and one add instead of three maxima, an add and a max -- the kernel is ALU-issue bound (ncu: 52 %)
-              float m3, m4;
-              asm("max.f32 %0, %1, %2, %3;" : "=f"(m3) : "f"(x00), "f"(x01), "f"(x10));
-              asm("max.f32 %0, %1, %2, %3;" : "=f"(m4) : "f"(m3), "f"(x11), "f"(nbias));
+              // maxima and one add instead of three maxima, an add and a max -- the epilogue is ALU-issue bound
+              const float m4 = fmaxf(fmaxf(fmaxf(x00, x01), fmaxf(x10, x11)), nbias);
               const float o = m4 + bias;
               reinterpret_cast<unsigned short*>(p.out)[off + (size_t)pw * 64] = (unsigned short)ptx::pack_bf16x2(o, o);   // F2FP (ALU), not F2F (XU)
             } else {
@@ -262,17 +245,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const Params p
           }
         }
       }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&tmem_empty[st]);
     }
-  }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, 512);
   }
 }
 

@@ -3,11 +3,11 @@
 //   dW1[r][s][co] = sum over pre-pool positions (h, w) of  data[h+r-1][w+s-1] * G[h][w][co]        db1[co] = sum G
 //   G = the pooled gradient d_a1 routed to the arg-max position of its 2x2 window where a1 > 0, zero elsewhere.
 //
-// The SIMT kernel (backward_kernels.cu) spends 36 masked FMAs per pooled (position, channel) and sat at 0.49 ms; as a GEMM the
+// The SIMT kernel (backward_kernels.cu) spends 36 masked FMAs per pooled (position, channel); as a GEMM the
 // layer is a 64 x 9 output with K = 8.4 M positions, i.e. nothing for the tensor pipe -- what costs is building the operands,
 // so they are arranged for the cheapest build:
 //
-//   D[128 x 64] += A[128 x K] * B[64 x K]^T     (bf16 in, f32 accumulate in TMEM for the WHOLE kernel: one epilogue per CTA)
+//   D[128 x 64] += A[128 x K] * B[64 x K]^T     (bf16 in, f32 accumulate in registers for the WHOLE kernel: one epilogue per CTA)
 //     K index = (pooled position, window slot dy*2+dx): the unpooled gradient is never materialised, a pooled value g lands in
 //               the slot its arg-max names and the other three slots of that K quad are zero
 //     A rows  0..63  channels, pooled rows 0,1 of the stage ("set 0");  rows 64..127 the same channels for pooled rows 2,3 ("set 1")
@@ -20,18 +20,19 @@
 // Channel c of a set sits in row (c & 7) * 8 + (c >> 3): a builder thread owns 8 consecutive channels (one uint4 of the NHWC
 // gradient) and its 8 entry stores then fall into 8 different bank groups across the quarter-warp.
 //
-// Roles (544 threads): warp 0 setup, warp 1 MMA issuer, warps 2..5 final epilogue (TMEM lane quadrants), warps 6..13 gradient
-// (A) builders, warps 14..16 patch (B) builders + input staging.  4-stage operand ring; a stage = 4 pooled rows x 16 pooled
-// columns = 64 pooled positions = 256 K per set = 16 tcgen05.mma (K = 16).
+// Roles (480 threads): warps 0..3 = the MMA warpgroup (accumulator rows 0..63 and 64..127 as two register sets) and the final
+// epilogue (row quadrants), warps 4..11 gradient (A) builders, warps 12..14 patch (B) builders + input staging.  4-stage operand
+// ring; a stage = 4 pooled rows x 16 pooled columns = 64 pooled positions = 256 K per set = 16 wgmma (K = 16) per row set.
 #pragma once
 #include <cuda.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace conv1wg {
 
-constexpr int NUM_THREADS = 544;
-constexpr int EPI_WARP0 = 2, A_WARP0 = 6, B_WARP0 = 14;
+constexpr int NUM_THREADS = 480;
+constexpr int A_WARP0 = 4, B_WARP0 = 12;
 constexpr int A_THREADS = 256, B_THREADS = 96;
 constexpr int NST = 4;
 constexpr int CHUNKS = 16;                          // K chunks of 8 per set and stage
@@ -62,7 +63,6 @@ __device__ __forceinline__ void quad_words(uint32_t gbits, uint32_t idx, uint32_
 }
 
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_wgrad_tc_kernel(const Params p) {
-  constexpr uint32_t IDESC = ptx::make_idesc_bf16(128, 64);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* smem_a = smem;
@@ -70,8 +70,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_wgrad_tc_kernel(const Pa
   float* s_in = reinterpret_cast<float*>(smem + OFF_IN);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + OFF_BAR);     // [NST]
   uint64_t* empty = full + NST;                                     // [NST]
-  uint64_t* done = empty + NST;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(done + 1);
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int H1 = p.W >> 1;
@@ -82,12 +80,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_wgrad_tc_kernel(const Pa
       ptx::mbar_init(&full[s], A_THREADS + B_THREADS);
       ptx::mbar_init(&empty[s], 1);
     }
-    ptx::mbar_init(done, 1);
     ptx::fence_barrier_init();
-  }
-  if (warp_idx == 1) {
-    ptx::tmem_alloc(tmem_ptr, 64);
-    ptx::tmem_relinquish();
   }
   // B: zero everything once, then the row of ones (tap slot 9 of the high part) of both sets; builders only ever write taps 0..8
   for (int e = threadIdx.x; e < NST * B_BYTES / 16; e += NUM_THREADS) {
@@ -96,33 +89,48 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_wgrad_tc_kernel(const Pa
     *reinterpret_cast<uint4*>(smem_b + (size_t)e * 16) = make_uint4(one2, one2, one2, one2);
   }
   ptx::fence_proxy_async_smem();
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp_idx == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      int st = 0;
-      uint32_t ph = 0;
-      bool first = true;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        ptx::mbar_wait(&full[st], ph);
-        ptx::tc_fence_after();
-        const uint32_t a_base = ptx::smem_u32(smem_a + st * A_BYTES), b_base = ptx::smem_u32(smem_b + st * B_BYTES);
+  if (warp_idx < A_WARP0) {
+    // ===================== MMA warpgroup, then the final epilogue: row = (set, row of the set), columns set*32 .. = [taps hi | ones | taps lo]
+    float d0[32], d1[32];
 #pragma unroll
-        for (int k = 0; k < CHUNKS / 2; ++k) {
-          ptx::mma_f16_ss(tmem_base, ptx::make_desc_k_nosw(a_base + k * 2 * 2048, 2048, 128),
-                          ptx::make_desc_k_nosw(b_base + k * 2 * 1024, 1024, 128), IDESC, (first && k == 0) ? 0u : 1u);
-        }
-        first = false;
-        ptx::tc_commit(&empty[st]);
-        if (++st == NST) { st = 0; ph ^= 1; }
+    for (int i = 0; i < 32; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
+    int st = 0;
+    uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      ptx::mbar_wait(&full[st], ph);
+      const uint32_t a_base = ptx::smem_u32(smem_a + st * A_BYTES), b_base = ptx::smem_u32(smem_b + st * B_BYTES);
+      wg::fence();
+#pragma unroll
+      for (int k = 0; k < CHUNKS / 2; ++k) {
+        const uint64_t bd = ptx::make_desc_k_nosw(b_base + k * 2 * 1024, 1024, 128);
+        wg::mma_bf16<64>(d0, ptx::make_desc_k_nosw(a_base + k * 2 * 2048, 2048, 128), bd, 1u);
+        wg::mma_bf16<64>(d1, ptx::make_desc_k_nosw(a_base + 64 * 16 + k * 2 * 2048, 2048, 128), bd, 1u);
       }
-      ptx::tc_commit(done);
+      wg::commit();
+      wg::wait<0>();
+      if (threadIdx.x == 0) ptx::mbar_arrive(&empty[st]);
+      if (++st == NST) { st = 0; ph ^= 1; }
     }
-    __syncwarp();
+    wg::fence_operand(d0);
+    wg::fence_operand(d1);
+    // every builder write has been consumed: the A ring is free and holds the staged accumulators [128][64] f32
+    float* acc_tile = reinterpret_cast<float*>(smem_a);
+    ptx::acc_store<64, 64>(acc_tile, d0, 0);
+    ptx::acc_store<64, 64>(acc_tile, d1, 64);
+    ptx::bar_sync(1, 128);
+    const int q = warp_idx & 3;
+    const int set = q >> 1;
+    const int mm = (q & 1) * 32 + lane;                      // row within the set
+    const int ch = (mm & 7) * 8 + (mm >> 3);
+    uint32_t v[32];
+    ptx::acc_ld<64, 32>(acc_tile, q * 32 + lane, set * 32, v);
+    if ((int)blockIdx.x < num_tiles) {
+#pragma unroll
+      for (int tap = 0; tap < 9; ++tap) atomicAdd(p.dW + tap * 64 + ch, __uint_as_float(v[tap]) + __uint_as_float(v[16 + tap]));
+      atomicAdd(p.db + ch, __uint_as_float(v[9]));
+    }
   } else if (warp_idx >= B_WARP0) {
     // ===================== patch (B) builders + input staging =====================
     const int bt = threadIdx.x - B_WARP0 * 32;              // 0..95: item (chunk 0..15, set, kernel row r)
@@ -148,7 +156,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_wgrad_tc_kernel(const Pa
         float* rowp = s_in + b * IN_ROWS * IN_STRIDE + bt * IN_STRIDE;
         rowp[0] = 0.f; rowp[33] = 0.f; rowp[34] = 0.f; rowp[35] = 0.f;
       }
-    // input rows are prefetched TWO tiles ahead in registers (a tile is ~1 us of work, about one HBM round trip: one tile ahead
+    // input rows are prefetched TWO tiles ahead in registers (a tile is about one HBM round trip of work: one tile ahead
     // left the load latency exposed every iteration) and parked in the other s_in buffer one tile ahead
     const int G = gridDim.x;
     float4 pre[2];
@@ -260,29 +268,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_wgrad_tc_kernel(const Pa
         if (++st == NST) { st = 0; ph ^= 1; }
       }
     }
-  } else if (warp_idx >= EPI_WARP0) {
-    // ===================== final epilogue: lane = (set, row of the set), columns set*32 .. = [taps hi | ones | taps lo] =====================
-    const int q = warp_idx & 3;
-    const int set = q >> 1;
-    const int mm = (q & 1) * 32 + lane;                      // row within the set
-    const int ch = (mm & 7) * 8 + (mm >> 3);
-    ptx::mbar_wait(done, 0);
-    ptx::tc_fence_after();
-    uint32_t v[32];
-    ptx::tmem_ld_32x32b_x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + set * 32, v);
-    ptx::tmem_ld_wait();
-    if ((int)blockIdx.x < num_tiles) {
-#pragma unroll
-      for (int tap = 0; tap < 9; ++tap) atomicAdd(p.dW + tap * 64 + ch, __uint_as_float(v[tap]) + __uint_as_float(v[16 + tap]));
-      atomicAdd(p.db + ch, __uint_as_float(v[9]));
-    }
-  }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, 64);
   }
 }
 

@@ -1,11 +1,10 @@
 // conv2 + bias + ReLU + 2x2 max-pool (lib/networks/LSTM_train.py:26-27) with the GEMM operands SWAPPED:
 //
-//   D^T[128 out-channels x 256 positions, f32 in TMEM] = W[128 x K] (bf16, K-major) * X[256 positions x K]^T (bf16, K-major)
+//   D^T[128 out-channels x 256 positions, f32] = W[128 x K] (bf16, K-major) * X[256 positions x K]^T (bf16, K-major)
 //
 // Why: with Cout = 128 the position-major kernel (gemm.cuh, M = 128 positions, N = 128 channels) moves 8 KB of operands
-// through shared memory per 128x128x16 MMA and cannot keep the tensor pipe fed (measured 874 TFLOP/s, pipe 43.6 %).  Putting
-// the 128 channels on the M side lets N be 256 POSITIONS: 12 KB per 128x256x16 MMA -- the same smem bytes per flop as the
-// Cout = 256 layers that run at 1450-1700 TFLOP/s.
+// through shared memory per 128x128x16 MMA and feeds the tensor pipe worse than the wide layers.  Putting the 128 channels on
+// the M side lets N be 256 POSITIONS: 12 KB per 128x256x16 MMA -- the same smem bytes per flop as the Cout = 256 layers.
 //
 // A tile = 16 H-rows x Wd(16) of one image = 256 positions; per K-block (= one 3x3 tap, Cin = 64) the producer issues two
 // 4-D TMA boxes of 128 positions at (r-1, s-1)-shifted coordinates (OOB zero fill = SAME padding, also past the image end)
@@ -15,17 +14,18 @@
 #include <cuda.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace convsw {
 
-constexpr int STAGES = 4;
+constexpr int STAGES = 2;                   // what fits next to the 128 KB staged accumulator tile
 constexpr int W_BYTES = 128 * 128;          // weights: 128 channels x 64 K (128 B rows, SW128)
 constexpr int X_BYTES = 256 * 128;          // activations: 256 positions x 64 K
 constexpr int STAGE_BYTES = W_BYTES + X_BYTES;
-constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
+constexpr int ACC_OFFSET = STAGES * STAGE_BYTES;
+constexpr int BAR_OFFSET = ACC_OFFSET + 128 * 256 * 4;
 constexpr int SMEM_BYTES = BAR_OFFSET + 256 + 1024;
-constexpr int NUM_THREADS = 320;            // warp 0 producer, warp 1 MMA, warps 2..9 epilogue
-constexpr int NUM_EPI_WARPS = 8;
+constexpr int NUM_THREADS = 384;            // warpgroup 0 producer, warpgroups 1..2 MMA (channels 0..63 / 64..127) + epilogue
 constexpr int NUM_TAPS = 9;
 
 struct Params {
@@ -40,14 +40,11 @@ struct Params {
 template <bool TRAIN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const Params p) {
-  constexpr uint32_t IDESC = ptx::make_idesc_bf16(128, 256);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + BAR_OFFSET);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  float* acc_tile = reinterpret_cast<float*>(smem + ACC_OFFSET);
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_tiles = p.Nimg * p.tiles_per_img;
@@ -57,26 +54,16 @@ conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
     ptx::prefetch_tmap(&tmW);
     for (int s = 0; s < STAGES; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      ptx::mbar_init(&tmem_full[s], 1);
-      ptx::mbar_init(&tmem_empty[s], NUM_EPI_WARPS);
+      ptx::mbar_init(&empty_bar[s], 2);        // one arrive per MMA warpgroup
     }
     ptx::fence_barrier_init();
   }
-  if (warp_idx == 1) {
-    ptx::tmem_alloc(tmem_ptr, 512);           // two 256-column accumulators
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp_idx == 0) {
+  if (warp_idx < 4) {
+    ptx::setmaxnreg_dec<40>();
     // ===================== TMA producer: lanes 0/1 = the two activation boxes, lane 2 = the weight box =====================
-    if (lane < 3) {
+    if (warp_idx == 0 && lane < 3) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -93,51 +80,45 @@ conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
         }
       }
     }
-    __syncwarp();
-  } else if (warp_idx == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      int stage = 0, it = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        const int acc = it & 1;
-        ptx::mbar_wait(&tmem_empty[acc], ((it >> 1) & 1) ^ 1);
-        ptx::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * 256;
-        for (int tap = 0; tap < NUM_TAPS; ++tap) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          ptx::tc_fence_after();
-          const uint64_t a_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem + stage * STAGE_BYTES));
-          const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem + stage * STAGE_BYTES + W_BYTES));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) ptx::mma_f16_ss(d_tmem, a_desc + 2 * k, b_desc + 2 * k, IDESC, (tap | k) != 0);
-          ptx::tc_commit(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        ptx::tc_commit(&tmem_full[acc]);
-      }
-    }
-    __syncwarp();
   } else {
-    // ===================== epilogue: lane quadrant q = 32 channels, column half ch = 8 of the tile's 16 H-rows =====================
+    ptx::setmaxnreg_inc<232>();
+    const int wgi = (warp_idx >> 2) - 1;             // accumulator rows (output channels) wgi*64 ..
+    const bool arriver = (warp_idx & 3) == 0 && lane == 0;
+    int stage = 0;
+    uint32_t phase = 0;
     const int q = warp_idx & 3;
-    const int ch = (warp_idx - 2) >> 2;
+    const int ch = (warp_idx - 4) >> 2;
     const int c = q * 32 + lane;                       // output channel of this thread
     const float bias = __ldg(p.bias + c);
     const int Hp = p.H >> 1;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int nl = tile / p.tiles_per_img, n = p.img0 + nl;
       const int h0 = (tile - nl * p.tiles_per_img) * 16;
-      const int acc = it & 1;
-      ptx::mbar_wait(&tmem_full[acc], (it >> 1) & 1);
-      ptx::tc_fence_after();
-      const uint32_t tbase = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * 256 + ch * 128;
+      float d[128];
+      int prev = -1;
+      for (int kb = 0; kb < NUM_TAPS; ++kb) {
+        ptx::mbar_wait(&full_bar[stage], phase);
+        const uint64_t a_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem + stage * STAGE_BYTES + wgi * 64 * 128));
+        const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem + stage * STAGE_BYTES + W_BYTES));
+        wg::fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wg::mma_bf16<256>(d, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
+        wg::commit();
+        wg::wait<1>();
+        if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wg::wait<0>();
+      wg::fence_operand(d);
+      if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
+      ptx::bar_sync(1, 256);                         // the previous tile's epilogue reads are done
+      ptx::acc_store<256, 256>(acc_tile, d, wgi * 64);
+      ptx::bar_sync(1, 256);
 #pragma unroll 1
       for (int pr = 0; pr < 4; ++pr) {
         uint32_t v[32];
-        ptx::tmem_ld_32x32b_x32(tbase + pr * 32, v);   // columns: [row h (16 w) | row h+1 (16 w)]
-        ptx::tmem_ld_wait();
+        ptx::acc_ld<256, 32>(acc_tile, q * 32 + lane, ch * 128 + pr * 32, v);   // columns: [row h (16 w) | row h+1 (16 w)]
         const int h = h0 + ch * 8 + 2 * pr;
         if (h < p.H) {                                  // H is even: both rows of the window are inside or outside together
           const size_t off = (((size_t)n * Hp + (h >> 1)) * 8) * 128 + c;
@@ -162,26 +143,16 @@ conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
           }
         }
       }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&tmem_empty[acc]);
     }
-  }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, 512);
   }
 }
 
 
 // ---------------------------------------------------------------------------------------------------------------------------
-// DATA gradients of the narrow layers (conv2: 64 input channels, conv3_1: 128) with the same operand swap (r2).  conv2:  d_a1[p, ci] = sum over taps, co of d_pre2[p + tap', co] * W'[ci][(tap', co)]
+// DATA gradients of the narrow layers (conv2: 64 input channels, conv3_1: 128) with the same operand swap.  conv2:  d_a1[p, ci] = sum over taps, co of d_pre2[p + tap', co] * W'[ci][(tap', co)]
 // is a 3x3 SAME convolution of the [N, H, 16, 128] gradient with the flipped / transposed kernel (Bd_c2, backward_kernels.cu):
-// only 64 output channels.  Position-major (gemm.cuh, BLOCK_N = 64) it ran the MMA at N = 64, a quarter of the 128x256x16 rate
-// (0.60 ms for 309 GFLOP).  Here the 64 channels sit on the M side (rows 64..127 of the weight box are out of bounds of the
+// only 64 output channels.  Position-major (gemm.cuh, BLOCK_N = 64) it would run the MMA at N = 64, a quarter of the N = 256
+// rate.  Here the 64 channels sit on the M side (rows 64..127 of the weight box are out of bounds of the
 // tensor map, i.e. zero-filled by TMA: half of the M = 128 MMA is padding) and N is 256 positions: half the padded work at the
 // full rate.  K-blocks = 9 taps x 2 blocks of 64 gradient channels.  Epilogue: lane = input channel (quadrants 0 and 1 only),
 // column = position; plain bf16 store (the ReLU / pool1 backward is folded into conv1's weight-gradient kernel).
@@ -197,7 +168,6 @@ struct DgradParams {
 template <int WD, int CB, int MVALID>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_dgrad_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const DgradParams p) {
-  constexpr uint32_t IDESC = ptx::make_idesc_bf16(128, 256);
   constexpr int NUM_KB = 9 * CB;             // 9 taps x CB channel blocks
   constexpr int RT = 256 / WD;               // H rows per tile (two TMA boxes of RT/2 rows)
   constexpr int RC = 32 / WD;                // H rows per 32-column accumulator chunk
@@ -205,9 +175,7 @@ conv_dgrad_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + BAR_OFFSET);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  float* acc_tile = reinterpret_cast<float*>(smem + ACC_OFFSET);
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_tiles = p.Nimg * p.tiles_per_img;
@@ -217,25 +185,15 @@ conv_dgrad_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
     ptx::prefetch_tmap(&tmW);
     for (int s = 0; s < STAGES; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      ptx::mbar_init(&tmem_full[s], 1);
-      ptx::mbar_init(&tmem_empty[s], NUM_EPI_WARPS);
+      ptx::mbar_init(&empty_bar[s], 2);        // one arrive per MMA warpgroup
     }
     ptx::fence_barrier_init();
   }
-  if (warp_idx == 1) {
-    ptx::tmem_alloc(tmem_ptr, 512);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp_idx == 0) {
-    if (lane < 3) {                          // lanes 0/1: the two 128-position gradient boxes, lane 2: the weight box
+  if (warp_idx < 4) {
+    ptx::setmaxnreg_dec<40>();
+    if (warp_idx == 0 && lane < 3) {                          // lanes 0/1: the two 128-position gradient boxes, lane 2: the weight box
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -253,48 +211,44 @@ conv_dgrad_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
         }
       }
     }
-    __syncwarp();
-  } else if (warp_idx == 1) {
-    if (lane == 0) {
-      int stage = 0, it = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        const int acc = it & 1;
-        ptx::mbar_wait(&tmem_empty[acc], ((it >> 1) & 1) ^ 1);
-        ptx::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * 256;
-        for (int kb = 0; kb < NUM_KB; ++kb) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          ptx::tc_fence_after();
-          const uint64_t a_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem + stage * STAGE_BYTES));
-          const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem + stage * STAGE_BYTES + W_BYTES));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) ptx::mma_f16_ss(d_tmem, a_desc + 2 * k, b_desc + 2 * k, IDESC, (kb | k) != 0);
-          ptx::tc_commit(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        ptx::tc_commit(&tmem_full[acc]);
-      }
-    }
-    __syncwarp();
   } else {
+    ptx::setmaxnreg_inc<232>();
+    const int wgi = (warp_idx >> 2) - 1;             // accumulator rows (output channels) wgi*64 ..
+    const bool arriver = (warp_idx & 3) == 0 && lane == 0;
+    int stage = 0;
+    uint32_t phase = 0;
     const int q = warp_idx & 3;
-    const int ch = (warp_idx - 2) >> 2;      // column half: RT/2 of the tile's RT H-rows
+    const int ch = (warp_idx - 4) >> 2;      // column half: RT/2 of the tile's RT H-rows
     const int c = q * 32 + lane;              // input channel of this thread (valid for c < MVALID)
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int n = tile / p.tiles_per_img;
       const int h0 = (tile - n * p.tiles_per_img) * RT;
-      const int acc = it & 1;
-      ptx::mbar_wait(&tmem_full[acc], (it >> 1) & 1);
-      ptx::tc_fence_after();
+      float d[128];
+      int prev = -1;
+      for (int kb = 0; kb < NUM_KB; ++kb) {
+        ptx::mbar_wait(&full_bar[stage], phase);
+        const uint64_t a_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem + stage * STAGE_BYTES + wgi * 64 * 128));
+        const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem + stage * STAGE_BYTES + W_BYTES));
+        wg::fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wg::mma_bf16<256>(d, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
+        wg::commit();
+        wg::wait<1>();
+        if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wg::wait<0>();
+      wg::fence_operand(d);
+      if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
+      ptx::bar_sync(1, 256);                         // the previous tile's epilogue reads are done
+      ptx::acc_store<256, 256>(acc_tile, d, wgi * 64);
+      ptx::bar_sync(1, 256);
       if (q * 32 < MVALID) {
-        const uint32_t tbase = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * 256 + ch * 128;
-#pragma unroll 1
+  #pragma unroll 1
         for (int pr = 0; pr < 4; ++pr) {
           uint32_t v[32];
-          ptx::tmem_ld_32x32b_x32(tbase + pr * 32, v);     // columns: RC consecutive H rows of WD positions each
-          ptx::tmem_ld_wait();
+          ptx::acc_ld<256, 32>(acc_tile, q * 32 + lane, ch * 128 + pr * 32, v);     // columns: RC consecutive H rows of WD positions each
 #pragma unroll
           for (int hr = 0; hr < RC; ++hr) {
             const int h = h0 + ch * (RT / 2) + pr * RC + hr;
@@ -306,17 +260,7 @@ conv_dgrad_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
           }
         }
       }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&tmem_empty[acc]);
     }
-  }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, 512);
   }
 }
 

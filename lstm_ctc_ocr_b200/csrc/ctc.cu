@@ -1,4 +1,4 @@
-// CTC loss (+ gradient) and greedy decode for C = 64 classes, sm_100a.
+// CTC loss (+ gradient) and greedy decode for C = 64 classes, sm_90a.
 //
 // Replaces warpctc_tensorflow.ctc at lib/networks/network.py:653-654 and the decode at
 // lib/networks/network.py:656-657 (+ zero stripping, lib/lstm/utils/training.py:32).
@@ -49,12 +49,8 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
-// 3-input maximum as ONE instruction (sm_100 FMNMX3); opaque to the compiler so that it cannot re-associate the operands
-__device__ __forceinline__ float max3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
+// 3-input maximum (exact: the order of two-operand maxima does not change the result)
+__device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 // log2(2^a + 2^b + 2^c) with -inf handling
 __device__ __forceinline__ float lse3(float a, float b, float c) {
   float m = fmaxf(a, fmaxf(b, c));
@@ -328,8 +324,8 @@ __global__ void __launch_bounds__(CTC_THREADS, 8) ctc_loss_kernel(const float* _
 
 
 // ---------------------------------------------------------------------------------------------------------------------------
-// Phase 1 of the S <= 32 kernels, alternative ("me" = mantissa/exponent, CRNN_CTC_RECUR=me).  The round-2 ncu source view put ~47 %
-// of the kernel on the 62-step alpha/beta chain: every step of the log2-space recursion is SHFL -> FMNMX3 -> FADD -> MUFU.EX2 -> FADD
+// Phase 1 of the S <= 32 kernels, alternative ("me" = mantissa/exponent, CRNN_CTC_RECUR=me).  The alpha/beta chain (62 dependent
+// steps at T = 63) is the longest part of the kernel: every step of the log2-space recursion is SHFL -> FMNMX3 -> FADD -> MUFU.EX2 -> FADD
 // -> FADD -> MUFU.LG2 -> FADD.  Here a state is carried as a PAIR
 // (m in [1,2) or 0, integer exponent e), value m * 2^e: the sum of the three predecessors is three exact power-of-two scalings
 // (integer shifts into the exponent field) and two FADDs, the emission is a multiplication by (ym, ye) -- split off the log2
@@ -338,9 +334,8 @@ __global__ void __launch_bounds__(CTC_THREADS, 8) ctc_loss_kernel(const float* _
 // range: the exponent is a 32-bit integer, so a state 2^-5000 below its neighbour is still carried (the log-space kernels' and
 // warp-ctc's behaviour on confidently-wrong frames).  What is stored per (t, s) is still log2(alpha) = lg2(m) + e (the LG2 is
 // off the chain), so phases 0 and 2 are unchanged.
-// MEASURED (B200, T=63, N=1024): 24.7 us vs 18.5 us for the log2-space chain -- the pair arithmetic needs ~3x the dependent
-// integer/select instructions per step, and with one or two warps per scheduler the chain is bound by instruction latency, not by
-// the MUFU pipe.  Kept as the high-accuracy option (costs agree with the fp64 oracle to ~1e-8 relative instead of ~1e-5).
+// The pair arithmetic needs ~3x the dependent integer/select instructions per step, and with one or two warps per scheduler the
+// chain is bound by instruction latency, not by the MUFU pipe, so this is not the faster option.  Kept as the high-accuracy option (costs agree with the fp64 oracle to ~1e-8 relative instead of ~1e-5).
 // ---------------------------------------------------------------------------------------------------------------------------
 constexpr int ME_EMIN = -(1 << 28);
 
@@ -616,8 +611,8 @@ ctc_fast_kernel(const float* __restrict__ logits, float* __restrict__ grad, cons
 
 
 // ---------------------------------------------------------------------------------------------------------------------------
-// ctc_tma_kernel: same arithmetic as ctc_fast_kernel, different data movement.  The round-1 ncu source view of
-// ctc_fast_kernel put ~1/3 of its samples on the per-thread `cp.async.bulk` issue loops: UBLKCP takes its operands from
+// ctc_tma_kernel: same arithmetic as ctc_fast_kernel, different data movement.  In ctc_fast_kernel every
+// thread issues its own `cp.async.bulk` row copies: UBLKCP takes its operands from
 // UNIFORM registers, so a warp whose 32 lanes each issue their own row copy executes them one lane at a time (ELECT / R2UR /
 // BRA.U.ANY).  Here ONE thread issues two tensor-map loads for the whole utterance -- logits [T,N,64] f32 viewed as
 // {32, 2, N, T} with a {32, 1, 1, T} box, i.e. the left and the right 128-byte half of all T rows -- into two 128B-swizzled
@@ -915,8 +910,8 @@ int make_tmap_ctc(CUtensorMap* m, const float* base, int T, int N) {
   return CRNN_OK;
 }
 
-// which S <= 32 kernel: "fast" (default: per-thread bulk row copies), "tma" (one tensor-map tile load/store per utterance: measured
-// 2 us SLOWER at C3, kept selectable and tested), "generic"
+// which S <= 32 kernel: "fast" (default: per-thread bulk row copies), "tma" (one tensor-map tile load/store per utterance, kept
+// selectable and tested), "generic"
 int ctc_kernel_choice() {
   const char* e = getenv("CRNN_CTC_KERNEL");
   if (e != nullptr && strcmp(e, "generic") == 0) return 2;
@@ -925,7 +920,7 @@ int ctc_kernel_choice() {
 }
 // alpha/beta recursion of the S <= 32 kernels: "log" (default: log2-space, 3 EX2 + 1 LG2 per step) or "me" (mantissa/exponent pairs:
 // no transcendental on the chain and ~1e-8 relative accuracy instead of ~1e-5, but MORE dependent integer/select instructions per
-// step -- measured 24.7 us vs 18.5 us at C3, so it is the accuracy option, not the speed option)
+// step, so it is the accuracy option, not the speed option)
 int ctc_recur_choice() {
   const char* e = getenv("CRNN_CTC_RECUR");
   return (e != nullptr && strcmp(e, "me") == 0) ? 1 : 0;

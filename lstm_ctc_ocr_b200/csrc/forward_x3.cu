@@ -1,24 +1,24 @@
 // f32-class forward paths (crnn_config.compute_dtype = 2 and 3) -- BASELINE configs[1]: "fp32 CRNN fwd + CTC loss, batch 256, 32x160".
 //
-// The reference computes everything in fp32 (lib/networks/LSTM_train.py:10, network.py:166,174).  The 5th-generation tensor
-// cores have no fp32 operand kind; the two ways to an fp32-class contraction are kind::tf32 (10-bit mantissa: 8x finer than
+// The reference computes everything in fp32 (lib/networks/LSTM_train.py:10, network.py:166,174).  The tensor cores have no
+// fp32 operand kind; the two ways to an fp32-class contraction are tf32 operands (10-bit mantissa: 8x finer than
 // bf16, still 2^13 coarser than fp32) and the split-operand scheme used here ("3xbf16"), which keeps ~16 mantissa bits per
-// operand and the f32 accumulator of tcgen05 kind::f16:
+// operand and the f32 accumulator of the bf16 wgmma:
 //
 //      a = ah + al,  w = wh + wl   (ah = bf16(a), al = bf16(a - ah), same for w)
 //      a*w ~= ah*wh + al*wh + ah*wl                      (the dropped al*wl term is 2^-18 relative)
 //
 // Every activation tensor is therefore stored as bf16 NHWC with 2C channels [hi(C) | lo(C)], every weight matrix as a K-major
-// B operand with a tripled K = [wh | wh | wl], and the SAME tcgen05/TMA implicit-GEMM kernels of gemm.cuh run over the virtual
+// B operand with a tripled K = [wh | wh | wl], and the SAME wgmma/TMA implicit-GEMM kernels of gemm.cuh run over the virtual
 // K = [hi | lo | hi] (the producer folds the third group back onto the hi half: gemm::Params::cin_phys / kb_phys).  The
 // accumulators leave the GEMM as raw f32 (EPI_CONV_F32 / EPI_F32); bias, batch-stat BN (f64 sums), ReLU, the max-pools and
 // the hi/lo split are done by the small HBM-bound kernels below in f32; conv1 (K = 9) runs as f32 FMAs; the LSTM cell uses
 // expf/tanhf and an f32 input projection.  Measured against the fp64 oracle: tests/test_gpu_x3.py.
 //
-// compute_dtype = 3 runs the same orchestration with kind::tf32 operands instead (template parameter TF of the kernels below,
+// compute_dtype = 3 runs the same orchestration with tf32 operands instead (template parameter TF of the kernels below,
 // gemm::gemm_kernel<..., KIND = 1>): activations stay f32 NHWC with C channels (the same bytes as the [hi | lo] bf16 rows), weights
 // are f32 K-major [Cout][K], both rounded to nearest tf32 where they are produced (the tensor core would truncate), 32 elements per
-// 128 B K-block, one pass over K at half the kind::f16 rate.  Operand precision 2^-11 instead of 2^-17: the middle point between
+// 128 B K-block, one pass over K at half the bf16 rate.  Operand precision 2^-11 instead of 2^-17: the middle point between
 // the bf16 throughput path and the split path, and the operand kind SURVEY 7.2(6) names for this configuration.
 //
 // This is the parity configuration (3x the MMA work, unfused elementwise passes, one GEMM + one cell launch per time step);
@@ -257,7 +257,7 @@ struct Plan {
 };
 
 struct State {
-  bool tf32 = false;         // compute_dtype 3: kind::tf32 operands
+  bool tf32 = false;         // compute_dtype 3: tf32 operands
   void* wblock = nullptr;
   uint8_t *Bc2, *Bc31, *Bc32, *Bc41, *Bc42, *Bc5, *Bx, *Bh, *Bl;
   CUtensorMap tB_c2, tB_c31, tB_c32, tB_c41, tB_c42, tB_c5, tB_x, tB_h, tB_l;

@@ -1,12 +1,13 @@
-// Persistent warp-specialised tcgen05 GEMM for sm_100a with fused epilogues.
+// Persistent warp-specialised wgmma GEMM for sm_90a with fused epilogues.
 //
-//   D[128 x BLOCK_N tile, f32 in TMEM] = A[rows x K] (bf16, K-major, TMA) * B[Nc x K]^T (bf16, K-major, TMA)
+//   D[128 x BLOCK_N tile, f32] = A[rows x K] (bf16, K-major, TMA) * B[Nc x K]^T (bf16, K-major, TMA)
 //
-// Roles (320 threads): warp 0 = TMA producer (one lane per box), warp 1 = tcgen05.mma issuer (one lane,
-// also owns the TMEM allocation), warps 2..9 = epilogue (TMEM lane quadrant = warp_idx % 4; two warps per quadrant,
-// each draining half of the tile's columns -- the plain-store epilogues were the bottleneck of the short-K GEMMs).
-// Pipelines: STAGES-deep smem ring (full/empty mbarriers, TMA <-> MMA) and a 2-deep TMEM accumulator
-// ring (tmem_full/tmem_empty, MMA <-> epilogue) so the epilogue of tile i overlaps the MMAs of tile i+1.
+// Roles (384 threads): warpgroup 0 = TMA producer (warp 0, one lane per box; the warpgroup gives its registers to the MMA
+// warpgroups), warpgroups 1 and 2 = MMA (rows 0..63 / 64..127 of the tile, accumulators in registers) and epilogue.
+// Pipeline: STAGES-deep smem ring (full/empty mbarriers, TMA <-> MMA; the producer runs ahead into the next tile while
+// the epilogue of this one drains).  The finished accumulators are staged in shared memory (ptx::acc_store) so that every
+// epilogue thread owns one accumulator ROW: 8 warps, accumulator quadrant q = warp % 4 (32 rows), two warps per quadrant
+// each draining half of the tile's columns.
 //
 // A-operand modes
 //   A_PLAIN  rows are consecutive rows of a 2-D [rows, K] tensor map; conv5 (2x2 VALID over [N,H,2,512]) reads
@@ -16,11 +17,12 @@
 //            64-channel block; the producer issues one 4-D TMA box per sub-box at coordinates shifted by
 //            (r-1, s-1) -- out-of-bounds elements are zero-filled by TMA, which *is* the SAME padding.
 //
-// Epilogues: see enum Epi.  Every epilogue thread owns one accumulator row (TMEM lane).
+// Epilogues: see enum Epi.  Every epilogue thread owns one accumulator row.
 #pragma once
 #include <cuda.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace gemm {
 
@@ -28,9 +30,8 @@ constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;                      // bf16 elements per K-block = one 128 B swizzle row
 constexpr int UMMA_K = 16;
 constexpr int A_STAGE_BYTES = BLOCK_M * 128;     // 16 KB
-constexpr int NUM_THREADS = 320;                 // warp 0 producer, warp 1 MMA, warps 2..9 epilogue
-constexpr int NUM_EPI_WARPS = 8;                 // two warps per TMEM lane quadrant, each draining half of the tile's columns
-constexpr int EPI_WARP0 = 2;
+constexpr int NUM_THREADS = 384;                 // warpgroup 0 producer, warpgroups 1..2 MMA + epilogue
+constexpr int MAX_SMEM = 232448;                 // opt-in shared memory per block (227 KB)
 
 enum AMode { A_PLAIN = 0, A_CONV3 = 1 };
 enum Epi {
@@ -119,17 +120,21 @@ __device__ __forceinline__ float warp_colsum32(const float (&v)[32], int lane) {
   return keep + __shfl_xor_sync(0xffffffffu, send, 1);
 }
 
+// STAGES is the requested ring depth; S the depth that fits next to the staged accumulator tile
 template <int BLOCK_N, int STAGES>
 struct Smem {
   static constexpr int B_STAGE_BYTES = BLOCK_N * 128;
-  static constexpr int BAR_OFFSET = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES);
+  static constexpr int ACC_BYTES = BLOCK_M * BLOCK_N * 4;
+  static constexpr int FIT = (MAX_SMEM - ACC_BYTES - 256 - 1024) / (A_STAGE_BYTES + B_STAGE_BYTES);
+  static constexpr int S = STAGES < FIT ? STAGES : FIT;
+  static constexpr int ACC_OFFSET = S * (A_STAGE_BYTES + B_STAGE_BYTES);
+  static constexpr int BAR_OFFSET = ACC_OFFSET + ACC_BYTES;
   static constexpr int BYTES = BAR_OFFSET + 256 + 1024;   // barriers + alignment slack
 };
 
-// Per-tile epilogue shared by the 1-CTA and 2-CTA kernels: thread (q, lane) owns accumulator row q*32+lane of the 128-row
-// tile held in its CTA's TMEM at `tbase` (lane quadrant and accumulator stage already applied).
+// Per-tile epilogue: thread (q, lane) owns accumulator row q*32+lane of the 128-row tile staged at `acc`.
 template <int BLOCK_N, int EPI>
-__device__ __forceinline__ void run_epilogue(const Params& p, const uint32_t tbase, const int m_blk, const int n_blk, const int q,
+__device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const int m_blk, const int n_blk, const int q,
                                              const int lane, const int c_lo = 0, const int c_hi = BLOCK_N) {
   const int row = q * 32 + lane;
   const int col0 = n_blk * BLOCK_N;
@@ -155,8 +160,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, const uint32_t tba
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::tmem_ld_32x32b_x32(tbase + c0, v);
-      ptx::tmem_ld_wait();
+      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
       if (grow < p.M) {
 #pragma unroll
         for (int i = 0; i < 32; i += 4)
@@ -176,8 +180,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, const uint32_t tba
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::tmem_ld_32x32b_x32(tbase + c0, v);
-      ptx::tmem_ld_wait();
+      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
       uint32_t pk[16];
 #pragma unroll
       for (int i = 0; i < 32; i += 4) {
@@ -199,8 +202,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, const uint32_t tba
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::tmem_ld_32x32b_x32(tbase + c0, v);
-      ptx::tmem_ld_wait();
+      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
       if (ok) {
 #pragma unroll
         for (int i = 0; i < 32; i += 4) {
@@ -221,8 +223,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, const uint32_t tba
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::tmem_ld_32x32b_x32(tbase + c0, v);
-      ptx::tmem_ld_wait();
+      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
       uint32_t pk[16];
 #pragma unroll
       for (int i = 0; i < 32; i += 4) {
@@ -269,8 +270,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, const uint32_t tba
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::tmem_ld_32x32b_x32(tbase + c0, v);
-      ptx::tmem_ld_wait();
+      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
       if (valid) {
 #pragma unroll
         for (int i = 0; i < 32; i += 16)
@@ -294,11 +294,10 @@ __device__ __forceinline__ void run_epilogue(const Params& p, const uint32_t tba
       uint4 mk[4];
       if (valid) {
 #pragma unroll
-        for (int i = 0; i < 4; ++i) mk[i] = __ldg(reinterpret_cast<const uint4*>(msk + c0) + i);     // issued before the TMEM wait
+        for (int i = 0; i < 4; ++i) mk[i] = __ldg(reinterpret_cast<const uint4*>(msk + c0) + i);     // issued before the accumulator reads
       }
       uint32_t v[32];
-      ptx::tmem_ld_32x32b_x32(tbase + c0, v);
-      ptx::tmem_ld_wait();
+      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
       if (valid) {
         const uint32_t* mw = reinterpret_cast<const uint32_t*>(mk);
         uint32_t pk[16];
@@ -324,8 +323,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, const uint32_t tba
 #pragma unroll
       for (int i = 0; i < 4; ++i) xq[i] = valid ? __ldg(reinterpret_cast<const uint4*>(xp + c0) + i) : make_uint4(0u, 0u, 0u, 0u);
       uint32_t v[32];
-      ptx::tmem_ld_32x32b_x32(tbase + c0, v);
-      ptx::tmem_ld_wait();
+      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
       const uint32_t* xw = reinterpret_cast<const uint32_t*>(xq);
       uint32_t pk[16];
       float f[32], f2[32];
@@ -361,8 +359,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, const uint32_t tba
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::tmem_ld_32x32b_x32(tbase + c0, v);
-      ptx::tmem_ld_wait();
+      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
       if (valid) {
 #pragma unroll
         for (int i = 0; i < 32; i += 4)
@@ -385,8 +382,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, const uint32_t tba
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::tmem_ld_32x32b_x32(tbase + c0, v);
-      ptx::tmem_ld_wait();
+      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
 #pragma unroll
       for (int i = 0; i < 32; i += 4) {
         const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + c0 + i));
@@ -435,8 +431,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, const uint32_t tba
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::tmem_ld_32x32b_x32(tbase + c0, v);
-      ptx::tmem_ld_wait();
+      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
       float f[32], f2[32];
       uint32_t pk[16];
 #pragma unroll
@@ -483,11 +478,10 @@ __device__ __forceinline__ void run_epilogue(const Params& p, const uint32_t tba
 #pragma unroll 1
     for (int u0 = (c_lo >> 2); u0 < (c_hi >> 2); u0 += 16) {
       uint32_t gi[16], gj[16], gf[16], go[16];
-      ptx::tmem_ld_32x32b_x16(tbase + u0, gi);
-      ptx::tmem_ld_32x32b_x16(tbase + 64 + u0, gj);
-      ptx::tmem_ld_32x32b_x16(tbase + 128 + u0, gf);
-      ptx::tmem_ld_32x32b_x16(tbase + 192 + u0, go);
-      ptx::tmem_ld_wait();
+      ptx::acc_ld<BLOCK_N, 16>(acc, row, u0, gi);
+      ptx::acc_ld<BLOCK_N, 16>(acc, row, 64 + u0, gj);
+      ptx::acc_ld<BLOCK_N, 16>(acc, row, 128 + u0, gf);
+      ptx::acc_ld<BLOCK_N, 16>(acc, row, 192 + u0, go);
       uint32_t hp[8];
       if (active) {
         uint4 xi[2], xj[2], xf[2], xo[2];
@@ -537,26 +531,24 @@ __device__ __forceinline__ void run_epilogue(const Params& p, const uint32_t tba
 
 }
 
-// KIND 0: bf16 operands (kind::f16), 64 elements per 128 B K-block.  KIND 1: f32 words read as tf32 (kind::tf32), 32 elements per
-// K-block (forward_x3.cu, compute_dtype 3); tensor maps are FLOAT32 with 32-element boxes, everything else is shared.
+// KIND 0: bf16 operands, 64 elements per 128 B K-block.  KIND 1: f32 words read as tf32, 32 elements per K-block
+// (forward_x3.cu, compute_dtype 3); tensor maps are FLOAT32 with 32-element boxes, everything else is shared.
 template <int BLOCK_N, int AMODE, int EPI, int STAGES, int KIND = 0>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Params p) {
   static_assert(BLOCK_N == 64 || BLOCK_N == 128 || BLOCK_N == 256, "BLOCK_N");
+  using SM = Smem<BLOCK_N, STAGES>;
+  constexpr int S = SM::S;
   constexpr int B_STAGE_BYTES = BLOCK_N * 128;
-  constexpr uint32_t TMEM_COLS = 2 * BLOCK_N;        // power of two >= 32
-  constexpr uint32_t IDESC = KIND ? ptx::make_idesc_tf32(BLOCK_M, BLOCK_N) : ptx::make_idesc_bf16(BLOCK_M, BLOCK_N);
   constexpr int KELEMS = KIND ? 32 : BLOCK_K;        // operand elements per 128 B K-block
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Smem<BLOCK_N, STAGES>::BAR_OFFSET);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  uint8_t* smem_b = smem + S * A_STAGE_BYTES;
+  float* acc_tile = reinterpret_cast<float*>(smem + SM::ACC_OFFSET);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + SM::BAR_OFFSET);
+  uint64_t* empty_bar = full_bar + S;
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -565,33 +557,22 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (warp_idx == 0 && lane == 0) {
     ptx::prefetch_tmap(&tmA);
     ptx::prefetch_tmap(&tmB);
-    for (int s = 0; s < STAGES; ++s) {
+    for (int s = 0; s < S; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      ptx::mbar_init(&tmem_full[s], 1);
-      ptx::mbar_init(&tmem_empty[s], NUM_EPI_WARPS);   // one arrive per epilogue warp
+      ptx::mbar_init(&empty_bar[s], 2);              // one arrive per MMA warpgroup
     }
     ptx::fence_barrier_init();
   }
-  if (warp_idx == 1) {
-    ptx::tmem_alloc(tmem_ptr, TMEM_COLS);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp_idx == 0) {
+  if (warp_idx < 4) {
     // ===================== TMA producer =====================
-    // One lane per TMA box: a single thread issuing 5 boxes per K-block was the bottleneck of the conv mainloop
-    // (~200 cycles per cp.async.bulk.tensor issue vs 512 MMA cycles per K-block).  Lanes 0..nA-1 load the A sub-boxes,
-    // lane nA loads B; lane 0 also arms the transaction count.  conv: when the tile's 4 sub-boxes are contiguous rows of
-    // one image (p.merged), a single 128-position box replaces them.
+    // One lane per TMA box: a single thread issuing 5 boxes per K-block serialises the conv mainloop on the issue latency.
+    // Lanes 0..nA-1 load the A sub-boxes, lane nA loads B; lane 0 also arms the transaction count.  conv: when the tile's 4
+    // sub-boxes are contiguous rows of one image (p.merged), a single 128-position box replaces them.
+    ptx::setmaxnreg_dec<40>();
     const int nA = (AMODE == A_CONV3 && !p.merged) ? 4 : 1;
-    if (lane <= nA) {
+    if (warp_idx == 0 && lane <= nA) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -629,65 +610,48 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             }
           }
           if (++cb == p.cin_blocks) { cb = 0; ++tap; }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          if (++stage == S) { stage = 0; phase ^= 1; }
         }
       }
     }
-    __syncwarp();
-  } else if (warp_idx == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        ptx::mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        ptx::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          ptx::tc_fence_after();
-          const uint64_t a_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_a + stage * A_STAGE_BYTES));
-          const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_b + stage * B_STAGE_BYTES));
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            // advance 16 bf16 (8 tf32) = 32 B along K inside the 128 B swizzle row: +2 in the (addr >> 4) field
-            if (KIND) ptx::mma_tf32_ss(d_tmem, a_desc + 2 * k, b_desc + 2 * k, IDESC, (kb | k) != 0);
-            else ptx::mma_f16_ss(d_tmem, a_desc + 2 * k, b_desc + 2 * k, IDESC, (kb | k) != 0);
-          }
-          ptx::tc_commit(&empty_bar[stage]);         // frees the smem slot once these MMAs retire
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        ptx::tc_commit(&tmem_full[acc]);             // accumulator complete -> epilogue
-      }
-    }
-    __syncwarp();
   } else {
-    // ===================== epilogue warps =====================
-    const int q = warp_idx & 3;                      // TMEM lane quadrant accessible to this warp
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+    // ===================== MMA warpgroups (rows wgi*64 ..) + epilogue =====================
+    ptx::setmaxnreg_inc<232>();
+    const int wgi = (warp_idx >> 2) - 1;
+    const int q = warp_idx & 3;                      // accumulator row quadrant drained by this warp
+    const int chalf = (warp_idx - 4) >> 2;           // warps 4..7 take columns [0, N/2), warps 8..11 take [N/2, N)
+    const bool arriver = (warp_idx & 3) == 0 && lane == 0;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m_blk = p.m_tile0 + tile / p.num_n_tiles, n_blk = tile % p.num_n_tiles;
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      ptx::mbar_wait(&tmem_full[acc], acc_phase);
-      ptx::tc_fence_after();
-      const uint32_t tbase = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BLOCK_N;
-      const int chalf = (warp_idx - 2) >> 2;           // warps 2..5 take columns [0, N/2), warps 6..9 take [N/2, N)
-      run_epilogue<BLOCK_N, EPI>(p, tbase, m_blk, n_blk, q, lane, chalf * (BLOCK_N / 2), (chalf + 1) * (BLOCK_N / 2));
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&tmem_empty[acc]);
+      float d[BLOCK_N / 2];
+      int prev = -1;
+      for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+        ptx::mbar_wait(&full_bar[stage], phase);
+        const uint64_t a_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_a + stage * A_STAGE_BYTES + wgi * 64 * 128));
+        const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_b + stage * B_STAGE_BYTES));
+        wg::fence();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
+          // advance 16 bf16 (8 tf32) = 32 B along K inside the 128 B swizzle row: +2 in the (addr >> 4) field
+          if (KIND) wg::mma_tf32<BLOCK_N>(d, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
+          else wg::mma_bf16<BLOCK_N>(d, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
+        }
+        wg::commit();
+        wg::wait<1>();                               // the previous K-block's MMAs have retired: free its smem slot
+        if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == S) { stage = 0; phase ^= 1; }
+      }
+      wg::wait<0>();
+      wg::fence_operand(d);
+      if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
+      ptx::bar_sync(1, 256);                         // the previous tile's epilogue reads are done
+      ptx::acc_store<BLOCK_N, BLOCK_N>(acc_tile, d, wgi * 64);
+      ptx::bar_sync(1, 256);
+      run_epilogue<BLOCK_N, EPI>(p, acc_tile, m_blk, n_blk, q, lane, chalf * (BLOCK_N / 2), (chalf + 1) * (BLOCK_N / 2));
     }
-  }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, TMEM_COLS);
   }
 }
 

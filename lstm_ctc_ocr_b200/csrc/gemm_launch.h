@@ -1,7 +1,6 @@
-// Launch helpers for the tcgen05 GEMM kernels (shared by model.cu and backward.cu).
+// Launch helpers for the wgmma GEMM kernels (shared by model.cu and backward.cu).
 #pragma once
 #include "gemm.cuh"
-#include "gemm2.cuh"
 #include "gemm_tn.cuh"
 #include <cstdlib>
 #include <string>
@@ -22,28 +21,9 @@ static int launch_gemm(const CUtensorMap& a, const CUtensorMap& b, const gemm::P
   return CRNN_OK;
 }
 
-// 2-CTA pairs: B map must have box rows = 128 (each CTA stages half of the 256-row N tile)
-template <int AM, int EPI, int ST, int BN = 256>
-static int launch_gemm2(const CUtensorMap& a, const CUtensorMap& b_half, const gemm::Params& p, int num_sms, cudaStream_t st) {
-  auto kern = gemm::gemm2_kernel<BN, AM, EPI, ST>;
-  constexpr int smem = gemm::Smem2<BN, ST>::BYTES;
-  static bool attr = false;
-  if (!attr) {
-    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr = true;
-  }
-  const int pairs = ((p.num_m_tiles + 1) / 2) * p.num_n_tiles;
-  int clusters = num_sms / 2;
-  if (pairs < clusters) clusters = pairs;
-  kern<<<2 * clusters, gemm::NUM_THREADS, smem, st>>>(a, b_half, p);
-  CUDA_TRY(cudaGetLastError());
-  return CRNN_OK;
-}
-
 // Split-K factor of a weight-gradient GEMM.  Work items (output tile x K chunk) all cost the same and the persistent CTAs take them
 // round-robin, so the launch lasts  ceil(items / workers) rounds x (K blocks per chunk + epilogue).  The first-generation rule
-// ("about 3 items per worker") left a mostly idle last round -- conv4_1: 18 tiles x 13 chunks = 234 items on 74 CTA pairs = 4 rounds
-// at 79 % occupancy; 18 x 4 = 72 items is ONE round at 97 %.  Pick the factor that minimises the modelled time (ties: fewer chunks =
+// ("about 3 items per worker") can leave a mostly idle last round.  Pick the factor that minimises the modelled time (ties: fewer chunks =
 // fewer f32 reduction atomics).  CRNN_KSPLIT=old restores the old rule.
 static inline int pick_k_splits(int tiles, int k_blocks_total, int workers) {
   static const bool old_rule = [] { const char* e = getenv("CRNN_KSPLIT"); return e && std::string(e) == "old"; }();
@@ -78,26 +58,6 @@ static int launch_gemm_tn(const CUtensorMap& a, const CUtensorMap& b, gemm_tn::P
   const int items = tiles * p.k_splits;
   const int grid = items < num_sms ? items : num_sms;
   kern<<<grid, gemm_tn::NUM_THREADS, smem, st>>>(a, b, p);
-  CUDA_TRY(cudaGetLastError());
-  return CRNN_OK;
-}
-
-// 2-CTA weight-gradient GEMM: p.num_m_tiles must count 256-row PAIRS and p.num_n_tiles 256-column tiles.
-template <int AM, int ST>
-static int launch_gemm_tn2(const CUtensorMap& a, const CUtensorMap& b, gemm_tn::Params p, int num_sms, cudaStream_t st) {
-  auto kern = gemm_tn::gemm_tn2_kernel<AM, ST>;
-  constexpr int smem = gemm_tn::Smem2<ST>::BYTES;
-  static bool attr = false;
-  if (!attr) {
-    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr = true;
-  }
-  const int tiles = p.num_taps * p.num_m_tiles * p.num_n_tiles;
-  const int max_clusters = num_sms / 2;
-  if (p.k_splits <= 0) p.k_splits = pick_k_splits(tiles, p.k_blocks_total, max_clusters);
-  const int items = tiles * p.k_splits;
-  const int clusters = items < max_clusters ? items : max_clusters;
-  kern<<<2 * clusters, gemm_tn::NUM_THREADS, smem, st>>>(a, b, p);
   CUDA_TRY(cudaGetLastError());
   return CRNN_OK;
 }

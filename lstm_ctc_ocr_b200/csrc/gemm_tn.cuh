@@ -1,11 +1,14 @@
-// "TN" tcgen05 GEMM for weight gradients:  D[M x N] += sum_k A[k][m] * B[k][n]
+// "TN" wgmma GEMM for weight gradients:  D[M x N] += sum_k A[k][m] * B[k][n]
 // Both operands are stored K-rows x channel-columns (channels contiguous) -- exactly how activations and their
 // gradients already sit in HBM (NHWC / [rows, C]) -- so they are fed to the tensor core as MN-MAJOR operands
-// (instruction descriptor a_major = b_major = 1) without any transposition pass.
+// (wgmma transpose flags set for A and B) without any transposition pass.
 //
 // smem tile per operand and stage: J blocks of [64 K-rows x 128 B] (64 channels), 128-byte swizzle as written by
 // TMA; canonical MN-major layout ((8,n),(8,k)) : leading byte offset = 8192 B between 64-channel blocks,
-// stride byte offset = 1024 B between 8-row K groups; one tcgen05.mma consumes 16 K-rows (= 2048 B advance).
+// stride byte offset = 1024 B between 8-row K groups; one wgmma consumes 16 K-rows (= 2048 B advance).
+//
+// Roles (384 threads): warpgroup 0 = TMA producer (warp 0), warpgroups 1 and 2 = MMA (M rows 0..63 / 64..127 = A block 0 / 1)
+// and epilogue (accumulators staged in shared memory, thread = one output row, two warps per 32-row quadrant).
 //
 // Split-K persistent scheduler: work item = (output tile, K-chunk); the f32 tile is reduced into global memory with
 // red.global.add.f32 (the gradient buffer is zeroed once per step).
@@ -16,12 +19,14 @@
 #include <cuda.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace gemm_tn {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;                 // K rows per stage
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = 384;
+constexpr int MAX_SMEM = 232448;
 constexpr int BLK_BYTES = BLOCK_K * 128;    // one [64 x 64ch] block = 8 KB
 
 enum AMode { TN_PLAIN = 0, TN_CONV = 1 };
@@ -55,40 +60,36 @@ __device__ __forceinline__ uint64_t make_desc_mn_sw128(uint32_t smem_addr) {
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(BLK_BYTES >> 4) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
-}
-__host__ __device__ constexpr uint32_t make_idesc_bf16_mn(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
 }
 
 template <int BLOCK_N, int STAGES>
 struct Smem {
   static constexpr int A_STAGE = (BLOCK_M / 64) * BLK_BYTES;
   static constexpr int B_STAGE = (BLOCK_N / 64) * BLK_BYTES;
-  static constexpr int BAR_OFFSET = STAGES * (A_STAGE + B_STAGE);
+  static constexpr int ACC_BYTES = BLOCK_M * BLOCK_N * 4;
+  static constexpr int FIT = (MAX_SMEM - ACC_BYTES - 256 - 1024) / (A_STAGE + B_STAGE);
+  static constexpr int S = STAGES < FIT ? STAGES : FIT;
+  static constexpr int ACC_OFFSET = S * (A_STAGE + B_STAGE);
+  static constexpr int BAR_OFFSET = ACC_OFFSET + ACC_BYTES;
   static constexpr int BYTES = BAR_OFFSET + 256 + 1024;
 };
 
 template <int BLOCK_N, int AMODE, int STAGES>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Params p) {
-  constexpr int A_STAGE = Smem<BLOCK_N, STAGES>::A_STAGE, B_STAGE = Smem<BLOCK_N, STAGES>::B_STAGE;
+  using SM = Smem<BLOCK_N, STAGES>;
+  constexpr int A_STAGE = SM::A_STAGE, B_STAGE = SM::B_STAGE, STG = SM::S;
   constexpr int JA = BLOCK_M / 64, JB = BLOCK_N / 64;
-  constexpr uint32_t TMEM_COLS = 2 * BLOCK_N;
-  constexpr uint32_t IDESC = make_idesc_bf16_mn(BLOCK_M, BLOCK_N);
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + STAGES * A_STAGE;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Smem<BLOCK_N, STAGES>::BAR_OFFSET);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  uint8_t* smem_b = smem + STG * A_STAGE;
+  float* acc_tile = reinterpret_cast<float*>(smem + SM::ACC_OFFSET);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + SM::BAR_OFFSET);
+  uint64_t* empty_bar = full_bar + STG;
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles = p.num_taps * p.num_m_tiles * p.num_n_tiles;
@@ -98,15 +99,10 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp_idx == 0 && lane == 0) {
     ptx::prefetch_tmap(&tmA);
     ptx::prefetch_tmap(&tmB);
-    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { ptx::mbar_init(&tmem_full[s], 1); ptx::mbar_init(&tmem_empty[s], 4); }
+    for (int s = 0; s < STG; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 2); }
     ptx::fence_barrier_init();
   }
-  if (warp_idx == 1) { ptx::tmem_alloc(tmem_ptr, TMEM_COLS); ptx::tmem_relinquish(); }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   // work item -> (tap, m_blk, n_blk, [kb0, kb1)) ; K-split is the slowest index so concurrently running CTAs work
   // on the same K-chunk of different tiles (operand reuse in L2)
@@ -119,9 +115,10 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     kb1 = min(kb0 + kb_per_split, p.k_blocks_total);
   };
 
-  if (warp_idx == 0) {
+  if (warp_idx < 4) {
     // one lane per 64-channel operand block (JA blocks of A, JB blocks of B); lane 0 also arms the transaction count
-    if (lane < JA + JB) {
+    ptx::setmaxnreg_dec<40>();
+    if (warp_idx == 0 && lane < JA + JB) {
       const bool isA = lane < JA;
       const int j = isA ? lane : lane - JA;
       int stage = 0; uint32_t phase = 0;
@@ -160,57 +157,52 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               ptx::tma_load_4d(tm, &full_bar[stage], dst + half * 4096, ccol, shifted ? s - 1 : 0, h0 + (shifted ? r - 1 : 0), n);
             }
           }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          if (++stage == STG) { stage = 0; phase ^= 1; }
         }
       }
     }
-    __syncwarp();
-  } else if (warp_idx == 1) {
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0; int it = 0;
-      for (int item = blockIdx.x; item < num_items; item += gridDim.x, ++it) {
-        int tap, m_blk, n_blk, kb0, kb1;
-        decode(item, tap, m_blk, n_blk, kb0, kb1);
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        ptx::mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        ptx::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          ptx::tc_fence_after();
-          const uint64_t a_desc = make_desc_mn_sw128(ptx::smem_u32(smem_a + stage * A_STAGE));
-          const uint64_t b_desc = make_desc_mn_sw128(ptx::smem_u32(smem_b + stage * B_STAGE));
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / 16; ++k)     // 16 K-rows = 2048 B -> +128 in the (addr >> 4) field
-            ptx::mma_f16_ss(d_tmem, a_desc + 128 * k, b_desc + 128 * k, IDESC, (kb > kb0 || k > 0) ? 1u : 0u);
-          ptx::tc_commit(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        ptx::tc_commit(&tmem_full[acc]);
-      }
-    }
-    __syncwarp();
   } else {
+    ptx::setmaxnreg_inc<232>();
+    const int wgi = (warp_idx >> 2) - 1;             // M rows wgi*64 .. = A block wgi
+    const int chalf = (warp_idx - 4) >> 2;           // warps 4..7 drain columns [0, N/2), warps 8..11 [N/2, N)
+    const bool arriver = (warp_idx & 3) == 0 && lane == 0;
+    int stage = 0; uint32_t phase = 0;
     const int q = warp_idx & 3;
     const int row = q * 32 + lane;
-    int it = 0;
-    for (int item = blockIdx.x; item < num_items; item += gridDim.x, ++it) {
+    for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
       int tap, m_blk, n_blk, kb0, kb1;
       decode(item, tap, m_blk, n_blk, kb0, kb1);
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      ptx::mbar_wait(&tmem_full[acc], acc_phase);
-      ptx::tc_fence_after();
-      const uint32_t tbase = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BLOCK_N;
+      float d[BLOCK_N / 2];
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) d[i] = 0.f;     // an empty K chunk reduces zeros
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        ptx::mbar_wait(&full_bar[stage], phase);
+        const uint64_t a_desc = make_desc_mn_sw128(ptx::smem_u32(smem_a + stage * A_STAGE + wgi * BLK_BYTES));
+        const uint64_t b_desc = make_desc_mn_sw128(ptx::smem_u32(smem_b + stage * B_STAGE));
+        wg::fence();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / 16; ++k)     // 16 K-rows = 2048 B -> +128 in the (addr >> 4) field
+          wg::mma_bf16<BLOCK_N, 1>(d, a_desc + 128 * k, b_desc + 128 * k, 1u);
+        wg::commit();
+        wg::wait<1>();
+        if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == STG) { stage = 0; phase ^= 1; }
+      }
+      wg::wait<0>();
+      wg::fence_operand(d);
+      if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
+      ptx::bar_sync(1, 256);
+      ptx::acc_store<BLOCK_N, BLOCK_N>(acc_tile, d, wgi * 64);
+      ptx::bar_sync(1, 256);
       const int m = m_blk * BLOCK_M + row;
       const bool okm = (m < p.M) && (kb1 > kb0);
       float* orow = p.out + (long long)tap * p.tap_stride + (long long)(m + p.out_row_offset) * p.ldo;
 #pragma unroll 1
-      for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
+      for (int c0 = chalf * (BLOCK_N / 2); c0 < (chalf + 1) * (BLOCK_N / 2); c0 += 32) {
         uint32_t v[32];
-        ptx::tmem_ld_32x32b_x32(tbase + c0, v);
-        ptx::tmem_ld_wait();
+        ptx::acc_ld<BLOCK_N, 32>(acc_tile, row, c0, v);
         if (AMODE == TN_CONV && p.tap_pack_n) {
           // swapped operands: row = output channel co, column = (tap, ci).  Written transposed into the HWIO gradient
           // out[(tap*64 + ci) * ldo + co]; the lanes of a warp are consecutive co -> one 128-byte segment per instruction
@@ -240,187 +232,10 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             ptx::red_add_v4_f32(dst + i, __uint_as_float(v[i]), __uint_as_float(v[i + 1]), __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
         }
       }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&tmem_empty[acc]);
     }
   }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) { ptx::tc_fence_after(); ptx::tmem_dealloc(tmem_base, TMEM_COLS); }
 }
 
 
-// ------------------------------------------------------------------------------------------------------------------
-// 2-CTA (cta_group::2) variant: a cluster of two CTAs accumulates a 256 (M) x 256 (N) output tile.  CTA `rank` stages its own
-// 128 M-channels of A and its own 128 N-channels of B (16 KB + 16 KB per 64-row K-block instead of 16 + 32), the leader
-// issues tcgen05.mma.cta_group::2 with M = 256; protocol identical to gemm2.cuh.  `num_m_tiles` counts 256-row PAIRS here.
-// ------------------------------------------------------------------------------------------------------------------
-template <int STAGES>
-struct Smem2 {
-  static constexpr int A_STAGE = 2 * BLK_BYTES;      // this CTA's 128 M-channels
-  static constexpr int B_STAGE = 2 * BLK_BYTES;      // this CTA's 128 of the 256 N-channels
-  static constexpr int BAR_OFFSET = STAGES * (A_STAGE + B_STAGE);
-  static constexpr int BYTES = BAR_OFFSET + 256 + 1024;
-};
-
-template <int AMODE, int STAGES>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS, 1)
-gemm_tn2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Params p) {
-  constexpr int BLOCK_N = 256;
-  constexpr int A_STAGE = Smem2<STAGES>::A_STAGE, B_STAGE = Smem2<STAGES>::B_STAGE;
-  constexpr uint32_t TMEM_COLS = 2 * BLOCK_N;
-  constexpr uint32_t IDESC = make_idesc_bf16_mn(256, BLOCK_N);
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + STAGES * A_STAGE;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Smem2<STAGES>::BAR_OFFSET);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
-  const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = ptx::cluster_ctarank();
-  const bool leader = rank == 0;
-  const int tiles = p.num_taps * p.num_m_tiles * p.num_n_tiles;
-  const int num_items = tiles * p.k_splits;
-  const int kb_per_split = (p.k_blocks_total + p.k_splits - 1) / p.k_splits;
-  const int num_clusters = gridDim.x >> 1, cluster_id = blockIdx.x >> 1;
-
-  if (warp_idx == 0 && lane == 0) {
-    ptx::prefetch_tmap(&tmA);
-    ptx::prefetch_tmap(&tmB);
-    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { ptx::mbar_init(&tmem_full[s], 1); ptx::mbar_init(&tmem_empty[s], 8); }
-    ptx::fence_barrier_init();
-  }
-  if (warp_idx == 1) { ptx::tmem_alloc_2cta(tmem_ptr, TMEM_COLS); ptx::tmem_relinquish_2cta(); }
-  ptx::tc_fence_before();
-  ptx::cluster_sync_all();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  auto decode = [&](int item, int& tap, int& m_blk, int& n_blk, int& kb0, int& kb1) {
-    const int split = item / tiles;
-    int t = item - split * tiles;
-    n_blk = t % p.num_n_tiles; t /= p.num_n_tiles;
-    m_blk = t % p.num_m_tiles; tap = t / p.num_m_tiles;
-    kb0 = split * kb_per_split;
-    kb1 = min(kb0 + kb_per_split, p.k_blocks_total);
-  };
-
-  if (warp_idx == 0) {
-    if (lane < 4) {                      // lanes 0,1: this CTA's two A blocks; lanes 2,3: its two B blocks
-      const bool isA = lane < 2;
-      const int j = lane & 1;
-      int stage = 0; uint32_t phase = 0;
-      for (int item = cluster_id; item < num_items; item += num_clusters) {
-        int tap, m_blk, n_blk, kb0, kb1;
-        decode(item, tap, m_blk, n_blk, kb0, kb1);
-        const int r = tap / 3, s = tap - 3 * r;
-        const int ccol = (isA ? m_blk * 256 : n_blk * BLOCK_N) + (int)rank * 128 + 64 * j;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-          const uint32_t lead_full = ptx::mapa(ptx::smem_u32(&full_bar[stage]), 0);
-          if (leader && lane == 0) ptx::mbar_arrive_expect_tx(&full_bar[stage], 2 * (A_STAGE + B_STAGE));
-          uint8_t* dst = (isA ? smem_a + stage * A_STAGE : smem_b + stage * B_STAGE) + j * BLK_BYTES;
-          const CUtensorMap* tm = isA ? &tmA : &tmB;
-          if (AMODE == TN_PLAIN) {
-            ptx::tma_load_2d_2cta(tm, lead_full, dst, ccol, kb * BLOCK_K + (isA ? p.a_row_shift : 0));
-          } else if (p.merged) {
-            const int n = kb / p.kb_per_img;
-            const int h0 = (kb - n * p.kb_per_img) * 2 * p.bh;
-            ptx::tma_load_4d_2cta(tm, lead_full, dst, ccol, isA ? s - 1 : 0, h0 + (isA ? r - 1 : 0), n);
-          } else {
-#pragma unroll
-            for (int half = 0; half < 2; ++half) {
-              const int g = kb * 2 + half;
-              const int n = g / p.sb_per_img;
-              const int h0 = (g - n * p.sb_per_img) * p.bh;
-              ptx::tma_load_4d_2cta(tm, lead_full, dst + half * 4096, ccol, isA ? s - 1 : 0, h0 + (isA ? r - 1 : 0), n);
-            }
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp_idx == 1) {
-    if (leader && lane == 0) {
-      int stage = 0; uint32_t phase = 0; int it = 0;
-      for (int item = cluster_id; item < num_items; item += num_clusters, ++it) {
-        int tap, m_blk, n_blk, kb0, kb1;
-        decode(item, tap, m_blk, n_blk, kb0, kb1);
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        ptx::mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        ptx::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          ptx::tc_fence_after();
-          const uint64_t a_desc = make_desc_mn_sw128(ptx::smem_u32(smem_a + stage * A_STAGE));
-          const uint64_t b_desc = make_desc_mn_sw128(ptx::smem_u32(smem_b + stage * B_STAGE));
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / 16; ++k)
-            ptx::mma_f16_ss_2cta(d_tmem, a_desc + 128 * k, b_desc + 128 * k, IDESC, (kb > kb0 || k > 0) ? 1u : 0u);
-          ptx::tc_commit_2cta_mc(&empty_bar[stage], 3);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        ptx::tc_commit_2cta_mc(&tmem_full[acc], 3);
-      }
-    }
-    __syncwarp();
-  } else {
-    const int q = warp_idx & 3;
-    const int row = q * 32 + lane;
-    int it = 0;
-    for (int item = cluster_id; item < num_items; item += num_clusters, ++it) {
-      int tap, m_blk, n_blk, kb0, kb1;
-      decode(item, tap, m_blk, n_blk, kb0, kb1);
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      ptx::mbar_wait(&tmem_full[acc], acc_phase);
-      ptx::tc_fence_after();
-      const uint32_t tbase = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BLOCK_N;
-      const int m = m_blk * 256 + (int)rank * 128 + row;
-      const bool okm = (m < p.M) && (kb1 > kb0);
-      float* orow = p.out + (long long)tap * p.tap_stride + (long long)(m + p.out_row_offset) * p.ldo;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
-        uint32_t v[32];
-        ptx::tmem_ld_32x32b_x32(tbase + c0, v);
-        ptx::tmem_ld_wait();
-        const int ncol = n_blk * BLOCK_N + c0;
-        if (okm && ncol < p.N) {
-          float* dst;
-          if (p.lstm_cols) {
-            const int dir = ncol >> 10, pc = ncol & 1023;
-            const int g = (pc & 127) >> 5, ub = pc >> 7;
-            dst = orow + (long long)dir * p.dir_stride + g * 256 + ub * 32;
-          } else {
-            dst = orow + ncol;
-          }
-          // split-K reduction straight into the gradient tensor: 128-bit vector reds (a quarter of the L2 atomic transactions of
-          // scalar atomicAdd; every destination is 16-byte aligned: tensor offsets, row strides and column starts are multiples of 4)
-#pragma unroll
-          for (int i = 0; i < 32; i += 4)
-            ptx::red_add_v4_f32(dst + i, __uint_as_float(v[i]), __uint_as_float(v[i + 1]), __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
-        }
-      }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&tmem_empty[acc]), 0));
-    }
-  }
-
-  ptx::tc_fence_before();
-  ptx::cluster_sync_all();
-  if (warp_idx == 1) { ptx::tc_fence_after(); ptx::tmem_dealloc_2cta(tmem_base, TMEM_COLS); }
-}
 
 }  // namespace gemm_tn

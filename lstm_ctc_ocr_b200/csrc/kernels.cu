@@ -35,7 +35,7 @@ __global__ void __launch_bounds__(256) conv1_pool_kernel(const float* __restrict
   const int slot = warp * 4 + (lane >> 3);          // 0..31
 
   // taps as f32x2 pairs of adjacent channels: the 288 FMAs per pooled position issue as 144 FFMA2 (the 3-register FFMA
-  // issues every other cycle per scheduler on sm_100, so the scalar loop sat at its ~37 TFLOP/s ceiling)
+  // issues every other cycle per scheduler, which caps the scalar loop)
   uint64_t wr[9][4];
   float br[8];
 #pragma unroll

@@ -1,4 +1,4 @@
-// Persistent BiLSTM recurrence for sm_100a: one thread-block CLUSTER per (direction, 128-sample batch tile).
+// Persistent BiLSTM recurrence for sm_90a: one thread-block CLUSTER per (direction, 128-sample batch tile).
 //
 // Replaces the tf.while_loop of tf.contrib.rnn.LSTMCell(256) under bidirectional_dynamic_rnn
 // (lib/networks/network.py:104-107): per step  z = x_t W_x + b (precomputed, `xproj`) + h_{t-1} W_h ;
@@ -8,15 +8,15 @@
 //   lstm_mc_kernel<CS, MODE, EW>   (further down; the default, MODE 2 = "ms") -- h exchanged as 8 KB slices that land directly in
 //                                  every CTA's no-swizzle A operand, signalled through mbarriers; no cluster barrier per step
 //   lstm_persistent_kernel<CS>     (first, below; CRNN_LSTM_IMPL=persistent) -- h through global memory, a 64 KB TMA fetch per CTA,
-//                                  fence.proxy.async and one barrier.cluster per step; its measured step timeline is the
+//                                  fence.proxy.async and one barrier.cluster per step; those per-step costs are the
 //                                  reason the second generation exists (see the comment above lstm_mc_kernel)
 //
 // First generation:
 // Cluster of CS CTAs; CTA `rank` owns UPC = 256/CS hidden units (4*UPC gate columns, ordered [i|j|f|o]):
 //   * its W_h slice [4*UPC x 256] bf16 stays resident in shared memory for all T steps (loaded once by TMA)
 //   * per step: TMA loads h_{t-1} [128 x 256] (written to global/L2 by the whole cluster in the previous step),
-//     one elected thread issues 16 tcgen05.mma (128 x 4*UPC x 16) into TMEM, 4 epilogue warps (thread = sample row)
-//     add the precomputed input projection (prefetched to registers before the MMA wait), run the cell with the
+//     two MMA warpgroups issue 16 wgmma (64 x 4*UPC x 16 each), the accumulators are staged in shared memory, 4 epilogue
+//     warps (thread = sample row) add the precomputed input projection (prefetched before the MMA), run the cell with the
 //     f32 cell state held in REGISTERS for the whole sequence, write h (bf16) for the next step and the output row
 //   * one barrier.cluster per step orders the h exchange (generic-proxy global stores -> fence.proxy.async ->
 //     release/acquire cluster barrier -> TMA loads of the next step)
@@ -27,10 +27,11 @@
 #include <cuda.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace lstm {
 
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = 384;     // warpgroup 0: TMA, warpgroups 1..2: MMA (rows 0..63 / 64..127); warps 4..7 epilogue
 constexpr int BLOCK_M = 128;
 
 struct Params {
@@ -68,7 +69,8 @@ struct Cfg {
   static constexpr int NCOLS = 4 * UPC;         // gate columns per CTA
   static constexpr int B_BYTES = 4 * NCOLS * 128;   // 4 K-blocks x [NCOLS rows x 128 B]
   static constexpr int A_BYTES = 4 * BLOCK_M * 128; // 4 K-blocks x [128 rows x 128 B]
-  static constexpr int BAR_OFFSET = A_BYTES + B_BYTES;
+  static constexpr int ACC_OFFSET = A_BYTES + B_BYTES;    // staged accumulators [128 rows][NCOLS] f32
+  static constexpr int BAR_OFFSET = ACC_OFFSET + BLOCK_M * NCOLS * 4;
   static constexpr int SMEM_BYTES = BAR_OFFSET + 128 + 1024;
 };
 
@@ -78,7 +80,6 @@ lstm_persistent_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_con
   static_assert(CS == 8, "register budget of the epilogue is sized for 32 units per CTA");
   using C = Cfg<CS>;
   constexpr int UPC = C::UPC, NCOLS = C::NCOLS;
-  constexpr uint32_t IDESC = ptx::make_idesc_bf16(BLOCK_M, NCOLS);
   constexpr int HALF = UPC / 2;                 // units processed per epilogue pass (register budget)
 
   extern __shared__ uint8_t smem_raw[];
@@ -87,8 +88,7 @@ lstm_persistent_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_con
   uint8_t* smem_b = smem + C::A_BYTES;
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + C::BAR_OFFSET);   // [4] one per K-block
   uint64_t* b_full = a_full + 4;
-  uint64_t* acc_full = b_full + 1;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_full + 1);
+  float* acc_tile = reinterpret_cast<float*>(smem + C::ACC_OFFSET);
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rank = (int)cluster_ctarank();
@@ -101,17 +101,9 @@ lstm_persistent_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_con
     ptx::prefetch_tmap(&tmW);
     for (int i = 0; i < 4; ++i) ptx::mbar_init(&a_full[i], 1);
     ptx::mbar_init(b_full, 1);
-    ptx::mbar_init(acc_full, 1);
     ptx::fence_barrier_init();
   }
-  if (warp_idx == 1) {
-    ptx::tmem_alloc(tmem_ptr, NCOLS);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   // resident recurrent weights: rows [dir*1024 + rank*NCOLS, +NCOLS) of Bh [2048, 256]
   if (warp_idx == 0 && lane == 0) {
@@ -120,46 +112,31 @@ lstm_persistent_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_con
       ptx::tma_load_2d(&tmW, b_full, smem_b + kb * NCOLS * 128, kb * 64, dir * 1024 + rank * NCOLS);
   }
 
-  // ---- per-thread epilogue state (warps 2..5): one sample row, UPC units, cell state in registers
+  // ---- per-thread epilogue state (warps 4..7): one sample row, UPC units, cell state in registers
   const int q = warp_idx & 3;
   const int row = q * 32 + lane;
   const int n = tile * BLOCK_M + row;
-  const bool is_epi = warp_idx >= 2;
+  const bool is_epi = warp_idx >= 4 && warp_idx < 8;
   const bool okn = is_epi && (n < p.Nimg);
   const int len = okn ? min(max(__ldg(p.seq_len + n), 0), p.T) : 0;
   float cst[UPC];
 #pragma unroll
   for (int i = 0; i < UPC; ++i) cst[i] = 0.f;
 
-  if (warp_idx == 1 && lane == 0) ptx::mbar_wait(b_full, 0);      // W_h slice resident before the first MMA / exit
+  if (warp_idx < 4) ptx::setmaxnreg_dec<40>();
+  else ptx::setmaxnreg_inc<232>();
+  if (warp_idx >= 4) ptx::mbar_wait(b_full, 0);      // W_h slice resident before the first MMA / exit
 
   for (int s = 0; s < p.T; ++s) {
-    if (warp_idx == 0) {
+    if (warp_idx < 4) {
       LSTM_TRACE(0);
-      if (lane < 4 && s > 0) {        // one lane per K-block: the four TMA issues overlap instead of serialising
+      if (warp_idx == 0 && lane < 4 && s > 0) {        // one lane per K-block: the four TMA issues overlap instead of serialising
         fence_proxy_async_all();
         const int hrow = ((s & 1) * 2 + dir) * p.Npad + tile * BLOCK_M;
         ptx::mbar_arrive_expect_tx(&a_full[lane], BLOCK_M * 128);
         ptx::tma_load_2d(&tmH, &a_full[lane], smem_a + lane * BLOCK_M * 128, lane * 64, hrow);
       }
       LSTM_TRACE(1);
-      __syncwarp();
-    } else if (warp_idx == 1) {
-      if (lane == 0 && s > 0) {
-        const uint32_t ph = (s - 1) & 1;
-        for (int kb = 0; kb < 4; ++kb) {
-          ptx::mbar_wait(&a_full[kb], ph);
-          if (kb == 0) LSTM_TRACE(2);
-          if (kb == 3) LSTM_TRACE(3);
-          ptx::tc_fence_after();
-          const uint64_t a_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_a + kb * BLOCK_M * 128));
-          const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_b + kb * NCOLS * 128));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) ptx::mma_f16_ss(tmem_base, a_desc + 2 * k, b_desc + 2 * k, IDESC, (kb | k) != 0);
-        }
-        ptx::tc_commit(acc_full);
-        LSTM_TRACE(4);
-      }
       __syncwarp();
     } else {
       const bool active = s < len;
@@ -171,13 +148,30 @@ lstm_persistent_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_con
 #pragma unroll
         for (int i = 0; i < UPC / 2; ++i) xp[i] = __ldg(src + i);
       }
-      if (warp_idx == 2) LSTM_TRACE(5);
+      if (warp_idx == 4) LSTM_TRACE(5);
       if (s > 0) {
-        ptx::mbar_wait(acc_full, (s - 1) & 1);
-        ptx::tc_fence_after();
+        // ===================== MMA: both warpgroups, rows wgi*64 .. =====================
+        const int wgi = (warp_idx >> 2) - 1;
+        const uint32_t ph = (s - 1) & 1;
+        float d[NCOLS / 2];
+        for (int kb = 0; kb < 4; ++kb) {
+          ptx::mbar_wait(&a_full[kb], ph);
+          if (kb == 0 && warp_idx == 4) LSTM_TRACE(2);
+          if (kb == 3 && warp_idx == 4) LSTM_TRACE(3);
+          const uint64_t a_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_a + kb * BLOCK_M * 128 + wgi * 64 * 128));
+          const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_b + kb * NCOLS * 128));
+          wg::fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wg::mma_bf16<NCOLS>(d, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
+          wg::commit();
+        }
+        wg::wait<0>();
+        wg::fence_operand(d);
+        if (warp_idx == 4) LSTM_TRACE(4);
+        ptx::acc_store<NCOLS, NCOLS>(acc_tile, d, wgi * 64);
+        ptx::bar_sync(1, 256);
       }
-      if (warp_idx == 2) LSTM_TRACE(6);
-      const uint32_t tbase = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
+      if (warp_idx == 4) LSTM_TRACE(6);
       __nv_bfloat16* hn = p.h_state + ((size_t)(((s + 1) & 1) * 2 + dir) * p.Npad + n) * 256 + rank * UPC;
       __nv_bfloat16* lo = p.lstm_out + ((size_t)n * p.H + t) * 512 + dir * 256 + rank * UPC;
       const uint32_t* xw = reinterpret_cast<const uint32_t*>(xp);    // gate g, unit u -> bf16 index g*UPC + u
@@ -185,13 +179,12 @@ lstm_persistent_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_con
       for (int hh = 0; hh < 2; ++hh) {
         const int u0 = hh * HALF;
         uint32_t gi[HALF], gj[HALF], gf[HALF], go[HALF];
-        if (s > 0) {
-          ptx::tmem_ld_32x32b_x16(tbase + 0 * UPC + u0, gi);
-          ptx::tmem_ld_32x32b_x16(tbase + 1 * UPC + u0, gj);
-          ptx::tmem_ld_32x32b_x16(tbase + 2 * UPC + u0, gf);
-          ptx::tmem_ld_32x32b_x16(tbase + 3 * UPC + u0, go);
-          ptx::tmem_ld_wait();
-          if (warp_idx == 2 && hh == 0) LSTM_TRACE(7);
+        if (s > 0 && is_epi) {
+          ptx::acc_ld<NCOLS, HALF>(acc_tile, row, 0 * UPC + u0, gi);
+          ptx::acc_ld<NCOLS, HALF>(acc_tile, row, 1 * UPC + u0, gj);
+          ptx::acc_ld<NCOLS, HALF>(acc_tile, row, 2 * UPC + u0, gf);
+          ptx::acc_ld<NCOLS, HALF>(acc_tile, row, 3 * UPC + u0, go);
+          if (warp_idx == 4 && hh == 0) LSTM_TRACE(7);
         } else {
 #pragma unroll
           for (int i = 0; i < HALF; ++i) { gi[i] = 0u; gj[i] = 0u; gf[i] = 0u; go[i] = 0u; }
@@ -246,35 +239,27 @@ lstm_persistent_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_con
         }
       }
       // make this thread's h stores visible to the async proxy (TMA loads of the next step) of the whole cluster
-      if (warp_idx == 2) LSTM_TRACE(8);
+      if (warp_idx == 4) LSTM_TRACE(8);
       fence_proxy_async_all();
-      ptx::tc_fence_before();
-      if (warp_idx == 2) LSTM_TRACE(9);
+      if (warp_idx == 4) LSTM_TRACE(9);
     }
     cluster_arrive_release();
-    if (warp_idx == 2) LSTM_TRACE(10);
+    if (warp_idx == 4) LSTM_TRACE(10);
     cluster_wait_acquire();
-    if (warp_idx == 2) LSTM_TRACE(11);
-  }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, NCOLS);
+    if (warp_idx == 4) LSTM_TRACE(11);
   }
 }
 
 
 // ---------------------------------------------------------------------------------------------------------------------------
 // v2: the same recurrence WITHOUT a cluster barrier (and without fence.proxy.async + a 64 KB TMA fetch per CTA) on the
-// per-step critical path.  Measured timeline of the v1 kernel above (clock64, B200, one step = 8866 cycles): producer-side
-// fence.proxy.async 2117, 64 KB TMA 1441, MMA tail 469, cell epilogue 2360, epilogue-side fence.proxy.async 1304,
-// barrier.cluster arrive(release)+wait 1012.
+// per-step critical path.  A step of the v1 kernel above serialises a producer-side fence.proxy.async, a 64 KB TMA fetch, the
+// MMA, the cell epilogue, an epilogue-side fence.proxy.async and a barrier.cluster arrive(release)+wait (CRNN_LSTM_TRACE=1 prints
+// the clock64 timeline).
 //
 //   * the A operand (h_{t-1}, [128 rows x 256]) lives in shared memory WITHOUT swizzle as [32 K-chunks][128 rows][16 B]
 //     (8-row x 16-B core matrices, LBO = 2048, SBO = 128), so the 32 units one CTA produces are ONE contiguous 8 KB slice
-//   * 8 epilogue warps (2 per TMEM lane quadrant, 16 units each) run the cell and write their h_t slice
+//   * 8 epilogue warps (2 per 32-row quadrant, 16 units each) run the cell and write their h_t slice
 //       DS = true : straight into this CTA's own copy of the next A buffer (st.shared), then 7 bulk copies
 //                   shared::cta -> shared::cluster push the slice into the peers' A buffers and credit THEIR mbarriers
 //       DS = false: into a private 8 KB global buffer, then one bulk copy global -> shared::cluster with cluster MULTICAST
@@ -282,15 +267,13 @@ lstm_persistent_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_con
 //   * the MMA thread of each CTA waits on its own mbarrier (8 slices) and goes; nobody waits for a cluster barrier
 //   * A is double buffered: a slice of h_t can only be sent after its sender saw h_{t-1} from every CTA, i.e. after every CTA's
 //     MMA of step t-1 (the last reader of that buffer) has completed -- causality replaces a "buffer free" handshake
-//   * the accumulator is single buffered for the same reason (MMA t+1 needs this CTA's own h_t, sent after its TMEM reads)
+//   * the accumulator is single buffered for the same reason (MMA t+1 needs this CTA's own h_t, sent after its accumulator reads)
 // Global exchange buffer (DS = false): p.h_state viewed as [2 bufs][2*tiles_per_dir units][8 ranks][8 KB].
-// EW epilogue warps (8 or 16): EW/4 per TMEM lane quadrant, each owning 32/(EW/4) of the CTA's units.  The cell is a chain of
-// MUFU latencies (ncu: XU pipe 22 %, issue slots 22 % busy), but 16 warps x 8 units measured SLOWER than 8 x 16 on the B200
-// (0.422 vs 0.402 ms: the longer 512-thread barrier and 4 tcgen05.ld per 8 units eat the gain); model.cu instantiates EW = 8.
+// EW = 8 epilogue warps = the two MMA warpgroups: two per 32-row quadrant, each owning 16 of the CTA's units.
 template <int EW>
 struct McThreads {
   static constexpr int EPI = EW * 32;
-  static constexpr int ALL = 64 + EPI;       // warp 0 setup, warp 1 MMA, warps 2.. epilogue
+  static constexpr int ALL = 128 + EPI;      // warpgroup 0 setup, warps 4.. MMA (two warpgroups) + epilogue
 };
 
 template <int CS>
@@ -300,7 +283,8 @@ struct CfgMc {
   static constexpr int B_BYTES = 4 * NCOLS * 128;         // resident W_h slice (SW128 K-major, 4 K-blocks of 64)
   static constexpr int A_BYTES = 32 * BLOCK_M * 16;       // [32 K-chunks][128 rows][16 B] = 64 KB per buffer
   static constexpr int SLICE_BYTES = A_BYTES / CS;        // 8 KB: the 4 K-chunks one CTA produces
-  static constexpr int BAR_OFFSET = 2 * A_BYTES + B_BYTES;
+  static constexpr int ACC_OFFSET = 2 * A_BYTES + B_BYTES;  // half of the accumulators [128 rows][4 gates x 16 units] f32
+  static constexpr int BAR_OFFSET = ACC_OFFSET + BLOCK_M * 64 * 4;
   static constexpr int SMEM_BYTES = BAR_OFFSET + 128 + 1024;
 };
 
@@ -321,10 +305,9 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
   static_assert(CS == 8, "8 CTAs x 32 units");
   using C = CfgMc<CS>;
   constexpr int UPC = C::UPC, NCOLS = C::NCOLS;
-  constexpr uint32_t IDESC = ptx::make_idesc_bf16(BLOCK_M, NCOLS);
-  constexpr int HALF = UPC / (EW / 4);                      // units per epilogue warp (16 or 8)
+  constexpr int HALF = UPC / (EW / 4);                      // units per epilogue warp
   constexpr int MC_EPI_THREADS = McThreads<EW>::EPI;
-  static_assert(EW == 8 || EW == 16, "epilogue warps");
+  static_assert(EW == 8, "epilogue warps = the two MMA warpgroups");
   constexpr bool DS = (MODE == 1), MS = (MODE == 2), GX = (MODE == 3), LOCAL = DS || MS;   // LOCAL: own slice written in place
   constexpr uint32_t FILL_TX = LOCAL ? (CS - 1) * C::SLICE_BYTES : C::A_BYTES;
 
@@ -334,9 +317,8 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
   uint8_t* smem_b = smem + 2 * C::A_BYTES;
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + C::BAR_OFFSET);   // [2] one per A buffer
   uint64_t* b_full = a_full + 2;
-  uint64_t* acc_full = b_full + 1;
-  uint64_t* part_ready = acc_full + 1;                      // [2] GX: the 8 CTAs' slices of one h buffer are in L2
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(part_ready + 2);
+  uint64_t* part_ready = b_full + 1;                      // [2] GX: the 8 CTAs' slices of one h buffer are in L2
+  float* acc_half = reinterpret_cast<float*>(smem + C::ACC_OFFSET);
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rank = (int)cluster_ctarank();
@@ -352,7 +334,6 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
     ptx::mbar_init(&a_full[0], GX ? MC_EPI_THREADS : LOCAL ? 2 : 1);      // GX: every epilogue thread copied its part of the tile
     ptx::mbar_init(&a_full[1], GX ? MC_EPI_THREADS : LOCAL ? 2 : 1);
     ptx::mbar_init(b_full, 1);
-    ptx::mbar_init(acc_full, 1);
     ptx::fence_barrier_init();
     // first fills: buffer 1 receives h_0 (consumed at step 1), buffer 0 receives h_1 (consumed at step 2)
     if (!GX && p.T > 1) ptx::mbar_arrive_expect_tx(&a_full[1], FILL_TX);
@@ -361,45 +342,19 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
     for (int kb = 0; kb < 4; ++kb)
       ptx::tma_load_2d(&tmW, b_full, smem_b + kb * NCOLS * 128, kb * 64, dir * 1024 + rank * NCOLS);
   }
-  if (warp_idx == 1) {
-    ptx::tmem_alloc(tmem_ptr, NCOLS);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   // peers write into this CTA's smem and credit its mbarriers: everything above must be in place cluster-wide first
   cluster_arrive_release();
   cluster_wait_acquire();
 
-  if (warp_idx == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      ptx::mbar_wait(b_full, 0);
-      for (int s = 1; s < p.T; ++s) {
-        const int b = s & 1;
-        ptx::mbar_wait(&a_full[b], ((s - 1) >> 1) & 1);
-        LSTM_TRACE(3);
-        ptx::tc_fence_after();
-        // next fill of this buffer is h_{s+1}, consumed at step s+2; its senders are all behind this wait (see header)
-        if (!GX && s + 2 < p.T) ptx::mbar_arrive_expect_tx(&a_full[b], FILL_TX);
-        const uint32_t a_base = ptx::smem_u32(smem_a + b * C::A_BYTES);
-#pragma unroll
-        for (int k = 0; k < 16; ++k) {
-          const uint64_t a_desc = p.swap_ls ? ptx::make_desc_k_nosw(a_base + k * 4096, 128, 2048) : ptx::make_desc_k_nosw(a_base + k * 4096, 2048, 128);
-          const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_b + (k >> 2) * NCOLS * 128)) + 2 * (k & 3);
-          ptx::mma_f16_ss(tmem_base, a_desc, b_desc, IDESC, k != 0);
-        }
-        ptx::tc_commit(acc_full);
-        LSTM_TRACE(4);
-      }
-    }
-    __syncwarp();
-  } else if (warp_idx >= 2) {
-    // ===================== epilogue: thread = (sample row, 16 of the CTA's 32 units); cell state in registers =====================
+  if (warp_idx < 4) {
+    ptx::setmaxnreg_dec<40>();
+  } else {
+    // ===================== MMA (rows wgi*64 ..) + epilogue: thread = (sample row, 16 of the CTA's 32 units); cell state in registers
+    ptx::setmaxnreg_inc<232>();
+    const int wgi = (warp_idx >> 2) - 1;
     const int q = warp_idx & 3;
-    const int hh = (warp_idx - 2) >> 2;               // which HALF-unit group of the CTA's units
+    const int hh = (warp_idx - 4) >> 2;               // which HALF-unit group of the CTA's units
     const int u0 = hh * HALF;
     const int row = q * 32 + lane;
     const int n = tile * BLOCK_M + row;
@@ -408,7 +363,7 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
     float cst[HALF];
 #pragma unroll
     for (int i = 0; i < HALF; ++i) cst[i] = 0.f;
-    const uint32_t tbase = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
+    ptx::mbar_wait(b_full, 0);
     // this thread's HALF/8 x 16 B of the h slice: K-chunks u0/8 .. at chunk*2048 + row*16 inside the CTA's 8 KB slice
     const uint32_t slice_off = rank * C::SLICE_BYTES + (u0 / 8) * 2048 + row * 16;
     uint8_t* hx0 = reinterpret_cast<uint8_t*>(p.h_state) + ((size_t)unit * CS + rank) * C::SLICE_BYTES;
@@ -426,25 +381,52 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
 #pragma unroll
           for (int v = 0; v < HALF / 8; ++v) xp[g][v] = __ldg(reinterpret_cast<const uint4*>(src + g * UPC) + v);
       }
-      if (warp_idx == 2) LSTM_TRACE(5);
+      if (warp_idx == 4) LSTM_TRACE(5);
       uint32_t gi[HALF], gj[HALF], gf[HALF], go[HALF];
       if (s > 0) {
-        ptx::mbar_wait(acc_full, (s - 1) & 1);
-        ptx::tc_fence_after();
-        if (warp_idx == 2) LSTM_TRACE(6);
-        if constexpr (HALF == 16) {
-          ptx::tmem_ld_32x32b_x16(tbase + 0 * UPC + u0, gi);
-          ptx::tmem_ld_32x32b_x16(tbase + 1 * UPC + u0, gj);
-          ptx::tmem_ld_32x32b_x16(tbase + 2 * UPC + u0, gf);
-          ptx::tmem_ld_32x32b_x16(tbase + 3 * UPC + u0, go);
-        } else {
-          ptx::tmem_ld_32x32b_x8(tbase + 0 * UPC + u0, gi);
-          ptx::tmem_ld_32x32b_x8(tbase + 1 * UPC + u0, gj);
-          ptx::tmem_ld_32x32b_x8(tbase + 2 * UPC + u0, gf);
-          ptx::tmem_ld_32x32b_x8(tbase + 3 * UPC + u0, go);
+        const int b = s & 1;
+        ptx::mbar_wait(&a_full[b], ((s - 1) >> 1) & 1);
+        if (warp_idx == 4) LSTM_TRACE(3);
+        // next fill of this buffer is h_{s+1}, consumed at step s+2; its senders are all behind this wait (see header)
+        if (!GX && s + 2 < p.T && threadIdx.x == 128) ptx::mbar_arrive_expect_tx(&a_full[b], FILL_TX);
+        const uint32_t a_base = ptx::smem_u32(smem_a + b * C::A_BYTES) + wgi * 64 * 16;
+        float d[NCOLS / 2];
+        wg::fence();
+#pragma unroll
+        for (int k = 0; k < 16; ++k) {
+          const uint64_t a_desc = p.swap_ls ? ptx::make_desc_k_nosw(a_base + k * 4096, 128, 2048) : ptx::make_desc_k_nosw(a_base + k * 4096, 2048, 128);
+          const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_b + (k >> 2) * NCOLS * 128)) + 2 * (k & 3);
+          wg::mma_bf16<NCOLS>(d, a_desc, b_desc, k != 0);
         }
-        ptx::tmem_ld_wait();
-        if (warp_idx == 2) LSTM_TRACE(7);
+        wg::commit();
+        wg::wait<0>();
+        wg::fence_operand(d);
+        if (warp_idx == 4) LSTM_TRACE(4);
+        // the accumulators go through shared memory in two halves (units 0..15, then 16..31 of every gate): staged columns
+        // [gate][16 units]; the warps with hh == r read their rows of half r
+        const int tt = threadIdx.x & 127, l = tt & 31;
+        const int r0 = wgi * 64 + 16 * (tt >> 5) + (l >> 2);
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          ptx::bar_sync(1, MC_EPI_THREADS);            // the other half's reads are done
+#pragma unroll
+          for (int g = 0; g < 4; ++g)
+#pragma unroll
+            for (int jj = 0; jj < 2; ++jj) {
+              const int j = 4 * g + 2 * r + jj;          // fragment column group: gate g, units 16r + 8jj ..
+              const int c = g * 16 + jj * 8 + 2 * (l & 3);
+              *reinterpret_cast<float2*>(ptx::acc_chunk<64>(acc_half, r0, c >> 2) + (c & 3)) = make_float2(d[4 * j], d[4 * j + 1]);
+              *reinterpret_cast<float2*>(ptx::acc_chunk<64>(acc_half, r0 + 8, c >> 2) + (c & 3)) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+            }
+          ptx::bar_sync(1, MC_EPI_THREADS);
+          if (hh == r) {
+            ptx::acc_ld<64, HALF>(acc_half, row, 0, gi);
+            ptx::acc_ld<64, HALF>(acc_half, row, 16, gj);
+            ptx::acc_ld<64, HALF>(acc_half, row, 32, gf);
+            ptx::acc_ld<64, HALF>(acc_half, row, 48, go);
+          }
+        }
+        if (warp_idx == 4) LSTM_TRACE(7);
       } else {
 #pragma unroll
         for (int i = 0; i < HALF; ++i) { gi[i] = 0u; gj[i] = 0u; gf[i] = 0u; go[i] = 0u; }
@@ -484,7 +466,7 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
 #pragma unroll
           for (int v = 0; v < HALF / 8; ++v)
             *reinterpret_cast<uint4*>(dst + v * 2048) = make_uint4(hp[4 * v], hp[4 * v + 1], hp[4 * v + 2], hp[4 * v + 3]);
-          ptx::fence_proxy_async_smem();                    // generic-proxy smem writes -> async proxy (bulk copies, tcgen05.mma)
+          ptx::fence_proxy_async_smem();                    // generic-proxy smem writes -> async proxy (bulk copies, wgmma)
         } else {
           uint8_t* dst = hx0 + (size_t)nb * hx_buf_stride + (u0 / 8) * 2048 + row * 16;
 #pragma unroll
@@ -492,10 +474,9 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
             *reinterpret_cast<uint4*>(dst + v * 2048) = make_uint4(hp[4 * v], hp[4 * v + 1], hp[4 * v + 2], hp[4 * v + 3]);
           if (!GX) fence_proxy_async_all();                 // generic-proxy global writes -> async proxy (bulk copy)
         }
-        if (warp_idx == 2) LSTM_TRACE(8);
-        ptx::tc_fence_before();
+        if (warp_idx == 4) LSTM_TRACE(8);
         asm volatile("bar.sync 1, %0;" ::"n"(MC_EPI_THREADS) : "memory");
-        if (warp_idx == 2) {
+        if (warp_idx == 4) {
           uint8_t* my_slice = smem_a + nb * C::A_BYTES + rank * C::SLICE_BYTES;
           if (DS) {
             if (lane < CS) {
@@ -530,7 +511,7 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
           ptx::mbar_wait_cluster(&part_ready[nb], (uint32_t)(s >> 1) & 1u);
           const uint8_t* g = reinterpret_cast<const uint8_t*>(p.h_state) + (size_t)nb * hx_buf_stride + (size_t)unit * CS * C::SLICE_BYTES;
           uint8_t* d = smem_a + nb * C::A_BYTES;
-          const int et = threadIdx.x - 64;                       // 0 .. MC_EPI_THREADS-1
+          const int et = threadIdx.x - 128;                      // 0 .. MC_EPI_THREADS-1
           uint4 v[C::A_BYTES / 16 / MC_EPI_THREADS];
 #pragma unroll
           for (int k = 0; k < C::A_BYTES / 16 / MC_EPI_THREADS; ++k) v[k] = __ldcg(reinterpret_cast<const uint4*>(g) + k * MC_EPI_THREADS + et);
@@ -559,18 +540,13 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
 #pragma unroll
         for (int i = 0; i < HALF; i += 4) *reinterpret_cast<float4*>(cs + (i >> 2) * LSTM_CCHUNK_STRIDE) = make_float4(cst[i], cst[i + 1], cst[i + 2], cst[i + 3]);
       }
-      if (warp_idx == 2) LSTM_TRACE(10);
+      if (warp_idx == 4) LSTM_TRACE(10);
     }
   }
 
-  ptx::tc_fence_before();
   __syncthreads();
   cluster_arrive_release();          // no CTA leaves (and frees its smem / mbarriers) while a peer may still write into it
   cluster_wait_acquire();
-  if (warp_idx == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, NCOLS);
-  }
 }
 
 }  // namespace lstm

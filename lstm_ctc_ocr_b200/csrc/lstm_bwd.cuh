@@ -1,4 +1,4 @@
-// Persistent backward recurrence (BPTT) of the BiLSTM for sm_100a; mirror image of csrc/lstm.cuh.
+// Persistent backward recurrence (BPTT) of the BiLSTM for sm_90a; mirror image of csrc/lstm.cuh.
 //
 // Restates what tf.gradients produces for tf.contrib.rnn.LSTMCell under bidirectional_dynamic_rnn
 // (lib/networks/network.py:104-107, lib/lstm/train.py:82).  Per step s = T-1 .. 0 (step space: frame t = s for the
@@ -8,29 +8,29 @@
 //   dc_{s->s-1} = dc * f
 // Cluster of 8 CTAs per (direction, 128-sample tile); CTA `rank` owns 32 hidden units: it keeps dc for them in
 // registers, holds W_h[units, all 1024 gate columns] (64 KB bf16, K-major over gates) resident in shared memory, and per
-// step computes dh_rec[128 x 32] = dz_{s+1}[128 x 1024] * W_h^T on tensor cores (64 x tcgen05.mma 128x32x16), streaming
+// step computes dh_rec[128 x 32] = dz_{s+1}[128 x 1024] * W_h^T on tensor cores (one warpgroup, 2 x 64 wgmma 64x32x16), streaming
 // dz_{s+1} (written to global/L2 by the whole cluster one step earlier) through a 6-stage TMA ring.  The tile is identical
 // for the 8 CTAs of a cluster, so each K-block is read from L2 ONCE and TMA-multicast into all 8 shared memories.
-// (Two alternatives were built and measured on the B200 and were NOT faster -- the step is bound by its serial latency chain,
-// not by MMA count or exchange volume: splitting the product along K with the dz slice written straight into shared memory and
-// the 8 partial products reduced through L2 (1.98 ms) or through DSMEM inboxes (1.81 ms) vs this version (1.68 ms).)
+// (The step is bound by its serial latency chain, not by MMA count or exchange volume.)
 // Outputs: dz for every (sample, frame) in FRAME order (`dz_all`, consumed by the dW_x / dW_h / dx GEMMs).
 #pragma once
 #include <cuda.h>
 
 #include "common.cuh"
 #include "lstm.cuh"
+#include "wgmma.cuh"
 
 namespace lstm_bwd {
 
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = 256;               // warpgroup 0: TMA (warp 0), warpgroup 1: MMA + epilogue
 constexpr int BLOCK_M = 128;
 constexpr int CS = 8;
 constexpr int UPC = 32;
 constexpr int STAGES = 6;
 constexpr int B_BYTES = 16 * UPC * 128;          // 16 K-blocks x [32 rows x 128 B] = 64 KB
 constexpr int A_STAGE = BLOCK_M * 128;           // 16 KB
-constexpr int BAR_OFFSET = B_BYTES + STAGES * A_STAGE;
+constexpr int ACC_OFFSET = B_BYTES + STAGES * A_STAGE;   // staged accumulators [128 rows][32] f32
+constexpr int BAR_OFFSET = ACC_OFFSET + BLOCK_M * UPC * 4;
 constexpr int SMEM_BYTES = BAR_OFFSET + 256 + 1024;
 
 struct Params {
@@ -54,7 +54,6 @@ __device__ __forceinline__ void unpack8(const uint4 q, float* v) {
 
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constant__ CUtensorMap tmW, const Params p) {
-  constexpr uint32_t IDESC = ptx::make_idesc_bf16(BLOCK_M, UPC);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_b = smem;
@@ -62,8 +61,7 @@ lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constant_
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + BAR_OFFSET);
   uint64_t* a_empty = a_full + STAGES;
   uint64_t* b_full = a_empty + STAGES;
-  uint64_t* acc_full = b_full + 1;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_full + 1);
+  float* acc_tile = reinterpret_cast<float*>(smem + ACC_OFFSET);
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rank = (int)lstm::cluster_ctarank();
@@ -76,14 +74,9 @@ lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constant_
     ptx::prefetch_tmap(&tmW);
     for (int i = 0; i < STAGES; ++i) { ptx::mbar_init(&a_full[i], 1); ptx::mbar_init(&a_empty[i], CS); }   // slot free = all 8 CTAs consumed it
     ptx::mbar_init(b_full, 1);
-    ptx::mbar_init(acc_full, 1);
     ptx::fence_barrier_init();
   }
-  if (warp_idx == 1) { ptx::tmem_alloc(tmem_ptr, 32); ptx::tmem_relinquish(); }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp_idx == 0 && lane == 0) {      // resident W_h rows [dir*256 + rank*32, +32) x 1024 gate columns
     ptx::mbar_arrive_expect_tx(b_full, B_BYTES);
@@ -93,25 +86,24 @@ lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constant_
   const int q = warp_idx & 3;
   const int row = q * 32 + lane;
   const int n = tile * BLOCK_M + row;
-  const bool is_epi = warp_idx >= 2;
+  const bool is_epi = warp_idx >= 4;
   const bool okn = is_epi && (n < p.Nimg);
   const int len = okn ? min(max(__ldg(p.seq_len + n), 0), p.T) : 0;
   float dcr[UPC];
 #pragma unroll
   for (int i = 0; i < UPC; ++i) dcr[i] = 0.f;
 
-  if (warp_idx == 1 && lane == 0) ptx::mbar_wait(b_full, 0);
+  if (is_epi) ptx::mbar_wait(b_full, 0);
 
   uint32_t prod_parity = 0;  // producer lane l: parity of ring slot l (flips on every use of that slot)
-  uint32_t mma_parity = 0;   // MMA lane: bit s = parity of ring slot s
-  int nmma = 0;              // number of accumulations completed (acc_full parity)
+  uint32_t mma_parity = 0;   // MMA threads: bit s = parity of ring slot s
 
   for (int s = p.T - 1; s >= 0; --s) {
     const bool has_rec = (s < p.T - 1);
-    if (warp_idx == 0) {
+    if (warp_idx < 4) {
       // K-block kb of every step lives in ring slot kb % STAGES.  Lanes 0..STAGES-1 own one slot each and issue their
       // K-blocks in lock-step (one SIMD cp.async.bulk.tensor per round instead of 16 serial single-thread issues).
-      if (lane < STAGES && has_rec) {
+      if (warp_idx == 0 && lane < STAGES && has_rec) {
         lstm::fence_proxy_async_all();
         const int zrow = ((((s + 1) & 1) * 2 + dir) * p.Npad) + tile * BLOCK_M;
         for (int kb = lane; kb < 16; kb += STAGES) {
@@ -123,22 +115,6 @@ lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constant_
             ptx::tma_load_2d_mc(&tmDz, &a_full[lane], smem_a + lane * A_STAGE, kb * 64, zrow, (uint16_t)0xFF);
           prod_parity ^= 1;
         }
-      }
-      __syncwarp();
-    } else if (warp_idx == 1) {
-      if (lane == 0 && has_rec) {
-        for (int kb = 0; kb < 16; ++kb) {
-          const int slot = kb % STAGES;
-          ptx::mbar_wait(&a_full[slot], (mma_parity >> slot) & 1u);
-          mma_parity ^= (1u << slot);
-          ptx::tc_fence_after();
-          const uint64_t a_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_a + slot * A_STAGE));
-          const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_b + kb * UPC * 128));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) ptx::mma_f16_ss(tmem_base, a_desc + 2 * k, b_desc + 2 * k, IDESC, (kb | k) != 0);
-          ptx::tc_commit_mc(&a_empty[slot], (uint16_t)0xFF);
-        }
-        ptx::tc_commit(acc_full);
       }
       __syncwarp();
     } else {
@@ -156,10 +132,37 @@ lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constant_
         asm volatile("prefetch.global.L2 [%0];" ::"l"(p.d_out + ((size_t)n * p.H + tp) * 512 + dir * 256 + rank * UPC));
       }
       if (has_rec) {
-        ptx::mbar_wait(acc_full, nmma & 1);
-        ptx::tc_fence_after();
+        // dh_rec = dz_{s+1} * W_h^T: rows 0..63 and 64..127 as two accumulator sets of this warpgroup
+        float d0[UPC / 2], d1[UPC / 2];
+        int prev = -1;
+        for (int kb = 0; kb < 16; ++kb) {
+          const int slot = kb % STAGES;
+          ptx::mbar_wait(&a_full[slot], (mma_parity >> slot) & 1u);
+          mma_parity ^= (1u << slot);
+          const uint64_t a_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_a + slot * A_STAGE));
+          const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_b + kb * UPC * 128));
+          wg::fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            wg::mma_bf16<UPC>(d0, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
+            wg::mma_bf16<UPC>(d1, a_desc + (64 * 128 >> 4) + 2 * k, b_desc + 2 * k, (kb | k) != 0);
+          }
+          wg::commit();
+          wg::wait<1>();
+          // the slot is free once every CTA of the cluster has consumed it: one release arrive on each CTA's a_empty
+          if (prev >= 0 && threadIdx.x == 128 + 0)
+            for (int r = 0; r < CS; ++r) ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&a_empty[prev]), (uint32_t)r));
+          prev = slot;
+        }
+        wg::wait<0>();
+        wg::fence_operand(d0);
+        wg::fence_operand(d1);
+        if (threadIdx.x == 128)
+          for (int r = 0; r < CS; ++r) ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&a_empty[prev]), (uint32_t)r));
+        ptx::acc_store<UPC, UPC>(acc_tile, d0, 0);
+        ptx::acc_store<UPC, UPC>(acc_tile, d1, 64);
+        ptx::bar_sync(1, 128);
       }
-      const uint32_t tbase = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
       __nv_bfloat16* zs = p.dz_state + ((size_t)(((s & 1) * 2 + dir) * p.Npad) + n) * 1024 + rank * 128;
       __nv_bfloat16* za = p.dz_all + ((size_t)n * p.H + t) * 2048 + dir * 1024 + rank * 128;
 #pragma unroll
@@ -167,8 +170,7 @@ lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constant_
         const int u0 = hh * 16;
         uint32_t acc[16];
         if (has_rec) {
-          ptx::tmem_ld_32x32b_x16(tbase + u0, acc);
-          ptx::tmem_ld_wait();
+          ptx::acc_ld<UPC, 16>(acc_tile, row, u0, acc);
         } else {
 #pragma unroll
           for (int i = 0; i < 16; ++i) acc[i] = 0u;
@@ -224,17 +226,11 @@ lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constant_
           }
         }
       }
-      if (has_rec) ++nmma;
       lstm::fence_proxy_async_all();
-      ptx::tc_fence_before();
     }
     lstm::cluster_arrive_release();
     lstm::cluster_wait_acquire();
   }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) { ptx::tc_fence_after(); ptx::tmem_dealloc(tmem_base, 32); }
 }
 
 
@@ -242,37 +238,36 @@ lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constant_
 // v2 ("ks"): the same recurrence with the product split along K and NOTHING but generic-proxy traffic between CTAs.
 //
 // v1 above moves the whole dz_{s+1} tile (128 x 1024, 256 KB) into every CTA each step (multicast ring with cluster-wide slot
-// hand-shakes), issues 64 tcgen05.mma of N = 32 (an MMA instruction costs >= ~128 cycles whatever its N) and pays two
-// fence.proxy.async and a cluster barrier per step: 26 us per step.  Here CTA `rank` multiplies ONLY ITS OWN dz slice
+// hand-shakes), issues MMAs of N = 32 only and pays two
+// fence.proxy.async and a cluster barrier per step.  Here CTA `rank` multiplies ONLY ITS OWN dz slice
 // (128 x 128 gate columns, written by its own epilogue straight into shared memory as the no-swizzle A operand) with the
-// resident W_h[all 256 units, its 128 gate columns]: 8 tcgen05.mma of 128 x 256 x 16 give its partial dh for ALL units.  The
+// resident W_h[all 256 units, its 128 gate columns]: 8 wgmma of 64 x 256 x 16 per warpgroup give its partial dh for ALL units.  The
 // partials are exchanged all-to-all through L2 as bf16 (8 KB per (source, destination) pair): plain st.global, one
 // release.cluster arrive on every peer's mbarrier, acquire.cluster wait, ld.global.cg of the 8 partial rows, f32 sum --
 // no async proxy, no proxy fences, no cluster barrier on the critical path.
 //   X[buf = s & 1][unit][dst][src][128 rows][32 units] bf16 is the exchange buffer (double buffered: a source can only reach
 //   step s-2 after every peer finished reading step s, because its own step s-1 needs all peers' step s-1 partials).
 namespace ks {
-constexpr int NUM_THREADS = 320;                 // warp 0 setup, warp 1 MMA, warps 2..9 epilogue
+constexpr int NUM_THREADS = 384;                 // warpgroup 0 setup, warpgroups 1..2 MMA (rows 0..63 / 64..127) + epilogue
 constexpr int EPI_THREADS = 256;
 constexpr int B_BYTES = 2 * 256 * 128;           // 2 K-blocks x [256 unit rows x 128 B] (SW128) = 64 KB
 constexpr int A_BYTES = 16 * BLOCK_M * 16;       // [16 K-chunks][128 rows][16 B] = 32 KB, no swizzle
-constexpr int BAR_OFFSET = B_BYTES + A_BYTES;
+constexpr int ACC_OFFSET = B_BYTES + A_BYTES;    // staged accumulators [128 rows][256] f32
+constexpr int BAR_OFFSET = ACC_OFFSET + BLOCK_M * 256 * 4;
 constexpr int SMEM_BYTES = BAR_OFFSET + 128 + 1024;
 constexpr int PAIR_BYTES = BLOCK_M * UPC * 2;    // one (source, destination) block of partial sums: 8 KB
 }  // namespace ks
 
 __global__ void __launch_bounds__(ks::NUM_THREADS, 1)
 lstm_bwd_ks_kernel(const __grid_constant__ CUtensorMap tmW, const Params p, uint8_t* __restrict__ xbuf) {
-  constexpr uint32_t IDESC = ptx::make_idesc_bf16(BLOCK_M, 256);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* smem_b = smem;
   uint8_t* smem_a = smem + ks::B_BYTES;
+  float* acc_tile = reinterpret_cast<float*>(smem + ks::ACC_OFFSET);
   uint64_t* b_full = reinterpret_cast<uint64_t*>(smem + ks::BAR_OFFSET);
-  uint64_t* acc_full = b_full + 1;
-  uint64_t* a_ready = acc_full + 1;
+  uint64_t* a_ready = b_full + 1;
   uint64_t* part_ready = a_ready + 1;            // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(part_ready + 2);
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rank = (int)lstm::cluster_ctarank();
@@ -284,7 +279,6 @@ lstm_bwd_ks_kernel(const __grid_constant__ CUtensorMap tmW, const Params p, uint
   if (warp_idx == 0 && lane == 0) {
     ptx::prefetch_tmap(&tmW);
     ptx::mbar_init(b_full, 1);
-    ptx::mbar_init(acc_full, 1);
     ptx::mbar_init(a_ready, ks::EPI_THREADS);
     ptx::mbar_init(&part_ready[0], CS);
     ptx::mbar_init(&part_ready[1], CS);
@@ -293,43 +287,24 @@ lstm_bwd_ks_kernel(const __grid_constant__ CUtensorMap tmW, const Params p, uint
     ptx::mbar_arrive_expect_tx(b_full, ks::B_BYTES);
     for (int kb = 0; kb < 2; ++kb) ptx::tma_load_2d(&tmW, b_full, smem_b + kb * 256 * 128, rank * 128 + kb * 64, dir * 256);
   }
-  if (warp_idx == 1) { ptx::tmem_alloc(tmem_ptr, 256); ptx::tmem_relinquish(); }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   lstm::cluster_arrive_release();                  // peers arrive on this CTA's part_ready barriers
   lstm::cluster_wait_acquire();
 
-  if (warp_idx == 1) {
-    // ===================== MMA issuer: partial dh[128 x 256] = dz_{s+1}[128 x own 128 gate columns] * W_h^T =====================
-    if (lane == 0) {
-      ptx::mbar_wait(b_full, 0);
-      for (int s = p.T - 2; s >= 0; --s) {
-        const uint32_t ph = (uint32_t)(p.T - 2 - s) & 1u;
-        ptx::mbar_wait(a_ready, ph);
-        ptx::tc_fence_after();
-        const uint32_t a_base = ptx::smem_u32(smem_a);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const uint64_t a_desc = ptx::make_desc_k_nosw(a_base + k * 4096, 2048, 128);
-          const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_b + (k >> 2) * 256 * 128)) + 2 * (k & 3);
-          ptx::mma_f16_ss(tmem_base, a_desc, b_desc, IDESC, k != 0);
-        }
-        ptx::tc_commit(acc_full);
-      }
-    }
-    __syncwarp();
-  } else if (warp_idx >= 2) {
-    // ===================== epilogue: thread = (sample row, half) =====================
+  if (warp_idx < 4) {
+    ptx::setmaxnreg_dec<40>();
+  } else {
+    // ===================== MMA: partial dh[128 x 256] = dz_{s+1}[128 x own 128 gate columns] * W_h^T; epilogue: thread = (sample row, half)
+    ptx::setmaxnreg_inc<232>();
+    const int wgi = (warp_idx >> 2) - 1;           // MMA rows wgi*64 ..
     const int q = warp_idx & 3;
-    const int hh = (warp_idx - 2) >> 2;            // exchange: destination CTAs hh*4 .. hh*4+3; cell: units hh*16 .. +16 of this CTA
+    const int hh = (warp_idx - 4) >> 2;            // exchange: destination CTAs hh*4 .. hh*4+3; cell: units hh*16 .. +16 of this CTA
     const int u0 = hh * 16;
     const int row = q * 32 + lane;
     const int n = tile * BLOCK_M + row;
     const bool okn = n < p.Nimg;
     const int len = okn ? min(max(__ldg(p.seq_len + n), 0), p.T) : 0;
-    const uint32_t tbase = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + hh * 128;
+    ptx::mbar_wait(b_full, 0);
     float dcr[16];
 #pragma unroll
     for (int i = 0; i < 16; ++i) dcr[i] = 0.f;
@@ -357,14 +332,28 @@ lstm_bwd_ks_kernel(const __grid_constant__ CUtensorMap tmW, const Params p, uint
       if (has_rec) {
         const int b = s & 1;
         uint8_t* xb = x_unit + (size_t)b * buf_stride;
-        ptx::mbar_wait(acc_full, (uint32_t)(p.T - 2 - s) & 1u);
-        ptx::tc_fence_after();
+        ptx::mbar_wait(a_ready, (uint32_t)(p.T - 2 - s) & 1u);
+        {
+          float d[128];
+          const uint32_t a_base = ptx::smem_u32(smem_a) + wgi * 64 * 16;
+          wg::fence();
+#pragma unroll
+          for (int k = 0; k < 8; ++k) {
+            const uint64_t a_desc = ptx::make_desc_k_nosw(a_base + k * 4096, 2048, 128);
+            const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_b + (k >> 2) * 256 * 128)) + 2 * (k & 3);
+            wg::mma_bf16<256>(d, a_desc, b_desc, k != 0);
+          }
+          wg::commit();
+          wg::wait<0>();
+          wg::fence_operand(d);
+          ptx::acc_store<256, 256>(acc_tile, d, wgi * 64);
+        }
+        ptx::bar_sync(1, ks::EPI_THREADS);
         // ---- this CTA's partial sums for destinations hh*4 .. hh*4+3 -> X[dst][src = rank][row]
 #pragma unroll 1
         for (int jj = 0; jj < 4; ++jj) {
           uint32_t v[32];
-          ptx::tmem_ld_32x32b_x32(tbase + jj * 32, v);
-          ptx::tmem_ld_wait();
+          ptx::acc_ld<256, 32>(acc_tile, row, hh * 128 + jj * 32, v);
           uint32_t w[16];
 #pragma unroll
           for (int i = 0; i < 16; ++i) w[i] = ptx::pack_bf16x2(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1]));
@@ -372,10 +361,9 @@ lstm_bwd_ks_kernel(const __grid_constant__ CUtensorMap tmW, const Params p, uint
           ptx::st_global_v8(dst, w[0], w[1], w[2], w[3], w[4], w[5], w[6], w[7]);
           ptx::st_global_v8(dst + 32, w[8], w[9], w[10], w[11], w[12], w[13], w[14], w[15]);
         }
-        ptx::tc_fence_before();
         asm volatile("bar.sync 1, %0;" ::"n"(ks::EPI_THREADS) : "memory");
         // one release.cluster arrive per peer (cumulative over the barrier above: covers every thread's stores)
-        if (warp_idx == 2 && lane < CS) ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&part_ready[b]), (uint32_t)lane));
+        if (warp_idx == 4 && lane < CS) ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&part_ready[b]), (uint32_t)lane));
       }
       // saved forward state of this step: issued before the exchange wait so that its latency hides behind it
       uint4 qg[4][2], qd[2];
@@ -462,11 +450,9 @@ lstm_bwd_ks_kernel(const __grid_constant__ CUtensorMap tmW, const Params p, uint
     }
   }
 
-  ptx::tc_fence_before();
   __syncthreads();
   lstm::cluster_arrive_release();                  // no CTA leaves while a peer may still arrive on its barriers
   lstm::cluster_wait_acquire();
-  if (warp_idx == 1) { ptx::tc_fence_after(); ptx::tmem_dealloc(tmem_base, 256); }
 }
 
 }  // namespace lstm_bwd

@@ -176,12 +176,11 @@ extern "C" int crnn_model_create(const crnn_config* cfg, crnn_model** out) {
     delete m;
     return crnn_fail(CRNN_CUDA_ERROR, "model_create: no CUDA device (this library has no CPU fallback)");
   }
-  if (prop.major != 10) {
+  if (prop.major != 9) {
     delete m;
-    return crnn_fail(CRNN_UNSUPPORTED, "model_create: needs sm_100 (found sm_%d%d)", prop.major, prop.minor);
+    return crnn_fail(CRNN_UNSUPPORTED, "model_create: needs sm_90 (found sm_%d%d)", prop.major, prop.minor);
   }
   m->num_sms = prop.multiProcessorCount;
-  if (const char* e = getenv("CRNN_GEMM2")) m->use_2cta = std::string(e) != "0";
   if (const char* e = getenv("CRNN_BPTT")) m->bptt_ks = std::string(e) != "ring";        // debug A/B switch
   if (const char* e = getenv("CRNN_CONV1")) m->conv1_tc = std::string(e) != "simt";    // debug A/B switch
   if (const char* e = getenv("CRNN_BN_FUSE")) m->bn_red_fused = std::string(e) != "0";            // debug A/B switch
@@ -217,13 +216,6 @@ extern "C" int crnn_model_create(const crnn_config* cfg, crnn_model** out) {
   if (st == CRNN_OK) st = make_tmap_2d(&m->tB_h, m->Bh, 2048, 256, 256, 256);
   if (st == CRNN_OK) st = make_tmap_2d(&m->tB_h128, m->Bh, 2048, 256, 256, 128);
   if (st == CRNN_OK) st = make_tmap_2d(&m->tB_l, m->Bl, 64, 512, 512, 64);
-  if (st == CRNN_OK) st = make_tmap_2d(&m->tBh_c2, m->Bc2, 128, 576, 576, 64);
-  if (st == CRNN_OK) st = make_tmap_2d(&m->tBh_c31, m->Bc31, 256, 1152, 1152, 128);
-  if (st == CRNN_OK) st = make_tmap_2d(&m->tBh_c32, m->Bc32, 256, 2304, 2304, 128);
-  if (st == CRNN_OK) st = make_tmap_2d(&m->tBh_c41, m->Bc41, 512, 2304, 2304, 128);
-  if (st == CRNN_OK) st = make_tmap_2d(&m->tBh_c42, m->Bc42, 512, 4608, 4608, 128);
-  if (st == CRNN_OK) st = make_tmap_2d(&m->tBh_c5, m->Bc5, 512, 2048, 2048, 128);
-  if (st == CRNN_OK) st = make_tmap_2d(&m->tBh_x, m->Bx, 2048, 512, 512, 128);
   if (st != CRNN_OK) { cudaFree(m->wblock); delete m; return st; }
   *out = m;
   return CRNN_OK;
@@ -433,7 +425,7 @@ int ensure_plan(crnn_model* m, int N, int W, void* ws, cudaStream_t st) {
 }
 
 // ---- host-side copy pool (crnn_forward_pageable): a pageable numpy batch has to be moved into page-locked staging before it can
-// be DMA'd; one thread moves 33.6 MB at 4-10 GB/s (3-8 ms, longer than the whole GPU step).  A few persistent workers split every
+// be DMA'd; one host thread alone takes longer for the 33.6 MB of a batch than the whole GPU step.  A few persistent workers split every
 // copy; the caller copies one share itself and waits for the rest.
 namespace {
 class CopyPool {
@@ -497,8 +489,7 @@ class CopyPool {
 
 // Forward pass.  `host_data` != nullptr (crnn_forward_host): the batch is still in page-locked HOST memory; it is cut into
 // `chunks` image ranges whose H2D copies run on `copy_st` while the batch-independent front end (conv1 .. conv3_2 + pools) of
-// the previous range runs on `st` -- the copy (33.6 MB at batch 1024 x 32x256, ~0.65 ms over PCIe 5) hides behind ~0.9 ms of
-// compute instead of preceding it.  From conv4_1 on (batch-statistics BatchNorm) the batch is processed whole.
+// the previous range runs on `st` -- the copy (33.6 MB at batch 1024 x 32x256) hides behind that compute instead of preceding it.  From conv4_1 on (batch-statistics BatchNorm) the batch is processed whole.
 // `pageable_src` != nullptr (crnn_forward_pageable): the batch is in ordinary host memory; every range is first moved into the
 // page-locked `host_data` staging by the copy pool, its DMA is issued, its front end is launched -- and the host moves the next
 // range while the GPU works on this one.
@@ -598,8 +589,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     {
       gemm::Params p = conv_params(N, H2, 8, 128, 256, 256, m->P("conv3_1/biases"), pl.a3, pl.mg3);
       if (chunks > 1) { p.m_tile0 = n0 * sb3 / 4; p.num_m_tiles = cn * sb3 / 4; }
-      if (m->use_2cta) CRNN_TRY((launch_gemm2<gemm::A_CONV3, gemm::EPI_RELU, 6>(pl.tA_c31, m->tBh_c31, p, sms, st)));
-      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4>(pl.tA_c31, m->tB_c31, p, sms, st)));
+      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4>(pl.tA_c31, m->tB_c31, p, sms, st)));
     }
     if (mark) STAGE_MARK();
     // conv3_2 + ReLU + height pool
@@ -608,11 +598,9 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
       if (chunks > 1) { p.m_tile0 = n0 * sb3 / 4; p.num_m_tiles = cn * sb3 / 4; }
       if (pl.train) {
         p.argmax = pl.am3;
-        if (m->use_2cta) CRNN_TRY((launch_gemm2<gemm::A_CONV3, gemm::EPI_RELU_POOL12_T, 6>(pl.tA_c32, m->tBh_c32, p, sms, st)));
-        else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12_T, 4>(pl.tA_c32, m->tB_c32, p, sms, st)));
+        CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12_T, 4>(pl.tA_c32, m->tB_c32, p, sms, st)));
       } else {
-        if (m->use_2cta) CRNN_TRY((launch_gemm2<gemm::A_CONV3, gemm::EPI_RELU_POOL12, 6>(pl.tA_c32, m->tBh_c32, p, sms, st)));
-        else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12, 4>(pl.tA_c32, m->tB_c32, p, sms, st)));
+        CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12, 4>(pl.tA_c32, m->tB_c32, p, sms, st)));
       }
     }
     if (mark) STAGE_MARK();
@@ -624,8 +612,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
   {
     gemm::Params p = conv_params(N, H2, 4, 256, 512, 256, m->P("conv4_1/biases"), pl.a4a_pre, pl.mg4);
     p.stats = pl.stats;
-    if (m->use_2cta) CRNN_TRY((launch_gemm2<gemm::A_CONV3, gemm::EPI_STATS, 6>(pl.tA_c41, m->tBh_c41, p, sms, st)));
-    else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c41, m->tB_c41, p, sms, st)));
+    CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c41, m->tB_c41, p, sms, st)));
     STAGE_MARK();
     float* bn = pl.bn;
     // batch statistics over the GLOBAL batch when the batch is sharded over ranks: the exchange is fused into the finalize kernel
@@ -642,8 +629,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
   {
     gemm::Params p = conv_params(N, H2, 4, 512, 512, 256, m->P("conv4_2/biases"), pl.a4b_pre, pl.mg4);
     p.stats = pl.stats + 1024;
-    if (m->use_2cta) CRNN_TRY((launch_gemm2<gemm::A_CONV3, gemm::EPI_STATS, 6>(pl.tA_c42, m->tBh_c42, p, sms, st)));
-    else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c42, m->tB_c42, p, sms, st)));
+    CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c42, m->tB_c42, p, sms, st)));
     STAGE_MARK();
     float* bn = pl.bn + 2048;
     if (m->dp_world > 1)
@@ -662,8 +648,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     p.M = N * H2;
     p.num_m_tiles = (p.M + 127) / 128; p.num_n_tiles = 2; p.num_k_blocks = 32; p.kb_per_shift = 16; p.row_shift_mul = 1;
     p.Nc = 512; p.bias = m->P("conv5/biases"); p.out = pl.a5; p.ldo = 512;
-    if (m->use_2cta) CRNN_TRY((launch_gemm2<gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 6>(pl.tA_c5, m->tBh_c5, p, sms, st)));
-    else CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tA_c5, m->tB_c5, p, sms, st)));
+    CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tA_c5, m->tB_c5, p, sms, st)));
   }
   STAGE_MARK();
   // LSTM input projection for all frames and both directions: [N*H2, 512] x [512, 2048]
@@ -674,8 +659,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     p.num_m_tiles = (p.M + 127) / 128; p.num_n_tiles = 8; p.num_k_blocks = 8; p.kb_per_shift = 8;
     p.Nc = 2048; p.bias = m->xbias; p.out = pl.xproj; p.ldo = 2048;
     p.H = H2; p.T = T; p.seq_len = time_step_len;
-    if (m->lstm_upc == 32 && m->use_2cta) CRNN_TRY((launch_gemm2<gemm::A_PLAIN, gemm::EPI_XPROJ, 6>(pl.tA_x, m->tBh_x, p, sms, st)));
-    else if (m->lstm_upc == 32) CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_XPROJ, 4>(pl.tA_x, m->tB_x, p, sms, st)));
+    if (m->lstm_upc == 32) CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_XPROJ, 4>(pl.tA_x, m->tB_x, p, sms, st)));
     else CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tA_x, m->tB_x, p, sms, st)));
   }
   STAGE_MARK();
@@ -858,14 +842,14 @@ extern "C" int crnn_debug_tap(crnn_model* m, const char* name, float* dst, size_
 
 extern "C" int crnn_test_gemm_bf16(const void* A, const void* B, float* D, int M, int Nc, int K, int block_n,
                                    crnn_stream_t stream) {
-  if (!A || !B || !D || M <= 0 || Nc <= 0 || K <= 0 || (K % 64) != 0 || (block_n != 512 && block_n != 384 && (Nc % block_n) != 0))
+  if (!A || !B || !D || M <= 0 || Nc <= 0 || K <= 0 || (K % 64) != 0 || (Nc % block_n) != 0)
     return crnn_fail(CRNN_INVALID_VALUE, "test_gemm: bad args");
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   CUtensorMap ta, tb;
   CRNN_TRY(make_tmap_2d(&ta, A, M, K, K, 128));
-  CRNN_TRY(make_tmap_2d(&tb, B, Nc, K, K, block_n >= 384 ? 256 : block_n));
+  CRNN_TRY(make_tmap_2d(&tb, B, Nc, K, K, block_n));
   gemm::Params p;
   memset(&p, 0, sizeof(p));
   p.M = M; p.Nc = Nc;
@@ -876,19 +860,5 @@ extern "C" int crnn_test_gemm_bf16(const void* A, const void* B, float* D, int M
   if (block_n == 64) return launch_gemm<64, gemm::A_PLAIN, gemm::EPI_F32, 8>(ta, tb, p, sms, st);
   if (block_n == 128) return launch_gemm<128, gemm::A_PLAIN, gemm::EPI_F32, 6>(ta, tb, p, sms, st);
   if (block_n == 256) return launch_gemm<256, gemm::A_PLAIN, gemm::EPI_F32, 4>(ta, tb, p, sms, st);
-  if (block_n == 512) {      // 2-CTA pairs (cta_group::2), 256 x 256 tile per cluster
-    if (Nc % 256) return crnn_fail(CRNN_INVALID_VALUE, "test_gemm: 2-CTA path needs Nc % 256 == 0");
-    CUtensorMap tbh;
-    CRNN_TRY(make_tmap_2d(&tbh, B, Nc, K, K, 128));
-    p.num_n_tiles = Nc / 256;
-    return launch_gemm2<gemm::A_PLAIN, gemm::EPI_F32, 6>(ta, tbh, p, sms, st);
-  }
-  if (block_n == 384) {      // 2-CTA pairs with a 128-column N tile (probe: does M = 256 restore the MMA rate at N = 128?)
-    if (Nc % 128) return crnn_fail(CRNN_INVALID_VALUE, "test_gemm: Nc % 128");
-    CUtensorMap tbh;
-    CRNN_TRY(make_tmap_2d(&tbh, B, Nc, K, K, 64));
-    p.num_n_tiles = Nc / 128;
-    return launch_gemm2<gemm::A_PLAIN, gemm::EPI_F32, 8, 128>(ta, tbh, p, sms, st);
-  }
-  return crnn_fail(CRNN_INVALID_VALUE, "test_gemm: block_n must be 64/128/256 (or 512 = 2-CTA pairs)");
+  return crnn_fail(CRNN_INVALID_VALUE, "test_gemm: block_n must be 64/128/256");
 }

@@ -10,7 +10,7 @@
 
 int make_tmap_2d(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t row_stride, uint32_t box_rows);
 int make_tmap_nhwc(CUtensorMap* m, const void* base, int N, int H, int Wd, int C, int bh);
-// f32 tensors read as kind::tf32 operands: 32-element (128 B) boxes along the contiguous dimension
+// f32 tensors read as tf32 operands: 32-element (128 B) boxes along the contiguous dimension
 int make_tmap_2d_f32(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t row_stride, uint32_t box_rows);
 int make_tmap_nhwc_f32(CUtensorMap* m, const void* base, int N, int H, int Wd, int C, int bh);
 size_t align_up(size_t v, size_t a = 1024);
@@ -74,7 +74,7 @@ struct Plan {
 
 struct crnn_model {
   crnn_config cfg;
-  int num_sms = 148;
+  int num_sms = 132;
   std::vector<TensorInfo> tensors;
   int64_t total = 0;
   float *params = nullptr, *grads = nullptr, *adam_m = nullptr, *adam_v = nullptr;
@@ -94,10 +94,7 @@ struct crnn_model {
   CUtensorMap tDs_c2;        // conv2 dgrad weights through a 128-row box (rows 64..127 out of bounds -> zero fill): conv2_dgrad_swap_kernel
   CUtensorMap tD_h256;       // same W_h^T operand, box = 256 unit rows (K-split BPTT)
   bool bptt_ks = true;       // BPTT through lstm_bwd::lstm_bwd_ks_kernel (K-split, generic-proxy exchange); CRNN_BPTT=ring -> v1
-  CUtensorMap tDh_c42, tDh_c41, tDh_c32, tDh_c5, tDh_x;     // box = 128 rows (2-CTA pairs)
   double* grad_sumsq = nullptr;
-  CUtensorMap tBh_c2, tBh_c31, tBh_c32, tBh_c41, tBh_c42, tBh_c5, tBh_x;   // same weights, box = 128 rows: per-CTA half of a 256-row N tile
-  bool use_2cta = true;      // cta_group::2 GEMM pairs for the Nc % 256 == 0 layers (CRNN_GEMM2=0 disables; debug A/B switch)
   bool conv1_tc = true;      // conv1 + pool1 on the tensor cores (conv1_tc.cuh, split-bf16 operands); CRNN_CONV1=simt -> kernels.cu
   bool bn_red_fused = true;       // conv4_1's BN-backward sums inside conv4_2's data-gradient epilogue (EPI_CONV_STORE_BNRED); CRNN_BN_FUSE=0 -> separate pass
   bool relu_mask_fused = true;    // conv3_1's ReLU backward inside conv3_2's data-gradient epilogue (EPI_CONV_STORE_MASK); CRNN_RELU_FUSE=0 -> separate pass

@@ -1,4 +1,4 @@
-// Thin inline-PTX layer for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA, TMEM).
+// Thin inline-PTX layer for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma descriptors, clusters.
 // No CUTLASS/CuTe dependency; bit layouts of the descriptors are documented next to each builder.
 #pragma once
 #include <cuda_runtime.h>
@@ -75,17 +75,6 @@ __device__ __forceinline__ void bulk_load_1d_mc(void* dst_smem, const void* src_
                ::"r"(smem_u32(dst_smem)), "l"(reinterpret_cast<uint64_t>(src_gmem)), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask)
                : "memory");
 }
-// Shared-memory matrix descriptor, K-major operand, NO swizzle: 8-row x 16-B core matrices (128 B contiguous);
-// `lbo` = byte distance between the two core matrices of one K=16 step, `sbo` = byte distance between 8-row groups.
-__device__ __forceinline__ uint64_t make_desc_k_nosw(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(lbo >> 4) << 16;
-  d |= static_cast<uint64_t>(sbo >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  return d;
-}
-
 // ------------------------------------------------------------------ TMA loads (tile mode, OOB -> 0)
 __device__ __forceinline__ void prefetch_tmap(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
@@ -117,49 +106,28 @@ __device__ __forceinline__ void tma_store_4d(const void* tmap, const void* src, 
                : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {   // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
+// ------------------------------------------------------------------ wgmma operand descriptors (sm_90)
+//   [0,14) start address >> 4   [16,30) leading byte offset >> 4   [32,46) stride byte offset >> 4
+//   [62,64) layout type: 0 = no swizzle (8-row x 16-B core matrices), 1 = SWIZZLE_128B
+// K-major, no swizzle: `lbo` = byte distance between the two core matrices of one K=16 step, `sbo` = between 8-row groups.
+__device__ __forceinline__ uint64_t make_desc_k_nosw(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+  d |= static_cast<uint64_t>(lbo >> 4) << 16;
+  d |= static_cast<uint64_t>(sbo >> 4) << 32;
+  return d;
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {     // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// tcgen05.commit: arrives (count 1) on the mbarrier once all previously issued MMAs of this thread retire.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16/fp16 operands with f32 accumulate.
-__device__ __forceinline__ void mma_f16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// K-major, 128-byte swizzle (rows of 128 B as written by TMA, 8-row atoms of 1024 B): SBO = 1024 B between 8-row groups.
+// One K step (16 bf16 / 8 tf32 = 32 B) inside the swizzle row is +2 in the address field.
+__device__ __forceinline__ uint64_t make_desc_k_sw128(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
+  return d;
 }
 
-// kind::tf32: operands are 32-bit words read as tf32 (sign, 8-bit exponent, 10-bit mantissa; the low 13 bits are ignored),
-// K = 8 per instruction (32 B of the swizzle row), f32 accumulate.  Half the kind::f16 rate.
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 // round-to-nearest f32 -> tf32 (the tensor core would otherwise truncate)
 __device__ __forceinline__ float round_tf32(float v) {
   uint32_t r;
@@ -167,65 +135,48 @@ __device__ __forceinline__ float round_tf32(float v) {
   return __uint_as_float(r);
 }
 
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle (rows of 128 B, 8-row atoms of 1024 B):
-//   [0,14)  start address >> 4        [16,30) leading byte offset >> 4 (ignored for swizzled K-major; 1)
-//   [32,46) stride byte offset >> 4 (= 1024 B between 8-row groups)
-//   [46,48) descriptor version = 1 (sm_100)      [61,64) layout type: 2 = SWIZZLE_128B
-__device__ __forceinline__ uint64_t make_desc_k_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
+// register budget of a warpgroup (all four warps execute it): producers give registers up, MMA warpgroups take them
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+__device__ __forceinline__ void bar_sync(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// Instruction descriptor (upper 32 bits of the PTX idesc operand), kind::f16:
-//   [4,6) D format (1 = f32)   [7,10) A format (1 = bf16)   [10,13) B format (1 = bf16)
-//   [15] A major (0 = K)       [16] B major (0 = K)         [17,23) N >> 3      [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
+// ------------------------------------------------------------------ accumulator tile staged in shared memory
+// The MMA warpgroups hold the accumulators in the wgmma fragment layout; the epilogues own one accumulator ROW per thread.
+// The tile goes through shared memory as [rows][NC] f32 whose 16-B chunks are XOR-swizzled by (row & 7): fragment stores are
+// at most 2-way conflicted and row-per-thread 16-B reads of a quarter-warp hit 8 different chunks (conflict-free).
+template <int NC>
+__device__ __forceinline__ float* acc_chunk(float* tile, int row, int c4) {
+  return tile + row * NC + ((c4 ^ (row & 7)) << 2);
 }
-// kind::tf32: same fields, A/B format code 2 (tf32)
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
+// fragment of one m64 x N wgmma (this thread's warpgroup) -> rows row0 .. row0+63, columns col0 .. col0+N-1
+template <int N, int NC>
+__device__ __forceinline__ void acc_store(float* tile, const float (&d)[N / 2], int row0, int col0 = 0) {
+  const int t = threadIdx.x & 127, l = t & 31;
+  const int r = row0 + 16 * (t >> 5) + (l >> 2);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const int c = col0 + 8 * j + 2 * (l & 3);
+    *reinterpret_cast<float2*>(acc_chunk<NC>(tile, r, c >> 2) + (c & 3)) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(acc_chunk<NC>(tile, r + 8, c >> 2) + (c & 3)) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
+}
+// row-per-thread read of NV consecutive columns c0 .. c0+NV-1 (c0 % 4 == 0) of `row`, as raw f32 bits
+template <int NC, int NV>
+__device__ __forceinline__ void acc_ld(float* tile, int row, int c0, uint32_t (&v)[NV]) {
+#pragma unroll
+  for (int i = 0; i < NV / 4; ++i) {
+    const float4 x = *reinterpret_cast<const float4*>(acc_chunk<NC>(tile, row, (c0 >> 2) + i));
+    v[4 * i] = __float_as_uint(x.x); v[4 * i + 1] = __float_as_uint(x.y);
+    v[4 * i + 2] = __float_as_uint(x.z); v[4 * i + 3] = __float_as_uint(x.w);
+  }
 }
 
-// TMEM -> registers: 32 lanes x 32 consecutive f32 columns; thread i of the warp gets lane (base+i).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-
-// ------------------------------------------------------------------ 2-CTA (cta_group::2) variants and cluster helpers
+// ------------------------------------------------------------------ cluster helpers
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -257,36 +208,6 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* dst_smem, uint32_t ncols) {   // one warp in EACH CTA of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2cta() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A (128 rows from each CTA's smem) * B (N/2 rows from each CTA's smem); issued by the leader CTA only
-__device__ __forceinline__ void mma_f16_ss_2cta(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (count 1) on the barrier at this smem offset in every CTA of `cta_mask` once the issued MMAs retire
-__device__ __forceinline__ void tc_commit_2cta_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-// tcgen05.commit (1-CTA MMAs) arriving on the barrier at this smem offset in EVERY CTA of `cta_mask`
-__device__ __forceinline__ void tc_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
 // TMA load multicast: the box lands at the same smem offset, and completes on the mbarrier at the same offset, in every CTA
 // of `cta_mask` (one L2 read feeds the whole cluster)
 __device__ __forceinline__ void tma_load_2d_mc(const void* tmap, uint64_t* bar, void* dst, int c0, int c1, uint16_t cta_mask) {
@@ -295,21 +216,6 @@ __device__ __forceinline__ void tma_load_2d_mc(const void* tmap, uint64_t* bar, 
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
-// TMA loads into THIS CTA's smem whose completion bytes are credited to an mbarrier given by shared::cluster address
-// (the leader CTA's full barrier)
-__device__ __forceinline__ void tma_load_2d_2cta(const void* tmap, uint32_t bar_cluster_addr, void* dst, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2cta(const void* tmap, uint32_t bar_cluster_addr, void* dst, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-
 // ------------------------------------------------------------------ misc math / packing
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 t = __floats2bfloat162_rn(lo, hi);
@@ -324,17 +230,15 @@ __device__ __forceinline__ uint32_t hmax2_bf16(uint32_t a, uint32_t b) {
 __device__ __forceinline__ float bf16_lo(uint32_t v) { return __uint_as_float(v << 16); }
 __device__ __forceinline__ float bf16_hi(uint32_t v) { return __uint_as_float(v & 0xFFFF0000u); }
 
-// ------------------------------------------------------------------ 256-bit global store (sm_100 STG.256; 32-B aligned address)
-// A row-per-thread epilogue store touches 32 different lines per instruction; with 16-B stores every instruction fills half a
-// 32-B sector per lane, with 32-B stores a whole one -- half the store wavefronts for the same bytes.
+// ------------------------------------------------------------------ 32-B global store as two 16-B stores (32-B aligned address)
 __device__ __forceinline__ void st_global_v8(void* ptr, uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t e, uint32_t f,
                                              uint32_t g, uint32_t h) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(ptr), "r"(a), "r"(b), "r"(c), "r"(d), "r"(e), "r"(f),
-               "r"(g), "r"(h)
-               : "memory");
+  uint4* p = reinterpret_cast<uint4*>(ptr);
+  p[0] = make_uint4(a, b, c, d);
+  p[1] = make_uint4(e, f, g, h);
 }
 
-// ------------------------------------------------------------------ packed f32x2 FMA (sm_100 FFMA2: two IEEE fma.rn per lane)
+// ------------------------------------------------------------------ f32 pairs packed in 64 bits (two IEEE fma.rn)
 __device__ __forceinline__ uint64_t pack_f32x2(float lo, float hi) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -344,9 +248,9 @@ __device__ __forceinline__ void unpack_f32x2(uint64_t v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ uint64_t ffma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpack_f32x2(a, a0, a1); unpack_f32x2(b, b0, b1); unpack_f32x2(c, c0, c1);
+  return pack_f32x2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 
 __device__ __forceinline__ float ex2(float x) {

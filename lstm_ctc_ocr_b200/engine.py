@@ -1,6 +1,6 @@
 """Device-side engine behind the reference-facing API.  PyTorch tensors are used purely as
 device-memory containers and for the current CUDA stream; every kernel on this path lives in
-libcrnnctc.so (hand-written sm_100a CUDA, see csrc/)."""
+libcrnnctc.so (hand-written sm_90a CUDA, see csrc/)."""
 from collections import OrderedDict
 
 import numpy as np
@@ -26,12 +26,12 @@ class CrnnModel:
 
     def __init__(self, weight_decay=1e-5, bn_eps=1e-3, device=None, compute_dtype="bf16"):
         if not torch.cuda.is_available():
-            raise CrnnError("lstm_ctc_ocr_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise CrnnError("lstm_ctc_ocr_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.lib = _lib.load()
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         torch.cuda.set_device(self.device)
         # "bf16": bf16 operands / f32 accumulate (throughput path); "f32": split-bf16 operands, f32-class (BASELINE configs[1]);
-        # "tf32": kind::tf32 operands, same forward-only orchestration as "f32"
+        # "tf32": tf32 operands, same forward-only orchestration as "f32"
         self.compute_dtype = {"bf16": 1, "f32": 2, "tf32": 3, 1: 1, 2: 2, 3: 3}[compute_dtype]
         cfg = CrnnConfig(32, NCLASSES, 512, bn_eps, weight_decay, self.compute_dtype)
         h = _lib.c_void_p()
@@ -264,7 +264,7 @@ def dense_decoded(out, out_len):
 
 
 def test_gemm_tn_bf16(A, B, block_n, k_splits=0):
-    """D[M,N] = A[K,M]^T @ B[K,N] through the MN-major tcgen05 path (tests only)."""
+    """D[M,N] = A[K,M]^T @ B[K,N] through the MN-major wgmma path (tests only)."""
     lib = _lib.load()
     K, M = A.shape
     Nc = B.shape[1]

@@ -1,7 +1,7 @@
 """Network object with the reference's attribute surface (lib/networks/network.py:40-95,647-664).
 
 The reference builds a TF1 graph through a chaining DSL; here the graph is fixed (it is the one
-LSTM_train.setup/LSTM_test.setup build, LSTM_train.py:22-38) and runs as hand-written sm_100a
+LSTM_train.setup/LSTM_test.setup build, LSTM_train.py:22-38) and runs as hand-written sm_90a
 kernels in libcrnnctc.so.  What is preserved is the *surface* the solver touches: placeholders
 ``data/labels/time_step_len/labels_len/keep_prob``, the ``layers`` dict, ``feed``/``get_output``,
 ``build_loss() -> (loss, dense_decoded)``; handles are evaluated by ``Session.run``."""
@@ -57,7 +57,7 @@ _OFF_PATH_LAYERS = ("lstm", "concat", "conv", "conv_zero", "conv_norm", "conv_fi
 
 
 class UnsupportedGraph(NotImplementedError):
-    """The declared layer chain is not the one the sm_100a kernels implement (there is no generic graph executor behind this
+    """The declared layer chain is not the one the sm_90a kernels implement (there is no generic graph executor behind this
     API and no fallback: the reference's LSTM_train / LSTM_test topology is the product)."""
 
 

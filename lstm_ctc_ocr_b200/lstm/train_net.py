@@ -37,7 +37,7 @@ def main(argv=None):
         cfg_from_list(args.set_cfgs)
     if not torch.cuda.is_available():
         from .._lib import CrnnError
-        raise CrnnError("train_net needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise CrnnError("train_net needs a CUDA device (sm_90a); there is no CPU fallback")
     if "LOCAL_RANK" in os.environ:                       # torchrun: one process per GPU, NCCL gradient all-reduce
         import torch.distributed as dist
         torch.cuda.set_device(int(os.environ["LOCAL_RANK"]))

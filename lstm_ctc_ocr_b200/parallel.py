@@ -74,8 +74,8 @@ class GradBuckets(object):
 
     The announced ranges arrive in descending address order and are contiguous, so they are merged until `min_bucket_bytes` are
     ready; each bucket is all-reduced on a side stream.  `sm_reserve` SMs are left free by the persistent backward kernels so the
-    collective's CTAs do not delay the tail of a 148-CTA grid (measured on 2 GPUs: 7 un-merged buckets on a full GPU cost +0.38 ms
-    per step over one all-reduce at the end -- every NCCL kernel displaced persistent CTAs for its whole duration)."""
+    collective's CTAs do not delay the tail of a full-GPU grid (without the reserve every NCCL kernel displaces persistent CTAs
+    for its whole duration)."""
 
     def __init__(self, eng, min_bucket_bytes=8 << 20, sm_reserve=8):
         self.eng = eng
@@ -146,10 +146,9 @@ class DataParallel(object):
         ... eng.forward / ctc_loss / eng.backward ...
         dp.step(lr, step)                     # gradient all-reduce, then clip + Adam on the reduced gradient
 
-    `overlap=True` reduces merged gradient buckets on a side stream while the backward still runs (GradBuckets).  Measured on
-    B200 it does NOT pay for this model (profiles/r2_scaling.md: 8 GPUs 13.41 ms vs 13.20 ms per step, 2 GPUs 13.25 vs 12.87):
-    the whole exchange is ~0.15 ms of a 13 ms step while every overlapped NCCL kernel displaces CTAs of the persistent
-    full-GPU GEMM grids for its duration -- so the default is ONE all-reduce of the flat buffer after the backward.
+    `overlap=True` reduces merged gradient buckets on a side stream while the backward still runs (GradBuckets).  Every
+    overlapped NCCL kernel displaces CTAs of the persistent full-GPU GEMM grids for its duration while the exchange itself is a
+    small part of the step, so the default is ONE all-reduce of the flat buffer after the backward.
     """
 
     def __init__(self, eng, sync_bn=True, overlap=False, peer_memory=True, min_bucket_bytes=8 << 20, sm_reserve=8):

@@ -1,5 +1,5 @@
 """``Session.run(fetches, feed_dict)`` -- the call the reference's solver makes every iteration
-(lib/lstm/train.py:129-130,160; lib/lstm/test.py:77), evaluated by the sm_100a engine.
+(lib/lstm/train.py:129-130,160; lib/lstm/test.py:77), evaluated by the sm_90a engine.
 
 Per run: feed_dict numpy arrays -> pinned host staging -> async H2D on the current stream ->
 crnn_forward -> crnn_ctc_loss / crnn_total_loss / crnn_ctc_greedy as the fetches require -> D2H of
@@ -133,7 +133,7 @@ class _Pinned(object):
 class Session(object):
     def __init__(self, device=None):
         if not torch.cuda.is_available():
-            raise CrnnError("Session needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise CrnnError("Session needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         self._engines = {}
         self._pinned = _Pinned()

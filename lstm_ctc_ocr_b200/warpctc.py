@@ -35,7 +35,7 @@ def _dev_i32(x, device):
 def ctc(activations, flat_labels, label_lengths, input_lengths, blank_label=0):
     as_numpy = not torch.is_tensor(activations)
     if not torch.cuda.is_available():
-        raise engine.CrnnError("ctc: needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise engine.CrnnError("ctc: needs a CUDA device (sm_90a); there is no CPU fallback")
     if as_numpy:
         activations = torch.as_tensor(np.asarray(activations, dtype=np.float32), device="cuda")
     if not activations.is_cuda:

@@ -25,7 +25,7 @@ own call sites.  What it IS pinned to (``tests/test_oracle.py``):
     layouts, not the network's sizes.
 BatchNorm and Adam have no externally held vector.
 
-Reference call sites restated (paths relative to /root/reference):
+Reference call sites restated (paths relative to the reference checkout):
   * topology / hyper-parameters ......... lib/networks/LSTM_train.py:22-38
   * conv -> bias -> BN -> ReLU order ..... lib/networks/network.py:160-191
   * max_pool ksize/stride mapping ....... lib/networks/network.py:343-350

@@ -1,7 +1,7 @@
 """Known-answer vectors published by the two third-party projects that hold the arithmetic of the reference's loss and
 decode call sites (lib/networks/network.py:653-657): TensorFlow (`tf.nn.ctc_loss`, `ctc_greedy_decoder`,
 `ctc_beam_search_decoder`) and baidu-research/warp-ctc (`compute_ctc_loss`).  Neither project is vendored under
-/root/reference nor installable here (SURVEY 8(c)), so these are the only externally held numbers the path can be pinned to.
+the reference checkout nor installable here (SURVEY 8(c)), so these are the only externally held numbers the path can be pinned to.
 
 Provenance [upstream-memory -- transcribed, not fetched: there is no network]:
   * CTC_LOSS: tensorflow/python/kernel_tests/ctc_loss_op_test.py::CTCLossTest.testBasic (two 5-frame, 6-class utterances,

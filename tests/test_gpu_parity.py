@@ -1,4 +1,4 @@
-"""Parity tests proper (need the B200): every call goes through the C ABI of libcrnnctc.so via ctypes.
+"""Parity tests proper (need the GPU): every call goes through the C ABI of libcrnnctc.so via ctypes.
 
 Stated tolerances for the bf16-operand / f32-accumulate path (north-star: 'within a stated fp tolerance'):
   * GEMM unit test vs f32 matmul of the same bf16 inputs ............ max-abs <= 2e-5 * K^0.5 relative to max|D|
@@ -95,7 +95,7 @@ def test_ctc_loss_and_grad_vs_oracle(case, kernel, monkeypatch):
 def test_ctc_fast_kernel_extreme_logits_match_generic(monkeypatch):
     """Very peaked rows (scale 30: per-frame probabilities down to 2^-130) keep the log-space recursion finite; both kernels
     agree with the oracle and with each other.  Tolerance: the f32 log2-domain scores reach |a| ~ 4e3 here, where one ulp is
-    2.4e-4, and the state posterior 2^(alpha+beta-e-ll) inherits a few ulps of that (measured 1.7e-3 on B200) -- the same
+    2.4e-4, and the state posterior 2^(alpha+beta-e-ll) inherits a few ulps of that -- the same
     resolution limit warp-ctc's f32 log-space recursion has; at the working range (|logit| < 10) the bound is 3.6e-5."""
     from lstm_ctc_ocr_b200 import engine
     rng = np.random.default_rng(5)
@@ -206,7 +206,7 @@ def test_forward_loss_decode_vs_committed_golden():
 @pytest.mark.parametrize("N,W,widths", [(3, 100, None), (5, 24, [24, 20, 9, 24, 16]), (2, 160, [160, 131]), (130, 40, None)])
 def test_forward_layers_vs_oracle(N, W, widths, front, monkeypatch):
     """Every layer against the fp64 oracle; conv1 and conv2 through both of their kernels: the defaults (conv1_tc.cuh: im2col +
-    split-bf16 tcgen05; conv_swap.cuh: channels on the MMA M side) and the first-generation ones (kernels.cu SIMT conv1,
+    split-bf16 wgmma; conv_swap.cuh: channels on the MMA M side) and the first-generation ones (kernels.cu SIMT conv1,
     CRNN_CONV1=simt; gemm.cuh positions-on-M conv2, CRNN_CONV2=pos)."""
     from lstm_ctc_ocr_b200 import engine
     from oracle import crnn_oracle as O

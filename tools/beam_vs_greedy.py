@@ -1,6 +1,6 @@
 """Side statistic asked for by SURVEY 8(c): how often does the reference's decode (TF beam search, width 100, merge_repeated=True,
 [upstream-memory] restatement in oracle/) agree with the greedy rule the product implements?  CPU only.
-Usage: python tools/beam_vs_greedy.py [lines_per_setting]  -> profiles/r1_beam_vs_greedy.json"""
+Usage: python tools/beam_vs_greedy.py [lines_per_setting]  -> one JSON line on stdout"""
 import json
 import os
 import sys
@@ -49,7 +49,7 @@ def main():
         print(res[-1], f"{time.time() - t0:.0f}s", flush=True)
     out = {"what": "greedy (product) vs TF beam search width 100 (reference, restated in oracle/crnn_oracle.py:beam_search_decode, "
                    "[upstream-memory], not pinned against TF); T in {19,39,63}, zeros stripped on both sides", "settings": res}
-    json.dump(out, open(os.path.join(ROOT, "profiles", "r1_beam_vs_greedy.json"), "w"), indent=1)
+    print(json.dumps(out))
 
 
 if __name__ == "__main__":

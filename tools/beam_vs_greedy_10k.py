@@ -3,7 +3,7 @@ host-side crnn_ctc_beam_search) and the north-star's greedy decoder agree on the
 fixture, through the TRAINED weights of tests/golden/trained_ref_cfg_bf16.npz.  CPU only: logits come from the oracle's fp32
 forward (the GPU path decodes these lines identically to it, tests/test_gpu_decode10k.py).  ~10 min on 8 cores.
 
-    python tools/beam_vs_greedy_10k.py [n_batches]  ->  profiles/r2_beam_vs_greedy_10k.json"""
+    python tools/beam_vs_greedy_10k.py [n_batches]  ->  one JSON line on stdout"""
 import importlib.util
 import json
 import os
@@ -57,8 +57,6 @@ def main():
     st["what"] = ("10 240 rendered lines (bucketed 512 x W in {80,160,256}) through the trained fixture weights; logits from the oracle's fp32 forward; "
                   "beam = crnn_ctc_beam_search width 100 (the reference's decoder, network.py:656: merge_repeated=True collapses repeated labels of the "
                   "DECODED sequence too), greedy = the north-star decoder; *_nomerge = the same beam search with merge_repeated=False")
-    with open(os.path.join(ROOT, "profiles", "r2_beam_vs_greedy_10k.json"), "w") as f:
-        json.dump(st, f, indent=1)
     print(json.dumps(st))
 
 

@@ -1,4 +1,4 @@
-"""Micro-probe: plain tcgen05 GEMM throughput vs operand bytes per MMA cycle (is the conv mainloop L2-feed-bound?)."""
+"""Micro-probe: plain wgmma GEMM throughput vs operand bytes per MMA cycle (is the conv mainloop L2-feed-bound?)."""
 import os
 import sys
 
@@ -9,7 +9,7 @@ from lstm_ctc_ocr_b200 import engine  # noqa: E402
 
 dev = torch.device("cuda:0")
 SKIP = os.environ.get('CRNN_PROBE_SKIP_TMA') == '1'
-for (M, Nc, K, bn) in [(8192, 8192, 8192, 384), (8192, 8192, 8192, 512), (262144, 512, 4608, 512), (8192, 8192, 8192, 256), (8192, 8192, 8192, 128), (8192, 8192, 8192, 64), (262144, 512, 4608, 256), (262144, 512, 2304, 256),
+for (M, Nc, K, bn) in [(8192, 8192, 8192, 256), (8192, 8192, 8192, 128), (8192, 8192, 8192, 64), (262144, 512, 4608, 256), (262144, 512, 2304, 256),
                        (16384, 256, 8192, 256)]:
     A = torch.randn(M, K, device=dev).to(torch.bfloat16)
     B = torch.randn(Nc, K, device=dev).to(torch.bfloat16)
@@ -26,8 +26,7 @@ for (M, Nc, K, bn) in [(8192, 8192, 8192, 384), (8192, 8192, 8192, 512), (262144
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / 5
-    nt = {512: 256, 384: 128}.get(bn, bn)
-    tiles = ((M + 127) // 128) * (Nc // nt)
-    bytes_l2 = tiles * (K // 64) * (16384 + {512: 128, 384: 64}.get(bn, bn) * 128)
+    tiles = ((M + 127) // 128) * (Nc // bn)
+    bytes_l2 = tiles * (K // 64) * (16384 + bn * 128)
     print(f"M={M} N={Nc} K={K} BLOCK_N={bn}: {ms:.3f} ms  {2.0*M*Nc*K/ms/1e9:.0f} TFLOP/s  smem-feed {bytes_l2/ms/1e9:.2f} TB/s (+ f32 D write {M*Nc*4/ms/1e9:.2f} TB/s)", flush=True)
     del A, B

@@ -1,6 +1,6 @@
 """Timeline of the persistent LSTM kernel (debug): CRNN_LSTM_TRACE=1 makes crnn_forward print clock64 stamps of CTAs 0 and 5
 for steps 8..11 to stderr (events: 0 step top, 1 TMA issued, 2 first K-block landed, 3 last K-block landed, 4 MMAs committed,
-5 xproj loads issued, 6 accumulator ready, 7 first TMEM half loaded, 8 cell + stores issued, 9 fence.proxy.async done,
+5 xproj loads issued, 6 accumulator ready, 7 first accumulator half loaded, 8 cell + stores issued, 9 fence.proxy.async done,
 10 cluster arrive, 11 cluster wait done).  Usage: python tools/lstm_trace.py [N] [W]"""
 import os
 import sys

@@ -10,6 +10,10 @@
 // 4-D TMA boxes of 128 positions at (r-1, s-1)-shifted coordinates (OOB zero fill = SAME padding, also past the image end)
 // and one 2-D box of the weights.  Accumulator lane = output channel, column = position, so the 2x2 pool is register-local
 // in the epilogue thread (columns hl*16+w: window = {2pw, 2pw+1} x {row, row+1}); a warp stores 32 consecutive channels.
+//
+// The accumulators drain through shared memory one 64-column slice at a time (128 x 64 f32 = 32 KB, ptx::acc_store_slice),
+// which leaves room for a 4-stage ring.  Slice j holds the 32-column chunks 2j and 2j+1; the two warps of a quadrant take one
+// chunk each (chunk = one pooled row pair here, RC rows of H in the data-gradient kernel below).
 #pragma once
 #include <cuda.h>
 
@@ -18,13 +22,15 @@
 
 namespace convsw {
 
-constexpr int STAGES = 2;                   // what fits next to the 128 KB staged accumulator tile
+constexpr int STAGES = 4;                   // what fits next to the 32 KB staged accumulator slice
+constexpr int SLICE_N = 64;                 // accumulator columns staged at a time
 constexpr int W_BYTES = 128 * 128;          // weights: 128 channels x 64 K (128 B rows, SW128)
 constexpr int X_BYTES = 256 * 128;          // activations: 256 positions x 64 K
 constexpr int STAGE_BYTES = W_BYTES + X_BYTES;
 constexpr int ACC_OFFSET = STAGES * STAGE_BYTES;
-constexpr int BAR_OFFSET = ACC_OFFSET + 128 * 256 * 4;
+constexpr int BAR_OFFSET = ACC_OFFSET + 128 * SLICE_N * 4;
 constexpr int SMEM_BYTES = BAR_OFFSET + 256 + 1024;
+static_assert(SMEM_BYTES <= 232448, "opt-in shared memory per block (227 KB)");
 constexpr int NUM_THREADS = 384;            // warpgroup 0 producer, warpgroups 1..2 MMA (channels 0..63 / 64..127) + epilogue
 constexpr int NUM_TAPS = 9;
 
@@ -87,7 +93,7 @@ conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
     int stage = 0;
     uint32_t phase = 0;
     const int q = warp_idx & 3;
-    const int ch = (warp_idx - 4) >> 2;
+    const int ch = (warp_idx - 4) >> 2;               // 32-column chunk of each staged slice
     const int c = q * 32 + lane;                       // output channel of this thread
     const float bias = __ldg(p.bias + c);
     const int Hp = p.H >> 1;
@@ -112,14 +118,14 @@ conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
       wg::wait<0>();
       wg::fence_operand(d);
       if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
-      ptx::bar_sync(1, 256);                         // the previous tile's epilogue reads are done
-      ptx::acc_store<256, 256>(acc_tile, d, wgi * 64);
-      ptx::bar_sync(1, 256);
-#pragma unroll 1
-      for (int pr = 0; pr < 4; ++pr) {
+#pragma unroll
+      for (int j = 0; j < 256 / SLICE_N; ++j) {
+        ptx::bar_sync(1, 256);                         // the previous slice's (tile's) epilogue reads are done
+        ptx::acc_store_slice<256, SLICE_N>(acc_tile, d, wgi * 64, j);
+        ptx::bar_sync(1, 256);
         uint32_t v[32];
-        ptx::acc_ld<256, 32>(acc_tile, q * 32 + lane, ch * 128 + pr * 32, v);   // columns: [row h (16 w) | row h+1 (16 w)]
-        const int h = h0 + ch * 8 + 2 * pr;
+        ptx::acc_ld<SLICE_N, 32>(acc_tile, q * 32 + lane, ch * 32, v);   // chunk 2j+ch, columns: [row h (16 w) | row h+1 (16 w)]
+        const int h = h0 + 2 * (2 * j + ch);
         if (h < p.H) {                                  // H is even: both rows of the window are inside or outside together
           const size_t off = (((size_t)n * Hp + (h >> 1)) * 8) * 128 + c;
 #pragma unroll
@@ -218,7 +224,7 @@ conv_dgrad_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
     int stage = 0;
     uint32_t phase = 0;
     const int q = warp_idx & 3;
-    const int ch = (warp_idx - 4) >> 2;      // column half: RT/2 of the tile's RT H-rows
+    const int ch = (warp_idx - 4) >> 2;      // 32-column chunk of each staged slice
     const int c = q * 32 + lane;              // input channel of this thread (valid for c < MVALID)
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int n = tile / p.tiles_per_img;
@@ -241,17 +247,17 @@ conv_dgrad_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
       wg::wait<0>();
       wg::fence_operand(d);
       if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
-      ptx::bar_sync(1, 256);                         // the previous tile's epilogue reads are done
-      ptx::acc_store<256, 256>(acc_tile, d, wgi * 64);
-      ptx::bar_sync(1, 256);
-      if (q * 32 < MVALID) {
-  #pragma unroll 1
-        for (int pr = 0; pr < 4; ++pr) {
+#pragma unroll
+      for (int j = 0; j < 256 / SLICE_N; ++j) {
+        ptx::bar_sync(1, 256);                         // the previous slice's (tile's) epilogue reads are done
+        ptx::acc_store_slice<256, SLICE_N>(acc_tile, d, wgi * 64, j);
+        ptx::bar_sync(1, 256);
+        if (q * 32 < MVALID) {
           uint32_t v[32];
-          ptx::acc_ld<256, 32>(acc_tile, q * 32 + lane, ch * 128 + pr * 32, v);     // columns: RC consecutive H rows of WD positions each
+          ptx::acc_ld<SLICE_N, 32>(acc_tile, q * 32 + lane, ch * 32, v);     // chunk 2j+ch, columns: RC consecutive H rows of WD positions each
 #pragma unroll
           for (int hr = 0; hr < RC; ++hr) {
-            const int h = h0 + ch * (RT / 2) + pr * RC + hr;
+            const int h = h0 + (2 * j + ch) * RC + hr;
             if (h < p.H) {
               __nv_bfloat16* o = p.out + (((size_t)n * p.H + h) * WD) * MVALID + c;
 #pragma unroll

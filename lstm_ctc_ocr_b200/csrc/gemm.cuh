@@ -5,9 +5,12 @@
 // Roles (384 threads): warpgroup 0 = TMA producer (warp 0, one lane per box; the warpgroup gives its registers to the MMA
 // warpgroups), warpgroups 1 and 2 = MMA (rows 0..63 / 64..127 of the tile, accumulators in registers) and epilogue.
 // Pipeline: STAGES-deep smem ring (full/empty mbarriers, TMA <-> MMA; the producer runs ahead into the next tile while
-// the epilogue of this one drains).  The finished accumulators are staged in shared memory (ptx::acc_store) so that every
-// epilogue thread owns one accumulator ROW: 8 warps, accumulator quadrant q = warp % 4 (32 rows), two warps per quadrant
-// each draining half of the tile's columns.
+// the epilogue of this one drains).  The finished accumulators are staged in shared memory (ptx::acc_store_slice) so that
+// every epilogue thread owns one accumulator ROW: 8 warps, accumulator quadrant q = warp % 4 (32 rows), two warps per
+// quadrant each draining half of the staged columns.  At BLOCK_N = 256 the tile goes through one 128 x 64 f32 buffer (32 KB)
+// a 64-column slice at a time, not as a whole (128 KB): that leaves room for a 4-stage ring, where the full tile would leave 2.
+// Narrower tiles, EPI_LSTM and EPI_CONV_STORE_BNRED stage the whole tile (slice_cols).  The MMA warpgroups run with 240
+// registers (the producer keeps 24): the first slices drain while the later slices' accumulators are still in registers.
 //
 // A-operand modes
 //   A_PLAIN  rows are consecutive rows of a 2-D [rows, K] tensor map; conv5 (2x2 VALID over [N,H,2,512]) reads
@@ -120,22 +123,32 @@ __device__ __forceinline__ float warp_colsum32(const float (&v)[32], int lane) {
   return keep + __shfl_xor_sync(0xffffffffu, send, 1);
 }
 
-// STAGES is the requested ring depth; S the depth that fits next to the staged accumulator tile
-template <int BLOCK_N, int STAGES>
+// Accumulator columns staged in shared memory at a time (see the header).  While a slice drains, the accumulators of the
+// later slices stay live in registers (96 at BLOCK_N = 256).  EPI_CONV_STORE_BNRED's epilogue does not fit in the registers
+// left beside them (it spills), so, like EPI_LSTM, it stages the whole tile; it only serves the training backward pass.
+// BLOCK_N = 128 measured slower in 64-column slices (6 stages) than whole (5 stages), so it stays whole.
+constexpr int slice_cols(int block_n, int epi) {
+  return (block_n < 256 || epi == EPI_LSTM || epi == EPI_CONV_STORE_BNRED) ? block_n : 64;
+}
+
+// STAGES is the requested ring depth; S the depth that fits next to the staged accumulator slice of SLICE_N columns
+template <int BLOCK_N, int STAGES, int SLICE_N>
 struct Smem {
   static constexpr int B_STAGE_BYTES = BLOCK_N * 128;
-  static constexpr int ACC_BYTES = BLOCK_M * BLOCK_N * 4;
+  static constexpr int ACC_BYTES = BLOCK_M * SLICE_N * 4;
   static constexpr int FIT = (MAX_SMEM - ACC_BYTES - 256 - 1024) / (A_STAGE_BYTES + B_STAGE_BYTES);
   static constexpr int S = STAGES < FIT ? STAGES : FIT;
   static constexpr int ACC_OFFSET = S * (A_STAGE_BYTES + B_STAGE_BYTES);
   static constexpr int BAR_OFFSET = ACC_OFFSET + ACC_BYTES;
   static constexpr int BYTES = BAR_OFFSET + 256 + 1024;   // barriers + alignment slack
 };
+static_assert(Smem<256, 4, 64>::S == 4, "a 64-column staging slice leaves room for a 4-stage ring at BLOCK_N = 256");
 
-// Per-tile epilogue: thread (q, lane) owns accumulator row q*32+lane of the 128-row tile staged at `acc`.
-template <int BLOCK_N, int EPI>
+// Epilogue of tile columns [c_lo, c_hi): thread (q, lane) owns accumulator row q*32+lane of the 128-row tile.  `acc` holds
+// the NC staged columns c_acc .. c_acc+NC-1 of the tile.
+template <int BLOCK_N, int NC, int EPI>
 __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const int m_blk, const int n_blk, const int q,
-                                             const int lane, const int c_lo = 0, const int c_hi = BLOCK_N) {
+                                             const int lane, const int c_lo, const int c_hi, const int c_acc) {
   const int row = q * 32 + lane;
   const int col0 = n_blk * BLOCK_N;
 
@@ -160,7 +173,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
+      ptx::acc_ld<NC, 32>(acc, row, c0 - c_acc, v);
       if (grow < p.M) {
 #pragma unroll
         for (int i = 0; i < 32; i += 4)
@@ -180,7 +193,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
+      ptx::acc_ld<NC, 32>(acc, row, c0 - c_acc, v);
       uint32_t pk[16];
 #pragma unroll
       for (int i = 0; i < 32; i += 4) {
@@ -202,7 +215,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
+      ptx::acc_ld<NC, 32>(acc, row, c0 - c_acc, v);
       if (ok) {
 #pragma unroll
         for (int i = 0; i < 32; i += 4) {
@@ -223,7 +236,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
+      ptx::acc_ld<NC, 32>(acc, row, c0 - c_acc, v);
       uint32_t pk[16];
 #pragma unroll
       for (int i = 0; i < 32; i += 4) {
@@ -270,7 +283,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
+      ptx::acc_ld<NC, 32>(acc, row, c0 - c_acc, v);
       if (valid) {
 #pragma unroll
         for (int i = 0; i < 32; i += 16)
@@ -297,7 +310,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
         for (int i = 0; i < 4; ++i) mk[i] = __ldg(reinterpret_cast<const uint4*>(msk + c0) + i);     // issued before the accumulator reads
       }
       uint32_t v[32];
-      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
+      ptx::acc_ld<NC, 32>(acc, row, c0 - c_acc, v);
       if (valid) {
         const uint32_t* mw = reinterpret_cast<const uint32_t*>(mk);
         uint32_t pk[16];
@@ -323,7 +336,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
 #pragma unroll
       for (int i = 0; i < 4; ++i) xq[i] = valid ? __ldg(reinterpret_cast<const uint4*>(xp + c0) + i) : make_uint4(0u, 0u, 0u, 0u);
       uint32_t v[32];
-      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
+      ptx::acc_ld<NC, 32>(acc, row, c0 - c_acc, v);
       const uint32_t* xw = reinterpret_cast<const uint32_t*>(xq);
       uint32_t pk[16];
       float f[32], f2[32];
@@ -359,7 +372,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
+      ptx::acc_ld<NC, 32>(acc, row, c0 - c_acc, v);
       if (valid) {
 #pragma unroll
         for (int i = 0; i < 32; i += 4)
@@ -382,7 +395,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
+      ptx::acc_ld<NC, 32>(acc, row, c0 - c_acc, v);
 #pragma unroll
       for (int i = 0; i < 32; i += 4) {
         const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + c0 + i));
@@ -431,7 +444,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
-      ptx::acc_ld<BLOCK_N, 32>(acc, row, c0, v);
+      ptx::acc_ld<NC, 32>(acc, row, c0 - c_acc, v);
       float f[32], f2[32];
       uint32_t pk[16];
 #pragma unroll
@@ -463,6 +476,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
     }
   } else if (EPI == EPI_LSTM) {
     // row = sample within the direction-stacked batch; tile columns = [i(64) j(64) f(64) o(64)] of 64 units
+    // (the whole tile is staged: NC == BLOCK_N, c_acc == 0)
     const int grow = m_blk * BLOCK_M + row;
     const int dir = (m_blk >= p.m_tiles_per_dir) ? 1 : 0;
     const int n = grow - dir * p.Npad;
@@ -478,10 +492,10 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
 #pragma unroll 1
     for (int u0 = (c_lo >> 2); u0 < (c_hi >> 2); u0 += 16) {
       uint32_t gi[16], gj[16], gf[16], go[16];
-      ptx::acc_ld<BLOCK_N, 16>(acc, row, u0, gi);
-      ptx::acc_ld<BLOCK_N, 16>(acc, row, 64 + u0, gj);
-      ptx::acc_ld<BLOCK_N, 16>(acc, row, 128 + u0, gf);
-      ptx::acc_ld<BLOCK_N, 16>(acc, row, 192 + u0, go);
+      ptx::acc_ld<NC, 16>(acc, row, u0, gi);
+      ptx::acc_ld<NC, 16>(acc, row, 64 + u0, gj);
+      ptx::acc_ld<NC, 16>(acc, row, 128 + u0, gf);
+      ptx::acc_ld<NC, 16>(acc, row, 192 + u0, go);
       uint32_t hp[8];
       if (active) {
         uint4 xi[2], xj[2], xf[2], xo[2];
@@ -537,7 +551,8 @@ template <int BLOCK_N, int AMODE, int EPI, int STAGES, int KIND = 0>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Params p) {
   static_assert(BLOCK_N == 64 || BLOCK_N == 128 || BLOCK_N == 256, "BLOCK_N");
-  using SM = Smem<BLOCK_N, STAGES>;
+  constexpr int SLICE_N = slice_cols(BLOCK_N, EPI);
+  using SM = Smem<BLOCK_N, STAGES, SLICE_N>;
   constexpr int S = SM::S;
   constexpr int B_STAGE_BYTES = BLOCK_N * 128;
   constexpr int KELEMS = KIND ? 32 : BLOCK_K;        // operand elements per 128 B K-block
@@ -570,7 +585,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     // One lane per TMA box: a single thread issuing 5 boxes per K-block serialises the conv mainloop on the issue latency.
     // Lanes 0..nA-1 load the A sub-boxes, lane nA loads B; lane 0 also arms the transaction count.  conv: when the tile's 4
     // sub-boxes are contiguous rows of one image (p.merged), a single 128-position box replaces them.
-    ptx::setmaxnreg_dec<40>();
+    ptx::setmaxnreg_dec<24>();
     const int nA = (AMODE == A_CONV3 && !p.merged) ? 4 : 1;
     if (warp_idx == 0 && lane <= nA) {
       int stage = 0;
@@ -616,10 +631,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     }
   } else {
     // ===================== MMA warpgroups (rows wgi*64 ..) + epilogue =====================
-    ptx::setmaxnreg_inc<232>();
+    ptx::setmaxnreg_inc<240>();
     const int wgi = (warp_idx >> 2) - 1;
     const int q = warp_idx & 3;                      // accumulator row quadrant drained by this warp
-    const int chalf = (warp_idx - 4) >> 2;           // warps 4..7 take columns [0, N/2), warps 8..11 take [N/2, N)
+    const int chalf = (warp_idx - 4) >> 2;           // warps 4..7 take the first half of each staged slice, warps 8..11 the second
     const bool arriver = (warp_idx & 3) == 0 && lane == 0;
     int stage = 0;
     uint32_t phase = 0;
@@ -647,10 +662,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       wg::wait<0>();
       wg::fence_operand(d);
       if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
-      ptx::bar_sync(1, 256);                         // the previous tile's epilogue reads are done
-      ptx::acc_store<BLOCK_N, BLOCK_N>(acc_tile, d, wgi * 64);
-      ptx::bar_sync(1, 256);
-      run_epilogue<BLOCK_N, EPI>(p, acc_tile, m_blk, n_blk, q, lane, chalf * (BLOCK_N / 2), (chalf + 1) * (BLOCK_N / 2));
+#pragma unroll
+      for (int s = 0; s < BLOCK_N / SLICE_N; ++s) {
+        ptx::bar_sync(1, 256);                       // the previous slice's (tile's) epilogue reads are done
+        ptx::acc_store_slice<BLOCK_N, SLICE_N>(acc_tile, d, wgi * 64, s);
+        ptx::bar_sync(1, 256);
+        const int c_lo = s * SLICE_N + chalf * (SLICE_N / 2);
+        run_epilogue<BLOCK_N, SLICE_N, EPI>(p, acc_tile, m_blk, n_blk, q, lane, c_lo, c_lo + SLICE_N / 2, s * SLICE_N);
+      }
     }
   }
 }

@@ -8,7 +8,7 @@
 template <int BN, int AM, int EPI, int ST, int KIND = 0>
 static int launch_gemm(const CUtensorMap& a, const CUtensorMap& b, const gemm::Params& p, int num_sms, cudaStream_t st) {
   auto kern = gemm::gemm_kernel<BN, AM, EPI, ST, KIND>;
-  constexpr int smem = gemm::Smem<BN, ST>::BYTES;
+  constexpr int smem = gemm::Smem<BN, ST, gemm::slice_cols(BN, EPI)>::BYTES;
   static bool attr = false;
   if (!attr) {
     CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));

@@ -164,6 +164,21 @@ __device__ __forceinline__ void acc_store(float* tile, const float (&d)[N / 2], 
     *reinterpret_cast<float2*>(acc_chunk<NC>(tile, r + 8, c >> 2) + (c & 3)) = make_float2(d[4 * j + 2], d[4 * j + 3]);
   }
 }
+// column slice s of the same fragment: columns s*NC .. s*NC+NC-1 (registers 4j .. 4j+3 of column groups j = s*NC/8 ..) ->
+// rows row0 .. row0+63, columns 0 .. NC-1 of an NC-wide tile.  Call it with a constant s (an unrolled slice loop), so that the
+// register indices stay compile-time constants.
+template <int N, int NC>
+__device__ __forceinline__ void acc_store_slice(float* tile, const float (&d)[N / 2], int row0, int s) {
+  const int t = threadIdx.x & 127, l = t & 31;
+  const int r = row0 + 16 * (t >> 5) + (l >> 2);
+#pragma unroll
+  for (int jj = 0; jj < NC / 8; ++jj) {
+    const int j = s * (NC / 8) + jj;
+    const int c = 8 * jj + 2 * (l & 3);
+    *reinterpret_cast<float2*>(acc_chunk<NC>(tile, r, c >> 2) + (c & 3)) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(acc_chunk<NC>(tile, r + 8, c >> 2) + (c & 3)) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
+}
 // row-per-thread read of NV consecutive columns c0 .. c0+NV-1 (c0 % 4 == 0) of `row`, as raw f32 bits
 template <int NC, int NV>
 __device__ __forceinline__ void acc_ld(float* tile, int row, int c0, uint32_t (&v)[NV]) {

@@ -124,7 +124,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
     memset(&p, 0, sizeof(p));
     p.M = (int)R; p.num_m_tiles = (p.M + 127) / 128; p.num_n_tiles = 2; p.num_k_blocks = 1; p.kb_per_shift = 1;
     p.Nc = 512; p.out = pl.d_lstm_out; p.ldo = 512;
-    CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tG_dl, m->tD_l, p, sms, st)));
+    CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tG_dl, m->tD_l, p, sms, st, &pl.tO_dlo)));
   }
   BMARK();
   // ------------------------------------------------------------------ BPTT through both directions
@@ -182,7 +182,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
       memset(&p, 0, sizeof(p));
       p.M = (int)R; p.num_m_tiles = (p.M + 127) / 128; p.num_n_tiles = 2; p.num_k_blocks = 32; p.kb_per_shift = 32;
       p.Nc = 512; p.out = pl.d_a5; p.ldo = 512;
-      CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tG_dz, m->tD_x, p, sms, st)));
+      CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tG_dz, m->tD_x, p, sms, st, &pl.tG_da5)));
     }
   }
   BMARK();
@@ -199,7 +199,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
     memset(&p, 0, sizeof(p));
     p.M = (int)R; p.num_m_tiles = (p.M + 127) / 128; p.num_n_tiles = 4; p.num_k_blocks = 16; p.kb_per_shift = 8; p.row_shift_mul = -1;
     p.Nc = 1024; p.out = pl.d_a4b; p.ldo = 1024;
-    CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tG_da5, m->tD_c5, p, sms, st)));
+    CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tG_da5, m->tD_c5, p, sms, st, &pl.tO_da4b)));
   }
   BMARK();
   // ------------------------------------------------------------------ conv4_2: pool3 + ReLU + batch-stat BN backward
@@ -233,7 +233,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
     if (m->bn_red_fused) {
       CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE_BNRED, 4>(pl.tG_p4b, m->tD_c42, p, sms, st)));
     } else {
-      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE, 4>(pl.tG_p4b, m->tD_c42, p, sms, st)));
+      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE, 4>(pl.tG_p4b, m->tD_c42, p, sms, st, &pl.tG_p4a)));
     }
   }
   BMARK();
@@ -253,7 +253,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
   BMARK();
   {
     gemm::Params p = conv_params(N, H2, 4, 512, 256, 256, nullptr, pl.d_a3p, pl.mg4);
-    CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE, 4>(pl.tG_p4a, m->tD_c41, p, sms, st)));
+    CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE, 4>(pl.tG_p4a, m->tD_c41, p, sms, st, &pl.tO_da3p)));
   }
   BMARK();
   // ------------------------------------------------------------------ conv3_2: 1x2 pool + ReLU backward
@@ -275,7 +275,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
     if (m->relu_mask_fused) {
       CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE_MASK, 4>(pl.tG_p32, m->tD_c32, p, sms, st)));
     } else {
-      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE, 4>(pl.tG_p32, m->tD_c32, p, sms, st)));
+      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE, 4>(pl.tG_p32, m->tD_c32, p, sms, st, &pl.tG_p31)));
     }
   }
   BMARK();

@@ -11,9 +11,12 @@
 // and one 2-D box of the weights.  Accumulator lane = output channel, column = position, so the 2x2 pool is register-local
 // in the epilogue thread (columns hl*16+w: window = {2pw, 2pw+1} x {row, row+1}); a warp stores 32 consecutive channels.
 //
-// The accumulators drain through shared memory one 64-column slice at a time (128 x 64 f32 = 32 KB, ptx::acc_store_slice),
-// which leaves room for a 4-stage ring.  Slice j holds the 32-column chunks 2j and 2j+1; the two warps of a quadrant take one
-// chunk each (chunk = one pooled row pair here, RC rows of H in the data-gradient kernel below).
+// Inference (TRAIN = false): the pool window is local to the accumulator fragment (w pair = columns 2c, 2c+1; H pair = 16 columns
+// apart), so pool, bias, ReLU and bf16 rounding happen in registers; the 16 KB pooled tile is written transposed into shared
+// memory and leaves through two asynchronous TMA stores while the next tile's MMAs run.
+// Training and the data-gradient kernel below drain the accumulators through shared memory one 64-column slice at a time
+// (128 x 64 f32 = 32 KB, ptx::acc_store_slice), which leaves room for a 4-stage ring.  Slice j holds the 32-column chunks 2j and
+// 2j+1; the two warps of a quadrant take one chunk each (chunk = one pooled row pair here, RC rows of H in the data-gradient kernel).
 #pragma once
 #include <cuda.h>
 
@@ -45,7 +48,8 @@ struct Params {
 
 template <bool TRAIN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const Params p) {
+conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmO,
+                  const Params p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + BAR_OFFSET);
@@ -58,6 +62,7 @@ conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
   if (warp_idx == 0 && lane == 0) {
     ptx::prefetch_tmap(&tmX);
     ptx::prefetch_tmap(&tmW);
+    if (!TRAIN) ptx::prefetch_tmap(&tmO);
     for (int s = 0; s < STAGES; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
       ptx::mbar_init(&empty_bar[s], 2);        // one arrive per MMA warpgroup
@@ -97,6 +102,13 @@ conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
     const int c = q * 32 + lane;                       // output channel of this thread
     const float bias = __ldg(p.bias + c);
     const int Hp = p.H >> 1;
+    // inference epilogue (fragment side): this thread's accumulator rows are channels f0 and f0 + 8
+    const int t = threadIdx.x & 127, l = t & 31;
+    const int f0 = wgi * 64 + 16 * (t >> 5) + (l >> 2);
+    const float bias0 = __ldg(p.bias + f0), bias8 = __ldg(p.bias + f0 + 8);
+    const bool even = ((l >> 2) & 1) == 0;           // lanes l and l ^ 4 hold channels f0 and f0 ^ 1
+    const bool issuer = !TRAIN && threadIdx.x == 128;
+    uint8_t* stg = smem + ACC_OFFSET;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int nl = tile / p.tiles_per_img, n = p.img0 + nl;
       const int h0 = (tile - nl * p.tiles_per_img) * 16;
@@ -118,6 +130,37 @@ conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
       wg::wait<0>();
       wg::fence_operand(d);
       if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
+      if (!TRAIN) {
+        // Pool, bias, ReLU and bf16 rounding in registers: fragment column 8j + 2(l%4) + {0,1} is a w pair of H row j/2 of the
+        // tile, the H row below it is column group j + 2.  The pooled tile (8 pooled rows x 8 x 128 channels, 16 KB) goes through
+        // shared memory as two [64 positions][64 channels] SWIZZLE_128B boxes and leaves with two TMA stores (rows >= H/2 dropped).
+        if (issuer) ptx::bulk_wait_read_all();       // the previous tile's stores have read the buffer
+        ptx::bar_sync(1, 256);
+#pragma unroll
+        for (int ph = 0; ph < 8; ++ph) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int j = 4 * ph + e;
+            const float m0 = fmaxf(fmaxf(d[4 * j], d[4 * j + 1]), fmaxf(d[4 * j + 8], d[4 * j + 9]));
+            const float m8 = fmaxf(fmaxf(d[4 * j + 2], d[4 * j + 3]), fmaxf(d[4 * j + 10], d[4 * j + 11]));
+            const uint32_t b0 = __bfloat16_as_ushort(__float2bfloat16_rn(fmaxf(m0 + bias0, 0.f)));
+            const uint32_t b8 = __bfloat16_as_ushort(__float2bfloat16_rn(fmaxf(m8 + bias8, 0.f)));
+            // exchange with lane l ^ 4 so that each lane holds an adjacent channel pair: (f0, f0 + 1) or (f0 + 7, f0 + 8)
+            const uint32_t r = __shfl_xor_sync(0xffffffffu, even ? b8 : b0, 4);
+            const uint32_t word = even ? (b0 | (r << 16)) : (r | (b8 << 16));
+            const int row = ph * 8 + 4 * e + (l & 3), ch = even ? f0 : f0 + 7;     // pooled position, first channel of the pair
+            *reinterpret_cast<uint32_t*>(stg + (ch >> 6) * 8192 + row * 128 + ((((ch >> 3) & 7) ^ (row & 7)) << 4) + ((ch & 7) << 1)) = word;
+          }
+        }
+        ptx::fence_proxy_async_smem();
+        ptx::bar_sync(1, 256);
+        if (issuer) {
+          ptx::tma_store_4d(&tmO, stg, 0, 0, h0 >> 1, n);
+          ptx::tma_store_4d(&tmO, stg + 8192, 64, 0, h0 >> 1, n);
+          ptx::bulk_commit();
+        }
+        continue;
+      }
 #pragma unroll
       for (int j = 0; j < 256 / SLICE_N; ++j) {
         ptx::bar_sync(1, 256);                         // the previous slice's (tile's) epilogue reads are done
@@ -132,10 +175,7 @@ conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
           for (int pw = 0; pw < 8; ++pw) {
             const float x00 = __uint_as_float(v[2 * pw]), x01 = __uint_as_float(v[2 * pw + 1]);
             const float x10 = __uint_as_float(v[16 + 2 * pw]), x11 = __uint_as_float(v[16 + 2 * pw + 1]);
-            if (!TRAIN) {
-              const float mx = fmaxf(fmaxf(x00, x01), fmaxf(x10, x11));
-              p.out[off + (size_t)pw * 128] = __float2bfloat16_rn(fmaxf(mx + bias, 0.f));
-            } else {
+            {
               // key = (bf16 bits of relu(x + b) << 2) | (3 - window index): the largest value wins, ties go to the FIRST
               // window position in (dy, dx) row-major order (same rule as gemm.cuh EPI_RELU_POOL22_T)
               const uint32_t p0 = ptx::pack_bf16x2(fmaxf(x00 + bias, 0.f), fmaxf(x01 + bias, 0.f));
@@ -150,6 +190,7 @@ conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
         }
       }
     }
+    if (issuer) ptx::bulk_wait_all();                  // the CTA's shared memory must outlive its last stores
   }
 }
 
@@ -273,7 +314,9 @@ conv_dgrad_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
 }  // namespace convsw
 
 template <bool TRAIN>
-static int launch_conv2_swap(const CUtensorMap& x, const CUtensorMap& w, const convsw::Params& p, int num_sms, cudaStream_t st) {
+// `out`: NHWC map of the pooled output [N, H/2, 8, 128], box [64, 8, 8, 1] (one tile = 8 pooled rows); only <false> stores through it
+static int launch_conv2_swap(const CUtensorMap& x, const CUtensorMap& w, const CUtensorMap& out, const convsw::Params& p, int num_sms,
+                             cudaStream_t st) {
   auto kern = convsw::conv2_swap_kernel<TRAIN>;
   static bool attr = false;
   if (!attr) {
@@ -282,7 +325,7 @@ static int launch_conv2_swap(const CUtensorMap& x, const CUtensorMap& w, const c
   }
   const int tiles = p.Nimg * p.tiles_per_img;
   const int grid = tiles < num_sms ? tiles : num_sms;
-  kern<<<grid, convsw::NUM_THREADS, convsw::SMEM_BYTES, st>>>(x, w, p);
+  kern<<<grid, convsw::NUM_THREADS, convsw::SMEM_BYTES, st>>>(x, w, out, p);
   CUDA_TRY(cudaGetLastError());
   return CRNN_OK;
 }

@@ -11,6 +11,9 @@
 // a 64-column slice at a time, not as a whole (128 KB): that leaves room for a 4-stage ring, where the full tile would leave 2.
 // Narrower tiles, EPI_LSTM and EPI_CONV_STORE_BNRED stage the whole tile (slice_cols).  The MMA warpgroups run with 240
 // registers (the producer keeps 24): the first slices drain while the later slices' accumulators are still in registers.
+// The bf16-output epilogues at BLOCK_N = 256 (frag_epi) do not stage f32 at all: they finish the values in the fragment registers,
+// write bf16 into the staging region (the whole 64 KB tile, 3 stages) in the layout of the output tensor map and leave through asynchronous TMA stores
+// (frag_epilogue), so the next tile's MMAs start while the stores drain.
 //
 // A-operand modes
 //   A_PLAIN  rows are consecutive rows of a 2-D [rows, K] tensor map; conv5 (2x2 VALID over [N,H,2,512]) reads
@@ -20,7 +23,7 @@
 //            64-channel block; the producer issues one 4-D TMA box per sub-box at coordinates shifted by
 //            (r-1, s-1) -- out-of-bounds elements are zero-filled by TMA, which *is* the SAME padding.
 //
-// Epilogues: see enum Epi.  Every epilogue thread owns one accumulator row.
+// Epilogues: see enum Epi.  In run_epilogue every epilogue thread owns one accumulator row; frag_epilogue works on the fragments.
 #pragma once
 #include <cuda.h>
 
@@ -63,6 +66,7 @@ struct Params {
                          // == num_k_blocks for an ordinary GEMM; conv5 (2x2 VALID) uses 16 -> rows t and t+1
   int merged;            // conv: the tile's 4 sub-boxes are contiguous H rows of one image -> one 128-position TMA box
   int debug_skip_tma;    // probe only: producer arrives without loading (measures the MMA/epilogue ceiling)
+  int debug_skip_epilogue;  // probe only: tiles end after the mainloop, nothing is stored (measures the mainloop alone)
   int row_shift_mul;     // +1 (conv5 forward: rows m, m+1) or -1 (conv5 data gradient: rows m, m-1)
   // split-bf16 ("3xbf16", f32-class) operands: the activation tensor stores [hi | lo] halves and the K loop visits
   // [hi | lo | hi] against weights [wh | wh | wl]; a virtual K-block index >= the fold wraps back onto the hi half.  0 = off.
@@ -126,9 +130,13 @@ __device__ __forceinline__ float warp_colsum32(const float (&v)[32], int lane) {
 // Accumulator columns staged in shared memory at a time (see the header).  While a slice drains, the accumulators of the
 // later slices stay live in registers (96 at BLOCK_N = 256).  EPI_CONV_STORE_BNRED's epilogue does not fit in the registers
 // left beside them (it spills), so, like EPI_LSTM, it stages the whole tile; it only serves the training backward pass.
-// BLOCK_N = 128 measured slower in 64-column slices (6 stages) than whole (5 stages), so it stays whole.
+// BLOCK_N = 128 measured slower in 64-column slices (6 stages) than whole (5 stages), so it stays whole.  The register-side
+// bf16 epilogues (frag_epi) stage the whole bf16 tile in the bytes of 128 f32 columns: with 3 stages that measured faster than
+// two 32 KB halves through one buffer with 4 stages (the halves wait on each other's stores).  EPI_RELU_POOL12's pooled tile
+// needs only 32 KB.
 constexpr int slice_cols(int block_n, int epi) {
-  return (block_n < 256 || epi == EPI_LSTM || epi == EPI_CONV_STORE_BNRED) ? block_n : 64;
+  return (block_n < 256 || epi == EPI_LSTM || epi == EPI_CONV_STORE_BNRED) ? block_n
+       : (epi == EPI_RELU || epi == EPI_STATS || epi == EPI_BIAS_BF16 || epi == EPI_XPROJ || epi == EPI_CONV_STORE) ? 128 : 64;
 }
 
 // STAGES is the requested ring depth; S the depth that fits next to the staged accumulator slice of SLICE_N columns
@@ -143,6 +151,160 @@ struct Smem {
   static constexpr int BYTES = BAR_OFFSET + 256 + 1024;   // barriers + alignment slack
 };
 static_assert(Smem<256, 4, 64>::S == 4, "a 64-column staging slice leaves room for a 4-stage ring at BLOCK_N = 256");
+
+// Epilogues that run on the accumulator fragments and leave through TMA stores (frag_epilogue); the staging region then holds the
+// bf16 tile (slice_cols = 128 "f32 columns" = 64 KB, 3 stages) or the pooled tile (32 KB, 4 stages) instead of an f32 slice.
+constexpr bool frag_epi(int block_n, int epi) {
+  return block_n == 256 && (epi == EPI_RELU || epi == EPI_RELU_POOL12 || epi == EPI_STATS || epi == EPI_BIAS_BF16 ||
+                            epi == EPI_XPROJ || epi == EPI_CONV_STORE);
+}
+
+// bf16x2 word of staged row `row`, tile-half column c (even) 0..127: [64-column box][row][128 B], 16-B chunks XOR-swizzled by
+// (row & 7) -- the SWIZZLE_128B layout the output tensor maps read, and conflict-free for fragment-order 32-bit writes
+__device__ __forceinline__ uint32_t* stg_word(uint8_t* buf, int box_bytes, int row, int c) {
+  return reinterpret_cast<uint32_t*>(buf + (c >> 6) * box_bytes + row * 128 + ((((c >> 3) & 7) ^ (row & 7)) << 4) + ((c & 7) << 1));
+}
+
+// EPI_STATS column sums of 32 staged rows rg*32 .. rg*32+31 at 32-bit word cw (two bf16 channels) of a 128-B box row:
+// {sum lo, sum hi, sum lo^2, sum hi^2}.  The rows are added in the order of warp_colsum32 over 32 lanes (rows 16 apart first,
+// then 8, 4, 2, 1), so the f32 partial sums are those of the row-per-thread epilogue, bit for bit.  Evaluated depth first:
+// few partial sums are live next to the accumulators of the tile's second half.
+template <int W>
+__device__ __forceinline__ float4 rowsum_tree(const uint8_t* box, int rg, int cw, int i) {
+  if constexpr (W == 32) {
+    const int r = rg * 32 + i;
+    const uint32_t v = *reinterpret_cast<const uint32_t*>(box + r * 128 + (((cw >> 2) ^ (r & 7)) << 4) + ((cw & 3) << 2));
+    const float x = ptx::bf16_lo(v), y = ptx::bf16_hi(v);
+    return make_float4(x, y, __fmul_rn(x, x), __fmul_rn(y, y));     // no contraction of the squares into the additions
+  } else {
+    const float4 a = rowsum_tree<W * 2>(box, rg, cw, i), b = rowsum_tree<W * 2>(box, rg, cw, i + W);
+    return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+  }
+}
+
+// conv tiles: accumulator row r of tile m_blk is a real output position (h < H, image < Nimg)
+__device__ __forceinline__ bool conv_row_valid(const Params& p, int m_blk, int r) {
+  const int g = m_blk * 4 + (r >> 5);
+  const int n_img = g / p.sb_per_img;
+  const int h = (g - n_img * p.sb_per_img) * p.bh + (r & 31) / p.Wd;
+  return n_img < p.Nimg && h < p.H;
+}
+
+// Register-side epilogue of one finished tile (frag_epi).  The MMA thread applies bias / ReLU / pooling to its own fragment
+// registers with the same per-element operations as run_epilogue, writes bf16x2 words into the swizzled staging buffer, and one
+// thread (`issuer`) sends the buffer to global memory with asynchronous TMA stores; the warpgroups then go on to the next
+// tile's mainloop while the stores drain.  The whole bf16 tile is staged (64 KB: a 3-stage ring, see slice_cols), written and
+// stored in two 128-column halves; before the first half of a tile is written, the issuer waits until the previous tile's stores
+// have read the buffer.  The pooled tile (64 rows, 32 KB) keeps the 4-stage ring.
+//   conv outputs: 4-D NHWC map, box [64 ch, Wd, bh (x4 when merged), 1]; TMA drops rows with h >= H or image >= Nimg.
+//   plain outputs: 2-D [M, ldo] map, box [64, 128]; rows >= M are dropped.
+//   EPI_STATS: per-channel sum / sum of squares of the bf16-rounded outputs, read back from the staging buffer (invalid rows
+//   are staged as zero): thread = (column pair, 32-row group), 2048 f64 atomics per tile.
+//   EPI_XPROJ, columns >= 1024: rows reversed by sequence length.  When H divides 128 a tile holds whole sequences, so the
+//   reversal is a permutation of staging rows; otherwise the thread stores its words to the reversed rows directly.
+template <int EPI>
+__device__ __forceinline__ void frag_epilogue(const Params& p, const float (&d)[128], uint8_t* stg, const CUtensorMap* tmO,
+                                              const int m_blk, const int n_blk, const int wgi, const bool issuer) {
+  constexpr bool POOL = (EPI == EPI_RELU_POOL12);
+  constexpr bool CONV = (EPI == EPI_RELU || POOL || EPI == EPI_STATS || EPI == EPI_CONV_STORE);
+  constexpr bool RELU = (EPI == EPI_RELU || POOL);
+  constexpr int BOX_BYTES = (POOL ? 64 : 128) * 128;     // one [rows][64 columns] bf16 box
+  const int t = threadIdx.x & 127, l = t & 31;
+  const int r0 = wgi * 64 + 16 * (t >> 5) + (l >> 2);   // fragment rows r0 and r0 + 8
+  const int col0 = n_blk * 256;
+  bool ok0 = true, ok1 = true;
+  if (EPI == EPI_STATS) { ok0 = conv_row_valid(p, m_blk, r0); ok1 = conv_row_valid(p, m_blk, r0 + 8); }
+  int s0 = r0, s1 = r0 + 8;                              // staging rows (EPI_XPROJ: destination rows)
+  bool direct = false;
+  if (EPI == EPI_XPROJ && col0 >= 1024) {
+    int dr[2] = {r0, r0 + 8};
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int grow = m_blk * 128 + dr[i];
+      if (grow < p.M) {
+        const int n = grow / p.H, tt = grow - n * p.H;
+        const int len = min(max(__ldg(p.seq_len + n), 0), p.T);
+        if (tt < len) dr[i] = n * p.H + (len - 1 - tt) - m_blk * 128;
+      }
+    }
+    s0 = dr[0]; s1 = dr[1];
+    direct = (128 % p.H) != 0;
+  }
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) {
+    uint8_t* buf = stg + hf * 2 * BOX_BYTES;
+    if (hf == 0) {
+      if (issuer) ptx::bulk_wait_read_all();            // the previous stores have read the buffer
+      ptx::bar_sync(1, 256);
+    }
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+      const int j = hf * 16 + jj;
+      const int c = 8 * jj + 2 * (l & 3);                // column within the half
+      float2 b = make_float2(0.f, 0.f);
+      if (EPI != EPI_CONV_STORE && p.bias) b = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + hf * 128 + c));
+      uint32_t v0, v1;
+      if (EPI == EPI_CONV_STORE) {
+        v0 = ptx::pack_bf16x2(d[4 * j], d[4 * j + 1]);
+        v1 = ptx::pack_bf16x2(d[4 * j + 2], d[4 * j + 3]);
+      } else if (RELU) {
+        v0 = ptx::pack_bf16x2(fmaxf(d[4 * j] + b.x, 0.f), fmaxf(d[4 * j + 1] + b.y, 0.f));
+        v1 = ptx::pack_bf16x2(fmaxf(d[4 * j + 2] + b.x, 0.f), fmaxf(d[4 * j + 3] + b.y, 0.f));
+      } else {
+        v0 = ptx::pack_bf16x2(d[4 * j] + b.x, d[4 * j + 1] + b.y);
+        v1 = ptx::pack_bf16x2(d[4 * j + 2] + b.x, d[4 * j + 3] + b.y);
+      }
+      if (POOL) {
+        // rows r and r ^ 1 (w pair) sit in lanes l and l ^ 4; rounding to bf16 is monotonic, so max after packing == packing after max
+        v0 = ptx::hmax2_bf16(v0, __shfl_xor_sync(0xffffffffu, v0, 4));
+        v1 = ptx::hmax2_bf16(v1, __shfl_xor_sync(0xffffffffu, v1, 4));
+        // both lanes of the pair now hold both pooled rows: lane l stores the first, lane l ^ 4 the second (conflict-free)
+        if ((l & 4) == 0) *stg_word(buf, BOX_BYTES, r0 >> 1, c) = v0;
+        else *stg_word(buf, BOX_BYTES, (r0 + 8) >> 1, c) = v1;
+      } else if (EPI == EPI_XPROJ && direct) {
+        __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out) + col0 + hf * 128 + c;
+        if (m_blk * 128 + r0 < p.M) *reinterpret_cast<uint32_t*>(out + (size_t)(m_blk * 128 + s0) * p.ldo) = v0;
+        if (m_blk * 128 + r0 + 8 < p.M) *reinterpret_cast<uint32_t*>(out + (size_t)(m_blk * 128 + s1) * p.ldo) = v1;
+      } else {
+        *stg_word(buf, BOX_BYTES, s0, c) = ok0 ? v0 : 0u;
+        *stg_word(buf, BOX_BYTES, s1, c) = ok1 ? v1 : 0u;
+      }
+    }
+    if (EPI == EPI_XPROJ && direct) continue;
+    ptx::fence_proxy_async_smem();                       // generic-proxy writes -> visible to the TMA (async proxy) reads
+    ptx::bar_sync(1, 256);
+    if (issuer) {
+#pragma unroll
+      for (int bx = 0; bx < 2; ++bx) {
+        const int c = col0 + hf * 128 + bx * 64;
+        uint8_t* src = buf + bx * BOX_BYTES;
+        if (CONV) {
+          const int nb = p.merged ? 1 : 4;
+          for (int sb = 0; sb < nb; ++sb) {
+            const int g = m_blk * 4 + sb;
+            const int n = g / p.sb_per_img;
+            ptx::tma_store_4d(tmO, src + sb * (BOX_BYTES / 4), c, 0, (g - n * p.sb_per_img) * p.bh, n);
+          }
+        } else {
+          ptx::tma_store_2d(tmO, src, c, m_blk * 128);
+        }
+      }
+      ptx::bulk_commit();
+    }
+    if (EPI == EPI_STATS) {
+      // thread = (column pair cp, rows rg*32 .. rg*32+31); a warp reads whole 128-B rows: conflict-free
+      const int tt = threadIdx.x - 128;
+      const int cp = tt & 63, rg = tt >> 6, cw = cp & 31;
+      const uint8_t* bb = buf + (cp >> 5) * BOX_BYTES;
+      const float4 s = rowsum_tree<1>(bb, rg, cw, 0);
+      const int c = col0 + hf * 128 + 2 * cp;
+      atomicAdd(p.stats + c, (double)s.x);
+      atomicAdd(p.stats + c + 1, (double)s.y);
+      atomicAdd(p.stats + p.Nc + c, (double)s.z);
+      atomicAdd(p.stats + p.Nc + c + 1, (double)s.w);
+    }
+  }
+}
 
 // Epilogue of tile columns [c_lo, c_hi): thread (q, lane) owns accumulator row q*32+lane of the 128-row tile.  `acc` holds
 // the NC staged columns c_acc .. c_acc+NC-1 of the tile.
@@ -549,8 +711,10 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
 // (forward_x3.cu, compute_dtype 3); tensor maps are FLOAT32 with 32-element boxes, everything else is shared.
 template <int BLOCK_N, int AMODE, int EPI, int STAGES, int KIND = 0>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Params p) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
+            const Params p) {
   static_assert(BLOCK_N == 64 || BLOCK_N == 128 || BLOCK_N == 256, "BLOCK_N");
+  constexpr bool FRAG = frag_epi(BLOCK_N, EPI);          // tmO (output map) is read only by these
   constexpr int SLICE_N = slice_cols(BLOCK_N, EPI);
   using SM = Smem<BLOCK_N, STAGES, SLICE_N>;
   constexpr int S = SM::S;
@@ -572,6 +736,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (warp_idx == 0 && lane == 0) {
     ptx::prefetch_tmap(&tmA);
     ptx::prefetch_tmap(&tmB);
+    if (FRAG) ptx::prefetch_tmap(&tmO);
     for (int s = 0; s < S; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
       ptx::mbar_init(&empty_bar[s], 2);              // one arrive per MMA warpgroup
@@ -636,6 +801,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     const int q = warp_idx & 3;                      // accumulator row quadrant drained by this warp
     const int chalf = (warp_idx - 4) >> 2;           // warps 4..7 take the first half of each staged slice, warps 8..11 the second
     const bool arriver = (warp_idx & 3) == 0 && lane == 0;
+    const bool issuer = FRAG && threadIdx.x == 128;  // issues and waits on the epilogue's TMA stores
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -662,15 +828,21 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       wg::wait<0>();
       wg::fence_operand(d);
       if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
+      if (p.debug_skip_epilogue) continue;
+      if constexpr (FRAG) {
+        frag_epilogue<EPI>(p, d, reinterpret_cast<uint8_t*>(acc_tile), &tmO, m_blk, n_blk, wgi, issuer);
+      } else {
 #pragma unroll
-      for (int s = 0; s < BLOCK_N / SLICE_N; ++s) {
-        ptx::bar_sync(1, 256);                       // the previous slice's (tile's) epilogue reads are done
-        ptx::acc_store_slice<BLOCK_N, SLICE_N>(acc_tile, d, wgi * 64, s);
-        ptx::bar_sync(1, 256);
-        const int c_lo = s * SLICE_N + chalf * (SLICE_N / 2);
-        run_epilogue<BLOCK_N, SLICE_N, EPI>(p, acc_tile, m_blk, n_blk, q, lane, c_lo, c_lo + SLICE_N / 2, s * SLICE_N);
+        for (int s = 0; s < BLOCK_N / SLICE_N; ++s) {
+          ptx::bar_sync(1, 256);                     // the previous slice's (tile's) epilogue reads are done
+          ptx::acc_store_slice<BLOCK_N, SLICE_N>(acc_tile, d, wgi * 64, s);
+          ptx::bar_sync(1, 256);
+          const int c_lo = s * SLICE_N + chalf * (SLICE_N / 2);
+          run_epilogue<BLOCK_N, SLICE_N, EPI>(p, acc_tile, m_blk, n_blk, q, lane, c_lo, c_lo + SLICE_N / 2, s * SLICE_N);
+        }
       }
     }
+    if (FRAG && issuer) ptx::bulk_wait_all();        // the CTA's shared memory must outlive its last stores
   }
 }
 

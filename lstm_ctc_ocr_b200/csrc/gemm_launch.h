@@ -5,8 +5,12 @@
 #include <cstdlib>
 #include <string>
 
+// `out` is the tensor map the register-side epilogues (gemm::frag_epi) store through: NHWC box [64, Wd, bh (x4 merged), 1] for
+// conv outputs, [64, 128] over [M, ldo] for plain ones.  The other epilogues take no map.
 template <int BN, int AM, int EPI, int ST, int KIND = 0>
-static int launch_gemm(const CUtensorMap& a, const CUtensorMap& b, const gemm::Params& p, int num_sms, cudaStream_t st) {
+static int launch_gemm(const CUtensorMap& a, const CUtensorMap& b, const gemm::Params& p, int num_sms, cudaStream_t st,
+                       const CUtensorMap* out = nullptr) {
+  if (gemm::frag_epi(BN, EPI) && out == nullptr) return crnn_fail(CRNN_INVALID_VALUE, "launch_gemm: epilogue %d needs an output tensor map", EPI);
   auto kern = gemm::gemm_kernel<BN, AM, EPI, ST, KIND>;
   constexpr int smem = gemm::Smem<BN, ST, gemm::slice_cols(BN, EPI)>::BYTES;
   static bool attr = false;
@@ -16,7 +20,7 @@ static int launch_gemm(const CUtensorMap& a, const CUtensorMap& b, const gemm::P
   }
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int grid = tiles < num_sms ? tiles : num_sms;
-  kern<<<grid, gemm::NUM_THREADS, smem, st>>>(a, b, p);
+  kern<<<grid, gemm::NUM_THREADS, smem, st>>>(a, b, out ? *out : a, p);
   CUDA_TRY(cudaGetLastError());
   return CRNN_OK;
 }

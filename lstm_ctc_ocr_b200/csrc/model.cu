@@ -374,6 +374,11 @@ static int build_plan(crnn_model* m, int N, int W, void* ws, cudaStream_t st) {
     CRNN_TRY(make_tmap_2d(&pl.tA_h[b], pl.h_state + (size_t)b * 2 * pl.Npad * 256, (uint64_t)2 * pl.Npad, 256, 256, 128));
   CRNN_TRY(make_tmap_2d(&pl.tA_hall, pl.h_state, (uint64_t)4 * pl.Npad, 256, 256, 128));
   CRNN_TRY(make_tmap_2d(&pl.tA_l, pl.lstm_out, (uint64_t)N * pl.H2, 512, 512, 128));
+  CRNN_TRY(make_tmap_nhwc(&pl.tO_c2s, pl.a2, N, pl.H2, 8, 128, 8));             // conv2_swap_kernel's pooled tile: 8 pooled rows
+  CRNN_TRY(make_tmap_nhwc(&pl.tO_c32, pl.a3p, N, pl.H2, 4, 256, pl.mg3 ? 16 : 4));     // conv3_2's pooled tile: 64 positions
+  CRNN_TRY(make_tmap_nhwc(&pl.tO_c41, pl.a4a_pre, N, pl.H2, 4, 512, pl.mg4 ? 32 : 8));
+  CRNN_TRY(make_tmap_nhwc(&pl.tO_c42, pl.a4b_pre, N, pl.H2, 4, 512, pl.mg4 ? 32 : 8));
+  CRNN_TRY(make_tmap_2d(&pl.tO_x, pl.xproj, (uint64_t)N * pl.H2, 2048, 2048, 128));
   // rows t = T (= H2-1) of lstm_out are never produced by a time step: keep them defined (zero)
   CUDA_TRY(cudaMemsetAsync(pl.lstm_out, 0, (size_t)N * pl.H2 * 512 * 2, st));
   if (pl.train) {
@@ -390,6 +395,9 @@ static int build_plan(crnn_model* m, int N, int W, void* ws, cudaStream_t st) {
     CRNN_TRY(make_tmap_nhwc(&pl.tG_p2, pl.d_pre2, N, pl.H1, 16, 128, pl.mg2 ? 8 : 2));
     CRNN_TRY(make_tmap_nhwc(&pl.tG_p2s, pl.d_pre2, N, pl.H1, 16, 128, 8));
     CRNN_TRY(make_tmap_nhwc(&pl.tG_p31s, pl.d_pre31, N, pl.H2, 8, 256, 16));
+    CRNN_TRY(make_tmap_2d(&pl.tO_dlo, pl.d_lstm_out, R, 512, 512, 128));
+    CRNN_TRY(make_tmap_2d(&pl.tO_da4b, pl.d_a4b, R, 1024, 1024, 128));
+    CRNN_TRY(make_tmap_nhwc(&pl.tO_da3p, pl.d_a3p, N, pl.H2, 4, 256, pl.mg4 ? 32 : 8));
     // weight-gradient (TN_CONV) views: 64-position boxes when two sub-boxes are contiguous rows of one image, else 32
     CRNN_TRY(make_tmap_nhwc(&pl.tW_a1, pl.a1, N, pl.H1, 16, 64, pl.wm2 ? 4 : 2));
     CRNN_TRY(make_tmap_nhwc(&pl.tW_p2, pl.d_pre2, N, pl.H1, 16, 128, pl.wm2 ? 4 : 2));
@@ -572,8 +580,8 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
       convsw::Params p;
       p.Nimg = cn; p.img0 = n0; p.H = H1; p.tiles_per_img = (H1 + 15) / 16; p.bias = m->P("conv2/biases"); p.out = pl.a2;
       p.argmax = pl.train ? pl.am2 : nullptr;
-      if (pl.train) CRNN_TRY(launch_conv2_swap<true>(pl.tA_c2s, m->tB_c2, p, sms, st));
-      else CRNN_TRY(launch_conv2_swap<false>(pl.tA_c2s, m->tB_c2, p, sms, st));
+      if (pl.train) CRNN_TRY(launch_conv2_swap<true>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st));
+      else CRNN_TRY(launch_conv2_swap<false>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st));
     } else {
       gemm::Params p = conv_params(N, H1, 16, 64, 128, 128, m->P("conv2/biases"), pl.a2, pl.mg2);
       if (chunks > 1) { p.m_tile0 = n0 * sb2 / 4; p.num_m_tiles = cn * sb2 / 4; }
@@ -589,7 +597,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     {
       gemm::Params p = conv_params(N, H2, 8, 128, 256, 256, m->P("conv3_1/biases"), pl.a3, pl.mg3);
       if (chunks > 1) { p.m_tile0 = n0 * sb3 / 4; p.num_m_tiles = cn * sb3 / 4; }
-      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4>(pl.tA_c31, m->tB_c31, p, sms, st)));
+      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4>(pl.tA_c31, m->tB_c31, p, sms, st, &pl.tA_c32)));
     }
     if (mark) STAGE_MARK();
     // conv3_2 + ReLU + height pool
@@ -600,7 +608,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
         p.argmax = pl.am3;
         CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12_T, 4>(pl.tA_c32, m->tB_c32, p, sms, st)));
       } else {
-        CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12, 4>(pl.tA_c32, m->tB_c32, p, sms, st)));
+        CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12, 4>(pl.tA_c32, m->tB_c32, p, sms, st, &pl.tO_c32)));
       }
     }
     if (mark) STAGE_MARK();
@@ -612,7 +620,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
   {
     gemm::Params p = conv_params(N, H2, 4, 256, 512, 256, m->P("conv4_1/biases"), pl.a4a_pre, pl.mg4);
     p.stats = pl.stats;
-    CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c41, m->tB_c41, p, sms, st)));
+    CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c41, m->tB_c41, p, sms, st, &pl.tO_c41)));
     STAGE_MARK();
     float* bn = pl.bn;
     // batch statistics over the GLOBAL batch when the batch is sharded over ranks: the exchange is fused into the finalize kernel
@@ -629,7 +637,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
   {
     gemm::Params p = conv_params(N, H2, 4, 512, 512, 256, m->P("conv4_2/biases"), pl.a4b_pre, pl.mg4);
     p.stats = pl.stats + 1024;
-    CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c42, m->tB_c42, p, sms, st)));
+    CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c42, m->tB_c42, p, sms, st, &pl.tO_c42)));
     STAGE_MARK();
     float* bn = pl.bn + 2048;
     if (m->dp_world > 1)
@@ -648,7 +656,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     p.M = N * H2;
     p.num_m_tiles = (p.M + 127) / 128; p.num_n_tiles = 2; p.num_k_blocks = 32; p.kb_per_shift = 16; p.row_shift_mul = 1;
     p.Nc = 512; p.bias = m->P("conv5/biases"); p.out = pl.a5; p.ldo = 512;
-    CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tA_c5, m->tB_c5, p, sms, st)));
+    CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tA_c5, m->tB_c5, p, sms, st, &pl.tA_x)));
   }
   STAGE_MARK();
   // LSTM input projection for all frames and both directions: [N*H2, 512] x [512, 2048]
@@ -659,8 +667,8 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     p.num_m_tiles = (p.M + 127) / 128; p.num_n_tiles = 8; p.num_k_blocks = 8; p.kb_per_shift = 8;
     p.Nc = 2048; p.bias = m->xbias; p.out = pl.xproj; p.ldo = 2048;
     p.H = H2; p.T = T; p.seq_len = time_step_len;
-    if (m->lstm_upc == 32) CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_XPROJ, 4>(pl.tA_x, m->tB_x, p, sms, st)));
-    else CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tA_x, m->tB_x, p, sms, st)));
+    if (m->lstm_upc == 32) CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_XPROJ, 4>(pl.tA_x, m->tB_x, p, sms, st, &pl.tO_x)));
+    else CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tA_x, m->tB_x, p, sms, st, &pl.tO_x)));
   }
   STAGE_MARK();
   if (m->lstm_upc == 32) {
@@ -856,7 +864,15 @@ extern "C" int crnn_test_gemm_bf16(const void* A, const void* B, float* D, int M
   p.num_m_tiles = (M + 127) / 128; p.num_n_tiles = Nc / block_n; p.num_k_blocks = K / 64; p.kb_per_shift = p.num_k_blocks;
   p.out = D;
   if (const char* e = getenv("CRNN_PROBE_SKIP_TMA")) p.debug_skip_tma = (e[0] == '1');
+  if (const char* e = getenv("CRNN_PROBE_SKIP_EPI")) p.debug_skip_epilogue = (e[0] == '1');
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  // probe: CRNN_PROBE_BF16_OUT=1 writes D as bf16 [M, Nc] (EPI_BIAS_BF16 without bias, the register-side epilogue with TMA stores)
+  if (const char* e = getenv("CRNN_PROBE_BF16_OUT"); e && e[0] == '1' && block_n == 256) {
+    CUtensorMap to;
+    CRNN_TRY(make_tmap_2d(&to, D, M, Nc, Nc, 128));
+    p.ldo = Nc;
+    return launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(ta, tb, p, sms, st, &to);
+  }
   if (block_n == 64) return launch_gemm<64, gemm::A_PLAIN, gemm::EPI_F32, 8>(ta, tb, p, sms, st);
   if (block_n == 128) return launch_gemm<128, gemm::A_PLAIN, gemm::EPI_F32, 6>(ta, tb, p, sms, st);
   if (block_n == 256) return launch_gemm<256, gemm::A_PLAIN, gemm::EPI_F32, 4>(ta, tb, p, sms, st);

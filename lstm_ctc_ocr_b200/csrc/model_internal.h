@@ -51,6 +51,9 @@ struct Plan {
   float* bn;            // [2 layers][4][512]: scale, shift, mean, invstd
   CUtensorMap tA_c2s;   // conv2 input through 128-position boxes regardless of H (swapped-operand kernel, conv_swap.cuh)
   CUtensorMap tA_c2, tA_c31, tA_c32, tA_c41, tA_c42, tA_c5, tA_x, tA_h[2], tA_l, tA_hall;
+  // output maps of the register-side GEMM epilogues (gemm::frag_epi) where no input map above has the producing layer's tile
+  // geometry: conv3_1 stores through tA_c32 and conv5 through tA_x
+  CUtensorMap tO_c2s, tO_c32, tO_c41, tO_c42, tO_x;
   // conv A maps use 128-position boxes (`mg*` = 1) when a tile's 4 sub-boxes are contiguous rows of one image;
   // the weight-gradient GEMMs read the same tensors through 64- or 32-position boxes (tW_*)
   int mg2 = 0, mg3 = 0, mg4 = 0, wm2 = 0, wm3 = 0, wm4 = 0;
@@ -68,6 +71,7 @@ struct Plan {
   // K-major A maps of gradient buffers (data-gradient GEMMs)
   CUtensorMap tG_dl, tG_dz, tG_da5, tG_p4b, tG_p4a, tG_p32, tG_p31, tG_p2, tG_dzstate;
   CUtensorMap tG_p2s, tG_p31s;                    // d_pre2 / d_pre31 through 128-position boxes regardless of H (conv_dgrad_swap_kernel)
+  CUtensorMap tO_dlo, tO_da4b, tO_da3p;           // data-gradient GEMM outputs (the others store through tG_da5 / tG_p4a / tG_p31)
   // MN-major (TN) maps: 2-D [rows, C] with 64x64 boxes, and the NHWC maps above reused for TN_CONV
   CUtensorMap tT_lstm_fw, tT_lstm_bw, tT_lstm_all, tT_dl, tT_a5, tT_dz, tT_dz_fw, tT_dz_bw, tT_a4b, tT_da5;
 };

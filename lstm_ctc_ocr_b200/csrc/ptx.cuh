@@ -68,6 +68,8 @@ __device__ __forceinline__ void bulk_store_1d(void* dst_gmem, const void* src_sm
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// every committed bulk group of this thread has completed (writes included): before a CTA that issued stores exits
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // 1-D bulk copy global -> the SAME smem offset of every CTA in `cta_mask`; each destination's mbarrier (same offset) gets the bytes
 __device__ __forceinline__ void bulk_load_1d_mc(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar, uint16_t cta_mask) {
@@ -103,6 +105,11 @@ __device__ __forceinline__ void red_add_v4_f32(float* addr, float a, float b, fl
 __device__ __forceinline__ void tma_store_4d(const void* tmap, const void* src, int c0, int c1, int c2, int c3) {
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
                ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void tma_store_2d(const void* tmap, const void* src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(src)), "r"(c0), "r"(c1)
                : "memory");
 }
 

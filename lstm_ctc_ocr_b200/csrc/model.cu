@@ -374,6 +374,7 @@ static int build_plan(crnn_model* m, int N, int W, void* ws, cudaStream_t st) {
     CRNN_TRY(make_tmap_2d(&pl.tA_h[b], pl.h_state + (size_t)b * 2 * pl.Npad * 256, (uint64_t)2 * pl.Npad, 256, 256, 128));
   CRNN_TRY(make_tmap_2d(&pl.tA_hall, pl.h_state, (uint64_t)4 * pl.Npad, 256, 256, 128));
   CRNN_TRY(make_tmap_2d(&pl.tA_l, pl.lstm_out, (uint64_t)N * pl.H2, 512, 512, 128));
+  CRNN_TRY(make_tmap_nhwc(&pl.tO_c1, pl.a1, N, pl.H1, 16, 64, 4));               // conv1_tc_kernel's pooled warpgroup tile: 4 pooled rows
   CRNN_TRY(make_tmap_nhwc(&pl.tO_c2s, pl.a2, N, pl.H2, 8, 128, 8));             // conv2_swap_kernel's pooled tile: 8 pooled rows
   CRNN_TRY(make_tmap_nhwc(&pl.tO_c32, pl.a3p, N, pl.H2, 4, 256, pl.mg3 ? 16 : 4));     // conv3_2's pooled tile: 64 positions
   CRNN_TRY(make_tmap_nhwc(&pl.tO_c41, pl.a4a_pre, N, pl.H2, 4, 512, pl.mg4 ? 32 : 8));
@@ -568,7 +569,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     {
       const size_t o1 = (size_t)n0 * H1 * 16 * 64;
       if (m->conv1_tc)
-        CRNN_TRY(launch_conv1_tc(data + (size_t)n0 * W * 32, m->P("conv1/weights"), m->P("conv1/biases"), pl.a1 + o1,
+        CRNN_TRY(launch_conv1_tc(pl.tO_c1, data + (size_t)n0 * W * 32, m->P("conv1/weights"), m->P("conv1/biases"), n0,
                                  pl.train ? pl.am1 + o1 : nullptr, cn, W, sms, st));
       else
         CRNN_TRY(launch_conv1_pool(data + (size_t)n0 * W * 32, m->P("conv1/weights"), m->P("conv1/biases"), pl.a1 + o1,

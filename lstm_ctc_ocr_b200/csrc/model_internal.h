@@ -52,8 +52,8 @@ struct Plan {
   CUtensorMap tA_c2s;   // conv2 input through 128-position boxes regardless of H (swapped-operand kernel, conv_swap.cuh)
   CUtensorMap tA_c2, tA_c31, tA_c32, tA_c41, tA_c42, tA_c5, tA_x, tA_h[2], tA_l, tA_hall;
   // output maps of the register-side GEMM epilogues (gemm::frag_epi) where no input map above has the producing layer's tile
-  // geometry: conv3_1 stores through tA_c32 and conv5 through tA_x
-  CUtensorMap tO_c2s, tO_c32, tO_c41, tO_c42, tO_x;
+  // geometry: conv3_1 stores through tA_c32 and conv5 through tA_x; conv1_tc_kernel stores its pooled tiles through tO_c1
+  CUtensorMap tO_c1, tO_c2s, tO_c32, tO_c41, tO_c42, tO_x;
   // conv A maps use 128-position boxes (`mg*` = 1) when a tile's 4 sub-boxes are contiguous rows of one image;
   // the weight-gradient GEMMs read the same tensors through 64- or 32-position boxes (tW_*)
   int mg2 = 0, mg3 = 0, mg4 = 0, wm2 = 0, wm3 = 0, wm4 = 0;

@@ -203,9 +203,18 @@ int     crnn_peer_error(crnn_model* m, int* err_host);   /* 1 if an exchange tim
 
 /* Debug/parity taps: copy a named intermediate of the last crnn_forward() as f32 into dst.
  * names: "conv1" "conv2" "conv3_1" "conv3_2" "conv4_1" "conv4_2" "conv5" "lstm_out"
- * (pooled / post-activation, NHWC, as the reference's layers dict holds them). */
+ * (pooled / post-activation, NHWC, as the reference's layers dict holds them), "xproj" (input projection,
+ * permuted gate columns, backward-direction rows reversed by length), "a4a_pre" "a4b_pre" (conv4_x before BatchNorm).
+ * Training-mode plans only (CRNN_INVALID_VALUE otherwise): "gates" (saved post-activation gates, layout of
+ * lstm_gate_off) and the backward buffers "dl_rows" "d_lstm_out" "dz_all" "d_a5" "d_a4b" "d_pre4b" "d_pre4a"
+ * "d_a3p" "d_pre32" "d_pre31" "d_a2" "d_pre2" "d_a1" of the last crnn_backward(). */
 int     crnn_debug_tap(crnn_model* m, const char* name, float* dst, size_t dst_elems,
                        void* workspace, crnn_stream_t stream);
+/* Same for the buffers that are not bf16, copied byte for byte: "bn" (f32 [2 layers][scale, shift, mean, invstd][512]),
+ * "stats" (f64 [2 layers][sum, sum of squares][512]) and, training-mode plans only, "am1" "am2" "am3" (u8 pool
+ * window index dy*2+dx per pooled element) and "csave" (f32 saved cell state, layout of lstm_c_off). */
+int     crnn_debug_tap_raw(crnn_model* m, const char* name, void* dst, size_t dst_bytes,
+                           void* workspace, crnn_stream_t stream);
 
 /* Per-stage timing of crnn_forward with CUDA events recorded on the caller's stream (bench.py's roofline line).
  * crnn_profile_begin arms the next `max_forwards` forward calls; crnn_profile_read synchronises on the events and

@@ -43,6 +43,7 @@ SIGNATURES = {
     "crnn_host_copy": (c_int, [c_void_p, c_void_p, c_size_t, c_int]),
     "crnn_total_loss": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "crnn_debug_tap": (c_int, [c_void_p, c_char_p, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "crnn_debug_tap_raw": (c_int, [c_void_p, c_char_p, c_void_p, c_size_t, c_void_p, c_void_p]),
     "crnn_profile_begin": (c_int, [c_void_p, c_int]),
     "crnn_profile_num_stages": (c_int, []),
     "crnn_profile_stage_name": (c_char_p, [c_int]),

@@ -844,9 +844,51 @@ extern "C" int crnn_debug_tap(crnn_model* m, const char* name, float* dst, size_
   else if (s == "conv5") { src = pl.a5; cnt = n * h2 * 512; }
   else if (s == "lstm_out") { src = pl.lstm_out; cnt = n * h2 * 512; }
   else if (s == "xproj") { src = pl.xproj; cnt = n * h2 * 2048; }
-  else return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: unknown tap %s", name);
+  else if (s == "a4a_pre") { src = pl.a4a_pre; cnt = n * h2 * 4 * 512; }
+  else if (s == "a4b_pre") { src = pl.a4b_pre; cnt = n * h2 * 4 * 512; }
+  else {
+    // saved state and backward buffers: only a training-mode plan holds them
+    const struct { const char* name; const __nv_bfloat16* p; size_t cnt; } train_taps[] = {
+        {"gates", pl.gates, (size_t)2 * pl.Npad * pl.T * 1024}, {"dl_rows", pl.dl_rows, n * h2 * 64},
+        {"d_lstm_out", pl.d_lstm_out, n * h2 * 512},           {"dz_all", pl.dz_all, n * h2 * 2048},
+        {"d_a5", pl.d_a5, n * h2 * 512},                       {"d_a4b", pl.d_a4b, n * h2 * 2 * 512},
+        {"d_pre4b", pl.d_pre4b, n * h2 * 4 * 512},             {"d_pre4a", pl.d_pre4a, n * h2 * 4 * 512},
+        {"d_a3p", pl.d_a3p, n * h2 * 4 * 256},                 {"d_pre32", pl.d_pre32, n * h2 * 8 * 256},
+        {"d_pre31", pl.d_pre31, n * h2 * 8 * 256},             {"d_a2", pl.d_a2, n * h2 * 8 * 128},
+        {"d_pre2", pl.d_pre2, n * h1 * 16 * 128},              {"d_a1", pl.d_a1, n * h1 * 16 * 64}};
+    for (auto& t : train_taps)
+      if (s == t.name) {
+        if (!pl.train) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: %s exists only in a training-mode plan", name);
+        src = t.p; cnt = t.cnt;
+      }
+    if (src == nullptr) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: unknown tap %s", name);
+  }
   if (dst_elems < cnt) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: dst too small (%zu < %zu)", dst_elems, cnt);
   return launch_bf16_to_f32(src, dst, cnt, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int crnn_debug_tap_raw(crnn_model* m, const char* name, void* dst, size_t dst_bytes, void* workspace,
+                                  crnn_stream_t stream) {
+  if (!m || !name || !dst) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: null");
+  if (m->cfg.compute_dtype >= 2) return crnn_fail(CRNN_UNSUPPORTED, "debug_tap_raw: only the bf16 path (compute_dtype 1) has these buffers");
+  Plan& pl = m->plan;
+  if (pl.ws == nullptr || pl.ws != workspace) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: no forward ran on this workspace");
+  const size_t n = pl.N, h1 = pl.H1, h2 = pl.H2;
+  const void* src = nullptr;
+  size_t bytes = 0;
+  bool train_only = false;
+  std::string s(name);
+  if (s == "bn") { src = pl.bn; bytes = 2 * 4 * 512 * sizeof(float); }
+  else if (s == "stats") { src = pl.stats; bytes = 2 * 2 * 512 * sizeof(double); }
+  else if (s == "am1") { src = pl.am1; bytes = n * h1 * 16 * 64; train_only = true; }
+  else if (s == "am2") { src = pl.am2; bytes = n * h2 * 8 * 128; train_only = true; }
+  else if (s == "am3") { src = pl.am3; bytes = n * h2 * 4 * 256; train_only = true; }
+  else if (s == "csave") { src = pl.csave; bytes = (size_t)2 * pl.Npad * pl.T * 256 * sizeof(float); train_only = true; }
+  else return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: unknown tap %s", name);
+  if (train_only && !pl.train) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: %s exists only in a training-mode plan", name);
+  if (dst_bytes < bytes) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: dst too small (%zu < %zu bytes)", dst_bytes, bytes);
+  CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, reinterpret_cast<cudaStream_t>(stream)));
+  return CRNN_OK;
 }
 
 extern "C" int crnn_test_gemm_bf16(const void* A, const void* B, float* D, int M, int Nc, int K, int block_n,

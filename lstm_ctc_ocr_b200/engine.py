@@ -186,15 +186,38 @@ class CrnnModel:
         return out, self._stage, self._copy_stream
 
     def tap(self, name, N, W):
-        """Intermediate of the last forward as f32 NHWC (tests only)."""
+        """Intermediate of the last forward (or, for the backward buffers, the last backward) as f32 NHWC (tests only)."""
         H1, H2 = W // 2, W // 4
+        Npad, T = (N + 127) // 128 * 128, H2 - 1
         shapes = {"conv1": (N, H1, 16, 64), "conv2": (N, H2, 8, 128), "conv3_1": (N, H2, 8, 256),
                   "conv3_2": (N, H2, 4, 256), "conv4_1": (N, H2, 4, 512), "conv4_2": (N, H2, 2, 512),
-                  "conv5": (N, H2, 512), "lstm_out": (N, H2, 512), "xproj": (N, H2, 2048)}
+                  "conv5": (N, H2, 512), "lstm_out": (N, H2, 512), "xproj": (N, H2, 2048),
+                  "a4a_pre": (N, H2, 4, 512), "a4b_pre": (N, H2, 4, 512),
+                  # training only; gates: [dir * Npad/128 + tile][step][gate i,j,f,o][unit / 8][row][unit % 8]
+                  "gates": (2 * Npad // 128, T, 4, 32, 128, 8), "dl_rows": (N, H2, 64), "d_lstm_out": (N, H2, 512),
+                  "dz_all": (N, H2, 2048), "d_a5": (N, H2, 512), "d_a4b": (N, H2, 2, 512), "d_pre4b": (N, H2, 4, 512),
+                  "d_pre4a": (N, H2, 4, 512), "d_a3p": (N, H2, 4, 256), "d_pre32": (N, H2, 8, 256),
+                  "d_pre31": (N, H2, 8, 256), "d_a2": (N, H2, 8, 128), "d_pre2": (N, H1, 16, 128), "d_a1": (N, H1, 16, 64)}
         shp = shapes[name]
         dst = torch.empty(shp, dtype=torch.float32, device=self.device)
         ws, _ = self._workspace(N, W)
         check(self.lib.crnn_debug_tap(self.handle, name.encode(), dst.data_ptr(), dst.numel(), ws, _stream()))
+        return dst
+
+    def tap_raw(self, name, N, W):
+        """Non-bf16 workspace buffer of the last forward, byte for byte (tests only): "bn" f32 [2][4][512] (scale, shift,
+        mean, invstd per BN layer), "stats" f64 [2][2][512]; training only: "am1" / "am2" / "am3" u8 pool window index
+        (dy*2+dx) in the pooled NHWC shape, "csave" f32 [dir * Npad/128 + tile][step][unit / 4][row][unit % 4]."""
+        H1, H2 = W // 2, W // 4
+        Npad, T = (N + 127) // 128 * 128, H2 - 1
+        shapes = {"bn": ((2, 4, 512), torch.float32), "stats": ((2, 2, 512), torch.float64),
+                  "am1": ((N, H1, 16, 64), torch.uint8), "am2": ((N, H2, 8, 128), torch.uint8),
+                  "am3": ((N, H2, 4, 256), torch.uint8), "csave": ((2 * Npad // 128, T, 64, 128, 4), torch.float32)}
+        shp, dt = shapes[name]
+        dst = torch.empty(shp, dtype=dt, device=self.device)
+        ws, _ = self._workspace(N, W)
+        check(self.lib.crnn_debug_tap_raw(self.handle, name.encode(), dst.data_ptr(), dst.numel() * dst.element_size(), ws,
+                                          _stream()))
         return dst
 
     # ---- loss / decode ------------------------------------------------------------------------

@@ -1,0 +1,503 @@
+"""fp64 restatements of every stage of the bf16 forward and backward path, each on that stage's OWN inputs.
+
+A stage function takes the operands the kernel reads (bf16 activations / gradients read back from the workspace, weights
+rounded to bf16 as prepare_weights() rounds them, f32 biases) as fp64 CPU tensors in the workspace layouts (NHWC, permuted
+LSTM gate columns, reversed backward-direction rows, time-major logits) and returns the stage's output computed in fp64.
+With the kernel's own inputs the only legitimate differences are the order of the f32 accumulation and the final rounding,
+so a test can bound each element by about one bf16 ulp plus a small multiple of `acc`: the same operation applied to
+|inputs| and |weights|, i.e. the scale the accumulation error is relative to.
+
+Data and weight gradients are written as tiny fp64 torch functions differentiated by torch.autograd.grad with the GPU's own
+upstream gradient as grad_outputs; `acc` is the same vector-Jacobian product on absolute values.
+
+`rnd` is the rounding the kernels apply INSIDE a stage (the bf16 h a recurrence step exchanges, the bf16 values the pool3
+backward compares).  The GPU tests pass `bf16`; tests/test_stage_refs_cpu.py passes `ident` and chains the stages from the
+oracle's fp64 activations, which must then reproduce the oracle's forward and gradients.
+
+Test infrastructure only (imported by tests/)."""
+import numpy as np
+import torch
+import torch.nn.functional as F
+
+HID = 256
+UPC = 32            # hidden units per [i|j|f|o] column group of the permuted LSTM layout (lstm_perm in kernels.cu)
+
+
+def bf16(x):
+    """Round to bf16 the way the kernels do (f32 value, then round-to-nearest-even)."""
+    return x.float().to(torch.bfloat16).double()
+
+
+def f32(x):
+    return x.float().double()
+
+
+def ident(x):
+    return x
+
+
+def nchw(x):
+    return x.permute(0, 3, 1, 2)
+
+
+def nhwc(x):
+    return x.permute(0, 2, 3, 1)
+
+
+# ---------------------------------------------------------------------------------------------------------- layouts
+def gate_perm(upc=UPC):
+    """TF gate column j = g*256 + u  ->  its column in the permuted [1024] layout (kernels.cu: lstm_perm)."""
+    j = np.arange(4 * HID)
+    g, u = j // HID, j % HID
+    return torch.as_tensor((u // upc) * 4 * upc + g * upc + u % upc)
+
+
+def to_perm(z):
+    """[..., 1024] TF gate order -> permuted column order."""
+    out = torch.empty_like(z)
+    out[..., gate_perm()] = z
+    return out
+
+
+def from_perm(z):
+    """[..., 1024] permuted column order -> TF gate order."""
+    return z[..., gate_perm()]
+
+
+def clamp_lens(lens, T):
+    return [min(max(int(v), 0), T) for v in lens]
+
+
+def reverse_rows(x, lens, T):
+    """tf.reverse_sequence over axis 1 of [N, H2, C]: row t < len goes to len-1-t, rows t >= len stay (an involution)."""
+    y = x.clone()
+    for n, L in enumerate(clamp_lens(lens, T)):
+        if L > 0:
+            y[n, :L] = x[n, :L].flip(0)
+    return y
+
+
+def unpack_gates(g, N):
+    """Workspace `gates` [2*tiles, T, 4, 32, 128, 8] (common.cuh: lstm_gate_off) -> [2 dirs, N, T steps, 4 gates, 256]."""
+    tiles = g.shape[0] // 2
+    T = g.shape[1]
+    return g.reshape(2, tiles, T, 4, 32, 128, 8).permute(0, 1, 5, 2, 3, 4, 6).reshape(2, tiles * 128, T, 4, HID)[:, :N]
+
+
+def pack_gates(g, Npad):
+    """Inverse of unpack_gates (rows past N zero)."""
+    _, N, T, _, _ = g.shape
+    full = g.new_zeros((2, Npad, T, 4, HID))
+    full[:, :N] = g
+    return full.reshape(2, Npad // 128, 128, T, 4, 32, 8).permute(0, 1, 3, 4, 5, 2, 6).reshape(2 * Npad // 128, T, 4, 32, 128, 8)
+
+
+def unpack_csave(c, N):
+    """Workspace `csave` [2*tiles, T, 64, 128, 4] (common.cuh: lstm_c_off) -> [2 dirs, N, T steps, 256]."""
+    tiles = c.shape[0] // 2
+    T = c.shape[1]
+    return c.reshape(2, tiles, T, 64, 128, 4).permute(0, 1, 4, 2, 3, 5).reshape(2, tiles * 128, T, HID)[:, :N]
+
+
+def pack_csave(c, Npad):
+    _, N, T, _ = c.shape
+    full = c.new_zeros((2, Npad, T, HID))
+    full[:, :N] = c
+    return full.reshape(2, Npad // 128, 128, T, 64, 4).permute(0, 1, 3, 4, 2, 5).reshape(2 * Npad // 128, T, 64, 128, 4)
+
+
+# ---------------------------------------------------------------------------------------------------------- helpers
+def _conv(x, w_hwio, b=None, padding=1):
+    """NHWC x HWIO -> NHWC (fp64), SAME for 3x3 (padding 1), VALID for padding 0."""
+    return nhwc(F.conv2d(nchw(x), w_hwio.permute(3, 2, 0, 1), b, padding=padding))
+
+
+def _conv_acc(x, w, b, padding=1):
+    y = _conv(x, w, b, padding)
+    acc = _conv(x.abs(), w.abs(), None if b is None else b.abs(), padding)
+    return y, acc
+
+
+def pool22(x):
+    """2x2 max pool of NHWC [N, H, W, C] -> (max, first arg-max dy*2+dx)."""
+    N, H, W, C = x.shape
+    v = x.reshape(N, H // 2, 2, W // 2, 2, C).permute(0, 1, 3, 5, 2, 4).reshape(N, H // 2, W // 2, C, 4)
+    return v.max(dim=-1).values, first_argmax(v)
+
+
+def pool12(x):
+    """1x2 max pool over the W axis of NHWC [N, H, W, C] -> (max, first arg-max dx)."""
+    N, H, W, C = x.shape
+    v = x.reshape(N, H, W // 2, 2, C).permute(0, 1, 2, 4, 3)
+    m, _ = v.max(dim=-1)
+    return m, first_argmax(v)
+
+
+def first_argmax(v):
+    """Index of the FIRST maximum along the last axis."""
+    m = v.max(dim=-1, keepdim=True).values
+    k = v.shape[-1]
+    idx = torch.arange(k).expand_as(v)
+    return torch.where(v == m, idx, torch.full_like(idx, k)).min(dim=-1).values
+
+
+def windows22(x):
+    """The four values of each 2x2 window of NHWC x, window index dy*2+dx last: [N, H/2, W/2, C, 4]."""
+    N, H, W, C = x.shape
+    return x.reshape(N, H // 2, 2, W // 2, 2, C).permute(0, 1, 3, 5, 2, 4).reshape(N, H // 2, W // 2, C, 4)
+
+
+def windows12(x):
+    N, H, W, C = x.shape
+    return x.reshape(N, H, W // 2, 2, C).permute(0, 1, 2, 4, 3)
+
+
+def vjp(fn, inputs, dy):
+    """fp64 autograd: gradients of fn(*inputs) w.r.t. every input, with dy as grad_outputs."""
+    xs = [t.detach().clone().requires_grad_(True) for t in inputs]
+    return [g.detach() if g is not None else None for g in torch.autograd.grad(fn(*xs), xs, dy, allow_unused=True)]
+
+
+def vjp_acc(fn, inputs, dy):
+    """(gradients, accumulation scale): the same vector-Jacobian product on |inputs| and |dy| (fn must be multilinear)."""
+    return vjp(fn, inputs, dy), vjp(fn, [t.abs() for t in inputs], dy.abs())
+
+
+# ---------------------------------------------------------------------------------------------------------- forward stages
+def conv1_stage(data, w, b):
+    """conv1 (3x3 SAME, Cin 1) + bias + ReLU + 2x2 pool.  data [N, W, 32] and w, b as f32 values (the kernel's split-bf16
+    operands drop only the lo*lo term).  Returns out [N, W/2, 16, 64], acc, pre (conv + bias before ReLU), am."""
+    x = data[..., None]
+    pre, acc = _conv_acc(x, w, b)
+    out, am = pool22(torch.relu(pre))
+    return dict(out=out, acc=windows22(acc).max(-1).values, pre=pre, am=am)
+
+
+def conv_relu_pool22_stage(x, w, b):
+    """conv2: 3x3 SAME + bias + ReLU + 2x2 pool."""
+    pre, acc = _conv_acc(x, w, b)
+    out, am = pool22(torch.relu(pre))
+    return dict(out=out, acc=windows22(acc).max(-1).values, pre=pre, am=am)
+
+
+def conv_relu_stage(x, w, b):
+    """conv3_1: 3x3 SAME + bias + ReLU."""
+    pre, acc = _conv_acc(x, w, b)
+    return dict(out=torch.relu(pre), acc=acc, pre=pre)
+
+
+def conv_relu_pool12_stage(x, w, b):
+    """conv3_2: 3x3 SAME + bias + ReLU + 1x2 pool over the image-height axis."""
+    pre, acc = _conv_acc(x, w, b)
+    out, am = pool12(torch.relu(pre))
+    return dict(out=out, acc=windows12(acc).max(-1).values, pre=pre, am=am)
+
+
+def conv_bias_stage(x, w, b):
+    """conv4_x GEMM (EPI_STATS): 3x3 SAME + bias, the pre-BatchNorm activation."""
+    out, acc = _conv_acc(x, w, b)
+    return dict(out=out, acc=acc)
+
+
+def bn_stats_stage(x_pre, gamma, beta, eps):
+    """Batch statistics over every position of x_pre [N, H2, 4, C] (kernels.cu: bn_finalize_kernel): sums, mean, population
+    variance, invstd, scale = gamma*invstd, shift = beta - mean*scale."""
+    x = x_pre.reshape(-1, x_pre.shape[-1])
+    cnt = x.shape[0]
+    s1, s2 = x.sum(0), (x * x).sum(0)
+    mean = s1 / cnt
+    var = (s2 / cnt - mean * mean).clamp_min(0)
+    invstd = 1.0 / torch.sqrt(var + eps)
+    scale = gamma * invstd
+    # error scales of the coefficients derived from (slightly perturbed) sums: the mean cancels down from sum|x| / cnt, the
+    # variance E[x^2] - mean^2 amplifies relative errors of the sums by E[x^2] / var, and the shift cancels beta against
+    # mean * scale
+    mean_acc = x.abs().sum(0) / cnt
+    cond = (s2 / cnt) / (var + eps)
+    acc = dict(mean=mean_acc, invstd=invstd.abs() * cond, scale=scale.abs() * cond,
+               shift=beta.abs() + scale.abs() * (mean_acc + mean.abs() * cond))
+    return dict(sum=s1, sumsq=s2, sum_acc=x.abs().sum(0), mean=mean, var=var, invstd=invstd, scale=scale,
+                shift=beta - mean * scale, acc=acc)
+
+
+def bn_apply_relu_stage(x_pre, scale, shift):
+    """max(x*scale + shift, 0) with the workspace's f32 scale / shift."""
+    y = x_pre * scale + shift
+    return dict(out=torch.relu(y), acc=(x_pre * scale).abs() + shift.abs())
+
+
+def bn_apply_relu_pool_stage(x_pre, scale, shift, rnd=bf16):
+    """pool3: max over image-height pairs of rnd(max(x*scale + shift, 0)) (the pair is compared after the per-position
+    rounding, kernels.cu: bn_apply_relu_pool12_kernel)."""
+    y = torch.relu(x_pre * scale + shift)
+    out, _ = pool12(rnd(y))
+    acc = windows12((x_pre * scale).abs() + shift.abs()).max(-1).values
+    return dict(out=out, acc=acc)
+
+
+def conv5_stage(a4b, w, b):
+    """conv5: 2x2 VALID over [N, H2, 2, 512] -> [N, T, 512] (frames t < T)."""
+    y, acc = _conv_acc(a4b, w, b, padding=0)
+    return dict(out=y[:, :, 0, :], acc=acc[:, :, 0, :])
+
+
+def xproj_stage(a5, wx_fw, wx_bw, b_fw, b_bw, lens, T, bias_rnd=f32):
+    """Input projection of both directions for all H2 rows of a5 [N, H2, 512]: z = a5 Wx + b (+1 on the forget gate, added
+    in f32 by lstm_bias_prep: `bias_rnd`), gate columns permuted, backward-direction rows reversed by length (rows t >= len,
+    the padding row t = T included, stay)."""
+    outs, accs = [], []
+    for d, (wx, b) in enumerate(((wx_fw, b_fw), (wx_bw, b_bw))):
+        bias = bias_rnd(b + torch.cat([torch.zeros(2 * HID), torch.ones(HID), torch.zeros(HID)]).to(b.dtype))
+        z = to_perm(a5 @ wx + bias)
+        acc = to_perm(a5.abs() @ wx.abs() + bias.abs())
+        if d == 1:
+            z, acc = reverse_rows(z, lens, T), reverse_rows(acc, lens, T)
+        outs.append(z)
+        accs.append(acc)
+    return dict(out=torch.cat(outs, -1), acc=torch.cat(accs, -1))
+
+
+def _cell(z, c_prev):
+    i, j, f, o = torch.sigmoid(z[..., :HID]), torch.tanh(z[..., HID:2 * HID]), torch.sigmoid(z[..., 2 * HID:3 * HID]), \
+        torch.sigmoid(z[..., 3 * HID:])
+    c = f * c_prev + i * j
+    return torch.stack([i, j, f, o], -2), c, o * torch.tanh(c)
+
+
+def recurrence_stage(xproj, wh_fw, wh_bw, lens, T, rnd=bf16):
+    """Both LSTM directions over T steps from the projected inputs `xproj` (workspace layout) and W_h [256, 1024]; h is
+    rounded by `rnd` before it feeds the next step.  Returns lstm_out [N, H2, 512] (frames t >= len and the padding row
+    zero), gates [2, N, T, 4, 256] and c [2, N, T, 256] per STEP (valid for steps < len)."""
+    N, H2, _ = xproj.shape
+    L = torch.as_tensor(clamp_lens(lens, T))
+    out = xproj.new_zeros((N, H2, 2 * HID))
+    gates = xproj.new_zeros((2, N, T, 4, HID))
+    cs = xproj.new_zeros((2, N, T, HID))
+    ar = torch.arange(N)
+    for d, wh in enumerate((wh_fw, wh_bw)):
+        xd = from_perm(xproj[..., d * 1024:(d + 1) * 1024])
+        h = xproj.new_zeros((N, HID))
+        c = xproj.new_zeros((N, HID))
+        for s in range(T):
+            act = (s < L)[:, None]
+            g, c_new, h_new = _cell(xd[:, s] + h @ wh, c)
+            gates[d, :, s] = g
+            cs[d, :, s] = c_new
+            t = torch.where(L > s, (L - 1 - s) if d else torch.full_like(L, s), torch.full_like(L, s))
+            sel = (s < L)
+            out[ar[sel], t[sel], d * HID:(d + 1) * HID] = h_new[sel]
+            c = torch.where(act, c_new, c)
+            h = torch.where(act, rnd(h_new), h)
+    return dict(out=out, gates=gates, c=cs)
+
+
+def recurrence_steps_isolated(xproj, wh_fw, wh_bw, lstm_out, c_steps, lens, T):
+    """Every recurrence step on its own inputs: z = xproj row + h_prev W_h with h_prev the step's predecessor read back from
+    `lstm_out` (the bf16 h the kernel exchanged) and c_prev from the saved cell state `c_steps` [2, N, T, 256].  Returns
+    gates / c [2, N, T, ...] and h [2, N, T, 256] per step (rows of steps >= len meaningless)."""
+    N = xproj.shape[0]
+    L = torch.as_tensor(clamp_lens(lens, T))
+    gates = xproj.new_zeros((2, N, T, 4, HID))
+    cs = xproj.new_zeros((2, N, T, HID))
+    hs = xproj.new_zeros((2, N, T, HID))
+    s = torch.arange(T)
+    for d, wh in enumerate((wh_fw, wh_bw)):
+        xd = from_perm(xproj[:, :T, d * 1024:(d + 1) * 1024])                     # [N, T(step), 1024]
+        # frame of step s, and of its predecessor s-1 (h_prev = 0 at s = 0)
+        t_of = (L[:, None] - 1 - s[None, :]).clamp_min(0) if d else s[None, :].expand(N, T)
+        ho = lstm_out[..., d * HID:(d + 1) * HID]
+        h_prev = torch.zeros((N, T, HID), dtype=xproj.dtype)
+        c_prev = torch.zeros((N, T, HID), dtype=xproj.dtype)
+        if T > 1:
+            h_prev[:, 1:] = torch.gather(ho, 1, t_of[:, :-1, None].expand(N, T - 1, HID))
+            c_prev[:, 1:] = c_steps[d, :, :-1]
+        g, c, h = _cell(xd + h_prev @ wh, c_prev)
+        gates[d], cs[d], hs[d] = g, c, h
+    return dict(gates=gates, c=cs, h=hs)
+
+
+def logits_stage(lstm_out, wl, bl, T):
+    """512 -> 64 projection of frames t < T, time-major [T, N, 64] (frames past len see zero rows: the bias alone)."""
+    x = lstm_out[:, :T]
+    y = x @ wl + bl
+    acc = x.abs() @ wl.abs() + bl.abs()
+    return dict(out=y.permute(1, 0, 2), acc=acc.permute(1, 0, 2))
+
+
+# ---------------------------------------------------------------------------------------------------------- backward stages
+def dl_rows_stage(dlogits, H2):
+    """dlogits [T, N, 64] (time-major) -> frame rows [N, H2, 64] (padding row t = T zero) and the logits bias gradient."""
+    T, N, _ = dlogits.shape
+    rows = dlogits.new_zeros((N, H2, 64))
+    rows[:, :T] = dlogits.permute(1, 0, 2)
+    return dict(dl_rows=rows, dbias=dlogits.sum((0, 1)), dbias_acc=dlogits.abs().sum((0, 1)))
+
+
+def logits_bwd(lstm_out, dl_rows, wl):
+    """From the frame rows of d logits: the 512 -> 64 weight gradient and d_lstm_out."""
+    (dx, dw), (ax, aw) = vjp_acc(lambda x, w: x @ w, [lstm_out, wl], dl_rows)
+    return dict(dw=dw, dw_acc=aw, d_lstm_out=dx, d_lstm_out_acc=ax)
+
+
+def bptt_stage(d_out, gates, c_steps, wh_fw, wh_bw, lens, T, dz_in=None, rnd=bf16):
+    """Backward recurrence of both directions.  gates [2, N, T, 4, 256] / c_steps [2, N, T, 256] are the saved per-step
+    values, d_out [N, H2, 512] the gradient w.r.t. lstm_out.  dz of step s+1 enters step s through W_h^T: taken from
+    `dz_in` (the workspace's dz_all: the bf16 values the kernel exchanged) when given, else rnd(own result).
+    Returns dz_all [N, H2, 2048] in frame order with permuted gate columns (zero for frames >= len)."""
+    N, H2, _ = d_out.shape
+    L = torch.as_tensor(clamp_lens(lens, T))
+    dz_all = d_out.new_zeros((N, H2, 2048))
+    ar = torch.arange(N)
+    for d, wh in enumerate((wh_fw, wh_bw)):
+        dz_next = d_out.new_zeros((N, 1024))
+        dc_next = d_out.new_zeros((N, HID))
+        f_next = d_out.new_zeros((N, HID))
+        for s in range(T - 1, -1, -1):
+            act = s < L
+            t = torch.where(act, (L - 1 - s) if d else torch.full_like(L, s), torch.full_like(L, s))
+            i, j, f, o = gates[d, :, s].unbind(-2)
+            c = c_steps[d, :, s]
+            c_prev = c_steps[d, :, s - 1] if s > 0 else torch.zeros_like(c)
+            dh = d_out[ar, t, d * HID:(d + 1) * HID] + dz_next @ wh.t()
+            tc = torch.tanh(c)
+            dc = dc_next * f_next + dh * o * (1 - tc * tc)
+            dz = torch.cat([dc * j * i * (1 - i), dc * i * (1 - j * j), dc * c_prev * f * (1 - f), dh * tc * o * (1 - o)], -1)
+            m = act[:, None]                 # select, never multiply: saved gates of inactive steps are never written
+            zero = torch.zeros((), dtype=dz.dtype)
+            dz = torch.where(m, dz, zero)
+            dz_all[ar[act], t[act], d * 1024:(d + 1) * 1024] = to_perm(dz)[act]
+            if dz_in is not None:
+                dz_next = torch.where(m, from_perm(dz_in[ar, t, d * 1024:(d + 1) * 1024]), zero)
+            else:
+                dz_next = rnd(dz)
+            dc_next, f_next = torch.where(m, dc, zero), torch.where(m, f, zero)
+    return dict(dz=dz_all)
+
+
+def lstm_grads_stage(dz_all, a5, lstm_out, wx_fw, wx_bw, wh_fw, wh_bw):
+    """Weight / bias gradients of both LSTM cells ([768, 1024] = [W_x; W_h], TF column order) and d_a5 = sum_dir dz W_x^T.
+    h_prev of frame t is frame t-1 (forward) / t+1 (backward) of lstm_out, zero past the ends."""
+    out = {}
+    d_a5 = torch.zeros_like(a5)
+    d_a5_acc = torch.zeros_like(a5)
+    for d, (wx, wh) in enumerate(((wx_fw, wh_fw), (wx_bw, wh_bw))):
+        dz = from_perm(dz_all[..., d * 1024:(d + 1) * 1024])
+        ho = lstm_out[..., d * HID:(d + 1) * HID]
+        hp = torch.zeros_like(ho)
+        if d == 0:
+            hp[:, 1:] = ho[:, :-1]
+        else:
+            hp[:, :-1] = ho[:, 1:]
+        fn = lambda x, h, a, b, bias: x @ a + h @ b + bias
+        (dx, _, dwx, dwh, db), (ax, _, awx, awh, ab) = vjp_acc(fn, [a5, hp, wx, wh, torch.zeros(1024, dtype=a5.dtype)], dz)
+        key = "fw" if d == 0 else "bw"
+        out[key + "/weights"] = torch.cat([dwx, dwh], 0)
+        out[key + "/weights_acc"] = torch.cat([awx, awh], 0)
+        out[key + "/biases"] = db
+        out[key + "/biases_acc"] = ab
+        d_a5 = d_a5 + dx
+        d_a5_acc = d_a5_acc + ax
+    out["d_a5"] = d_a5
+    out["d_a5_acc"] = d_a5_acc
+    return out
+
+
+def conv_bwd(dy, x, w, padding=1):
+    """Data and weight gradients of a bias-free 3x3 SAME (padding 1) or 2x2 VALID (padding 0) conv, bias gradient = sum dy."""
+    (dx, dw), (ax, aw) = vjp_acc(lambda a, b: _conv(a, b, None, padding), [x, w], dy)
+    return dict(dx=dx, dx_acc=ax, dw=dw, dw_acc=aw, db=dy.sum((0, 1, 2)), db_acc=dy.abs().sum((0, 1, 2)))
+
+
+def conv5_bwd(d_a5, a4b, w):
+    """conv5 from d_a5 [N, H2, 512] (frames t < T): d_a4b, weight and bias gradients."""
+    T = a4b.shape[1] - 1
+    return conv_bwd(d_a5[:, :T, None, :], a4b, w, padding=0)
+
+
+def _bn_bwd_acc(dy_abs, x, xhat, invstd, gamma, red):
+    """Scale of dx = gamma*invstd*(dy - mean(dy) - xhat*mean(dy*xhat)) summed in absolute values.  The kernels evaluate it
+    as A*dy + B + C*x with f32 coefficients (backward_kernels.cu: bn_bwd_coef_kernel), where B and C*x cancel down to the
+    centred term; the 2^-8 share of |B| + |C*x| lets a 2^-16 * acc bound cover their f32 rounding (2^-24)."""
+    m1 = dy_abs.mean(red, keepdim=True)
+    m2 = (dy_abs * xhat.abs()).mean(red, keepdim=True)
+    mu = x.mean(red, keepdim=True)
+    cx = (gamma * invstd * invstd).abs() * m2 * (x.abs() + mu.abs())
+    return (gamma * invstd).abs() * (dy_abs + m1 + xhat.abs() * m2) + 2.0 ** -8 * cx
+
+
+def bn_relu_pool_bwd_stage(d_pooled, x_pre, bn, gamma, beta, eps, rnd=bf16):
+    """BN4_2 + ReLU + pool3 backward: x_pre [N, H2, 4, C] pre-BN, d_pooled [N, H2, 2, C], bn [4, C] = the workspace's
+    scale, shift, mean, invstd.  The pooled gradient goes to the FIRST position of the pair whose rnd(max(x*scale+shift, 0))
+    is the larger (the forward rounded each position before taking the max), and only where that max is > 0.  The BN itself
+    is differentiated in fp64 with the statistics recomputed from x_pre."""
+    sc, sh = bn[0], bn[1]
+    yq = windows12(rnd(torch.relu(x_pre * sc + sh)))
+    first = yq[..., 0] >= yq[..., 1]
+    pos = torch.maximum(yq[..., 0], yq[..., 1]) > 0
+    mask = torch.stack([first & pos, ~first & pos], -1).to(x_pre.dtype)       # [N, H2, 2, C, 2]
+
+    def fn(x, g, b):
+        mean = x.mean((0, 1, 2))
+        var = x.var((0, 1, 2), unbiased=False)
+        y = windows12((x - mean) / torch.sqrt(var + eps) * g + b)
+        return (y * mask).sum(-1)
+
+    dx, dg, db = vjp(fn, [x_pre, gamma, beta], d_pooled)
+    N, H2, W4, C = x_pre.shape
+    dyr = (d_pooled[..., None] * mask).permute(0, 1, 2, 4, 3).reshape(N, H2, W4, C)
+    invstd = 1.0 / torch.sqrt(x_pre.var((0, 1, 2), unbiased=False) + eps)
+    xhat = (x_pre - x_pre.mean((0, 1, 2))) * invstd
+    acc = _bn_bwd_acc(dyr.abs(), x_pre, xhat, invstd, gamma, (0, 1, 2))
+    return dict(dx=dx, dx_acc=acc, dgamma=dg, dbeta=db, dgamma_acc=(dyr * xhat).abs().sum((0, 1, 2)),
+                dbeta_acc=dyr.abs().sum((0, 1, 2)))
+
+
+def conv_bn_relu_bwd_stage(dy, x_pre, bn, gamma, beta, w, eps, mask=None, rnd=bf16):
+    """conv4_2 data gradient + conv4_1's ReLU mask + BN4_1 backward as one stage (the workspace's d_pre4a is overwritten in
+    place by the BN apply): x_pre [N, H2, 4, 512] pre-BN conv4_1, dy = d_pre4b.  The data gradient is stored as bf16 and
+    both BN passes read that (`rnd`).  The ReLU mask defaults to x*scale + shift > 0 on the workspace's f32 scale / shift
+    (what the forward applied)."""
+    if mask is None:
+        mask = (f32(x_pre * bn[0] + bn[1]) > 0).to(x_pre.dtype)
+    (g,), (g_abs,) = vjp_acc(lambda a: _conv(a, w), [torch.zeros_like(x_pre)], dy)
+    g = rnd(g) * mask
+
+    def fn(x, ga, b):
+        mean = x.mean((0, 1, 2))
+        var = x.var((0, 1, 2), unbiased=False)
+        return (x - mean) / torch.sqrt(var + eps) * ga + b
+
+    dx, dg, db = vjp(fn, [x_pre, gamma, beta], g)
+    # accumulation scale: the dgrad sum on absolute values plus one bf16 ulp of the stored gradient (its rounding may fall
+    # either way where the f32 and fp64 sums straddle a rounding boundary), then the BN backward on that
+    invstd = 1.0 / torch.sqrt(x_pre.var((0, 1, 2), unbiased=False) + eps)
+    xhat = (x_pre - x_pre.mean((0, 1, 2))) * invstd
+    g_acc = g_abs * mask + 2.0 ** 9 * g.abs()
+    acc = _bn_bwd_acc(g_acc, x_pre, xhat, invstd, gamma, (0, 1, 2))
+    return dict(dx=dx, dx_acc=acc, dgamma=dg, dbeta=db, dgamma_acc=(g_acc * xhat.abs()).sum((0, 1, 2)),
+                dbeta_acc=g_acc.sum((0, 1, 2)))
+
+
+def unpool_stage(d_pooled, pooled, am, win):
+    """Un-pool + ReLU backward: the pooled gradient where pooled > 0, routed to window position am (dy*2+dx for the 2x2
+    pool, dx for the 1x2 pool); zeros elsewhere.  Exact copies, no arithmetic."""
+    g = torch.where(pooled > 0, d_pooled, torch.zeros_like(d_pooled))
+    N, Hp, Wp, C = g.shape
+    sel = torch.stack([(am == k).to(g.dtype) for k in range(win)], -1) * g[..., None]
+    if win == 4:
+        return sel.reshape(N, Hp, Wp, C, 2, 2).permute(0, 1, 4, 2, 5, 3).reshape(N, 2 * Hp, 2 * Wp, C)
+    return sel.permute(0, 1, 2, 4, 3).reshape(N, Hp, 2 * Wp, C)
+
+
+def masked_colsum(d_pooled, pooled):
+    """Bias gradient of a conv followed by ReLU + max-pool: column sums of the pooled gradient where the pooled output > 0."""
+    g = torch.where(pooled > 0, d_pooled, torch.zeros_like(d_pooled))
+    return g.sum((0, 1, 2)), g.abs().sum((0, 1, 2))
+
+
+def conv1_wgrad_stage(d_a1, a1, am1, data, w):
+    """conv1 weight / bias gradient: d_a1 where a1 > 0, routed by am1 to its pre-pool position, against the f32 image."""
+    g = unpool_stage(d_a1, a1, am1, 4)
+    (dw,) = vjp(lambda b: _conv(data[..., None], b), [w], g)
+    (aw,) = vjp(lambda b: _conv(data.abs()[..., None], b), [w.abs()], g.abs())
+    return dict(dw=dw, dw_acc=aw, db=g.sum((0, 1, 2)), db_acc=g.abs().sum((0, 1, 2)))

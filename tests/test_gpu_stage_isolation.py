@@ -1,0 +1,374 @@
+"""Every forward and backward stage of the bf16 path in isolation, against an fp64 restatement of that one operation.
+
+Each stage's inputs are its OWN bf16 operands read back from the workspace (crnn_debug_tap / crnn_debug_tap_raw), so the
+only legitimate differences from tests/stage_refs.py are the order of the f32 accumulation and the final rounding.  Error
+does not compound from layer to layer, and a wrong element fails wherever it sits.  The whole-chain tests
+(test_gpu_parity.py, test_gpu_shapes.py, test_gpu_training.py) pin the composition; these pin the kernels.
+
+Per-element bounds (ratio = |gpu - ref| / bound must be <= 1):
+  bf16 outputs:  ulp_bf16(|ref|) + c * acc      (acc: the same operation on |inputs| and |weights|)
+  f32 outputs:   c * acc per element, and relative L2 <= 1e-4   (logits, weight / bias gradients)
+The recurrence, its isolated steps and the BPTT (bf16 h / dz exchange, approximate tanh / sigmoid, up to 63 serial steps)
+use c * max|ref| of the tensor instead of acc.  Those c, and the c of the f32 outputs, are about 4x the largest error
+measured over all shapes below on one H100 80GB HBM3 (SXM): the whole recurrence now holds lstm_out to 6.5e-3 of its max,
+where the whole-chain test allows 9e-2.  The bf16 stages measured at most 0.5 ulp, the final rounding alone, so their
+bound stays at one ulp.  Every run appends the measured maxima to build/stage_isolation_report.jsonl, one line per stage
+and shape.
+
+Ties: conv1 picks the first maximum on the f32 accumulators, the other pooled training epilogues on the bf16-rounded
+values, and the pool3 backward re-derives the pair maximum from bf16-rounded BN outputs; the arg-max checks accept any
+position within the bound of the maximum, and the pool3 reference routes by the same bf16 comparison."""
+import json
+import os
+import sys
+import time
+
+import numpy as np
+import pytest
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import stage_refs as S  # noqa: E402
+
+pytestmark = pytest.mark.gpu
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+DEV = "cuda:0"
+FW, BW = "logits/bidirectional_rnn/fw/lstm_cell", "logits/bidirectional_rnn/bw/lstm_cell"
+_REPORT_RUN = None          # start time of this session's report (the report file is truncated once per session)
+
+# stage -> (ulps of |ref|, c); c multiplies acc (bf16 / f32 outputs) or max|ref| (recurrence, BPTT)
+STAGE_BOUNDS = {
+    "conv1": (1, 2 ** -15), "conv2": (1, 2 ** -16), "conv3_1": (1, 2 ** -16), "conv3_2": (1, 2 ** -16),
+    "a4a_pre": (1, 2 ** -16), "conv4_1": (1, 2 ** -16), "a4b_pre": (1, 2 ** -16), "conv4_2": (1, 2 ** -16),
+    "conv5": (1, 2 ** -16), "xproj": (1, 2 ** -16),
+    "lstm_out": (1, 6.5e-3), "step_gates": (1, 4e-3), "step_c": (0, 3e-5), "step_h": (1, 4e-3),
+    "logits": (0, 1e-6),
+    "d_lstm_out": (1, 2 ** -16), "dz_all": (1, 7e-3), "d_a5": (1, 2 ** -16), "d_a4b": (1, 2 ** -16),
+    "d_pre4b": (1, 2 ** -16), "d_pre4a": (1, 2 ** -16), "d_a3p": (1, 2 ** -16), "d_pre31": (1, 2 ** -16),
+    "d_a2": (1, 2 ** -16), "d_a1": (1, 2 ** -16),
+    "wgrad": (0, 2.5e-5), "bn41_affine": (0, 2.5e-5),
+    # BatchNorm statistics: the f64 sums hold f32 partial sums over 32-row groups (c times sum|x| resp. sum x^2; measured
+    # up to 1.9e-7); the f32 mean / invstd / scale / shift are bounded by c times their error scales from
+    # stage_refs.bn_stats_stage (measured up to 2.2e-7)
+    "bn_sums": (0, 1e-6), "bn_coef": (0, 3e-6),
+}
+# relative L2 limit of the f32 outputs.  conv4_1's gamma / beta gradients are sums over the bf16-STORED conv4_2 data
+# gradient: where the f32 and the fp64 dgrad straddle a bf16 rounding boundary the stored value differs by one ulp, which
+# happens to a sizeable share of the elements and leaves up to 3.1e-4 (measured) in these cancelling sums.
+L2_LIMIT = {"bn41_affine": 1.2e-3}
+
+SHAPES = [
+    pytest.param(2, 256, [256, 201], id="N2_W256"),
+    pytest.param(3, 160, [160, 8, 97], id="N3_W160"),
+    pytest.param(5, 80, [80, 4, 8, 57, 33], id="N5_W80"),
+    pytest.param(3, 100, [100, 4, 61], id="N3_W100"),
+    pytest.param(130, 40, "cycle", id="N130_W40"),
+    pytest.param(5, 24, [24, 4, 8, 12, 20], id="N5_W24"),
+]
+
+
+def _widths(N, W, widths):
+    if widths == "cycle":                                  # lengths 0, 1, T and in between, over two 128-row tiles
+        return [[W, 4, 8, 12, 20, 28, 36][i % 7] for i in range(N)]
+    return widths
+
+
+def ulp_bf16(x):
+    a = np.maximum(np.abs(x), 2.0 ** -126)
+    return 2.0 ** (np.floor(np.log2(a)) - 7)
+
+
+class Checker:
+    def __init__(self, case):
+        self.case = case
+        self.fail = []
+        self.rows = []
+
+    def _record(self, stage, ratio, **kv):
+        self.rows.append(dict(case=self.case, stage=stage, max_ratio=float(ratio), **kv))
+        if not ratio <= 1.0:
+            self.fail.append(f"{stage}: max |gpu-ref|/bound = {ratio:.3g} {kv}")
+
+    def close(self, stage, gpu, ref, acc, key=None, mask=None):
+        """bf16 (ulps > 0) or f32 (ulps == 0) output against the fp64 reference, per element."""
+        ulps, c = STAGE_BOUNDS[key or stage]
+        g, r = np.asarray(gpu, np.float64), np.asarray(ref, np.float64)
+        a = np.broadcast_to(np.asarray(acc, np.float64), r.shape)
+        if mask is not None:
+            g, r, a = g[mask], r[mask], a[mask]
+        if r.size == 0:
+            return
+        err = np.abs(g - r)
+        bound = ulps * ulp_bf16(r) + c * a if ulps else c * a + 1e-30
+        ratio = err / bound
+        i = int(np.argmax(ratio))
+        kv = dict(max_abs_err=float(err.max()), worst_gpu=float(g.flat[i]), worst_ref=float(r.flat[i]),
+                  worst_acc=float(a.flat[i]), ulps=ulps, c=c)
+        if not ulps:
+            l2 = float(np.linalg.norm(g - r) / max(np.linalg.norm(r), 1e-30))
+            kv["rel_l2"] = l2
+            lim = L2_LIMIT.get(key or stage, 1e-4)
+            if l2 > lim:
+                self.fail.append(f"{stage}: relative L2 {l2:.3g} > {lim:g}")
+        self._record(stage, float(ratio.max()), **kv)
+
+    def close_scaled(self, stage, gpu, ref, mask=None):
+        """Recurrence / BPTT: bound ulps * ulp(|ref|) + c * max|ref|."""
+        r = np.asarray(ref, np.float64)
+        self.close(stage, gpu, ref, np.abs(r[mask] if mask is not None else r).max(), mask=mask)
+
+    def exact(self, stage, gpu, ref):
+        g, r = np.asarray(gpu), np.asarray(ref)
+        bad = int((g != r).sum())
+        self._record(stage, 0.0 if bad == 0 else float("inf"), mismatches=bad)
+
+    def report(self):
+        """Rows of this test session only: the first report of a session truncates the file, every row carries the
+        session's start time."""
+        global _REPORT_RUN
+        os.makedirs(os.path.join(ROOT, "build"), exist_ok=True)
+        mode = "a" if _REPORT_RUN else "w"
+        if not _REPORT_RUN:
+            _REPORT_RUN = time.strftime("%Y-%m-%dT%H:%M:%S")
+        with open(os.path.join(ROOT, "build", "stage_isolation_report.jsonl"), mode) as f:
+            for row in self.rows:
+                f.write(json.dumps(dict(run=_REPORT_RUN, **row)) + "\n")
+
+    def assert_ok(self):
+        self.report()
+        assert not self.fail, "\n".join(self.fail)
+
+
+def argmax_check(ck, stage, am, pre, pooled, c):
+    """Pool window bytes: in range; where the pooled output is > 0 and the two largest fp64 window values are separated by
+    more than the bf16 bound, the byte is the first fp64 arg-max; otherwise it points at a value within the bound of the max."""
+    am = np.asarray(am).astype(np.int64)
+    win = pre.shape[-1]
+    bad_range = int((am >= win).sum())
+    srt = np.sort(pre, axis=-1)
+    mx, second = srt[..., -1], srt[..., -2]
+    bound = ulp_bf16(mx) + c
+    first = np.argmax(pre, axis=-1)
+    chosen = np.take_along_axis(pre, np.minimum(am, win - 1)[..., None], -1)[..., 0]
+    live = np.asarray(pooled) > 0
+    clear = live & (mx - second > bound)
+    wrong_clear = int((clear & (am != first)).sum())
+    wrong_near = int((live & ~clear & (mx - chosen > bound)).sum())
+    ck._record(stage, 0.0 if bad_range + wrong_clear + wrong_near == 0 else float("inf"), out_of_range=bad_range,
+               wrong_clear=wrong_clear, wrong_near_tie=wrong_near, live=int(live.sum()))
+
+
+def _setup(N, W, widths, seed=5):
+    from lstm_ctc_ocr_b200 import engine
+    from oracle import crnn_oracle as O
+    pn = O.randomize_params(O.init_params(3, dtype=np.float32, logits_scale=10.0))
+    data, lab, ll, tsl = O.synth_batch(N, W, seed=seed, widths=_widths(N, W, widths), min_len=1, max_len=4)
+    m = engine.CrnnModel(device=DEV)
+    m.load_params(pn)
+    return m, pn, data, tsl
+
+
+def _run_stage_checks(case, N, W, widths):
+    m, pn, data, tsl = _setup(N, W, widths)
+    T, H2 = W // 4 - 1, W // 4
+    t = lambda a: torch.tensor(a, device=DEV)
+    m.set_training(True)
+    d_data, d_tsl = t(data), t(tsl)
+    logits = m.forward(d_data, d_tsl)
+    gen = torch.Generator(device="cpu").manual_seed(17)
+    dlogits = (torch.randn((T, N, 64), generator=gen) * 0.05).float()
+    torch.cuda.synchronize()
+    tap = lambda k: m.tap(k, N, W).double().cpu()
+    raw = lambda k: m.tap_raw(k, N, W).cpu()
+    G = {k: tap(k) for k in ("conv1", "conv2", "conv3_1", "conv3_2", "a4a_pre", "conv4_1", "a4b_pre", "conv4_2", "conv5",
+                             "xproj", "lstm_out", "gates")}
+    R = {k: raw(k) for k in ("bn", "stats", "am1", "am2", "am3", "csave")}
+    logits = logits.double().cpu()
+    m.backward(d_data, d_tsl, dlogits.to(DEV))
+    torch.cuda.synchronize()
+    for k in ("dl_rows", "d_lstm_out", "dz_all", "d_a5", "d_a4b", "d_pre4b", "d_pre4a", "d_a3p", "d_pre32", "d_pre31", "d_a2",
+              "d_pre2", "d_a1"):
+        G[k] = tap(k)
+    grad = {k: m.grad_tensor(k).double().cpu() for k in m.table}
+    P = {k: torch.as_tensor(np.asarray(v, np.float64)) for k, v in pn.items()}
+    Wb = {k: S.bf16(v) for k, v in P.items() if k.endswith("weights")}
+    eps = float(np.float32(1e-3))
+    L = S.clamp_lens(tsl, T)
+    ck = Checker(case)
+
+    # ---------------------------------------------------------------- forward
+    x = torch.as_tensor(data, dtype=torch.float64)
+    r = S.conv1_stage(x, P["conv1/weights"], P["conv1/biases"])
+    ck.close("conv1", G["conv1"], r["out"], r["acc"])
+    argmax_check(ck, "am1", R["am1"], S.windows22(r["pre"]).numpy(), G["conv1"], 2 ** -15 * r["acc"].numpy())
+    r = S.conv_relu_pool22_stage(G["conv1"], Wb["conv2/weights"], P["conv2/biases"])
+    ck.close("conv2", G["conv2"], r["out"], r["acc"])
+    argmax_check(ck, "am2", R["am2"], S.windows22(r["pre"]).numpy(), G["conv2"], 2 ** -16 * r["acc"].numpy())
+    r = S.conv_relu_stage(G["conv2"], Wb["conv3_1/weights"], P["conv3_1/biases"])
+    ck.close("conv3_1", G["conv3_1"], r["out"], r["acc"])
+    r = S.conv_relu_pool12_stage(G["conv3_1"], Wb["conv3_2/weights"], P["conv3_2/biases"])
+    ck.close("conv3_2", G["conv3_2"], r["out"], r["acc"])
+    argmax_check(ck, "am3", R["am3"], S.windows12(r["pre"]).numpy(), G["conv3_2"], 2 ** -16 * r["acc"].numpy())
+    bn = R["bn"].double()
+    for li, (name, src, pre, out) in enumerate((("conv4_1", "conv3_2", "a4a_pre", "conv4_1"),
+                                                ("conv4_2", "conv4_1", "a4b_pre", "conv4_2"))):
+        r = S.conv_bias_stage(G[src], Wb[f"{name}/weights"], P[f"{name}/biases"])
+        ck.close(pre, G[pre], r["out"], r["acc"])
+        st = S.bn_stats_stage(G[pre], P[f"{name}/{name}/gamma"], P[f"{name}/{name}/beta"], eps)
+        stats = R["stats"][li]
+        ck.close(f"{name}_stats", stats[0], st["sum"], st["sum_acc"], key="bn_sums")
+        ck.close(f"{name}_stats_sq", stats[1], st["sumsq"], st["sumsq"], key="bn_sums")
+        for j, k in enumerate(("scale", "shift", "mean", "invstd")):        # f32 roundings of f64 values of those sums
+            ck.close(f"{name}_bn_{k}", bn[li, j], st[k], st["acc"][k], key="bn_coef")
+        if li == 0:
+            r = S.bn_apply_relu_stage(G[pre], bn[0, 0], bn[0, 1])
+        else:
+            r = S.bn_apply_relu_pool_stage(G[pre], bn[1, 0], bn[1, 1])
+        ck.close(out, G[out], r["out"], r["acc"] * 2 ** -8)        # one f32 fma, then the bf16 rounding: <= 1 ulp
+    r = S.conv5_stage(G["conv4_2"], Wb["conv5/weights"], P["conv5/biases"])
+    ck.close("conv5", G["conv5"][:, :T], r["out"], r["acc"])
+    r = S.xproj_stage(G["conv5"], Wb[FW + "/weights"][:512], Wb[BW + "/weights"][:512], P[FW + "/biases"], P[BW + "/biases"],
+                      tsl, T)
+    ck.close("xproj", G["xproj"], r["out"], r["acc"])
+    wh = (Wb[FW + "/weights"][512:], Wb[BW + "/weights"][512:])
+    r = S.recurrence_stage(G["xproj"], wh[0], wh[1], tsl, T)
+    valid = np.zeros((N, H2), bool)
+    for n in range(N):
+        valid[n, :L[n]] = True
+    ck.exact("lstm_out_past_len_zero", G["lstm_out"].numpy()[~valid], 0.0)
+    ck.close_scaled("lstm_out", G["lstm_out"], r["out"], mask=np.broadcast_to(valid[..., None], r["out"].shape))
+    gates = S.unpack_gates(G["gates"], N)
+    csave = S.unpack_csave(R["csave"].double(), N)
+    iso = S.recurrence_steps_isolated(G["xproj"], wh[0], wh[1], G["lstm_out"], csave, tsl, T)
+    act = (torch.arange(T)[None, :] < torch.as_tensor(L)[:, None]).numpy()
+    act2 = np.broadcast_to(act[None], (2, N, T))
+    ck.close_scaled("step_gates", gates.numpy()[act2], iso["gates"].numpy()[act2])
+    ck.close_scaled("step_c", csave.numpy()[act2], iso["c"].numpy()[act2])
+    h_gpu = torch.zeros_like(iso["h"])
+    for d in range(2):
+        for n in range(N):
+            for s in range(L[n]):
+                h_gpu[d, n, s] = G["lstm_out"][n, (L[n] - 1 - s) if d else s, d * 256:(d + 1) * 256]
+    ck.close_scaled("step_h", h_gpu.numpy()[act2], iso["h"].numpy()[act2])
+    r = S.logits_stage(G["lstm_out"], Wb["logits/weights"], P["logits/biases"], T)
+    ck.close("logits", logits, r["out"], r["acc"])
+    past = np.zeros((T, N), bool)
+    for n in range(N):
+        past[L[n]:, n] = True
+    ck.exact("logits_past_len_bias", logits.numpy()[past], np.broadcast_to(np.float32(pn["logits/biases"]), (int(past.sum()), 64)))
+
+    # ---------------------------------------------------------------- backward
+    dl = S.dl_rows_stage(dlogits.double(), H2)
+    ck.exact("dl_rows", G["dl_rows"].numpy(), S.bf16(dl["dl_rows"]).numpy())
+    ck.close("logits/biases", grad["logits/biases"], dl["dbias"], dl["dbias_acc"], key="wgrad")
+    r = S.logits_bwd(G["lstm_out"], G["dl_rows"], Wb["logits/weights"])
+    ck.close("logits/weights", grad["logits/weights"], r["dw"], r["dw_acc"], key="wgrad")
+    ck.close("d_lstm_out", G["d_lstm_out"], r["d_lstm_out"], r["d_lstm_out_acc"])
+    r = S.bptt_stage(G["d_lstm_out"], gates, csave, wh[0], wh[1], tsl, T, dz_in=G["dz_all"])
+    ck.exact("dz_all_past_len_zero", G["dz_all"].numpy()[~valid], 0.0)
+    ck.close_scaled("dz_all", G["dz_all"], r["dz"], mask=np.broadcast_to(valid[..., None], r["dz"].shape))
+    r = S.lstm_grads_stage(G["dz_all"], G["conv5"], G["lstm_out"], Wb[FW + "/weights"][:512], Wb[BW + "/weights"][:512],
+                           wh[0], wh[1])
+    for d, scope in (("fw", FW), ("bw", BW)):
+        ck.close(scope + "/weights", grad[scope + "/weights"], r[d + "/weights"], r[d + "/weights_acc"], key="wgrad")
+        ck.close(scope + "/biases", grad[scope + "/biases"], r[d + "/biases"], r[d + "/biases_acc"], key="wgrad")
+    ck.close("d_a5", G["d_a5"], r["d_a5"], r["d_a5_acc"])
+    r = S.conv5_bwd(G["d_a5"], G["conv4_2"], Wb["conv5/weights"])
+    ck.close("conv5/weights", grad["conv5/weights"], r["dw"], r["dw_acc"], key="wgrad")
+    ck.close("conv5/biases", grad["conv5/biases"], r["db"], r["db_acc"], key="wgrad")
+    ck.close("d_a4b", G["d_a4b"], r["dx"], r["dx_acc"])
+    r = S.bn_relu_pool_bwd_stage(G["d_a4b"], G["a4b_pre"], bn[1], P["conv4_2/conv4_2/gamma"], P["conv4_2/conv4_2/beta"], eps)
+    ck.close("d_pre4b", G["d_pre4b"], r["dx"], r["dx_acc"])
+    ck.close("conv4_2/gamma", grad["conv4_2/conv4_2/gamma"], r["dgamma"], r["dgamma_acc"], key="wgrad")
+    ck.close("conv4_2/beta", grad["conv4_2/conv4_2/beta"], r["dbeta"], r["dbeta_acc"], key="wgrad")
+    r = S.conv_bwd(G["d_pre4b"], G["conv4_1"], Wb["conv4_2/weights"])
+    ck.close("conv4_2/weights", grad["conv4_2/weights"], r["dw"], r["dw_acc"], key="wgrad")
+    ck.exact("conv4_2/biases_zero", grad["conv4_2/biases"].numpy(), 0.0)
+    r = S.conv_bn_relu_bwd_stage(G["d_pre4b"], G["a4a_pre"], bn[0], P["conv4_1/conv4_1/gamma"], P["conv4_1/conv4_1/beta"],
+                                 Wb["conv4_2/weights"], eps)
+    ck.close("d_pre4a", G["d_pre4a"], r["dx"], r["dx_acc"])
+    ck.close("conv4_1/gamma", grad["conv4_1/conv4_1/gamma"], r["dgamma"], r["dgamma_acc"], key="bn41_affine")
+    ck.close("conv4_1/beta", grad["conv4_1/conv4_1/beta"], r["dbeta"], r["dbeta_acc"], key="bn41_affine")
+    r = S.conv_bwd(G["d_pre4a"], G["conv3_2"], Wb["conv4_1/weights"])
+    ck.close("conv4_1/weights", grad["conv4_1/weights"], r["dw"], r["dw_acc"], key="wgrad")
+    ck.exact("conv4_1/biases_zero", grad["conv4_1/biases"].numpy(), 0.0)
+    ck.close("d_a3p", G["d_a3p"], r["dx"], r["dx_acc"])
+    ck.exact("d_pre32", G["d_pre32"].numpy(), S.unpool_stage(G["d_a3p"], G["conv3_2"], R["am3"].long(), 2).numpy())
+    db, dba = S.masked_colsum(G["d_a3p"], G["conv3_2"])
+    ck.close("conv3_2/biases", grad["conv3_2/biases"], db, dba, key="wgrad")
+    r = S.conv_bwd(G["d_pre32"], G["conv3_1"], Wb["conv3_2/weights"])
+    ck.close("conv3_2/weights", grad["conv3_2/weights"], r["dw"], r["dw_acc"], key="wgrad")
+    ck.close("d_pre31", G["d_pre31"], r["dx"] * (G["conv3_1"] > 0), r["dx_acc"])
+    r = S.conv_bwd(G["d_pre31"], G["conv2"], Wb["conv3_1/weights"])
+    ck.close("conv3_1/weights", grad["conv3_1/weights"], r["dw"], r["dw_acc"], key="wgrad")
+    ck.close("conv3_1/biases", grad["conv3_1/biases"], r["db"], r["db_acc"], key="wgrad")
+    ck.close("d_a2", G["d_a2"], r["dx"], r["dx_acc"])
+    ck.exact("d_pre2", G["d_pre2"].numpy(), S.unpool_stage(G["d_a2"], G["conv2"], R["am2"].long(), 4).numpy())
+    db, dba = S.masked_colsum(G["d_a2"], G["conv2"])
+    ck.close("conv2/biases", grad["conv2/biases"], db, dba, key="wgrad")
+    r = S.conv_bwd(G["d_pre2"], G["conv1"], Wb["conv2/weights"])
+    ck.close("conv2/weights", grad["conv2/weights"], r["dw"], r["dw_acc"], key="wgrad")
+    ck.close("d_a1", G["d_a1"], r["dx"], r["dx_acc"])
+    r = S.conv1_wgrad_stage(G["d_a1"], G["conv1"], R["am1"].long(), x, P["conv1/weights"])
+    ck.close("conv1/weights", grad["conv1/weights"], r["dw"], r["dw_acc"], key="wgrad")
+    ck.close("conv1/biases", grad["conv1/biases"], r["db"], r["db_acc"], key="wgrad")
+    ck.assert_ok()
+    return m, G
+
+
+@pytest.mark.parametrize("N,W,widths", SHAPES)
+def test_every_stage_against_fp64_on_its_own_inputs(N, W, widths, request):
+    _run_stage_checks(request.node.callspec.id, N, W, widths)
+
+
+ALT_SWITCHES = [
+    pytest.param({"CRNN_CONV1": "simt", "CRNN_CONV2": "pos"}, id="conv1_simt_conv2_pos"),
+    pytest.param({"CRNN_CONV2_DGRAD": "old", "CRNN_CONV2_WGRAD": "old", "CRNN_CONV1_WGRAD": "simt"}, id="old_conv_grads"),
+    pytest.param({"CRNN_BPTT": "ring", "CRNN_RELU_FUSE": "0", "CRNN_BN_FUSE": "0"}, id="bptt_ring_unfused"),
+]
+
+
+@pytest.mark.parametrize("env", ALT_SWITCHES)
+def test_alternative_kernels_against_the_same_references(env, monkeypatch, request):
+    """The kernels kept selectable by environment switches (read when a model is created), same checks at 3 x 100."""
+    for k, v in env.items():
+        monkeypatch.setenv(k, v)
+    _run_stage_checks("N3_W100/" + request.node.callspec.id, 3, 100, [100, 4, 61])
+
+
+@pytest.mark.parametrize("N,W,widths", [SHAPES[0], SHAPES[3], SHAPES[4]])
+def test_training_forward_taps_match_inference(N, W, widths):
+    """conv1 .. conv3_2 come before any atomics: the training variants (arg-max bytes) must write bit-identical values.
+    conv4_1 and conv4_2 may differ by 1 bf16 ulp (order of the f64 atomics of the BatchNorm statistics).  The per-stage
+    checks above run on training-mode plans; from conv5 on the kernels are the same in both modes, and the inference-mode
+    outputs past conv4_2 are pinned by the whole-chain tests only."""
+    m, pn, data, tsl = _setup(N, W, widths)
+    t = lambda a: torch.tensor(a, device=DEV)
+    names = ("conv1", "conv2", "conv3_1", "conv3_2", "conv4_1", "conv4_2")
+    m.forward(t(data), t(tsl))
+    inf = {k: m.tap(k, N, W).cpu().numpy() for k in names}
+    m.set_training(True)
+    m.forward(t(data), t(tsl))
+    trn = {k: m.tap(k, N, W).cpu().numpy() for k in names}
+    for k in names[:4]:
+        assert np.array_equal(inf[k], trn[k]), k
+    for k in names[4:]:
+        d = np.abs(inf[k] - trn[k])
+        assert (d <= ulp_bf16(np.maximum(np.abs(inf[k]), np.abs(trn[k])))).all(), k
+
+
+@pytest.mark.parametrize("N,W,widths", [SHAPES[0], pytest.param(8, 64, [64, 4, 8, 33, 64, 61, 12, 40], id="N8_W64")])
+def test_chunked_front_end_is_bit_identical(N, W, widths):
+    """forward_host(chunks=4) runs conv1 .. conv3_2 per image range (the img0 coordinate of conv1's output map): the front-end
+    taps must equal the one-range forward bit for bit."""
+    m, pn, data, tsl = _setup(N, W, widths)
+    t = lambda a: torch.tensor(a, device=DEV)
+    names = ("conv1", "conv2", "conv3_1", "conv3_2")
+    m.forward(t(data), t(tsl))
+    one = {k: m.tap(k, N, W).cpu().numpy() for k in names}
+    host = torch.empty((N, W, 32), dtype=torch.float32, pin_memory=True)
+    host.copy_(torch.as_tensor(data))
+    m.forward_host(host.numpy(), t(tsl), chunks=4)
+    torch.cuda.synchronize()
+    for k in names:
+        assert np.array_equal(m.tap(k, N, W).cpu().numpy(), one[k]), k

@@ -6,7 +6,7 @@ import sys
 ROOT = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(ROOT, "lstm_ctc_ocr_b200", "csrc")
 OUT = os.path.join(ROOT, "lstm_ctc_ocr_b200", "libcrnnctc.so")
-SOURCES = ["ctc.cu", "kernels.cu", "model.cu", "backward_kernels.cu", "backward.cu", "forward_x3.cu", "peer.cu", "beam.cpp"]
+SOURCES = ["ctc.cu", "kernels.cu", "model.cu", "backward_kernels.cu", "backward.cu", "forward_x3.cu", "peer.cu", "beam.cpp", "beam.cu"]
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-I/usr/local/cuda/include"]
 
@@ -27,7 +27,7 @@ def build(force=False, verbose=False):
     procs = []
     os.makedirs(os.path.join(ROOT, "build"), exist_ok=True)
     for src in SOURCES:
-        obj = os.path.join(ROOT, "build", os.path.splitext(src)[0] + ".o")
+        obj = os.path.join(ROOT, "build", src + ".o")        # beam.cpp and beam.cu both exist
         cmd = [nvcc, "-c", os.path.join(CSRC, src), "-o", obj] + FLAGS + (["-Xptxas", "-v"] if verbose else [])
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
         objs.append(obj)

@@ -76,6 +76,20 @@ int crnn_ctc_beam_search(const float* logits_host, const int* input_len_host, in
                          int merge_repeated, int strip, int* out_host, int* out_len_host, float* neg_log_prob_host,
                          int num_threads);
 
+/* The same beam-search decode on the DEVICE: labellings identical to crnn_ctc_beam_search on the same logits (the
+ * algorithm, its visit order and its tie rules are those of the host decoder; the double exp / log are the device's).  Same
+ * layouts and meanings, but every pointer is a DEVICE pointer: logits [T,N,C] f32, input_len [N] i32, out [N,T] i32 zero
+ * padded, out_len [N] i32, neg_log_prob [N] f32 or NULL.  Asynchronous on `stream`; no host synchronisation and no
+ * allocation inside the call.  input_len is clamped to [0,T] (it cannot be checked without a sync): a negative length
+ * decodes as 0 frames, one above T as T frames.  Supported: 2 <= C <= 64, 1 <= beam_width <= 128, else CRNN_UNSUPPORTED.
+ * The workspace (16-byte aligned, size from crnn_ctc_beam_workspace_size, CRNN_WORKSPACE_TOO_SMALL when short) holds each
+ * utterance's prefix tree: 64 bytes per entry, 1 + beam_width*(T+C) entries per utterance, a bound that depends on the
+ * shapes alone (about 0.83 GB at T = 63, N = 1024, C = 64, width 100). */
+int crnn_ctc_beam_workspace_size(int T, int N, int C, int beam_width, size_t* bytes);
+int crnn_ctc_beam_search_device(const float* logits, const int* input_len, int T, int N, int C, int beam_width,
+                                int merge_repeated, int strip, int* out, int* out_len, float* neg_log_prob,
+                                void* workspace, size_t workspace_bytes, crnn_stream_t stream);
+
 /* 1 when `host_ptr` lies in page-locked (cudaHostAlloc / cudaHostRegister) memory, else 0.  The Python feed path uses it to
  * decide whether a fed numpy batch can be DMA'd in place (crnn_forward_host) or has to be staged. */
 int crnn_host_is_pinned(const void* host_ptr);

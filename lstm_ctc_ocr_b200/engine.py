@@ -280,6 +280,48 @@ def ctc_beam_search(logits, input_len, beam_width=100, merge_repeated=True, stri
     return out, out_len, nlp
 
 
+_beam_ws = {}        # device -> ((T, N, C, beam_width), workspace tensor): the last shape's workspace, reused call to call
+
+
+def beam_workspace_bytes(T, N, C, beam_width):
+    """Bytes of device workspace crnn_ctc_beam_search_device needs for this shape (no CUDA call)."""
+    nbytes = _lib.c_size_t()
+    check(_lib.load().crnn_ctc_beam_workspace_size(int(T), int(N), int(C), int(beam_width), nbytes))
+    return int(nbytes.value)
+
+
+def ctc_beam_search_device(logits, input_len, beam_width=100, merge_repeated=True, strip=0):
+    """The same decoder as ctc_beam_search (labellings identical to the host's), run on the GPU from device logits: one warp
+    per utterance, asynchronous on the current stream, no host sync.  logits [T,N,C] f32 cuda (2 <= C <= 64), input_len [N]
+    i32 cuda (clamped to [0, T]), 1 <= beam_width <= 128.  Returns device (out [N,T] i32 zero padded, out_len [N] i32,
+    neg_log_prob [N] f32).  There is no host fallback: CPU tensors or an unsupported shape raise CrnnError."""
+    if not (torch.is_tensor(logits) and logits.is_cuda and torch.is_tensor(input_len) and input_len.is_cuda):
+        raise CrnnError("ctc_beam_search_device needs CUDA tensors; ctc_beam_search is the host decoder")
+    if logits.dtype != torch.float32 or logits.dim() != 3 or input_len.dtype != torch.int32:
+        raise CrnnError("ctc_beam_search_device: logits must be [T,N,C] f32 and input_len i32")
+    lib = _lib.load()
+    logits = logits.contiguous()
+    input_len = input_len.contiguous()
+    T, N, C = logits.shape
+    if input_len.numel() != N:
+        raise CrnnError("ctc_beam_search_device: input_len must hold one entry per utterance")
+    key = (T, N, C, int(beam_width))
+    dev = logits.device
+    cached = _beam_ws.get(dev)
+    if cached is None or cached[0] != key:
+        _beam_ws.pop(dev, None)
+        nbytes = beam_workspace_bytes(T, N, C, beam_width)
+        cached = _beam_ws[dev] = (key, torch.empty(nbytes, dtype=torch.uint8, device=dev))
+    ws = cached[1]
+    out = torch.empty((N, T), dtype=torch.int32, device=dev)
+    out_len = torch.empty(N, dtype=torch.int32, device=dev)
+    nlp = torch.empty(N, dtype=torch.float32, device=dev)
+    check(lib.crnn_ctc_beam_search_device(logits.data_ptr(), input_len.data_ptr(), T, N, C, int(beam_width), 1 if merge_repeated else 0,
+                                          int(strip), out.data_ptr(), out_len.data_ptr(), nlp.data_ptr(), ws.data_ptr(), ws.numel(),
+                                          _stream()))
+    return out, out_len, nlp
+
+
 def dense_decoded(out, out_len):
     """sparse_tensor_to_dense(default 0) shape [N, max_len] (network.py:657); one D2H sync."""
     m = int(out_len.max().item()) if out_len.numel() else 0

@@ -34,7 +34,7 @@ _DEFAULTS = {
     "CHARSET": _CHARSET, "NCLASSES": len(_CHARSET) + 2,        # + CTC blank (0) + decoder blank (63)
     "FONT": "fonts/Ubuntu-M.ttf",
     # not in the reference: which decoder `dense_decoded` runs -- "greedy" (GPU kernel, the hot path) or "beam" (the reference's
-    # ctc_beam_search_decoder semantics, host side, network.py:656)
+    # ctc_beam_search_decoder semantics, network.py:656; decoded on the GPU, width BEAM_WIDTH <= 128)
     "DECODER": "greedy", "BEAM_WIDTH": 100,
     "NET_NAME": "lstm", "EXP_DIR": "default", "LOG_DIR": "default", "RNG_SEED": 3,
     "TRAIN": {

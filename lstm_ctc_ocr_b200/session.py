@@ -366,10 +366,10 @@ class Session(object):
             elif k == "dense_decoded":
                 from .lib.lstm.config import cfg
                 if str(cfg.get("DECODER", "greedy")) == "beam":
-                    # the reference's own decoder (network.py:656): host-side prefix beam search, width 100, blank 63
-                    o, ol, _ = engine.ctc_beam_search(logits, tsl, beam_width=int(cfg.get("BEAM_WIDTH", 100)), merge_repeated=True)
-                    m_ = int(ol.max()) if ol.size else 0
-                    v = np.ascontiguousarray(o[:, :m_])
+                    # the reference's own decoder (network.py:656): prefix beam search, width 100, blank 63, on the device
+                    o, ol, _ = engine.ctc_beam_search_device(logits, d_tsl, beam_width=int(cfg.get("BEAM_WIDTH", 100)),
+                                                             merge_repeated=True)
+                    v = engine.dense_decoded(o, ol).cpu().numpy()
                 else:
                     o, ol = engine.ctc_greedy(logits, d_tsl)
                     v = engine.dense_decoded(o, ol).cpu().numpy()

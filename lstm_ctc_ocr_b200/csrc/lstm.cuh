@@ -5,8 +5,10 @@
 // i,j,f,o = split(z); c = sigma(f+1) c + sigma(i) tanh(j); h = sigma(o) tanh(c); zero output past sequence_length.
 //
 // Two generations live in this file:
-//   lstm_mc_kernel<CS, MODE, EW>   (further down; the default, MODE 2 = "ms") -- h exchanged as 8 KB slices that land directly in
-//                                  every CTA's no-swizzle A operand, signalled through mbarriers; no cluster barrier per step
+//   lstm_mc_kernel<CS, MODE, EW>   (further down; the default, MODE 2 = "ms") -- two independent 64-row half pipelines per CTA;
+//                                  the cell runs on the wgmma accumulator fragments, h is exchanged as 4 KB half slices that
+//                                  land directly in every CTA's no-swizzle A operand, signalled through mbarriers; no cluster
+//                                  barrier per step
 //   lstm_persistent_kernel<CS>     (first, below; CRNN_LSTM_IMPL=persistent) -- h through global memory, a 64 KB TMA fetch per CTA,
 //                                  fence.proxy.async and one barrier.cluster per step; those per-step costs are the
 //                                  reason the second generation exists (see the comment above lstm_mc_kernel)
@@ -44,15 +46,16 @@ struct Params {
   __nv_bfloat16* gates;         // post-activation gates i,j,f,o, coalesced per batch tile: layout in common.cuh (lstm_gate_off)
   float* csave;                 // cell state after the step (lstm_c_off)
   int swap_ls;                  // debug (CRNN_LSTM_SWAPLS=1): exchange the LBO/SBO fields of the no-swizzle A descriptor
-  long long* trace;             // debug (CRNN_LSTM_TRACE=1): clock64 stamps of CTAs 0 and 5, steps 8..11, 16 events each
+  long long* trace;             // debug (CRNN_LSTM_TRACE=1): clock64 stamps [CTA 0 / 5][warpgroup slot 0 / 1][steps 8..11][16 events]
 };
 
-// debug timeline: one stamp per (selected CTA, step, event); all stamps of a CTA come from the same SM clock
-#define LSTM_TRACE(ev)                                                                                  \
+// debug timeline: one stamp per (selected CTA, warpgroup slot, step, event); all stamps of a CTA come from the same SM clock
+#define LSTM_TRACE_WG(wg, ev)                                                                           \
   do {                                                                                                  \
     if (p.trace != nullptr && lane == 0 && s >= 8 && s < 12 && (blockIdx.x == 0 || blockIdx.x == 5))    \
-      p.trace[(((blockIdx.x ? 1 : 0) * 4 + (s - 8)) * 16) + (ev)] = clock64();                          \
+      p.trace[((((blockIdx.x ? 1 : 0) * 2 + (wg)) * 4 + (s - 8)) * 16) + (ev)] = clock64();             \
   } while (0)
+#define LSTM_TRACE(ev) LSTM_TRACE_WG(0, ev)
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
@@ -257,23 +260,31 @@ lstm_persistent_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_con
 // MMA, the cell epilogue, an epilogue-side fence.proxy.async and a barrier.cluster arrive(release)+wait (CRNN_LSTM_TRACE=1 prints
 // the clock64 timeline).
 //
-//   * the A operand (h_{t-1}, [128 rows x 256]) lives in shared memory WITHOUT swizzle as [32 K-chunks][128 rows][16 B]
-//     (8-row x 16-B core matrices, LBO = 2048, SBO = 128), so the 32 units one CTA produces are ONE contiguous 8 KB slice
-//   * 8 epilogue warps (2 per 32-row quadrant, 16 units each) run the cell and write their h_t slice
-//       DS = true : straight into this CTA's own copy of the next A buffer (st.shared), then 7 bulk copies
-//                   shared::cta -> shared::cluster push the slice into the peers' A buffers and credit THEIR mbarriers
-//       DS = false: into a private 8 KB global buffer, then one bulk copy global -> shared::cluster with cluster MULTICAST
-//                   lands it in all 8 CTAs (L2 is read once per slice instead of 8 times)
-//   * the MMA thread of each CTA waits on its own mbarrier (8 slices) and goes; nobody waits for a cluster barrier
+//   * rows of a batch tile never interact, so the two MMA warpgroups run two INDEPENDENT recurrences, warpgroup `wgi` over rows
+//     64*wgi .. 64*wgi+63 (a "half"): each half has its own A buffers, mbarriers, named barrier and exchange, and never waits
+//     for the other half's rows (in practice the halves stay close to lockstep: their peers deliver both at about the same time)
+//   * the A operand (h_{t-1}) lives in shared memory WITHOUT swizzle, half-major as [2 halves][32 K-chunks][64 rows][16 B]
+//     (8-row x 16-B core matrices, LBO = 1024, SBO = 128), so the 32 units one CTA produces for one half are ONE contiguous
+//     4 KB slice
+//   * the cell runs on the wgmma accumulator fragment itself (wgmma.cuh): with the columns of Bh ordered [i|j|f|o] x 32 units,
+//     a thread's m64n128 fragment holds all four gates of units 8k + 2(l%4) + {0,1} (k = 0..3) for rows 16w + l/4 and +8;
+//     the cell state of those 16 cells stays in registers for all T steps.  No accumulator staging, no barrier before the cell.
+//   * each thread stores its h_t words (bf16 pairs) into the half's slice, then
+//       MODE ds: straight into this CTA's own copy of the next A buffer (st.shared), then 7 bulk copies
+//                shared::cta -> shared::cluster push the slice into the peers' A buffers and credit THEIR mbarriers
+//       MODE mc: into a private 4 KB global buffer, then one bulk copy global -> shared::cluster with cluster MULTICAST
+//                lands it in all 8 CTAs (L2 is read once per slice instead of 8 times)
+//       MODE ms / gx: below
+//   * the MMA warpgroup of each half waits on its own mbarrier (8 slices) and goes; nobody waits for a cluster barrier
 //   * A is double buffered: a slice of h_t can only be sent after its sender saw h_{t-1} from every CTA, i.e. after every CTA's
-//     MMA of step t-1 (the last reader of that buffer) has completed -- causality replaces a "buffer free" handshake
-//   * the accumulator is single buffered for the same reason (MMA t+1 needs this CTA's own h_t, sent after its accumulator reads)
-// Global exchange buffer (DS = false): p.h_state viewed as [2 bufs][2*tiles_per_dir units][8 ranks][8 KB].
-// EW = 8 epilogue warps = the two MMA warpgroups: two per 32-row quadrant, each owning 16 of the CTA's units.
+//     MMA of step t-1 of the same half (the last reader of that buffer) has completed -- causality replaces a "buffer free"
+//     handshake.  A half runs and exchanges all T steps even when none of its rows is valid: its peers wait for its slices.
+// Global exchange buffer (modes mc, ms, gx): p.h_state viewed as [2 bufs][2*tiles_per_dir units][2 halves][8 ranks][4 KB].
+// EW = 8 epilogue warps = the two MMA warpgroups.
 template <int EW>
 struct McThreads {
   static constexpr int EPI = EW * 32;
-  static constexpr int ALL = 128 + EPI;      // warpgroup 0 setup, warps 4.. MMA (two warpgroups) + epilogue
+  static constexpr int ALL = 128 + EPI;      // warpgroup 0 setup, warps 4.. MMA + cell (two warpgroups, one per half)
 };
 
 template <int CS>
@@ -281,10 +292,11 @@ struct CfgMc {
   static constexpr int UPC = 256 / CS;
   static constexpr int NCOLS = 4 * UPC;
   static constexpr int B_BYTES = 4 * NCOLS * 128;         // resident W_h slice (SW128 K-major, 4 K-blocks of 64)
-  static constexpr int A_BYTES = 32 * BLOCK_M * 16;       // [32 K-chunks][128 rows][16 B] = 64 KB per buffer
-  static constexpr int SLICE_BYTES = A_BYTES / CS;        // 8 KB: the 4 K-chunks one CTA produces
-  static constexpr int ACC_OFFSET = 2 * A_BYTES + B_BYTES;  // half of the accumulators [128 rows][4 gates x 16 units] f32
-  static constexpr int BAR_OFFSET = ACC_OFFSET + BLOCK_M * 64 * 4;
+  static constexpr int HALF_ROWS = BLOCK_M / 2;           // rows of one half (one MMA warpgroup)
+  static constexpr int HALF_A_BYTES = 32 * HALF_ROWS * 16;  // [32 K-chunks][64 rows][16 B] = 32 KB
+  static constexpr int A_BYTES = 2 * HALF_A_BYTES;        // one A buffer, both halves: 64 KB
+  static constexpr int SLICE_BYTES = HALF_A_BYTES / CS;   // 4 KB: the 4 K-chunks one CTA produces for one half
+  static constexpr int BAR_OFFSET = 2 * A_BYTES + B_BYTES;
   static constexpr int SMEM_BYTES = BAR_OFFSET + 128 + 1024;
 };
 
@@ -298,27 +310,25 @@ __device__ __forceinline__ void bulk_copy_s2s_cluster(uint32_t dst_cluster_addr,
 // MODE: 0 = global slice + multicast ("mc"), 1 = smem -> peer smem pushes ("ds"), 2 = smem slice -> bulk store to global ->
 // multicast to the 7 peers ("ms": no generic-proxy global stores, hence no full fence.proxy.async on the critical path),
 // 3 = generic proxy only ("gx"): st.global slice -> release.cluster arrive on every peer's mbarrier -> acquire.cluster wait ->
-// the 8 epilogue warps copy the 64 KB h tile L2 -> smem with ld.global.cg / st.shared (the exchange the K-split BPTT uses)
+// the half's 4 warps copy its 32 KB h image L2 -> smem with ld.global.cg / st.shared (the exchange the K-split BPTT uses)
 template <int CS, int MODE, int EW>
 __global__ void __launch_bounds__(McThreads<EW>::ALL, 1)
 lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
   static_assert(CS == 8, "8 CTAs x 32 units");
   using C = CfgMc<CS>;
   constexpr int UPC = C::UPC, NCOLS = C::NCOLS;
-  constexpr int HALF = UPC / (EW / 4);                      // units per epilogue warp
-  constexpr int MC_EPI_THREADS = McThreads<EW>::EPI;
   static_assert(EW == 8, "epilogue warps = the two MMA warpgroups");
+  static_assert(NCOLS == 128, "fragment column group j = gate j/4, units 8(j%4) ..: one m64n128 product per half and step");
   constexpr bool DS = (MODE == 1), MS = (MODE == 2), GX = (MODE == 3), LOCAL = DS || MS;   // LOCAL: own slice written in place
-  constexpr uint32_t FILL_TX = LOCAL ? (CS - 1) * C::SLICE_BYTES : C::A_BYTES;
+  constexpr uint32_t FILL_TX = LOCAL ? (CS - 1) * C::SLICE_BYTES : C::HALF_A_BYTES;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);   // offset arithmetic keeps the shared address space (STS)
-  uint8_t* smem_a = smem;                                   // [2][A_BYTES]
+  uint8_t* smem_a = smem;                                   // [2 bufs][2 halves][HALF_A_BYTES]
   uint8_t* smem_b = smem + 2 * C::A_BYTES;
-  uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + C::BAR_OFFSET);   // [2] one per A buffer
-  uint64_t* b_full = a_full + 2;
-  uint64_t* part_ready = b_full + 1;                      // [2] GX: the 8 CTAs' slices of one h buffer are in L2
-  float* acc_half = reinterpret_cast<float*>(smem + C::ACC_OFFSET);
+  uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + C::BAR_OFFSET);   // [2 halves][2 bufs]
+  uint64_t* b_full = a_full + 4;
+  uint64_t* part_ready = b_full + 1;                      // [2 halves][2 bufs] GX: the 8 CTAs' slices of one half's h buffer are in L2
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rank = (int)cluster_ctarank();
@@ -328,16 +338,18 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
 
   if (warp_idx == 0 && lane == 0) {
     ptx::prefetch_tmap(&tmW);
-    ptx::mbar_init(&part_ready[0], CS);
-    ptx::mbar_init(&part_ready[1], CS);
-    // DS: one arrival arms the byte count (MMA thread), the other says "the local slice is in place" (epilogue)
-    ptx::mbar_init(&a_full[0], GX ? MC_EPI_THREADS : LOCAL ? 2 : 1);      // GX: every epilogue thread copied its part of the tile
-    ptx::mbar_init(&a_full[1], GX ? MC_EPI_THREADS : LOCAL ? 2 : 1);
+    // DS / MS: one arrival arms the byte count (MMA warpgroup), the other says "the local slice is in place" (exchange lane)
+    for (int i = 0; i < 4; ++i) {
+      ptx::mbar_init(&part_ready[i], CS);
+      ptx::mbar_init(&a_full[i], GX ? 128 : LOCAL ? 2 : 1);     // GX: every thread of the half copied its part of the image
+    }
     ptx::mbar_init(b_full, 1);
     ptx::fence_barrier_init();
-    // first fills: buffer 1 receives h_0 (consumed at step 1), buffer 0 receives h_1 (consumed at step 2)
-    if (!GX && p.T > 1) ptx::mbar_arrive_expect_tx(&a_full[1], FILL_TX);
-    if (!GX && p.T > 2) ptx::mbar_arrive_expect_tx(&a_full[0], FILL_TX);
+    // first fills of each half: buffer 1 receives h_0 (consumed at step 1), buffer 0 receives h_1 (consumed at step 2)
+    for (int hf = 0; hf < 2; ++hf) {
+      if (!GX && p.T > 1) ptx::mbar_arrive_expect_tx(&a_full[2 * hf + 1], FILL_TX);
+      if (!GX && p.T > 2) ptx::mbar_arrive_expect_tx(&a_full[2 * hf + 0], FILL_TX);
+    }
     ptx::mbar_arrive_expect_tx(b_full, C::B_BYTES);
     for (int kb = 0; kb < 4; ++kb)
       ptx::tma_load_2d(&tmW, b_full, smem_b + kb * NCOLS * 128, kb * 64, dir * 1024 + rank * NCOLS);
@@ -350,197 +362,198 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
   if (warp_idx < 4) {
     ptx::setmaxnreg_dec<40>();
   } else {
-    // ===================== MMA (rows wgi*64 ..) + epilogue: thread = (sample row, 16 of the CTA's 32 units); cell state in registers
+    // ===================== one half per MMA warpgroup: MMA + cell on the accumulator fragment, cell state in registers
     ptx::setmaxnreg_inc<232>();
-    const int wgi = (warp_idx >> 2) - 1;
-    const int q = warp_idx & 3;
-    const int hh = (warp_idx - 4) >> 2;               // which HALF-unit group of the CTA's units
-    const int u0 = hh * HALF;
-    const int row = q * 32 + lane;
-    const int n = tile * BLOCK_M + row;
-    const bool okn = n < p.Nimg;
-    const int len = okn ? min(max(__ldg(p.seq_len + n), 0), p.T) : 0;
-    float cst[HALF];
+    const int wgi = (warp_idx >> 2) - 1;              // half: rows 64*wgi .. of the batch tile
+    const int w = warp_idx & 3, q4 = lane & 3;
+    const int rr0 = 16 * w + (lane >> 2);             // fragment rows rr0 and rr0 + 8 of the half
+    int n[2], len[2];
+    bool okn[2];
 #pragma unroll
-    for (int i = 0; i < HALF; ++i) cst[i] = 0.f;
+    for (int rh = 0; rh < 2; ++rh) {
+      n[rh] = tile * BLOCK_M + wgi * C::HALF_ROWS + rr0 + 8 * rh;
+      okn[rh] = n[rh] < p.Nimg;
+      len[rh] = okn[rh] ? min(max(__ldg(p.seq_len + n[rh]), 0), p.T) : 0;
+    }
+    float cst[2][4][2];                               // [row][k][unit 8k + 2*q4 + e]
+#pragma unroll
+    for (int rh = 0; rh < 2; ++rh)
+#pragma unroll
+      for (int k = 0; k < 4; ++k) { cst[rh][k][0] = 0.f; cst[rh][k][1] = 0.f; }
+    uint64_t* my_full = a_full + 2 * wgi;
+    uint64_t* my_ready = part_ready + 2 * wgi;
     ptx::mbar_wait(b_full, 0);
-    // this thread's HALF/8 x 16 B of the h slice: K-chunks u0/8 .. at chunk*2048 + row*16 inside the CTA's 8 KB slice
-    const uint32_t slice_off = rank * C::SLICE_BYTES + (u0 / 8) * 2048 + row * 16;
-    uint8_t* hx0 = reinterpret_cast<uint8_t*>(p.h_state) + ((size_t)unit * CS + rank) * C::SLICE_BYTES;
-    const size_t hx_buf_stride = (size_t)2 * p.tiles_per_dir * CS * C::SLICE_BYTES;
+    // this thread's 4-byte h words inside a half slice: K-chunk k (units 8k ..) at k*1024, row at 16 B per row, + 4 B per lane pair
+    const uint32_t word_off = rr0 * 16 + q4 * 4;
+    uint8_t* hx_half = reinterpret_cast<uint8_t*>(p.h_state) + (size_t)(unit * 2 + wgi) * C::HALF_A_BYTES;
+    const size_t hx_buf_stride = (size_t)2 * p.tiles_per_dir * C::A_BYTES;
 
     for (int s = 0; s < p.T; ++s) {
-      const bool active = s < len;
-      const int t = active ? (dir ? (len - 1 - s) : s) : s;
-      // this step's input projection (row n, step s; bw rows were stored reversed by the projection GEMM): 4 gates x 16 units
-      uint4 xp[4][HALF / 8];
-      if (active) {
-        const __nv_bfloat16* src = p.xproj + ((size_t)n * p.H + s) * 2048 + dir * 1024 + rank * NCOLS + u0;
+      bool active[2];
+      int t[2];
+      // this step's input projection (row n, step s; bw rows were stored reversed by the projection GEMM): [row][gate][k] bf16 pairs,
+      // issued before the h wait so that the loads are in flight during it
+      uint32_t xw[2][4][4];
 #pragma unroll
-        for (int g = 0; g < 4; ++g)
+      for (int rh = 0; rh < 2; ++rh) {
+        active[rh] = s < len[rh];
+        t[rh] = active[rh] ? (dir ? (len[rh] - 1 - s) : s) : s;
+        if (active[rh]) {
+          const uint32_t* src = reinterpret_cast<const uint32_t*>(p.xproj + ((size_t)n[rh] * p.H + s) * 2048 + dir * 1024 + rank * NCOLS + 2 * q4);
 #pragma unroll
-          for (int v = 0; v < HALF / 8; ++v) xp[g][v] = __ldg(reinterpret_cast<const uint4*>(src + g * UPC) + v);
+          for (int g = 0; g < 4; ++g)
+#pragma unroll
+            for (int k = 0; k < 4; ++k) xw[rh][g][k] = __ldg(src + (g * UPC + 8 * k) / 2);
+        } else {
+#pragma unroll
+          for (int g = 0; g < 4; ++g)
+#pragma unroll
+            for (int k = 0; k < 4; ++k) xw[rh][g][k] = 0u;
+        }
       }
-      if (warp_idx == 4) LSTM_TRACE(5);
-      uint32_t gi[HALF], gj[HALF], gf[HALF], go[HALF];
+      // the next step's 2 x 128-B lines of the same rows into L2: xproj (268 MB at the benchmark shape) comes from HBM, and a
+      // miss there would otherwise surface in the cell of the next step (the loads above have one h wait to land, not more)
+      if (q4 < 2) {
+#pragma unroll
+        for (int rh = 0; rh < 2; ++rh)
+          if (s + 1 < len[rh])
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(p.xproj + ((size_t)n[rh] * p.H + s + 1) * 2048 + dir * 1024 + rank * NCOLS + q4 * 64));
+      }
+      if (w == 0) LSTM_TRACE_WG(wgi, 5);
+      float d[NCOLS / 2];
       if (s > 0) {
         const int b = s & 1;
-        ptx::mbar_wait(&a_full[b], ((s - 1) >> 1) & 1);
-        if (warp_idx == 4) LSTM_TRACE(3);
+        ptx::mbar_wait(&my_full[b], ((s - 1) >> 1) & 1);
+        if (w == 0) LSTM_TRACE_WG(wgi, 3);
         // next fill of this buffer is h_{s+1}, consumed at step s+2; its senders are all behind this wait (see header)
-        if (!GX && s + 2 < p.T && threadIdx.x == 128) ptx::mbar_arrive_expect_tx(&a_full[b], FILL_TX);
-        const uint32_t a_base = ptx::smem_u32(smem_a + b * C::A_BYTES) + wgi * 64 * 16;
-        float d[NCOLS / 2];
+        if (!GX && s + 2 < p.T && (threadIdx.x & 127) == 0) ptx::mbar_arrive_expect_tx(&my_full[b], FILL_TX);
+        const uint32_t a_base = ptx::smem_u32(smem_a + b * C::A_BYTES + wgi * C::HALF_A_BYTES);
         wg::fence();
 #pragma unroll
         for (int k = 0; k < 16; ++k) {
-          const uint64_t a_desc = p.swap_ls ? ptx::make_desc_k_nosw(a_base + k * 4096, 128, 2048) : ptx::make_desc_k_nosw(a_base + k * 4096, 2048, 128);
+          const uint64_t a_desc = p.swap_ls ? ptx::make_desc_k_nosw(a_base + k * 2048, 128, 1024) : ptx::make_desc_k_nosw(a_base + k * 2048, 1024, 128);
           const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_b + (k >> 2) * NCOLS * 128)) + 2 * (k & 3);
           wg::mma_bf16<NCOLS>(d, a_desc, b_desc, k != 0);
         }
         wg::commit();
         wg::wait<0>();
         wg::fence_operand(d);
-        if (warp_idx == 4) LSTM_TRACE(4);
-        // the accumulators go through shared memory in two halves (units 0..15, then 16..31 of every gate): staged columns
-        // [gate][16 units]; the warps with hh == r read their rows of half r
-        const int tt = threadIdx.x & 127, l = tt & 31;
-        const int r0 = wgi * 64 + 16 * (tt >> 5) + (l >> 2);
+        if (w == 0) LSTM_TRACE_WG(wgi, 4);
+      } else {
 #pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          ptx::bar_sync(1, MC_EPI_THREADS);            // the other half's reads are done
+        for (int i = 0; i < NCOLS / 2; ++i) d[i] = 0.f;
+      }
+      // ---- the cell on the fragment: gate g of (row rh, unit 8k + 2*q4 + e) is d[16g + 4k + 2rh + e]; the activations overwrite
+      // the (then dead) pre-activations for the saved training state
+      uint32_t hw[2][4];                              // h_t as bf16 pairs [row][k]
 #pragma unroll
-          for (int g = 0; g < 4; ++g)
+      for (int rh = 0; rh < 2; ++rh)
 #pragma unroll
-            for (int jj = 0; jj < 2; ++jj) {
-              const int j = 4 * g + 2 * r + jj;          // fragment column group: gate g, units 16r + 8jj ..
-              const int c = g * 16 + jj * 8 + 2 * (l & 3);
-              *reinterpret_cast<float2*>(ptx::acc_chunk<64>(acc_half, r0, c >> 2) + (c & 3)) = make_float2(d[4 * j], d[4 * j + 1]);
-              *reinterpret_cast<float2*>(ptx::acc_chunk<64>(acc_half, r0 + 8, c >> 2) + (c & 3)) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+        for (int k = 0; k < 4; ++k) {
+          hw[rh][k] = 0u;                             // zero output past sequence_length (and for padding rows)
+          if (active[rh]) {
+            float hv[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int f = 4 * k + 2 * rh + e;
+              const float zi = d[f] + (e ? ptx::bf16_hi(xw[rh][0][k]) : ptx::bf16_lo(xw[rh][0][k]));
+              const float zj = d[16 + f] + (e ? ptx::bf16_hi(xw[rh][1][k]) : ptx::bf16_lo(xw[rh][1][k]));
+              const float zf = d[32 + f] + (e ? ptx::bf16_hi(xw[rh][2][k]) : ptx::bf16_lo(xw[rh][2][k]));
+              const float zo = d[48 + f] + (e ? ptx::bf16_hi(xw[rh][3][k]) : ptx::bf16_lo(xw[rh][3][k]));
+              const float ai = ptx::fast_sigmoid(zi), aj = ptx::fast_tanh(zj), af = ptx::fast_sigmoid(zf), ao = ptx::fast_sigmoid(zo);
+              const float c = af * cst[rh][k][e] + ai * aj;      // forget_bias (+1.0) is folded into the projected bias
+              cst[rh][k][e] = c;
+              hv[e] = ao * ptx::fast_tanh(c);
+              d[f] = ai; d[16 + f] = aj; d[32 + f] = af; d[48 + f] = ao;
             }
-          ptx::bar_sync(1, MC_EPI_THREADS);
-          if (hh == r) {
-            ptx::acc_ld<64, HALF>(acc_half, row, 0, gi);
-            ptx::acc_ld<64, HALF>(acc_half, row, 16, gj);
-            ptx::acc_ld<64, HALF>(acc_half, row, 32, gf);
-            ptx::acc_ld<64, HALF>(acc_half, row, 48, go);
+            hw[rh][k] = ptx::pack_bf16x2(hv[0], hv[1]);
           }
         }
-        if (warp_idx == 4) LSTM_TRACE(7);
-      } else {
-#pragma unroll
-        for (int i = 0; i < HALF; ++i) { gi[i] = 0u; gj[i] = 0u; gf[i] = 0u; go[i] = 0u; }
-      }
-      uint32_t hp[HALF / 2];
-      if (active) {
-        const uint32_t* xi = reinterpret_cast<const uint32_t*>(xp[0]);
-        const uint32_t* xj = reinterpret_cast<const uint32_t*>(xp[1]);
-        const uint32_t* xf = reinterpret_cast<const uint32_t*>(xp[2]);
-        const uint32_t* xo = reinterpret_cast<const uint32_t*>(xp[3]);
-        float hv[HALF];
-#pragma unroll
-        for (int i = 0; i < HALF; ++i) {
-          const float zi = __uint_as_float(gi[i]) + ((i & 1) ? ptx::bf16_hi(xi[i >> 1]) : ptx::bf16_lo(xi[i >> 1]));
-          const float zj = __uint_as_float(gj[i]) + ((i & 1) ? ptx::bf16_hi(xj[i >> 1]) : ptx::bf16_lo(xj[i >> 1]));
-          const float zf = __uint_as_float(gf[i]) + ((i & 1) ? ptx::bf16_hi(xf[i >> 1]) : ptx::bf16_lo(xf[i >> 1]));
-          const float zo = __uint_as_float(go[i]) + ((i & 1) ? ptx::bf16_hi(xo[i >> 1]) : ptx::bf16_lo(xo[i >> 1]));
-          const float ai = ptx::fast_sigmoid(zi), aj = ptx::fast_tanh(zj), af = ptx::fast_sigmoid(zf), ao = ptx::fast_sigmoid(zo);
-          const float c = af * cst[i] + ai * aj;                 // forget_bias (+1.0) is folded into the projected bias
-          cst[i] = c;
-          hv[i] = ao * ptx::fast_tanh(c);
-          if (p.gates != nullptr) {                              // reuse the (now dead) accumulator registers as staging
-            gi[i] = __float_as_uint(ai); gj[i] = __float_as_uint(aj); gf[i] = __float_as_uint(af); go[i] = __float_as_uint(ao);
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < HALF / 2; ++i) hp[i] = ptx::pack_bf16x2(hv[2 * i], hv[2 * i + 1]);
-      } else {
-#pragma unroll
-        for (int i = 0; i < HALF / 2; ++i) hp[i] = 0u;     // zero output past sequence_length (and for padding rows)
-      }
+      if (w == 0) LSTM_TRACE_WG(wgi, 7);
       // ---- h_t slice first (it is on the critical path), bookkeeping stores afterwards
       if (s + 1 < p.T) {
         const int nb = (s + 1) & 1;
-        if (LOCAL) {
-          uint8_t* dst = smem_a + nb * C::A_BYTES + slice_off;
+        uint8_t* my_slice = smem_a + nb * C::A_BYTES + wgi * C::HALF_A_BYTES + rank * C::SLICE_BYTES;
+        uint8_t* hx_slice = hx_half + (size_t)nb * hx_buf_stride + rank * C::SLICE_BYTES;
+        // a warp's 4-byte stores cover 8 rows x 16 B of one K-chunk: conflict-free in shared memory, 128 B contiguous in global
+        uint8_t* dst = (LOCAL ? my_slice : hx_slice) + word_off;
 #pragma unroll
-          for (int v = 0; v < HALF / 8; ++v)
-            *reinterpret_cast<uint4*>(dst + v * 2048) = make_uint4(hp[4 * v], hp[4 * v + 1], hp[4 * v + 2], hp[4 * v + 3]);
-          ptx::fence_proxy_async_smem();                    // generic-proxy smem writes -> async proxy (bulk copies, wgmma)
-        } else {
-          uint8_t* dst = hx0 + (size_t)nb * hx_buf_stride + (u0 / 8) * 2048 + row * 16;
+        for (int rh = 0; rh < 2; ++rh)
 #pragma unroll
-          for (int v = 0; v < HALF / 8; ++v)
-            *reinterpret_cast<uint4*>(dst + v * 2048) = make_uint4(hp[4 * v], hp[4 * v + 1], hp[4 * v + 2], hp[4 * v + 3]);
-          if (!GX) fence_proxy_async_all();                 // generic-proxy global writes -> async proxy (bulk copy)
-        }
-        if (warp_idx == 4) LSTM_TRACE(8);
-        asm volatile("bar.sync 1, %0;" ::"n"(MC_EPI_THREADS) : "memory");
-        if (warp_idx == 4) {
-          uint8_t* my_slice = smem_a + nb * C::A_BYTES + rank * C::SLICE_BYTES;
+          for (int k = 0; k < 4; ++k) *reinterpret_cast<uint32_t*>(dst + k * 1024 + rh * 128) = hw[rh][k];
+        if (LOCAL) ptx::fence_proxy_async_smem();           // generic-proxy smem writes -> async proxy (bulk copies, wgmma)
+        else if (!GX) fence_proxy_async_all();              // generic-proxy global writes -> async proxy (bulk copy)
+        if (w == 0) LSTM_TRACE_WG(wgi, 8);
+        if (wgi == 0) ptx::bar_sync(1, 128);                // the half's slice is complete (named barrier 1 / 2 per half)
+        else ptx::bar_sync(2, 128);
+        if (w == 0) {
           if (DS) {
             if (lane < CS) {
               if (lane == rank) {
-                ptx::mbar_arrive(&a_full[nb]);
+                ptx::mbar_arrive(&my_full[nb]);
               } else {
-                const uint32_t dst = ptx::mapa(ptx::smem_u32(my_slice), (uint32_t)lane);
-                const uint32_t bar = ptx::mapa(ptx::smem_u32(&a_full[nb]), (uint32_t)lane);
-                bulk_copy_s2s_cluster(dst, my_slice, C::SLICE_BYTES, bar);
+                const uint32_t dst_peer = ptx::mapa(ptx::smem_u32(my_slice), (uint32_t)lane);
+                const uint32_t bar = ptx::mapa(ptx::smem_u32(&my_full[nb]), (uint32_t)lane);
+                bulk_copy_s2s_cluster(dst_peer, my_slice, C::SLICE_BYTES, bar);
               }
             }
           } else if (MS) {
             if (lane == 0) {
-              uint8_t* g = hx0 + (size_t)nb * hx_buf_stride;
-              ptx::bulk_store_1d(g, my_slice, C::SLICE_BYTES);                // async proxy: smem -> global (L2)
+              ptx::bulk_store_1d(hx_slice, my_slice, C::SLICE_BYTES);          // async proxy: smem -> global (L2)
               ptx::bulk_commit();
               asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");       // writes performed, not just the smem reads
-              ptx::bulk_load_1d_mc(my_slice, g, C::SLICE_BYTES, &a_full[nb], (uint16_t)(((1u << CS) - 1) & ~(1u << rank)));
-              ptx::mbar_arrive(&a_full[nb]);                                  // the local slice is already in place
+              ptx::bulk_load_1d_mc(my_slice, hx_slice, C::SLICE_BYTES, &my_full[nb], (uint16_t)(((1u << CS) - 1) & ~(1u << rank)));
+              ptx::mbar_arrive(&my_full[nb]);                                 // the local slice is already in place
             }
           } else if (GX) {
-            // cumulative over the barrier above: the release covers every epilogue thread's slice stores
-            if (lane < CS) ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&part_ready[nb]), (uint32_t)lane));
+            // cumulative over the barrier above: the release covers every thread's slice stores of this half
+            if (lane < CS) ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&my_ready[nb]), (uint32_t)lane));
           } else if (lane == 0) {
-            ptx::bulk_load_1d_mc(my_slice, hx0 + (size_t)nb * hx_buf_stride, C::SLICE_BYTES, &a_full[nb], (uint16_t)((1u << CS) - 1));
+            ptx::bulk_load_1d_mc(my_slice, hx_slice, C::SLICE_BYTES, &my_full[nb], (uint16_t)((1u << CS) - 1));
           }
           __syncwarp();
-          LSTM_TRACE(9);
+          LSTM_TRACE_WG(wgi, 9);
         }
         if (GX) {
-          // h_t of the whole tile = the cluster's 8 contiguous slices = exactly the A operand image: 64 KB, 16 B per thread per pass
-          ptx::mbar_wait_cluster(&part_ready[nb], (uint32_t)(s >> 1) & 1u);
-          const uint8_t* g = reinterpret_cast<const uint8_t*>(p.h_state) + (size_t)nb * hx_buf_stride + (size_t)unit * CS * C::SLICE_BYTES;
-          uint8_t* d = smem_a + nb * C::A_BYTES;
-          const int et = threadIdx.x - 128;                      // 0 .. MC_EPI_THREADS-1
-          uint4 v[C::A_BYTES / 16 / MC_EPI_THREADS];
+          // h_t of the half = the cluster's 8 contiguous slices = exactly the half's A operand image: 32 KB, 16 B per thread per pass
+          ptx::mbar_wait_cluster(&my_ready[nb], (uint32_t)(s >> 1) & 1u);
+          const uint8_t* g = hx_half + (size_t)nb * hx_buf_stride;
+          uint8_t* a = smem_a + nb * C::A_BYTES + wgi * C::HALF_A_BYTES;
+          const int et = threadIdx.x & 127;
+          uint4 v[C::HALF_A_BYTES / 16 / 128];
 #pragma unroll
-          for (int k = 0; k < C::A_BYTES / 16 / MC_EPI_THREADS; ++k) v[k] = __ldcg(reinterpret_cast<const uint4*>(g) + k * MC_EPI_THREADS + et);
+          for (int k = 0; k < C::HALF_A_BYTES / 16 / 128; ++k) v[k] = __ldcg(reinterpret_cast<const uint4*>(g) + k * 128 + et);
 #pragma unroll
-          for (int k = 0; k < C::A_BYTES / 16 / MC_EPI_THREADS; ++k) *(reinterpret_cast<uint4*>(d) + k * MC_EPI_THREADS + et) = v[k];
+          for (int k = 0; k < C::HALF_A_BYTES / 16 / 128; ++k) *(reinterpret_cast<uint4*>(a) + k * 128 + et) = v[k];
           ptx::fence_proxy_async_smem();
-          ptx::mbar_arrive(&a_full[nb]);
+          ptx::mbar_arrive(&my_full[nb]);
         }
       }
-      if (okn) {
-        __nv_bfloat16* lo = p.lstm_out + ((size_t)n * p.H + t) * 512 + dir * 256 + rank * UPC + u0;
-        if constexpr (HALF == 16) ptx::st_global_v8(lo, hp[0], hp[1], hp[2], hp[3], hp[4], hp[5], hp[6], hp[7]);
-        else *reinterpret_cast<uint4*>(lo) = make_uint4(hp[0], hp[1], hp[2], hp[3]);
-      }
-      if (active && p.gates != nullptr) {
-        const size_t dts = (size_t)unit * p.T + s;                  // coalesced saved-state layout, common.cuh
-        __nv_bfloat16* gs = p.gates + lstm_gate_off(dts, 0, rank * UPC + u0, row);
-        float* cs = p.csave + lstm_c_off(dts, rank * UPC + u0, row);
 #pragma unroll
-        for (int i = 0; i < HALF; i += 8) {
-          *reinterpret_cast<uint4*>(gs + 0 * LSTM_GATE_STRIDE + (i >> 3) * LSTM_GCHUNK_STRIDE) = make_uint4(ptx::pack_bf16x2(__uint_as_float(gi[i]), __uint_as_float(gi[i + 1])), ptx::pack_bf16x2(__uint_as_float(gi[i + 2]), __uint_as_float(gi[i + 3])), ptx::pack_bf16x2(__uint_as_float(gi[i + 4]), __uint_as_float(gi[i + 5])), ptx::pack_bf16x2(__uint_as_float(gi[i + 6]), __uint_as_float(gi[i + 7])));
-          *reinterpret_cast<uint4*>(gs + 1 * LSTM_GATE_STRIDE + (i >> 3) * LSTM_GCHUNK_STRIDE) = make_uint4(ptx::pack_bf16x2(__uint_as_float(gj[i]), __uint_as_float(gj[i + 1])), ptx::pack_bf16x2(__uint_as_float(gj[i + 2]), __uint_as_float(gj[i + 3])), ptx::pack_bf16x2(__uint_as_float(gj[i + 4]), __uint_as_float(gj[i + 5])), ptx::pack_bf16x2(__uint_as_float(gj[i + 6]), __uint_as_float(gj[i + 7])));
-          *reinterpret_cast<uint4*>(gs + 2 * LSTM_GATE_STRIDE + (i >> 3) * LSTM_GCHUNK_STRIDE) = make_uint4(ptx::pack_bf16x2(__uint_as_float(gf[i]), __uint_as_float(gf[i + 1])), ptx::pack_bf16x2(__uint_as_float(gf[i + 2]), __uint_as_float(gf[i + 3])), ptx::pack_bf16x2(__uint_as_float(gf[i + 4]), __uint_as_float(gf[i + 5])), ptx::pack_bf16x2(__uint_as_float(gf[i + 6]), __uint_as_float(gf[i + 7])));
-          *reinterpret_cast<uint4*>(gs + 3 * LSTM_GATE_STRIDE + (i >> 3) * LSTM_GCHUNK_STRIDE) = make_uint4(ptx::pack_bf16x2(__uint_as_float(go[i]), __uint_as_float(go[i + 1])), ptx::pack_bf16x2(__uint_as_float(go[i + 2]), __uint_as_float(go[i + 3])), ptx::pack_bf16x2(__uint_as_float(go[i + 4]), __uint_as_float(go[i + 5])), ptx::pack_bf16x2(__uint_as_float(go[i + 6]), __uint_as_float(go[i + 7])));
+      for (int rh = 0; rh < 2; ++rh) {
+        if (okn[rh]) {
+          __nv_bfloat16* lo = p.lstm_out + ((size_t)n[rh] * p.H + t[rh]) * 512 + dir * 256 + rank * UPC + 2 * q4;
+#pragma unroll
+          for (int k = 0; k < 4; ++k) *reinterpret_cast<uint32_t*>(lo + 8 * k) = hw[rh][k];
         }
+        if (active[rh] && p.gates != nullptr) {
+          // coalesced saved-state layout (common.cuh): a warp's stores of one (gate, K-chunk) cover 8 rows x 16 B = 128 B contiguous
+          const size_t dts = (size_t)unit * p.T + s;
+          const int row = wgi * C::HALF_ROWS + rr0 + 8 * rh;
+          __nv_bfloat16* gs = p.gates + lstm_gate_off(dts, 0, rank * UPC, row) + 2 * q4;
+          float* cs = p.csave + lstm_c_off(dts, rank * UPC, row) + 2 * (q4 & 1);
 #pragma unroll
-        for (int i = 0; i < HALF; i += 4) *reinterpret_cast<float4*>(cs + (i >> 2) * LSTM_CCHUNK_STRIDE) = make_float4(cst[i], cst[i + 1], cst[i + 2], cst[i + 3]);
+          for (int g = 0; g < 4; ++g)
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+              *reinterpret_cast<uint32_t*>(gs + g * LSTM_GATE_STRIDE + k * LSTM_GCHUNK_STRIDE) =
+                  ptx::pack_bf16x2(d[16 * g + 4 * k + 2 * rh], d[16 * g + 4 * k + 2 * rh + 1]);
+#pragma unroll
+          for (int k = 0; k < 4; ++k)      // units 8k + 2*q4 .. = 4-unit chunk 2k + q4/2, position 2*(q4&1)
+            *reinterpret_cast<float2*>(cs + (2 * k + (q4 >> 1)) * LSTM_CCHUNK_STRIDE) = make_float2(cst[rh][k][0], cst[rh][k][1]);
+        }
       }
-      if (warp_idx == 4) LSTM_TRACE(10);
+      if (w == 0) LSTM_TRACE_WG(wgi, 10);
     }
   }
 

@@ -681,8 +681,8 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     lp.gates = pl.train ? pl.gates : nullptr; lp.csave = pl.train ? pl.csave : nullptr;
     static long long* d_trace = nullptr;          // debug timeline (CRNN_LSTM_TRACE=1), printed to stderr after every launch
     const bool want_trace = getenv("CRNN_LSTM_TRACE") != nullptr;
-    if (want_trace && d_trace == nullptr) CUDA_TRY(cudaMalloc(&d_trace, 2 * 4 * 16 * sizeof(long long)));
-    if (want_trace) CUDA_TRY(cudaMemsetAsync(d_trace, 0, 2 * 4 * 16 * sizeof(long long), st));
+    if (want_trace && d_trace == nullptr) CUDA_TRY(cudaMalloc(&d_trace, 2 * 2 * 4 * 16 * sizeof(long long)));
+    if (want_trace) CUDA_TRY(cudaMemsetAsync(d_trace, 0, 2 * 2 * 4 * 16 * sizeof(long long), st));
     lp.trace = want_trace ? d_trace : nullptr;
     lp.swap_ls = getenv("CRNN_LSTM_SWAPLS") != nullptr;
     auto kern = lstm::lstm_persistent_kernel<CS>;
@@ -715,15 +715,24 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     else if (m->lstm_mc == 1) CUDA_TRY(cudaLaunchKernelEx(&cfg, kern_mc, m->tB_h128, lp));
     else CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, pl.tA_hall, m->tB_h128, lp));
     if (want_trace) {
-      long long h[2 * 4 * 16];
+      long long h[2 * 2 * 4 * 16];            // [CTA 0 / 5][warpgroup slot][step 8..11][event]
       CUDA_TRY(cudaStreamSynchronize(st));
       CUDA_TRY(cudaMemcpy(h, d_trace, sizeof(h), cudaMemcpyDeviceToHost));
-      for (int c = 0; c < 2; ++c)
-        for (int s = 0; s < 4; ++s) {
-          fprintf(stderr, "lstm_trace cta%d step%d:", c ? 5 : 0, 8 + s);
-          for (int e = 0; e < 12; ++e) fprintf(stderr, " %lld", h[(c * 4 + s) * 16 + e] ? h[(c * 4 + s) * 16 + e] - h[(c * 4) * 16] : -1);
-          fprintf(stderr, "\n");
-        }
+      for (int c = 0; c < 2; ++c) {
+        long long t0 = 0;                       // earliest stamp of the CTA: both warpgroups on one time axis
+        for (int i = c * 128; i < (c + 1) * 128; ++i)
+          if (h[i] && (!t0 || h[i] < t0)) t0 = h[i];
+        for (int wg = 0; wg < 2; ++wg)
+          for (int s = 0; s < 4; ++s) {
+            const long long* r = h + ((c * 2 + wg) * 4 + s) * 16;
+            bool any = false;
+            for (int e = 0; e < 16; ++e) any = any || r[e];
+            if (!any) continue;
+            fprintf(stderr, "lstm_trace cta%d wg%d step%d:", c ? 5 : 0, wg, 8 + s);
+            for (int e = 0; e < 12; ++e) fprintf(stderr, " %lld", r[e] ? r[e] - t0 : -1);
+            fprintf(stderr, "\n");
+          }
+      }
     }
   } else {
     // per-step launches (debug fallback, CRNN_LSTM_IMPL=step): both directions stacked along M

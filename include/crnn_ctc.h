@@ -221,12 +221,20 @@ int     crnn_peer_error(crnn_model* m, int* err_host);   /* 1 if an exchange tim
  * permuted gate columns, backward-direction rows reversed by length), "a4a_pre" "a4b_pre" (conv4_x before BatchNorm).
  * Training-mode plans only (CRNN_INVALID_VALUE otherwise): "gates" (saved post-activation gates, layout of
  * lstm_gate_off) and the backward buffers "dl_rows" "d_lstm_out" "dz_all" "d_a5" "d_a4b" "d_pre4b" "d_pre4a"
- * "d_a3p" "d_pre32" "d_pre31" "d_a2" "d_pre2" "d_a1" of the last crnn_backward(). */
+ * "d_a3p" "d_pre32" "d_pre31" "d_a2" "d_pre2" "d_a1" of the last crnn_backward().
+ * f32-class models (compute_dtype 2, 3): the eight activation names (split mode: the f32 sum hi + lo) and "xproj", which
+ * there is f32 [N, H2, 2048]: both directions' x W_x in natural [i|j|f|o] column order, WITHOUT bias and with the rows
+ * of the backward direction NOT reversed (the cell adds the bias and indexes frame len-1-step).  Other names fail with
+ * CRNN_INVALID_VALUE. */
 int     crnn_debug_tap(crnn_model* m, const char* name, float* dst, size_t dst_elems,
                        void* workspace, crnn_stream_t stream);
 /* Same for the buffers that are not bf16, copied byte for byte: "bn" (f32 [2 layers][scale, shift, mean, invstd][512]),
  * "stats" (f64 [2 layers][sum, sum of squares][512]) and, training-mode plans only, "am1" "am2" "am3" (u8 pool
- * window index dy*2+dx per pooled element) and "csave" (f32 saved cell state, layout of lstm_c_off). */
+ * window index dy*2+dx per pooled element) and "csave" (f32 saved cell state, layout of lstm_c_off).
+ * f32-class models: "bn" and "stats" (same layouts), "cst" (f32 final cell state [2 dirs][Npad][256]) and the
+ * activation buffers as stored under their tap names "conv1" .. "conv5", "lstm_out": split mode (2) bf16 rows
+ * [hi(G*C) | lo(G*C)] of G consecutive positions (G = 2 for "conv4_2", else 1), tf32 mode (3) f32 [positions][C]
+ * rounded to tf32.  Other names (am1..3, csave, the backward buffers) fail with CRNN_INVALID_VALUE. */
 int     crnn_debug_tap_raw(crnn_model* m, const char* name, void* dst, size_t dst_bytes,
                            void* workspace, crnn_stream_t stream);
 

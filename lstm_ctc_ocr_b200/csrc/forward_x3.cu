@@ -534,25 +534,46 @@ int x3_forward(crnn_model* m, const float* data, const int* time_step_len, int N
   return CRNN_OK;
 }
 
+namespace x3 {
+// activation buffer of a tap name: npos positions of C channels, G positions per [hi | lo] row (split mode)
+static bool act_buffer(const Plan& pl, const std::string& k, const uint8_t** src, size_t* npos, int* C, int* G) {
+  const size_t n = pl.N, h1 = pl.H1, h2 = pl.H2;
+  *G = 1;
+  if (k == "conv1") { *src = pl.s1; *npos = n * h1 * 16; *C = 64; }
+  else if (k == "conv2") { *src = pl.s2; *npos = n * h2 * 8; *C = 128; }
+  else if (k == "conv3_1") { *src = pl.s3; *npos = n * h2 * 8; *C = 256; }
+  else if (k == "conv3_2") { *src = pl.s3p; *npos = n * h2 * 4; *C = 256; }
+  else if (k == "conv4_1") { *src = pl.s4a; *npos = n * h2 * 4; *C = 512; }
+  else if (k == "conv4_2") { *src = pl.s4b; *npos = n * h2 * 2; *C = 512; *G = 2; }
+  else if (k == "conv5") { *src = pl.s5; *npos = n * h2; *C = 512; }
+  else if (k == "lstm_out") { *src = pl.slo; *npos = n * h2; *C = 512; }
+  else return false;
+  return true;
+}
+
+static State* tapped_state(crnn_model* m, void* workspace) {
+  State* s = reinterpret_cast<State*>(m->x3);
+  return (!s || s->plan.ws == nullptr || s->plan.ws != workspace) ? nullptr : s;
+}
+}  // namespace x3
+
 int x3_debug_tap(crnn_model* m, const char* name, float* dst, size_t dst_elems, void* workspace, cudaStream_t st) {
   using namespace x3;
-  State* s = reinterpret_cast<State*>(m->x3);
-  if (!s || s->plan.ws == nullptr || s->plan.ws != workspace) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: no forward ran on this workspace");
+  State* s = tapped_state(m, workspace);
+  if (!s) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: no forward ran on this workspace");
   x3::Plan& pl = s->plan;
-  const size_t n = pl.N, h1 = pl.H1, h2 = pl.H2;
+  const std::string k(name);
+  if (k == "xproj") {                 // f32 already, both directions in natural [i|j|f|o] order, no bias, rows not reversed
+    const size_t cnt = (size_t)pl.N * pl.H2 * 2048;
+    if (dst_elems < cnt) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: dst too small");
+    CUDA_TRY(cudaMemcpyAsync(dst, pl.xproj, cnt * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return CRNN_OK;
+  }
   const uint8_t* src = nullptr;
   size_t npos = 0;
   int C = 0, G = 1;
-  std::string k(name);
-  if (k == "conv1") { src = pl.s1; npos = n * h1 * 16; C = 64; }
-  else if (k == "conv2") { src = pl.s2; npos = n * h2 * 8; C = 128; }
-  else if (k == "conv3_1") { src = pl.s3; npos = n * h2 * 8; C = 256; }
-  else if (k == "conv3_2") { src = pl.s3p; npos = n * h2 * 4; C = 256; }
-  else if (k == "conv4_1") { src = pl.s4a; npos = n * h2 * 4; C = 512; }
-  else if (k == "conv4_2") { src = pl.s4b; npos = n * h2 * 2; C = 512; G = 2; }
-  else if (k == "conv5") { src = pl.s5; npos = n * h2; C = 512; }
-  else if (k == "lstm_out") { src = pl.slo; npos = n * h2; C = 512; }
-  else return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: unknown tap %s", name);
+  if (!act_buffer(pl, k, &src, &npos, &C, &G))
+    return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: %s does not exist on the f32-class paths (compute_dtype 2, 3)", name);
   if (dst_elems < npos * C) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: dst too small");
   if (s->tf32) {
     CUDA_TRY(cudaMemcpyAsync(dst, src, npos * C * sizeof(float), cudaMemcpyDeviceToDevice, st));   // plain f32 NHWC already
@@ -560,5 +581,28 @@ int x3_debug_tap(crnn_model* m, const char* name, float* dst, size_t dst_elems, 
   }
   split_to_f32_kernel<<<(unsigned)((npos * C + 255) / 256), 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(src), dst, npos, C, G);
   CUDA_TRY(cudaGetLastError());
+  return CRNN_OK;
+}
+
+// Byte-for-byte copies of the f32-class workspace: "bn", "stats", "cst" and the activation buffers as stored (split mode:
+// bf16 [hi | lo] rows, G positions per row; tf32 mode: f32 rows).  The same bytes per position in both modes.
+int x3_debug_tap_raw(crnn_model* m, const char* name, void* dst, size_t dst_bytes, void* workspace, cudaStream_t st) {
+  using namespace x3;
+  State* s = tapped_state(m, workspace);
+  if (!s) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: no forward ran on this workspace");
+  x3::Plan& pl = s->plan;
+  const std::string k(name);
+  const void* src = nullptr;
+  size_t bytes = 0;
+  const uint8_t* act = nullptr;
+  size_t npos = 0;
+  int C = 0, G = 1;
+  if (k == "bn") { src = pl.bn; bytes = 2 * 4 * 512 * sizeof(float); }
+  else if (k == "stats") { src = pl.stats; bytes = 2 * 2 * 512 * sizeof(double); }
+  else if (k == "cst") { src = pl.cst; bytes = (size_t)2 * pl.Npad * 256 * sizeof(float); }
+  else if (act_buffer(pl, k, &act, &npos, &C, &G)) { src = act; bytes = npos * C * 4; }     // 2 x bf16 or 1 x f32 per value
+  else return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: %s does not exist on the f32-class paths (compute_dtype 2, 3)", name);
+  if (dst_bytes < bytes) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: dst too small (%zu < %zu bytes)", dst_bytes, bytes);
+  CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st));
   return CRNN_OK;
 }

@@ -879,7 +879,7 @@ extern "C" int crnn_debug_tap(crnn_model* m, const char* name, float* dst, size_
 extern "C" int crnn_debug_tap_raw(crnn_model* m, const char* name, void* dst, size_t dst_bytes, void* workspace,
                                   crnn_stream_t stream) {
   if (!m || !name || !dst) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: null");
-  if (m->cfg.compute_dtype >= 2) return crnn_fail(CRNN_UNSUPPORTED, "debug_tap_raw: only the bf16 path (compute_dtype 1) has these buffers");
+  if (m->cfg.compute_dtype >= 2) return x3_debug_tap_raw(m, name, dst, dst_bytes, workspace, reinterpret_cast<cudaStream_t>(stream));
   Plan& pl = m->plan;
   if (pl.ws == nullptr || pl.ws != workspace) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: no forward ran on this workspace");
   const size_t n = pl.N, h1 = pl.H1, h2 = pl.H2;

@@ -142,6 +142,7 @@ size_t x3_workspace_size(int N, int W);
 int x3_forward(crnn_model* m, const float* data, const int* time_step_len, int N, int W, float* logits_out, void* workspace,
                size_t workspace_bytes, cudaStream_t st);
 int x3_debug_tap(crnn_model* m, const char* name, float* dst, size_t dst_elems, void* workspace, cudaStream_t st);
+int x3_debug_tap_raw(crnn_model* m, const char* name, void* dst, size_t dst_bytes, void* workspace, cudaStream_t st);
 void x3_destroy(crnn_model* m);
 void x3_params_changed(crnn_model* m);
 

@@ -206,14 +206,30 @@ class CrnnModel:
 
     def tap_raw(self, name, N, W):
         """Non-bf16 workspace buffer of the last forward, byte for byte (tests only): "bn" f32 [2][4][512] (scale, shift,
-        mean, invstd per BN layer), "stats" f64 [2][2][512]; training only: "am1" / "am2" / "am3" u8 pool window index
-        (dy*2+dx) in the pooled NHWC shape, "csave" f32 [dir * Npad/128 + tile][step][unit / 4][row][unit % 4]."""
+        mean, invstd per BN layer), "stats" f64 [2][2][512]; bf16 path, training only: "am1" / "am2" / "am3" u8 pool window
+        index (dy*2+dx) in the pooled NHWC shape, "csave" f32 [dir * Npad/128 + tile][step][unit / 4][row][unit % 4].
+        f32-class paths: "cst" f32 [2][Npad][256] (final cell state) and the stored activations "conv1" .. "conv5",
+        "lstm_out": "f32" (split) bf16 [..., 2 (hi, lo), C] per position, conv4_2 [N, H2, 2 (hi, lo), 2 positions, 512]
+        (rows of G = 2 positions); "tf32" f32 in the tap shape."""
         H1, H2 = W // 2, W // 4
         Npad, T = (N + 127) // 128 * 128, H2 - 1
-        shapes = {"bn": ((2, 4, 512), torch.float32), "stats": ((2, 2, 512), torch.float64),
-                  "am1": ((N, H1, 16, 64), torch.uint8), "am2": ((N, H2, 8, 128), torch.uint8),
-                  "am3": ((N, H2, 4, 256), torch.uint8), "csave": ((2 * Npad // 128, T, 64, 128, 4), torch.float32)}
-        shp, dt = shapes[name]
+        shapes = {"bn": ((2, 4, 512), torch.float32), "stats": ((2, 2, 512), torch.float64)}
+        if self.compute_dtype == 1:
+            shapes.update({"am1": ((N, H1, 16, 64), torch.uint8), "am2": ((N, H2, 8, 128), torch.uint8),
+                           "am3": ((N, H2, 4, 256), torch.uint8), "csave": ((2 * Npad // 128, T, 64, 128, 4), torch.float32)})
+        else:
+            acts = {"conv1": (N, H1, 16), "conv2": (N, H2, 8), "conv3_1": (N, H2, 8), "conv3_2": (N, H2, 4),
+                    "conv4_1": (N, H2, 4), "conv4_2": (N, H2), "conv5": (N, H2), "lstm_out": (N, H2)}
+            chans = {"conv1": 64, "conv2": 128, "conv3_1": 256, "conv3_2": 256}
+            shapes["cst"] = ((2, Npad, 256), torch.float32)
+            for k, lead in acts.items():
+                C = chans.get(k, 512)
+                if self.compute_dtype == 3:
+                    shapes[k] = (lead + ((2,) if k == "conv4_2" else ()) + (C,), torch.float32)
+                else:
+                    shapes[k] = (lead + (2,) + ((2,) if k == "conv4_2" else ()) + (C,), torch.bfloat16)
+        # a name this path does not have goes to the library as well, which refuses it with CRNN_INVALID_VALUE
+        shp, dt = shapes.get(name, ((1,), torch.uint8))
         dst = torch.empty(shp, dtype=dt, device=self.device)
         ws, _ = self._workspace(N, W)
         check(self.lib.crnn_debug_tap_raw(self.handle, name.encode(), dst.data_ptr(), dst.numel() * dst.element_size(), ws,

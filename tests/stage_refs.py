@@ -14,6 +14,13 @@ upstream gradient as grad_outputs; `acc` is the same vector-Jacobian product on 
 backward compares).  The GPU tests pass `bf16`; tests/test_stage_refs_cpu.py passes `ident` and chains the stages from the
 oracle's fp64 activations, which must then reproduce the oracle's forward and gradients.
 
+The f32-class paths (csrc/forward_x3.cu) use the same functions.  Their split-bf16 operands enter as (hi, lo) pairs
+(`split`): wherever an activation and a weight are both pairs, the linear part of a stage is the split-operand product
+ah*wh + al*wh + ah*wl that the kernels' virtual K = [hi | lo | hi] against [wh | wh | wl] computes, evaluated in fp64, so
+the one dropped term al*wl is left out of the reference as well.  tf32 operands enter as plain values rounded by
+`tf32_rna`.  `x3=True` selects the recurrence layout of that path: an input projection without bias in natural gate order
+and natural frame order, the bias (+1 on f) added by the cell, the backward direction reading frame len-1-step.
+
 Test infrastructure only (imported by tests/)."""
 import numpy as np
 import torch
@@ -34,6 +41,58 @@ def f32(x):
 
 def ident(x):
     return x
+
+
+# ---------------------------------------------------------------------------------------------------------- operands
+def split(x):
+    """(hi, lo) of the f32 value of x as forward_x3.cu's split2 stores it: hi = bf16 round-to-nearest-even of x, lo = bf16
+    round-to-nearest-even of the f32 difference x - hi (exact in f32)."""
+    x32 = x.float()
+    hi = x32.to(torch.bfloat16)
+    lo = (x32 - hi.float()).to(torch.bfloat16)
+    return hi.double(), lo.double()
+
+
+def split_value(x):
+    """The value a split-stored x carries: hi + lo."""
+    hi, lo = split(x)
+    return hi + lo
+
+
+def tf32_rna(x):
+    """Round the f32 value of x to tf32 (10 explicit mantissa bits), nearest with ties away from zero
+    (cvt.rna.tf32.f32): add half of the dropped 13-bit field to the magnitude bits, then clear the field."""
+    u = x.float().contiguous().view(torch.int32).to(torch.int64) & 0xFFFFFFFF
+    r = (u & 0x80000000) | (((u & 0x7FFFFFFF) + 0x1000) & 0xFFFFE000)
+    r = torch.where(r >= 2 ** 31, r - 2 ** 32, r)                 # back to the int32 bit pattern
+    return r.to(torch.int32).view(torch.float32).double()
+
+
+def is_pair(x):
+    return isinstance(x, tuple)
+
+
+def pair_value(x):
+    return x[0] + x[1] if is_pair(x) else x
+
+
+def pair_map(fn, x):
+    """fn applied to a value or to both halves of a pair (slicing, reshaping, gathering)."""
+    return (fn(x[0]), fn(x[1])) if is_pair(x) else fn(x)
+
+
+def bilinear(fn, x, w):
+    """fn(x, w) in fp64 for a bilinear fn (conv, matmul), and acc = fn(|x|, |w|).  If either operand is a (hi, lo) pair the
+    result is the split-operand product fn(xh, wh) + fn(xl, wh) + fn(xh, wl) (a plain value counts as (value, 0))."""
+    if not (is_pair(x) or is_pair(w)):
+        return fn(x, w), fn(x.abs(), w.abs())
+    xh, xl = x if is_pair(x) else (x, None)
+    wh, wl = w if is_pair(w) else (w, None)
+    y = fn(xh, wh if wl is None else wh + wl)           # xh*wh + xh*wl in one pass (wh + wl is exact in fp64)
+    if xl is not None:
+        y = y + fn(xl, wh)
+    return y, fn(pair_value(x).abs() if xl is None else xh.abs() + xl.abs(),
+                 pair_value(w).abs() if wl is None else wh.abs() + wl.abs())
 
 
 def nchw(x):
@@ -113,8 +172,10 @@ def _conv(x, w_hwio, b=None, padding=1):
 
 
 def _conv_acc(x, w, b, padding=1):
-    y = _conv(x, w, b, padding)
-    acc = _conv(x.abs(), w.abs(), None if b is None else b.abs(), padding)
+    """conv + bias and its accumulation scale; x and w may be split (hi, lo) pairs (see `bilinear`)."""
+    y, acc = bilinear(lambda a, k: _conv(a, k, None, padding), x, w)
+    if b is not None:
+        y, acc = y + b, acc + b.abs()
     return y, acc
 
 
@@ -199,12 +260,13 @@ def conv_bias_stage(x, w, b):
     return dict(out=out, acc=acc)
 
 
-def bn_stats_stage(x_pre, gamma, beta, eps):
+def bn_stats_stage(x_pre, gamma, beta, eps, sums=None):
     """Batch statistics over every position of x_pre [N, H2, 4, C] (kernels.cu: bn_finalize_kernel): sums, mean, population
-    variance, invstd, scale = gamma*invstd, shift = beta - mean*scale."""
+    variance, invstd, scale = gamma*invstd, shift = beta - mean*scale.  sums = (sum, sum of squares): finalize those (the
+    workspace's own f64 sums) instead of x_pre's; the error scales still come from x_pre."""
     x = x_pre.reshape(-1, x_pre.shape[-1])
     cnt = x.shape[0]
-    s1, s2 = x.sum(0), (x * x).sum(0)
+    s1, s2 = (x.sum(0), (x * x).sum(0)) if sums is None else sums
     mean = s1 / cnt
     var = (s2 / cnt - mean * mean).clamp_min(0)
     invstd = 1.0 / torch.sqrt(var + eps)
@@ -241,13 +303,23 @@ def conv5_stage(a4b, w, b):
     return dict(out=y[:, :, 0, :], acc=acc[:, :, 0, :])
 
 
-def xproj_stage(a5, wx_fw, wx_bw, b_fw, b_bw, lens, T, bias_rnd=f32):
+def _forget_one(b):
+    return torch.cat([torch.zeros(2 * HID), torch.ones(HID), torch.zeros(HID)]).to(b.dtype)
+
+
+def xproj_stage(a5, wx_fw, wx_bw, b_fw, b_bw, lens, T, bias_rnd=f32, x3=False):
     """Input projection of both directions for all H2 rows of a5 [N, H2, 512]: z = a5 Wx + b (+1 on the forget gate, added
     in f32 by lstm_bias_prep: `bias_rnd`), gate columns permuted, backward-direction rows reversed by length (rows t >= len,
-    the padding row t = T included, stay)."""
+    the padding row t = T included, stay).  x3: z = a5 Wx only (the f32-class cell adds the bias), natural [i|j|f|o]
+    columns and frame order in both directions; a5 and the weights may be split pairs."""
     outs, accs = [], []
     for d, (wx, b) in enumerate(((wx_fw, b_fw), (wx_bw, b_bw))):
-        bias = bias_rnd(b + torch.cat([torch.zeros(2 * HID), torch.ones(HID), torch.zeros(HID)]).to(b.dtype))
+        if x3:
+            z, acc = bilinear(torch.matmul, a5, wx)
+            outs.append(z)
+            accs.append(acc)
+            continue
+        bias = bias_rnd(b + _forget_one(b))
         z = to_perm(a5 @ wx + bias)
         acc = to_perm(a5.abs() @ wx.abs() + bias.abs())
         if d == 1:
@@ -264,10 +336,17 @@ def _cell(z, c_prev):
     return torch.stack([i, j, f, o], -2), c, o * torch.tanh(c)
 
 
-def recurrence_stage(xproj, wh_fw, wh_bw, lens, T, rnd=bf16):
+def _step_frames(L, s, d):
+    """Frame each row reads at step s (of a [N] or [N, 1] step grid): s forward, len-1-s backward (s where s >= len)."""
+    return torch.where(L > s, (L - 1 - s) if d else s + 0 * L, s + 0 * L)
+
+
+def recurrence_stage(xproj, wh_fw, wh_bw, lens, T, rnd=bf16, biases=None):
     """Both LSTM directions over T steps from the projected inputs `xproj` (workspace layout) and W_h [256, 1024]; h is
-    rounded by `rnd` before it feeds the next step.  Returns lstm_out [N, H2, 512] (frames t >= len and the padding row
-    zero), gates [2, N, T, 4, 256] and c [2, N, T, 256] per STEP (valid for steps < len)."""
+    rounded by `rnd` (to a value) before it feeds the next step.  Returns lstm_out [N, H2, 512] (frames t >= len and the
+    padding row zero), gates [2, N, T, 4, 256] and c [2, N, T, 256] per STEP (valid for steps < len).
+    biases = (b_fw, b_bw) selects the x3 layout (xproj_stage(x3=True)): the step adds the bias and 1 on f itself and reads
+    the xproj row of its own frame; W_h may then be a split pair."""
     N, H2, _ = xproj.shape
     L = torch.as_tensor(clamp_lens(lens, T))
     out = xproj.new_zeros((N, H2, 2 * HID))
@@ -275,15 +354,21 @@ def recurrence_stage(xproj, wh_fw, wh_bw, lens, T, rnd=bf16):
     cs = xproj.new_zeros((2, N, T, HID))
     ar = torch.arange(N)
     for d, wh in enumerate((wh_fw, wh_bw)):
-        xd = from_perm(xproj[..., d * 1024:(d + 1) * 1024])
+        xd = xproj[..., d * 1024:(d + 1) * 1024]
+        if biases is None:
+            xd = from_perm(xd)
         h = xproj.new_zeros((N, HID))
         c = xproj.new_zeros((N, HID))
         for s in range(T):
             act = (s < L)[:, None]
-            g, c_new, h_new = _cell(xd[:, s] + h @ wh, c)
+            t = _step_frames(L, s, d)
+            if biases is None:
+                z = xd[:, s] + h @ wh
+            else:
+                z = xd[ar, t] + bilinear(torch.matmul, h, wh)[0] + biases[d] + _forget_one(biases[d])
+            g, c_new, h_new = _cell(z, c)
             gates[d, :, s] = g
             cs[d, :, s] = c_new
-            t = torch.where(L > s, (L - 1 - s) if d else torch.full_like(L, s), torch.full_like(L, s))
             sel = (s < L)
             out[ar[sel], t[sel], d * HID:(d + 1) * HID] = h_new[sel]
             c = torch.where(act, c_new, c)
@@ -291,10 +376,12 @@ def recurrence_stage(xproj, wh_fw, wh_bw, lens, T, rnd=bf16):
     return dict(out=out, gates=gates, c=cs)
 
 
-def recurrence_steps_isolated(xproj, wh_fw, wh_bw, lstm_out, c_steps, lens, T):
+def recurrence_steps_isolated(xproj, wh_fw, wh_bw, lstm_out, c_steps, lens, T, biases=None):
     """Every recurrence step on its own inputs: z = xproj row + h_prev W_h with h_prev the step's predecessor read back from
     `lstm_out` (the bf16 h the kernel exchanged) and c_prev from the saved cell state `c_steps` [2, N, T, 256].  Returns
-    gates / c [2, N, T, ...] and h [2, N, T, 256] per step (rows of steps >= len meaningless)."""
+    gates / c [2, N, T, ...] and h [2, N, T, 256] per step (rows of steps >= len meaningless).
+    biases = (b_fw, b_bw): the x3 layout (see recurrence_stage); lstm_out and W_h may be split pairs.  c_steps = None
+    (the f32-class path saves no per-step cell state): c is carried in fp64 from step to step, teacher-forced by h only."""
     N = xproj.shape[0]
     L = torch.as_tensor(clamp_lens(lens, T))
     gates = xproj.new_zeros((2, N, T, 4, HID))
@@ -302,25 +389,42 @@ def recurrence_steps_isolated(xproj, wh_fw, wh_bw, lstm_out, c_steps, lens, T):
     hs = xproj.new_zeros((2, N, T, HID))
     s = torch.arange(T)
     for d, wh in enumerate((wh_fw, wh_bw)):
-        xd = from_perm(xproj[:, :T, d * 1024:(d + 1) * 1024])                     # [N, T(step), 1024]
         # frame of step s, and of its predecessor s-1 (h_prev = 0 at s = 0)
         t_of = (L[:, None] - 1 - s[None, :]).clamp_min(0) if d else s[None, :].expand(N, T)
-        ho = lstm_out[..., d * HID:(d + 1) * HID]
-        h_prev = torch.zeros((N, T, HID), dtype=xproj.dtype)
+        if biases is None:
+            xd = from_perm(xproj[:, :T, d * 1024:(d + 1) * 1024])                 # [N, T(step), 1024]
+        else:
+            xd = torch.gather(xproj[..., d * 1024:(d + 1) * 1024], 1, t_of[..., None].expand(N, T, 4 * HID))
+            xd = xd + biases[d] + _forget_one(biases[d])
+        def prev_h(out_d):
+            """h of each step's predecessor from this direction's lstm_out columns [N, H2, 256] (zero at step 0)."""
+            h = torch.zeros((N, T, HID), dtype=xproj.dtype)
+            if T > 1:
+                h[:, 1:] = torch.gather(out_d, 1, t_of[:, :-1, None].expand(N, T - 1, HID))
+            return h
+
+        h_prev = pair_map(lambda v: prev_h(v[..., d * HID:(d + 1) * HID]), lstm_out)   # a pair stays a pair
         c_prev = torch.zeros((N, T, HID), dtype=xproj.dtype)
-        if T > 1:
-            h_prev[:, 1:] = torch.gather(ho, 1, t_of[:, :-1, None].expand(N, T - 1, HID))
+        if T > 1 and c_steps is not None:
             c_prev[:, 1:] = c_steps[d, :, :-1]
-        g, c, h = _cell(xd + h_prev @ wh, c_prev)
+        z = xd + bilinear(torch.matmul, h_prev, wh)[0]
+        if c_steps is not None:
+            g, c, h = _cell(z, c_prev)
+        else:
+            c = xproj.new_zeros((N, HID))
+            g, cc, h = [], [], []
+            for k in range(T):
+                gk, c, hk = _cell(z[:, k], c)
+                g.append(gk); cc.append(c); h.append(hk)
+            g, c, h = torch.stack(g, 1), torch.stack(cc, 1), torch.stack(h, 1)
         gates[d], cs[d], hs[d] = g, c, h
     return dict(gates=gates, c=cs, h=hs)
 
 
 def logits_stage(lstm_out, wl, bl, T):
     """512 -> 64 projection of frames t < T, time-major [T, N, 64] (frames past len see zero rows: the bias alone)."""
-    x = lstm_out[:, :T]
-    y = x @ wl + bl
-    acc = x.abs() @ wl.abs() + bl.abs()
+    y, acc = bilinear(torch.matmul, pair_map(lambda v: v[:, :T], lstm_out), wl)
+    y, acc = y + bl, acc + bl.abs()
     return dict(out=y.permute(1, 0, 2), acc=acc.permute(1, 0, 2))
 
 

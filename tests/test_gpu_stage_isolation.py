@@ -18,10 +18,8 @@ and shape.
 Ties: conv1 picks the first maximum on the f32 accumulators, the other pooled training epilogues on the bf16-rounded
 values, and the pool3 backward re-derives the pair maximum from bf16-rounded BN outputs; the arg-max checks accept any
 position within the bound of the maximum, and the pool3 reference routes by the same bf16 comparison."""
-import json
 import os
 import sys
-import time
 
 import numpy as np
 import pytest
@@ -29,12 +27,12 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import stage_refs as S  # noqa: E402
+from stage_check import SHAPES, ulp_bf16, widths_of  # noqa: E402
+from stage_check import Checker as _Checker  # noqa: E402
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DEV = "cuda:0"
 FW, BW = "logits/bidirectional_rnn/fw/lstm_cell", "logits/bidirectional_rnn/bw/lstm_cell"
-_REPORT_RUN = None          # start time of this session's report (the report file is truncated once per session)
 
 # stage -> (ulps of |ref|, c); c multiplies acc (bf16 / f32 outputs) or max|ref| (recurrence, BPTT)
 STAGE_BOUNDS = {
@@ -57,87 +55,9 @@ STAGE_BOUNDS = {
 # happens to a sizeable share of the elements and leaves up to 3.1e-4 (measured) in these cancelling sums.
 L2_LIMIT = {"bn41_affine": 1.2e-3}
 
-SHAPES = [
-    pytest.param(2, 256, [256, 201], id="N2_W256"),
-    pytest.param(3, 160, [160, 8, 97], id="N3_W160"),
-    pytest.param(5, 80, [80, 4, 8, 57, 33], id="N5_W80"),
-    pytest.param(3, 100, [100, 4, 61], id="N3_W100"),
-    pytest.param(130, 40, "cycle", id="N130_W40"),
-    pytest.param(5, 24, [24, 4, 8, 12, 20], id="N5_W24"),
-]
 
-
-def _widths(N, W, widths):
-    if widths == "cycle":                                  # lengths 0, 1, T and in between, over two 128-row tiles
-        return [[W, 4, 8, 12, 20, 28, 36][i % 7] for i in range(N)]
-    return widths
-
-
-def ulp_bf16(x):
-    a = np.maximum(np.abs(x), 2.0 ** -126)
-    return 2.0 ** (np.floor(np.log2(a)) - 7)
-
-
-class Checker:
-    def __init__(self, case):
-        self.case = case
-        self.fail = []
-        self.rows = []
-
-    def _record(self, stage, ratio, **kv):
-        self.rows.append(dict(case=self.case, stage=stage, max_ratio=float(ratio), **kv))
-        if not ratio <= 1.0:
-            self.fail.append(f"{stage}: max |gpu-ref|/bound = {ratio:.3g} {kv}")
-
-    def close(self, stage, gpu, ref, acc, key=None, mask=None):
-        """bf16 (ulps > 0) or f32 (ulps == 0) output against the fp64 reference, per element."""
-        ulps, c = STAGE_BOUNDS[key or stage]
-        g, r = np.asarray(gpu, np.float64), np.asarray(ref, np.float64)
-        a = np.broadcast_to(np.asarray(acc, np.float64), r.shape)
-        if mask is not None:
-            g, r, a = g[mask], r[mask], a[mask]
-        if r.size == 0:
-            return
-        err = np.abs(g - r)
-        bound = ulps * ulp_bf16(r) + c * a if ulps else c * a + 1e-30
-        ratio = err / bound
-        i = int(np.argmax(ratio))
-        kv = dict(max_abs_err=float(err.max()), worst_gpu=float(g.flat[i]), worst_ref=float(r.flat[i]),
-                  worst_acc=float(a.flat[i]), ulps=ulps, c=c)
-        if not ulps:
-            l2 = float(np.linalg.norm(g - r) / max(np.linalg.norm(r), 1e-30))
-            kv["rel_l2"] = l2
-            lim = L2_LIMIT.get(key or stage, 1e-4)
-            if l2 > lim:
-                self.fail.append(f"{stage}: relative L2 {l2:.3g} > {lim:g}")
-        self._record(stage, float(ratio.max()), **kv)
-
-    def close_scaled(self, stage, gpu, ref, mask=None):
-        """Recurrence / BPTT: bound ulps * ulp(|ref|) + c * max|ref|."""
-        r = np.asarray(ref, np.float64)
-        self.close(stage, gpu, ref, np.abs(r[mask] if mask is not None else r).max(), mask=mask)
-
-    def exact(self, stage, gpu, ref):
-        g, r = np.asarray(gpu), np.asarray(ref)
-        bad = int((g != r).sum())
-        self._record(stage, 0.0 if bad == 0 else float("inf"), mismatches=bad)
-
-    def report(self):
-        """Rows of this test session only: the first report of a session truncates the file, every row carries the
-        session's start time."""
-        global _REPORT_RUN
-        os.makedirs(os.path.join(ROOT, "build"), exist_ok=True)
-        mode = "a" if _REPORT_RUN else "w"
-        if not _REPORT_RUN:
-            _REPORT_RUN = time.strftime("%Y-%m-%dT%H:%M:%S")
-        with open(os.path.join(ROOT, "build", "stage_isolation_report.jsonl"), mode) as f:
-            for row in self.rows:
-                f.write(json.dumps(dict(run=_REPORT_RUN, **row)) + "\n")
-
-    def assert_ok(self):
-        self.report()
-        assert not self.fail, "\n".join(self.fail)
-
+def Checker(case):
+    return _Checker(case, STAGE_BOUNDS, "stage_isolation_report.jsonl", ulp_bf16, L2_LIMIT)
 
 def argmax_check(ck, stage, am, pre, pooled, c):
     """Pool window bytes: in range; where the pooled output is > 0 and the two largest fp64 window values are separated by
@@ -162,7 +82,7 @@ def _setup(N, W, widths, seed=5):
     from lstm_ctc_ocr_b200 import engine
     from oracle import crnn_oracle as O
     pn = O.randomize_params(O.init_params(3, dtype=np.float32, logits_scale=10.0))
-    data, lab, ll, tsl = O.synth_batch(N, W, seed=seed, widths=_widths(N, W, widths), min_len=1, max_len=4)
+    data, lab, ll, tsl = O.synth_batch(N, W, seed=seed, widths=widths_of(N, W, widths), min_len=1, max_len=4)
     m = engine.CrnnModel(device=DEV)
     m.load_params(pn)
     return m, pn, data, tsl

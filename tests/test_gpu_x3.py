@@ -8,7 +8,8 @@ Operands are split into bf16 hi + bf16 lo and multiplied as hi*hi + lo*hi + hi*l
 "tf32": the same orchestration on tf32 wgmma operands (2^-11 per operand, rounded to nearest where produced); stated
 tolerances: taps 4e-3, logits 2.5e-3, loss 5e-4 (SURVEY 7.2(6) asks for 2e-3), decode of the SOFT random-weight lines
 >= 97 % unfiltered (the trained 10k-line fixture: tests/test_gpu_decode10k.py).  Each run appends its measured errors to
-build/parity_report.jsonl."""
+build/parity_report.jsonl.  These whole-chain bounds pin the composition; every single stage of both modes is checked per
+element on its own operands in tests/test_gpu_x3_stage_isolation.py."""
 import json
 import os
 

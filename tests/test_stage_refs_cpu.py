@@ -169,3 +169,161 @@ def test_backward_stage_chain_reproduces_oracle_gradients(chain):
     for k in ("conv4_1/biases", "conv4_2/biases"):
         assert float(G[k].abs().max()) < 1e-12 * float(G[k.replace("biases", "weights")].abs().max()) + 1e-15
     assert len(got) == len(G) - 2
+
+
+# ---------------------------------------------------------------------------------------------------------- f32-class path
+def _zero_pair(x):
+    return (x, torch.zeros_like(x))
+
+
+def test_x3_stage_chain_reproduces_the_oracle(chain):
+    """The f32-class layouts with lo = 0, wl = 0 and identity rounding: split-pair conv / GEMM stages, an input projection
+    without bias in natural gate and frame order, the cell adding the bias and reading frame len-1-step backwards."""
+    c = chain
+    P, A, T, H2, tsl = c["P"], c["A"], c["T"], c["H2"], c["tsl"]
+    Wp = {k: _zero_pair(v) for k, v in P.items() if k.endswith("weights")}
+    for k, src, fn in (("conv2", "conv1", S.conv_relu_pool22_stage), ("conv3_1", "conv2", S.conv_relu_stage),
+                       ("conv3_2", "conv3_1", S.conv_relu_pool12_stage)):
+        assert rel(fn(_zero_pair(A[src]), Wp[f"{k}/weights"], P[f"{k}/biases"])["out"], A[k]) < TOL, k
+    for name, src in (("conv4_1", "conv3_2"), ("conv4_2", "conv4_1")):
+        pre = S.conv_bias_stage(_zero_pair(A[src]), Wp[f"{name}/weights"], P[f"{name}/biases"])["out"]
+        st = S.bn_stats_stage(pre, P[f"{name}/{name}/gamma"], P[f"{name}/{name}/beta"], O.BN_EPS)
+        fn = S.bn_apply_relu_stage if name == "conv4_1" else lambda x, a, b: S.bn_apply_relu_pool_stage(x, a, b, rnd=S.ident)
+        assert rel(fn(pre, st["scale"], st["shift"])["out"], A[name]) < TOL, name
+    assert rel(S.conv5_stage(_zero_pair(A["conv4_2"]), Wp["conv5/weights"], P["conv5/biases"])["out"], A["reshaped_layer"]) < TOL
+    a5 = _pad_rows(A["reshaped_layer"], H2)
+    wx = [S.pair_map(lambda v: v[:512], Wp[f"{s}/weights"]) for s in (FW, BW)]
+    wh = [S.pair_map(lambda v: v[512:], Wp[f"{s}/weights"]) for s in (FW, BW)]
+    biases = (P[f"{FW}/biases"], P[f"{BW}/biases"])
+    xp = S.xproj_stage(_zero_pair(a5), wx[0], wx[1], None, None, tsl, T, x3=True)["out"]
+    # natural layout: plain a5 W_x per direction, no bias, no permutation, no reversal
+    assert rel(xp, torch.cat([a5 @ P[f"{s}/weights"][:512] for s in (FW, BW)], -1)) < TOL
+    rec = S.recurrence_stage(xp, wh[0], wh[1], tsl, T, rnd=S.ident, biases=biases)
+    assert rel(rec["out"], _pad_rows(A["lstm_out"].detach(), H2)) < TOL
+    # the bf16-layout chain gives the same gates and cell states step for step
+    ref = _forward_chain(c)["rec"]
+    assert rel(rec["gates"], ref["gates"]) < TOL and rel(rec["c"], ref["c"]) < TOL
+    assert rel(S.logits_stage(_zero_pair(rec["out"]), Wp["logits/weights"], P["logits/biases"], T)["out"], c["logits"]) < TOL
+    # teacher-forced steps with the cell state carried in fp64 reproduce every active step's h and c
+    iso = S.recurrence_steps_isolated(xp, wh[0], wh[1], _zero_pair(rec["out"]), None, tsl, T, biases=biases)
+    act = torch.arange(T)[None, :] < torch.as_tensor(S.clamp_lens(tsl, T))[:, None]
+    assert rel(iso["c"][:, act], rec["c"][:, act]) < TOL
+    L = S.clamp_lens(tsl, T)
+    for d in range(2):
+        for n in range(c["N"]):
+            for s in range(L[n]):
+                t = (L[n] - 1 - s) if d else s
+                assert rel(iso["h"][d, n, s], rec["out"][n, t, d * 256:(d + 1) * 256]) < TOL
+
+
+def test_split_product_leaves_out_only_lo_times_lo():
+    """A pair against a pair is ah*wh + al*wh + ah*wl = (ah+al)(wh+wl) - al*wl, for convolutions and matmuls alike."""
+    g = torch.Generator().manual_seed(3)
+    x = torch.randn(2, 6, 4, 64, generator=g, dtype=torch.float64)
+    w = torch.randn(3, 3, 64, 32, generator=g, dtype=torch.float64) * 0.1
+    xs, ws = S.split(x), S.split(w)
+    got = S.conv_bias_stage(xs, ws, None)["out"]
+    want = S._conv(xs[0] + xs[1], ws[0] + ws[1]) - S._conv(xs[1], ws[1])
+    assert rel(got, want) < 1e-12
+    a = torch.randn(40, 512, generator=g, dtype=torch.float64)
+    b = torch.randn(512, 96, generator=g, dtype=torch.float64)
+    (ah, al), (bh, bl) = S.split(a), S.split(b)
+    y, acc = S.bilinear(torch.matmul, (ah, al), (bh, bl))
+    assert rel(y, (ah + al) @ (bh + bl) - al @ bl) < 1e-12
+    assert rel(y, ah @ bh + al @ bh + ah @ bl) < 1e-12
+    assert rel(acc, (ah.abs() + al.abs()) @ (bh.abs() + bl.abs())) < 1e-12
+
+
+def test_dropped_term_size():
+    """|lo| <= 2^-8 |x| (half a bf16 ulp), so one dropped al*wl is at most 2^-16 of |a||w| and about 2^-19 on average;
+    summed over a K = 512 contraction with mixed signs it stays below 2^-18 of sum |a||w|."""
+    g = torch.Generator().manual_seed(5)
+    a = torch.randn(512, 512, generator=g, dtype=torch.float64).float().double()
+    w = torch.randn(512, 256, generator=g, dtype=torch.float64).float().double()
+    (ah, al), (wh, wl) = S.split(a), S.split(w)
+    assert float((al.abs() / a.abs()).max()) <= 2.0 ** -8
+    per = (al[:256, :256] * wl[:256]).abs() / (a[:256, :256] * w[:256]).abs()       # 65536 single products
+    assert float(per.max()) <= 2.0 ** -16 and float(per.mean()) <= 2.0 ** -18
+    assert float(((al @ wl).abs() / (a.abs() @ w.abs())).max()) <= 2.0 ** -18
+
+
+def _bits(x):
+    return [int(v) & 0xFFFFFFFF for v in torch.as_tensor(x, dtype=torch.float64).float().view(torch.int32)]
+
+
+def test_split_bit_patterns():
+    """hi = bf16 RNE(x), lo = bf16 RNE(x - hi): ties to even in both halves, signs, powers of two, exact bf16 values."""
+    cases = [
+        (1.0, 0x3F800000, 0x00000000),                                 # power of two: lo = 0
+        (-0.375, 0xBEC00000, 0x00000000),                              # negative, exactly a bf16 value
+        (1 + 2 ** -8, 0x3F800000, 0x3B800000),                         # tie, even hi below: lo = +2^-8
+        (1 + 3 * 2 ** -8, 0x3F820000, 0xBB800000),                     # tie, even hi above: lo = -2^-8
+        (-(1 + 2 ** -8), 0xBF800000, 0xBB800000),                      # negative tie
+        (1 + 2 ** -9 + 2 ** -20, 0x3F800000, 0x3B000000),              # lo rounds away the 2^-20 bit
+        (2.0 ** -30 * (1 + 2 ** -7 + 2 ** -12), 0x30810000, 0x2A800000),   # small exponents: lo = 2^-42
+    ]
+    for x, hi, lo in cases:
+        h, l = S.split(torch.tensor([x], dtype=torch.float64))
+        assert _bits(h) == [hi] and _bits(l) == [lo], (x, hex(_bits(h)[0]), hex(_bits(l)[0]))
+        assert float(h + l) == float(np.float32(x)) or abs(float(h + l) - x) <= 2.0 ** -16 * abs(x)
+
+
+def test_tf32_rna_bit_patterns():
+    """Round to nearest with ties AWAY from zero on the 13 dropped mantissa bits (cvt.rna.tf32.f32)."""
+    cases = [
+        (1.0, 0x3F800000),
+        (1 + 2 ** -11, 0x3F802000),                                     # tie -> away: 1 + 2^-10
+        (1 + 3 * 2 ** -11, 0x3F804000),                                # tie -> away (not to even): 1 + 2^-9
+        (-(1 + 2 ** -11), 0xBF802000),                                 # negative tie -> away from zero
+        (1 + 2 ** -11 - 2 ** -23, 0x3F800000),                         # just below the tie -> down
+        (2.0 - 2 ** -23, 0x40000000),                                  # carries into the exponent
+        (-(2.0 ** -20), 0xB5800000),                                   # power of two, negative: unchanged
+        (0.0, 0x00000000),
+    ]
+    for x, want in cases:
+        got = _bits(S.tf32_rna(torch.tensor([x], dtype=torch.float64)))[0]
+        assert got == want, (x, hex(got), hex(want))
+        assert got & 0x1FFF == 0
+
+
+def _truncate_tf32(x):
+    """What a producer without cvt.rna would store: the low 13 mantissa bits cleared (round toward zero)."""
+    return (x.float().contiguous().view(torch.int32) & ~0x1FFF).view(torch.float32).double()
+
+
+def _truncate_bf16(x):
+    return (x.float().contiguous().view(torch.int32) & ~0xFFFF).view(torch.float32).double()
+
+
+@pytest.mark.parametrize("mode", ["f32", "tf32"])
+def test_x3_storage_checks_reject_a_truncating_store(mode):
+    """The checks the f32-class stage isolation applies to a stored activation hold a round-to-nearest store of an f32 dot
+    product (K = 2304, like conv3_2) and reject the same store with truncation in place of rounding.  tf32: the value
+    bound (half a tf32 ulp + c * acc) fails, while the low 13 bits are zero either way.  Split: a truncated hi leaves a lo
+    that still carries the value, so the value bound (a quarter of the lo-half ulp + c * acc) passes and the canonical-form
+    check fails.  A split store that truncated only lo would err by less than 2^-16 of the value, below the stage's f32
+    accumulation error c * acc, so no per-element check resolves it."""
+    import test_gpu_x3_stage_isolation as X3           # the enforced checks; importing the module needs no GPU
+    from stage_check import Checker
+    g = torch.Generator().manual_seed(9)
+    a = torch.randn(192, 2304, generator=g, dtype=torch.float64)
+    w = torch.randn(2304, 128, generator=g, dtype=torch.float64) * 0.05
+    ref, acc = a @ w, a.abs() @ w.abs()
+    v = ref.float()                                     # an f32 accumulator off by at most 2^-24 |ref|
+    if mode == "tf32":
+        stores = {"rna": S.tf32_rna(v).float(), "truncated": _truncate_tf32(v).float()}
+        value = {k: x.double() for k, x in stores.items()}
+    else:
+        hi_t = _truncate_bf16(v).float()
+        stores = {"rna": torch.stack([t.to(torch.bfloat16) for t in S.split(v)], -2),
+                  "truncated hi": torch.stack([hi_t.to(torch.bfloat16), (v - hi_t).to(torch.bfloat16)], -2)}
+        value = {k: x[..., 0, :].double() + x[..., 1, :].double() for k, x in stores.items()}
+    for name, raw in stores.items():
+        ck = Checker(name, X3.BOUNDS[mode], ulp=X3.STORAGE_ULP[mode])
+        ck.close("conv3_2", value[name], ref, acc)
+        X3._canonical(ck, mode, "conv3_2", raw)
+        if name == "rna":
+            assert not ck.fail, ck.fail
+        else:
+            assert ck.fail, (name, ck.rows)
+            assert ck.fail[0].startswith("conv3_2: " if mode == "tf32" else "conv3_2_canonical"), ck.fail

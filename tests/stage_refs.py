@@ -1,14 +1,15 @@
 """fp64 restatements of every stage of the bf16 forward and backward path, each on that stage's OWN inputs.
 
 A stage function takes the operands the kernel reads (bf16 activations / gradients read back from the workspace, weights
-rounded to bf16 as prepare_weights() rounds them, f32 biases) as fp64 CPU tensors in the workspace layouts (NHWC, permuted
+rounded to bf16 as prepare_weights() rounds them, f32 biases) as fp64 tensors, on any one device, in the workspace layouts (NHWC, permuted
 LSTM gate columns, reversed backward-direction rows, time-major logits) and returns the stage's output computed in fp64.
 With the kernel's own inputs the only legitimate differences are the order of the f32 accumulation and the final rounding,
 so a test can bound each element by about one bf16 ulp plus a small multiple of `acc`: the same operation applied to
 |inputs| and |weights|, i.e. the scale the accumulation error is relative to.
 
 Data and weight gradients are written as tiny fp64 torch functions differentiated by torch.autograd.grad with the GPU's own
-upstream gradient as grad_outputs; `acc` is the same vector-Jacobian product on absolute values.
+upstream gradient as grad_outputs; `acc` is the same vector-Jacobian product on absolute values.  The BatchNorm backwards
+are written out, so that a batch can be evaluated in image chunks: their batch sums (bn_sums, bn_bwd_sums) add over chunks.
 
 `rnd` is the rounding the kernels apply INSIDE a stage (the bf16 h a recurrence step exchanges, the bf16 values the pool3
 backward compares).  The GPU tests pass `bf16`; tests/test_stage_refs_cpu.py passes `ident` and chains the stages from the
@@ -104,23 +105,23 @@ def nhwc(x):
 
 
 # ---------------------------------------------------------------------------------------------------------- layouts
-def gate_perm(upc=UPC):
+def gate_perm(upc=UPC, device=None):
     """TF gate column j = g*256 + u  ->  its column in the permuted [1024] layout (kernels.cu: lstm_perm)."""
-    j = np.arange(4 * HID)
+    j = torch.arange(4 * HID, device=device)
     g, u = j // HID, j % HID
-    return torch.as_tensor((u // upc) * 4 * upc + g * upc + u % upc)
+    return (u // upc) * 4 * upc + g * upc + u % upc
 
 
 def to_perm(z):
     """[..., 1024] TF gate order -> permuted column order."""
     out = torch.empty_like(z)
-    out[..., gate_perm()] = z
+    out[..., gate_perm(device=z.device)] = z
     return out
 
 
 def from_perm(z):
     """[..., 1024] permuted column order -> TF gate order."""
-    return z[..., gate_perm()]
+    return z[..., gate_perm(device=z.device)]
 
 
 def clamp_lens(lens, T):
@@ -129,11 +130,22 @@ def clamp_lens(lens, T):
 
 def reverse_rows(x, lens, T):
     """tf.reverse_sequence over axis 1 of [N, H2, C]: row t < len goes to len-1-t, rows t >= len stay (an involution)."""
-    y = x.clone()
-    for n, L in enumerate(clamp_lens(lens, T)):
-        if L > 0:
-            y[n, :L] = x[n, :L].flip(0)
-    return y
+    L = torch.as_tensor(clamp_lens(lens, T), device=x.device)[:, None]
+    t = torch.arange(x.shape[1], device=x.device)[None, :]
+    src = torch.where(t < L, L - 1 - t, t)
+    return torch.gather(x, 1, src[..., None].expand(x.shape))
+
+
+def step_h(lstm_out, lens, T):
+    """The h each recurrence step wrote, from lstm_out [N, H2, 512]: [2 dirs, N, T steps, 256], step s of the backward
+    direction at frame len-1-s (rows of steps >= len meaningless)."""
+    N = lstm_out.shape[0]
+    L = torch.as_tensor(clamp_lens(lens, T), device=lstm_out.device)
+    out = []
+    for d in range(2):
+        t = _step_frames(L[:, None], torch.arange(T, device=lstm_out.device)[None, :], d)
+        out.append(torch.gather(lstm_out[..., d * HID:(d + 1) * HID], 1, t[..., None].expand(N, T, HID)))
+    return torch.stack(out)
 
 
 def unpack_gates(g, N):
@@ -198,7 +210,7 @@ def first_argmax(v):
     """Index of the FIRST maximum along the last axis."""
     m = v.max(dim=-1, keepdim=True).values
     k = v.shape[-1]
-    idx = torch.arange(k).expand_as(v)
+    idx = torch.arange(k, device=v.device).expand_as(v)
     return torch.where(v == m, idx, torch.full_like(idx, k)).min(dim=-1).values
 
 
@@ -260,13 +272,21 @@ def conv_bias_stage(x, w, b):
     return dict(out=out, acc=acc)
 
 
-def bn_stats_stage(x_pre, gamma, beta, eps, sums=None):
+def bn_sums(x_pre):
+    """The batch sums BatchNorm statistics come from, additive over image chunks: sum, sum of squares and sum of |x| per
+    channel over every position of x_pre [N, H2, 4, C], and the count."""
+    x = x_pre.reshape(-1, x_pre.shape[-1])
+    return dict(sum=x.sum(0), sumsq=(x * x).sum(0), sum_acc=x.abs().sum(0), cnt=x.shape[0])
+
+
+def bn_stats_stage(x_pre, gamma, beta, eps, sums=None, parts=None):
     """Batch statistics over every position of x_pre [N, H2, 4, C] (kernels.cu: bn_finalize_kernel): sums, mean, population
     variance, invstd, scale = gamma*invstd, shift = beta - mean*scale.  sums = (sum, sum of squares): finalize those (the
-    workspace's own f64 sums) instead of x_pre's; the error scales still come from x_pre."""
-    x = x_pre.reshape(-1, x_pre.shape[-1])
-    cnt = x.shape[0]
-    s1, s2 = (x.sum(0), (x * x).sum(0)) if sums is None else sums
+    workspace's own f64 sums) instead of x_pre's; the error scales still come from x_pre.  parts = bn_sums() added over
+    the image chunks of a batch stands for x_pre's (x_pre is then not read)."""
+    p = bn_sums(x_pre) if parts is None else parts
+    cnt = p["cnt"]
+    s1, s2 = (p["sum"], p["sumsq"]) if sums is None else sums
     mean = s1 / cnt
     var = (s2 / cnt - mean * mean).clamp_min(0)
     invstd = 1.0 / torch.sqrt(var + eps)
@@ -274,11 +294,11 @@ def bn_stats_stage(x_pre, gamma, beta, eps, sums=None):
     # error scales of the coefficients derived from (slightly perturbed) sums: the mean cancels down from sum|x| / cnt, the
     # variance E[x^2] - mean^2 amplifies relative errors of the sums by E[x^2] / var, and the shift cancels beta against
     # mean * scale
-    mean_acc = x.abs().sum(0) / cnt
+    mean_acc = p["sum_acc"] / cnt
     cond = (s2 / cnt) / (var + eps)
     acc = dict(mean=mean_acc, invstd=invstd.abs() * cond, scale=scale.abs() * cond,
                shift=beta.abs() + scale.abs() * (mean_acc + mean.abs() * cond))
-    return dict(sum=s1, sumsq=s2, sum_acc=x.abs().sum(0), mean=mean, var=var, invstd=invstd, scale=scale,
+    return dict(sum=s1, sumsq=s2, sum_acc=p["sum_acc"], mean=mean, var=var, invstd=invstd, scale=scale,
                 shift=beta - mean * scale, acc=acc)
 
 
@@ -304,7 +324,7 @@ def conv5_stage(a4b, w, b):
 
 
 def _forget_one(b):
-    return torch.cat([torch.zeros(2 * HID), torch.ones(HID), torch.zeros(HID)]).to(b.dtype)
+    return torch.cat([torch.zeros(2 * HID), torch.ones(HID), torch.zeros(HID)]).to(b.device, b.dtype)
 
 
 def xproj_stage(a5, wx_fw, wx_bw, b_fw, b_bw, lens, T, bias_rnd=f32, x3=False):
@@ -348,11 +368,11 @@ def recurrence_stage(xproj, wh_fw, wh_bw, lens, T, rnd=bf16, biases=None):
     biases = (b_fw, b_bw) selects the x3 layout (xproj_stage(x3=True)): the step adds the bias and 1 on f itself and reads
     the xproj row of its own frame; W_h may then be a split pair."""
     N, H2, _ = xproj.shape
-    L = torch.as_tensor(clamp_lens(lens, T))
+    L = torch.as_tensor(clamp_lens(lens, T), device=xproj.device)
     out = xproj.new_zeros((N, H2, 2 * HID))
     gates = xproj.new_zeros((2, N, T, 4, HID))
     cs = xproj.new_zeros((2, N, T, HID))
-    ar = torch.arange(N)
+    ar = torch.arange(N, device=xproj.device)
     for d, wh in enumerate((wh_fw, wh_bw)):
         xd = xproj[..., d * 1024:(d + 1) * 1024]
         if biases is None:
@@ -383,11 +403,11 @@ def recurrence_steps_isolated(xproj, wh_fw, wh_bw, lstm_out, c_steps, lens, T, b
     biases = (b_fw, b_bw): the x3 layout (see recurrence_stage); lstm_out and W_h may be split pairs.  c_steps = None
     (the f32-class path saves no per-step cell state): c is carried in fp64 from step to step, teacher-forced by h only."""
     N = xproj.shape[0]
-    L = torch.as_tensor(clamp_lens(lens, T))
+    L = torch.as_tensor(clamp_lens(lens, T), device=xproj.device)
     gates = xproj.new_zeros((2, N, T, 4, HID))
     cs = xproj.new_zeros((2, N, T, HID))
     hs = xproj.new_zeros((2, N, T, HID))
-    s = torch.arange(T)
+    s = torch.arange(T, device=xproj.device)
     for d, wh in enumerate((wh_fw, wh_bw)):
         # frame of step s, and of its predecessor s-1 (h_prev = 0 at s = 0)
         t_of = (L[:, None] - 1 - s[None, :]).clamp_min(0) if d else s[None, :].expand(N, T)
@@ -398,13 +418,13 @@ def recurrence_steps_isolated(xproj, wh_fw, wh_bw, lstm_out, c_steps, lens, T, b
             xd = xd + biases[d] + _forget_one(biases[d])
         def prev_h(out_d):
             """h of each step's predecessor from this direction's lstm_out columns [N, H2, 256] (zero at step 0)."""
-            h = torch.zeros((N, T, HID), dtype=xproj.dtype)
+            h = xproj.new_zeros((N, T, HID))
             if T > 1:
                 h[:, 1:] = torch.gather(out_d, 1, t_of[:, :-1, None].expand(N, T - 1, HID))
             return h
 
         h_prev = pair_map(lambda v: prev_h(v[..., d * HID:(d + 1) * HID]), lstm_out)   # a pair stays a pair
-        c_prev = torch.zeros((N, T, HID), dtype=xproj.dtype)
+        c_prev = xproj.new_zeros((N, T, HID))
         if T > 1 and c_steps is not None:
             c_prev[:, 1:] = c_steps[d, :, :-1]
         z = xd + bilinear(torch.matmul, h_prev, wh)[0]
@@ -449,9 +469,9 @@ def bptt_stage(d_out, gates, c_steps, wh_fw, wh_bw, lens, T, dz_in=None, rnd=bf1
     `dz_in` (the workspace's dz_all: the bf16 values the kernel exchanged) when given, else rnd(own result).
     Returns dz_all [N, H2, 2048] in frame order with permuted gate columns (zero for frames >= len)."""
     N, H2, _ = d_out.shape
-    L = torch.as_tensor(clamp_lens(lens, T))
+    L = torch.as_tensor(clamp_lens(lens, T), device=d_out.device)
     dz_all = d_out.new_zeros((N, H2, 2048))
-    ar = torch.arange(N)
+    ar = torch.arange(N, device=d_out.device)
     for d, wh in enumerate((wh_fw, wh_bw)):
         dz_next = d_out.new_zeros((N, 1024))
         dc_next = d_out.new_zeros((N, HID))
@@ -467,7 +487,7 @@ def bptt_stage(d_out, gates, c_steps, wh_fw, wh_bw, lens, T, dz_in=None, rnd=bf1
             dc = dc_next * f_next + dh * o * (1 - tc * tc)
             dz = torch.cat([dc * j * i * (1 - i), dc * i * (1 - j * j), dc * c_prev * f * (1 - f), dh * tc * o * (1 - o)], -1)
             m = act[:, None]                 # select, never multiply: saved gates of inactive steps are never written
-            zero = torch.zeros((), dtype=dz.dtype)
+            zero = dz.new_zeros(())
             dz = torch.where(m, dz, zero)
             dz_all[ar[act], t[act], d * 1024:(d + 1) * 1024] = to_perm(dz)[act]
             if dz_in is not None:
@@ -493,7 +513,7 @@ def lstm_grads_stage(dz_all, a5, lstm_out, wx_fw, wx_bw, wh_fw, wh_bw):
         else:
             hp[:, :-1] = ho[:, 1:]
         fn = lambda x, h, a, b, bias: x @ a + h @ b + bias
-        (dx, _, dwx, dwh, db), (ax, _, awx, awh, ab) = vjp_acc(fn, [a5, hp, wx, wh, torch.zeros(1024, dtype=a5.dtype)], dz)
+        (dx, _, dwx, dwh, db), (ax, _, awx, awh, ab) = vjp_acc(fn, [a5, hp, wx, wh, a5.new_zeros(1024)], dz)
         key = "fw" if d == 0 else "bw"
         out[key + "/weights"] = torch.cat([dwx, dwh], 0)
         out[key + "/weights_acc"] = torch.cat([awx, awh], 0)
@@ -518,68 +538,78 @@ def conv5_bwd(d_a5, a4b, w):
     return conv_bwd(d_a5[:, :T, None, :], a4b, w, padding=0)
 
 
-def _bn_bwd_acc(dy_abs, x, xhat, invstd, gamma, red):
-    """Scale of dx = gamma*invstd*(dy - mean(dy) - xhat*mean(dy*xhat)) summed in absolute values.  The kernels evaluate it
-    as A*dy + B + C*x with f32 coefficients (backward_kernels.cu: bn_bwd_coef_kernel), where B and C*x cancel down to the
-    centred term; the 2^-8 share of |B| + |C*x| lets a 2^-16 * acc bound cover their f32 rounding (2^-24)."""
-    m1 = dy_abs.mean(red, keepdim=True)
-    m2 = (dy_abs * xhat.abs()).mean(red, keepdim=True)
-    mu = x.mean(red, keepdim=True)
-    cx = (gamma * invstd * invstd).abs() * m2 * (x.abs() + mu.abs())
-    return (gamma * invstd).abs() * (dy_abs + m1 + xhat.abs() * m2) + 2.0 ** -8 * cx
+def bn_batch(x_pre, eps, parts=None):
+    """fp64 batch mean and invstd of x_pre [N, H2, 4, C] (from bn_sums() over the whole batch when given as `parts`)."""
+    p = bn_sums(x_pre) if parts is None else parts
+    mean = p["sum"] / p["cnt"]
+    var = (p["sumsq"] / p["cnt"] - mean * mean).clamp_min(0)
+    return dict(mean=mean, invstd=1.0 / torch.sqrt(var + eps), cnt=p["cnt"])
 
 
-def bn_relu_pool_bwd_stage(d_pooled, x_pre, bn, gamma, beta, eps, rnd=bf16):
-    """BN4_2 + ReLU + pool3 backward: x_pre [N, H2, 4, C] pre-BN, d_pooled [N, H2, 2, C], bn [4, C] = the workspace's
-    scale, shift, mean, invstd.  The pooled gradient goes to the FIRST position of the pair whose rnd(max(x*scale+shift, 0))
-    is the larger (the forward rounded each position before taking the max), and only where that max is > 0.  The BN itself
-    is differentiated in fp64 with the statistics recomputed from x_pre."""
-    sc, sh = bn[0], bn[1]
-    yq = windows12(rnd(torch.relu(x_pre * sc + sh)))
+def bn_bwd_sums(dy, dy_acc, x_pre, stats):
+    """The batch reductions of a BatchNorm backward, additive over image chunks: d beta = sum dy, d gamma = sum dy*xhat
+    and the same on the accumulation scale dy_acc of dy (at least |dy|)."""
+    xhat = (x_pre - stats["mean"]) * stats["invstd"]
+    red = (0, 1, 2)
+    return dict(dbeta=dy.sum(red), dgamma=(dy * xhat).sum(red), dbeta_acc=dy_acc.sum(red),
+                dgamma_acc=(dy_acc * xhat.abs()).sum(red))
+
+
+def _bn_bwd(dy, dy_acc, x_pre, gamma, eps, stats, sums):
+    """dx = gamma*invstd*(dy - mean(dy) - xhat*mean(dy*xhat)) with the batch statistics and sums of the whole batch (of
+    dy's own images when not given), and its scale summed in absolute values.  The kernels evaluate it as A*dy + B + C*x
+    with f32 coefficients (backward_kernels.cu: bn_bwd_coef_kernel), where B and C*x cancel down to the centred term; the
+    2^-8 share of |B| + |C*x| lets a 2^-16 * acc bound cover their f32 rounding (2^-24)."""
+    stats = bn_batch(x_pre, eps) if stats is None else stats
+    sums = bn_bwd_sums(dy, dy_acc, x_pre, stats) if sums is None else sums
+    mean, invstd, cnt = stats["mean"], stats["invstd"], stats["cnt"]
+    xhat = (x_pre - mean) * invstd
+    dx = gamma * invstd * (dy - sums["dbeta"] / cnt - xhat * (sums["dgamma"] / cnt))
+    m1, m2 = sums["dbeta_acc"] / cnt, sums["dgamma_acc"] / cnt
+    cx = (gamma * invstd * invstd).abs() * m2 * (x_pre.abs() + mean.abs())
+    acc = (gamma * invstd).abs() * (dy_acc + m1 + xhat.abs() * m2) + 2.0 ** -8 * cx
+    return dict(dx=dx, dx_acc=acc, **sums)
+
+
+def bn_relu_pool_route(d_pooled, x_pre, bn, rnd=bf16):
+    """The gradient at the BN4_2 output: the pooled gradient d_pooled [N, H2, 2, C] goes to the FIRST position of the pair
+    whose rnd(max(x*scale+shift, 0)) is the larger (the forward rounded each position before taking the max), and only
+    where that max is > 0; bn = the workspace's scale, shift."""
+    yq = windows12(rnd(torch.relu(x_pre * bn[0] + bn[1])))
     first = yq[..., 0] >= yq[..., 1]
     pos = torch.maximum(yq[..., 0], yq[..., 1]) > 0
     mask = torch.stack([first & pos, ~first & pos], -1).to(x_pre.dtype)       # [N, H2, 2, C, 2]
-
-    def fn(x, g, b):
-        mean = x.mean((0, 1, 2))
-        var = x.var((0, 1, 2), unbiased=False)
-        y = windows12((x - mean) / torch.sqrt(var + eps) * g + b)
-        return (y * mask).sum(-1)
-
-    dx, dg, db = vjp(fn, [x_pre, gamma, beta], d_pooled)
     N, H2, W4, C = x_pre.shape
-    dyr = (d_pooled[..., None] * mask).permute(0, 1, 2, 4, 3).reshape(N, H2, W4, C)
-    invstd = 1.0 / torch.sqrt(x_pre.var((0, 1, 2), unbiased=False) + eps)
-    xhat = (x_pre - x_pre.mean((0, 1, 2))) * invstd
-    acc = _bn_bwd_acc(dyr.abs(), x_pre, xhat, invstd, gamma, (0, 1, 2))
-    return dict(dx=dx, dx_acc=acc, dgamma=dg, dbeta=db, dgamma_acc=(dyr * xhat).abs().sum((0, 1, 2)),
-                dbeta_acc=dyr.abs().sum((0, 1, 2)))
+    return (d_pooled[..., None] * mask).permute(0, 1, 2, 4, 3).reshape(N, H2, W4, C)
 
 
-def conv_bn_relu_bwd_stage(dy, x_pre, bn, gamma, beta, w, eps, mask=None, rnd=bf16):
-    """conv4_2 data gradient + conv4_1's ReLU mask + BN4_1 backward as one stage (the workspace's d_pre4a is overwritten in
-    place by the BN apply): x_pre [N, H2, 4, 512] pre-BN conv4_1, dy = d_pre4b.  The data gradient is stored as bf16 and
-    both BN passes read that (`rnd`).  The ReLU mask defaults to x*scale + shift > 0 on the workspace's f32 scale / shift
-    (what the forward applied)."""
+def bn_relu_pool_bwd_stage(d_pooled, x_pre, bn, gamma, eps, rnd=bf16, stats=None, sums=None):
+    """BN4_2 + ReLU + pool3 backward: x_pre [N, H2, 4, C] pre-BN, d_pooled [N, H2, 2, C], bn [4, C] = the workspace's
+    scale, shift, mean, invstd.  The gradient is routed by bn_relu_pool_route; the BN itself is differentiated in fp64 with
+    the statistics recomputed from x_pre.  Over image chunks of a batch, stats = bn_batch() of the whole batch and sums =
+    bn_bwd_sums() added over its chunks (the dgamma / dbeta returned are then those of the whole batch)."""
+    dyr = bn_relu_pool_route(d_pooled, x_pre, bn, rnd)
+    return _bn_bwd(dyr, dyr.abs(), x_pre, gamma, eps, stats, sums)
+
+
+def conv_relu_dgrad(dy, x_pre, bn, w, mask=None, rnd=bf16):
+    """conv4_2's data gradient of dy = d_pre4b, stored as bf16 (`rnd`) and masked by conv4_1's ReLU: x*scale + shift > 0
+    on the workspace's f32 scale / shift (what the forward applied) unless `mask` is given.  Returns it and its
+    accumulation scale: the dgrad sum on absolute values plus one bf16 ulp of the stored gradient (its rounding may fall
+    either way where the f32 and fp64 sums straddle a rounding boundary)."""
     if mask is None:
         mask = (f32(x_pre * bn[0] + bn[1]) > 0).to(x_pre.dtype)
     (g,), (g_abs,) = vjp_acc(lambda a: _conv(a, w), [torch.zeros_like(x_pre)], dy)
     g = rnd(g) * mask
+    return g, g_abs * mask + 2.0 ** 9 * g.abs()
 
-    def fn(x, ga, b):
-        mean = x.mean((0, 1, 2))
-        var = x.var((0, 1, 2), unbiased=False)
-        return (x - mean) / torch.sqrt(var + eps) * ga + b
 
-    dx, dg, db = vjp(fn, [x_pre, gamma, beta], g)
-    # accumulation scale: the dgrad sum on absolute values plus one bf16 ulp of the stored gradient (its rounding may fall
-    # either way where the f32 and fp64 sums straddle a rounding boundary), then the BN backward on that
-    invstd = 1.0 / torch.sqrt(x_pre.var((0, 1, 2), unbiased=False) + eps)
-    xhat = (x_pre - x_pre.mean((0, 1, 2))) * invstd
-    g_acc = g_abs * mask + 2.0 ** 9 * g.abs()
-    acc = _bn_bwd_acc(g_acc, x_pre, xhat, invstd, gamma, (0, 1, 2))
-    return dict(dx=dx, dx_acc=acc, dgamma=dg, dbeta=db, dgamma_acc=(g_acc * xhat.abs()).sum((0, 1, 2)),
-                dbeta_acc=g_acc.sum((0, 1, 2)))
+def conv_bn_relu_bwd_stage(dy, x_pre, bn, gamma, w, eps, mask=None, rnd=bf16, stats=None, sums=None):
+    """conv4_2 data gradient + conv4_1's ReLU mask + BN4_1 backward as one stage (the workspace's d_pre4a is overwritten in
+    place by the BN apply): x_pre [N, H2, 4, 512] pre-BN conv4_1, dy = d_pre4b, the gradient from conv_relu_dgrad; stats /
+    sums as in bn_relu_pool_bwd_stage."""
+    g, g_acc = conv_relu_dgrad(dy, x_pre, bn, w, mask, rnd)
+    return _bn_bwd(g, g_acc, x_pre, gamma, eps, stats, sums)
 
 
 def unpool_stage(d_pooled, pooled, am, win):

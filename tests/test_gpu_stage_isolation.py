@@ -3,7 +3,9 @@
 Each stage's inputs are its OWN bf16 operands read back from the workspace (crnn_debug_tap / crnn_debug_tap_raw), so the
 only legitimate differences from tests/stage_refs.py are the order of the f32 accumulation and the final rounding.  Error
 does not compound from layer to layer, and a wrong element fails wherever it sits.  The whole-chain tests
-(test_gpu_parity.py, test_gpu_shapes.py, test_gpu_training.py) pin the composition; these pin the kernels.
+(test_gpu_parity.py, test_gpu_shapes.py, test_gpu_training.py) pin the composition; these pin the kernels.  The shapes
+here hold at most 130 images; test_gpu_stage_isolation_batch.py runs the same checks (_run_stage_checks, _forward_checks)
+at the batch sizes the project runs, the inference plan included.
 
 Per-element bounds (ratio = |gpu - ref| / bound must be <= 1):
   bf16 outputs:  ulp_bf16(|ref|) + c * acc      (acc: the same operation on |inputs| and |weights|)
@@ -61,16 +63,17 @@ def Checker(case):
 
 def argmax_check(ck, stage, am, pre, pooled, c):
     """Pool window bytes: in range; where the pooled output is > 0 and the two largest fp64 window values are separated by
-    more than the bf16 bound, the byte is the first fp64 arg-max; otherwise it points at a value within the bound of the max."""
-    am = np.asarray(am).astype(np.int64)
+    more than the bf16 bound, the byte is the first fp64 arg-max; otherwise it points at a value within the bound of the max.
+    Torch tensors on one device."""
+    am = am.long()
     win = pre.shape[-1]
     bad_range = int((am >= win).sum())
-    srt = np.sort(pre, axis=-1)
+    srt = pre.sort(-1).values
     mx, second = srt[..., -1], srt[..., -2]
     bound = ulp_bf16(mx) + c
-    first = np.argmax(pre, axis=-1)
-    chosen = np.take_along_axis(pre, np.minimum(am, win - 1)[..., None], -1)[..., 0]
-    live = np.asarray(pooled) > 0
+    first = S.first_argmax(pre)
+    chosen = torch.gather(pre, -1, am.clamp_max(win - 1)[..., None])[..., 0]
+    live = pooled > 0
     clear = live & (mx - second > bound)
     wrong_clear = int((clear & (am != first)).sum())
     wrong_near = int((live & ~clear & (mx - chosen > bound)).sum())
@@ -85,160 +88,229 @@ def _setup(N, W, widths, seed=5):
     data, lab, ll, tsl = O.synth_batch(N, W, seed=seed, widths=widths_of(N, W, widths), min_len=1, max_len=4)
     m = engine.CrnnModel(device=DEV)
     m.load_params(pn)
-    return m, pn, data, tsl
+    return m, pn, data, lab, ll, tsl
 
 
-def _run_stage_checks(case, N, W, widths):
-    m, pn, data, tsl = _setup(N, W, widths)
-    T, H2 = W // 4 - 1, W // 4
+FWD_TAPS = ("conv1", "conv2", "conv3_1", "conv3_2", "a4a_pre", "conv4_1", "a4b_pre", "conv4_2", "conv5", "xproj", "lstm_out")
+BWD_TAPS = ("dl_rows", "d_lstm_out", "dz_all", "d_a5", "d_a4b", "d_pre4b", "d_pre4a", "d_a3p", "d_pre32", "d_pre31", "d_a2",
+            "d_pre2", "d_a1")
+EPS = float(np.float32(1e-3))
+
+
+def _sum_into(tot, r):
+    """Add one image chunk's batch reductions r (name -> tensor) into tot."""
+    for k, v in r.items():
+        tot[k] = tot[k] + v if k in tot else v
+
+
+class _Refs:
+    """The operands of one checked batch: the GPU's taps (f32 on the GPU, fp64 on `dev` one image chunk at a time), the
+    parameters on `dev`, and the image chunks the references are evaluated over."""
+
+    def __init__(self, pn, G, R, data, tsl, logits, N, W, dev, chunk):
+        self.pn, self.G, self.data, self.logits, self.dev = pn, G, data, logits, dev
+        self.R = {k: v.to(dev) for k, v in R.items()}
+        self.N, self.T, self.H2 = N, W // 4 - 1, W // 4
+        self.tsl = np.asarray(tsl)
+        self.L = torch.as_tensor(S.clamp_lens(tsl, self.T), device=dev)
+        self.P = {k: torch.as_tensor(np.asarray(v, np.float64)).to(dev) for k, v in pn.items()}
+        self.Wb = {k: S.bf16(v) for k, v in self.P.items() if k.endswith("weights")}
+        self.wh = (self.Wb[FW + "/weights"][512:], self.Wb[BW + "/weights"][512:])
+        self.parts = [slice(i, min(i + (chunk or N), N)) for i in range(0, N, chunk or N)]
+
+    def g(self, k, s):
+        return self.G[k][s].to(self.dev, torch.float64)
+
+    def steps(self, k, s):                     # unpacked saved gates / cell state [2, n, T, ...] of the images s
+        return self.G[k][:, s].to(self.dev, torch.float64)
+
+    def x(self, s):
+        return torch.as_tensor(self.data[s], dtype=torch.float64, device=self.dev)
+
+    def valid(self, s):                        # [n, H2]: frames t < len
+        return torch.arange(self.H2, device=self.dev)[None, :] < self.L[s][:, None]
+
+
+def _forward_checks(ck, F_, train=True):
+    """Every forward stage on its own inputs, image chunk by image chunk; the BatchNorm sums and coefficients from the sums
+    over all chunks.  train: also the arg-max bytes and the isolated recurrence steps on the saved gates / cell state.
+    Returns the BatchNorm partial sums of both layers' pre-activations."""
+    P, Wb, T, dev = F_.P, F_.Wb, F_.T, F_.dev
+    g, R = F_.g, F_.R
+    bn = R["bn"].double()
+    bnp = [{}, {}]
+    for s in F_.parts:
+        lens, Ls = F_.tsl[s], F_.L[s]
+        r = S.conv1_stage(F_.x(s), P["conv1/weights"], P["conv1/biases"])
+        ck.close("conv1", g("conv1", s), r["out"], r["acc"])
+        if train:
+            argmax_check(ck, "am1", R["am1"][s], S.windows22(r["pre"]), g("conv1", s), 2 ** -15 * r["acc"])
+        r = S.conv_relu_pool22_stage(g("conv1", s), Wb["conv2/weights"], P["conv2/biases"])
+        ck.close("conv2", g("conv2", s), r["out"], r["acc"])
+        if train:
+            argmax_check(ck, "am2", R["am2"][s], S.windows22(r["pre"]), g("conv2", s), 2 ** -16 * r["acc"])
+        r = S.conv_relu_stage(g("conv2", s), Wb["conv3_1/weights"], P["conv3_1/biases"])
+        ck.close("conv3_1", g("conv3_1", s), r["out"], r["acc"])
+        r = S.conv_relu_pool12_stage(g("conv3_1", s), Wb["conv3_2/weights"], P["conv3_2/biases"])
+        ck.close("conv3_2", g("conv3_2", s), r["out"], r["acc"])
+        if train:
+            argmax_check(ck, "am3", R["am3"][s], S.windows12(r["pre"]), g("conv3_2", s), 2 ** -16 * r["acc"])
+        del r
+        for li, (name, src, pre, out) in enumerate((("conv4_1", "conv3_2", "a4a_pre", "conv4_1"),
+                                                    ("conv4_2", "conv4_1", "a4b_pre", "conv4_2"))):
+            r = S.conv_bias_stage(g(src, s), Wb[f"{name}/weights"], P[f"{name}/biases"])
+            ck.close(pre, g(pre, s), r["out"], r["acc"])
+            _sum_into(bnp[li], S.bn_sums(g(pre, s)))
+            if li == 0:
+                r = S.bn_apply_relu_stage(g(pre, s), bn[0, 0], bn[0, 1])
+            else:
+                r = S.bn_apply_relu_pool_stage(g(pre, s), bn[1, 0], bn[1, 1])
+            ck.close(out, g(out, s), r["out"], r["acc"] * 2 ** -8)        # one f32 fma, then the bf16 rounding: <= 1 ulp
+        r = S.conv5_stage(g("conv4_2", s), Wb["conv5/weights"], P["conv5/biases"])
+        ck.close("conv5", g("conv5", s)[:, :T], r["out"], r["acc"])
+        r = S.xproj_stage(g("conv5", s), Wb[FW + "/weights"][:512], Wb[BW + "/weights"][:512], P[FW + "/biases"],
+                          P[BW + "/biases"], lens, T)
+        ck.close("xproj", g("xproj", s), r["out"], r["acc"])
+        r = S.recurrence_stage(g("xproj", s), F_.wh[0], F_.wh[1], lens, T)
+        valid = F_.valid(s)
+        ck.exact("lstm_out_past_len_zero", g("lstm_out", s)[~valid], 0.0)
+        ck.close_scaled("lstm_out", g("lstm_out", s), r["out"], mask=valid[..., None].expand(r["out"].shape))
+        if train:
+            gates, csave = F_.steps("gates_steps", s), F_.steps("csave_steps", s)
+            iso = S.recurrence_steps_isolated(g("xproj", s), F_.wh[0], F_.wh[1], g("lstm_out", s), csave, lens, T)
+            act2 = (torch.arange(T, device=dev)[None, :] < Ls[:, None])[None].expand(2, -1, -1)
+            ck.close_scaled("step_gates", gates[act2], iso["gates"][act2])
+            ck.close_scaled("step_c", csave[act2], iso["c"][act2])
+            ck.close_scaled("step_h", S.step_h(g("lstm_out", s), lens, T)[act2], iso["h"][act2])
+        r = S.logits_stage(g("lstm_out", s), Wb["logits/weights"], P["logits/biases"], T)
+        lg = F_.logits[:, s].to(dev)
+        ck.close("logits", lg, r["out"], r["acc"])
+        past = torch.arange(T, device=dev)[:, None] >= Ls[None, :]
+        ck.exact("logits_past_len_bias", lg[past], P["logits/biases"].float())
+    stats = R["stats"]
+    for li, name in enumerate(("conv4_1", "conv4_2")):
+        st = S.bn_stats_stage(None, P[f"{name}/{name}/gamma"], P[f"{name}/{name}/beta"], EPS, parts=bnp[li])
+        ck.close(f"{name}_stats", stats[li, 0], st["sum"], st["sum_acc"], key="bn_sums")
+        ck.close(f"{name}_stats_sq", stats[li, 1], st["sumsq"], st["sumsq"], key="bn_sums")
+        for j, k in enumerate(("scale", "shift", "mean", "invstd")):        # f32 roundings of f64 values of those sums
+            ck.close(f"{name}_bn_{k}", bn[li, j], st[k], st["acc"][k], key="bn_coef")
+    return bnp
+
+
+def _backward_checks(ck, F_, grad, dlogits, bnp):
+    """Every backward stage on its own inputs, image chunk by image chunk, and the 24 gradient tensors from the reference
+    sums over all chunks.  The BatchNorm backwards need batch sums of their own input gradient first, so the chunks are
+    walked three times: up to d_a4b (+ BN4_2's sums), d_pre4b (+ BN4_1's sums), the rest."""
+    P, Wb, T, H2 = F_.P, F_.Wb, F_.T, F_.H2
+    g, R = F_.g, F_.R
+    bn = R["bn"].double()
+    st = [S.bn_batch(None, EPS, parts=p) for p in bnp]
+    tot, s42, s41 = {}, {}, {}
+    for s in F_.parts:
+        lens = F_.tsl[s]
+        dl = S.dl_rows_stage(dlogits[:, s].to(F_.dev, torch.float64), H2)
+        ck.exact("dl_rows", g("dl_rows", s), S.bf16(dl["dl_rows"]))
+        _sum_into(tot, {"logits/biases": dl["dbias"], "logits/biases_acc": dl["dbias_acc"]})
+        r = S.logits_bwd(g("lstm_out", s), g("dl_rows", s), Wb["logits/weights"])
+        _sum_into(tot, {"logits/weights": r["dw"], "logits/weights_acc": r["dw_acc"]})
+        ck.close("d_lstm_out", g("d_lstm_out", s), r["d_lstm_out"], r["d_lstm_out_acc"])
+        r = S.bptt_stage(g("d_lstm_out", s), F_.steps("gates_steps", s), F_.steps("csave_steps", s), F_.wh[0], F_.wh[1],
+                         lens, T, dz_in=g("dz_all", s))
+        valid = F_.valid(s)
+        ck.exact("dz_all_past_len_zero", g("dz_all", s)[~valid], 0.0)
+        ck.close_scaled("dz_all", g("dz_all", s), r["dz"], mask=valid[..., None].expand(r["dz"].shape))
+        r = S.lstm_grads_stage(g("dz_all", s), g("conv5", s), g("lstm_out", s), Wb[FW + "/weights"][:512],
+                               Wb[BW + "/weights"][:512], F_.wh[0], F_.wh[1])
+        for d, scope in (("fw", FW), ("bw", BW)):
+            _sum_into(tot, {scope + k: r[d + k] for k in ("/weights", "/weights_acc", "/biases", "/biases_acc")})
+        ck.close("d_a5", g("d_a5", s), r["d_a5"], r["d_a5_acc"])
+        r = S.conv5_bwd(g("d_a5", s), g("conv4_2", s), Wb["conv5/weights"])
+        _sum_into(tot, {"conv5/weights": r["dw"], "conv5/weights_acc": r["dw_acc"], "conv5/biases": r["db"],
+                        "conv5/biases_acc": r["db_acc"]})
+        ck.close("d_a4b", g("d_a4b", s), r["dx"], r["dx_acc"])
+        dyr = S.bn_relu_pool_route(g("d_a4b", s), g("a4b_pre", s), bn[1])
+        _sum_into(s42, S.bn_bwd_sums(dyr, dyr.abs(), g("a4b_pre", s), st[1]))
+    ck.close("conv4_2/gamma", grad["conv4_2/conv4_2/gamma"], s42["dgamma"], s42["dgamma_acc"], key="wgrad")
+    ck.close("conv4_2/beta", grad["conv4_2/conv4_2/beta"], s42["dbeta"], s42["dbeta_acc"], key="wgrad")
+    w42 = Wb["conv4_2/weights"]
+    for s in F_.parts:
+        r = S.bn_relu_pool_bwd_stage(g("d_a4b", s), g("a4b_pre", s), bn[1], P["conv4_2/conv4_2/gamma"], EPS, stats=st[1],
+                                     sums=s42)
+        ck.close("d_pre4b", g("d_pre4b", s), r["dx"], r["dx_acc"])
+        r = S.conv_bwd(g("d_pre4b", s), g("conv4_1", s), w42)
+        _sum_into(tot, {"conv4_2/weights": r["dw"], "conv4_2/weights_acc": r["dw_acc"]})
+        d, d_acc = S.conv_relu_dgrad(g("d_pre4b", s), g("a4a_pre", s), bn[0], w42)
+        _sum_into(s41, S.bn_bwd_sums(d, d_acc, g("a4a_pre", s), st[0]))
+    ck.close("conv4_1/gamma", grad["conv4_1/conv4_1/gamma"], s41["dgamma"], s41["dgamma_acc"], key="bn41_affine")
+    ck.close("conv4_1/beta", grad["conv4_1/conv4_1/beta"], s41["dbeta"], s41["dbeta_acc"], key="bn41_affine")
+    for s in F_.parts:
+        r = S.conv_bn_relu_bwd_stage(g("d_pre4b", s), g("a4a_pre", s), bn[0], P["conv4_1/conv4_1/gamma"], w42, EPS,
+                                     stats=st[0], sums=s41)
+        ck.close("d_pre4a", g("d_pre4a", s), r["dx"], r["dx_acc"])
+        r = S.conv_bwd(g("d_pre4a", s), g("conv3_2", s), Wb["conv4_1/weights"])
+        _sum_into(tot, {"conv4_1/weights": r["dw"], "conv4_1/weights_acc": r["dw_acc"]})
+        ck.close("d_a3p", g("d_a3p", s), r["dx"], r["dx_acc"])
+        ck.exact("d_pre32", g("d_pre32", s), S.unpool_stage(g("d_a3p", s), g("conv3_2", s), R["am3"][s].long(), 2))
+        db, dba = S.masked_colsum(g("d_a3p", s), g("conv3_2", s))
+        _sum_into(tot, {"conv3_2/biases": db, "conv3_2/biases_acc": dba})
+        r = S.conv_bwd(g("d_pre32", s), g("conv3_1", s), Wb["conv3_2/weights"])
+        _sum_into(tot, {"conv3_2/weights": r["dw"], "conv3_2/weights_acc": r["dw_acc"]})
+        ck.close("d_pre31", g("d_pre31", s), r["dx"] * (g("conv3_1", s) > 0), r["dx_acc"])
+        r = S.conv_bwd(g("d_pre31", s), g("conv2", s), Wb["conv3_1/weights"])
+        _sum_into(tot, {"conv3_1/weights": r["dw"], "conv3_1/weights_acc": r["dw_acc"], "conv3_1/biases": r["db"],
+                        "conv3_1/biases_acc": r["db_acc"]})
+        ck.close("d_a2", g("d_a2", s), r["dx"], r["dx_acc"])
+        ck.exact("d_pre2", g("d_pre2", s), S.unpool_stage(g("d_a2", s), g("conv2", s), R["am2"][s].long(), 4))
+        db, dba = S.masked_colsum(g("d_a2", s), g("conv2", s))
+        _sum_into(tot, {"conv2/biases": db, "conv2/biases_acc": dba})
+        r = S.conv_bwd(g("d_pre2", s), g("conv1", s), Wb["conv2/weights"])
+        _sum_into(tot, {"conv2/weights": r["dw"], "conv2/weights_acc": r["dw_acc"]})
+        ck.close("d_a1", g("d_a1", s), r["dx"], r["dx_acc"])
+        r = S.conv1_wgrad_stage(g("d_a1", s), g("conv1", s), R["am1"][s].long(), F_.x(s), P["conv1/weights"])
+        _sum_into(tot, {"conv1/weights": r["dw"], "conv1/weights_acc": r["dw_acc"], "conv1/biases": r["db"],
+                        "conv1/biases_acc": r["db_acc"]})
+    for k in [k for k in tot if not k.endswith("_acc")]:                  # a tensor's own bound "wgrad/<name>" if any
+        ck.close(k, grad[k], tot[k], tot[k + "_acc"], key=f"wgrad/{k}" if f"wgrad/{k}" in ck.bounds else "wgrad")
+    ck.exact("conv4_2/biases_zero", grad["conv4_2/biases"], 0.0)
+    ck.exact("conv4_1/biases_zero", grad["conv4_1/biases"], 0.0)
+
+
+def _run_stage_checks(case, N, W, widths, dev="cpu", chunk=None, ctc=None, ck=None):
+    """The training-mode forward and backward of one batch, every stage checked on its own inputs.  dev: where the fp64
+    references run; chunk: images per reference evaluation (the whole batch by default).  ctc(ck, logits, lab, ll, tsl):
+    returns the backward's d logits (default: a seeded random one).  Returns the model, the operands (_Refs) and the
+    checker (Checker(case) unless given), not yet asserted."""
+    m, pn, data, lab, ll, tsl = _setup(N, W, widths)
+    T = W // 4 - 1
     t = lambda a: torch.tensor(a, device=DEV)
     m.set_training(True)
     d_data, d_tsl = t(data), t(tsl)
     logits = m.forward(d_data, d_tsl)
-    gen = torch.Generator(device="cpu").manual_seed(17)
-    dlogits = (torch.randn((T, N, 64), generator=gen) * 0.05).float()
     torch.cuda.synchronize()
-    tap = lambda k: m.tap(k, N, W).double().cpu()
-    raw = lambda k: m.tap_raw(k, N, W).cpu()
-    G = {k: tap(k) for k in ("conv1", "conv2", "conv3_1", "conv3_2", "a4a_pre", "conv4_1", "a4b_pre", "conv4_2", "conv5",
-                             "xproj", "lstm_out", "gates")}
-    R = {k: raw(k) for k in ("bn", "stats", "am1", "am2", "am3", "csave")}
-    logits = logits.double().cpu()
-    m.backward(d_data, d_tsl, dlogits.to(DEV))
+    G = {k: m.tap(k, N, W) for k in FWD_TAPS}
+    G["gates_steps"] = S.unpack_gates(m.tap("gates", N, W), N)
+    R = {k: m.tap_raw(k, N, W) for k in ("bn", "stats", "am1", "am2", "am3")}
+    G["csave_steps"] = S.unpack_csave(m.tap_raw("csave", N, W), N)
+    ck = ck or Checker(case)
+    if ctc is None:
+        gen = torch.Generator(device="cpu").manual_seed(17)
+        dlogits = (torch.randn((T, N, 64), generator=gen) * 0.05).float().to(DEV)
+    else:
+        dlogits = ctc(ck, logits, lab, ll, tsl)
+    m.backward(d_data, d_tsl, dlogits)
     torch.cuda.synchronize()
-    for k in ("dl_rows", "d_lstm_out", "dz_all", "d_a5", "d_a4b", "d_pre4b", "d_pre4a", "d_a3p", "d_pre32", "d_pre31", "d_a2",
-              "d_pre2", "d_a1"):
-        G[k] = tap(k)
-    grad = {k: m.grad_tensor(k).double().cpu() for k in m.table}
-    P = {k: torch.as_tensor(np.asarray(v, np.float64)) for k, v in pn.items()}
-    Wb = {k: S.bf16(v) for k, v in P.items() if k.endswith("weights")}
-    eps = float(np.float32(1e-3))
-    L = S.clamp_lens(tsl, T)
-    ck = Checker(case)
-
-    # ---------------------------------------------------------------- forward
-    x = torch.as_tensor(data, dtype=torch.float64)
-    r = S.conv1_stage(x, P["conv1/weights"], P["conv1/biases"])
-    ck.close("conv1", G["conv1"], r["out"], r["acc"])
-    argmax_check(ck, "am1", R["am1"], S.windows22(r["pre"]).numpy(), G["conv1"], 2 ** -15 * r["acc"].numpy())
-    r = S.conv_relu_pool22_stage(G["conv1"], Wb["conv2/weights"], P["conv2/biases"])
-    ck.close("conv2", G["conv2"], r["out"], r["acc"])
-    argmax_check(ck, "am2", R["am2"], S.windows22(r["pre"]).numpy(), G["conv2"], 2 ** -16 * r["acc"].numpy())
-    r = S.conv_relu_stage(G["conv2"], Wb["conv3_1/weights"], P["conv3_1/biases"])
-    ck.close("conv3_1", G["conv3_1"], r["out"], r["acc"])
-    r = S.conv_relu_pool12_stage(G["conv3_1"], Wb["conv3_2/weights"], P["conv3_2/biases"])
-    ck.close("conv3_2", G["conv3_2"], r["out"], r["acc"])
-    argmax_check(ck, "am3", R["am3"], S.windows12(r["pre"]).numpy(), G["conv3_2"], 2 ** -16 * r["acc"].numpy())
-    bn = R["bn"].double()
-    for li, (name, src, pre, out) in enumerate((("conv4_1", "conv3_2", "a4a_pre", "conv4_1"),
-                                                ("conv4_2", "conv4_1", "a4b_pre", "conv4_2"))):
-        r = S.conv_bias_stage(G[src], Wb[f"{name}/weights"], P[f"{name}/biases"])
-        ck.close(pre, G[pre], r["out"], r["acc"])
-        st = S.bn_stats_stage(G[pre], P[f"{name}/{name}/gamma"], P[f"{name}/{name}/beta"], eps)
-        stats = R["stats"][li]
-        ck.close(f"{name}_stats", stats[0], st["sum"], st["sum_acc"], key="bn_sums")
-        ck.close(f"{name}_stats_sq", stats[1], st["sumsq"], st["sumsq"], key="bn_sums")
-        for j, k in enumerate(("scale", "shift", "mean", "invstd")):        # f32 roundings of f64 values of those sums
-            ck.close(f"{name}_bn_{k}", bn[li, j], st[k], st["acc"][k], key="bn_coef")
-        if li == 0:
-            r = S.bn_apply_relu_stage(G[pre], bn[0, 0], bn[0, 1])
-        else:
-            r = S.bn_apply_relu_pool_stage(G[pre], bn[1, 0], bn[1, 1])
-        ck.close(out, G[out], r["out"], r["acc"] * 2 ** -8)        # one f32 fma, then the bf16 rounding: <= 1 ulp
-    r = S.conv5_stage(G["conv4_2"], Wb["conv5/weights"], P["conv5/biases"])
-    ck.close("conv5", G["conv5"][:, :T], r["out"], r["acc"])
-    r = S.xproj_stage(G["conv5"], Wb[FW + "/weights"][:512], Wb[BW + "/weights"][:512], P[FW + "/biases"], P[BW + "/biases"],
-                      tsl, T)
-    ck.close("xproj", G["xproj"], r["out"], r["acc"])
-    wh = (Wb[FW + "/weights"][512:], Wb[BW + "/weights"][512:])
-    r = S.recurrence_stage(G["xproj"], wh[0], wh[1], tsl, T)
-    valid = np.zeros((N, H2), bool)
-    for n in range(N):
-        valid[n, :L[n]] = True
-    ck.exact("lstm_out_past_len_zero", G["lstm_out"].numpy()[~valid], 0.0)
-    ck.close_scaled("lstm_out", G["lstm_out"], r["out"], mask=np.broadcast_to(valid[..., None], r["out"].shape))
-    gates = S.unpack_gates(G["gates"], N)
-    csave = S.unpack_csave(R["csave"].double(), N)
-    iso = S.recurrence_steps_isolated(G["xproj"], wh[0], wh[1], G["lstm_out"], csave, tsl, T)
-    act = (torch.arange(T)[None, :] < torch.as_tensor(L)[:, None]).numpy()
-    act2 = np.broadcast_to(act[None], (2, N, T))
-    ck.close_scaled("step_gates", gates.numpy()[act2], iso["gates"].numpy()[act2])
-    ck.close_scaled("step_c", csave.numpy()[act2], iso["c"].numpy()[act2])
-    h_gpu = torch.zeros_like(iso["h"])
-    for d in range(2):
-        for n in range(N):
-            for s in range(L[n]):
-                h_gpu[d, n, s] = G["lstm_out"][n, (L[n] - 1 - s) if d else s, d * 256:(d + 1) * 256]
-    ck.close_scaled("step_h", h_gpu.numpy()[act2], iso["h"].numpy()[act2])
-    r = S.logits_stage(G["lstm_out"], Wb["logits/weights"], P["logits/biases"], T)
-    ck.close("logits", logits, r["out"], r["acc"])
-    past = np.zeros((T, N), bool)
-    for n in range(N):
-        past[L[n]:, n] = True
-    ck.exact("logits_past_len_bias", logits.numpy()[past], np.broadcast_to(np.float32(pn["logits/biases"]), (int(past.sum()), 64)))
-
-    # ---------------------------------------------------------------- backward
-    dl = S.dl_rows_stage(dlogits.double(), H2)
-    ck.exact("dl_rows", G["dl_rows"].numpy(), S.bf16(dl["dl_rows"]).numpy())
-    ck.close("logits/biases", grad["logits/biases"], dl["dbias"], dl["dbias_acc"], key="wgrad")
-    r = S.logits_bwd(G["lstm_out"], G["dl_rows"], Wb["logits/weights"])
-    ck.close("logits/weights", grad["logits/weights"], r["dw"], r["dw_acc"], key="wgrad")
-    ck.close("d_lstm_out", G["d_lstm_out"], r["d_lstm_out"], r["d_lstm_out_acc"])
-    r = S.bptt_stage(G["d_lstm_out"], gates, csave, wh[0], wh[1], tsl, T, dz_in=G["dz_all"])
-    ck.exact("dz_all_past_len_zero", G["dz_all"].numpy()[~valid], 0.0)
-    ck.close_scaled("dz_all", G["dz_all"], r["dz"], mask=np.broadcast_to(valid[..., None], r["dz"].shape))
-    r = S.lstm_grads_stage(G["dz_all"], G["conv5"], G["lstm_out"], Wb[FW + "/weights"][:512], Wb[BW + "/weights"][:512],
-                           wh[0], wh[1])
-    for d, scope in (("fw", FW), ("bw", BW)):
-        ck.close(scope + "/weights", grad[scope + "/weights"], r[d + "/weights"], r[d + "/weights_acc"], key="wgrad")
-        ck.close(scope + "/biases", grad[scope + "/biases"], r[d + "/biases"], r[d + "/biases_acc"], key="wgrad")
-    ck.close("d_a5", G["d_a5"], r["d_a5"], r["d_a5_acc"])
-    r = S.conv5_bwd(G["d_a5"], G["conv4_2"], Wb["conv5/weights"])
-    ck.close("conv5/weights", grad["conv5/weights"], r["dw"], r["dw_acc"], key="wgrad")
-    ck.close("conv5/biases", grad["conv5/biases"], r["db"], r["db_acc"], key="wgrad")
-    ck.close("d_a4b", G["d_a4b"], r["dx"], r["dx_acc"])
-    r = S.bn_relu_pool_bwd_stage(G["d_a4b"], G["a4b_pre"], bn[1], P["conv4_2/conv4_2/gamma"], P["conv4_2/conv4_2/beta"], eps)
-    ck.close("d_pre4b", G["d_pre4b"], r["dx"], r["dx_acc"])
-    ck.close("conv4_2/gamma", grad["conv4_2/conv4_2/gamma"], r["dgamma"], r["dgamma_acc"], key="wgrad")
-    ck.close("conv4_2/beta", grad["conv4_2/conv4_2/beta"], r["dbeta"], r["dbeta_acc"], key="wgrad")
-    r = S.conv_bwd(G["d_pre4b"], G["conv4_1"], Wb["conv4_2/weights"])
-    ck.close("conv4_2/weights", grad["conv4_2/weights"], r["dw"], r["dw_acc"], key="wgrad")
-    ck.exact("conv4_2/biases_zero", grad["conv4_2/biases"].numpy(), 0.0)
-    r = S.conv_bn_relu_bwd_stage(G["d_pre4b"], G["a4a_pre"], bn[0], P["conv4_1/conv4_1/gamma"], P["conv4_1/conv4_1/beta"],
-                                 Wb["conv4_2/weights"], eps)
-    ck.close("d_pre4a", G["d_pre4a"], r["dx"], r["dx_acc"])
-    ck.close("conv4_1/gamma", grad["conv4_1/conv4_1/gamma"], r["dgamma"], r["dgamma_acc"], key="bn41_affine")
-    ck.close("conv4_1/beta", grad["conv4_1/conv4_1/beta"], r["dbeta"], r["dbeta_acc"], key="bn41_affine")
-    r = S.conv_bwd(G["d_pre4a"], G["conv3_2"], Wb["conv4_1/weights"])
-    ck.close("conv4_1/weights", grad["conv4_1/weights"], r["dw"], r["dw_acc"], key="wgrad")
-    ck.exact("conv4_1/biases_zero", grad["conv4_1/biases"].numpy(), 0.0)
-    ck.close("d_a3p", G["d_a3p"], r["dx"], r["dx_acc"])
-    ck.exact("d_pre32", G["d_pre32"].numpy(), S.unpool_stage(G["d_a3p"], G["conv3_2"], R["am3"].long(), 2).numpy())
-    db, dba = S.masked_colsum(G["d_a3p"], G["conv3_2"])
-    ck.close("conv3_2/biases", grad["conv3_2/biases"], db, dba, key="wgrad")
-    r = S.conv_bwd(G["d_pre32"], G["conv3_1"], Wb["conv3_2/weights"])
-    ck.close("conv3_2/weights", grad["conv3_2/weights"], r["dw"], r["dw_acc"], key="wgrad")
-    ck.close("d_pre31", G["d_pre31"], r["dx"] * (G["conv3_1"] > 0), r["dx_acc"])
-    r = S.conv_bwd(G["d_pre31"], G["conv2"], Wb["conv3_1/weights"])
-    ck.close("conv3_1/weights", grad["conv3_1/weights"], r["dw"], r["dw_acc"], key="wgrad")
-    ck.close("conv3_1/biases", grad["conv3_1/biases"], r["db"], r["db_acc"], key="wgrad")
-    ck.close("d_a2", G["d_a2"], r["dx"], r["dx_acc"])
-    ck.exact("d_pre2", G["d_pre2"].numpy(), S.unpool_stage(G["d_a2"], G["conv2"], R["am2"].long(), 4).numpy())
-    db, dba = S.masked_colsum(G["d_a2"], G["conv2"])
-    ck.close("conv2/biases", grad["conv2/biases"], db, dba, key="wgrad")
-    r = S.conv_bwd(G["d_pre2"], G["conv1"], Wb["conv2/weights"])
-    ck.close("conv2/weights", grad["conv2/weights"], r["dw"], r["dw_acc"], key="wgrad")
-    ck.close("d_a1", G["d_a1"], r["dx"], r["dx_acc"])
-    r = S.conv1_wgrad_stage(G["d_a1"], G["conv1"], R["am1"].long(), x, P["conv1/weights"])
-    ck.close("conv1/weights", grad["conv1/weights"], r["dw"], r["dw_acc"], key="wgrad")
-    ck.close("conv1/biases", grad["conv1/biases"], r["db"], r["db_acc"], key="wgrad")
-    ck.assert_ok()
-    return m, G
+    for k in BWD_TAPS:
+        G[k] = m.tap(k, N, W)
+    F_ = _Refs(pn, G, R, data, tsl, logits, N, W, dev, chunk)
+    grad = {k: m.grad_tensor(k).to(dev, torch.float64) for k in m.table}
+    bnp = _forward_checks(ck, F_)
+    _backward_checks(ck, F_, grad, dlogits, bnp)
+    return m, F_, ck
 
 
 @pytest.mark.parametrize("N,W,widths", SHAPES)
 def test_every_stage_against_fp64_on_its_own_inputs(N, W, widths, request):
-    _run_stage_checks(request.node.callspec.id, N, W, widths)
+    _run_stage_checks(request.node.callspec.id, N, W, widths)[2].assert_ok()
 
 
 ALT_SWITCHES = [
@@ -253,16 +325,16 @@ def test_alternative_kernels_against_the_same_references(env, monkeypatch, reque
     """The kernels kept selectable by environment switches (read when a model is created), same checks at 3 x 100."""
     for k, v in env.items():
         monkeypatch.setenv(k, v)
-    _run_stage_checks("N3_W100/" + request.node.callspec.id, 3, 100, [100, 4, 61])
+    _run_stage_checks("N3_W100/" + request.node.callspec.id, 3, 100, [100, 4, 61])[2].assert_ok()
 
 
 @pytest.mark.parametrize("N,W,widths", [SHAPES[0], SHAPES[3], SHAPES[4]])
 def test_training_forward_taps_match_inference(N, W, widths):
     """conv1 .. conv3_2 come before any atomics: the training variants (arg-max bytes) must write bit-identical values.
     conv4_1 and conv4_2 may differ by 1 bf16 ulp (order of the f64 atomics of the BatchNorm statistics).  The per-stage
-    checks above run on training-mode plans; from conv5 on the kernels are the same in both modes, and the inference-mode
-    outputs past conv4_2 are pinned by the whole-chain tests only."""
-    m, pn, data, tsl = _setup(N, W, widths)
+    checks above run on training-mode plans; from conv5 on the kernels are the same in both modes.  The inference plan is
+    checked stage by stage at 1024 x 256 in test_gpu_stage_isolation_batch.py, which also repeats this comparison there."""
+    m, pn, data, _, _, tsl = _setup(N, W, widths)
     t = lambda a: torch.tensor(a, device=DEV)
     names = ("conv1", "conv2", "conv3_1", "conv3_2", "conv4_1", "conv4_2")
     m.forward(t(data), t(tsl))
@@ -281,7 +353,7 @@ def test_training_forward_taps_match_inference(N, W, widths):
 def test_chunked_front_end_is_bit_identical(N, W, widths):
     """forward_host(chunks=4) runs conv1 .. conv3_2 per image range (the img0 coordinate of conv1's output map): the front-end
     taps must equal the one-range forward bit for bit."""
-    m, pn, data, tsl = _setup(N, W, widths)
+    m, pn, data, _, _, tsl = _setup(N, W, widths)
     t = lambda a: torch.tensor(a, device=DEV)
     names = ("conv1", "conv2", "conv3_1", "conv3_2")
     m.forward(t(data), t(tsl))

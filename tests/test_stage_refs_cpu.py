@@ -140,13 +140,13 @@ def test_backward_stage_chain_reproduces_oracle_gradients(chain):
     c5 = S.conv5_bwd(lg["d_a5"], A["conv4_2"], P["conv5/weights"])
     got["conv5/weights"], got["conv5/biases"] = c5["dw"], c5["db"]
     d_a4b = c5["dx"]
-    b42 = S.bn_relu_pool_bwd_stage(d_a4b, r["conv4_2"]["pre"], r["conv4_2"]["bn"], P["conv4_2/conv4_2/gamma"],
-                                   P["conv4_2/conv4_2/beta"], eps, rnd=S.ident)
+    b42 = S.bn_relu_pool_bwd_stage(d_a4b, r["conv4_2"]["pre"], r["conv4_2"]["bn"], P["conv4_2/conv4_2/gamma"], eps,
+                                   rnd=S.ident)
     got["conv4_2/conv4_2/gamma"], got["conv4_2/conv4_2/beta"] = b42["dgamma"], b42["dbeta"]
     got["conv4_2/weights"] = S.conv_bwd(b42["dx"], A["conv4_1"], P["conv4_2/weights"])["dw"]
     bn41 = r["conv4_1"]["bn"]
-    b41 = S.conv_bn_relu_bwd_stage(b42["dx"], r["conv4_1"]["pre"], bn41, P["conv4_1/conv4_1/gamma"], P["conv4_1/conv4_1/beta"],
-                                   P["conv4_2/weights"], eps, mask=(r["conv4_1"]["pre"] * bn41[0] + bn41[1] > 0).double(), rnd=S.ident)
+    b41 = S.conv_bn_relu_bwd_stage(b42["dx"], r["conv4_1"]["pre"], bn41, P["conv4_1/conv4_1/gamma"], P["conv4_2/weights"], eps,
+                                   mask=(r["conv4_1"]["pre"] * bn41[0] + bn41[1] > 0).double(), rnd=S.ident)
     got["conv4_1/conv4_1/gamma"], got["conv4_1/conv4_1/beta"] = b41["dgamma"], b41["dbeta"]
     c41 = S.conv_bwd(b41["dx"], A["conv3_2"], P["conv4_1/weights"])
     got["conv4_1/weights"] = c41["dw"]
@@ -327,3 +327,130 @@ def test_x3_storage_checks_reject_a_truncating_store(mode):
         else:
             assert ck.fail, (name, ck.rows)
             assert ck.fail[0].startswith("conv3_2: " if mode == "tf32" else "conv3_2_canonical"), ck.fail
+
+
+# ---------------------------------------------------------------------------------------------------------- batch scale
+def test_vectorised_layout_helpers_equal_their_loops():
+    """reverse_rows, step_h, gate_perm and first_argmax (device-agnostic, no per-row loops) equal plain loops."""
+    g = torch.Generator().manual_seed(1)
+    N, H2, T = 6, 9, 8
+    lens = [8, 0, 1, 5, 12, 3]                        # 12 > T: clamped
+    L = S.clamp_lens(lens, T)
+    x = torch.randn(N, H2, 7, generator=g, dtype=torch.float64)
+    want = x.clone()
+    for n in range(N):
+        if L[n] > 0:
+            want[n, :L[n]] = x[n, :L[n]].flip(0)
+    assert torch.equal(S.reverse_rows(x, lens, T), want)
+    out = torch.randn(N, H2, 512, generator=g, dtype=torch.float64)
+    h = S.step_h(out, lens, T)
+    for d in range(2):
+        for n in range(N):
+            for s in range(L[n]):
+                assert torch.equal(h[d, n, s], out[n, (L[n] - 1 - s) if d else s, d * 256:(d + 1) * 256])
+    j = np.arange(1024)
+    assert np.array_equal(S.gate_perm().numpy(), (j % 256 // 32) * 128 + j // 256 * 32 + j % 32)
+    v = torch.randint(0, 3, (50, 4), generator=g).double()
+    assert np.array_equal(S.first_argmax(v).numpy(), np.argmax(v.numpy(), -1))
+
+
+def test_chunked_references_equal_the_whole_batch(chain):
+    """Per-image stages over image chunks concatenate to the whole-batch result exactly; the batch reductions (BatchNorm
+    sums and backward, weight and bias gradients, masked column sums) summed over chunks agree to 1e-12."""
+    c = chain
+    r = _forward_chain(c)
+    P, A, T, H2, tsl, eps = c["P"], c["A"], c["T"], c["H2"], c["tsl"], O.BN_EPS
+    parts = [slice(0, 2), slice(2, 3)]
+    cat = lambda f: {k: torch.cat([f(s)[k] for s in parts]) for k in f(parts[0]) if torch.is_tensor(f(parts[0])[k])}
+    for k, v in cat(lambda s: S.conv_relu_pool22_stage(A["conv1"][s], P["conv2/weights"], P["conv2/biases"])).items():
+        assert torch.equal(v, S.conv_relu_pool22_stage(A["conv1"], P["conv2/weights"], P["conv2/biases"])[k]), k
+    xp = r["xproj"]["out"]
+    rec = [S.recurrence_stage(xp[s], P[f"{FW}/weights"][512:], P[f"{BW}/weights"][512:], tsl[s], T) for s in parts]
+    whole = S.recurrence_stage(xp, P[f"{FW}/weights"][512:], P[f"{BW}/weights"][512:], tsl, T)
+    assert torch.equal(torch.cat([x["out"] for x in rec]), whole["out"])
+    assert torch.equal(torch.cat([x["gates"] for x in rec], 1), whole["gates"])
+    pre, bn = r["conv4_2"]["pre"], r["conv4_2"]["bn"]
+    tot = {}
+    for s in parts:
+        for k, v in S.bn_sums(pre[s]).items():
+            tot[k] = tot[k] + v if k in tot else v
+    st = S.bn_stats_stage(None, P["conv4_2/conv4_2/gamma"], P["conv4_2/conv4_2/beta"], eps, parts=tot)
+    st1 = S.bn_stats_stage(pre, P["conv4_2/conv4_2/gamma"], P["conv4_2/conv4_2/beta"], eps)
+    for k in ("sum", "sumsq", "mean", "invstd", "scale", "shift"):
+        assert rel(st[k], st1[k]) < 1e-12, k
+    d = torch.randn(pre.shape[:2] + (2, pre.shape[3]), dtype=torch.float64)
+    gamma = P["conv4_2/conv4_2/gamma"]
+    stats = S.bn_batch(None, eps, parts=tot)
+    sums = {}
+    for s in parts:
+        dyr = S.bn_relu_pool_route(d[s], pre[s], bn, rnd=S.ident)
+        for k, v in S.bn_bwd_sums(dyr, dyr.abs(), pre[s], stats).items():
+            sums[k] = sums[k] + v if k in sums else v
+    whole = S.bn_relu_pool_bwd_stage(d, pre, bn, gamma, eps, rnd=S.ident)
+    got = [S.bn_relu_pool_bwd_stage(d[s], pre[s], bn, gamma, eps, rnd=S.ident, stats=stats, sums=sums) for s in parts]
+    assert rel(torch.cat([x["dx"] for x in got]), whole["dx"]) < 1e-12
+    assert rel(torch.cat([x["dx_acc"] for x in got]), whole["dx_acc"]) < 1e-12
+    for k in ("dgamma", "dbeta", "dgamma_acc", "dbeta_acc"):
+        assert rel(got[0][k], whole[k]) < 1e-12, k
+    dy = torch.randn(A["conv3_1"].shape, dtype=torch.float64)
+    w = S.conv_bwd(dy, A["conv3_1"], P["conv3_2/weights"])
+    ws = [S.conv_bwd(dy[s], A["conv3_1"][s], P["conv3_2/weights"]) for s in parts]
+    assert torch.equal(torch.cat([x["dx"] for x in ws]), w["dx"])
+    for k in ("dw", "dw_acc", "db", "db_acc"):
+        assert rel(sum(x[k] for x in ws), w[k]) < 1e-12, k
+    cs = [S.masked_colsum(dy[s], A["conv3_1"][s]) for s in parts]
+    assert rel(sum(x[0] for x in cs), S.masked_colsum(dy, A["conv3_1"])[0]) < 1e-12
+
+
+def test_checker_rows_from_torch_equal_numpy():
+    """Checker.close / close_scaled / exact give the same row from torch tensors as from numpy arrays, and a stage checked
+    in image chunks merges into one row with the worst element, the maxima and the L2 of the whole."""
+    from stage_check import Checker, ulp_bf16
+    g = torch.Generator().manual_seed(2)
+    ref = torch.randn(40, 33, generator=g, dtype=torch.float64) * 10 ** torch.randint(-3, 3, (40, 33), generator=g)
+    gpu = S.bf16(ref * (1 + 2.0 ** -10 * torch.randn(40, 33, generator=g, dtype=torch.float64)))
+    acc = ref.abs() + 0.1
+    mask = torch.rand(40, 33, generator=g) > 0.3
+    bounds = {"a": (1, 2 ** -12), "b": (0, 1e-3), "c": (1, 1e-3)}
+    cks = {}
+    for kind, cv in (("np", lambda t: t.numpy()), ("torch", lambda t: t)):
+        ck = cks[kind] = Checker("x", bounds, ulp=ulp_bf16)
+        ck.close("a", cv(gpu), cv(ref), cv(acc))
+        ck.close("b", cv(gpu), cv(ref), cv(acc), mask=cv(mask))
+        ck.close_scaled("c", cv(gpu), cv(ref), mask=cv(mask))
+        ck.exact("e", cv(gpu), cv(ref))
+    for a, b in zip(cks["np"].rows, cks["torch"].rows):          # the L2 norms may differ in the last bits
+        for k in ("rel_l2", "_err_sq", "_ref_sq"):
+            if k in a:
+                va, vb = a.pop(k), b.pop(k)
+                assert abs(va - vb) <= 1e-12 * abs(va), k
+        assert a == b
+    whole = Checker("x", bounds, ulp=ulp_bf16)
+    whole.close("b", gpu, ref, acc)
+    parts = Checker("x", bounds, ulp=ulp_bf16)
+    for s in (slice(0, 7), slice(7, 40)):
+        parts.close("b", gpu[s], ref[s], acc[s])
+    (w,), (p,) = whole.rows, parts.rows
+    for k in ("rel_l2", "_err_sq", "_ref_sq"):
+        vp, vw = p.pop(k), w.pop(k)
+        assert abs(vp - vw) <= 1e-12 * abs(vw), k
+    assert p == w
+    # a NaN in any chunk fails the merged row, whichever chunk comes after it
+    bad = gpu.clone()
+    bad[3, 5] = float("nan")
+    for order in ((bad, gpu, gpu), (gpu, bad, gpu), (gpu, gpu, bad)):
+        for use_torch in (True, False):
+            ck = Checker("x", bounds, ulp=ulp_bf16)
+            for g_ in order:
+                args = (g_, ref, acc) if use_torch else (g_.numpy(), ref.numpy(), acc.numpy())
+                ck.close("a", *args)
+                ck.exact("e", *args[:2])
+            (ra, re) = ck.rows
+            assert np.isnan(ra["max_ratio"]) and np.isnan(ra["c_needed"]) and np.isnan(ra["max_abs_err"])
+            assert np.isnan(ra["worst_gpu"]) and re["mismatches"] >= 1
+            assert any(f.startswith("a: ") for f in ck.fail)
+    # one stage name for two kinds of check is refused
+    ck = Checker("x", bounds, ulp=ulp_bf16)
+    ck.exact("a", gpu, gpu)
+    with pytest.raises(AssertionError, match="different kinds"):
+        ck.close("a", gpu, ref, acc)

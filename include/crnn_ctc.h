@@ -52,6 +52,14 @@ const char* crnn_last_error(void);           /* host string, valid until the nex
  * negative or above max_label_len, gets cost NaN and an all-zero gradient -- the kernels never index with such an id.
  * input_len is clamped to [0,T].  flat_labels MUST hold sum(label_len) entries (its length is not passed and cannot be
  * checked on the device; the Python wrappers check it).
+ * Frame limits: alpha / beta live in shared memory (at most 200 KB per utterance), so T is bounded per max_label_len.
+ *   max_label_len <= 15: T <= 256 tensor-map kernel (CRNN_CTC_KERNEL=tma), T <= floor(51200 / (70 + 2*AS + ES)) fast
+ *                        kernel (AS = (2*max_label_len+1)|1, ES = max_label_len|1: 348 at 15, 550 at 4), beyond that
+ *                        the generic kernel to T <= 517; the largest supported T is the larger of 517 and the fast limit
+ *   max_label_len 16..31: T <= 259;   32..63: T <= 130;   above 63: CRNN_UNSUPPORTED
+ * Logits or a gradient not 16-byte aligned (4-byte alignment is enough) take the generic kernel (T <= 517 / 259 / 130).
+ * A T above the limit returns CRNN_UNSUPPORTED without touching costs or grad; crnn_last_error() names T and the shared
+ * memory it needed.
  * ---------------------------------------------------------------------------------------- */
 int crnn_ctc_workspace_size(int T, int N, int C, int max_label_len, size_t* bytes);
 int crnn_ctc_loss(const float* logits, float* grad, const int* flat_labels, const int* label_len,
@@ -62,7 +70,7 @@ int crnn_ctc_loss(const float* logits, float* grad, const int* flat_labels, cons
 /* Greedy decode.  Replaces tf.nn.ctc_*_decoder(merge_repeated=True) + sparse_tensor_to_dense
  * at lib/networks/network.py:656-657 and the zero stripping of lib/lstm/utils/training.py:32:
  * per frame argmax (lowest index on ties) for t < input_len; emit iff != tf_blank and != the
- * previous raw argmax; drop `strip`.  out [N,T] i32 zero padded, out_len [N] i32. */
+ * previous raw argmax; drop `strip`.  out [N,T] i32 zero padded, out_len [N] i32.  logits need 4-byte alignment only. */
 int crnn_ctc_greedy(const float* logits, const int* input_len, int T, int N, int C, int tf_blank,
                     int strip, int* out, int* out_len, crnn_stream_t stream);
 

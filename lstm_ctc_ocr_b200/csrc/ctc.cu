@@ -49,6 +49,19 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+// Two adjacent floats of a logit / gradient row.  The generic kernel also takes pointers that are only 4-byte aligned
+// (every misaligned call is routed to it); there the pair is moved as two scalars, with the same values.
+__device__ __forceinline__ float2 ld_pair(const float* p, bool vec) {
+  return vec ? __ldg(reinterpret_cast<const float2*>(p)) : make_float2(__ldg(p), __ldg(p + 1));
+}
+__device__ __forceinline__ void st_pair(float* p, float2 v, bool vec) {
+  if (vec) {
+    *reinterpret_cast<float2*>(p) = v;
+  } else {
+    p[0] = v.x;
+    p[1] = v.y;
+  }
+}
 // 3-input maximum (exact: the order of two-operand maxima does not change the result)
 __device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 // log2(2^a + 2^b + 2^c) with -inf handling
@@ -82,6 +95,7 @@ __global__ void __launch_bounds__(CTC_THREADS, 8) ctc_loss_kernel(const float* _
   int Tn = input_len[n];
   Tn = max(0, min(Tn, T));
   const int S = 2 * L + 1;
+  const bool lvec = (reinterpret_cast<uintptr_t>(logits) & 7) == 0, gvec = (reinterpret_cast<uintptr_t>(grad) & 7) == 0;
 
   // label offset = sum(label_len[0..n))
   if (warp == 0) {
@@ -119,7 +133,7 @@ __global__ void __launch_bounds__(CTC_THREADS, 8) ctc_loss_kernel(const float* _
     if (threadIdx.x == 0) costs[n] = too_long ? __int_as_float(0x7fc00000) : 0.0f;
     if (grad != nullptr) {
       for (int t = warp; t < T; t += CTC_WARPS)
-        *reinterpret_cast<float2*>(grad + ((size_t)t * N + n) * CTC_C + 2 * lane) = make_float2(0.f, 0.f);
+        st_pair(grad + ((size_t)t * N + n) * CTC_C + 2 * lane, make_float2(0.f, 0.f), gvec);
     }
     return;
   }
@@ -133,8 +147,7 @@ __global__ void __launch_bounds__(CTC_THREADS, 8) ctc_loss_kernel(const float* _
 #pragma unroll
     for (int u = 0; u < CTC_RB; ++u) {
       const int t = t0 + CTC_WARPS * u;
-      xr[u] = (t < Tn) ? __ldg(reinterpret_cast<const float2*>(logits + ((size_t)t * N + n) * CTC_C) + lane)
-                       : make_float2(0.f, 0.f);
+      xr[u] = (t < Tn) ? ld_pair(logits + ((size_t)t * N + n) * CTC_C + 2 * lane, lvec) : make_float2(0.f, 0.f);
     }
 #pragma unroll
     for (int g = 0; g < CTC_RB; g += CTC_RG) {
@@ -262,7 +275,7 @@ __global__ void __launch_bounds__(CTC_THREADS, 8) ctc_loss_kernel(const float* _
 #pragma unroll
     for (int u = 0; u < CTC_RB; ++u) {
       const int t = t0 + CTC_WARPS * u;
-      xr[u] = ((t < Tn) && (ll2 != NEG_INF)) ? __ldg(reinterpret_cast<const float2*>(logits + ((size_t)t * N + n) * CTC_C) + lane)
+      xr[u] = ((t < Tn) && (ll2 != NEG_INF)) ? ld_pair(logits + ((size_t)t * N + n) * CTC_C + 2 * lane, lvec)
                                              : make_float2(0.f, 0.f);
     }
 #pragma unroll
@@ -308,13 +321,14 @@ __global__ void __launch_bounds__(CTC_THREADS, 8) ctc_loss_kernel(const float* _
       for (int u = 0; u < CTC_RG; ++u) {
         const int t = t0 + CTC_WARPS * (g + u);
         if (t >= T) continue;
-        float2* gp = reinterpret_cast<float2*>(grad + ((size_t)t * N + n) * CTC_C) + lane;
+        float* gp = grad + ((size_t)t * N + n) * CTC_C + 2 * lane;
         if (!live[u]) {
-          *gp = make_float2(0.f, 0.f);
+          st_pair(gp, make_float2(0.f, 0.f), gvec);
         } else {
           const float lse = s_lse[t];
           const float y0 = ptx::ex2(xr[g + u].x * LOG2E - lse), y1 = ptx::ex2(xr[g + u].y * LOG2E - lse);
-          *gp = make_float2(grad_scale * (y0 - acc[u * CTC_C + 2 * lane]), grad_scale * (y1 - acc[u * CTC_C + 2 * lane + 1]));
+          st_pair(gp, make_float2(grad_scale * (y0 - acc[u * CTC_C + 2 * lane]), grad_scale * (y1 - acc[u * CTC_C + 2 * lane + 1])),
+                  gvec);
         }
       }
       __syncwarp();
@@ -828,7 +842,9 @@ size_t ctc_fast_smem_bytes(int T, int max_label_len) {
   return sizeof(float) * (size_t)T * (FAST_XS + 2 * fast_alpha_stride(max_label_len) + fast_label_stride(max_label_len) + 2);
 }
 
-// Greedy decode: one warp per utterance, lane = frame (chunks of 32 frames).
+// Greedy decode: one warp per utterance, lane = frame (chunks of 32 frames).  VEC: logits 16-byte aligned (float4 row
+// loads); otherwise the same values are read one float at a time.
+template <bool VEC>
 __global__ void __launch_bounds__(128) ctc_greedy_kernel(const float* __restrict__ logits,
                                                          const int* __restrict__ input_len, int T, int N,
                                                          int tf_blank, int strip, int* __restrict__ out,
@@ -843,12 +859,13 @@ __global__ void __launch_bounds__(128) ctc_greedy_kernel(const float* __restrict
     int t = t0 + lane;
     int best = -1;
     if (t < Tn) {
-      const float4* row = reinterpret_cast<const float4*>(logits + ((size_t)t * N + n) * CTC_C);
+      const float* row = logits + ((size_t)t * N + n) * CTC_C;
       float bv = -INFINITY;
       best = 0;
 #pragma unroll
       for (int q = 0; q < CTC_C / 4; ++q) {
-        float4 v = __ldg(row + q);
+        const float4 v = VEC ? __ldg(reinterpret_cast<const float4*>(row) + q)
+                             : make_float4(__ldg(row + 4 * q), __ldg(row + 4 * q + 1), __ldg(row + 4 * q + 2), __ldg(row + 4 * q + 3));
         if (v.x > bv) { bv = v.x; best = 4 * q; }
         if (v.y > bv) { bv = v.y; best = 4 * q + 1; }
         if (v.z > bv) { bv = v.z; best = 4 * q + 2; }
@@ -874,7 +891,9 @@ template <int KS>
 int launch_ctc(const float* logits, float* grad, const int* flat_labels, const int* label_len, const int* input_len,
                int T, int N, int blank, float grad_scale, float* costs, cudaStream_t st) {
   size_t smem = ctc_smem_bytes(T, KS);
-  if (smem > 200 * 1024) return CRNN_UNSUPPORTED;
+  if (smem > 200 * 1024)
+    return crnn_fail(CRNN_UNSUPPORTED, "ctc_loss: T = %d frames need %zu bytes of shared memory at KS = %d (limit %d)", T, smem, KS,
+                     200 * 1024);
   CUDA_TRY(cudaFuncSetAttribute(ctc_loss_kernel<KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   ctc_loss_kernel<KS><<<N, CTC_THREADS, smem, st>>>(logits, grad, flat_labels, label_len, input_len, T, N, blank, grad_scale,
                                            costs);
@@ -980,7 +999,10 @@ extern "C" int crnn_ctc_greedy(const float* logits, const int* input_len, int T,
   if (!logits || !input_len || !out || !out_len || T <= 0 || N <= 0) return crnn_fail(CRNN_INVALID_VALUE, "ctc_greedy: bad args");
   if (C != CTC_C) return crnn_fail(CRNN_UNSUPPORTED, "ctc: C must be 64");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  ctc_greedy_kernel<<<(N + 3) / 4, 128, 0, st>>>(logits, input_len, T, N, tf_blank, strip, out, out_len);
+  if (reinterpret_cast<uintptr_t>(logits) % 16 == 0)
+    ctc_greedy_kernel<true><<<(N + 3) / 4, 128, 0, st>>>(logits, input_len, T, N, tf_blank, strip, out, out_len);
+  else
+    ctc_greedy_kernel<false><<<(N + 3) / 4, 128, 0, st>>>(logits, input_len, T, N, tf_blank, strip, out, out_len);
   CUDA_TRY(cudaGetLastError());
   return CRNN_OK;
 }

@@ -22,7 +22,7 @@ W = 100
 T = W // 4 - 1
 
 
-def _batch(N):
+def _batch(N, W=W):
     from oracle import crnn_oracle as O
     pn = O.randomize_params(O.init_params(3, dtype=np.float32, logits_scale=10.0))
     rng = np.random.default_rng(N)
@@ -41,7 +41,8 @@ def _per_sample(x, N):
 
 def _run(mode, pn, data, tsl, training):
     from lstm_ctc_ocr_b200 import engine
-    N = data.shape[0]
+    N, W = data.shape[:2]
+    T = W // 4 - 1
     os.environ["CRNN_LSTM_IMPL"] = mode
     try:
         m = engine.CrnnModel(device=DEV)
@@ -70,6 +71,7 @@ def _same_rows(a, b):
 
 
 def _assert_same(a, b, tsl, what):
+    T = a["lstm_out"].shape[1]
     same = _same_rows(a, b)
     assert np.array_equal(a["lstm_out"][same], b["lstm_out"][same]), f"{what}: lstm_out"
     if "gates" in a and "gates" in b:
@@ -80,9 +82,10 @@ def _assert_same(a, b, tsl, what):
                 assert np.array_equal(a[k][:, n, :L], b[k][:, n, :L]), f"{what}: {k} of sample {n}"
 
 
-@pytest.mark.parametrize("N", [1, 63, 130, 200, 1024])
-def test_exchange_modes_and_training_are_bit_identical(N):
-    pn, data, tsl = _batch(N)
+def check_modes_bit_identical(N, W=W):
+    """Every exchange mode, inference and training, two launches each, on one batch of N lines of width W."""
+    T = W // 4 - 1
+    pn, data, tsl = _batch(N, W)
     ref_inf = ref_trn = None
     for mode in MODES:
         inf = _run(mode, pn, data, tsl, training=False)
@@ -99,3 +102,8 @@ def test_exchange_modes_and_training_are_bit_identical(N):
     L = np.minimum(np.maximum(tsl, 0), T)
     past = np.arange(T)[None, :] >= L[:, None]
     assert not ref_inf["lstm_out"][past].any()
+
+
+@pytest.mark.parametrize("N", [1, 63, 130, 200, 1024])
+def test_exchange_modes_and_training_are_bit_identical(N):
+    check_modes_bit_identical(N)

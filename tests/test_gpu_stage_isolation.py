@@ -81,11 +81,11 @@ def argmax_check(ck, stage, am, pre, pooled, c):
                wrong_clear=wrong_clear, wrong_near_tie=wrong_near, live=int(live.sum()))
 
 
-def _setup(N, W, widths, seed=5):
+def _setup(N, W, widths, seed=5, max_label=4):
     from lstm_ctc_ocr_b200 import engine
     from oracle import crnn_oracle as O
     pn = O.randomize_params(O.init_params(3, dtype=np.float32, logits_scale=10.0))
-    data, lab, ll, tsl = O.synth_batch(N, W, seed=seed, widths=widths_of(N, W, widths), min_len=1, max_len=4)
+    data, lab, ll, tsl = O.synth_batch(N, W, seed=seed, widths=widths_of(N, W, widths), min_len=1, max_len=max_label)
     m = engine.CrnnModel(device=DEV)
     m.load_params(pn)
     return m, pn, data, lab, ll, tsl
@@ -275,12 +275,12 @@ def _backward_checks(ck, F_, grad, dlogits, bnp):
     ck.exact("conv4_1/biases_zero", grad["conv4_1/biases"], 0.0)
 
 
-def _run_stage_checks(case, N, W, widths, dev="cpu", chunk=None, ctc=None, ck=None):
+def _run_stage_checks(case, N, W, widths, dev="cpu", chunk=None, ctc=None, ck=None, max_label=4):
     """The training-mode forward and backward of one batch, every stage checked on its own inputs.  dev: where the fp64
     references run; chunk: images per reference evaluation (the whole batch by default).  ctc(ck, logits, lab, ll, tsl):
-    returns the backward's d logits (default: a seeded random one).  Returns the model, the operands (_Refs) and the
-    checker (Checker(case) unless given), not yet asserted."""
-    m, pn, data, lab, ll, tsl = _setup(N, W, widths)
+    returns the backward's d logits (default: a seeded random one).  max_label: label lengths are drawn from 1 ..
+    max_label.  Returns the model, the operands (_Refs) and the checker (Checker(case) unless given), not yet asserted."""
+    m, pn, data, lab, ll, tsl = _setup(N, W, widths, max_label=max_label)
     T = W // 4 - 1
     t = lambda a: torch.tensor(a, device=DEV)
     m.set_training(True)

@@ -143,9 +143,9 @@ def _ref_self_check(ck, F_):
         ck.close("ref_cpu/" + k, out[F_.dev][k]["out"].cpu(), cpu["out"], cpu["acc"], key="ref_cpu")
 
 
-def _inference_plan_checks(ck, F_, N, W):
-    """bench.py's plan: a fresh model in inference mode on the same batch, every forward stage against the references,
-    and its front end against the training plan's taps."""
+def _inference_plan_checks(ck, F_, N, W, chunk=CHUNK):
+    """bench.py's plan: a fresh model in inference mode on the same batch, every forward stage against the references
+    (over chunks of `chunk` images), and its front end against the training plan's taps."""
     from lstm_ctc_ocr_b200 import engine
     m = engine.CrnnModel(device=DEV)
     m.load_params(F_.pn)
@@ -159,7 +159,7 @@ def _inference_plan_checks(ck, F_, N, W):
         a, b = G[k].double(), F_.G[k].double()
         ck._record(f"{k}_within_1ulp_of_training_plan", float(((a - b).abs() / ulp_bf16(torch.maximum(a.abs(), b.abs()))).max()))
     F_.G.clear()
-    Fi = B._Refs(F_.pn, G, R, F_.data, F_.tsl, logits, N, W, F_.dev, CHUNK)
+    Fi = B._Refs(F_.pn, G, R, F_.data, F_.tsl, logits, N, W, F_.dev, chunk)
     B._forward_checks(ck, Fi, train=False)
 
 

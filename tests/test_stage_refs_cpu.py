@@ -27,12 +27,16 @@ def rel(a, b):
     return float((a - b).abs().max() / max(float(b.abs().max()), 1e-30))
 
 
-@pytest.fixture(scope="module")
-def chain():
+# the widths evaluation feeds beyond 3 x 24: T = 1 and 2 (a crop a few pixels wide; lengths 0, 1 and 2) and T = 128
+# (W = 516, H = 129: the backward rows of the input projection cross a 128-row tile)
+EDGE_CHAINS = [pytest.param((3, 8, [8, 8, 4]), id="N3_W8"), pytest.param((2, 12, [12, 9]), id="N2_W12"),
+               pytest.param((1, 516, [516]), id="N1_W516")]
+
+
+def _make_chain(N, W, widths):
     torch.manual_seed(0)
-    N, W = 3, 24
     p = O.randomize_params(O.init_params(3, dtype=np.float64, logits_scale=3.0), scale=0.3)
-    data, lab, ll, tsl = O.synth_batch(N, W, seed=7, widths=[24, 17, 4], min_len=1, max_len=2, dtype=np.float64)
+    data, lab, ll, tsl = O.synth_batch(N, W, seed=7, widths=widths, min_len=1, max_len=2, dtype=np.float64)
     pt = O.to_torch(p, requires_grad=True)
     logits, acts = O.forward(pt, data, tsl, return_all=True)
     loss = O.ctc_loss_torch(logits, lab, ll, tsl).mean()
@@ -44,6 +48,16 @@ def chain():
     A = {k: (S.nhwc(v.detach()) if isinstance(v, torch.Tensor) and v.dim() == 4 else v) for k, v in acts.items()}
     return dict(N=N, W=W, T=W // 4 - 1, H2=W // 4, tsl=tsl, data=torch.as_tensor(data), P=P, A=A, logits=logits.detach(),
                 dlogits=dlogits, grads=grads)
+
+
+@pytest.fixture(scope="module")
+def chain():
+    return _make_chain(3, 24, [24, 17, 4])
+
+
+@pytest.fixture(scope="module", params=EDGE_CHAINS)
+def edge_chain(request):
+    return _make_chain(*request.param)
 
 
 def _pad_rows(x, H2):
@@ -78,7 +92,14 @@ def _forward_chain(c):
 
 
 def test_forward_stage_chain_reproduces_the_oracle(chain):
-    c = chain
+    _check_forward_chain(chain)
+
+
+def test_forward_stage_chain_at_edge_widths(edge_chain):
+    _check_forward_chain(edge_chain)
+
+
+def _check_forward_chain(c):
     r = _forward_chain(c)
     A, T, H2 = c["A"], c["T"], c["H2"]
     for k in ("conv1", "conv2", "conv3_1", "conv3_2", "conv4_1", "conv4_2"):
@@ -118,7 +139,14 @@ def test_layout_helpers_round_trip():
 
 
 def test_backward_stage_chain_reproduces_oracle_gradients(chain):
-    c = chain
+    _check_backward_chain(chain)
+
+
+def test_backward_stage_chain_at_edge_widths(edge_chain):
+    _check_backward_chain(edge_chain)
+
+
+def _check_backward_chain(c):
     r = _forward_chain(c)
     P, A, G, T, H2, tsl, eps = c["P"], c["A"], c["grads"], c["T"], c["H2"], c["tsl"], O.BN_EPS
     got = {}
@@ -177,9 +205,16 @@ def _zero_pair(x):
 
 
 def test_x3_stage_chain_reproduces_the_oracle(chain):
+    _check_x3_chain(chain)
+
+
+def test_x3_stage_chain_at_edge_widths(edge_chain):
+    _check_x3_chain(edge_chain)
+
+
+def _check_x3_chain(c):
     """The f32-class layouts with lo = 0, wl = 0 and identity rounding: split-pair conv / GEMM stages, an input projection
     without bias in natural gate and frame order, the cell adding the bias and reading frame len-1-step backwards."""
-    c = chain
     P, A, T, H2, tsl = c["P"], c["A"], c["T"], c["H2"], c["tsl"]
     Wp = {k: _zero_pair(v) for k, v in P.items() if k.endswith("weights")}
     for k, src, fn in (("conv2", "conv1", S.conv_relu_pool22_stage), ("conv3_1", "conv2", S.conv_relu_stage),
@@ -355,12 +390,20 @@ def test_vectorised_layout_helpers_equal_their_loops():
 
 
 def test_chunked_references_equal_the_whole_batch(chain):
+    _check_chunked_references(chain)
+
+
+def test_chunked_references_at_edge_widths(edge_chain):
+    _check_chunked_references(edge_chain)
+
+
+def _check_chunked_references(c):
     """Per-image stages over image chunks concatenate to the whole-batch result exactly; the batch reductions (BatchNorm
     sums and backward, weight and bias gradients, masked column sums) summed over chunks agree to 1e-12."""
-    c = chain
     r = _forward_chain(c)
     P, A, T, H2, tsl, eps = c["P"], c["A"], c["T"], c["H2"], c["tsl"], O.BN_EPS
-    parts = [slice(0, 2), slice(2, 3)]
+    cut = max(1, c["N"] - 1)                               # the last image on its own (one chunk when N = 1)
+    parts = [slice(0, cut)] + ([slice(cut, c["N"])] if cut < c["N"] else [])
     cat = lambda f: {k: torch.cat([f(s)[k] for s in parts]) for k in f(parts[0]) if torch.is_tensor(f(parts[0])[k])}
     for k, v in cat(lambda s: S.conv_relu_pool22_stage(A["conv1"][s], P["conv2/weights"], P["conv2/biases"])).items():
         assert torch.equal(v, S.conv_relu_pool22_stage(A["conv1"], P["conv2/weights"], P["conv2/biases"])[k]), k

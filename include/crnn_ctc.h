@@ -174,11 +174,11 @@ int     crnn_total_loss(crnn_model* m, const float* costs, int N, float* loss_ou
                         crnn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
- * Training.  Replaces tf.gradients + tf.clip_by_global_norm(., 10.0) + AdamOptimizer.apply_gradients
+ * Training.  Replaces tf.gradients + tf.clip_by_global_norm(., 10.0) + {Adam, RMSProp, Momentum}Optimizer.apply_gradients
  * (lib/lstm/train.py:73-83).  Protocol per step:
  *   crnn_model_set_training(m, 1) once; crnn_forward (saves what the backward needs in the workspace);
  *   crnn_ctc_loss with grad != NULL and grad_scale = 1/N  -> dlogits;  crnn_backward -> flat `grads` buffer;
- *   [data parallel: all-reduce(SUM) `grads` across ranks];  crnn_clip_adam_step.
+ *   [data parallel: all-reduce(SUM) `grads` across ranks];  crnn_clip_adam_step (or _momentum_step / _rmsprop_step).
  * ---------------------------------------------------------------------------------------- */
 int     crnn_model_set_training(crnn_model* m, int flag);
 int     crnn_backward(crnn_model* m, const float* data, const int* time_step_len, const float* dlogits,
@@ -188,6 +188,20 @@ int     crnn_backward(crnn_model* m, const float* data, const int* time_step_len
  * Single GPU: grad_mul = wd_mul = 1.  Data parallel after a SUM all-reduce: grad_mul = 1/world, wd_mul = world. */
 int     crnn_clip_adam_step(crnn_model* m, float lr, float clip, int step, float grad_mul, float wd_mul,
                             crnn_stream_t stream);
+/* The reference's other two solvers (cfg.TRAIN.SOLVER, lib/lstm/train.py:73-76), with the same gradient finish, averaging and
+ * global-norm clip as crnn_clip_adam_step (same grad_mul / wd_mul meaning); g below is the clipped gradient.  Their state lives
+ * in the two slot buffers bound through crnn_model_bind:
+ *   Momentum (TF MomentumOptimizer, no Nesterov): adam_m holds accum (initialise to 0; adam_v is not used and may be NULL).
+ *     accum = accum*momentum + g;  theta -= lr*accum.
+ *   RMSProp (TF RMSPropOptimizer, not centred; TF's defaults decay 0.9, momentum 0, epsilon 1e-10): adam_m holds mom
+ *     (initialise to 0), adam_v holds ms, which THE CALLER MUST INITIALISE TO 1.0 as TF does.
+ *     ms += (g*g - ms)*(1 - decay);  mom = mom*momentum + lr*g/sqrt(ms + epsilon);  theta -= mom.
+ * CRNN_NOT_BOUND when params, grads or a slot the solver uses is not bound; CRNN_INVALID_VALUE for momentum < 0, decay outside
+ * [0, 1], epsilon < 0, or no prior crnn_model_set_training(m, 1).  crnn_last_grad_norm reports the norm of either step. */
+int     crnn_clip_momentum_step(crnn_model* m, float lr, float momentum, float clip, float grad_mul, float wd_mul,
+                                crnn_stream_t stream);
+int     crnn_clip_rmsprop_step(crnn_model* m, float lr, float decay, float momentum, float epsilon, float clip,
+                               float grad_mul, float wd_mul, crnn_stream_t stream);
 int     crnn_last_grad_norm(crnn_model* m, float grad_mul, float* out_host, crnn_stream_t stream);   /* syncs */
 
 /* ------------------------------------------------------------------------------------------

@@ -57,6 +57,8 @@ SIGNATURES = {
     "crnn_model_set_training": (c_int, [c_void_p, c_int]),
     "crnn_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "crnn_clip_adam_step": (c_int, [c_void_p, c_float, c_float, c_int, c_float, c_float, c_void_p]),
+    "crnn_clip_momentum_step": (c_int, [c_void_p, c_float, c_float, c_float, c_float, c_float, c_void_p]),
+    "crnn_clip_rmsprop_step": (c_int, [c_void_p, c_float, c_float, c_float, c_float, c_float, c_float, c_float, c_void_p]),
     "crnn_last_grad_norm": (c_int, [c_void_p, c_float, ctypes.POINTER(c_float), c_void_p]),
     "crnn_model_set_data_parallel": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "crnn_model_set_grad_ready_callback": (c_int, [c_void_p, c_void_p, c_void_p]),

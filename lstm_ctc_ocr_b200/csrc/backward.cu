@@ -1,9 +1,9 @@
-// Backward pass + optimizer orchestration: what tf.gradients / clip_by_global_norm / AdamOptimizer.apply_gradients do in
-// the reference's train_op (lib/lstm/train.py:73-83), as hand-written sm_90a kernels.
+// Backward pass + optimizer orchestration: what tf.gradients / clip_by_global_norm / {Adam, RMSProp, Momentum}Optimizer
+// .apply_gradients do in the reference's train_op (lib/lstm/train.py:73-83), as hand-written sm_90a kernels.
 //   data gradients   : K-major wgmma GEMMs (csrc/gemm.cuh) with transformed weights
 //   weight gradients : MN-major "TN" wgmma GEMMs with split-K f32 reduction (csrc/gemm_tn.cuh)
 //   BPTT             : persistent cluster kernel (csrc/lstm_bwd.cuh)
-//   BN / pool / ReLU / bias / conv1 / clip+Adam : HBM-bound kernels (csrc/backward_kernels.cu)
+//   BN / pool / ReLU / bias / conv1 / clip + solver update : HBM-bound kernels (csrc/backward_kernels.cu)
 #include <cmath>
 #include <cstring>
 
@@ -339,14 +339,10 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
   return CRNN_OK;
 }
 
-// grads <- grads + wd*wd_mul*w on the regularised tensors; g <- g*grad_mul; clip by global norm; TF Adam.
-// Data-parallel use: all-reduce(SUM) the flat gradient buffer first, then call with grad_mul = 1/world, wd_mul = world.
-extern "C" int crnn_clip_adam_step(crnn_model* m, float lr, float clip, int step, float grad_mul, float wd_mul,
-                                   crnn_stream_t stream) {
-  if (!m || step < 1) return crnn_fail(CRNN_INVALID_VALUE, "clip_adam_step: bad args");
-  if (!m->params || !m->grads || !m->adam_m || !m->adam_v) return crnn_fail(CRNN_NOT_BOUND, "clip_adam_step: bind params, grads and Adam slots");
-  if (!m->grad_sumsq) return crnn_fail(CRNN_INVALID_VALUE, "clip_adam_step: call crnn_model_set_training(m, 1) first");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+// The half of every solver step that does not depend on the solver: grads <- grads + wd*wd_mul*w on the L2-regularised tensors
+// (conv kernels + logits matrix) and the global sum of squares into m->grad_sumsq, which the update kernels turn into the clip
+// scale.
+static int finish_gradients(crnn_model* m, float wd_mul, cudaStream_t st) {
   WdSegs segs;
   segs.n = 0;
   for (auto& c : kConvs) {
@@ -355,7 +351,18 @@ extern "C" int crnn_clip_adam_step(crnn_model* m, float lr, float clip, int step
   }
   const TensorInfo* t = m->find("logits/weights");
   segs.off[segs.n] = t->offset; segs.cnt[segs.n] = t->count; segs.n++;
-  CRNN_TRY(launch_grad_finish(m->grads, m->params, segs, m->cfg.weight_decay * wd_mul, m->total, m->grad_sumsq, st));
+  return launch_grad_finish(m->grads, m->params, segs, m->cfg.weight_decay * wd_mul, m->total, m->grad_sumsq, st);
+}
+
+// grads <- grads + wd*wd_mul*w on the regularised tensors; g <- g*grad_mul; clip by global norm; TF Adam.
+// Data-parallel use: all-reduce(SUM) the flat gradient buffer first, then call with grad_mul = 1/world, wd_mul = world.
+extern "C" int crnn_clip_adam_step(crnn_model* m, float lr, float clip, int step, float grad_mul, float wd_mul,
+                                   crnn_stream_t stream) {
+  if (!m || step < 1) return crnn_fail(CRNN_INVALID_VALUE, "clip_adam_step: bad args");
+  if (!m->params || !m->grads || !m->adam_m || !m->adam_v) return crnn_fail(CRNN_NOT_BOUND, "clip_adam_step: bind params, grads and Adam slots");
+  if (!m->grad_sumsq) return crnn_fail(CRNN_INVALID_VALUE, "clip_adam_step: call crnn_model_set_training(m, 1) first");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CRNN_TRY(finish_gradients(m, wd_mul, st));
   const double b1 = 0.9, b2 = 0.999;
   const float lr_t = (float)(lr * std::sqrt(1.0 - std::pow(b2, step)) / (1.0 - std::pow(b1, step)));
   CRNN_TRY(launch_clip_adam(m->params, m->grads, m->adam_m, m->adam_v, m->grad_sumsq, grad_mul, clip, lr_t, (float)b1, (float)b2, 1e-8f,
@@ -365,7 +372,38 @@ extern "C" int crnn_clip_adam_step(crnn_model* m, float lr, float clip, int step
   return CRNN_OK;
 }
 
-// global gradient norm of the last crnn_clip_adam_step (before clipping, after averaging); host-synchronising helper
+// Same gradient finish and clip, then TF MomentumOptimizer; accum lives in the buffer bound as adam_m.
+extern "C" int crnn_clip_momentum_step(crnn_model* m, float lr, float momentum, float clip, float grad_mul, float wd_mul,
+                                       crnn_stream_t stream) {
+  if (!m || !(momentum >= 0.f)) return crnn_fail(CRNN_INVALID_VALUE, "clip_momentum_step: bad args (momentum must be >= 0)");
+  if (!m->params || !m->grads || !m->adam_m) return crnn_fail(CRNN_NOT_BOUND, "clip_momentum_step: bind params, grads and adam_m (accum)");
+  if (!m->grad_sumsq) return crnn_fail(CRNN_INVALID_VALUE, "clip_momentum_step: call crnn_model_set_training(m, 1) first");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CRNN_TRY(finish_gradients(m, wd_mul, st));
+  CRNN_TRY(launch_clip_momentum(m->params, m->grads, m->adam_m, m->grad_sumsq, grad_mul, clip, lr, momentum, m->total, st));
+  m->dirty = true;
+  m->dirty_bwd = true;
+  return CRNN_OK;
+}
+
+// Same gradient finish and clip, then TF RMSPropOptimizer (not centred); mom lives in adam_m, ms in adam_v.
+extern "C" int crnn_clip_rmsprop_step(crnn_model* m, float lr, float decay, float momentum, float epsilon, float clip, float grad_mul,
+                                      float wd_mul, crnn_stream_t stream) {
+  if (!m || !(decay >= 0.f && decay <= 1.f) || !(momentum >= 0.f) || !(epsilon >= 0.f))
+    return crnn_fail(CRNN_INVALID_VALUE, "clip_rmsprop_step: bad args (decay in [0, 1], momentum >= 0, epsilon >= 0)");
+  if (!m->params || !m->grads || !m->adam_m || !m->adam_v)
+    return crnn_fail(CRNN_NOT_BOUND, "clip_rmsprop_step: bind params, grads, adam_m (mom) and adam_v (ms)");
+  if (!m->grad_sumsq) return crnn_fail(CRNN_INVALID_VALUE, "clip_rmsprop_step: call crnn_model_set_training(m, 1) first");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CRNN_TRY(finish_gradients(m, wd_mul, st));
+  CRNN_TRY(launch_clip_rmsprop(m->params, m->grads, m->adam_m, m->adam_v, m->grad_sumsq, grad_mul, clip, lr, decay, momentum, epsilon,
+                               m->total, st));
+  m->dirty = true;
+  m->dirty_bwd = true;
+  return CRNN_OK;
+}
+
+// global gradient norm of the last solver step (before clipping, after averaging); host-synchronising helper
 extern "C" int crnn_last_grad_norm(crnn_model* m, float grad_mul, float* out, crnn_stream_t stream) {
   if (!m || !out || !m->grad_sumsq) return crnn_fail(CRNN_INVALID_VALUE, "last_grad_norm: bad args");
   double v = 0;

@@ -489,7 +489,7 @@ __global__ void cast_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* _
     dst[i] = __float2bfloat16_rn(src[i]);
 }
 
-// ---- optimizer: L2-term gradient + global norm, then clip + Adam (TF formulas, lib/lstm/train.py:73-83) -----------
+// ---- optimizer: L2-term gradient + global norm, then clip + Adam / Momentum / RMSProp (TF formulas, lib/lstm/train.py:73-83)
 __global__ void __launch_bounds__(256) grad_finish_kernel(float* __restrict__ grads, const float* __restrict__ params,
                                                           WdSegs segs, float wd, long long total, double* __restrict__ sumsq) {
   double acc = 0.0;
@@ -516,13 +516,17 @@ __global__ void __launch_bounds__(256) grad_finish_kernel(float* __restrict__ gr
     atomicAdd(sumsq, t);
   }
 }
+// Factor applied to every raw gradient element: the averaging factor times tf.clip_by_global_norm's clip / max(norm, clip),
+// where the global norm of the (already averaged) gradient is sqrt(sumsq) * grad_mul.  clip <= 0 disables clipping.
+__device__ __forceinline__ float clip_scale(const double* __restrict__ sumsq, float grad_mul, float clip) {
+  const float gn = (float)sqrt(*sumsq) * grad_mul;
+  return grad_mul * (clip > 0.f ? clip / fmaxf(gn, clip) : 1.f);
+}
 __global__ void __launch_bounds__(256) clip_adam_kernel(float* __restrict__ params, const float* __restrict__ grads,
                                                         float* __restrict__ m, float* __restrict__ v,
                                                         const double* __restrict__ sumsq, float grad_mul, float clip, float lr_t,
                                                         float b1, float b2, float eps, long long total) {
-  // global norm of the (already averaged) gradient: sqrt(sumsq) * grad_mul
-  const float gn = (float)sqrt(*sumsq) * grad_mul;
-  const float scale = grad_mul * (clip > 0.f ? clip / fmaxf(gn, clip) : 1.f);
+  const float scale = clip_scale(sumsq, grad_mul, clip);
   for (long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4; i < total; i += (long long)gridDim.x * blockDim.x * 4) {
     const float4 g4 = __ldg(reinterpret_cast<const float4*>(grads + i));
     float4 p4 = *reinterpret_cast<float4*>(params + i), m4 = *reinterpret_cast<float4*>(m + i), v4 = *reinterpret_cast<float4*>(v + i);
@@ -537,6 +541,49 @@ __global__ void __launch_bounds__(256) clip_adam_kernel(float* __restrict__ para
     *reinterpret_cast<float4*>(params + i) = p4;
     *reinterpret_cast<float4*>(m + i) = m4;
     *reinterpret_cast<float4*>(v + i) = v4;
+  }
+}
+// TF MomentumOptimizer (use_nesterov=False, ApplyMomentum): accum = accum*momentum + g; var -= lr*accum.  lr multiplies the whole
+// accumulator when it is applied, so a decayed lr shrinks the step taken from the accumulated velocity at once.
+__global__ void __launch_bounds__(256) clip_momentum_kernel(float* __restrict__ params, const float* __restrict__ grads,
+                                                            float* __restrict__ accum, const double* __restrict__ sumsq, float grad_mul,
+                                                            float clip, float lr, float momentum, long long total) {
+  const float scale = clip_scale(sumsq, grad_mul, clip);
+  for (long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4; i < total; i += (long long)gridDim.x * blockDim.x * 4) {
+    const float4 g4 = __ldg(reinterpret_cast<const float4*>(grads + i));
+    float4 p4 = *reinterpret_cast<float4*>(params + i), a4 = *reinterpret_cast<float4*>(accum + i);
+    float* pp = &p4.x; float* aa = &a4.x; const float* gg = &g4.x;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float g = gg[k] * scale;
+      aa[k] = aa[k] * momentum + g;
+      pp[k] -= lr * aa[k];
+    }
+    *reinterpret_cast<float4*>(params + i) = p4;
+    *reinterpret_cast<float4*>(accum + i) = a4;
+  }
+}
+// TF RMSPropOptimizer (centered=False, ApplyRMSProp): ms += (g*g - ms)*(1 - decay); mom = mom*momentum + lr*g/sqrt(ms + eps);
+// var -= mom.  eps sits inside the square root; TF starts ms at 1.0 (the caller initialises it).
+__global__ void __launch_bounds__(256) clip_rmsprop_kernel(float* __restrict__ params, const float* __restrict__ grads,
+                                                           float* __restrict__ mom, float* __restrict__ ms,
+                                                           const double* __restrict__ sumsq, float grad_mul, float clip, float lr,
+                                                           float decay, float momentum, float eps, long long total) {
+  const float scale = clip_scale(sumsq, grad_mul, clip);
+  for (long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4; i < total; i += (long long)gridDim.x * blockDim.x * 4) {
+    const float4 g4 = __ldg(reinterpret_cast<const float4*>(grads + i));
+    float4 p4 = *reinterpret_cast<float4*>(params + i), m4 = *reinterpret_cast<float4*>(mom + i), s4 = *reinterpret_cast<float4*>(ms + i);
+    float* pp = &p4.x; float* mm = &m4.x; float* ss = &s4.x; const float* gg = &g4.x;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float g = gg[k] * scale;
+      ss[k] += (g * g - ss[k]) * (1.f - decay);
+      mm[k] = mm[k] * momentum + lr * g / sqrtf(ss[k] + eps);
+      pp[k] -= mm[k];
+    }
+    *reinterpret_cast<float4*>(params + i) = p4;
+    *reinterpret_cast<float4*>(mom + i) = m4;
+    *reinterpret_cast<float4*>(ms + i) = s4;
   }
 }
 
@@ -633,5 +680,15 @@ int launch_grad_finish(float* grads, const float* params, const WdSegs& segs, fl
 int launch_clip_adam(float* params, const float* grads, float* m, float* v, const double* sumsq, float grad_mul, float clip, float lr_t,
                      float b1, float b2, float eps, long long total, cudaStream_t st) {
   clip_adam_kernel<<<4 * device_sms(), 256, 0, st>>>(params, grads, m, v, sumsq, grad_mul, clip, lr_t, b1, b2, eps, total);
+  LAUNCH_CHECK();
+}
+int launch_clip_momentum(float* params, const float* grads, float* accum, const double* sumsq, float grad_mul, float clip, float lr,
+                         float momentum, long long total, cudaStream_t st) {
+  clip_momentum_kernel<<<4 * device_sms(), 256, 0, st>>>(params, grads, accum, sumsq, grad_mul, clip, lr, momentum, total);
+  LAUNCH_CHECK();
+}
+int launch_clip_rmsprop(float* params, const float* grads, float* mom, float* ms, const double* sumsq, float grad_mul, float clip,
+                        float lr, float decay, float momentum, float eps, long long total, cudaStream_t st) {
+  clip_rmsprop_kernel<<<4 * device_sms(), 256, 0, st>>>(params, grads, mom, ms, sumsq, grad_mul, clip, lr, decay, momentum, eps, total);
   LAUNCH_CHECK();
 }

@@ -28,3 +28,7 @@ int launch_cast_bf16(const float* src, __nv_bfloat16* dst, size_t n, cudaStream_
 int launch_grad_finish(float* grads, const float* params, const WdSegs& segs, float wd, long long total, double* sumsq, cudaStream_t st);
 int launch_clip_adam(float* params, const float* grads, float* m, float* v, const double* sumsq, float grad_mul, float clip, float lr_t,
                      float b1, float b2, float eps, long long total, cudaStream_t st);
+int launch_clip_momentum(float* params, const float* grads, float* accum, const double* sumsq, float grad_mul, float clip, float lr,
+                         float momentum, long long total, cudaStream_t st);
+int launch_clip_rmsprop(float* params, const float* grads, float* mom, float* ms, const double* sumsq, float grad_mul, float clip,
+                        float lr, float decay, float momentum, float eps, long long total, cudaStream_t st);

@@ -27,7 +27,7 @@ int crnn_fail(int status, const char* fmt, ...) {
   return status;
 }
 extern "C" const char* crnn_last_error(void) { return g_err; }
-extern "C" int crnn_version(void) { return 100; }
+extern "C" int crnn_version(void) { return 101; }
 extern "C" const char* crnn_status_string(int s) {
   switch (s) {
     case CRNN_OK: return "CRNN_OK";

@@ -12,6 +12,13 @@ from ._lib import CrnnConfig, CrnnError, check
 NCLASSES = 64
 TF_BLANK = NCLASSES - 1
 
+# solver -> (checkpoint key prefix, slot buffer) pairs; the keys are TF-style slot names, the buffers those bound as adam_m / adam_v
+SOLVER_SLOTS = {"Adam": (("adam_m", "adam_m"), ("adam_v", "adam_v")),
+                "Momentum": (("momentum", "adam_m"),),
+                "RMS": (("rms", "adam_v"), ("rms_momentum", "adam_m"))}
+# tf.train.RMSPropOptimizer defaults: the reference constructs it with the learning rate alone (lib/lstm/train.py:75)
+RMS_DECAY, RMS_MOMENTUM, RMS_EPSILON = 0.9, 0.0, 1e-10
+
 
 def _stream():
     return torch.cuda.current_stream().cuda_stream
@@ -48,6 +55,8 @@ class CrnnModel:
         self.grads = None
         self.adam_m = None
         self.adam_v = None
+        self.solver = "Adam"
+        self.momentum = 0.9
         self._bind()
         self._ws = None
         self._ws_key = None
@@ -55,16 +64,48 @@ class CrnnModel:
 
     # ---- training --------------------------------------------------------------------------
     def set_training(self, flag=True):
-        """Allocate the gradient / Adam-slot buffers (flat f32, same layout as params) and switch the forward to the
-        variant that saves what the backward pass needs."""
+        """Allocate the gradient / solver-slot buffers (flat f32, same layout as params), initialised for the recorded solver,
+        and switch the forward to the variant that saves what the backward pass needs."""
         if flag and self.grads is None:
             self.grads = torch.zeros_like(self.params)
             self.adam_m = torch.zeros_like(self.params)
             self.adam_v = torch.zeros_like(self.params)
+            self.reset_slots()
             self._bind()
         check(self.lib.crnn_model_set_training(self.handle, 1 if flag else 0))
         self.training = bool(flag)
         self._ws_key = None
+
+    def set_solver(self, name, momentum=0.9):
+        """Record the optimizer apply_gradients runs and reset its slots as TensorFlow initialises them.  `name` is one of
+        "Adam" (m = v = 0), "Momentum" (accum = 0 in the adam_m buffer) and "RMS" (mom = 0 in adam_m, ms = 1 in adam_v).
+        `momentum` is MomentumOptimizer's coefficient; RMSProp runs with TF's defaults (decay 0.9, momentum 0, epsilon 1e-10)."""
+        if name not in SOLVER_SLOTS:
+            raise CrnnError(f"unknown solver {name!r}: expected one of {sorted(SOLVER_SLOTS)}")
+        self.solver, self.momentum = name, float(momentum)
+        self.reset_slots()
+
+    def reset_slots(self):
+        """Slots as TF's slot initialisers leave them: zeros, except RMSProp's mean square (adam_v), which starts at 1.0."""
+        if self.adam_m is not None:
+            self.adam_m.zero_()
+            self.adam_v.fill_(1.0 if self.solver == "RMS" else 0.0)
+
+    def apply_gradients(self, lr, step, clip=10.0, grad_mul=1.0, wd_mul=1.0):
+        """Gradient finish (L2 term, global norm), clip by global norm and one update of the recorded solver.  `step` is the
+        1-based global step (only Adam's bias correction reads it); grad_mul / wd_mul as in clip_adam_step."""
+        if self.solver == "Adam":
+            self.clip_adam_step(lr, step, clip=clip, grad_mul=grad_mul, wd_mul=wd_mul)
+        elif self.solver == "Momentum":
+            check(self.lib.crnn_clip_momentum_step(self.handle, float(lr), self.momentum, float(clip), float(grad_mul), float(wd_mul),
+                                                   _stream()))
+        else:
+            check(self.lib.crnn_clip_rmsprop_step(self.handle, float(lr), RMS_DECAY, RMS_MOMENTUM, RMS_EPSILON, float(clip), float(grad_mul),
+                                                  float(wd_mul), _stream()))
+
+    def solver_slots(self):
+        """{checkpoint key prefix: flat slot buffer} of the recorded solver."""
+        return {prefix: getattr(self, buf) for prefix, buf in SOLVER_SLOTS[self.solver]}
 
     def grad_tensor(self, name):
         off, shp = self.table[name]

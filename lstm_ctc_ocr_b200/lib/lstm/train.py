@@ -2,8 +2,13 @@
 output_dir, logdir)``, ``snapshot``, ``restoreLabel``, ``train_model(sess, max_iters, restore)``, ``train_net(...)``.
 
 Every iteration runs ``sess.run([loss, train_op], feed_dict)`` (train.py:129-130): forward, CTC loss + gradient, backward,
-global-norm clip 10.0, Adam -- all on the GPU engine.  Checkpoints are ``.npz`` files holding the TF variable names/layouts,
-Adam slots, lr and the step, named ``<prefix>_ctc_iter_<k>.ckpt.npz`` with a TF-style ``checkpoint`` index file."""
+global-norm clip 10.0 and the optimizer ``cfg.TRAIN.SOLVER`` selects -- all on the GPU engine.  The selection is the reference's
+(train.py:74-76): ``Adam`` -> AdamOptimizer(lr), ``RMS`` -> RMSPropOptimizer(lr) with TF's defaults (decay 0.9, momentum 0,
+epsilon 1e-10), ANY other value -> MomentumOptimizer(lr, cfg.TRAIN.MOMENTUM).
+
+Checkpoints are ``.npz`` files holding the TF variable names/layouts, the solver's slots, lr and the step, named
+``<prefix>_ctc_iter_<k>.ckpt.npz`` with a TF-style ``checkpoint`` index file.  Slot keys per solver: ``adam_m/<var>`` and
+``adam_v/<var>`` (Adam), ``momentum/<var>`` (Momentum), ``rms/<var>`` (the mean square) and ``rms_momentum/<var>`` (RMSProp)."""
 import os
 import re
 
@@ -43,10 +48,18 @@ class TrainOp(Fetch):
         self.global_step.assign(self.global_step.eval() + 1)
         dp = getattr(eng, "_dp", None)
         if dp is not None:
-            dp.step(self.lr.eval(), self.global_step.eval(), clip=self.clip)       # waits for the buckets; clip + Adam on the SUM / world
+            dp.step(self.lr.eval(), self.global_step.eval(), clip=self.clip)       # waits for the buckets; clip + update on the SUM / world
         else:
-            eng.clip_adam_step(self.lr.eval(), self.global_step.eval(), clip=self.clip)
+            eng.apply_gradients(self.lr.eval(), self.global_step.eval(), clip=self.clip)
         return None
+
+
+def solver_from_cfg(train_cfg):
+    """cfg.TRAIN -> (engine solver name, momentum), chosen as the reference chooses its optimizer (train.py:74-76): SOLVER 'Adam'
+    -> "Adam", 'RMS' -> "RMS" (TF defaults, no config key), every other value -> "Momentum" with TRAIN.MOMENTUM.  The momentum is
+    returned for every solver; only Momentum reads it."""
+    name = {"Adam": "Adam", "RMS": "RMS"}.get(train_cfg.SOLVER, "Momentum")
+    return name, float(train_cfg.MOMENTUM)
 
 
 class SolverWrapper(object):
@@ -68,10 +81,7 @@ class SolverWrapper(object):
         eng = sess.engine_for(self.net)
         blob = dict(eng.state_dict())
         if eng.adam_m is not None:
-            for k, (off, shp) in eng.table.items():
-                n = int(np.prod(shp))
-                blob["adam_m/" + k] = eng.adam_m[off:off + n].view(*shp).cpu().numpy()
-                blob["adam_v/" + k] = eng.adam_v[off:off + n].view(*shp).cpu().numpy()
+            blob.update(slot_arrays(eng))
         blob["global_step"] = np.array(getattr(self, "_global_step", Variable(0)).eval())
         blob["lr"] = np.array(getattr(self, "_lr", Variable(cfg.TRAIN.LEARNING_RATE)).eval())
         np.savez(path + ".npz", **blob)
@@ -91,11 +101,8 @@ class SolverWrapper(object):
         blob = np.load(path + ".npz")
         eng = sess.engine_for(self.net)
         eng.load_params({k: blob[k] for k in eng.table})
-        if "adam_m/" + next(iter(eng.table)) in blob.files and eng.adam_m is not None:
-            for k, (off, shp) in eng.table.items():
-                n = int(np.prod(shp))
-                eng.adam_m[off:off + n].copy_(_to_dev(blob["adam_m/" + k], eng))
-                eng.adam_v[off:off + n].copy_(_to_dev(blob["adam_v/" + k], eng))
+        if eng.adam_m is not None:
+            restore_slots(eng, blob)
         return blob
 
     def restoreLabel(self, label_vec, label_len):
@@ -122,6 +129,11 @@ class SolverWrapper(object):
         if not getattr(eng, "_initialised", False):
             eng.load_params(synthetic.init_params(cfg.RNG_SEED))       # global_variables_initializer
             eng._initialised = True
+        solver, momentum = solver_from_cfg(cfg.TRAIN)
+        if eng.solver != solver:
+            eng.set_solver(solver, momentum)                          # the slots start from TF's initial values
+        else:
+            eng.momentum = momentum                                   # same solver: its slots carry over (a second train_model)
         eng.set_training(True)
         if parallel.world_size() > 1 and getattr(eng, "_dp", None) is None:
             # parameter broadcast, global-batch BatchNorm over peer memory, overlapped gradient buckets (parallel.DataParallel)
@@ -152,8 +164,6 @@ class SolverWrapper(object):
 
     def train_model(self, sess, max_iters, restore=False, train_gen=None, val_gen=None):
         from ... import parallel
-        if cfg.TRAIN.SOLVER != "Adam":
-            raise NotImplementedError("only the Adam solver of lstm/lstm.yml is implemented (RMS/Momentum are unused upstream)")
         train_gen = train_gen or get_batch(num_workers=12, batch_size=cfg.TRAIN.BATCH_SIZE, vis=False)
         val_gen = val_gen or get_batch(num_workers=1, batch_size=cfg.VAL.BATCH_SIZE, vis=False)
         loss, dense_decoded = self.net.build_loss()
@@ -194,6 +204,36 @@ class SolverWrapper(object):
 def _to_dev(arr, eng):
     import torch
     return torch.as_tensor(np.asarray(arr, dtype=np.float32).reshape(-1), device=eng.device)
+
+
+def slot_arrays(eng):
+    """{"<slot prefix>/<TF variable>": array} of the engine's current solver slots (engine.SOLVER_SLOTS names the prefixes)."""
+    out = {}
+    for prefix, buf in eng.solver_slots().items():
+        for k, (off, shp) in eng.table.items():
+            n = int(np.prod(shp))
+            out[prefix + "/" + k] = buf[off:off + n].view(*shp).cpu().numpy()
+    return out
+
+
+def restore_slots(eng, blob):
+    """Load the configured solver's slots from a checkpoint that holds them.  A params-only checkpoint leaves the slots freshly
+    initialised as TF initialises them; one that holds only another solver's slots raises, as TF's Saver fails on a checkpoint
+    without the graph's slot variables."""
+    from ...engine import SOLVER_SLOTS
+    slots = eng.solver_slots()
+    files = set(blob.files)
+    if all(p + "/" + k in files for p in slots for k in eng.table):
+        for prefix, buf in slots.items():
+            for k, (off, shp) in eng.table.items():
+                buf[off:off + int(np.prod(shp))].copy_(_to_dev(blob[prefix + "/" + k], eng))
+        return
+    known = {p for pairs in SOLVER_SLOTS.values() for p, _ in pairs}
+    held = sorted({f.split("/", 1)[0] for f in files if "/" in f} & known)
+    if held:
+        raise KeyError("checkpoint holds the slots {} but not all of those of the configured solver {} ({})".format(
+            held, eng.solver, sorted(slots)))
+    eng.reset_slots()
 
 
 def train_net(network, imgdb, pre_train, output_dir, log_dir, max_iters=40000, restore=False):

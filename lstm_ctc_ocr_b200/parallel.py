@@ -7,8 +7,9 @@ The reference is single-device; reproducing ITS function on a sharded batch need
   release/acquire flags at system scope, fixed-order summation -> bit-identical statistics on all ranks, no collective launch);
   ``setup_peer_memory`` creates the inboxes (cudaMalloc + CUDA IPC, handles exchanged through torch.distributed).  Without peer
   memory the C library calls back into ``_allreduce_cb`` (an NCCL all-reduce of the 8 KB buffer).
-* **Gradients**: SUM over ranks of the flat f32 buffer (7 158 592 floats, 28.6 MB), then ``crnn_clip_adam_step(grad_mul=1/world,
-  wd_mul=world)`` -- the global-norm clip sees the reduced gradient (train.py:81-83).  ``crnn_backward`` announces each contiguous
+* **Gradients**: SUM over ranks of the flat f32 buffer (7 158 592 floats, 28.6 MB), then the configured solver's step
+  (``CrnnModel.apply_gradients(grad_mul=1/world, wd_mul=world)``: Adam, Momentum or RMSProp) -- the global-norm clip sees the
+  reduced gradient (train.py:81-83).  ``crnn_backward`` announces each contiguous
   range of the buffer as soon as it is final (LSTM+logits first, conv1+conv2 last); ``GradBuckets`` all-reduces every range
   on a side stream while the rest of the backward pass runs, and ``finish()`` makes the compute stream wait for them.
 """
@@ -248,7 +249,7 @@ class DataParallel(object):
 
     def step(self, lr, step, clip=10.0):
         self.reduce_gradients()
-        self.eng.clip_adam_step(lr, step, clip=clip, grad_mul=1.0 / self.world, wd_mul=float(self.world))
+        self.eng.apply_gradients(lr, step, clip=clip, grad_mul=1.0 / self.world, wd_mul=float(self.world))
 
     def close(self):
         if self.buckets is not None:

@@ -164,6 +164,20 @@ int     crnn_forward_pageable(crnn_model* m, const float* pageable_data, float* 
                               size_t workspace_bytes, int chunks, int host_threads, crnn_stream_t stream,
                               crnn_stream_t copy_stream);
 
+/* Packed evaluation: N text lines of different widths in one call, each computed as if it were fed alone to crnn_forward as
+ * [1, W_i, 32].  data [N,W,32] f32: line i in columns [0, W_i) of its slot (columns past W_i are ignored); line_width [N] i32 =
+ * W_i, clamped on the device to [8, W] and rounded down to a multiple of 4; time_step_len [N] i32 -> logits_out [W/4-1, N, 64].
+ * Every SAME convolution sees zero padding at the line's own right edge, and conv4_1 / conv4_2 normalise with the line's own
+ * batch statistics (count W_i, like the reference's one-line-per-run evaluation, lib/lstm/test.py).  Only frames t < W_i/4 - 1
+ * are defined: time_step_len[i] must be <= W_i/4 - 1; like input_len elsewhere it cannot be checked without a sync.
+ * All pointers are device pointers; asynchronous on `stream`, no allocation.  The workspace (crnn_lines_workspace_size) is
+ * the inference plan's plus the per-line statistics and coefficients (about 33 MB more at N = 1024).
+ * CRNN_INVALID_VALUE for a model in training mode (training uses whole-batch statistics) and the shape errors of
+ * crnn_forward; CRNN_UNSUPPORTED for compute_dtype 2 or 3.  crnn_debug_tap / _raw read this forward afterwards. */
+int     crnn_lines_workspace_size(const crnn_model* m, int N, int W, size_t* bytes);
+int     crnn_forward_lines(crnn_model* m, const float* data, const int* line_width, const int* time_step_len, int N, int W,
+                           float* logits_out, void* workspace, size_t workspace_bytes, crnn_stream_t stream);
+
 /* The host-side copy crnn_forward_pageable uses, on its own: `bytes` from `src` to `dst` (plain host pointers, non-overlapping) split
  * over `threads` threads of the library's persistent pool (the caller's thread included).  No CUDA call is made. */
 int     crnn_host_copy(void* dst, const void* src, size_t bytes, int threads);
@@ -251,7 +265,8 @@ int     crnn_peer_error(crnn_model* m, int* err_host);   /* 1 if an exchange tim
 int     crnn_debug_tap(crnn_model* m, const char* name, float* dst, size_t dst_elems,
                        void* workspace, crnn_stream_t stream);
 /* Same for the buffers that are not bf16, copied byte for byte: "bn" (f32 [2 layers][scale, shift, mean, invstd][512]),
- * "stats" (f64 [2 layers][sum, sum of squares][512]) and, training-mode plans only, "am1" "am2" "am3" (u8 pool
+ * "stats" (f64 [2 layers][sum, sum of squares][512]); after crnn_forward_lines per line: "bn" f32 [2 layers][N][4][512], "stats"
+ * f64 [2 layers][N][2][512].  And, training-mode plans only, "am1" "am2" "am3" (u8 pool
  * window index dy*2+dx per pooled element) and "csave" (f32 saved cell state, layout of lstm_c_off).
  * f32-class models: "bn" and "stats" (same layouts), "cst" (f32 final cell state [2 dirs][Npad][256]) and the
  * activation buffers as stored under their tap names "conv1" .. "conv5", "lstm_out": split mode (2) bf16 rows

@@ -69,10 +69,12 @@ struct Params {
   uint8_t* argmax;          // TRAIN: window index (dy*2+dx) of the max, [N, W/2, 16, 64] (this launch's images)
   int N, W, tiles_per_img;  // tiles_per_img = ceil(W / 16)
   int img0;                 // image coordinate of the first image in the output map
+  const int* line_w;        // LINES: [N] clamped line widths (this launch's images); input columns >= line_w read as zero and
+                            // pooled rows >= line_w / 2 are stored as zero (packed evaluation, crnn_forward_lines)
 };
 
 // `tmO`: NHWC map of the whole pooled output [*, W/2, 16, 64] bf16, box [64, 16, 4, 1], SWIZZLE_128B
-template <bool TRAIN>
+template <bool TRAIN, bool LINES = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const __grid_constant__ CUtensorMap tmO, const Params p) {
   extern __shared__ uint8_t smem_raw[];
   // aligned by OFFSET (not by casting through an integer): the pointers stay in the shared address space -> LDS/STS, not LD/ST
@@ -127,13 +129,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const __grid_c
     auto fetch = [&](int tile, float4 (&v)[2]) {
       const int n = tile / p.tiles_per_img;
       const int h0 = (tile - n * p.tiles_per_img) * 16;
+      const int wl = LINES ? __ldg(p.line_w + n) : p.W;
 #pragma unroll
       for (int k = 0; k < 2; ++k) {
         const int e = bt + k * BUILD_THREADS;
         const int r = e >> 3, c4 = e & 7;
         const int gr = h0 - 1 + r;
         v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (e < IN_ROWS * 8 && gr >= 0 && gr < p.W) v[k] = __ldg(reinterpret_cast<const float4*>(p.data + ((size_t)n * p.W + gr) * 32) + c4);
+        if (e < IN_ROWS * 8 && gr >= 0 && gr < wl) v[k] = __ldg(reinterpret_cast<const float4*>(p.data + ((size_t)n * p.W + gr) * 32) + c4);
       }
     };
     auto stash = [&](float* stg, const float4 (&v)[2]) {
@@ -230,6 +233,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const __grid_c
       // previous tile's barrier.
       uint8_t* so = stg_out + (it & 1) * OUT_BYTES;
       uint8_t* sa = stg_am + (it & 1) * AM_BYTES;
+      const int hl_end = LINES ? (__ldg(p.line_w + nl) >> 1) - ((h0 >> 1) + 4 * wgi) : 4;   // pooled rows of this tile inside the line
 #pragma unroll
       for (int pr = 0; pr < 4; ++pr) {                       // pooled row pr: image rows 2pr, 2pr+1 = column groups 8pr + i, 8pr + i + 4
 #pragma unroll
@@ -263,6 +267,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const __grid_c
             const uint32_t r = __shfl_xor_sync(0xffffffffu, even ? s8 : s0, 4);
             wv[e] = even ? ((s0 & 0xFFFFu) | (r << 16)) : ((r & 0xFFFFu) | (v & 0xFFFF0000u));
             if (TRAIN) wa[e] = even ? (a0 | ((r >> 16) << 8)) : ((r >> 16) | (a8 << 8));
+            if (LINES && pr >= hl_end) wv[e] = 0u;
           }
           // Odd lanes store their two positions in the other order: in each store instruction the even lanes' rows (chunk
           // 2*warp) and the odd lanes' rows (chunk 2*warp + 1) are 4 rows apart, so the swizzled 16-B chunks of the warp are all
@@ -293,20 +298,23 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const __grid_c
 }  // namespace conv1tc
 
 // `out`: NHWC map of the pooled output [*, W/2, 16, 64] bf16 with box [64, 16, 4, 1]; this launch writes images
-// img0 .. img0+N-1 of it (`data` and `argmax` point at image img0)
+// img0 .. img0+N-1 of it (`data` and `argmax` point at image img0).  `line_w` != nullptr: packed evaluation lines (inference only)
 static int launch_conv1_tc(const CUtensorMap& out, const float* data, const float* w, const float* b, int img0, uint8_t* argmax,
-                           int N, int W, int num_sms, cudaStream_t st) {
+                           int N, int W, int num_sms, cudaStream_t st, const int* line_w = nullptr) {
   conv1tc::Params p;
   p.data = data; p.wgt = w; p.bias = b; p.argmax = argmax; p.N = N; p.W = W; p.tiles_per_img = (W + 15) / 16; p.img0 = img0;
+  p.line_w = line_w;
   static bool attr = false;
   if (!attr) {
     CUDA_TRY(cudaFuncSetAttribute(conv1tc::conv1_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv1tc::SMEM_BYTES));
     CUDA_TRY(cudaFuncSetAttribute(conv1tc::conv1_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv1tc::SMEM_BYTES));
+    CUDA_TRY(cudaFuncSetAttribute(conv1tc::conv1_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv1tc::SMEM_BYTES));
     attr = true;
   }
   const int tiles = N * p.tiles_per_img;
   const int grid = tiles < num_sms ? tiles : num_sms;
-  if (argmax != nullptr) conv1tc::conv1_tc_kernel<true><<<grid, conv1tc::NUM_THREADS, conv1tc::SMEM_BYTES, st>>>(out, p);
+  if (line_w != nullptr) conv1tc::conv1_tc_kernel<false, true><<<grid, conv1tc::NUM_THREADS, conv1tc::SMEM_BYTES, st>>>(out, p);
+  else if (argmax != nullptr) conv1tc::conv1_tc_kernel<true><<<grid, conv1tc::NUM_THREADS, conv1tc::SMEM_BYTES, st>>>(out, p);
   else conv1tc::conv1_tc_kernel<false><<<grid, conv1tc::NUM_THREADS, conv1tc::SMEM_BYTES, st>>>(out, p);
   CUDA_TRY(cudaGetLastError());
   return CRNN_OK;

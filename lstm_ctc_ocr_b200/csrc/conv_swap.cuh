@@ -44,9 +44,10 @@ struct Params {
   const float* bias;      // [128]
   __nv_bfloat16* out;
   uint8_t* argmax;        // TRAIN: window index (dy*2+dx) of the max, same shape as out
+  const int* line_w;      // LINES: [images] clamped line widths (input columns); pooled rows >= line_w / 4 are stored as zero
 };
 
-template <bool TRAIN>
+template <bool TRAIN, bool LINES = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmO,
                   const Params p) {
@@ -136,6 +137,7 @@ conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
         // shared memory as two [64 positions][64 channels] SWIZZLE_128B boxes and leaves with two TMA stores (rows >= H/2 dropped).
         if (issuer) ptx::bulk_wait_read_all();       // the previous tile's stores have read the buffer
         ptx::bar_sync(1, 256);
+        const int ph_end = LINES ? (__ldg(p.line_w + n) >> 2) - (h0 >> 1) : 8;   // pooled rows of this tile inside the line
 #pragma unroll
         for (int ph = 0; ph < 8; ++ph) {
 #pragma unroll
@@ -147,7 +149,8 @@ conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
             const uint32_t b8 = __bfloat16_as_ushort(__float2bfloat16_rn(fmaxf(m8 + bias8, 0.f)));
             // exchange with lane l ^ 4 so that each lane holds an adjacent channel pair: (f0, f0 + 1) or (f0 + 7, f0 + 8)
             const uint32_t r = __shfl_xor_sync(0xffffffffu, even ? b8 : b0, 4);
-            const uint32_t word = even ? (b0 | (r << 16)) : (r | (b8 << 16));
+            uint32_t word = even ? (b0 | (r << 16)) : (r | (b8 << 16));
+            if (LINES && ph >= ph_end) word = 0u;
             const int row = ph * 8 + 4 * e + (l & 3), ch = even ? f0 : f0 + 7;     // pooled position, first channel of the pair
             *reinterpret_cast<uint32_t*>(stg + (ch >> 6) * 8192 + row * 128 + ((((ch >> 3) & 7) ^ (row & 7)) << 4) + ((ch & 7) << 1)) = word;
           }
@@ -313,11 +316,12 @@ conv_dgrad_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
 
 }  // namespace convsw
 
-template <bool TRAIN>
+template <bool TRAIN, bool LINES = false>
 // `out`: NHWC map of the pooled output [N, H/2, 8, 128], box [64, 8, 8, 1] (one tile = 8 pooled rows); only <false> stores through it
 static int launch_conv2_swap(const CUtensorMap& x, const CUtensorMap& w, const CUtensorMap& out, const convsw::Params& p, int num_sms,
                              cudaStream_t st) {
-  auto kern = convsw::conv2_swap_kernel<TRAIN>;
+  static_assert(!(TRAIN && LINES), "line masks exist in the inference epilogue only");
+  auto kern = convsw::conv2_swap_kernel<TRAIN, LINES>;
   static bool attr = false;
   if (!attr) {
     CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, convsw::SMEM_BYTES));

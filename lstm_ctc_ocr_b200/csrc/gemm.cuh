@@ -93,6 +93,9 @@ struct Params {
   __nv_bfloat16* lstm_out;      // [Nimg*H, 512]
   const int* seq_len;           // [Nimg]
   int step, Npad, m_tiles_per_dir, T;
+  // LINES instantiations (packed evaluation, crnn_forward_lines): [Nimg] clamped line widths in input columns; conv rows at
+  // h >= line_w[n] / 4 (every LINES layer runs at H = W/4) are stored as zero, and EPI_STATS sums go to slot n of `stats` [Nimg][2][Nc]
+  const int* line_w;
 };
 
 __device__ __forceinline__ float warp_colsum32(const float (&v)[32], int lane) {
@@ -182,11 +185,13 @@ __device__ __forceinline__ float4 rowsum_tree(const uint8_t* box, int rg, int cw
   }
 }
 
-// conv tiles: accumulator row r of tile m_blk is a real output position (h < H, image < Nimg)
+// conv tiles: accumulator row r of tile m_blk is a real output position (h < H, image < Nimg); LINES: and h lies inside its line
+template <bool LINES>
 __device__ __forceinline__ bool conv_row_valid(const Params& p, int m_blk, int r) {
   const int g = m_blk * 4 + (r >> 5);
   const int n_img = g / p.sb_per_img;
   const int h = (g - n_img * p.sb_per_img) * p.bh + (r & 31) / p.Wd;
+  if (LINES) return n_img < p.Nimg && h < (__ldg(p.line_w + n_img) >> 2);
   return n_img < p.Nimg && h < p.H;
 }
 
@@ -202,7 +207,9 @@ __device__ __forceinline__ bool conv_row_valid(const Params& p, int m_blk, int r
 //   are staged as zero): thread = (column pair, 32-row group), 2048 f64 atomics per tile.
 //   EPI_XPROJ, columns >= 1024: rows reversed by sequence length.  When H divides 128 a tile holds whole sequences, so the
 //   reversal is a permutation of staging rows; otherwise the thread stores its words to the reversed rows directly.
-template <int EPI>
+//   LINES (conv epilogues): rows past their line are staged as zero like invalid rows, and a 32-row statistics group -- one
+//   sub-box, which never spans two images -- adds into its own image's sums.
+template <int EPI, bool LINES = false>
 __device__ __forceinline__ void frag_epilogue(const Params& p, const float (&d)[128], uint8_t* stg, const CUtensorMap* tmO,
                                               const int m_blk, const int n_blk, const int wgi, const bool issuer) {
   constexpr bool POOL = (EPI == EPI_RELU_POOL12);
@@ -213,7 +220,7 @@ __device__ __forceinline__ void frag_epilogue(const Params& p, const float (&d)[
   const int r0 = wgi * 64 + 16 * (t >> 5) + (l >> 2);   // fragment rows r0 and r0 + 8
   const int col0 = n_blk * 256;
   bool ok0 = true, ok1 = true;
-  if (EPI == EPI_STATS) { ok0 = conv_row_valid(p, m_blk, r0); ok1 = conv_row_valid(p, m_blk, r0 + 8); }
+  if (EPI == EPI_STATS || LINES) { ok0 = conv_row_valid<LINES>(p, m_blk, r0); ok1 = conv_row_valid<LINES>(p, m_blk, r0 + 8); }
   int s0 = r0, s1 = r0 + 8;                              // staging rows (EPI_XPROJ: destination rows)
   bool direct = false;
   if (EPI == EPI_XPROJ && col0 >= 1024) {
@@ -258,9 +265,10 @@ __device__ __forceinline__ void frag_epilogue(const Params& p, const float (&d)[
         // rows r and r ^ 1 (w pair) sit in lanes l and l ^ 4; rounding to bf16 is monotonic, so max after packing == packing after max
         v0 = ptx::hmax2_bf16(v0, __shfl_xor_sync(0xffffffffu, v0, 4));
         v1 = ptx::hmax2_bf16(v1, __shfl_xor_sync(0xffffffffu, v1, 4));
-        // both lanes of the pair now hold both pooled rows: lane l stores the first, lane l ^ 4 the second (conflict-free)
-        if ((l & 4) == 0) *stg_word(buf, BOX_BYTES, r0 >> 1, c) = v0;
-        else *stg_word(buf, BOX_BYTES, (r0 + 8) >> 1, c) = v1;
+        // both lanes of the pair now hold both pooled rows: lane l stores the first, lane l ^ 4 the second (conflict-free); the
+        // rows of a w pair share h, so either lane's validity is the pooled row's
+        if ((l & 4) == 0) *stg_word(buf, BOX_BYTES, r0 >> 1, c) = ok0 ? v0 : 0u;
+        else *stg_word(buf, BOX_BYTES, (r0 + 8) >> 1, c) = ok1 ? v1 : 0u;
       } else if (EPI == EPI_XPROJ && direct) {
         __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out) + col0 + hf * 128 + c;
         if (m_blk * 128 + r0 < p.M) *reinterpret_cast<uint32_t*>(out + (size_t)(m_blk * 128 + s0) * p.ldo) = v0;
@@ -298,10 +306,16 @@ __device__ __forceinline__ void frag_epilogue(const Params& p, const float (&d)[
       const uint8_t* bb = buf + (cp >> 5) * BOX_BYTES;
       const float4 s = rowsum_tree<1>(bb, rg, cw, 0);
       const int c = col0 + hf * 128 + 2 * cp;
-      atomicAdd(p.stats + c, (double)s.x);
-      atomicAdd(p.stats + c + 1, (double)s.y);
-      atomicAdd(p.stats + p.Nc + c, (double)s.z);
-      atomicAdd(p.stats + p.Nc + c + 1, (double)s.w);
+      double* st = p.stats;
+      if (LINES) {
+        const int n = (m_blk * 4 + rg) / p.sb_per_img;
+        if (n >= p.Nimg) continue;                         // padding sub-box past the last image: all rows zero
+        st += (size_t)n * 2 * p.Nc;
+      }
+      atomicAdd(st + c, (double)s.x);
+      atomicAdd(st + c + 1, (double)s.y);
+      atomicAdd(st + p.Nc + c, (double)s.z);
+      atomicAdd(st + p.Nc + c + 1, (double)s.w);
     }
   }
 }
@@ -709,12 +723,14 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
 
 // KIND 0: bf16 operands, 64 elements per 128 B K-block.  KIND 1: f32 words read as tf32, 32 elements per K-block
 // (forward_x3.cu, compute_dtype 3); tensor maps are FLOAT32 with 32-element boxes, everything else is shared.
-template <int BLOCK_N, int AMODE, int EPI, int STAGES, int KIND = 0>
+// LINES: packed evaluation lines (Params::line_w), frag_epi conv epilogues only
+template <int BLOCK_N, int AMODE, int EPI, int STAGES, int KIND = 0, bool LINES = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
             const Params p) {
   static_assert(BLOCK_N == 64 || BLOCK_N == 128 || BLOCK_N == 256, "BLOCK_N");
   constexpr bool FRAG = frag_epi(BLOCK_N, EPI);          // tmO (output map) is read only by these
+  static_assert(!LINES || (FRAG && AMODE == A_CONV3 && KIND == 0), "line masks exist in the register-side conv epilogues only");
   constexpr int SLICE_N = slice_cols(BLOCK_N, EPI);
   using SM = Smem<BLOCK_N, STAGES, SLICE_N>;
   constexpr int S = SM::S;
@@ -830,7 +846,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
       if (p.debug_skip_epilogue) continue;
       if constexpr (FRAG) {
-        frag_epilogue<EPI>(p, d, reinterpret_cast<uint8_t*>(acc_tile), &tmO, m_blk, n_blk, wgi, issuer);
+        frag_epilogue<EPI, LINES>(p, d, reinterpret_cast<uint8_t*>(acc_tile), &tmO, m_blk, n_blk, wgi, issuer);
       } else {
 #pragma unroll
         for (int s = 0; s < BLOCK_N / SLICE_N; ++s) {

@@ -7,11 +7,11 @@
 
 // `out` is the tensor map the register-side epilogues (gemm::frag_epi) store through: NHWC box [64, Wd, bh (x4 merged), 1] for
 // conv outputs, [64, 128] over [M, ldo] for plain ones.  The other epilogues take no map.
-template <int BN, int AM, int EPI, int ST, int KIND = 0>
+template <int BN, int AM, int EPI, int ST, int KIND = 0, bool LINES = false>
 static int launch_gemm(const CUtensorMap& a, const CUtensorMap& b, const gemm::Params& p, int num_sms, cudaStream_t st,
                        const CUtensorMap* out = nullptr) {
   if (gemm::frag_epi(BN, EPI) && out == nullptr) return crnn_fail(CRNN_INVALID_VALUE, "launch_gemm: epilogue %d needs an output tensor map", EPI);
-  auto kern = gemm::gemm_kernel<BN, AM, EPI, ST, KIND>;
+  auto kern = gemm::gemm_kernel<BN, AM, EPI, ST, KIND, LINES>;
   constexpr int smem = gemm::Smem<BN, ST, gemm::slice_cols(BN, EPI)>::BYTES;
   static bool attr = false;
   if (!attr) {

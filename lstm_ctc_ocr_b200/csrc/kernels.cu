@@ -200,6 +200,87 @@ __global__ void __launch_bounds__(256) bn_apply_relu_pool12_kernel(const uint4* 
   out[i] = o;
 }
 
+// ---- per-line BatchNorm of packed evaluation (crnn_forward_lines): every line normalises over its own W_i positions, as when it
+// is evaluated alone.  line_w [N] = clamped line widths; a line's positions are its H rows h < line_w / 4 times Wd.
+// stats [N][2][C] -> bn [N][4][C] (scale, shift, mean, invstd); one thread per (line, channel), count = line_w[n] (= H2_i * 4)
+__global__ void bn_finalize_lines_kernel(const double* __restrict__ stats, const int* __restrict__ line_w, const float* __restrict__ gamma,
+                                         const float* __restrict__ beta, float eps, float* __restrict__ bn, int N, int C) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N * C) return;
+  const int n = i / C, c = i - n * C;
+  const double count = (double)line_w[n];
+  const double* st = stats + (size_t)n * 2 * C;
+  float* o = bn + (size_t)n * 4 * C;
+  const double mean = st[c] / count;
+  double var = st[C + c] / count - mean * mean;        // population variance
+  if (var < 0) var = 0;
+  const double invstd = 1.0 / sqrt(var + (double)eps);
+  o[c] = (float)(gamma[c] * invstd);
+  o[C + c] = (float)(beta[c] - mean * gamma[c] * invstd);
+  o[2 * C + c] = (float)mean;
+  o[3 * C + c] = (float)invstd;
+}
+
+// bn_apply_relu_kernel with each line's own scale / shift; positions at h >= line_w / 4 are written as zero (SAME padding of the
+// next conv).  in/out [N, H, Wd, C]
+__global__ void __launch_bounds__(256) bn_apply_relu_lines_kernel(const uint4* __restrict__ in, uint4* __restrict__ out,
+                                                                  const float* __restrict__ bn, const int* __restrict__ line_w,
+                                                                  size_t nvec, int H, int Wd, int C) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nvec) return;
+  const int vpc = C / 8;
+  const size_t pos = i / vpc;
+  const int c = (int)(i - pos * vpc) * 8;
+  const size_t row = pos / Wd;                           // n * H + h
+  const int n = (int)(row / H), h = (int)(row - (size_t)n * H);
+  uint4 v = make_uint4(0u, 0u, 0u, 0u);
+  if (h < (__ldg(line_w + n) >> 2)) {
+    const float* scale = bn + (size_t)n * 4 * C;
+    const float* shift = scale + C;
+    const float4 s0 = __ldg(reinterpret_cast<const float4*>(scale + c)), s1 = __ldg(reinterpret_cast<const float4*>(scale + c + 4));
+    const float4 h0 = __ldg(reinterpret_cast<const float4*>(shift + c)), h1 = __ldg(reinterpret_cast<const float4*>(shift + c + 4));
+    v = __ldg(in + i);
+    v.x = bn_relu2(v.x, s0.x, h0.x, s0.y, h0.y);
+    v.y = bn_relu2(v.y, s0.z, h0.z, s0.w, h0.w);
+    v.z = bn_relu2(v.z, s1.x, h1.x, s1.y, h1.y);
+    v.w = bn_relu2(v.w, s1.z, h1.z, s1.w, h1.w);
+  }
+  out[i] = v;
+}
+
+// bn_apply_relu_pool12_kernel with each line's own scale / shift and zero at h >= line_w / 4.  in [N, H, 2*Wo, C] -> out [N, H, Wo, C]
+__global__ void __launch_bounds__(256) bn_apply_relu_pool12_lines_kernel(const uint4* __restrict__ in, uint4* __restrict__ out,
+                                                                         const float* __restrict__ bn, const int* __restrict__ line_w,
+                                                                         size_t nvec_out, int H, int Wo, int C) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nvec_out) return;
+  const int vpc = C / 8;
+  const size_t pos = i / vpc;
+  const int cv = (int)(i - pos * vpc);
+  const int c = cv * 8;
+  const size_t row = pos / Wo;
+  const int n = (int)(row / H), h = (int)(row - (size_t)n * H);
+  uint4 o = make_uint4(0u, 0u, 0u, 0u);
+  if (h < (__ldg(line_w + n) >> 2)) {
+    const float* scale = bn + (size_t)n * 4 * C;
+    const float* shift = scale + C;
+    const float4 s0 = __ldg(reinterpret_cast<const float4*>(scale + c)), s1 = __ldg(reinterpret_cast<const float4*>(scale + c + 4));
+    const float4 h0 = __ldg(reinterpret_cast<const float4*>(shift + c)), h1 = __ldg(reinterpret_cast<const float4*>(shift + c + 4));
+    const uint4 a = __ldg(in + (2 * pos) * vpc + cv), b = __ldg(in + (2 * pos + 1) * vpc + cv);
+    o.x = ptx::hmax2_bf16(bn_relu2(a.x, s0.x, h0.x, s0.y, h0.y), bn_relu2(b.x, s0.x, h0.x, s0.y, h0.y));
+    o.y = ptx::hmax2_bf16(bn_relu2(a.y, s0.z, h0.z, s0.w, h0.w), bn_relu2(b.y, s0.z, h0.z, s0.w, h0.w));
+    o.z = ptx::hmax2_bf16(bn_relu2(a.z, s1.x, h1.x, s1.y, h1.y), bn_relu2(b.z, s1.x, h1.x, s1.y, h1.y));
+    o.w = ptx::hmax2_bf16(bn_relu2(a.w, s1.z, h1.z, s1.w, h1.w), bn_relu2(b.w, s1.z, h1.z, s1.w, h1.w));
+  }
+  out[i] = o;
+}
+
+// line widths as every packed-evaluation kernel reads them: clamped to [8, W] and rounded down to a multiple of 4
+__global__ void clamp_line_width_kernel(const int* __restrict__ in, int* __restrict__ out, int N, int W) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < N) out[i] = min(max(in[i], 8), W) & ~3;
+}
+
 // ------------------------------------------------------------------------------------------------
 // weight re-layout: dst[perm(c)][r] (bf16, K-major GEMM B operand) = src[r][c] (f32, TF layout)
 // perm_mode 0: identity; upc > 0: LSTM gate permutation  j = g*256+u  ->  (u/upc)*4*upc + g*upc + u%upc
@@ -318,6 +399,33 @@ int launch_bn_apply_relu_pool12(const __nv_bfloat16* in, __nv_bfloat16* out, con
   const size_t nvec = out_positions * C / 8;
   bn_apply_relu_pool12_kernel<<<(unsigned)((nvec + 255) / 256), 256, 0, st>>>(
       reinterpret_cast<const uint4*>(in), reinterpret_cast<uint4*>(out), scale, shift, nvec, C);
+  CUDA_TRY(cudaGetLastError());
+  return CRNN_OK;
+}
+int launch_clamp_line_width(const int* in, int* out, int N, int W, cudaStream_t st) {
+  clamp_line_width_kernel<<<(N + 255) / 256, 256, 0, st>>>(in, out, N, W);
+  CUDA_TRY(cudaGetLastError());
+  return CRNN_OK;
+}
+int launch_bn_finalize_lines(const double* stats, const int* line_w, const float* gamma, const float* beta, float eps, float* bn, int N,
+                             int C, cudaStream_t st) {
+  bn_finalize_lines_kernel<<<(N * C + 127) / 128, 128, 0, st>>>(stats, line_w, gamma, beta, eps, bn, N, C);
+  CUDA_TRY(cudaGetLastError());
+  return CRNN_OK;
+}
+int launch_bn_apply_relu_lines(const __nv_bfloat16* in, __nv_bfloat16* out, const float* bn, const int* line_w, int N, int H, int Wd,
+                               int C, cudaStream_t st) {
+  const size_t nvec = (size_t)N * H * Wd * C / 8;
+  bn_apply_relu_lines_kernel<<<(unsigned)((nvec + 255) / 256), 256, 0, st>>>(reinterpret_cast<const uint4*>(in), reinterpret_cast<uint4*>(out),
+                                                                             bn, line_w, nvec, H, Wd, C);
+  CUDA_TRY(cudaGetLastError());
+  return CRNN_OK;
+}
+int launch_bn_apply_relu_pool12_lines(const __nv_bfloat16* in, __nv_bfloat16* out, const float* bn, const int* line_w, int N, int H,
+                                      int Wo, int C, cudaStream_t st) {
+  const size_t nvec = (size_t)N * H * Wo * C / 8;
+  bn_apply_relu_pool12_lines_kernel<<<(unsigned)((nvec + 255) / 256), 256, 0, st>>>(
+      reinterpret_cast<const uint4*>(in), reinterpret_cast<uint4*>(out), bn, line_w, nvec, H, Wo, C);
   CUDA_TRY(cudaGetLastError());
   return CRNN_OK;
 }

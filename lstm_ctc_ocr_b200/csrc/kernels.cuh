@@ -16,6 +16,15 @@ int launch_bn_apply_relu(const __nv_bfloat16* in, __nv_bfloat16* out, const floa
                          int C, cudaStream_t st);
 int launch_bn_apply_relu_pool12(const __nv_bfloat16* in, __nv_bfloat16* out, const float* scale, const float* shift,
                                 size_t out_positions, int C, cudaStream_t st);
+// packed evaluation (crnn_forward_lines): line widths clamped once, per-line BatchNorm finalize (bn [N][4][C] from stats [N][2][C])
+// and apply (zero at h >= line_w / 4)
+int launch_clamp_line_width(const int* in, int* out, int N, int W, cudaStream_t st);
+int launch_bn_finalize_lines(const double* stats, const int* line_w, const float* gamma, const float* beta, float eps, float* bn, int N,
+                             int C, cudaStream_t st);
+int launch_bn_apply_relu_lines(const __nv_bfloat16* in, __nv_bfloat16* out, const float* bn, const int* line_w, int N, int H, int Wd,
+                               int C, cudaStream_t st);
+int launch_bn_apply_relu_pool12_lines(const __nv_bfloat16* in, __nv_bfloat16* out, const float* bn, const int* line_w, int N, int H,
+                                      int Wo, int C, cudaStream_t st);
 int launch_transpose_cast(const float* src, int R, int Cc, int ld_src, __nv_bfloat16* dst, int ld_dst, int perm_mode,
                           cudaStream_t st);
 int launch_lstm_bias_prep(const float* b_fw, const float* b_bw, float* xbias, int upc, cudaStream_t st);

@@ -502,9 +502,11 @@ class CopyPool {
 // `pageable_src` != nullptr (crnn_forward_pageable): the batch is in ordinary host memory; every range is first moved into the
 // page-locked `host_data` staging by the copy pool, its DMA is issued, its front end is launched -- and the host moves the next
 // range while the GPU works on this one.
+// `line_width` != nullptr (crnn_forward_lines, device-fed, inference plan): every image is a line evaluated as if alone -- the conv
+// epilogues zero each activation past the line's width and conv4_x use per-line batch statistics.
 static int forward_impl(crnn_model* m, const float* data, const float* host_data, const int* time_step_len, int N, int W,
                         float* logits_out, void* workspace, size_t workspace_bytes, int chunks, cudaStream_t st, cudaStream_t copy_st,
-                        const float* pageable_src = nullptr, int host_threads = 1) {
+                        const float* pageable_src = nullptr, int host_threads = 1, const int* line_width = nullptr) {
   if (!m || !data || !time_step_len || !logits_out || !workspace) return crnn_fail(CRNN_INVALID_VALUE, "forward: null pointer");
   if (!m->params) return crnn_fail(CRNN_NOT_BOUND, "forward: call crnn_model_bind first");
   if (N <= 0 || W < 8 || (W % 4) != 0) return crnn_fail(CRNN_INVALID_VALUE, "forward: need N>0, W>=8, W%%4==0");
@@ -524,6 +526,16 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
   Plan& pl = m->plan;
   CRNN_TRY(ensure_plan(m, N, W, workspace, st));
   const int H1 = pl.H1, H2 = pl.H2, T = pl.T, sms = m->num_sms;
+  const bool lines = line_width != nullptr;
+  pl.line_w = nullptr;
+  if (lines) {
+    Plan tmp;
+    uint8_t* x = reinterpret_cast<uint8_t*>(workspace) + layout_plan(tmp, N, W, nullptr, false);
+    pl.line_w = reinterpret_cast<int*>(x); x += align_up((size_t)N * 4);
+    pl.stats_l = reinterpret_cast<double*>(x); x += align_up((size_t)2 * N * 2 * 512 * 8);
+    pl.bn_l = reinterpret_cast<float*>(x);
+    CRNN_TRY(launch_clamp_line_width(line_width, pl.line_w, N, W, st));
+  }
   cudaEvent_t* ev = nullptr;
   if (m->prof_on && m->prof_used < m->prof_slots) ev = &m->prof_events[(size_t)(m->prof_used++) * (kNumStages + 1)];
   int evi = 0;
@@ -570,7 +582,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
       const size_t o1 = (size_t)n0 * H1 * 16 * 64;
       if (m->conv1_tc)
         CRNN_TRY(launch_conv1_tc(pl.tO_c1, data + (size_t)n0 * W * 32, m->P("conv1/weights"), m->P("conv1/biases"), n0,
-                                 pl.train ? pl.am1 + o1 : nullptr, cn, W, sms, st));
+                                 pl.train ? pl.am1 + o1 : nullptr, cn, W, sms, st, pl.line_w));
       else
         CRNN_TRY(launch_conv1_pool(data + (size_t)n0 * W * 32, m->P("conv1/weights"), m->P("conv1/biases"), pl.a1 + o1,
                                    pl.train ? pl.am1 + o1 : nullptr, cn, W, sms, st));
@@ -581,7 +593,9 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
       convsw::Params p;
       p.Nimg = cn; p.img0 = n0; p.H = H1; p.tiles_per_img = (H1 + 15) / 16; p.bias = m->P("conv2/biases"); p.out = pl.a2;
       p.argmax = pl.train ? pl.am2 : nullptr;
+      p.line_w = pl.line_w;
       if (pl.train) CRNN_TRY(launch_conv2_swap<true>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st));
+      else if (lines) CRNN_TRY((launch_conv2_swap<false, true>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st)));
       else CRNN_TRY(launch_conv2_swap<false>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st));
     } else {
       gemm::Params p = conv_params(N, H1, 16, 64, 128, 128, m->P("conv2/biases"), pl.a2, pl.mg2);
@@ -598,7 +612,9 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     {
       gemm::Params p = conv_params(N, H2, 8, 128, 256, 256, m->P("conv3_1/biases"), pl.a3, pl.mg3);
       if (chunks > 1) { p.m_tile0 = n0 * sb3 / 4; p.num_m_tiles = cn * sb3 / 4; }
-      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4>(pl.tA_c31, m->tB_c31, p, sms, st, &pl.tA_c32)));
+      p.line_w = pl.line_w;
+      if (lines) CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4, 0, true>(pl.tA_c31, m->tB_c31, p, sms, st, &pl.tA_c32)));
+      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4>(pl.tA_c31, m->tB_c31, p, sms, st, &pl.tA_c32)));
     }
     if (mark) STAGE_MARK();
     // conv3_2 + ReLU + height pool
@@ -608,6 +624,9 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
       if (pl.train) {
         p.argmax = pl.am3;
         CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12_T, 4>(pl.tA_c32, m->tB_c32, p, sms, st)));
+      } else if (lines) {
+        p.line_w = pl.line_w;
+        CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12, 4, 0, true>(pl.tA_c32, m->tB_c32, p, sms, st, &pl.tO_c32)));
       } else {
         CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12, 4>(pl.tA_c32, m->tB_c32, p, sms, st, &pl.tO_c32)));
       }
@@ -615,41 +634,62 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     if (mark) STAGE_MARK();
   }
   if (chunks > 1) for (int i = 0; i < 4; ++i) STAGE_MARK();     // keep the event layout (front-end stages read as ~0)
-  CUDA_TRY(cudaMemsetAsync(pl.stats, 0, 2 * 2 * 512 * sizeof(double), st));
-  const double bn_count = (double)N * H2 * 4;
-  // conv4_1 + bias -> batch statistics -> BN + ReLU
-  {
-    gemm::Params p = conv_params(N, H2, 4, 256, 512, 256, m->P("conv4_1/biases"), pl.a4a_pre, pl.mg4);
-    p.stats = pl.stats;
-    CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c41, m->tB_c41, p, sms, st, &pl.tO_c41)));
+  if (lines) {
+    // conv4_x with per-line statistics: each line's own sums, scale and shift; zero at h >= W_i/4
+    CUDA_TRY(cudaMemsetAsync(pl.stats_l, 0, (size_t)2 * N * 2 * 512 * sizeof(double), st));
+    const struct { const char* name; const CUtensorMap* tA; const CUtensorMap* tB; const CUtensorMap* tO; int cin; __nv_bfloat16* pre; } L[2] = {
+        {"conv4_1", &pl.tA_c41, &m->tB_c41, &pl.tO_c41, 256, pl.a4a_pre}, {"conv4_2", &pl.tA_c42, &m->tB_c42, &pl.tO_c42, 512, pl.a4b_pre}};
+    for (int l = 0; l < 2; ++l) {
+      const std::string nm(L[l].name);
+      gemm::Params p = conv_params(N, H2, 4, L[l].cin, 512, 256, m->P(nm + "/biases"), L[l].pre, pl.mg4);
+      p.stats = pl.stats_l + (size_t)l * N * 2 * 512;
+      p.line_w = pl.line_w;
+      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4, 0, true>(*L[l].tA, *L[l].tB, p, sms, st, L[l].tO)));
+      STAGE_MARK();
+      float* bn = pl.bn_l + (size_t)l * N * 4 * 512;
+      CRNN_TRY(launch_bn_finalize_lines(p.stats, pl.line_w, m->P(nm + "/" + nm + "/gamma"), m->P(nm + "/" + nm + "/beta"), m->cfg.bn_eps,
+                                        bn, N, 512, st));
+      if (l == 0) CRNN_TRY(launch_bn_apply_relu_lines(pl.a4a_pre, pl.a4a, bn, pl.line_w, N, H2, 4, 512, st));
+      else CRNN_TRY(launch_bn_apply_relu_pool12_lines(pl.a4b_pre, pl.a4b, bn, pl.line_w, N, H2, 2, 512, st));
+      STAGE_MARK();
+    }
+  } else {
+    CUDA_TRY(cudaMemsetAsync(pl.stats, 0, 2 * 2 * 512 * sizeof(double), st));
+    const double bn_count = (double)N * H2 * 4;
+    // conv4_1 + bias -> batch statistics -> BN + ReLU
+    {
+      gemm::Params p = conv_params(N, H2, 4, 256, 512, 256, m->P("conv4_1/biases"), pl.a4a_pre, pl.mg4);
+      p.stats = pl.stats;
+      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c41, m->tB_c41, p, sms, st, &pl.tO_c41)));
+      STAGE_MARK();
+      float* bn = pl.bn;
+      // batch statistics over the GLOBAL batch when the batch is sharded over ranks: the exchange is fused into the finalize kernel
+      if (m->dp_world > 1)
+        CRNN_TRY(dp_allreduce_bn_finalize(m, pl.stats, bn_count * m->dp_world, m->P("conv4_1/conv4_1/gamma"), m->P("conv4_1/conv4_1/beta"),
+                                          m->cfg.bn_eps, bn, st));
+      else
+      CRNN_TRY(launch_bn_finalize(pl.stats, bn_count, m->P("conv4_1/conv4_1/gamma"), m->P("conv4_1/conv4_1/beta"),
+                                  m->cfg.bn_eps, bn, bn + 512, bn + 1024, bn + 1536, 512, st));
+      CRNN_TRY(launch_bn_apply_relu(pl.a4a_pre, pl.a4a, bn, bn + 512, (size_t)N * H2 * 4, 512, st));
+    }
     STAGE_MARK();
-    float* bn = pl.bn;
-    // batch statistics over the GLOBAL batch when the batch is sharded over ranks: the exchange is fused into the finalize kernel
-    if (m->dp_world > 1)
-      CRNN_TRY(dp_allreduce_bn_finalize(m, pl.stats, bn_count * m->dp_world, m->P("conv4_1/conv4_1/gamma"), m->P("conv4_1/conv4_1/beta"),
-                                        m->cfg.bn_eps, bn, st));
-    else
-    CRNN_TRY(launch_bn_finalize(pl.stats, bn_count, m->P("conv4_1/conv4_1/gamma"), m->P("conv4_1/conv4_1/beta"),
-                                m->cfg.bn_eps, bn, bn + 512, bn + 1024, bn + 1536, 512, st));
-    CRNN_TRY(launch_bn_apply_relu(pl.a4a_pre, pl.a4a, bn, bn + 512, (size_t)N * H2 * 4, 512, st));
-  }
-  STAGE_MARK();
-  // conv4_2 + bias -> batch statistics -> BN + ReLU + height pool (pool3)
-  {
-    gemm::Params p = conv_params(N, H2, 4, 512, 512, 256, m->P("conv4_2/biases"), pl.a4b_pre, pl.mg4);
-    p.stats = pl.stats + 1024;
-    CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c42, m->tB_c42, p, sms, st, &pl.tO_c42)));
+    // conv4_2 + bias -> batch statistics -> BN + ReLU + height pool (pool3)
+    {
+      gemm::Params p = conv_params(N, H2, 4, 512, 512, 256, m->P("conv4_2/biases"), pl.a4b_pre, pl.mg4);
+      p.stats = pl.stats + 1024;
+      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c42, m->tB_c42, p, sms, st, &pl.tO_c42)));
+      STAGE_MARK();
+      float* bn = pl.bn + 2048;
+      if (m->dp_world > 1)
+        CRNN_TRY(dp_allreduce_bn_finalize(m, pl.stats + 1024, bn_count * m->dp_world, m->P("conv4_2/conv4_2/gamma"),
+                                          m->P("conv4_2/conv4_2/beta"), m->cfg.bn_eps, bn, st));
+      else
+      CRNN_TRY(launch_bn_finalize(pl.stats + 1024, bn_count, m->P("conv4_2/conv4_2/gamma"), m->P("conv4_2/conv4_2/beta"),
+                                  m->cfg.bn_eps, bn, bn + 512, bn + 1024, bn + 1536, 512, st));
+      CRNN_TRY(launch_bn_apply_relu_pool12(pl.a4b_pre, pl.a4b, bn, bn + 512, (size_t)N * H2 * 2, 512, st));
+    }
     STAGE_MARK();
-    float* bn = pl.bn + 2048;
-    if (m->dp_world > 1)
-      CRNN_TRY(dp_allreduce_bn_finalize(m, pl.stats + 1024, bn_count * m->dp_world, m->P("conv4_2/conv4_2/gamma"),
-                                        m->P("conv4_2/conv4_2/beta"), m->cfg.bn_eps, bn, st));
-    else
-    CRNN_TRY(launch_bn_finalize(pl.stats + 1024, bn_count, m->P("conv4_2/conv4_2/gamma"), m->P("conv4_2/conv4_2/beta"),
-                                m->cfg.bn_eps, bn, bn + 512, bn + 1024, bn + 1536, 512, st));
-    CRNN_TRY(launch_bn_apply_relu_pool12(pl.a4b_pre, pl.a4b, bn, bn + 512, (size_t)N * H2 * 2, 512, st));
   }
-  STAGE_MARK();
   // conv5 (2x2 VALID, no activation): plain GEMM, K-blocks 0..15 from row m, 16..31 from row m+1
   {
     gemm::Params p;
@@ -778,6 +818,32 @@ extern "C" int crnn_forward_host(crnn_model* m, const float* host_data, float* d
                       reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<cudaStream_t>(copy_stream));
 }
 
+// packed evaluation: the inference plan, then line widths [N] i32, per-line statistics [2][N][2][512] f64, coefficients [2][N][4][512] f32
+extern "C" int crnn_lines_workspace_size(const crnn_model* m, int N, int W, size_t* bytes) {
+  if (!m || !bytes) return crnn_fail(CRNN_INVALID_VALUE, "lines_workspace_size: null");
+  if (N <= 0 || W < 8 || (W % 4) != 0) return crnn_fail(CRNN_INVALID_VALUE, "lines_workspace_size: need N>0, W>=8, W%%4==0");
+  if (m->cfg.compute_dtype >= 2) return crnn_fail(CRNN_UNSUPPORTED, "lines_workspace_size: packed evaluation runs on the bf16 path (compute_dtype 1)");
+  Plan pl;
+  *bytes = layout_plan(pl, N, W, nullptr, false) + align_up((size_t)N * 4) + align_up((size_t)2 * N * 2 * 512 * 8) +
+           align_up((size_t)2 * N * 4 * 512 * 4);
+  return CRNN_OK;
+}
+
+extern "C" int crnn_forward_lines(crnn_model* m, const float* data, const int* line_width, const int* time_step_len, int N, int W,
+                                  float* logits_out, void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
+  if (!m || !data || !line_width || !time_step_len || !logits_out || !workspace) return crnn_fail(CRNN_INVALID_VALUE, "forward_lines: null pointer");
+  if (m->cfg.compute_dtype >= 2) return crnn_fail(CRNN_UNSUPPORTED, "forward_lines: packed evaluation runs on the bf16 path (compute_dtype 1)");
+  if (m->training)
+    return crnn_fail(CRNN_INVALID_VALUE, "forward_lines: evaluation only; the model is in training mode (training uses whole-batch statistics)");
+  size_t need = 0;
+  CRNN_TRY(crnn_lines_workspace_size(m, N, W, &need));
+  if (workspace_bytes < need) return crnn_fail(CRNN_WORKSPACE_TOO_SMALL, "forward_lines: workspace %zu < %zu", workspace_bytes, need);
+  if (!m->conv1_tc || !m->conv2_swap)
+    return crnn_fail(CRNN_UNSUPPORTED, "forward_lines: the line masks live in conv1_tc_kernel and conv2_swap_kernel (unset CRNN_CONV1 / CRNN_CONV2)");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return forward_impl(m, data, nullptr, time_step_len, N, W, logits_out, workspace, workspace_bytes, 1, st, st, nullptr, 1, line_width);
+}
+
 extern "C" int crnn_host_copy(void* dst, const void* src, size_t bytes, int threads) {
   if ((!dst || !src) && bytes) return crnn_fail(CRNN_INVALID_VALUE, "host_copy: null pointer");
   CopyPool::get().copy(dst, src, bytes, threads < 1 ? 1 : threads);
@@ -887,7 +953,9 @@ extern "C" int crnn_debug_tap_raw(crnn_model* m, const char* name, void* dst, si
   size_t bytes = 0;
   bool train_only = false;
   std::string s(name);
-  if (s == "bn") { src = pl.bn; bytes = 2 * 4 * 512 * sizeof(float); }
+  if (s == "bn" && pl.line_w) { src = pl.bn_l; bytes = 2 * n * 4 * 512 * sizeof(float); }
+  else if (s == "stats" && pl.line_w) { src = pl.stats_l; bytes = 2 * n * 2 * 512 * sizeof(double); }
+  else if (s == "bn") { src = pl.bn; bytes = 2 * 4 * 512 * sizeof(float); }
   else if (s == "stats") { src = pl.stats; bytes = 2 * 2 * 512 * sizeof(double); }
   else if (s == "am1") { src = pl.am1; bytes = n * h1 * 16 * 64; train_only = true; }
   else if (s == "am2") { src = pl.am2; bytes = n * h2 * 8 * 128; train_only = true; }

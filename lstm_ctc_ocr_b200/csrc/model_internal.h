@@ -49,6 +49,10 @@ struct Plan {
   float* c_state;
   double* stats;        // [2 layers][2][512]
   float* bn;            // [2 layers][4][512]: scale, shift, mean, invstd
+  // packed evaluation (crnn_forward_lines), past the inference layout; line_w == nullptr after any other forward
+  int* line_w = nullptr;      // [N] clamped line widths
+  double* stats_l;            // [2 layers][N][2][512]
+  float* bn_l;                // [2 layers][N][4][512]
   CUtensorMap tA_c2s;   // conv2 input through 128-position boxes regardless of H (swapped-operand kernel, conv_swap.cuh)
   CUtensorMap tA_c2, tA_c31, tA_c32, tA_c41, tA_c42, tA_c5, tA_x, tA_h[2], tA_l, tA_hall;
   // output maps of the register-side GEMM epilogues (gemm::frag_epi) where no input map above has the producing layer's tile

@@ -60,6 +60,7 @@ class CrnnModel:
         self._bind()
         self._ws = None
         self._ws_key = None
+        self._ws_lines = False
         self.training = False
 
     # ---- training --------------------------------------------------------------------------
@@ -155,14 +156,19 @@ class CrnnModel:
         return OrderedDict((k, self.tensor(k).detach().cpu().numpy().copy()) for k in self.table)
 
     # ---- forward ----------------------------------------------------------------------------
-    def _workspace(self, N, W):
+    def _workspace(self, N, W, lines=False):
+        # a packed-evaluation workspace holds the inference plan too, so it serves both forwards (and the taps after either)
         key = (N, W, self.training)
-        if self._ws_key != key:
+        if self._ws_key != key or (lines and not self._ws_lines):
             nbytes = _lib.c_size_t()
-            check(self.lib.crnn_model_workspace_size(self.handle, N, W, 1 if self.training else 0, nbytes))
+            if lines:
+                check(self.lib.crnn_lines_workspace_size(self.handle, N, W, nbytes))
+            else:
+                check(self.lib.crnn_model_workspace_size(self.handle, N, W, 1 if self.training else 0, nbytes))
             self._ws = None
             self._ws = torch.empty(nbytes.value + 1024, dtype=torch.uint8, device=self.device)
             self._ws_key = key
+            self._ws_lines = lines
         base = self._ws.data_ptr()
         aligned = (base + 1023) // 1024 * 1024
         return aligned, self._ws.numel() - (aligned - base)
@@ -180,6 +186,26 @@ class CrnnModel:
         ws, nbytes = self._workspace(N, W)
         check(self.lib.crnn_forward(self.handle, data.data_ptr(), time_step_len.data_ptr(), N, W, out.data_ptr(), ws,
                                     nbytes, _stream()))
+        return out
+
+    def forward_lines(self, data, line_width, time_step_len, out=None):
+        """Packed evaluation: data [N,W,32] f32 cuda holding line i in columns [0, W_i), line_width [N] i32 cuda (W_i, a multiple
+        of 4 in [8, W]), time_step_len [N] i32 cuda (<= W_i/4 - 1) -> logits [W/4-1,N,64] f32, each line's frames t < W_i/4 - 1
+        as forward() computes them for that line fed alone as [1, W_i, 32] (per-line BatchNorm statistics and width boundaries).
+        Evaluation only: a model in training mode is refused."""
+        assert data.is_cuda and data.dtype == torch.float32 and data.is_contiguous()
+        assert line_width.is_cuda and line_width.dtype == torch.int32 and time_step_len.is_cuda and time_step_len.dtype == torch.int32
+        N, W, Hh = data.shape
+        if Hh != 32:
+            raise CrnnError("data must be [N, W, 32] (cfg.NUM_FEATURES = 32)")
+        if self.training:
+            raise CrnnError("forward_lines is evaluation only: the model is in training mode (training uses whole-batch statistics)")
+        T = W // 4 - 1
+        if out is None:
+            out = torch.empty((T, N, NCLASSES), dtype=torch.float32, device=self.device)
+        ws, nbytes = self._workspace(N, W, lines=True)
+        check(self.lib.crnn_forward_lines(self.handle, data.data_ptr(), line_width.data_ptr(), time_step_len.data_ptr(), N, W,
+                                          out.data_ptr(), ws, nbytes, _stream()))
         return out
 
     def forward_host(self, host_data, time_step_len, chunks=4, out=None, wait_copy=True):
@@ -245,16 +271,19 @@ class CrnnModel:
         check(self.lib.crnn_debug_tap(self.handle, name.encode(), dst.data_ptr(), dst.numel(), ws, _stream()))
         return dst
 
-    def tap_raw(self, name, N, W):
+    def tap_raw(self, name, N, W, lines=False):
         """Non-bf16 workspace buffer of the last forward, byte for byte (tests only): "bn" f32 [2][4][512] (scale, shift,
         mean, invstd per BN layer), "stats" f64 [2][2][512]; bf16 path, training only: "am1" / "am2" / "am3" u8 pool window
         index (dy*2+dx) in the pooled NHWC shape, "csave" f32 [dir * Npad/128 + tile][step][unit / 4][row][unit % 4].
         f32-class paths: "cst" f32 [2][Npad][256] (final cell state) and the stored activations "conv1" .. "conv5",
         "lstm_out": "f32" (split) bf16 [..., 2 (hi, lo), C] per position, conv4_2 [N, H2, 2 (hi, lo), 2 positions, 512]
-        (rows of G = 2 positions); "tf32" f32 in the tap shape."""
+        (rows of G = 2 positions); "tf32" f32 in the tap shape.  lines=True (after forward_lines): per-line "bn" f32 [2][N][4][512]
+        and "stats" f64 [2][N][2][512]."""
         H1, H2 = W // 2, W // 4
         Npad, T = (N + 127) // 128 * 128, H2 - 1
         shapes = {"bn": ((2, 4, 512), torch.float32), "stats": ((2, 2, 512), torch.float64)}
+        if lines:
+            shapes = {"bn": ((2, N, 4, 512), torch.float32), "stats": ((2, N, 2, 512), torch.float64)}
         if self.compute_dtype == 1:
             shapes.update({"am1": ((N, H1, 16, 64), torch.uint8), "am2": ((N, H2, 8, 128), torch.uint8),
                            "am3": ((N, H2, 4, 256), torch.uint8), "csave": ((2 * Npad // 128, T, 64, 128, 4), torch.float32)})

@@ -4,7 +4,12 @@
 Per file (test.py:57-88): read as gray, right-pad the width to a multiple of POOL_SCALE with 0, /255, transpose to
 [1, W, 32], decode, map ids -> chars, exact match against the label encoded in the file name (``<idx>_<chars>.png``).
 Deviation from the reference, per SURVEY §3.4: ``time_step_len`` is fed as W//4 - 1 (the data layer's convention,
-gen.py:54), not the off-by-one W//4 of test.py:74 which exceeds the number of conv frames."""
+gen.py:54), not the off-by-one W//4 of test.py:74 which exceeds the number of conv frames.
+
+Lines are evaluated in packed batches of ``cfg.TEST.BATCH_SIZE`` (``pack_lines`` + the ``line_width`` feed): every line is still
+computed as if it were run alone, as the reference runs it -- its own BatchNorm statistics, zero padding at its own right edge --
+so the decodes are those of one line per run.  Files are grouped by width to cut padding; the report keeps the reference's
+order (sorted names) and charges each file its batch's time divided by the batch's lines."""
 import math
 import os
 
@@ -42,6 +47,29 @@ def prepare_line(img):
     return data, np.array([max(w // cfg.POOL_SCALE + cfg.OFFSET_TIME_STEP, 0)], np.int32)
 
 
+def pack_lines(lines):
+    """[(data [1, W_i, 32] f32, time_step_len [1] i32) as prepare_line returns them] -> (data [N, W, 32] f32 with line i in columns
+    [0, W_i) of slot i and zero beyond, line_width [N] i32 = W_i, time_step_len [N] i32), W = max W_i: the feed of a packed run."""
+    if not lines:
+        raise ValueError("pack_lines: no lines")
+    widths = []
+    for d, t in lines:
+        d, t = np.asarray(d), np.asarray(t)
+        if d.ndim != 3 or d.shape[0] != 1 or d.shape[2] != cfg.NUM_FEATURES:
+            raise ValueError(f"pack_lines: each line must be [1, W_i, {cfg.NUM_FEATURES}], got {d.shape}")
+        w = d.shape[1]
+        if w < 8 or w % cfg.POOL_SCALE:
+            raise ValueError(f"pack_lines: line width {w} must be a multiple of {cfg.POOL_SCALE} and >= 8")
+        if t.shape != (1,) or t[0] < 0 or t[0] > w // cfg.POOL_SCALE - 1:
+            raise ValueError(f"pack_lines: time_step_len {t} must lie in [0, {w // cfg.POOL_SCALE - 1}] for a line {w} wide")
+        widths.append(w)
+    data = np.zeros((len(lines), max(widths), cfg.NUM_FEATURES), np.float32)
+    for i, (d, _) in enumerate(lines):
+        data[i, :widths[i]] = d[0]
+    tsl = np.array([int(np.asarray(t)[0]) for _, t in lines], np.int32)
+    return data, np.array(widths, np.int32), tsl
+
+
 def decodeRes(nums, ignore=0):
     _, decode_maps = get_encode_decode_dict()
     return [decode_maps[int(i)] for i in nums if i != ignore]
@@ -71,23 +99,31 @@ class SolverWrapper(object):
                 print("done")
             except Exception:
                 raise Exception("Check your pretrained {:s}".format(str(path)))
+        files = sorted(os.listdir(testDir))
+        lines = [prepare_line(load_line_image(os.path.join(testDir, f))) for f in files]
+        # batches of lines of similar width (stable sort: ties keep name order), so little of a batch is padding
+        order = sorted(range(len(files)), key=lambda i: lines[i][0].shape[1])
+        bs = max(1, int(cfg.TEST.BATCH_SIZE))
         timer = Timer()
-        total = correct = 0
-        for file in sorted(os.listdir(testDir)):
+        res_of, time_of = {}, {}
+        for b0 in range(0, len(order), bs):
+            idx = order[b0:b0 + bs]
             timer.tic()
+            data, lw, tsl = pack_lines([lines[i] for i in idx])
+            feed_dict = {self.net.data: data, self.net.line_width: lw, self.net.time_step_len: tsl, self.net.keep_prob: 1.0}
+            dense = sess.run(fetches=dense_decoded, feed_dict=feed_dict)
+            dt = timer.toc(average=False) / len(idx)
+            for r, i in enumerate(idx):
+                res_of[i] = "".join(decodeRes(dense[r]))
+                time_of[i] = dt
+        total = correct = 0
+        for i, file in enumerate(files):
             total += 1
-            img = load_line_image(os.path.join(testDir, file))
-            print(file, end=" ")
-            data, tsl = prepare_line(img)
-            feed_dict = {self.net.data: data, self.net.time_step_len: tsl, self.net.keep_prob: 1.0}
-            res = sess.run(fetches=dense_decoded, feed_dict=feed_dict)
-            res = res[0] if len(res) else []
             org = file.split(".")[0].split("_")[1]
-            res = "".join(decodeRes(res))
-            if org == res:
+            if org == res_of[i]:
                 correct += 1
-            _diff_time = timer.toc(average=False)
-            print("cost time: {:.3f},\n    res: {}".format(_diff_time, res))
+            print(file, end=" ")
+            print("cost time: {:.3f},\n    res: {}".format(time_of[i], res_of[i]))
         print("total acc:{}/{}={:.4f}".format(correct, total, correct / max(total, 1)))
         return correct, total
 

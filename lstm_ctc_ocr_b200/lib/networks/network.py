@@ -101,6 +101,16 @@ class Network(object):
             self.inputs.append(layer)
         return self
 
+    @property
+    def line_width(self):
+        """Optional placeholder, not in the reference: each line's padded width W_i when several lines are packed into one batch.
+        Feeding it evaluates every line as if it were run alone (per-line BatchNorm statistics and width boundaries,
+        crnn_forward_lines).  Shared by every network built on this class."""
+        ph = self.__dict__.get("_line_width")
+        if ph is None:
+            ph = self.__dict__["_line_width"] = Placeholder("line_width", "int32", [None])
+        return ph
+
     def get_output(self, layer):
         try:
             return self.layers[layer]

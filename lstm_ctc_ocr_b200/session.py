@@ -254,8 +254,9 @@ class Session(object):
 
     # ---- run ------------------------------------------------------------------------------
     @staticmethod
-    def validate_feed(data, tsl, labels, labels_len):
-        """Host-side checks the C ABI cannot do without a device sync (SURVEY §8(b): invalid lengths)."""
+    def validate_feed(data, tsl, labels, labels_len, line_width=None):
+        """Host-side checks the C ABI cannot do without a device sync (SURVEY §8(b): invalid lengths).  With `line_width` (packed
+        evaluation) every W_i must be a multiple of 4 in [8, W] and time_step_len[i] at most W_i/4 - 1."""
         if data.ndim != 3 or data.shape[2] != 32:
             raise ValueError(f"data must be [N, W, 32], got {data.shape}")
         N, W, _ = data.shape
@@ -273,6 +274,13 @@ class Session(object):
                 raise ValueError("sum(labels_len) != len(labels)")
             if labels.size and (labels.min() < 1 or labels.max() > 62):
                 raise ValueError("label ids must lie in 1..62 (0 is the CTC blank, 63 the decoder blank)")
+        if line_width is not None:
+            if line_width.shape != (N,):
+                raise ValueError("line_width must be [N]")
+            if line_width.min() < 8 or line_width.max() > W or (line_width % 4).any():
+                raise ValueError(f"line_width must hold multiples of 4 in [8, {W}] (each line's padded width)")
+            if (tsl > line_width // 4 - 1).any():
+                raise ValueError("time_step_len[i] must be <= line_width[i]/4 - 1 (frames past a line are not defined)")
 
     def run(self, fetches, feed_dict=None):
         single = not isinstance(fetches, (list, tuple))
@@ -297,6 +305,8 @@ class Session(object):
         llen = np.asarray(feeds["labels_len"], dtype=np.int32) if need_labels else None
         eng = self.engine_for(net)
         dev = self.device
+        if feeds.get("line_width") is not None:
+            return self._run_lines(flist, single, net, eng, data, tsl, labels, llen, np.asarray(feeds["line_width"], dtype=np.int32))
         # training mode is sticky: its forward is a superset (it also saves what the backward needs), and switching back
         # and forth would re-plan the multi-GB workspace
         if any(k == "train_op" for k in kinds) and not eng.training:
@@ -364,15 +374,7 @@ class Session(object):
             elif k == "logits":
                 v = logits.cpu().numpy()
             elif k == "dense_decoded":
-                from .lib.lstm.config import cfg
-                if str(cfg.get("DECODER", "greedy")) == "beam":
-                    # the reference's own decoder (network.py:656): prefix beam search, width 100, blank 63, on the device
-                    o, ol, _ = engine.ctc_beam_search_device(logits, d_tsl, beam_width=int(cfg.get("BEAM_WIDTH", 100)),
-                                                             merge_repeated=True)
-                    v = engine.dense_decoded(o, ol).cpu().numpy()
-                else:
-                    o, ol = engine.ctc_greedy(logits, d_tsl)
-                    v = engine.dense_decoded(o, ol).cpu().numpy()
+                v = self._decode(logits, d_tsl)
             elif k == "train_op":
                 v = f.step_fn(eng, logits, grad, d_data, d_tsl)
                 self._stage_ahead()
@@ -394,3 +396,61 @@ class Session(object):
             ev.record(torch.cuda.current_stream(self.device))
         self._pinned.wait_pending()
         return out[0] if single else out
+
+    def _run_lines(self, flist, single, net, eng, data, tsl, labels, llen, line_width):
+        """Packed evaluation (``line_width`` fed): the batch is staged to the device and every line is evaluated as if it were run
+        alone (engine.CrnnModel.forward_lines).  Evaluation fetches only."""
+        kinds = [f.kind for f in flist]
+        if "train_op" in kinds:
+            raise ValueError("line_width (packed evaluation) cannot be fed with train_op: training uses whole-batch statistics")
+        if eng.training:
+            raise ValueError("line_width (packed evaluation) needs a model that has not been switched to training")
+        data = np.ascontiguousarray(data)
+        self.validate_feed(data, tsl, labels, llen, line_width)
+        ints = {"tsl": tsl, "lw": line_width}
+        if labels is not None:
+            ints["labels"], ints["llen"] = labels, llen
+        d_ints = self._pinned.stage_ints(ints, self.device)
+        d_tsl = d_ints["tsl"]
+        d_data = self._pinned.stage("data", data, self.device)
+        self.h2d_bytes = data.nbytes + tsl.nbytes + line_width.nbytes + (labels.nbytes + llen.nbytes if labels is not None else 0)
+        self.last_feed_path = "staged"
+        logits = eng.forward_lines(d_data, d_ints["lw"], d_tsl)
+        costs = grad = loss = None
+        if labels is not None:
+            costs, grad = engine.ctc_loss(logits, d_ints["labels"], d_ints["llen"], d_tsl, want_grad="ctc_grad" in kinds,
+                                          grad_scale=1.0 / data.shape[0], max_label_len=int(llen.max()) if llen.size else 0)
+            loss = eng.total_loss(costs)
+        out = []
+        for k in kinds:
+            if k == "loss":
+                v = loss.cpu().numpy()[0]
+            elif k == "ctc_costs":
+                v = costs.cpu().numpy()
+            elif k == "ctc_grad":
+                v = grad.cpu().numpy()
+            elif k == "logits":
+                v = logits.cpu().numpy()
+            elif k == "dense_decoded":
+                v = self._decode(logits, d_tsl)
+            elif k.startswith("layer:"):
+                name = k.split(":", 1)[1]
+                tapname = {"pool1": "conv1", "pool2": "conv3_2", "pool3": "conv4_2", "reshaped_layer": "conv5"}.get(name, name)
+                v = eng.tap(tapname, data.shape[0], data.shape[1]).cpu().numpy()
+            else:
+                raise ValueError(f"unknown fetch kind {k!r}")
+            out.append(v)
+        self.d2h_bytes = sum(v.nbytes if isinstance(v, np.ndarray) else 4 for v in out)
+        self._pinned.wait_pending()
+        return out[0] if single else out
+
+    @staticmethod
+    def _decode(logits, d_tsl):
+        """dense_decoded of device logits with cfg.DECODER (greedy, or the reference's beam search on the device)."""
+        from .lib.lstm.config import cfg
+        if str(cfg.get("DECODER", "greedy")) == "beam":
+            # the reference's own decoder (network.py:656): prefix beam search, width 100, blank 63, on the device
+            o, ol, _ = engine.ctc_beam_search_device(logits, d_tsl, beam_width=int(cfg.get("BEAM_WIDTH", 100)), merge_repeated=True)
+        else:
+            o, ol = engine.ctc_greedy(logits, d_tsl)
+        return engine.dense_decoded(o, ol).cpu().numpy()

@@ -52,14 +52,23 @@ const char* crnn_last_error(void);           /* host string, valid until the nex
  * negative or above max_label_len, gets cost NaN and an all-zero gradient -- the kernels never index with such an id.
  * input_len is clamped to [0,T].  flat_labels MUST hold sum(label_len) entries (its length is not passed and cannot be
  * checked on the device; the Python wrappers check it).
- * Frame limits: alpha / beta live in shared memory (at most 200 KB per utterance), so T is bounded per max_label_len.
+ * Frame limits and the workspace.  Without a workspace alpha / beta live in shared memory (at most 200 KB per utterance),
+ * so T is bounded per max_label_len:
  *   max_label_len <= 15: T <= 256 tensor-map kernel (CRNN_CTC_KERNEL=tma), T <= floor(51200 / (70 + 2*AS + ES)) fast
  *                        kernel (AS = (2*max_label_len+1)|1, ES = max_label_len|1: 348 at 15, 550 at 4), beyond that
  *                        the generic kernel to T <= 517; the largest supported T is the larger of 517 and the fast limit
- *   max_label_len 16..31: T <= 259;   32..63: T <= 130;   above 63: CRNN_UNSUPPORTED
+ *   max_label_len 16..31: T <= 259;   32..63: T <= 130
  * Logits or a gradient not 16-byte aligned (4-byte alignment is enough) take the generic kernel (T <= 517 / 259 / 130).
- * A T above the limit returns CRNN_UNSUPPORTED without touching costs or grad; crnn_last_error() names T and the shared
- * memory it needed.
+ * Beyond these limits -- max_label_len up to 639 (S = 2L+1 <= 1279 states) and any T -- the workspace kernel runs, as
+ * warp-ctc's GPU path does: crnn_ctc_workspace_size returns 0 where a shared-memory kernel serves the shape at any
+ * alignment (max_label_len <= 63 and T <= 517 / 259 / 130), else 4 * N * T * (64 + S_pad) + 256 bytes (S_pad = 2L+1
+ * rounded up to a multiple of 4: the log-softmax and alpha tables; any alignment); CRNN_UNSUPPORTED above max_label_len
+ * 639 or when the per-utterance float count overflows an int or the total a size_t.  A call gets the kernel it gets with
+ * no workspace, with the same bits, wherever that succeeds; otherwise the workspace kernel when workspace_bytes is at
+ * least the size.  Its results are the same bits from run to run (no float atomics).  With neither, the call returns
+ * CRNN_UNSUPPORTED without touching costs or grad; crnn_last_error() names T and the shared memory it needed (or
+ * max_label_len above 63) and, when in range, the workspace bytes that would run it.  CRNN_CTC_KERNEL=long runs the
+ * workspace kernel at every shape (the size query then returns its size everywhere).
  * ---------------------------------------------------------------------------------------- */
 int crnn_ctc_workspace_size(int T, int N, int C, int max_label_len, size_t* bytes);
 int crnn_ctc_loss(const float* logits, float* grad, const int* flat_labels, const int* label_len,

@@ -22,9 +22,14 @@
 //            (lane owns KS consecutive states, neighbours via __shfl_up/__shfl_down), all in log2 space
 //   phase 2  both warps, rows interleaved: re-read the logits row (L2 hit), y = softmax, per-class
 //            sum of alpha*beta/y via shared-memory accumulators, write grad row (HBM write, coalesced)
+// ctc_long_kernel (max_label_len <= 639, any T): the caller's workspace holds the log-softmax and alpha tables that do not
+//   fit in shared memory; it runs where the kernels above cannot (see its comment below).
 // No tensor cores: the dynamic program is a scan, not a contraction.
 #include "common.cuh"
 #include <cuda.h>
+#include <limits.h>
+#include <stdint.h>
+#include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -885,15 +890,280 @@ __global__ void __launch_bounds__(128) ctc_greedy_kernel(const float* __restrict
   if (lane == 0) out_len[n] = count;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// ctc_long_kernel: the workspace path, for max_label_len <= 639 (S <= 1279 states) and any T the workspace holds -- the
+// shapes whose alpha / beta tables do not fit in shared memory.  Same semantics and log2-space arithmetic as the kernels
+// above.  One CTA of 320 threads per utterance, 4 consecutive states per thread (S_pad <= 1280).
+//   prologue  warp = frame: log2-softmax of each frame's 64 logits -> workspace row lp[t][64]
+//   alpha     one frame per step: the previous row ping-pongs in shared memory (one barrier per frame); each row is also
+//             stored to the workspace.  The next frames' emissions are loaded two steps ahead, off the dependency chain.
+//   beta      recomputed row by row from T-1 down; at each frame every state's posterior alpha*beta/y/p against the stored
+//             alpha row goes to a shared row, and the frame's gradient row is formed one step later: each class sums its
+//             posteriors over a per-utterance class -> state list (built once, in label order), the blank over its L+1 even
+//             states, a lane-strided sum then a fixed xor tree.  No float atomics: the result is the same bits run to run.
+// Logits and gradient are read and written one float at a time (4-byte alignment is enough).
+// ---------------------------------------------------------------------------------------------------------------------------
+constexpr int LONG_MAX_LABEL = 639;
+constexpr int LONG_MAX_THREADS = 320;
+constexpr int LONG_WS_ALIGN = 256;           // the launch rounds the workspace pointer up to this; the size query includes it
+
+inline int long_stride(int max_label_len) { return (2 * max_label_len + 1 + 3) & ~3; }            // S_pad, a multiple of 4
+inline size_t long_smem_bytes(int max_label_len) {
+  const size_t AS = long_stride(max_label_len);
+  return sizeof(float) * (2 * (AS + 8) + 2 * AS) + sizeof(int) * (AS + (size_t)(max_label_len > 0 ? max_label_len : 1) + 65);
+}
+
+__global__ void __launch_bounds__(LONG_MAX_THREADS)
+ctc_long_kernel(const float* __restrict__ logits, float* __restrict__ grad, const int* __restrict__ flat_labels,
+                const int* __restrict__ label_len, const int* __restrict__ input_len, int T, int N, int blank, int max_label_len,
+                float grad_scale, float* __restrict__ costs, float* __restrict__ ws) {
+  extern __shared__ __align__(16) float lsm[];
+  const int AS = (2 * max_label_len + 1 + 3) & ~3;
+  const int BS = AS + 8;                              // a row: 4 pad, AS states, 4 pad (pads stay -inf)
+  float* s_buf = lsm;                                 // [2][BS] alpha, then beta rows
+  float* s_w = s_buf + 2 * BS;                        // [2][AS] posteriors of one frame
+  int* s_ext = reinterpret_cast<int*>(s_w + 2 * AS);  // [AS] class of each state (blank past S)
+  int* s_list = s_ext + AS;                           // [max_label_len] odd states grouped by class, in label order
+  int* s_cstart = s_list + (max_label_len > 0 ? max_label_len : 1);   // [65] class c's states: s_list[s_cstart[c] .. s_cstart[c+1])
+  __shared__ int s_off, s_repeats, s_bad;
+
+  const int n = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+  const int warp = tid >> 5, lane = tid & 31, nw = nt >> 5;
+  const int L = label_len[n];
+  const int Tn = max(0, min(input_len[n], T));
+  const int S = 2 * L + 1;
+  float* lp = ws + (size_t)n * T * CTC_C;                               // [T][64] log2 y
+  float* al = ws + (size_t)N * T * CTC_C + (size_t)n * T * AS;          // [T][AS] log2 alpha
+
+  if (warp == 0) {
+    int acc = 0;
+    for (int i = lane; i < n; i += 32) acc += __ldg(label_len + i);
+    acc = __reduce_add_sync(0xffffffffu, acc);
+    if (lane == 0) { s_off = acc; s_repeats = 0; s_bad = 0; }
+  }
+  __syncthreads();
+  bool too_long = (L < 0) || (L > max_label_len);
+  if (!too_long) {
+    int rep = 0, bad = 0;
+    for (int s = tid; s < AS; s += nt) {
+      int v = blank;
+      if (s < S && (s & 1)) {
+        v = flat_labels[s_off + (s >> 1)];
+        // ids outside [0,C) or equal to the blank are never used as indices: the sample is rejected (cost NaN, zero gradient)
+        if (v < 0 || v >= CTC_C || v == blank) { bad = 1; v = blank; }
+        if (s >= 3 && v == flat_labels[s_off + (s >> 1) - 1]) rep++;
+      }
+      s_ext[s] = v;
+    }
+    if (rep) atomicAdd(&s_repeats, rep);
+    if (bad) atomicOr(&s_bad, 1);
+  }
+  __syncthreads();
+  too_long = too_long || (s_bad != 0);
+  const bool feasible = !too_long && Tn > 0 && (L + s_repeats <= Tn);
+  if (!feasible) {
+    if (tid == 0) costs[n] = too_long ? __int_as_float(0x7fc00000) : 0.0f;
+    if (grad != nullptr)
+      for (int i = tid; i < T * CTC_C; i += nt) grad[((size_t)(i / CTC_C) * N + n) * CTC_C + (i % CTC_C)] = 0.f;
+    return;
+  }
+
+  if (grad != nullptr) {   // class -> state lists: count, exclusive scan, fill (ballot order = label order)
+    for (int c = warp; c < CTC_C; c += nw) {
+      int cnt = 0;
+      for (int k0 = 0; k0 < L; k0 += 32) cnt += __popc(__ballot_sync(0xffffffffu, k0 + lane < L && s_ext[2 * (k0 + lane) + 1] == c));
+      if (lane == 0) s_cstart[c] = cnt;
+    }
+    __syncthreads();
+    if (tid == 0) {
+      int acc = 0;
+      for (int c = 0; c < CTC_C; ++c) { const int v = s_cstart[c]; s_cstart[c] = acc; acc += v; }
+      s_cstart[CTC_C] = acc;
+    }
+    __syncthreads();
+    for (int c = warp; c < CTC_C; c += nw) {
+      int pos = s_cstart[c];
+      for (int k0 = 0; k0 < L; k0 += 32) {
+        const int k = k0 + lane;
+        const bool hit = k < L && s_ext[2 * k + 1] == c;
+        const unsigned b = __ballot_sync(0xffffffffu, hit);
+        if (hit) s_list[pos + __popc(b & ((1u << lane) - 1))] = 2 * k + 1;
+        pos += __popc(b);
+      }
+    }
+  }
+
+  // ---------------- prologue: warp = frame, log2-softmax rows to the workspace ----------------
+  for (int t0 = warp; t0 < Tn; t0 += 4 * nw) {
+    float x0[4], x1[4], m[4], sum[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int t = min(t0 + u * nw, Tn - 1);
+      const float* x = logits + ((size_t)t * N + n) * CTC_C;
+      x0[u] = __ldg(x + lane) * LOG2E;
+      x1[u] = __ldg(x + lane + 32) * LOG2E;
+      m[u] = fmaxf(x0[u], x1[u]);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+      for (int u = 0; u < 4; ++u) m[u] = fmaxf(m[u], __shfl_xor_sync(0xffffffffu, m[u], o));
+#pragma unroll
+    for (int u = 0; u < 4; ++u) sum[u] = ptx::ex2(x0[u] - m[u]) + ptx::ex2(x1[u] - m[u]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+      for (int u = 0; u < 4; ++u) sum[u] += __shfl_xor_sync(0xffffffffu, sum[u], o);
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int t = t0 + u * nw;
+      const float lse = m[u] + ptx::lg2(sum[u]);
+      if (t < Tn) {
+        lp[(size_t)t * CTC_C + lane] = x0[u] - lse;
+        lp[(size_t)t * CTC_C + lane + 32] = x1[u] - lse;
+      }
+    }
+  }
+  for (int i = tid; i < 2 * BS; i += nt) s_buf[i] = NEG_INF;
+  __syncthreads();
+
+  const int s0 = 4 * tid;                    // this thread's states s0 .. s0+3 (none when s0 >= AS)
+  const bool act = s0 < AS;
+  int cls[4];
+  bool skin[4], skout[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int s = s0 + k;
+    cls[k] = act ? s_ext[s] : blank;
+    skin[k] = act && s >= 2 && s < S && s_ext[s] != blank && s_ext[s] != s_ext[s - 2];
+    skout[k] = act && s + 2 < S && s_ext[s + 2] != blank && s_ext[s + 2] != s_ext[s];
+  }
+  auto emit = [&](int t, float* e) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) e[k] = lp[(size_t)t * CTC_C + cls[k]];
+  };
+
+  // ---------------- alpha ----------------
+  float a[4], e1[4] = {0.f, 0.f, 0.f, 0.f}, e2[4] = {0.f, 0.f, 0.f, 0.f};
+  if (act) {
+    float e0[4];
+    emit(0, e0);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) a[k] = (s0 + k < 2 && s0 + k < S) ? e0[k] : NEG_INF;
+    const float4 v = make_float4(a[0], a[1], a[2], a[3]);
+    *reinterpret_cast<float4*>(s_buf + 4 + s0) = v;
+    *reinterpret_cast<float4*>(al + s0) = v;
+    if (Tn > 1) emit(1, e1);
+    if (Tn > 2) emit(2, e2);
+  }
+  __syncthreads();
+  for (int t = 1; t < Tn; ++t) {
+    if (act) {
+      const float* prev = s_buf + ((t - 1) & 1) * BS;
+      float* cur = s_buf + (t & 1) * BS;
+      float e[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) { e[k] = e1[k]; e1[k] = e2[k]; }
+      if (t + 2 < Tn) emit(t + 2, e2);
+      const float2 lo = *reinterpret_cast<const float2*>(prev + 4 + s0 - 2);     // states s0-2, s0-1
+      const float v[6] = {lo.x, lo.y, a[0], a[1], a[2], a[3]};
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float nv = lse3(v[k + 2], v[k + 1], skin[k] ? v[k] : NEG_INF) + e[k];
+        a[k] = (s0 + k < S) ? nv : NEG_INF;
+      }
+      const float4 o = make_float4(a[0], a[1], a[2], a[3]);
+      *reinterpret_cast<float4*>(cur + 4 + s0) = o;
+      *reinterpret_cast<float4*>(al + (size_t)t * AS + s0) = o;
+    }
+    __syncthreads();
+  }
+
+  const float* last = s_buf + ((Tn - 1) & 1) * BS + 4;
+  const float ll2 = lse3(last[S - 1], (S >= 2) ? last[S - 2] : NEG_INF, NEG_INF);
+  if (tid == 0) costs[n] = -ll2 * LN2;
+  if (grad == nullptr) return;
+  {
+    const int z0 = (ll2 == NEG_INF) ? 0 : Tn;      // frames past the length (all of them when p underflows) get zero
+    for (int i = tid; i < (T - z0) * CTC_C; i += nt) grad[((size_t)(z0 + i / CTC_C) * N + n) * CTC_C + (i % CTC_C)] = 0.f;
+  }
+  if (ll2 == NEG_INF) return;
+  __syncthreads();                                  // every thread has read the last alpha row
+
+  // ---------------- beta, posteriors, gradient rows ----------------
+  // The gradient row of frame t+1 is formed while beta of frame t is computed: lane j of warp w owns class w + nw*j.
+  const int ncls = (CTC_C + nw - 1) / nw;
+  auto ycls = [&](int t) { const int c = warp + nw * lane; return (lane < ncls && c < CTC_C) ? lp[(size_t)t * CTC_C + c] : 0.f; };
+  auto grad_row = [&](int t, const float* sw, float yl) {
+    float* g = grad + ((size_t)t * N + n) * CTC_C;
+    for (int j = 0; j < ncls; ++j) {
+      const int c = warp + nw * j;
+      if (c >= CTC_C) break;
+      float acc = 0.f;
+      if (c == blank) {
+        for (int i = lane; i <= L; i += 32) acc += sw[2 * i];
+      } else {
+        for (int i = s_cstart[c] + lane; i < s_cstart[c + 1]; i += 32) acc += sw[s_list[i]];
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+      if (lane == j) g[c] = grad_scale * (ptx::ex2(yl) - acc);
+    }
+  };
+  float b[4], ec[4], en1[4] = {0.f, 0.f, 0.f, 0.f}, en2[4] = {0.f, 0.f, 0.f, 0.f};
+  float4 ac = make_float4(0.f, 0.f, 0.f, 0.f), an1 = ac, an2 = ac;
+  if (act) {
+    emit(Tn - 1, ec);
+    ac = *reinterpret_cast<const float4*>(al + (size_t)(Tn - 1) * AS + s0);
+    if (Tn > 1) { emit(Tn - 2, en1); an1 = *reinterpret_cast<const float4*>(al + (size_t)(Tn - 2) * AS + s0); }
+    if (Tn > 2) { emit(Tn - 3, en2); an2 = *reinterpret_cast<const float4*>(al + (size_t)(Tn - 3) * AS + s0); }
+  }
+  float ynext = ycls(Tn - 1), ycur = 0.f;
+  for (int t = Tn - 1; t >= 0; --t) {
+    const float yrow = ycur;                        // class values of frame t+1
+    ycur = ynext;
+    if (t > 0) ynext = ycls(t - 1);
+    if (act) {
+      const float* prev = s_buf + ((t + 1) & 1) * BS;
+      float* cur = s_buf + (t & 1) * BS;
+      if (t == Tn - 1) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) b[k] = (s0 + k < S && s0 + k >= S - 2) ? ec[k] : NEG_INF;
+      } else {
+        const float2 hi = *reinterpret_cast<const float2*>(prev + 4 + s0 + 4);   // states s0+4, s0+5
+        const float v[6] = {b[0], b[1], b[2], b[3], hi.x, hi.y};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const float nv = lse3(v[k], v[k + 1], skout[k] ? v[k + 2] : NEG_INF) + ec[k];
+          b[k] = (s0 + k < S) ? nv : NEG_INF;
+        }
+      }
+      *reinterpret_cast<float4*>(cur + 4 + s0) = make_float4(b[0], b[1], b[2], b[3]);
+      const float av[4] = {ac.x, ac.y, ac.z, ac.w};
+      float w[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) w[k] = ptx::ex2(av[k] + b[k] - ec[k] - ll2);   // alpha*beta / y / p(l|x)
+      *reinterpret_cast<float4*>(s_w + (t & 1) * AS + s0) = make_float4(w[0], w[1], w[2], w[3]);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) { ec[k] = en1[k]; en1[k] = en2[k]; }
+      ac = an1; an1 = an2;
+      if (t >= 3) { emit(t - 3, en2); an2 = *reinterpret_cast<const float4*>(al + (size_t)(t - 3) * AS + s0); }
+    }
+    if (t + 1 < Tn) grad_row(t + 1, s_w + ((t + 1) & 1) * AS, yrow);
+    __syncthreads();
+  }
+  grad_row(0, s_w, ycur);
+}
+
 size_t ctc_smem_bytes(int T, int KS) { return sizeof(float) * ((size_t)T + 3 * (size_t)T * 32 * KS + CTC_WARPS * 4 * CTC_C); }
 
 template <int KS>
 int launch_ctc(const float* logits, float* grad, const int* flat_labels, const int* label_len, const int* input_len,
-               int T, int N, int blank, float grad_scale, float* costs, cudaStream_t st) {
+               int T, int N, int blank, float grad_scale, float* costs, cudaStream_t st, const char* more) {
   size_t smem = ctc_smem_bytes(T, KS);
   if (smem > 200 * 1024)
-    return crnn_fail(CRNN_UNSUPPORTED, "ctc_loss: T = %d frames need %zu bytes of shared memory at KS = %d (limit %d)", T, smem, KS,
-                     200 * 1024);
+    return crnn_fail(CRNN_UNSUPPORTED, "ctc_loss: T = %d frames need %zu bytes of shared memory at KS = %d (limit %d)%s", T, smem, KS,
+                     200 * 1024, more);
   CUDA_TRY(cudaFuncSetAttribute(ctc_loss_kernel<KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   ctc_loss_kernel<KS><<<N, CTC_THREADS, smem, st>>>(logits, grad, flat_labels, label_len, input_len, T, N, blank, grad_scale,
                                            costs);
@@ -945,12 +1215,57 @@ int ctc_recur_choice() {
   return (e != nullptr && strcmp(e, "me") == 0) ? 1 : 0;
 }
 
+// CRNN_CTC_KERNEL=long runs ctc_long_kernel at every shape (the size query then returns its bytes everywhere), so that the
+// workspace kernel can be checked at the shapes the shared-memory kernels serve
+bool ctc_force_long() {
+  const char* e = getenv("CRNN_CTC_KERNEL");
+  return e != nullptr && strcmp(e, "long") == 0;
+}
+
+// states-per-lane variant of the generic kernel, and whether its shared memory holds T frames (every alignment)
+int ctc_generic_ks(int max_label_len) {
+  const int S = 2 * max_label_len + 1;
+  return S <= 32 ? 1 : S <= 64 ? 2 : S <= 128 ? 4 : 0;
+}
+bool ctc_generic_fits(int T, int max_label_len) {
+  const int ks = ctc_generic_ks(max_label_len);
+  return ks != 0 && ctc_smem_bytes(T, ks) <= 200 * 1024;
+}
+
+// Workspace of ctc_long_kernel: per utterance T log2-softmax rows (64 floats) and T alpha rows (S_pad floats), plus the
+// alignment slack.  The per-utterance float count must fit an int; the total must fit a size_t.  No crnn_fail here.
+int ctc_long_bytes(int T, int N, int max_label_len, size_t* bytes) {
+  if (max_label_len > LONG_MAX_LABEL) return CRNN_UNSUPPORTED;
+  const size_t per = (size_t)T * (size_t)(CTC_C + long_stride(max_label_len));
+  if (per > (size_t)INT_MAX || per > (SIZE_MAX - LONG_WS_ALIGN) / sizeof(float) / (size_t)N) return CRNN_UNSUPPORTED;
+  *bytes = per * (size_t)N * sizeof(float) + LONG_WS_ALIGN;
+  return CRNN_OK;
+}
+
+int launch_ctc_long(const float* logits, float* grad, const int* flat_labels, const int* label_len, const int* input_len, int T,
+                    int N, int blank, int max_label_len, float grad_scale, float* costs, void* workspace, cudaStream_t st) {
+  float* ws = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(workspace) + LONG_WS_ALIGN - 1) & ~uintptr_t(LONG_WS_ALIGN - 1));
+  // always 320 threads: short labels leave threads idle in the recursions, but the per-frame class sums still get 10 warps
+  ctc_long_kernel<<<N, LONG_MAX_THREADS, long_smem_bytes(max_label_len), st>>>(
+      logits, grad, flat_labels, label_len, input_len, T, N, blank, max_label_len, grad_scale, costs, ws);
+  CUDA_TRY(cudaGetLastError());
+  return CRNN_OK;
+}
+
 }  // namespace
 
 extern "C" int crnn_ctc_workspace_size(int T, int N, int C, int max_label_len, size_t* bytes) {
   if (!bytes || T <= 0 || N <= 0 || max_label_len < 0) return crnn_fail(CRNN_INVALID_VALUE, "ctc_workspace_size: bad args");
   if (C != CTC_C) return crnn_fail(CRNN_UNSUPPORTED, "ctc: C must be 64");
-  *bytes = 0;   // alpha/beta live in shared memory; kept for warp-ctc call-shape compatibility
+  if (ctc_generic_fits(T, max_label_len) && !ctc_force_long()) {
+    *bytes = 0;   // a shared-memory kernel serves the shape at any alignment
+    return CRNN_OK;
+  }
+  size_t need = 0;
+  if (ctc_long_bytes(T, N, max_label_len, &need) != CRNN_OK)
+    return crnn_fail(CRNN_UNSUPPORTED, "ctc_workspace_size: max_label_len = %d, T = %d, N = %d is beyond the workspace kernel "
+                     "(max_label_len <= %d, per-utterance and total sizes within int / size_t)", max_label_len, T, N, LONG_MAX_LABEL);
+  *bytes = need;
   return CRNN_OK;
 }
 
@@ -958,12 +1273,25 @@ extern "C" int crnn_ctc_loss(const float* logits, float* grad, const int* flat_l
                              const int* input_len, int T, int N, int C, int blank, int max_label_len,
                              float grad_scale, float* costs, void* workspace, size_t workspace_bytes,
                              crnn_stream_t stream) {
-  (void)workspace; (void)workspace_bytes;
   if (!logits || !flat_labels || !label_len || !input_len || !costs) return crnn_fail(CRNN_INVALID_VALUE, "ctc_loss: null pointer");
   if (T <= 0 || N <= 0 || blank < 0 || blank >= C || max_label_len < 0) return crnn_fail(CRNN_INVALID_VALUE, "ctc_loss: bad shape");
   if (C != CTC_C) return crnn_fail(CRNN_UNSUPPORTED, "ctc: C must be 64");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   int S = 2 * max_label_len + 1;
+  // The workspace kernel runs only where no shared-memory kernel can (or when forced): every other call takes the kernel
+  // and computes the bits it would without a workspace.
+  size_t need = 0;
+  const bool long_ok = ctc_long_bytes(T, N, max_label_len, &need) == CRNN_OK;
+  const bool force_long = ctc_force_long();
+  if (force_long) {
+    if (long_ok && workspace != nullptr && workspace_bytes >= need)
+      return launch_ctc_long(logits, grad, flat_labels, label_len, input_len, T, N, blank, max_label_len, grad_scale, costs, workspace, st);
+    if (!long_ok)
+      return crnn_fail(CRNN_UNSUPPORTED, "ctc_loss: CRNN_CTC_KERNEL=long: max_label_len = %d, T = %d is beyond the workspace kernel",
+                       max_label_len, T);
+    return crnn_fail(CRNN_UNSUPPORTED, "ctc_loss: CRNN_CTC_KERNEL=long needs a workspace of %zu bytes, got %zu", need,
+                     workspace != nullptr ? workspace_bytes : (size_t)0);
+  }
   const bool aligned = (reinterpret_cast<uintptr_t>(logits) % 16 == 0) && (grad == nullptr || reinterpret_cast<uintptr_t>(grad) % 16 == 0);
   if (S <= 32 && aligned && T <= 256 && ctc_kernel_choice() == 0 && ctc_tma_smem_bytes(T, max_label_len) <= 200 * 1024) {
     CUtensorMap tl, tg;
@@ -988,10 +1316,16 @@ extern "C" int crnn_ctc_loss(const float* logits, float* grad, const int* flat_l
     CUDA_TRY(cudaGetLastError());
     return CRNN_OK;
   }
-  if (S <= 32) return launch_ctc<1>(logits, grad, flat_labels, label_len, input_len, T, N, blank, grad_scale, costs, st);
-  if (S <= 64) return launch_ctc<2>(logits, grad, flat_labels, label_len, input_len, T, N, blank, grad_scale, costs, st);
-  if (S <= 128) return launch_ctc<4>(logits, grad, flat_labels, label_len, input_len, T, N, blank, grad_scale, costs, st);
-  return crnn_fail(CRNN_UNSUPPORTED, "ctc: max_label_len > 63");
+  const bool run_long = !ctc_generic_fits(T, max_label_len) && long_ok && workspace != nullptr && workspace_bytes >= need;
+  if (run_long)
+    return launch_ctc_long(logits, grad, flat_labels, label_len, input_len, T, N, blank, max_label_len, grad_scale, costs, workspace, st);
+  // no kernel runs: the failure names what the shared-memory kernels needed and, in range, the workspace that would run it
+  char more[96] = "";
+  if (long_ok) snprintf(more, sizeof more, "; a workspace of %zu bytes runs it", need);
+  if (S <= 32) return launch_ctc<1>(logits, grad, flat_labels, label_len, input_len, T, N, blank, grad_scale, costs, st, more);
+  if (S <= 64) return launch_ctc<2>(logits, grad, flat_labels, label_len, input_len, T, N, blank, grad_scale, costs, st, more);
+  if (S <= 128) return launch_ctc<4>(logits, grad, flat_labels, label_len, input_len, T, N, blank, grad_scale, costs, st, more);
+  return crnn_fail(CRNN_UNSUPPORTED, "ctc: max_label_len > 63%s", more);
 }
 
 extern "C" int crnn_ctc_greedy(const float* logits, const int* input_len, int T, int N, int C, int tf_blank,

@@ -313,9 +313,36 @@ class CrnnModel:
         return loss
 
 
+CTC_MAX_LABEL_LEN = 639       # the workspace kernel's limit (S = 2L+1 <= 1279 states), warp-ctc's on the GPU
+_ctc_ws = {}                  # device -> workspace tensor of the largest size asked for so far, reused call to call
+
+
+def ctc_workspace_bytes(T, N, C, max_label_len):
+    """Bytes of device workspace crnn_ctc_loss needs for this shape: 0 where a shared-memory kernel serves it at any alignment
+    (max_label_len <= 63 and T within 517 / 259 / 130), else the workspace kernel's size.  CrnnError (CRNN_UNSUPPORTED) above
+    max_label_len 639 or when the size overflows.  No CUDA call."""
+    nbytes = _lib.c_size_t()
+    check(_lib.load().crnn_ctc_workspace_size(int(T), int(N), int(C), int(max_label_len), nbytes))
+    return int(nbytes.value)
+
+
+def _auto_ctc_workspace(T, N, C, max_label_len, device):
+    nbytes = ctc_workspace_bytes(T, N, C, max_label_len)
+    if nbytes == 0:
+        return None
+    ws = _ctc_ws.get(device)
+    if ws is None or ws.numel() < nbytes:
+        _ctc_ws.pop(device, None)
+        ws = _ctc_ws[device] = torch.empty(nbytes, dtype=torch.uint8, device=device)
+    return ws
+
+
 def ctc_loss(logits, flat_labels, label_len, input_len, blank=0, want_grad=False, grad_scale=1.0, max_label_len=None,
-             costs=None, grad=None, validate=False):
-    """logits [T,N,64] f32 cuda; integer tensors i32 cuda.  Returns (costs [N], grad [T,N,64] | None)."""
+             costs=None, grad=None, validate=False, workspace=None):
+    """logits [T,N,64] f32 cuda; integer tensors i32 cuda.  Returns (costs [N], grad [T,N,64] | None).
+    workspace: None passes none (shapes beyond the shared-memory kernels fail with CRNN_UNSUPPORTED); "auto" sizes it with
+    ctc_workspace_bytes and reuses a per-device buffer; a uint8 cuda tensor is passed as given.  Shapes a shared-memory kernel
+    serves give the same bits with or without a workspace."""
     lib = _lib.load()
     assert logits.is_cuda and logits.dtype == torch.float32 and logits.is_contiguous()
     T, N, C = logits.shape
@@ -333,9 +360,18 @@ def ctc_loss(logits, flat_labels, label_len, input_len, blank=0, want_grad=False
         costs = torch.empty(N, dtype=torch.float32, device=logits.device)
     if want_grad and grad is None:
         grad = torch.empty_like(logits)
+    if isinstance(workspace, str):
+        if workspace != "auto":
+            raise CrnnError(f"ctc_loss: workspace must be None, 'auto' or a cuda tensor, got {workspace!r}")
+        workspace = _auto_ctc_workspace(T, N, C, max_label_len, logits.device)
+    ws_ptr, ws_bytes = 0, 0
+    if workspace is not None:
+        if not (torch.is_tensor(workspace) and workspace.is_cuda and workspace.is_contiguous()):
+            raise CrnnError("ctc_loss: workspace must be a contiguous cuda tensor")
+        ws_ptr, ws_bytes = workspace.data_ptr(), workspace.numel() * workspace.element_size()
     check(lib.crnn_ctc_loss(logits.data_ptr(), _ptr(grad) if want_grad else 0, flat_labels.data_ptr(),
                             label_len.data_ptr(), input_len.data_ptr(), T, N, C, blank, int(max_label_len),
-                            float(grad_scale), costs.data_ptr(), 0, 0, _stream()))
+                            float(grad_scale), costs.data_ptr(), ws_ptr, ws_bytes, _stream()))
     return costs, (grad if want_grad else None)
 
 

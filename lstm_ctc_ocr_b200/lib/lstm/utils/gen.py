@@ -147,6 +147,23 @@ def render_line(chars, height=60, width=None, rng=random):
     return np.asarray(img, dtype=np.uint8)
 
 
+def line_width_bound(max_len=None):
+    """Padded width of the widest batch render_line + groupBatch can make from lines of at most ``max_len`` characters
+    (cfg.MAX_LEN by default): the widest glyph advance of cfg.CHARSET (cached like render_line's), MAX_LEN of them plus the
+    28 px margin at height 60, resized to height 32, rounded up to a multiple of POOL_SCALE."""
+    n = cfg.MAX_LEN if max_len is None else int(max_len)
+    font = _font(42)
+    advc = _glyphs(font)["adv"]
+    widest = 0
+    for c in cfg.CHARSET:
+        a = advc.get(c)
+        if a is None:
+            a = advc[c] = int(font.getlength(c))
+        widest = max(widest, a)
+    nw = int(cfg.IMG_HEIGHT / 60 * (n * widest + 28))
+    return int(math.ceil(nw / cfg.POOL_SCALE) * cfg.POOL_SCALE)
+
+
 def generateImg(rng=random):
     """(gray uint8 image, its characters): the reference's per-sample entry (gen.py:29-35; it returns the captcha's RGB array and
     converts to gray in the generator, gen.py:79 -- here the line is rendered gray directly)."""
@@ -187,9 +204,11 @@ def batch_seed(k, seed=None, rank=0, world=1):
     return int(cfg.RNG_SEED if seed is None else seed) + k * int(world) + int(rank)
 
 
-def make_batch(k, batch_size=32, render=True, seed=None, rank=0, world=1, bucket=None, width=None):
+def make_batch(k, batch_size=32, render=True, seed=None, rank=0, world=1, bucket=None, width=None, lens=None):
     """Batch k of a deterministic stream (picklable entry point of the feeder's worker processes).
-    ``bucket`` = None: the reference's 4-6 character lines padded to the batch max width; else one of BUCKETS."""
+    ``bucket`` = None: the reference's 4-6 character lines padded to the batch max width; else one of BUCKETS.
+    ``lens`` = (min, max) characters per line of the bucket-less stream, cfg.MIN_LEN / cfg.MAX_LEN when None (worker
+    processes start from the default configuration, so the feeder passes the parent's values)."""
     s = batch_seed(k, seed, rank, world)
     if not render:
         if width is not None:                  # full-width synthetic lines (the throughput workloads)
@@ -202,7 +221,7 @@ def make_batch(k, batch_size=32, render=True, seed=None, rank=0, world=1, bucket
         return list(data), lab.tolist(), ll.tolist(), tsl.tolist()
     rng = random.Random(s)
     if bucket is None:
-        labels = [gen_rand(rng) for _ in range(batch_size)]
+        labels = [gen_rand(rng, *(lens or (None, None))) for _ in range(batch_size)]
         return groupBatch([render_line(l, rng=rng) for l in labels], labels)
     lo = max([b for b in BUCKETS if b < bucket] or [0])
     cmin, cmax = BUCKET_CHARS[bucket]
@@ -450,11 +469,18 @@ def get_batch(num_workers, **kwargs):
         rank, world = _dist_rank_world()
     bucket = kwargs.pop("bucket", None)
 
+    lens = (cfg.MIN_LEN, cfg.MAX_LEN)          # this process's configuration (e.g. --set MIN_LEN 30 MAX_LEN 70), for the workers
+
     def arg_fn(k):
-        return dict(k=k, batch_size=batch_size, render=render, seed=seed, rank=rank, world=world, bucket=bucket)
+        return dict(k=k, batch_size=batch_size, render=render, seed=seed, rank=rank, world=world, bucket=bucket, lens=lens)
     if num_workers is None or num_workers <= 1 or not render:
         return (make_batch(**arg_fn(k)) for k in _count())
-    return PrefetchFeeder(arg_fn, num_workers=num_workers, depth=3, max_width=kwargs.pop("max_width", 256), batch_size=batch_size)
+    # ring slots hold the widest batch the configured line lengths can render (cfg.MAX_LEN 70 lines are about 1 000 px wide);
+    # never less than the widest bucket, 256
+    max_width = kwargs.pop("max_width", None)
+    if max_width is None:
+        max_width = max(256, line_width_bound())
+    return PrefetchFeeder(arg_fn, num_workers=num_workers, depth=3, max_width=max_width, batch_size=batch_size)
 
 
 def _count():

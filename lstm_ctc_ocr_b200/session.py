@@ -274,6 +274,9 @@ class Session(object):
                 raise ValueError("sum(labels_len) != len(labels)")
             if labels.size and (labels.min() < 1 or labels.max() > 62):
                 raise ValueError("label ids must lie in 1..62 (0 is the CTC blank, 63 the decoder blank)")
+            if labels_len.size and int(labels_len.max()) > engine.CTC_MAX_LABEL_LEN:
+                raise ValueError(f"a label of {int(labels_len.max())} ids is longer than the {engine.CTC_MAX_LABEL_LEN} the CTC kernels "
+                                 "support")
         if line_width is not None:
             if line_width.shape != (N,):
                 raise ValueError("line_width must be [N]")
@@ -356,7 +359,7 @@ class Session(object):
             N = data.shape[0]
             # warp-ctc computes the gradient inside its forward op; so does this kernel (one launch)
             costs, grad = engine.ctc_loss(logits, d_lab, d_ll, d_tsl, want_grad=True, grad_scale=1.0 / N,
-                                          max_label_len=int(llen.max()) if llen.size else 0)
+                                          max_label_len=int(llen.max()) if llen.size else 0, workspace="auto")
             loss = eng.total_loss(costs)
         has_train = any(k == "train_op" for k in kinds)
         if not has_train:
@@ -419,7 +422,8 @@ class Session(object):
         costs = grad = loss = None
         if labels is not None:
             costs, grad = engine.ctc_loss(logits, d_ints["labels"], d_ints["llen"], d_tsl, want_grad="ctc_grad" in kinds,
-                                          grad_scale=1.0 / data.shape[0], max_label_len=int(llen.max()) if llen.size else 0)
+                                          grad_scale=1.0 / data.shape[0], max_label_len=int(llen.max()) if llen.size else 0,
+                                          workspace="auto")
             loss = eng.total_loss(costs)
         out = []
         for k in kinds:

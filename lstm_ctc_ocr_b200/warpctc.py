@@ -5,7 +5,8 @@
 activations: [T, N, 64] f32 *unnormalised* logits (torch CUDA tensor, or numpy -> staged to the GPU);
 returns costs [N] in the same container type.  With a torch tensor that requires grad the result is
 differentiable: the kernel produces d cost/d logits in the same launch (as warp-ctc's op does) and the
-backward is ``grad * dloss[None, :, None]`` -- the gradient the TF binding registers."""
+backward is ``grad * dloss[None, :, None]`` -- the gradient the TF binding registers.  Like the TF binding, every call
+sizes and passes a device workspace, so labels up to 639 ids and any number of frames run."""
 import numpy as np
 import torch
 
@@ -16,7 +17,7 @@ class _CTC(torch.autograd.Function):
     @staticmethod
     def forward(ctx, activations, flat_labels, label_lengths, input_lengths, blank, max_label_len):
         costs, grad = engine.ctc_loss(activations.contiguous(), flat_labels, label_lengths, input_lengths, blank=blank,
-                                      want_grad=True, max_label_len=max_label_len)
+                                      want_grad=True, max_label_len=max_label_len, workspace="auto")
         ctx.save_for_backward(grad)
         return costs
 
@@ -48,6 +49,8 @@ def ctc(activations, flat_labels, label_lengths, input_lengths, blank_label=0):
     n_lab = int(flat_labels.numel()) if torch.is_tensor(flat_labels) else int(np.asarray(flat_labels).size)
     if ll_host.shape != (N,) or (ll_host.size and int(ll_host.min()) < 0):
         raise ValueError("ctc: label_lengths must be [N], non-negative")
+    if mll > engine.CTC_MAX_LABEL_LEN:
+        raise ValueError(f"ctc: a label of {mll} ids is longer than the {engine.CTC_MAX_LABEL_LEN} the CTC kernels support")
     if int(ll_host.sum()) != n_lab:
         raise ValueError(f"ctc: sum(label_lengths) = {int(ll_host.sum())} but flat_labels holds {n_lab} ids")
     if not torch.is_tensor(flat_labels) and n_lab:
@@ -58,5 +61,5 @@ def ctc(activations, flat_labels, label_lengths, input_lengths, blank_label=0):
     if activations.requires_grad:
         costs = _CTC.apply(activations, fl, ll, il, int(blank_label), mll)
     else:
-        costs, _ = engine.ctc_loss(activations.contiguous(), fl, ll, il, blank=int(blank_label), max_label_len=mll)
+        costs, _ = engine.ctc_loss(activations.contiguous(), fl, ll, il, blank=int(blank_label), max_label_len=mll, workspace="auto")
     return costs.cpu().numpy() if as_numpy else costs

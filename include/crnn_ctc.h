@@ -127,7 +127,11 @@ typedef struct crnn_config {
                          *     accumulate and f32 elementwise math (the reference computes in fp32, LSTM_train.py:10);
                          *     forward + CTC only (BASELINE configs[1])
                          * 3 = tf32: the same forward-only orchestration on tf32 wgmma operands (f32 tensors, rounded to
-                         *     nearest tf32 where produced; 10-bit mantissa, one pass over K at half the bf16 rate) */
+                         *     nearest tf32 where produced; 10-bit mantissa, one pass over K at half the bf16 rate)
+                         * 4 = fp8, inference only: conv3_1, conv3_2, conv4_1, conv4_2 and conv5 run on e4m3 wgmma operands
+                         *     (twice the bf16 tensor rate); everything else is the bf16 path.  Weights get one scale per
+                         *     output channel (amax / 448); each of the five activation operands one power-of-two scale that
+                         *     crnn_model_calibrate_fp8 or crnn_model_set_fp8_scales provides (see below) */
 } crnn_config;
 
 int     crnn_model_create(const crnn_config* cfg, crnn_model** out);
@@ -186,6 +190,24 @@ int     crnn_forward_pageable(crnn_model* m, const float* pageable_data, float* 
 int     crnn_lines_workspace_size(const crnn_model* m, int N, int W, size_t* bytes);
 int     crnn_forward_lines(crnn_model* m, const float* data, const int* line_width, const int* time_step_len, int N, int W,
                            float* logits_out, void* workspace, size_t workspace_bytes, crnn_stream_t stream);
+
+/* fp8 models (compute_dtype 4).  The scales of the five e4m3 activation operands -- conv2's pooled output a2, conv3_1's a3,
+ * conv3_2's pooled a3p and the BatchNorm + ReLU outputs a4a (conv4_1) and a4b (conv4_2, pooled) -- are
+ *   s = 2^max(-126, ceil(log2(amax / 448)))   (the f32 quotient; 1 when amax is 0 or not finite)
+ * so that dividing by them is exact; values above the calibrated range saturate to +-448.
+ * crnn_model_calibrate_fp8 runs the bf16 forward's front end (conv1 .. conv4_2's BatchNorm) on a caller-supplied batch (the
+ * layouts of crnn_forward; the workspace of crnn_model_workspace_size(train = 0)) and reduces the five amaxes on the device:
+ * asynchronous, no host sync, no allocation (an fp8 model allocates its e4m3 weights and scales in crnn_model_create),
+ * deterministic.  Any parameter change (crnn_model_bind, crnn_model_params_changed)
+ * invalidates the scales; an fp8 forward without valid scales returns CRNN_INVALID_VALUE ("calibration is missing") and leaves
+ * its outputs untouched.  get (syncs the device) and set (host arrays of 5 floats; set refuses anything but powers of two in
+ * [2^-126, 2^127] with CRNN_INVALID_VALUE) restate them.  On a model of another compute_dtype all three return CRNN_UNSUPPORTED.
+ * crnn_forward, _host and _pageable (copy, then compute) and crnn_forward_lines run the fp8 path on an fp8 model;
+ * crnn_model_set_training(m, 1) and a training workspace return CRNN_UNSUPPORTED. */
+int     crnn_model_calibrate_fp8(crnn_model* m, const float* data, const int* time_step_len, int N, int W, void* workspace,
+                                 size_t workspace_bytes, crnn_stream_t stream);
+int     crnn_model_get_fp8_scales(crnn_model* m, float* scales_host);
+int     crnn_model_set_fp8_scales(crnn_model* m, const float* scales_host);
 
 /* The host-side copy crnn_forward_pageable uses, on its own: `bytes` from `src` to `dst` (plain host pointers, non-overlapping) split
  * over `threads` threads of the library's persistent pool (the caller's thread included).  No CUDA call is made. */
@@ -280,7 +302,12 @@ int     crnn_debug_tap(crnn_model* m, const char* name, float* dst, size_t dst_e
  * f32-class models: "bn" and "stats" (same layouts), "cst" (f32 final cell state [2 dirs][Npad][256]) and the
  * activation buffers as stored under their tap names "conv1" .. "conv5", "lstm_out": split mode (2) bf16 rows
  * [hi(G*C) | lo(G*C)] of G consecutive positions (G = 2 for "conv4_2", else 1), tf32 mode (3) f32 [positions][C]
- * rounded to tf32.  Other names (am1..3, csave, the backward buffers) fail with CRNN_INVALID_VALUE. */
+ * rounded to tf32.  Other names (am1..3, csave, the backward buffers) fail with CRNN_INVALID_VALUE.
+ * fp8 models (compute_dtype 4): crnn_debug_tap returns "conv2" "conv3_1" "conv3_2" "conv4_1" "conv4_2" dequantised (e4m3 value
+ * x its scale), the other names as on the bf16 path; crnn_debug_tap_raw returns those five as the raw e4m3 bytes (same NHWC
+ * shapes), "fp8_scales" (f32 [5]: a2, a3, a3p, a4a, a4b), "fp8_wscale" and "fp8_colscale" (f32 [5 layers][512]: per output
+ * channel weight scale and activation x weight scale of conv3_1, conv3_2, conv4_1, conv4_2, conv5; conv3_x fill 256 columns),
+ * "fp8_w_conv3_1" .. "fp8_w_conv5" (u8 e4m3 weights [Cout][K], K in (kh, kw, ci) order), and "bn" / "stats" as above. */
 int     crnn_debug_tap_raw(crnn_model* m, const char* name, void* dst, size_t dst_bytes,
                            void* workspace, crnn_stream_t stream);
 

@@ -45,6 +45,9 @@ SIGNATURES = {
                                       c_int, c_void_p, c_void_p]),
     "crnn_lines_workspace_size": (c_int, [c_void_p, c_int, c_int, ctypes.POINTER(c_size_t)]),
     "crnn_forward_lines": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "crnn_model_calibrate_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "crnn_model_get_fp8_scales": (c_int, [c_void_p, c_void_p]),
+    "crnn_model_set_fp8_scales": (c_int, [c_void_p, c_void_p]),
     "crnn_host_copy": (c_int, [c_void_p, c_void_p, c_size_t, c_int]),
     "crnn_total_loss": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "crnn_debug_tap": (c_int, [c_void_p, c_char_p, c_void_p, c_size_t, c_void_p, c_void_p]),

@@ -17,7 +17,7 @@
 
 extern "C" int crnn_model_set_training(crnn_model* m, int flag) {
   if (!m) return crnn_fail(CRNN_INVALID_VALUE, "set_training: null model");
-  if (flag && m->cfg.compute_dtype >= 2) return crnn_fail(CRNN_UNSUPPORTED, "set_training: the f32-class paths (compute_dtype 2, 3) are forward + CTC only");
+  if (flag && m->cfg.compute_dtype >= 2) return crnn_fail(CRNN_UNSUPPORTED, "set_training: the f32-class and fp8 paths (compute_dtype 2, 3, 4) are forward only");
   if (flag && !m->wblock_bwd) {
     const size_t nB[9] = {512 * 4608, 256 * 4608, 256 * 2304, 128 * 2304, 64 * 1152, 1024 * 1024, 512 * 64, 512 * 2048, 512 * 1024};
     size_t tot = 1024;

@@ -45,9 +45,10 @@ struct Params {
   __nv_bfloat16* out;
   uint8_t* argmax;        // TRAIN: window index (dy*2+dx) of the max, same shape as out
   const int* line_w;      // LINES: [images] clamped line widths (input columns); pooled rows >= line_w / 4 are stored as zero
+  const float* oscale;    // FP8: out is e4m3 [*, H/2, 8, 128] = e4m3(pooled value / *oscale) (a power of two)
 };
 
-template <bool TRAIN, bool LINES = false>
+template <bool TRAIN, bool LINES = false, bool FP8 = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmO,
                   const Params p) {
@@ -138,6 +139,33 @@ conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
         if (issuer) ptx::bulk_wait_read_all();       // the previous tile's stores have read the buffer
         ptx::bar_sync(1, 256);
         const int ph_end = LINES ? (__ldg(p.line_w + n) >> 2) - (h0 >> 1) : 8;   // pooled rows of this tile inside the line
+        if constexpr (FP8) {
+          // e4m3 output: the pooled tile is one [64 positions][128 channels] box of bytes; each lane writes its two channels' bytes
+          // (lanes l, l ^ 4, l ^ 8, .. hold neighbouring channels of one position: the bytes of a 4-byte word, no bank conflict)
+          const float inv_os = 1.f / __ldg(p.oscale);
+#pragma unroll
+          for (int ph = 0; ph < 8; ++ph) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int j = 4 * ph + e;
+              const float m0 = fmaxf(fmaxf(d[4 * j], d[4 * j + 1]), fmaxf(d[4 * j + 8], d[4 * j + 9]));
+              const float m8 = fmaxf(fmaxf(d[4 * j + 2], d[4 * j + 3]), fmaxf(d[4 * j + 10], d[4 * j + 11]));
+              uint32_t q = ptx::pack_e4m3x2(fmaxf(m0 + bias0, 0.f) * inv_os, fmaxf(m8 + bias8, 0.f) * inv_os);
+              if (LINES && ph >= ph_end) q = 0u;
+              const int row = ph * 8 + 4 * e + (l & 3);
+              uint8_t* rb = stg + row * 128;
+              rb[(((f0 >> 4) ^ (row & 7)) << 4) + (f0 & 15)] = (uint8_t)(q & 0xFFu);
+              rb[((((f0 + 8) >> 4) ^ (row & 7)) << 4) + ((f0 + 8) & 15)] = (uint8_t)(q >> 8);
+            }
+          }
+          ptx::fence_proxy_async_smem();
+          ptx::bar_sync(1, 256);
+          if (issuer) {
+            ptx::tma_store_4d(&tmO, stg, 0, 0, h0 >> 1, n);
+            ptx::bulk_commit();
+          }
+          continue;
+        }
 #pragma unroll
         for (int ph = 0; ph < 8; ++ph) {
 #pragma unroll
@@ -316,12 +344,13 @@ conv_dgrad_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
 
 }  // namespace convsw
 
-template <bool TRAIN, bool LINES = false>
-// `out`: NHWC map of the pooled output [N, H/2, 8, 128], box [64, 8, 8, 1] (one tile = 8 pooled rows); only <false> stores through it
+template <bool TRAIN, bool LINES = false, bool FP8 = false>
+// `out`: NHWC map of the pooled output [N, H/2, 8, 128], box [64, 8, 8, 1] (one tile = 8 pooled rows); only <false> stores through it.
+// FP8: a UINT8 map of the e4m3 output, box [128, 8, 8, 1]
 static int launch_conv2_swap(const CUtensorMap& x, const CUtensorMap& w, const CUtensorMap& out, const convsw::Params& p, int num_sms,
                              cudaStream_t st) {
-  static_assert(!(TRAIN && LINES), "line masks exist in the inference epilogue only");
-  auto kern = convsw::conv2_swap_kernel<TRAIN, LINES>;
+  static_assert(!(TRAIN && (LINES || FP8)), "line masks and e4m3 output exist in the inference epilogue only");
+  auto kern = convsw::conv2_swap_kernel<TRAIN, LINES, FP8>;
   static bool attr = false;
   if (!attr) {
     CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, convsw::SMEM_BYTES));

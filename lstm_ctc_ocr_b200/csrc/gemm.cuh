@@ -96,6 +96,10 @@ struct Params {
   // LINES instantiations (packed evaluation, crnn_forward_lines): [Nimg] clamped line widths in input columns; conv rows at
   // h >= line_w[n] / 4 (every LINES layer runs at H = W/4) are stored as zero, and EPI_STATS sums go to slot n of `stats` [Nimg][2][Nc]
   const int* line_w;
+  // KIND 2 (e4m3 operands, forward_fp8.cu): y = acc * colscale[col] + bias[col] (colscale = activation scale x weight scale);
+  // EPI_RELU / EPI_RELU_POOL12 store e4m3(y / *oscale), the next GEMM's operand scale (a power of two)
+  const float* colscale;
+  const float* oscale;
 };
 
 __device__ __forceinline__ float warp_colsum32(const float (&v)[32], int lane) {
@@ -167,6 +171,10 @@ constexpr bool frag_epi(int block_n, int epi) {
 __device__ __forceinline__ uint32_t* stg_word(uint8_t* buf, int box_bytes, int row, int c) {
   return reinterpret_cast<uint32_t*>(buf + (c >> 6) * box_bytes + row * 128 + ((((c >> 3) & 7) ^ (row & 7)) << 4) + ((c & 7) << 1));
 }
+// e4m3 word (4 columns, c % 4 == 0) of staged row `row`, tile-half column c 0..127: one [row][128 B] box per half, same swizzle
+__device__ __forceinline__ uint32_t* stg_word8(uint8_t* buf, int row, int c) {
+  return reinterpret_cast<uint32_t*>(buf + row * 128 + ((((c >> 4) & 7) ^ (row & 7)) << 4) + (c & 15));
+}
 
 // EPI_STATS column sums of 32 staged rows rg*32 .. rg*32+31 at 32-bit word cw (two bf16 channels) of a 128-B box row:
 // {sum lo, sum hi, sum lo^2, sum hi^2}.  The rows are added in the order of warp_colsum32 over 32 lanes (rows 16 apart first,
@@ -209,13 +217,18 @@ __device__ __forceinline__ bool conv_row_valid(const Params& p, int m_blk, int r
 //   reversal is a permutation of staging rows; otherwise the thread stores its words to the reversed rows directly.
 //   LINES (conv epilogues): rows past their line are staged as zero like invalid rows, and a 32-row statistics group -- one
 //   sub-box, which never spans two images -- adds into its own image's sums.
-template <int EPI, bool LINES = false>
+//   KIND 2 (e4m3 operands): every value is acc * colscale + bias first; EPI_RELU / EPI_RELU_POOL12 (Q8) then store e4m3 of
+//   y / oscale: the pool max is taken in f32 (rounding is monotonic), lane l ^ 1 holds the neighbouring column pair, so one
+//   shuffle turns two 2-byte pairs into one 4-column word, and a half tile is one [rows][128 B] box.
+template <int EPI, bool LINES = false, int KIND = 0>
 __device__ __forceinline__ void frag_epilogue(const Params& p, const float (&d)[128], uint8_t* stg, const CUtensorMap* tmO,
                                               const int m_blk, const int n_blk, const int wgi, const bool issuer) {
   constexpr bool POOL = (EPI == EPI_RELU_POOL12);
   constexpr bool CONV = (EPI == EPI_RELU || POOL || EPI == EPI_STATS || EPI == EPI_CONV_STORE);
   constexpr bool RELU = (EPI == EPI_RELU || POOL);
-  constexpr int BOX_BYTES = (POOL ? 64 : 128) * 128;     // one [rows][64 columns] bf16 box
+  constexpr bool Q8 = (KIND == 2) && RELU;              // e4m3 output
+  constexpr int BOX_BYTES = (POOL ? 64 : 128) * 128;     // one [rows][64 columns] bf16 box = one [rows][128 columns] e4m3 box
+  constexpr int NBX = Q8 ? 1 : 2;                        // boxes per 128-column half
   const int t = threadIdx.x & 127, l = t & 31;
   const int r0 = wgi * 64 + 16 * (t >> 5) + (l >> 2);   // fragment rows r0 and r0 + 8
   const int col0 = n_blk * 256;
@@ -237,9 +250,11 @@ __device__ __forceinline__ void frag_epilogue(const Params& p, const float (&d)[
     s0 = dr[0]; s1 = dr[1];
     direct = (128 % p.H) != 0;
   }
+  float inv_os = 1.f;
+  if constexpr (Q8) inv_os = 1.f / __ldg(p.oscale);     // a power of two: multiplying by it is the exact division
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
-    uint8_t* buf = stg + hf * 2 * BOX_BYTES;
+    uint8_t* buf = stg + hf * NBX * BOX_BYTES;
     if (hf == 0) {
       if (issuer) ptx::bulk_wait_read_all();            // the previous stores have read the buffer
       ptx::bar_sync(1, 256);
@@ -251,6 +266,37 @@ __device__ __forceinline__ void frag_epilogue(const Params& p, const float (&d)[
       float2 b = make_float2(0.f, 0.f);
       if (EPI != EPI_CONV_STORE && p.bias) b = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + hf * 128 + c));
       uint32_t v0, v1;
+      if constexpr (KIND == 2) {
+        const float2 cs = __ldg(reinterpret_cast<const float2*>(p.colscale + col0 + hf * 128 + c));
+        float y0 = __fmaf_rn(d[4 * j], cs.x, b.x), y1 = __fmaf_rn(d[4 * j + 1], cs.y, b.y);
+        float y2 = __fmaf_rn(d[4 * j + 2], cs.x, b.x), y3 = __fmaf_rn(d[4 * j + 3], cs.y, b.y);
+        if constexpr (Q8) {
+          y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); y2 = fmaxf(y2, 0.f); y3 = fmaxf(y3, 0.f);
+          if (POOL) {                                    // rows r and r ^ 1 (w pair) sit in lanes l and l ^ 4
+            y0 = fmaxf(y0, __shfl_xor_sync(0xffffffffu, y0, 4));
+            y1 = fmaxf(y1, __shfl_xor_sync(0xffffffffu, y1, 4));
+            y2 = fmaxf(y2, __shfl_xor_sync(0xffffffffu, y2, 4));
+            y3 = fmaxf(y3, __shfl_xor_sync(0xffffffffu, y3, 4));
+          }
+          const uint32_t q0 = ptx::pack_e4m3x2(y0 * inv_os, y1 * inv_os), q8 = ptx::pack_e4m3x2(y2 * inv_os, y3 * inv_os);
+          // even lanes keep row r0 (columns c .. c+3), odd lanes row r0 + 8 (columns c-2 .. c+1)
+          const bool even = (l & 1) == 0;
+          const uint32_t r = __shfl_xor_sync(0xffffffffu, even ? q8 : q0, 1);
+          const uint32_t word = even ? (q0 | (r << 16)) : (r | (q8 << 16));
+          const int row = even ? r0 : r0 + 8;
+          const bool ok = even ? ok0 : ok1;
+          // pooled: lanes l and l ^ 4 hold the same pooled rows; the lanes with (l & 4) == 0 store them
+          if (!POOL || (l & 4) == 0) *stg_word8(buf, POOL ? row >> 1 : row, even ? c : c - 2) = ok ? word : 0u;
+          continue;
+        }
+        v0 = ptx::pack_bf16x2(y0, y1);
+        v1 = ptx::pack_bf16x2(y2, y3);
+        if (EPI == EPI_BIAS_BF16 || EPI == EPI_STATS) {
+          *stg_word(buf, BOX_BYTES, s0, c) = ok0 ? v0 : 0u;
+          *stg_word(buf, BOX_BYTES, s1, c) = ok1 ? v1 : 0u;
+          continue;
+        }
+      }
       if (EPI == EPI_CONV_STORE) {
         v0 = ptx::pack_bf16x2(d[4 * j], d[4 * j + 1]);
         v1 = ptx::pack_bf16x2(d[4 * j + 2], d[4 * j + 3]);
@@ -283,7 +329,7 @@ __device__ __forceinline__ void frag_epilogue(const Params& p, const float (&d)[
     ptx::bar_sync(1, 256);
     if (issuer) {
 #pragma unroll
-      for (int bx = 0; bx < 2; ++bx) {
+      for (int bx = 0; bx < NBX; ++bx) {
         const int c = col0 + hf * 128 + bx * 64;
         uint8_t* src = buf + bx * BOX_BYTES;
         if (CONV) {
@@ -723,6 +769,8 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
 
 // KIND 0: bf16 operands, 64 elements per 128 B K-block.  KIND 1: f32 words read as tf32, 32 elements per K-block
 // (forward_x3.cu, compute_dtype 3); tensor maps are FLOAT32 with 32-element boxes, everything else is shared.
+// KIND 2: e4m3 operands, 128 elements per K-block (forward_fp8.cu, compute_dtype 4); UINT8 tensor maps with 128-element
+// boxes, four k32 MMAs per K-block, register-side epilogues only (see frag_epilogue).
 // LINES: packed evaluation lines (Params::line_w), frag_epi conv epilogues only
 template <int BLOCK_N, int AMODE, int EPI, int STAGES, int KIND = 0, bool LINES = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
@@ -730,12 +778,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             const Params p) {
   static_assert(BLOCK_N == 64 || BLOCK_N == 128 || BLOCK_N == 256, "BLOCK_N");
   constexpr bool FRAG = frag_epi(BLOCK_N, EPI);          // tmO (output map) is read only by these
-  static_assert(!LINES || (FRAG && AMODE == A_CONV3 && KIND == 0), "line masks exist in the register-side conv epilogues only");
+  static_assert(!LINES || (FRAG && AMODE == A_CONV3 && (KIND == 0 || KIND == 2)), "line masks exist in the register-side conv epilogues only");
+  static_assert(KIND != 2 || (BLOCK_N == 256 && (EPI == EPI_RELU || EPI == EPI_RELU_POOL12 || EPI == EPI_STATS || EPI == EPI_BIAS_BF16)),
+                "e4m3 GEMMs: conv3_1, conv3_2, conv4_x and conv5");
   constexpr int SLICE_N = slice_cols(BLOCK_N, EPI);
   using SM = Smem<BLOCK_N, STAGES, SLICE_N>;
   constexpr int S = SM::S;
   constexpr int B_STAGE_BYTES = BLOCK_N * 128;
-  constexpr int KELEMS = KIND ? 32 : BLOCK_K;        // operand elements per 128 B K-block
+  constexpr int KELEMS = KIND == 2 ? 128 : KIND ? 32 : BLOCK_K;        // operand elements per 128 B K-block
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -831,8 +881,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         wg::fence();
 #pragma unroll
         for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-          // advance 16 bf16 (8 tf32) = 32 B along K inside the 128 B swizzle row: +2 in the (addr >> 4) field
-          if (KIND) wg::mma_tf32<BLOCK_N>(d, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
+          // advance 16 bf16 (8 tf32, 32 e4m3) = 32 B along K inside the 128 B swizzle row: +2 in the (addr >> 4) field
+          if constexpr (KIND == 2) wg::mma_e4m3<BLOCK_N>(d, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
+          else if (KIND) wg::mma_tf32<BLOCK_N>(d, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
           else wg::mma_bf16<BLOCK_N>(d, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
         }
         wg::commit();
@@ -846,7 +897,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
       if (p.debug_skip_epilogue) continue;
       if constexpr (FRAG) {
-        frag_epilogue<EPI, LINES>(p, d, reinterpret_cast<uint8_t*>(acc_tile), &tmO, m_blk, n_blk, wgi, issuer);
+        frag_epilogue<EPI, LINES, KIND>(p, d, reinterpret_cast<uint8_t*>(acc_tile), &tmO, m_blk, n_blk, wgi, issuer);
       } else {
 #pragma unroll
         for (int s = 0; s < BLOCK_N / SLICE_N; ++s) {

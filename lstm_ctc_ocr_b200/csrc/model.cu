@@ -27,7 +27,7 @@ int crnn_fail(int status, const char* fmt, ...) {
   return status;
 }
 extern "C" const char* crnn_last_error(void) { return g_err; }
-extern "C" int crnn_version(void) { return 102; }
+extern "C" int crnn_version(void) { return 103; }
 extern "C" const char* crnn_status_string(int s) {
   switch (s) {
     case CRNN_OK: return "CRNN_OK";
@@ -132,6 +132,32 @@ int make_tmap_nhwc_f32(CUtensorMap* m, const void* base, int N, int H, int Wd, i
   if (r != CUDA_SUCCESS) return crnn_fail(CRNN_CUDA_ERROR, "cuTensorMapEncodeTiled(4d f32) failed: %d", (int)r);
   return CRNN_OK;
 }
+int make_tmap_2d_u8(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t row_stride, uint32_t box_rows) {
+  PFN_encodeTiled enc = get_encode();
+  if (!enc) return crnn_fail(CRNN_CUDA_ERROR, "cuTensorMapEncodeTiled unavailable");
+  cuuint64_t dims[2] = {cols, rows};
+  cuuint64_t strides[1] = {row_stride};
+  cuuint32_t box[2] = {128, box_rows};
+  cuuint32_t es[2] = {1, 1};
+  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), dims, strides, box, es,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return crnn_fail(CRNN_CUDA_ERROR, "cuTensorMapEncodeTiled(2d u8) failed: %d", (int)r);
+  return CRNN_OK;
+}
+int make_tmap_nhwc_u8(CUtensorMap* m, const void* base, int N, int H, int Wd, int C, int bh) {
+  PFN_encodeTiled enc = get_encode();
+  if (!enc) return crnn_fail(CRNN_CUDA_ERROR, "cuTensorMapEncodeTiled unavailable");
+  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)Wd, (cuuint64_t)H, (cuuint64_t)N};
+  cuuint64_t strides[3] = {(cuuint64_t)C, (cuuint64_t)Wd * C, (cuuint64_t)H * Wd * C};
+  cuuint32_t box[4] = {128, (cuuint32_t)Wd, (cuuint32_t)bh, 1};
+  cuuint32_t es[4] = {1, 1, 1, 1};
+  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, const_cast<void*>(base), dims, strides, box, es,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return crnn_fail(CRNN_CUDA_ERROR, "cuTensorMapEncodeTiled(4d u8) failed: %d", (int)r);
+  return CRNN_OK;
+}
 
 static void add_tensor(crnn_model* m, const std::string& name, std::initializer_list<int64_t> shp) {
   TensorInfo t;
@@ -150,8 +176,9 @@ extern "C" int crnn_model_create(const crnn_config* cfg, crnn_model** out) {
   if (!cfg || !out) return crnn_fail(CRNN_INVALID_VALUE, "model_create: null");
   if (cfg->img_height != 32 || cfg->nclasses != 64 || cfg->num_hid != 512)
     return crnn_fail(CRNN_UNSUPPORTED, "model_create: only IMG_HEIGHT=32, NCLASSES=64, NUM_HID=512 (the reference's net)");
-  if (cfg->compute_dtype < 1 || cfg->compute_dtype > 3)
-    return crnn_fail(CRNN_UNSUPPORTED, "model_create: compute_dtype must be 1 (bf16 operands), 2 (f32-class split-bf16 operands) or 3 (tf32 operands)");
+  if (cfg->compute_dtype < 1 || cfg->compute_dtype > 4)
+    return crnn_fail(CRNN_UNSUPPORTED, "model_create: compute_dtype must be 1 (bf16 operands), 2 (f32-class split-bf16 operands), 3 (tf32 "
+                                       "operands) or 4 (e4m3 operands in conv3_1 .. conv5, inference only)");
   crnn_model* m = new crnn_model();
   m->cfg = *cfg;
   for (auto& c : kConvs) {
@@ -216,6 +243,7 @@ extern "C" int crnn_model_create(const crnn_config* cfg, crnn_model** out) {
   if (st == CRNN_OK) st = make_tmap_2d(&m->tB_h, m->Bh, 2048, 256, 256, 256);
   if (st == CRNN_OK) st = make_tmap_2d(&m->tB_h128, m->Bh, 2048, 256, 256, 128);
   if (st == CRNN_OK) st = make_tmap_2d(&m->tB_l, m->Bl, 64, 512, 512, 64);
+  if (st == CRNN_OK && cfg->compute_dtype == 4) st = fp8_create(m);
   if (st != CRNN_OK) { cudaFree(m->wblock); delete m; return st; }
   *out = m;
   return CRNN_OK;
@@ -224,6 +252,7 @@ extern "C" int crnn_model_create(const crnn_config* cfg, crnn_model** out) {
 extern "C" int crnn_model_destroy(crnn_model* m) {
   if (!m) return CRNN_OK;
   x3_destroy(m);
+  fp8_destroy(m);
   if (m->wblock) cudaFree(m->wblock);
   if (m->wblock_bwd) cudaFree(m->wblock_bwd);
   if (m->d_peers) cudaFree(m->d_peers);
@@ -251,6 +280,7 @@ extern "C" int crnn_model_bind(crnn_model* m, float* params, float* grads, float
   m->dirty = true;
   m->dirty_bwd = true;
   x3_params_changed(m);
+  fp8_params_changed(m);
   return CRNN_OK;
 }
 extern "C" int crnn_model_params_changed(crnn_model* m) {
@@ -258,6 +288,7 @@ extern "C" int crnn_model_params_changed(crnn_model* m) {
   m->dirty = true;
   m->dirty_bwd = true;
   x3_params_changed(m);
+  fp8_params_changed(m);
   return CRNN_OK;
 }
 
@@ -345,7 +376,8 @@ size_t layout_plan(Plan& pl, int N, int W, uint8_t* base, bool train) {
 extern "C" int crnn_model_workspace_size(const crnn_model* m, int N, int W, int train, size_t* bytes) {
   if (!m || !bytes) return crnn_fail(CRNN_INVALID_VALUE, "workspace_size: null");
   if (N <= 0 || W < 8 || (W % 4) != 0) return crnn_fail(CRNN_INVALID_VALUE, "workspace_size: need N>0, W>=8, W%%4==0 (gen.py:58)");
-  if (m->cfg.compute_dtype >= 2) {
+  if (m->cfg.compute_dtype == 4 && train) return crnn_fail(CRNN_UNSUPPORTED, "workspace_size: the fp8 path (compute_dtype 4) is inference only");
+  if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3) {
     if (train) return crnn_fail(CRNN_UNSUPPORTED, "workspace_size: the f32-class paths (compute_dtype 2, 3) are forward + CTC only");
     *bytes = x3_workspace_size(N, W);
     return CRNN_OK;
@@ -380,6 +412,7 @@ static int build_plan(crnn_model* m, int N, int W, void* ws, cudaStream_t st) {
   CRNN_TRY(make_tmap_nhwc(&pl.tO_c41, pl.a4a_pre, N, pl.H2, 4, 512, pl.mg4 ? 32 : 8));
   CRNN_TRY(make_tmap_nhwc(&pl.tO_c42, pl.a4b_pre, N, pl.H2, 4, 512, pl.mg4 ? 32 : 8));
   CRNN_TRY(make_tmap_2d(&pl.tO_x, pl.xproj, (uint64_t)N * pl.H2, 2048, 2048, 128));
+  if (m->cfg.compute_dtype == 4) CRNN_TRY(fp8_plan_maps(pl));
   // rows t = T (= H2-1) of lstm_out are never produced by a time step: keep them defined (zero)
   CUDA_TRY(cudaMemsetAsync(pl.lstm_out, 0, (size_t)N * pl.H2 * 512 * 2, st));
   if (pl.train) {
@@ -504,17 +537,36 @@ class CopyPool {
 // range while the GPU works on this one.
 // `line_width` != nullptr (crnn_forward_lines, device-fed, inference plan): every image is a line evaluated as if alone -- the conv
 // epilogues zero each activation past the line's width and conv4_x use per-line batch statistics.
+// compute_dtype 4: FWD_FP8 runs conv3_1 .. conv5 on e4m3 operands (forward_fp8.cu); from host memory it copies, then computes.
+// FWD_CALIB (crnn_model_calibrate_fp8) runs the bf16 front end up to conv4_2's BatchNorm (a4b), then reduces the fp8 scales.
+enum FwdPrec { FWD_BF16 = 0, FWD_FP8 = 1, FWD_CALIB = 2 };
 static int forward_impl(crnn_model* m, const float* data, const float* host_data, const int* time_step_len, int N, int W,
                         float* logits_out, void* workspace, size_t workspace_bytes, int chunks, cudaStream_t st, cudaStream_t copy_st,
-                        const float* pageable_src = nullptr, int host_threads = 1, const int* line_width = nullptr) {
-  if (!m || !data || !time_step_len || !logits_out || !workspace) return crnn_fail(CRNN_INVALID_VALUE, "forward: null pointer");
+                        const float* pageable_src = nullptr, int host_threads = 1, const int* line_width = nullptr, int prec = FWD_BF16) {
+  const bool fp8 = prec == FWD_FP8, calib = prec == FWD_CALIB;
+  if (!m || !data || !time_step_len || (!logits_out && !calib) || !workspace) return crnn_fail(CRNN_INVALID_VALUE, "forward: null pointer");
   if (!m->params) return crnn_fail(CRNN_NOT_BOUND, "forward: call crnn_model_bind first");
   if (N <= 0 || W < 8 || (W % 4) != 0) return crnn_fail(CRNN_INVALID_VALUE, "forward: need N>0, W>=8, W%%4==0");
   size_t need = 0;
   CRNN_TRY(crnn_model_workspace_size(m, N, W, m->training ? 1 : 0, &need));
   if (workspace_bytes < need) return crnn_fail(CRNN_WORKSPACE_TOO_SMALL, "forward: workspace %zu < %zu", workspace_bytes, need);
   if ((reinterpret_cast<uintptr_t>(workspace) & 1023) != 0) return crnn_fail(CRNN_INVALID_VALUE, "forward: workspace must be 1024-byte aligned");
-  if (m->cfg.compute_dtype >= 2) {
+  if (fp8 || calib) {
+    if (fp8 && !fp8_calibrated(m))
+      return crnn_fail(CRNN_INVALID_VALUE, "forward: the fp8 model (compute_dtype 4) has no activation scales: calibration is missing "
+                                           "(crnn_model_calibrate_fp8 or crnn_model_set_fp8_scales after the last parameter change)");
+    if (!m->conv2_swap) return crnn_fail(CRNN_UNSUPPORTED, "forward: the fp8 path writes a2 from conv2_swap_kernel (unset CRNN_CONV2)");
+    if (m->dp_world > 1) return crnn_fail(CRNN_UNSUPPORTED, "forward: the fp8 path runs on one device (no data parallelism)");
+    if (host_data != nullptr) {
+      // copy-then-compute, as the f32-class paths do
+      if (pageable_src != nullptr) CopyPool::get().copy(const_cast<float*>(host_data), pageable_src, (size_t)N * W * 32 * sizeof(float), host_threads);
+      CUDA_TRY(cudaMemcpyAsync(const_cast<float*>(data), host_data, (size_t)N * W * 32 * sizeof(float), cudaMemcpyHostToDevice, st));
+      host_data = nullptr;
+      pageable_src = nullptr;
+    }
+    chunks = 1;
+  }
+  if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3) {
     // f32-class paths (forward_x3.cu): copy-then-compute when fed from host memory
     if (host_data != nullptr) {
       if (pageable_src != nullptr) CopyPool::get().copy(const_cast<float*>(host_data), pageable_src, (size_t)N * W * 32 * sizeof(float), host_threads);
@@ -523,6 +575,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     return x3_forward(m, data, time_step_len, N, W, logits_out, workspace, workspace_bytes, st);
   }
   if (m->dirty) CRNN_TRY(prepare_weights(m, st));
+  if (fp8) CRNN_TRY(fp8_prepare(m, st));
   Plan& pl = m->plan;
   CRNN_TRY(ensure_plan(m, N, W, workspace, st));
   const int H1 = pl.H1, H2 = pl.H2, T = pl.T, sms = m->num_sms;
@@ -537,7 +590,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     CRNN_TRY(launch_clamp_line_width(line_width, pl.line_w, N, W, st));
   }
   cudaEvent_t* ev = nullptr;
-  if (m->prof_on && m->prof_used < m->prof_slots) ev = &m->prof_events[(size_t)(m->prof_used++) * (kNumStages + 1)];
+  if (!calib && m->prof_on && m->prof_used < m->prof_slots) ev = &m->prof_events[(size_t)(m->prof_used++) * (kNumStages + 1)];
   int evi = 0;
 #define STAGE_MARK() do { if (ev) CUDA_TRY(cudaEventRecord(ev[evi++], st)); } while (0)
   STAGE_MARK();
@@ -594,7 +647,8 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
       p.Nimg = cn; p.img0 = n0; p.H = H1; p.tiles_per_img = (H1 + 15) / 16; p.bias = m->P("conv2/biases"); p.out = pl.a2;
       p.argmax = pl.train ? pl.am2 : nullptr;
       p.line_w = pl.line_w;
-      if (pl.train) CRNN_TRY(launch_conv2_swap<true>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st));
+      if (fp8) CRNN_TRY(fp8_conv2(m, p, lines, sms, st));
+      else if (pl.train) CRNN_TRY(launch_conv2_swap<true>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st));
       else if (lines) CRNN_TRY((launch_conv2_swap<false, true>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st)));
       else CRNN_TRY(launch_conv2_swap<false>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st));
     } else {
@@ -613,7 +667,8 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
       gemm::Params p = conv_params(N, H2, 8, 128, 256, 256, m->P("conv3_1/biases"), pl.a3, pl.mg3);
       if (chunks > 1) { p.m_tile0 = n0 * sb3 / 4; p.num_m_tiles = cn * sb3 / 4; }
       p.line_w = pl.line_w;
-      if (lines) CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4, 0, true>(pl.tA_c31, m->tB_c31, p, sms, st, &pl.tA_c32)));
+      if (fp8) CRNN_TRY(fp8_conv_gemm(m, 0, p, lines, sms, st));
+      else if (lines) CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4, 0, true>(pl.tA_c31, m->tB_c31, p, sms, st, &pl.tA_c32)));
       else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4>(pl.tA_c31, m->tB_c31, p, sms, st, &pl.tA_c32)));
     }
     if (mark) STAGE_MARK();
@@ -621,7 +676,10 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     {
       gemm::Params p = conv_params(N, H2, 8, 256, 256, 256, m->P("conv3_2/biases"), pl.a3p, pl.mg3);
       if (chunks > 1) { p.m_tile0 = n0 * sb3 / 4; p.num_m_tiles = cn * sb3 / 4; }
-      if (pl.train) {
+      if (fp8) {
+        p.line_w = pl.line_w;
+        CRNN_TRY(fp8_conv_gemm(m, 1, p, lines, sms, st));
+      } else if (pl.train) {
         p.argmax = pl.am3;
         CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12_T, 4>(pl.tA_c32, m->tB_c32, p, sms, st)));
       } else if (lines) {
@@ -644,12 +702,14 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
       gemm::Params p = conv_params(N, H2, 4, L[l].cin, 512, 256, m->P(nm + "/biases"), L[l].pre, pl.mg4);
       p.stats = pl.stats_l + (size_t)l * N * 2 * 512;
       p.line_w = pl.line_w;
-      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4, 0, true>(*L[l].tA, *L[l].tB, p, sms, st, L[l].tO)));
+      if (fp8) CRNN_TRY(fp8_conv_gemm(m, 2 + l, p, true, sms, st));
+      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4, 0, true>(*L[l].tA, *L[l].tB, p, sms, st, L[l].tO)));
       STAGE_MARK();
       float* bn = pl.bn_l + (size_t)l * N * 4 * 512;
       CRNN_TRY(launch_bn_finalize_lines(p.stats, pl.line_w, m->P(nm + "/" + nm + "/gamma"), m->P(nm + "/" + nm + "/beta"), m->cfg.bn_eps,
                                         bn, N, 512, st));
-      if (l == 0) CRNN_TRY(launch_bn_apply_relu_lines(pl.a4a_pre, pl.a4a, bn, pl.line_w, N, H2, 4, 512, st));
+      if (fp8) CRNN_TRY(fp8_bn_apply(m, l, bn, true, st));
+      else if (l == 0) CRNN_TRY(launch_bn_apply_relu_lines(pl.a4a_pre, pl.a4a, bn, pl.line_w, N, H2, 4, 512, st));
       else CRNN_TRY(launch_bn_apply_relu_pool12_lines(pl.a4b_pre, pl.a4b, bn, pl.line_w, N, H2, 2, 512, st));
       STAGE_MARK();
     }
@@ -660,7 +720,8 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     {
       gemm::Params p = conv_params(N, H2, 4, 256, 512, 256, m->P("conv4_1/biases"), pl.a4a_pre, pl.mg4);
       p.stats = pl.stats;
-      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c41, m->tB_c41, p, sms, st, &pl.tO_c41)));
+      if (fp8) CRNN_TRY(fp8_conv_gemm(m, 2, p, false, sms, st));
+      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c41, m->tB_c41, p, sms, st, &pl.tO_c41)));
       STAGE_MARK();
       float* bn = pl.bn;
       // batch statistics over the GLOBAL batch when the batch is sharded over ranks: the exchange is fused into the finalize kernel
@@ -670,14 +731,16 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
       else
       CRNN_TRY(launch_bn_finalize(pl.stats, bn_count, m->P("conv4_1/conv4_1/gamma"), m->P("conv4_1/conv4_1/beta"),
                                   m->cfg.bn_eps, bn, bn + 512, bn + 1024, bn + 1536, 512, st));
-      CRNN_TRY(launch_bn_apply_relu(pl.a4a_pre, pl.a4a, bn, bn + 512, (size_t)N * H2 * 4, 512, st));
+      if (fp8) CRNN_TRY(fp8_bn_apply(m, 0, bn, false, st));
+      else CRNN_TRY(launch_bn_apply_relu(pl.a4a_pre, pl.a4a, bn, bn + 512, (size_t)N * H2 * 4, 512, st));
     }
     STAGE_MARK();
     // conv4_2 + bias -> batch statistics -> BN + ReLU + height pool (pool3)
     {
       gemm::Params p = conv_params(N, H2, 4, 512, 512, 256, m->P("conv4_2/biases"), pl.a4b_pre, pl.mg4);
       p.stats = pl.stats + 1024;
-      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c42, m->tB_c42, p, sms, st, &pl.tO_c42)));
+      if (fp8) CRNN_TRY(fp8_conv_gemm(m, 3, p, false, sms, st));
+      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c42, m->tB_c42, p, sms, st, &pl.tO_c42)));
       STAGE_MARK();
       float* bn = pl.bn + 2048;
       if (m->dp_world > 1)
@@ -686,10 +749,12 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
       else
       CRNN_TRY(launch_bn_finalize(pl.stats + 1024, bn_count, m->P("conv4_2/conv4_2/gamma"), m->P("conv4_2/conv4_2/beta"),
                                   m->cfg.bn_eps, bn, bn + 512, bn + 1024, bn + 1536, 512, st));
-      CRNN_TRY(launch_bn_apply_relu_pool12(pl.a4b_pre, pl.a4b, bn, bn + 512, (size_t)N * H2 * 2, 512, st));
+      if (fp8) CRNN_TRY(fp8_bn_apply(m, 1, bn, false, st));
+      else CRNN_TRY(launch_bn_apply_relu_pool12(pl.a4b_pre, pl.a4b, bn, bn + 512, (size_t)N * H2 * 2, 512, st));
     }
     STAGE_MARK();
   }
+  if (calib) return fp8_finish_calibration(m, st);
   // conv5 (2x2 VALID, no activation): plain GEMM, K-blocks 0..15 from row m, 16..31 from row m+1
   {
     gemm::Params p;
@@ -697,7 +762,8 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     p.M = N * H2;
     p.num_m_tiles = (p.M + 127) / 128; p.num_n_tiles = 2; p.num_k_blocks = 32; p.kb_per_shift = 16; p.row_shift_mul = 1;
     p.Nc = 512; p.bias = m->P("conv5/biases"); p.out = pl.a5; p.ldo = 512;
-    CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tA_c5, m->tB_c5, p, sms, st, &pl.tA_x)));
+    if (fp8) CRNN_TRY(fp8_conv5(m, p, sms, st));
+    else CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tA_c5, m->tB_c5, p, sms, st, &pl.tA_x)));
   }
   STAGE_MARK();
   // LSTM input projection for all frames and both directions: [N*H2, 512] x [512, 2048]
@@ -804,10 +870,13 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
   return CRNN_OK;
 }
 
+static int fwd_prec(const crnn_model* m) { return (m && m->cfg.compute_dtype == 4) ? FWD_FP8 : FWD_BF16; }
+
 extern "C" int crnn_forward(crnn_model* m, const float* data, const int* time_step_len, int N, int W, float* logits_out,
                             void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return forward_impl(m, data, nullptr, time_step_len, N, W, logits_out, workspace, workspace_bytes, 1, st, st);
+  return forward_impl(m, data, nullptr, time_step_len, N, W, logits_out, workspace, workspace_bytes, 1, st, st, nullptr, 1, nullptr,
+                      fwd_prec(m));
 }
 
 extern "C" int crnn_forward_host(crnn_model* m, const float* host_data, float* data_staging, const int* time_step_len, int N, int W,
@@ -815,14 +884,34 @@ extern "C" int crnn_forward_host(crnn_model* m, const float* host_data, float* d
                                  crnn_stream_t copy_stream) {
   if (!host_data || !data_staging) return crnn_fail(CRNN_INVALID_VALUE, "forward_host: null pointer");
   return forward_impl(m, data_staging, host_data, time_step_len, N, W, logits_out, workspace, workspace_bytes, chunks,
-                      reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<cudaStream_t>(copy_stream));
+                      reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<cudaStream_t>(copy_stream), nullptr, 1, nullptr, fwd_prec(m));
+}
+
+// ---- fp8 (compute_dtype 4) scales
+extern "C" int crnn_model_calibrate_fp8(crnn_model* m, const float* data, const int* time_step_len, int N, int W, void* workspace,
+                                        size_t workspace_bytes, crnn_stream_t stream) {
+  if (!m) return crnn_fail(CRNN_INVALID_VALUE, "calibrate_fp8: null model");
+  if (m->cfg.compute_dtype != 4) return crnn_fail(CRNN_UNSUPPORTED, "calibrate_fp8: the model is not an fp8 model (compute_dtype 4)");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return forward_impl(m, data, nullptr, time_step_len, N, W, nullptr, workspace, workspace_bytes, 1, st, st, nullptr, 1, nullptr, FWD_CALIB);
+}
+extern "C" int crnn_model_get_fp8_scales(crnn_model* m, float* scales_host) {
+  if (!m || !scales_host) return crnn_fail(CRNN_INVALID_VALUE, "get_fp8_scales: null");
+  if (m->cfg.compute_dtype != 4) return crnn_fail(CRNN_UNSUPPORTED, "get_fp8_scales: the model is not an fp8 model (compute_dtype 4)");
+  return fp8_get_scales(m, scales_host);
+}
+extern "C" int crnn_model_set_fp8_scales(crnn_model* m, const float* scales_host) {
+  if (!m || !scales_host) return crnn_fail(CRNN_INVALID_VALUE, "set_fp8_scales: null");
+  if (m->cfg.compute_dtype != 4) return crnn_fail(CRNN_UNSUPPORTED, "set_fp8_scales: the model is not an fp8 model (compute_dtype 4)");
+  return fp8_set_scales(m, scales_host);
 }
 
 // packed evaluation: the inference plan, then line widths [N] i32, per-line statistics [2][N][2][512] f64, coefficients [2][N][4][512] f32
 extern "C" int crnn_lines_workspace_size(const crnn_model* m, int N, int W, size_t* bytes) {
   if (!m || !bytes) return crnn_fail(CRNN_INVALID_VALUE, "lines_workspace_size: null");
   if (N <= 0 || W < 8 || (W % 4) != 0) return crnn_fail(CRNN_INVALID_VALUE, "lines_workspace_size: need N>0, W>=8, W%%4==0");
-  if (m->cfg.compute_dtype >= 2) return crnn_fail(CRNN_UNSUPPORTED, "lines_workspace_size: packed evaluation runs on the bf16 path (compute_dtype 1)");
+  if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3)
+    return crnn_fail(CRNN_UNSUPPORTED, "lines_workspace_size: packed evaluation runs on the bf16 and fp8 paths (compute_dtype 1, 4)");
   Plan pl;
   *bytes = layout_plan(pl, N, W, nullptr, false) + align_up((size_t)N * 4) + align_up((size_t)2 * N * 2 * 512 * 8) +
            align_up((size_t)2 * N * 4 * 512 * 4);
@@ -832,7 +921,8 @@ extern "C" int crnn_lines_workspace_size(const crnn_model* m, int N, int W, size
 extern "C" int crnn_forward_lines(crnn_model* m, const float* data, const int* line_width, const int* time_step_len, int N, int W,
                                   float* logits_out, void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
   if (!m || !data || !line_width || !time_step_len || !logits_out || !workspace) return crnn_fail(CRNN_INVALID_VALUE, "forward_lines: null pointer");
-  if (m->cfg.compute_dtype >= 2) return crnn_fail(CRNN_UNSUPPORTED, "forward_lines: packed evaluation runs on the bf16 path (compute_dtype 1)");
+  if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3)
+    return crnn_fail(CRNN_UNSUPPORTED, "forward_lines: packed evaluation runs on the bf16 and fp8 paths (compute_dtype 1, 4)");
   if (m->training)
     return crnn_fail(CRNN_INVALID_VALUE, "forward_lines: evaluation only; the model is in training mode (training uses whole-batch statistics)");
   size_t need = 0;
@@ -841,7 +931,8 @@ extern "C" int crnn_forward_lines(crnn_model* m, const float* data, const int* l
   if (!m->conv1_tc || !m->conv2_swap)
     return crnn_fail(CRNN_UNSUPPORTED, "forward_lines: the line masks live in conv1_tc_kernel and conv2_swap_kernel (unset CRNN_CONV1 / CRNN_CONV2)");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return forward_impl(m, data, nullptr, time_step_len, N, W, logits_out, workspace, workspace_bytes, 1, st, st, nullptr, 1, line_width);
+  return forward_impl(m, data, nullptr, time_step_len, N, W, logits_out, workspace, workspace_bytes, 1, st, st, nullptr, 1, line_width,
+                      fwd_prec(m));
 }
 
 extern "C" int crnn_host_copy(void* dst, const void* src, size_t bytes, int threads) {
@@ -856,7 +947,7 @@ extern "C" int crnn_forward_pageable(crnn_model* m, const float* pageable_data, 
   if (!pageable_data || !pinned_staging || !data_staging) return crnn_fail(CRNN_INVALID_VALUE, "forward_pageable: null pointer");
   return forward_impl(m, data_staging, pinned_staging, time_step_len, N, W, logits_out, workspace, workspace_bytes, chunks,
                       reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<cudaStream_t>(copy_stream), pageable_data,
-                      host_threads < 1 ? 1 : host_threads);
+                      host_threads < 1 ? 1 : host_threads, nullptr, fwd_prec(m));
 }
 
 // ------------------------------------------------------------------------------------------------ profiling
@@ -903,7 +994,8 @@ extern "C" int crnn_total_loss(crnn_model* m, const float* costs, int N, float* 
 extern "C" int crnn_debug_tap(crnn_model* m, const char* name, float* dst, size_t dst_elems, void* workspace,
                               crnn_stream_t stream) {
   if (!m || !name || !dst) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: null");
-  if (m->cfg.compute_dtype >= 2) return x3_debug_tap(m, name, dst, dst_elems, workspace, reinterpret_cast<cudaStream_t>(stream));
+  if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3)
+    return x3_debug_tap(m, name, dst, dst_elems, workspace, reinterpret_cast<cudaStream_t>(stream));
   Plan& pl = m->plan;
   if (pl.ws == nullptr || pl.ws != workspace) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: no forward ran on this workspace");
   const size_t n = pl.N, h1 = pl.H1, h2 = pl.H2;
@@ -939,21 +1031,39 @@ extern "C" int crnn_debug_tap(crnn_model* m, const char* name, float* dst, size_
     if (src == nullptr) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: unknown tap %s", name);
   }
   if (dst_elems < cnt) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: dst too small (%zu < %zu)", dst_elems, cnt);
+  if (m->cfg.compute_dtype == 4) {
+    // the five e4m3 operands, dequantised with their scale (a calibration leaves the bf16 values in the same buffers, but a tap
+    // reads the last forward, which an fp8 model runs in e4m3)
+    const __nv_bfloat16* q[5] = {pl.a2, pl.a3, pl.a3p, pl.a4a, pl.a4b};
+    for (int i = 0; i < 5; ++i)
+      if (src == q[i]) return fp8_dequant_tap(m, i, src, dst, cnt, reinterpret_cast<cudaStream_t>(stream));
+  }
   return launch_bf16_to_f32(src, dst, cnt, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int crnn_debug_tap_raw(crnn_model* m, const char* name, void* dst, size_t dst_bytes, void* workspace,
                                   crnn_stream_t stream) {
   if (!m || !name || !dst) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: null");
-  if (m->cfg.compute_dtype >= 2) return x3_debug_tap_raw(m, name, dst, dst_bytes, workspace, reinterpret_cast<cudaStream_t>(stream));
+  if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3)
+    return x3_debug_tap_raw(m, name, dst, dst_bytes, workspace, reinterpret_cast<cudaStream_t>(stream));
+  std::string s(name);
+  if (m->cfg.compute_dtype == 4) {
+    int status = CRNN_OK;
+    if (fp8_debug_tap_raw(m, s, dst, dst_bytes, reinterpret_cast<cudaStream_t>(stream), &status)) return status;
+  }
   Plan& pl = m->plan;
   if (pl.ws == nullptr || pl.ws != workspace) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: no forward ran on this workspace");
   const size_t n = pl.N, h1 = pl.H1, h2 = pl.H2;
   const void* src = nullptr;
   size_t bytes = 0;
   bool train_only = false;
-  std::string s(name);
-  if (s == "bn" && pl.line_w) { src = pl.bn_l; bytes = 2 * n * 4 * 512 * sizeof(float); }
+  const bool q8 = m->cfg.compute_dtype == 4;
+  if (q8 && s == "conv2") { src = pl.a2; bytes = n * h2 * 8 * 128; }                 // e4m3 operands, byte for byte
+  else if (q8 && s == "conv3_1") { src = pl.a3; bytes = n * h2 * 8 * 256; }
+  else if (q8 && s == "conv3_2") { src = pl.a3p; bytes = n * h2 * 4 * 256; }
+  else if (q8 && s == "conv4_1") { src = pl.a4a; bytes = n * h2 * 4 * 512; }
+  else if (q8 && s == "conv4_2") { src = pl.a4b; bytes = n * h2 * 2 * 512; }
+  else if (s == "bn" && pl.line_w) { src = pl.bn_l; bytes = 2 * n * 4 * 512 * sizeof(float); }
   else if (s == "stats" && pl.line_w) { src = pl.stats_l; bytes = 2 * n * 2 * 512 * sizeof(double); }
   else if (s == "bn") { src = pl.bn; bytes = 2 * 4 * 512 * sizeof(float); }
   else if (s == "stats") { src = pl.stats; bytes = 2 * 2 * 512 * sizeof(double); }

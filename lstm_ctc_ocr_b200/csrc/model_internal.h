@@ -13,6 +13,9 @@ int make_tmap_nhwc(CUtensorMap* m, const void* base, int N, int H, int Wd, int C
 // f32 tensors read as tf32 operands: 32-element (128 B) boxes along the contiguous dimension
 int make_tmap_2d_f32(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t row_stride, uint32_t box_rows);
 int make_tmap_nhwc_f32(CUtensorMap* m, const void* base, int N, int H, int Wd, int C, int bh);
+// e4m3 tensors (UINT8 elements): 128-element (128 B) boxes along the contiguous dimension
+int make_tmap_2d_u8(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t row_stride, uint32_t box_rows);
+int make_tmap_nhwc_u8(CUtensorMap* m, const void* base, int N, int H, int Wd, int C, int bh);
 size_t align_up(size_t v, size_t a = 1024);
 int make_tmap_2d_box(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t row_stride, uint32_t box_cols,
                      uint32_t box_rows);
@@ -62,6 +65,9 @@ struct Plan {
   // the weight-gradient GEMMs read the same tensors through 64- or 32-position boxes (tW_*)
   int mg2 = 0, mg3 = 0, mg4 = 0, wm2 = 0, wm3 = 0, wm4 = 0;
   CUtensorMap tW_a1, tW_a2, tW_a3, tW_a3p, tW_a4a, tW_p4b, tW_p4a, tW_p32, tW_p31, tW_p2;
+  // compute_dtype 4: UINT8 views of the e4m3 activations, which live in the first half of the bf16 buffers a2, a3, a3p, a4a, a4b
+  // (forward_fp8.cu): A operands of conv3_1 .. conv5, conv3_1 stores through q_c32, conv2 / conv3_2 through qO_c2s / qO_c32
+  CUtensorMap q_c31, q_c32, q_c41, q_c42, q_c5, qO_c2s, qO_c32;
   // ---- training only -------------------------------------------------------------------------------------------
   bool train = false;
   uint8_t *am1, *am2, *am3;                       // arg-max window indices of pool1 / pool2 / the 1x2 pool after conv3_2
@@ -116,6 +122,7 @@ struct crnn_model {
   int lstm_upc = 32;         // hidden units per gate tile: 32 = persistent cluster kernel (default), 64 = per-step launches
   Plan plan;
   void* x3 = nullptr;        // state of the f32-class path (compute_dtype 2, forward_x3.cu)
+  void* fp8 = nullptr;       // e4m3 weights and scales of compute_dtype 4 (forward_fp8.cu)
   // ---- data parallelism (SURVEY 8(e)): BatchNorm statistics over the GLOBAL batch + per-bucket "gradient ready" notifications
   int dp_rank = 0, dp_world = 1;
   crnn_allreduce_fn xchg_cb = nullptr;   // fallback exchange of the [2][512] f64 BN sums (e.g. NCCL through the host language)
@@ -149,6 +156,24 @@ int x3_debug_tap(crnn_model* m, const char* name, float* dst, size_t dst_elems, 
 int x3_debug_tap_raw(crnn_model* m, const char* name, void* dst, size_t dst_bytes, void* workspace, cudaStream_t st);
 void x3_destroy(crnn_model* m);
 void x3_params_changed(crnn_model* m);
+
+// fp8 inference path (compute_dtype 4), forward_fp8.cu; the orchestration is model.cu's forward
+namespace convsw { struct Params; }
+int fp8_create(crnn_model* m);        // e4m3 weights, scales and scratch of a compute_dtype 4 model, allocated once at create
+void fp8_destroy(crnn_model* m);
+void fp8_params_changed(crnn_model* m);
+bool fp8_calibrated(const crnn_model* m);
+int fp8_prepare(crnn_model* m, cudaStream_t st);
+int fp8_plan_maps(Plan& pl);
+int fp8_conv2(crnn_model* m, convsw::Params p, bool lines, int sms, cudaStream_t st);
+int fp8_conv_gemm(crnn_model* m, int layer, gemm::Params p, bool lines, int sms, cudaStream_t st);
+int fp8_bn_apply(crnn_model* m, int layer, const float* bn, bool lines, cudaStream_t st);
+int fp8_conv5(crnn_model* m, gemm::Params p, int sms, cudaStream_t st);
+int fp8_finish_calibration(crnn_model* m, cudaStream_t st);
+int fp8_get_scales(crnn_model* m, float* host);
+int fp8_set_scales(crnn_model* m, const float* host);
+int fp8_dequant_tap(crnn_model* m, int idx, const void* src, float* dst, size_t n, cudaStream_t st);
+int fp8_debug_tap_raw(crnn_model* m, const std::string& name, void* dst, size_t dst_bytes, cudaStream_t st, int* status);
 
 // SyncBN exchange (peer.cu): sums of `in` [1024] f64 over all ranks -> `out` (may alias `in`); optionally fused with the BN finalize
 int dp_allreduce_1024(crnn_model* m, const double* in, double* out, cudaStream_t st);

@@ -249,6 +249,21 @@ __device__ __forceinline__ uint32_t hmax2_bf16(uint32_t a, uint32_t b) {
   __nv_bfloat162 r = __hmax2(x, y);
   return *reinterpret_cast<uint32_t*>(&r);
 }
+// two f32 -> two e4m3 (round to nearest even, saturating to +-448; NaN stays NaN): `lo` in bits 0..7, `hi` in bits 8..15
+__device__ __forceinline__ uint32_t pack_e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+// four f32 -> one 32-bit word of e4m3, a in the lowest byte
+__device__ __forceinline__ uint32_t pack_e4m3x4(float a, float b, float c, float d) {
+  return pack_e4m3x2(a, b) | (pack_e4m3x2(c, d) << 16);
+}
+__device__ __forceinline__ float e4m3_to_f32(uint32_t byte) {
+  uint32_t h;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h) : "h"((uint16_t)byte));
+  return __half2float(__ushort_as_half((unsigned short)(h & 0xFFFFu)));
+}
 __device__ __forceinline__ float bf16_lo(uint32_t v) { return __uint_as_float(v << 16); }
 __device__ __forceinline__ float bf16_hi(uint32_t v) { return __uint_as_float(v & 0xFFFF0000u); }
 

@@ -18,6 +18,9 @@ SOLVER_SLOTS = {"Adam": (("adam_m", "adam_m"), ("adam_v", "adam_v")),
                 "RMS": (("rms", "adam_v"), ("rms_momentum", "adam_m"))}
 # tf.train.RMSPropOptimizer defaults: the reference constructs it with the learning rate alone (lib/lstm/train.py:75)
 RMS_DECAY, RMS_MOMENTUM, RMS_EPSILON = 0.9, 0.0, 1e-10
+# the five e4m3 GEMMs of compute_dtype "fp8": layer -> (K, Cout) of its [Cout][K] weight operand
+FP8_WEIGHTS = OrderedDict([("conv3_1", (1152, 256)), ("conv3_2", (2304, 256)), ("conv4_1", (2304, 512)), ("conv4_2", (4608, 512)),
+                           ("conv5", (2048, 512))])
 
 
 def _stream():
@@ -38,8 +41,9 @@ class CrnnModel:
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         torch.cuda.set_device(self.device)
         # "bf16": bf16 operands / f32 accumulate (throughput path); "f32": split-bf16 operands, f32-class (BASELINE configs[1]);
-        # "tf32": tf32 operands, same forward-only orchestration as "f32"
-        self.compute_dtype = {"bf16": 1, "f32": 2, "tf32": 3, 1: 1, 2: 2, 3: 3}[compute_dtype]
+        # "tf32": tf32 operands, same forward-only orchestration as "f32"; "fp8": e4m3 operands in conv3_1 .. conv5, inference
+        # only, after calibrate_fp8 / set_fp8_scales
+        self.compute_dtype = {"bf16": 1, "f32": 2, "tf32": 3, "fp8": 4, 1: 1, 2: 2, 3: 3, 4: 4}[compute_dtype]
         cfg = CrnnConfig(32, NCLASSES, 512, bn_eps, weight_decay, self.compute_dtype)
         h = _lib.c_void_p()
         check(self.lib.crnn_model_create(cfg, h))
@@ -62,6 +66,7 @@ class CrnnModel:
         self._ws_key = None
         self._ws_lines = False
         self.training = False
+        self.fp8_calibrated = False     # fp8: activation scales valid for the loaded parameters (load_params invalidates them)
 
     # ---- training --------------------------------------------------------------------------
     def set_training(self, flag=True):
@@ -129,6 +134,7 @@ class CrnnModel:
 
     def _bind(self):
         check(self.lib.crnn_model_bind(self.handle, _ptr(self.params), _ptr(self.grads), _ptr(self.adam_m), _ptr(self.adam_v)))
+        self.fp8_calibrated = False     # a bind invalidates the fp8 scales, as a parameter change does
 
     def __del__(self):
         try:
@@ -151,6 +157,7 @@ class CrnnModel:
             v = torch.as_tensor(np.asarray(v, dtype=np.float32)) if not torch.is_tensor(v) else v.detach().float().cpu()
             self.tensor(name).copy_(v.to(self.device))
         check(self.lib.crnn_model_params_changed(self.handle))
+        self.fp8_calibrated = False
 
     def state_dict(self):
         return OrderedDict((k, self.tensor(k).detach().cpu().numpy().copy()) for k in self.table)
@@ -187,6 +194,31 @@ class CrnnModel:
         check(self.lib.crnn_forward(self.handle, data.data_ptr(), time_step_len.data_ptr(), N, W, out.data_ptr(), ws,
                                     nbytes, _stream()))
         return out
+
+    # ---- fp8 scales (compute_dtype "fp8") -----------------------------------------------------
+    def calibrate_fp8(self, data, time_step_len):
+        """Set the five activation scales of an fp8 model from a calibration batch (data [N,W,32] f32 cuda, time_step_len [N]
+        i32 cuda): the bf16 front end runs on it and each scale becomes 2^ceil(log2(amax / 448)).  Asynchronous, on the device."""
+        assert data.is_cuda and data.dtype == torch.float32 and data.is_contiguous()
+        assert time_step_len.is_cuda and time_step_len.dtype == torch.int32
+        N, W, Hh = data.shape
+        if Hh != 32:
+            raise CrnnError("data must be [N, W, 32] (cfg.NUM_FEATURES = 32)")
+        ws, nbytes = self._workspace(N, W)
+        check(self.lib.crnn_model_calibrate_fp8(self.handle, data.data_ptr(), time_step_len.data_ptr(), N, W, ws, nbytes, _stream()))
+        self.fp8_calibrated = True
+
+    def fp8_scales(self):
+        """The five activation scales (a2, a3, a3p, a4a, a4b) as a float32 numpy array; synchronises the device."""
+        out = np.zeros(5, dtype=np.float32)
+        check(self.lib.crnn_model_get_fp8_scales(self.handle, out.ctypes.data))
+        return out
+
+    def set_fp8_scales(self, scales):
+        """Set the five activation scales (powers of two, else CrnnError with CRNN_INVALID_VALUE)."""
+        s = np.ascontiguousarray(np.asarray(scales, dtype=np.float32).reshape(5))
+        check(self.lib.crnn_model_set_fp8_scales(self.handle, s.ctypes.data))
+        self.fp8_calibrated = True
 
     def forward_lines(self, data, line_width, time_step_len, out=None):
         """Packed evaluation: data [N,W,32] f32 cuda holding line i in columns [0, W_i), line_width [N] i32 cuda (W_i, a multiple
@@ -278,7 +310,8 @@ class CrnnModel:
         f32-class paths: "cst" f32 [2][Npad][256] (final cell state) and the stored activations "conv1" .. "conv5",
         "lstm_out": "f32" (split) bf16 [..., 2 (hi, lo), C] per position, conv4_2 [N, H2, 2 (hi, lo), 2 positions, 512]
         (rows of G = 2 positions); "tf32" f32 in the tap shape.  lines=True (after forward_lines): per-line "bn" f32 [2][N][4][512]
-        and "stats" f64 [2][N][2][512]."""
+        and "stats" f64 [2][N][2][512].  "fp8": the e4m3 operands "conv2" .. "conv4_2" as u8 bytes in the tap shape, "fp8_scales"
+        f32 [5], "fp8_wscale" / "fp8_colscale" f32 [5][512], "fp8_w_<layer>" u8 [Cout][K] (FP8_WEIGHTS)."""
         H1, H2 = W // 2, W // 4
         Npad, T = (N + 127) // 128 * 128, H2 - 1
         shapes = {"bn": ((2, 4, 512), torch.float32), "stats": ((2, 2, 512), torch.float64)}
@@ -287,6 +320,14 @@ class CrnnModel:
         if self.compute_dtype == 1:
             shapes.update({"am1": ((N, H1, 16, 64), torch.uint8), "am2": ((N, H2, 8, 128), torch.uint8),
                            "am3": ((N, H2, 4, 256), torch.uint8), "csave": ((2 * Npad // 128, T, 64, 128, 4), torch.float32)})
+        elif self.compute_dtype == 4:
+            # fp8: the e4m3 operands as stored, the activation scales, per-layer weight scales and colscale ([5][512]), e4m3 weights
+            shapes.update({"conv2": ((N, H2, 8, 128), torch.uint8), "conv3_1": ((N, H2, 8, 256), torch.uint8),
+                           "conv3_2": ((N, H2, 4, 256), torch.uint8), "conv4_1": ((N, H2, 4, 512), torch.uint8),
+                           "conv4_2": ((N, H2, 2, 512), torch.uint8), "fp8_scales": ((5,), torch.float32),
+                           "fp8_wscale": ((5, 512), torch.float32), "fp8_colscale": ((5, 512), torch.float32)})
+            for k, (K, co) in FP8_WEIGHTS.items():
+                shapes["fp8_w_" + k] = ((co, K), torch.uint8)
         else:
             acts = {"conv1": (N, H1, 16), "conv2": (N, H2, 8), "conv3_1": (N, H2, 8), "conv3_2": (N, H2, 4),
                     "conv4_1": (N, H2, 4), "conv4_2": (N, H2), "conv5": (N, H2), "lstm_out": (N, H2)}

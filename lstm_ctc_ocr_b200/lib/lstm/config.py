@@ -48,7 +48,10 @@ _DEFAULTS = {
     "VAL": {"TXT": "annotation_val.txt", "VAL_STEP": 1000, "NUM_EPOCHS": 1000, "BATCH_SIZE": 128, "PRINT_NUM": 5},
     # not in the reference (one line per run): lines per packed evaluation batch of test_model, each line still evaluated as if
     # alone (DESIGN §5 has the measured rates behind the default)
-    "TEST": {"BATCH_SIZE": 64},
+    "TEST": {"BATCH_SIZE": 64,
+             # not in the reference: "fp8" evaluates LSTM_test networks with e4m3 operands in conv3_1 .. conv5 (compute_dtype 4),
+             # calibrated on a fixed rendered set when the weights are assigned
+             "COMPUTE_DTYPE": "bf16"},
 }
 
 

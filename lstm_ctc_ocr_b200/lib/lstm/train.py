@@ -101,6 +101,9 @@ class SolverWrapper(object):
         blob = np.load(path + ".npz")
         eng = sess.engine_for(self.net)
         eng.load_params({k: blob[k] for k in eng.table})
+        loaded = getattr(sess, "params_loaded", None)     # Session: an fp8 evaluation engine recalibrates for the restored weights
+        if loaded is not None:
+            loaded(self.net)
         if eng.adam_m is not None:
             restore_slots(eng, blob)
         return blob

@@ -118,10 +118,24 @@ def _draw_glyph(d, g, font, ch, x, y, fill):
     d.draw.draw_bitmap((x + off[0], y + off[1]), mask, d.draw.draw_ink(fill))
 
 
-def render_line(chars, height=60, width=None, rng=random):
-    """Gray uint8 HxW image of the text (stand-in for ImageCaptcha.generate_image + gray conversion, gen.py:31-37,79)."""
+def embedded_font(size=42):
+    """Pillow's embedded scalable font, the one CRNN_FONT=default selects: the same glyphs on every machine with the same
+    Pillow, whatever fonts are installed."""
+    from PIL import ImageFont
+    key = (None, size)
+    if key not in _FONT_CACHE:
+        try:
+            _FONT_CACHE[key] = ImageFont.load_default(size)
+        except Exception:
+            _FONT_CACHE[key] = ImageFont.load_default()
+    return _FONT_CACHE[key]
+
+
+def render_line(chars, height=60, width=None, rng=random, font=None):
+    """Gray uint8 HxW image of the text (stand-in for ImageCaptcha.generate_image + gray conversion, gen.py:31-37,79).
+    `font`: a PIL font to draw with instead of the configured one (_font)."""
     from PIL import Image, ImageDraw
-    font = _font(42)
+    font = _font(42) if font is None else font
     g = _glyphs(font)
     advc = g["adv"]
     adv = []

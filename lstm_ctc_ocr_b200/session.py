@@ -235,7 +235,12 @@ class Session(object):
         eng = self._engines.get(id(net))
         if eng is None:
             from .lib.lstm.config import cfg
-            eng = engine.CrnnModel(weight_decay=float(getattr(net, "_wd", cfg.TRAIN.WEIGHT_DECAY)), device=self.device)
+            # evaluation networks run in cfg.TEST.COMPUTE_DTYPE ("bf16" or "fp8"); training networks ignore the key
+            dt = str(cfg.TEST.get("COMPUTE_DTYPE", "bf16")) if type(net).__name__ == "LSTM_test" else "bf16"
+            if dt not in ("bf16", "fp8"):
+                raise ValueError(f"cfg.TEST.COMPUTE_DTYPE must be 'bf16' or 'fp8', got {dt!r}")
+            eng = engine.CrnnModel(weight_decay=float(getattr(net, "_wd", cfg.TRAIN.WEIGHT_DECAY)), device=self.device,
+                                   compute_dtype=dt)
             self._engines[id(net)] = eng
         return eng
 
@@ -248,6 +253,33 @@ class Session(object):
             elif not ignore_missing:
                 raise KeyError(k)
         eng.load_params(full)
+        self.params_loaded(net)
+
+    def params_loaded(self, net):
+        """Call after a network's parameters were (re)loaded -- assign and checkpoint restores do.  An fp8 engine gets its
+        activation scales here: a parameter change invalidates them."""
+        eng = self.engine_for(net)
+        if eng.compute_dtype == 4:
+            self._calibrate_fp8(eng)
+
+    FP8_CALIBRATION_LINES, FP8_CALIBRATION_WIDTH = 256, 256
+
+    def _calibrate_fp8(self, eng):
+        """An fp8 engine's activation scales from a fixed calibration set the package renders itself: 256 lines of the data
+        path's default stream (seed cfg.RNG_SEED) drawn in Pillow's embedded font (whatever fonts the machine has), padded to
+        256 px.  The scales depend on the weights (and the Pillow version) alone, never on the lines being evaluated, so a
+        line evaluated in a packed batch still computes as if alone."""
+        import random
+        from .lib.lstm.config import cfg
+        from .lib.lstm.utils import gen
+        if getattr(self, "_fp8_cal", None) is None:
+            rng = random.Random(int(cfg.RNG_SEED))
+            font = gen.embedded_font(42)
+            labels = [gen.gen_rand(rng) for _ in range(self.FP8_CALIBRATION_LINES)]
+            imgs, _, _, tsl = gen.groupBatch([gen.render_line(t, rng=rng, font=font) for t in labels], labels,
+                                             pad_to=self.FP8_CALIBRATION_WIDTH)
+            self._fp8_cal = (torch.tensor(np.stack(imgs), device=self.device), torch.tensor(np.asarray(tsl, np.int32), device=self.device))
+        eng.calibrate_fp8(*self._fp8_cal)
 
     def variables(self, net):
         return self.engine_for(net).state_dict()
@@ -307,6 +339,8 @@ class Session(object):
         labels = np.asarray(feeds["labels"], dtype=np.int32) if need_labels else None
         llen = np.asarray(feeds["labels_len"], dtype=np.int32) if need_labels else None
         eng = self.engine_for(net)
+        if eng.compute_dtype == 4 and not eng.fp8_calibrated:
+            self._calibrate_fp8(eng)        # parameters loaded straight into the engine (not through assign / a restore)
         dev = self.device
         if feeds.get("line_width") is not None:
             return self._run_lines(flist, single, net, eng, data, tsl, labels, llen, np.asarray(feeds["line_width"], dtype=np.int32))

@@ -144,3 +144,79 @@ def test_stage_references_chain_to_the_direct_quantised_graph():
     direct = _direct_quantised_graph(a1, W, b, bn, s, eps)
     assert out.shape == direct.shape == (2, 5, 512)
     assert float((out - direct).abs().max()) <= 1e-9 * float(direct.abs().max())
+
+
+# ---------------------------------------------------------------------------------------------------------- packed lines
+PACKED_WIDTHS = [8, 12, 20, 36]
+
+
+def _quantised_weights(seed=3):
+    from oracle import crnn_oracle as O
+    pn = O.randomize_params(O.init_params(seed, dtype=np.float32, logits_scale=10.0), seed=seed + 8)
+    P = {k: torch.as_tensor(np.asarray(v, np.float64)) for k, v in pn.items()}
+    W = {"conv2": S.bf16(P["conv2/weights"])}
+    for k in ("conv3_1", "conv3_2", "conv4_1", "conv4_2", "conv5"):
+        q, sw = weight_restatement(pn[k + "/weights"])
+        co, kh = q.shape[0], 2 if k == "conv5" else 3
+        W[k] = (q.view(torch.float8_e4m3fn).double() * sw.double()[:, None]).reshape(co, kh, kh, -1).permute(1, 2, 3, 0)
+    b = {k: P[k + "/biases"] for k in W}
+    bn = {k: (P[f"{k}/{k}/gamma"], P[f"{k}/{k}/beta"]) for k in ("conv4_1", "conv4_2")}
+    return W, b, bn
+
+
+def packed_fp8_reference(a1, lw, Wq, b, bn, scales=None, masks=True):
+    """The fp8 graph conv2 .. conv5 over a packed batch as tests/test_gpu_fp8_edges.py restates it: each stage over the
+    whole packed tensor through the stage references, then the line mask (zero at h >= W_i / 4) on the result; BatchNorm per
+    line with count W_i.  a1 [N, H1, 16, 64] is zero at h >= W_i / 2.  scales None: each from the rule on its own amax.
+    Returns the stage outputs (e4m3 values times their scale, bf16 pre-BN values, conv5) and the scales used."""
+    N, H2 = a1.shape[0], a1.shape[1] // 2
+    keep = torch.stack([torch.arange(H2) < (w // 4 if masks else H2) for w in lw]).double()[:, :, None, None]
+    s = [] if scales is None else list(scales)
+    out = {}
+
+    def quant(name, i, y):
+        if scales is None:
+            s.append(float(scale_rule(float(y.abs().max()))))
+        out[name] = e4m3(y * keep / s[i]) * s[i]
+        return out[name]
+    x = quant("conv2", 0, S.conv_relu_pool22_stage(a1, Wq["conv2"], b["conv2"])["out"])
+    x = quant("conv3_1", 1, S.conv_relu_stage(x, Wq["conv3_1"], b["conv3_1"])["out"])
+    x = quant("conv3_2", 2, S.conv_relu_pool12_stage(x, Wq["conv3_2"], b["conv3_2"])["out"])
+    cnt = torch.tensor(lw, dtype=torch.float64)[:, None]
+    for l, (k, pre) in enumerate((("conv4_1", "a4a_pre"), ("conv4_2", "a4b_pre"))):
+        p = out[pre] = S.bf16(S.conv_bias_stage(x, Wq[k], b[k])["out"]) * keep
+        st = S.bn_stats_stage(None, *bn[k], float(np.float32(1e-3)),
+                              parts=dict(sum=p.sum((1, 2)), sumsq=(p * p).sum((1, 2)), sum_acc=p.abs().sum((1, 2)), cnt=cnt))
+        sc, sh = st["scale"][:, None, None, :], st["shift"][:, None, None, :]
+        y = S.bn_apply_relu_stage(p, sc, sh)["out"] if l == 0 else S.bn_apply_relu_pool_stage(p, sc, sh, rnd=S.ident)["out"]
+        x = quant(k, 3 + l, y)
+    out["conv5"] = S.conv5_stage(x, Wq["conv5"], b["conv5"])["out"]
+    return out, s
+
+
+def _packed_vs_alone(masks):
+    """Worst relative difference, over every stage and line, between the packed reference and each line fed alone."""
+    Wq, b, bn = _quantised_weights()
+    W = max(PACKED_WIDTHS)
+    rng = np.random.default_rng(4)
+    a1 = torch.zeros((len(PACKED_WIDTHS), W // 2, 16, 64), dtype=torch.float64)
+    for i, w in enumerate(PACKED_WIDTHS):
+        a1[i, :w // 2] = torch.as_tensor(rng.random((w // 2, 16, 64)))
+    packed, scales = packed_fp8_reference(a1, PACKED_WIDTHS, Wq, b, bn, masks=masks)
+    worst = 0.0
+    for i, w in enumerate(PACKED_WIDTHS):
+        alone, _ = packed_fp8_reference(a1[i:i + 1, :w // 2], [w], Wq, b, bn, scales=scales)
+        for k, a in alone.items():
+            p = packed[k][i:i + 1, :a.shape[1]]
+            worst = max(worst, float((p - a).abs().max()) / max(float(a.abs().max()), 1e-30))
+    return worst
+
+
+def test_packed_fp8_reference_equals_each_line_alone():
+    """The shortcut of the GPU's packed-line check: a SAME convolution over the packed tensor (zero past each line), masked
+    by line, is each line's own zero-padded convolution -- through e4m3 quantisation, per-line BatchNorm and conv5."""
+    assert _packed_vs_alone(masks=True) <= 1e-12
+
+
+def test_packed_fp8_reference_without_masks_differs():
+    assert _packed_vs_alone(masks=False) > 1e-3

@@ -10,7 +10,11 @@ e4m3 wgmma operands.  Need the GPU.
      bf16 outputs (conv4_x pre-BN, conv5):   half a bf16 ulp + c * acc
    acc = the same operation on absolute values.  BatchNorm + ReLU (+ pool3) into e4m3 must equal the e4m3 rounding of the
    f32 value exactly.  The weight operands and scales must equal their restatement bit for bit.  MEASURED holds the largest c
-   each stage needed on an H100 80GB HBM3; the bound is 4.5x it.
+   each stage needed on an H100 80GB HBM3; the bound is 4.5x it.  The f64 BatchNorm sums (against fp64 sums of the GPU's own
+   bf16 pre-activations) and the f32 coefficients (against the fp64 finalize of those sums), and the stages after conv5 --
+   input projection, recurrence (free-running, and every step teacher-forced by the GPU's own h), lstm_out zero past each
+   length, logits, the bias past each length -- run the bf16 path's kernels and keep its bounds (test_gpu_stage_isolation).
+   tests/test_gpu_fp8_edges.py runs the same checks at the widths, batches and state changes evaluation meets.
 2. Whole chain against the fp64 oracle of the unquantised weights: tap, logit and loss errors, bounded at 4.5x their measured
    value and appended to build/parity_report.jsonl; logits past each length are exactly the projection bias.
 3. Packed evaluation: every evaluation line's fp8 logits in a packed batch equal the line run alone through crnn_forward with
@@ -26,7 +30,9 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import stage_refs as S  # noqa: E402
+import test_gpu_stage_isolation as B  # noqa: E402
 from stage_check import SHAPES, Checker, ulp_bf16, widths_of  # noqa: E402
+from test_gpu_stage_isolation_batch import PEAK_LIMIT  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -66,8 +72,16 @@ def decode(raw):
 
 
 def _params(seed):
+    """Random test weights whose fp8 layers scale each output channel by its own 2^U(-1, 1).  The xavier-uniform init alone
+    puts every channel's amax within 0.1 % of the same limit, so the per-channel weight scales (and colscale) would be
+    nearly equal and an epilogue reading the wrong channel's scale would go unnoticed."""
     from oracle import crnn_oracle as O
-    return O.randomize_params(O.init_params(seed, dtype=np.float32, logits_scale=10.0), seed=seed + 8)
+    p = O.randomize_params(O.init_params(seed, dtype=np.float32, logits_scale=10.0), seed=seed + 8)
+    rng = np.random.default_rng(seed + 100)
+    for k in FP8_LAYERS:
+        w = p[k + "/weights"]
+        p[k + "/weights"] = (w * np.exp2(rng.uniform(-1.0, 1.0, w.shape[-1]))).astype(np.float32)
+    return p
 
 
 def _model(pn, mode="fp8"):
@@ -117,32 +131,89 @@ def weight_restatement(w):
 
 
 # ------------------------------------------------------------------------------------------------ 1. stage isolation
-def _stage_checks(case, N, W, widths, seed=5, sample=None, shrink=1):
-    """shrink > 1: run with every activation scale `shrink` times below the calibrated one, so that the producers saturate."""
+REPORT = "fp8_stage_isolation_report.jsonl"
+# the stages after conv5 run the bf16 path's kernels (input projection, recurrence, logits) on the fp8 conv5 output, and the
+# fp8 path's BatchNorm statistics are the bf16 path's f64 sums of bf16 pre-activations: they keep the bf16 path's bounds
+BF16_BOUNDS = dict(B.STAGE_BOUNDS, **BOUNDS)
+
+
+def e4m3_stage(ck8, saturated, stage, gpu_q, ref, acc, s_out):
+    """An e4m3 producer: within half an e4m3 ulp + c * acc of ref / s_out, and exactly 448 where that exceeds the range."""
+    r, a = ref / s_out, acc / s_out
+    sat = r > 448.0 + BOUNDS[stage][1] * a
+    saturated[stage] = saturated.get(stage, 0) + int(sat.sum())
+    ck8.exact(stage + "_saturated", gpu_q[sat], 448.0)
+    ck8.close(stage, gpu_q, r.clamp(max=448.0), a)
+
+
+def bn_apply_want(x_pre, scale, shift, s_out, pool):
+    """BatchNorm + ReLU (+ pool3) into e4m3: the e4m3 rounding of the f32 fma, and the count of values past the range."""
+    y = torch.relu((x_pre * scale + shift).float().double())               # fma in f32: one rounding of the exact value
+    if pool:
+        y, _ = S.pool12(y)
+    return e4m3(y * (1.0 / s_out)), int((y * (1.0 / s_out) > 448.0).sum())
+
+
+def tail_checks(ck, P, G, logits, tsl, T, parts):
+    """The stages after conv5, on the images of `parts` (lists of image indices), each on its own GPU operands: the input
+    projection from the tapped conv5 (backward rows reversed by length), the free-running recurrence, every step teacher-forced
+    by the GPU's own h (the inference plan keeps no gates or cell state, so c is carried in fp64 from step to step and enters
+    through h), the logits; on the whole batch lstm_out's raw bits zero past each length and the logits there the bias."""
+    Wb = {k: S.bf16(v) for k, v in P.items() if k.endswith("weights")}
+    wh = (Wb[B.FW + "/weights"][512:], Wb[B.BW + "/weights"][512:])
+    tsl = np.asarray(tsl)
+    N, H2 = G["lstm_out"].shape[:2]
+    L = torch.as_tensor(S.clamp_lens(tsl, T), device=DEV)
+    valid = torch.arange(H2, device=DEV)[None, :] < L[:, None]
+    ck.exact("lstm_out_past_len_zero", G["lstm_out"][~valid].view(torch.int32), 0)
+    past = torch.arange(T, device=DEV)[:, None] >= L[None, :]
+    ck.exact("logits_past_len_bias", logits[past], P["logits/biases"].float())
+    for s in parts:
+        lens = tsl[s]
+        xp, lo = G["xproj"][s].double(), G["lstm_out"][s].double()
+        r = S.xproj_stage(G["conv5"][s].double(), Wb[B.FW + "/weights"][:512], Wb[B.BW + "/weights"][:512],
+                          P[B.FW + "/biases"], P[B.BW + "/biases"], lens, T)
+        ck.close("xproj", xp, r["out"], r["acc"])
+        r = S.recurrence_stage(xp, wh[0], wh[1], lens, T)
+        ck.close_scaled("lstm_out", lo, r["out"], mask=valid[s][..., None].expand(r["out"].shape))
+        iso = S.recurrence_steps_isolated(xp, wh[0], wh[1], lo, None, lens, T)
+        act2 = (torch.arange(T, device=DEV)[None, :] < L[s][:, None])[None].expand(2, -1, -1)
+        ck.close_scaled("step_h", S.step_h(lo, lens, T)[act2], iso["h"][act2])
+        r = S.logits_stage(lo, Wb["logits/weights"], P["logits/biases"], T)
+        ck.close("logits", logits[:, s], r["out"], r["acc"])
+
+
+def _stage_checks(case, N, W, widths, seed=5, sample=None, shrink=1, chunk=None, m=None, pn=None, report=REPORT,
+                  extra_bounds=None, peak=False):
+    """One fp8 forward, every stage against fp64 on its own operands.  shrink > 1: run with every activation scale `shrink`
+    times below the calibrated one, so that the producers saturate.  chunk: images per fp64 restatement (the whole batch by
+    default).  sample: the images of the per-image front-end and tail stages (conv4_x, the BatchNorms and conv5 always run on
+    the whole batch).  m / pn: a model to reuse and the parameters it holds.  extra_bounds override the bf16-output bounds.
+    peak: record the peak GPU memory.  Returns (saturated counts, the forward's bits: logits and the stored operands)."""
     from oracle import crnn_oracle as O
-    pn = _params(3)
-    m = _model(pn)
+    pn = _params(3) if pn is None else pn
+    m = _model(pn) if m is None else m
     data, lab, ll, tsl = O.synth_batch(N, W, seed=seed, widths=widths_of(N, W, widths), min_len=1, max_len=4)
     d, tl = _t(data), _t(tsl)
     m.calibrate_fp8(d, tl)
     if shrink > 1:
         m.set_fp8_scales(m.fp8_scales() / np.float32(shrink))
-    m.forward(d, tl)
+    logits = m.forward(d, tl)
     torch.cuda.synchronize()
     T = W // 4 - 1
     # everything on the device in fp64: the C3 restatement is a few TFLOP
     scales = m.tap_raw("fp8_scales", N, W).double()
-    raw = {k: m.tap_raw(k, N, W) for k in FP8_ACTS + ("bn",)}
-    q = {k: decode(raw[k]) for k in FP8_ACTS}
-    val = {k: q[k] * scales[i] for i, k in enumerate(FP8_ACTS)}
-    a1 = m.tap("conv1", N, W).double()
-    pre = {k: m.tap(k, N, W).double() for k in ("a4a_pre", "a4b_pre")}
-    a5 = m.tap("conv5", N, W).double()
+    raw = {k: m.tap_raw(k, N, W) for k in FP8_ACTS + ("bn", "stats")}
+    G = {k: m.tap(k, N, W) for k in ("conv1", "a4a_pre", "a4b_pre", "conv5", "xproj", "lstm_out")}
     Wq, Wraw, wsc = _weights(m, N, W)
     P = {k: torch.as_tensor(np.asarray(v, np.float64), device=DEV) for k, v in pn.items()}
-    img = list(range(N)) if sample is None else sample
-    ck8 = Checker(f"fp8/{case}", BOUNDS, "fp8_stage_isolation_report.jsonl", ulp_e4m3)
-    ckb = Checker(f"fp8_bf16/{case}", BOUNDS, "fp8_stage_isolation_report.jsonl", ulp_bf16)
+    img = list(range(N)) if sample is None else list(sample)
+    n = chunk or N
+    parts = lambda idx: [idx[i:i + n] for i in range(0, len(idx), n)]  # noqa: E731
+    q = lambda k, s: decode(raw[k][s])                                   # noqa: E731
+    val = lambda k, s: q(k, s) * scales[FP8_ACTS.index(k)]              # noqa: E731
+    ck8 = Checker(f"fp8/{case}", BOUNDS, report, ulp_e4m3)
+    ckb = Checker(f"fp8_bf16/{case}", dict(BF16_BOUNDS, **(extra_bounds or {})), report, ulp_bf16)
 
     # weight operands: bit for bit their restatement
     for l, k in enumerate(FP8_LAYERS):
@@ -151,44 +222,56 @@ def _stage_checks(case, N, W, widths, seed=5, sample=None, shrink=1):
         ck8.exact(f"wscale_{k}", wsc[l, :qr.shape[0]].float().cpu().numpy(), sr.numpy())
 
     saturated = {}
-
-    def e4m3_stage(stage, gpu_q, ref, acc, s_out):
-        r, a = ref / s_out, acc / s_out
-        c = BOUNDS[stage][1]
-        sat = r > 448.0 + c * a
-        saturated[stage] = int(sat.sum())
-        ck8.exact(stage + "_saturated", gpu_q[sat], 448.0)
-        ck8.close(stage, gpu_q, r.clamp(max=448.0), a)
-
-    # conv2 (bf16 mainloop) -> e4m3 a2
-    r = S.conv_relu_pool22_stage(a1[img], S.bf16(P["conv2/weights"]), P["conv2/biases"])
-    e4m3_stage("conv2", q["conv2"][img], r["out"], r["acc"], scales[0])
-    # conv3_1 (e4m3 x e4m3) -> e4m3 a3
-    r = S.conv_relu_stage(val["conv2"][img], Wq["conv3_1"], P["conv3_1/biases"])
-    e4m3_stage("conv3_1", q["conv3_1"][img], r["out"], r["acc"], scales[1])
-    # conv3_2 + pool -> e4m3 a3p
-    r = S.conv_relu_pool12_stage(val["conv3_1"][img], Wq["conv3_2"], P["conv3_2/biases"])
-    e4m3_stage("conv3_2", q["conv3_2"][img], r["out"], r["acc"], scales[2])
-    # conv4_1 / conv4_2 -> bf16 pre-BN (whole batch: the statistics need every image)
-    r = S.conv_bias_stage(val["conv3_2"], Wq["conv4_1"], P["conv4_1/biases"])
-    ckb.close("conv4_1", pre["a4a_pre"], r["out"], r["acc"])
-    r = S.conv_bias_stage(val["conv4_1"], Wq["conv4_2"], P["conv4_2/biases"])
-    ckb.close("conv4_2", pre["a4b_pre"], r["out"], r["acc"])
-    # BatchNorm + ReLU (+ pool3) into e4m3: the e4m3 rounding of the f32 value, exactly
+    for s in parts(img):
+        # conv2 (bf16 mainloop) -> e4m3 a2
+        r = S.conv_relu_pool22_stage(G["conv1"][s].double(), S.bf16(P["conv2/weights"]), P["conv2/biases"])
+        e4m3_stage(ck8, saturated, "conv2", q("conv2", s), r["out"], r["acc"], scales[0])
+        # conv3_1 (e4m3 x e4m3) -> e4m3 a3
+        r = S.conv_relu_stage(val("conv2", s), Wq["conv3_1"], P["conv3_1/biases"])
+        e4m3_stage(ck8, saturated, "conv3_1", q("conv3_1", s), r["out"], r["acc"], scales[1])
+        # conv3_2 + pool -> e4m3 a3p
+        r = S.conv_relu_pool12_stage(val("conv3_1", s), Wq["conv3_2"], P["conv3_2/biases"])
+        e4m3_stage(ck8, saturated, "conv3_2", q("conv3_2", s), r["out"], r["acc"], scales[2])
+        del r
     bn = raw["bn"].double()
-    for l, (k, x) in enumerate((("conv4_1", pre["a4a_pre"]), ("conv4_2", pre["a4b_pre"]))):
-        y = torch.relu((x * bn[l, 0] + bn[l, 1]).float().double())        # fma in f32: one rounding of the exact value
-        if k == "conv4_2":
-            y, _ = S.pool12(y)
-        want = e4m3(y * (1.0 / scales[3 + l]))
-        saturated[f"bn_apply_{k}"] = int((y * (1.0 / scales[3 + l]) > 448.0).sum())
-        ck8.exact(f"bn_apply_{k}", q[k], want)
-    # conv5 (2x2 VALID over e4m3 a4b) -> bf16
-    r = S.conv5_stage(val["conv4_2"], Wq["conv5"], P["conv5/biases"])
-    ckb.close("conv5", a5[:, :T], r["out"], r["acc"])
-    ck8.assert_ok()
-    ckb.assert_ok()
-    return saturated
+    bnp = [{}, {}]
+    for s in parts(list(range(N))):
+        for l, (k, src, pre) in enumerate((("conv4_1", "conv3_2", "a4a_pre"), ("conv4_2", "conv4_1", "a4b_pre"))):
+            # conv4_1 / conv4_2 -> bf16 pre-BN, and the batch sums of those bf16 values
+            x = G[pre][s].double()
+            r = S.conv_bias_stage(val(src, s), Wq[k], P[k + "/biases"])
+            ckb.close(k, x, r["out"], r["acc"])
+            B._sum_into(bnp[l], S.bn_sums(x))
+            # BatchNorm + ReLU (+ pool3) into e4m3 with the GPU's coefficients: the e4m3 rounding of the f32 value, exactly
+            want, sat = bn_apply_want(x, bn[l, 0], bn[l, 1], scales[3 + l], l == 1)
+            saturated[f"bn_apply_{k}"] = saturated.get(f"bn_apply_{k}", 0) + sat
+            ck8.exact(f"bn_apply_{k}", q(k, s), want)
+        # conv5 (2x2 VALID over e4m3 a4b) -> bf16
+        r = S.conv5_stage(val("conv4_2", s), Wq["conv5"], P["conv5/biases"])
+        ckb.close("conv5", G["conv5"][s][:, :T], r["out"], r["acc"])
+        del r, x, want
+    # the f64 statistics against fp64 sums of the GPU's own bf16 pre-BN values, and the f32 coefficients against the fp64
+    # finalize of the workspace's own sums
+    stats = raw["stats"]
+    for l, k in enumerate(("conv4_1", "conv4_2")):
+        gamma, beta = P[f"{k}/{k}/gamma"], P[f"{k}/{k}/beta"]
+        st = S.bn_stats_stage(None, gamma, beta, B.EPS, parts=bnp[l])
+        ckb.close(f"{k}_stats", stats[l, 0], st["sum"], st["sum_acc"], key="bn_sums")
+        ckb.close(f"{k}_stats_sq", stats[l, 1], st["sumsq"], st["sumsq"], key="bn_sums")
+        st = S.bn_stats_stage(None, gamma, beta, B.EPS, sums=(stats[l, 0], stats[l, 1]), parts=bnp[l])
+        for j, c in enumerate(("scale", "shift", "mean", "invstd")):
+            ckb.close(f"{k}_bn_{c}", bn[l, j], st[c], st["acc"][c], key="bn_coef")
+    tail_checks(ckb, P, G, logits, tsl, T, parts(img))
+    if peak:
+        ckb._record("peak_gpu_memory", torch.cuda.max_memory_allocated() / PEAK_LIMIT,
+                    max_memory_allocated=torch.cuda.max_memory_allocated())
+    fail = []
+    for c in (ck8, ckb):
+        c.report()
+        fail += c.fail
+    assert not fail, "\n".join(fail)
+    bits = dict(logits=logits, **{k: raw[k] for k in FP8_ACTS}, **{k: G[k] for k in ("a4a_pre", "a4b_pre")})
+    return saturated, bits
 
 
 @pytest.mark.parametrize("N,W,widths", SHAPES)
@@ -199,13 +282,13 @@ def test_fp8_stages_per_element(N, W, widths, request):
 def test_fp8_stages_saturate_exactly():
     """Scales 8x below the calibrated ones: every e4m3 producer (conv2, conv3_1, conv3_2, both BatchNorm applies) has elements
     past the range, each stored as exactly 448, and the rest still within the stage bounds."""
-    saturated = _stage_checks("N3_W160_saturating", 3, 160, [160, 8, 97], shrink=8)
+    saturated, _ = _stage_checks("N3_W160_saturating", 3, 160, [160, 8, 97], shrink=8)
     assert all(v > 0 for v in saturated.values()), saturated
 
 
 def test_fp8_stages_per_element_c3():
-    """C3: batch 1024 x 32x256, the per-image stages on a sample of images, conv4_x and the BatchNorm applies on the batch."""
-    _stage_checks("C3_N1024_W256", 1024, 256, None, sample=[0, 1, 255, 256, 511, 1023])
+    """C3: batch 1024 x 32x256, the per-image stages on a sample of images, conv4_x and the BatchNorms on the batch."""
+    _stage_checks("C3_N1024_W256", 1024, 256, None, sample=[0, 1, 255, 256, 511, 1023], chunk=128)
 
 
 # ------------------------------------------------------------------------------------------------ 2. whole chain vs fp64
@@ -290,6 +373,12 @@ def test_fp8_chain_at_benchmark_configurations(N, W):
 
 
 # ------------------------------------------------------------------------------------------------ 3. packed evaluation
+# |packed - line alone| / max|line alone logit| over the 67 lines, in batches of 1 and of 64, on an H100 80GB HBM3: 0 -- every
+# line bit-identical in both batchings, as on the bf16 path -- so the bound is exact equality
+MEASURED_PACKED = 0.0
+PACKED_BOUND = 4.5 * MEASURED_PACKED
+
+
 def test_fp8_packed_equals_line_alone(monkeypatch):
     from lstm_ctc_ocr_b200 import engine
     from lstm_ctc_ocr_b200.lib.lstm.test import pack_lines
@@ -315,6 +404,7 @@ def test_fp8_packed_equals_line_alone(monkeypatch):
     for d, t in lines:
         alone.append(m.forward(_t(np.ascontiguousarray(d)), _t(np.asarray(t, np.int32)))[:, 0])
     for group in (1, 64):
+        identical, worst = 0, 0.0
         for g0 in range(0, len(lines), group):
             idx = list(range(g0, min(g0 + group, len(lines))))
             data, lw, tsl = pack_lines([lines[i] for i in idx])
@@ -323,11 +413,15 @@ def test_fp8_packed_equals_line_alone(monkeypatch):
             for r, i in enumerate(idx):
                 t = int(tsl[r])
                 a, p = alone[i][:t], logits[:t, r]
-                # bit-identical except where the order of the f64 BatchNorm atomics differs (as the bf16 packed test allows)
-                assert torch.equal(a, p) or float((a - p).abs().max() / a.abs().max()) < 1e-5, (group, i)
+                if torch.equal(a, p):
+                    identical += 1
+                else:
+                    worst = max(worst, float((a - p).abs().max() / a.abs().max().clamp_min(1e-30)))
                 t1 = _t(np.asarray([t], np.int32))
                 ag, agl = engine.ctc_greedy(a[:, None].contiguous(), t1)
                 assert go[r, :gl[r]].tolist() == ag[0, :agl[0]].tolist(), (group, i)
+        _report("fp8_packed_equals_line_alone", group=group, lines=len(lines), bit_identical=identical, worst_rel=worst)
+        assert worst <= PACKED_BOUND, (group, identical, worst)
 
 
 # ------------------------------------------------------------------------------------------------ 4. contract

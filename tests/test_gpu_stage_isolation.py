@@ -131,10 +131,27 @@ class _Refs:
         return torch.arange(self.H2, device=self.dev)[None, :] < self.L[s][:, None]
 
 
-def _forward_checks(ck, F_, train=True):
+def _global_parts(p, v, world):
+    """One rank's BatchNorm parts p (bn_sums() over its images) plus the other ranks' f64 sums v = [sum x | sum x^2]: the
+    parts of the global batch of `world` equal shards.  The injected sums are operands, so their share of the error scale
+    is their magnitude."""
+    v = v.to(p["sum"].device)
+    return dict(sum=p["sum"] + v[:512], sumsq=p["sumsq"] + v[512:], sum_acc=p["sum_acc"] + v[:512].abs(), cnt=p["cnt"] * world)
+
+
+def _global_bwd_sums(s, v):
+    """One rank's BatchNorm backward sums s (bn_bwd_sums() over its images) plus the other ranks' f64 [sum dy | sum dy*xhat]."""
+    v = v.to(s["dbeta"].device)
+    return dict(dbeta=s["dbeta"] + v[:512], dgamma=s["dgamma"] + v[512:], dbeta_acc=s["dbeta_acc"] + v[:512].abs(),
+                dgamma_acc=s["dgamma_acc"] + v[512:].abs())
+
+
+def _forward_checks(ck, F_, train=True, inject=None):
     """Every forward stage on its own inputs, image chunk by image chunk; the BatchNorm sums and coefficients from the sums
     over all chunks.  train: also the arg-max bytes and the isolated recurrence steps on the saved gates / cell state.
-    Returns the BatchNorm partial sums of both layers' pre-activations."""
+    inject: data parallelism emulated on one device, dict(world=w, fwd=[v41, v42], bwd=[v42, v41]) with the f64 sums the
+    other ranks contributed to each exchange; the "stats" tap then holds the global sums and the coefficients are those of
+    the global batch.  Returns this rank's BatchNorm partial sums of both layers' pre-activations."""
     P, Wb, T, dev = F_.P, F_.Wb, F_.T, F_.dev
     g, R = F_.g, F_.R
     bn = R["bn"].double()
@@ -189,7 +206,8 @@ def _forward_checks(ck, F_, train=True):
         ck.exact("logits_past_len_bias", lg[past], P["logits/biases"].float())
     stats = R["stats"]
     for li, name in enumerate(("conv4_1", "conv4_2")):
-        st = S.bn_stats_stage(None, P[f"{name}/{name}/gamma"], P[f"{name}/{name}/beta"], EPS, parts=bnp[li])
+        p = bnp[li] if inject is None else _global_parts(bnp[li], inject["fwd"][li], inject["world"])
+        st = S.bn_stats_stage(None, P[f"{name}/{name}/gamma"], P[f"{name}/{name}/beta"], EPS, parts=p)
         ck.close(f"{name}_stats", stats[li, 0], st["sum"], st["sum_acc"], key="bn_sums")
         ck.close(f"{name}_stats_sq", stats[li, 1], st["sumsq"], st["sumsq"], key="bn_sums")
         for j, k in enumerate(("scale", "shift", "mean", "invstd")):        # f32 roundings of f64 values of those sums
@@ -197,13 +215,19 @@ def _forward_checks(ck, F_, train=True):
     return bnp
 
 
-def _backward_checks(ck, F_, grad, dlogits, bnp):
+def _backward_checks(ck, F_, grad, dlogits, bnp, inject=None):
     """Every backward stage on its own inputs, image chunk by image chunk, and the 24 gradient tensors from the reference
     sums over all chunks.  The BatchNorm backwards need batch sums of their own input gradient first, so the chunks are
-    walked three times: up to d_a4b (+ BN4_2's sums), d_pre4b (+ BN4_1's sums), the rest."""
+    walked three times: up to d_a4b (+ BN4_2's sums), d_pre4b (+ BN4_1's sums), the rest.  inject (see _forward_checks):
+    the statistics and the data gradients of both BatchNorms are the global batch's, gamma / beta gradients this rank's
+    own sums (the flat gradient buffer is summed over ranks afterwards).  Returns this rank's BatchNorm backward sums of
+    conv4_2 and conv4_1."""
     P, Wb, T, H2 = F_.P, F_.Wb, F_.T, F_.H2
     g, R = F_.g, F_.R
     bn = R["bn"].double()
+    if inject is not None:
+        bnp = [_global_parts(p, v, inject["world"]) for p, v in zip(bnp, inject["fwd"])]
+    glob = (lambda s, i: s) if inject is None else (lambda s, i: _global_bwd_sums(s, inject["bwd"][i]))
     st = [S.bn_batch(None, EPS, parts=p) for p in bnp]
     tot, s42, s41 = {}, {}, {}
     for s in F_.parts:
@@ -235,7 +259,7 @@ def _backward_checks(ck, F_, grad, dlogits, bnp):
     w42 = Wb["conv4_2/weights"]
     for s in F_.parts:
         r = S.bn_relu_pool_bwd_stage(g("d_a4b", s), g("a4b_pre", s), bn[1], P["conv4_2/conv4_2/gamma"], EPS, stats=st[1],
-                                     sums=s42)
+                                     sums=glob(s42, 0))
         ck.close("d_pre4b", g("d_pre4b", s), r["dx"], r["dx_acc"])
         r = S.conv_bwd(g("d_pre4b", s), g("conv4_1", s), w42)
         _sum_into(tot, {"conv4_2/weights": r["dw"], "conv4_2/weights_acc": r["dw_acc"]})
@@ -245,7 +269,7 @@ def _backward_checks(ck, F_, grad, dlogits, bnp):
     ck.close("conv4_1/beta", grad["conv4_1/conv4_1/beta"], s41["dbeta"], s41["dbeta_acc"], key="bn41_affine")
     for s in F_.parts:
         r = S.conv_bn_relu_bwd_stage(g("d_pre4b", s), g("a4a_pre", s), bn[0], P["conv4_1/conv4_1/gamma"], w42, EPS,
-                                     stats=st[0], sums=s41)
+                                     stats=st[0], sums=glob(s41, 1))
         ck.close("d_pre4a", g("d_pre4a", s), r["dx"], r["dx_acc"])
         r = S.conv_bwd(g("d_pre4a", s), g("conv3_2", s), Wb["conv4_1/weights"])
         _sum_into(tot, {"conv4_1/weights": r["dw"], "conv4_1/weights_acc": r["dw_acc"]})
@@ -273,6 +297,7 @@ def _backward_checks(ck, F_, grad, dlogits, bnp):
         ck.close(k, grad[k], tot[k], tot[k + "_acc"], key=f"wgrad/{k}" if f"wgrad/{k}" in ck.bounds else "wgrad")
     ck.exact("conv4_2/biases_zero", grad["conv4_2/biases"], 0.0)
     ck.exact("conv4_1/biases_zero", grad["conv4_1/biases"], 0.0)
+    return s42, s41
 
 
 def _run_stage_checks(case, N, W, widths, dev="cpu", chunk=None, ctc=None, ck=None, max_label=4):

@@ -445,6 +445,62 @@ def _check_chunked_references(c):
     assert rel(sum(x[0] for x in cs), S.masked_colsum(dy, A["conv3_1"])[0]) < 1e-12
 
 
+@pytest.fixture(scope="module")
+def chain4():
+    return _make_chain(4, 24, [24, 17, 4, 12])
+
+
+@pytest.mark.parametrize("world", [2, 4])
+def test_sharded_references_with_injected_sums_equal_the_whole_batch(chain4, world):
+    """The data-parallel rule the GPU stage checks use (test_gpu_stage_isolation._global_parts / _global_bwd_sums): each of
+    `world` equal shards, its own BatchNorm sums plus the other shards' f64 sums injected, gives the whole batch's
+    statistics and data gradients, and its gamma / beta gradients from its OWN sums add up over the shards to the whole
+    batch's, all to 1e-12.  Taking gamma / beta from the global sums instead counts them `world` times."""
+    import test_gpu_stage_isolation as B
+    c = chain4
+    r = _forward_chain(c)
+    P, eps, N = c["P"], O.BN_EPS, c["N"]
+    n = N // world
+    shards = [slice(k * n, (k + 1) * n) for k in range(world)]
+    others = lambda vs, k: sum(v for q, v in enumerate(vs) if q != k)
+    gen = torch.Generator().manual_seed(3)
+    w42 = P["conv4_2/weights"]
+    for name in ("conv4_2", "conv4_1"):
+        pre, bn = r[name]["pre"], r[name]["bn"]
+        gamma, beta = P[f"{name}/{name}/gamma"], P[f"{name}/{name}/beta"]
+        local = [S.bn_sums(pre[s]) for s in shards]
+        fwd = [torch.cat([p["sum"], p["sumsq"]]) for p in local]
+        whole_st = S.bn_stats_stage(pre, gamma, beta, eps)
+        parts = [B._global_parts(local[k], others(fwd, k), world) for k in range(world)]
+        for p in parts:
+            st = S.bn_stats_stage(None, gamma, beta, eps, parts=p)
+            for k in ("sum", "sumsq", "mean", "invstd", "scale", "shift"):
+                assert rel(st[k], whole_st[k]) < 1e-12, (name, k)
+        stats = S.bn_batch(pre, eps)
+        if name == "conv4_2":
+            d = torch.randn(pre.shape[:2] + (2, pre.shape[3]), dtype=torch.float64, generator=gen)
+            stage = lambda s, **kw: S.bn_relu_pool_bwd_stage(d[s], pre[s], bn, gamma, eps, rnd=S.ident, **kw)
+            dys = [S.bn_relu_pool_route(d[s], pre[s], bn, rnd=S.ident) for s in shards]
+            dys = [(x, x.abs()) for x in dys]
+        else:
+            d = torch.randn(pre.shape, dtype=torch.float64, generator=gen)
+            stage = lambda s, **kw: S.conv_bn_relu_bwd_stage(d[s], pre[s], bn, gamma, w42, eps, rnd=S.ident, **kw)
+            dys = [S.conv_relu_dgrad(d[s], pre[s], bn, w42, rnd=S.ident) for s in shards]
+        whole = stage(slice(None))
+        st_k = [S.bn_batch(None, eps, parts=p) for p in parts]
+        for k in range(world):
+            assert rel(st_k[k]["mean"], stats["mean"]) < 1e-12 and rel(st_k[k]["invstd"], stats["invstd"]) < 1e-12
+        ls = [S.bn_bwd_sums(dys[k][0], dys[k][1], pre[shards[k]], st_k[k]) for k in range(world)]
+        bwd = [torch.cat([x["dbeta"], x["dgamma"]]) for x in ls]
+        got = [stage(shards[k], stats=st_k[k], sums=B._global_bwd_sums(ls[k], others(bwd, k))) for k in range(world)]
+        assert rel(torch.cat([x["dx"] for x in got]), whole["dx"]) < 1e-12, name
+        for k in ("dgamma", "dbeta"):
+            assert rel(sum(x[k] for x in ls), whole[k]) < 1e-12, (name, k)
+            # the global sums in every shard's gamma / beta gradient: `world` times the whole batch's after the SUM
+            assert rel(sum(x[k] for x in got), whole[k]) > 0.5, (name, k)
+            assert rel(sum(x[k] for x in got), world * whole[k]) < 1e-12, (name, k)
+
+
 def test_checker_rows_from_torch_equal_numpy():
     """Checker.close / close_scaled / exact give the same row from torch tensors as from numpy arrays, and a stage checked
     in image chunks merges into one row with the worst element, the maxima and the L2 of the whole."""

@@ -31,12 +31,10 @@ extern "C" int crnn_model_set_training(crnn_model* m, int flag) {
     CRNN_TRY(make_tmap_2d(&m->tD_c41, m->Bd_c41, 256, 4608, 4608, 256));
     CRNN_TRY(make_tmap_2d(&m->tD_c32, m->Bd_c32, 256, 2304, 2304, 256));
     CRNN_TRY(make_tmap_2d(&m->tD_c31, m->Bd_c31, 128, 2304, 2304, 128));
-    CRNN_TRY(make_tmap_2d(&m->tD_c2, m->Bd_c2, 64, 1152, 1152, 64));
     CRNN_TRY(make_tmap_2d(&m->tDs_c2, m->Bd_c2, 64, 1152, 1152, 128));
     CRNN_TRY(make_tmap_2d(&m->tD_c5, m->Bd_c5, 1024, 1024, 1024, 256));
     CRNN_TRY(make_tmap_2d(&m->tD_l, m->Bld, 512, 64, 64, 256));
     CRNN_TRY(make_tmap_2d(&m->tD_x, m->Bxb, 512, 2048, 2048, 256));
-    CRNN_TRY(make_tmap_2d(&m->tD_h, m->Bhb, 512, 1024, 1024, 32));
     CRNN_TRY(make_tmap_2d(&m->tD_h256, m->Bhb, 512, 1024, 1024, 256));
     m->dirty_bwd = true;
   }
@@ -53,7 +51,7 @@ static int prepare_weights_bwd(crnn_model* m, cudaStream_t st) {
   CRNN_TRY(launch_conv5_dgrad_weight(m->P("conv5/weights"), m->Bd_c5, st));
   CRNN_TRY(launch_cast_bf16(m->P("logits/weights"), m->Bld, 512 * 64, st));
   CRNN_TRY(launch_lstm_bwd_weight(m->P("logits/bidirectional_rnn/fw/lstm_cell/weights"), m->P("logits/bidirectional_rnn/bw/lstm_cell/weights"),
-                                  m->Bxb, m->Bhb, 32, st));
+                                  m->Bxb, m->Bhb, st));
   m->dirty_bwd = false;
   return CRNN_OK;
 }
@@ -130,33 +128,31 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
   // ------------------------------------------------------------------ BPTT through both directions
   {
     lstm_bwd::Params lp;
-    lp.gates = pl.gates; lp.csave = pl.csave; lp.d_out = pl.d_lstm_out; lp.dz_state = pl.dz_state; lp.dz_all = pl.dz_all;
+    lp.gates = pl.gates; lp.csave = pl.csave; lp.d_out = pl.d_lstm_out; lp.dz_all = pl.dz_all;
     lp.seq_len = time_step_len; lp.Nimg = N; lp.Npad = pl.Npad; lp.H = H2; lp.T = T; lp.tiles_per_dir = pl.Npad / 128;
     static bool attr = false;
     if (!attr) {
-      CUDA_TRY(cudaFuncSetAttribute(lstm_bwd::lstm_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lstm_bwd::SMEM_BYTES));
       CUDA_TRY(cudaFuncSetAttribute(lstm_bwd::lstm_bwd_ks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lstm_bwd::ks::SMEM_BYTES));
       attr = true;
     }
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(lstm_bwd::CS * 2 * lp.tiles_per_dir);
-    cfg.blockDim = dim3(m->bptt_ks ? lstm_bwd::ks::NUM_THREADS : lstm_bwd::NUM_THREADS);
-    cfg.dynamicSmemBytes = m->bptt_ks ? lstm_bwd::ks::SMEM_BYTES : lstm_bwd::SMEM_BYTES;
+    cfg.blockDim = dim3(lstm_bwd::ks::NUM_THREADS);
+    cfg.dynamicSmemBytes = lstm_bwd::ks::SMEM_BYTES;
     cfg.stream = st;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeClusterDimension;
     at[0].val.clusterDim.x = lstm_bwd::CS; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
-    if (m->bptt_ks) CUDA_TRY(cudaLaunchKernelEx(&cfg, lstm_bwd::lstm_bwd_ks_kernel, m->tD_h256, lp, pl.bptt_x));
-    else CUDA_TRY(cudaLaunchKernelEx(&cfg, lstm_bwd::lstm_bwd_kernel, pl.tG_dzstate, m->tD_h, lp));
+    CUDA_TRY(cudaLaunchKernelEx(&cfg, lstm_bwd::lstm_bwd_ks_kernel, m->tD_h256, lp, pl.bptt_x));
   }
   BMARK();
   {
     const std::string fw = "logits/bidirectional_rnn/fw/lstm_cell", bw = "logits/bidirectional_rnn/bw/lstm_cell";
     const long long dW = m->find(bw + "/weights")->offset - m->find(fw + "/weights")->offset;
     const long long db = m->find(bw + "/biases")->offset - m->find(fw + "/biases")->offset;
-    CRNN_TRY(launch_colsum_bf16(pl.dz_all, R, 2048, G(fw + "/biases"), 32, db, st));
+    CRNN_TRY(launch_colsum_bf16(pl.dz_all, R, 2048, G(fw + "/biases"), true, db, st));
     {  // dW_x (rows 0..511 of both [768,1024] matrices) = a5^T dz
       gemm_tn::Params p = tn_plain(512, 2048, R, G(fw + "/weights"), 1024);
       p.num_n_tiles = 8; p.lstm_cols = 1; p.dir_stride = dW;
@@ -187,7 +183,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
   }
   BMARK();
   // ------------------------------------------------------------------ conv5 (2x2 VALID)
-  CRNN_TRY(launch_colsum_bf16(pl.d_a5, R, 512, G("conv5/biases"), 0, 0, st));
+  CRNN_TRY(launch_colsum_bf16(pl.d_a5, R, 512, G("conv5/biases"), false, 0, st));
   for (int r = 0; r < 2; ++r) {
     gemm_tn::Params p = tn_plain(1024, 512, R, G("conv5/weights") + (size_t)r * 1024 * 512, 512);
     p.num_n_tiles = 2; p.a_row_shift = r;
@@ -211,7 +207,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
   double* sums41 = pl.bn_bwd_sums;
   double* gsum42 = m->dp_world > 1 ? pl.bn_bwd_sums + 3072 : sums42;
   double* gsum41 = m->dp_world > 1 ? pl.bn_bwd_sums + 2048 : sums41;
-  CRNN_TRY(launch_bn_bwd_reduce(true, pl.d_a4b, pl.a4b_pre, pl.bn + 2048, sums42, P4 / 2, 512, st));
+  CRNN_TRY(launch_bn_bwd_reduce(pl.d_a4b, pl.a4b_pre, pl.bn + 2048, sums42, P4 / 2, 512, st));
   if (m->dp_world > 1) CRNN_TRY(dp_allreduce_1024(m, sums42, gsum42, st));
   CRNN_TRY(launch_bn_bwd_apply(true, pl.d_a4b, pl.a4b_pre, pl.d_pre4b, pl.bn + 2048, m->P("conv4_2/conv4_2/gamma"), gsum42, sums42, P4g,
                                P4 / 2, 512, pl.bn_bwd_coef, G("conv4_2/conv4_2/gamma"), G("conv4_2/conv4_2/beta"), st));
@@ -230,15 +226,10 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
     // 268 MB gradient + 268 MB pre-BN activation
     gemm::Params p = conv_params(N, H2, 4, 512, 512, 256, nullptr, pl.d_pre4a, pl.mg4);
     p.mask = pl.a4a_pre; p.bnp = pl.bn; p.stats = sums41;
-    if (m->bn_red_fused) {
-      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE_BNRED, 4>(pl.tG_p4b, m->tD_c42, p, sms, st)));
-    } else {
-      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE, 4>(pl.tG_p4b, m->tD_c42, p, sms, st, &pl.tG_p4a)));
-    }
+    CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE_BNRED, 4>(pl.tG_p4b, m->tD_c42, p, sms, st)));
   }
   BMARK();
   // ------------------------------------------------------------------ conv4_1: ReLU + BN backward
-  if (!m->bn_red_fused) CRNN_TRY(launch_bn_bwd_reduce(false, pl.d_pre4a, pl.a4a_pre, pl.bn, sums41, P4, 512, st));
   if (m->dp_world > 1) CRNN_TRY(dp_allreduce_1024(m, sums41, gsum41, st));
   CRNN_TRY(launch_bn_bwd_apply(false, pl.d_pre4a, pl.a4a_pre, pl.d_pre4a, pl.bn, m->P("conv4_1/conv4_1/gamma"), gsum41, sums41, P4g, P4, 512,
                                pl.bn_bwd_coef, G("conv4_1/conv4_1/gamma"), G("conv4_1/conv4_1/beta"), st));
@@ -272,16 +263,11 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
     // conv3_1's ReLU backward rides in this epilogue (zero where a3 == 0): saves one read + one write of the 268 MB gradient
     gemm::Params p = conv_params(N, H2, 8, 256, 256, 256, nullptr, pl.d_pre31, pl.mg3);
     p.mask = pl.a3;
-    if (m->relu_mask_fused) {
-      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE_MASK, 4>(pl.tG_p32, m->tD_c32, p, sms, st)));
-    } else {
-      CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE, 4>(pl.tG_p32, m->tD_c32, p, sms, st, &pl.tG_p31)));
-    }
+    CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_CONV_STORE_MASK, 4>(pl.tG_p32, m->tD_c32, p, sms, st)));
   }
   BMARK();
-  // ------------------------------------------------------------------ conv3_1: ReLU backward (unless fused above), bias gradient
-  if (!m->relu_mask_fused) CRNN_TRY(launch_relu_bwd(pl.d_pre31, pl.a3, (size_t)N * H2 * 8 * 256, st));
-  CRNN_TRY(launch_colsum_bf16(pl.d_pre31, (long long)N * H2 * 8, 256, G("conv3_1/biases"), 0, 0, st));
+  // ------------------------------------------------------------------ conv3_1: bias gradient (its ReLU backward is fused above)
+  CRNN_TRY(launch_colsum_bf16(pl.d_pre31, (long long)N * H2 * 8, 256, G("conv3_1/biases"), false, 0, st));
   BMARK();
   {
     gemm_tn::Params p = tn_conv(N, H2, 8, 128, 256, G("conv3_1/weights"), pl.wm3);
@@ -290,49 +276,36 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
   }
   notify("conv3_1/weights", "conv3_2/weights");
   BMARK();
-  if (m->conv2_dgrad_swap) {
+  {
     // conv3_1's data gradient has 128 output channels: position-major it is an N = 128 tile (half the MMA rate); swapped, the 128
     // channels fill the M side and N is 256 positions (32 H rows x 8)
     convsw::DgradParams p;
     p.Nimg = N; p.H = H2; p.tiles_per_img = (H2 + 31) / 32; p.out = pl.d_a2;
     CRNN_TRY((launch_conv_dgrad_swap<8, 4, 128>(pl.tG_p31s, m->tD_c31, p, sms, st)));
-  } else {
-    gemm::Params p = conv_params(N, H2, 8, 256, 128, 128, nullptr, pl.d_a2, pl.mg3);
-    CRNN_TRY((launch_gemm<128, gemm::A_CONV3, gemm::EPI_CONV_STORE, 6>(pl.tG_p31, m->tD_c31, p, sms, st)));
   }
   BMARK();
   // ------------------------------------------------------------------ conv2: 2x2 pool + ReLU backward
   CRNN_TRY(launch_unpool_relu_bwd(4, pl.d_a2, pl.a2, pl.am2, pl.d_pre2, (size_t)N * H2 * 8, H2, 8, 128, st));
   CRNN_TRY(launch_colsum_masked_bf16(pl.d_a2, pl.a2, (long long)N * H2 * 8, 128, G("conv2/biases"), st));
   BMARK();
-  if (m->conv2_wgrad_swap) {
+  {
     // operands swapped: A = d(pre-activation) [positions x 128 co] on the M side, B = a1 with FOUR tap-shifted 64-channel boxes
     // per 256-column N tile (columns = (tap, ci)); 3 N tiles cover the 9 taps.  N = 256 runs the MMA at full rate where the
     // Cout = 128 N tile of the straight formulation halves it.
     gemm_tn::Params p = tn_conv(N, H1, 16, 64, 128, G("conv2/weights"), pl.wm2);
     p.tap_pack_n = 1; p.num_taps = 1; p.num_m_tiles = 1; p.num_n_tiles = 3; p.M = 128; p.N = 9 * 64; p.ldo = 128; p.tap_stride = 0;
     CRNN_TRY((launch_gemm_tn<256, gemm_tn::TN_CONV, 4>(pl.tW_p2, pl.tW_a1, p, sms, st)));
-  } else {
-    gemm_tn::Params p = tn_conv(N, H1, 16, 64, 128, G("conv2/weights"), pl.wm2);
-    p.num_n_tiles = 1;
-    // Cin = 64 fills only half of a 128-row MMA tile: view dW [9*64, 128] as ONE matrix and let each tile hold two taps
-    p.tap_pack = 1; p.num_taps = 1; p.num_m_tiles = 5; p.M = 9 * 64; p.tap_stride = 0;
-    CRNN_TRY((launch_gemm_tn<128, gemm_tn::TN_CONV, 6>(pl.tW_a1, pl.tW_p2, p, sms, st)));
   }
   BMARK();
-  if (m->conv2_dgrad_swap) {
+  {
     convsw::DgradParams p;
     p.Nimg = N; p.H = H1; p.tiles_per_img = (H1 + 15) / 16; p.out = pl.d_a1;
     CRNN_TRY((launch_conv_dgrad_swap<16, 2, 64>(pl.tG_p2s, m->tDs_c2, p, sms, st)));
-  } else {
-    gemm::Params p = conv_params(N, H1, 16, 128, 64, 64, nullptr, pl.d_a1, pl.mg2);
-    CRNN_TRY((launch_gemm<64, gemm::A_CONV3, gemm::EPI_CONV_STORE, 8>(pl.tG_p2, m->tD_c2, p, sms, st)));
   }
   BMARK();
   // ------------------------------------------------------------------ conv1 (Cin = 1): pool1 + ReLU backward folded in; tensor-core
-  // kernel with thread-built operands (conv1_wgrad_tc.cuh), CRNN_CONV1_WGRAD=simt -> the FMA kernel of backward_kernels.cu
-  if (m->conv1_wgrad_tc) CRNN_TRY(launch_conv1_wgrad_tc(pl.d_a1, pl.a1, pl.am1, data, G("conv1/weights"), G("conv1/biases"), N, W, sms, st));
-  else CRNN_TRY(launch_conv1_wgrad(pl.d_a1, pl.a1, pl.am1, data, G("conv1/weights"), G("conv1/biases"), N, W, st));
+  // kernel with thread-built operands (conv1_wgrad_tc.cuh)
+  CRNN_TRY(launch_conv1_wgrad_tc(pl.d_a1, pl.a1, pl.am1, data, G("conv1/weights"), G("conv1/biases"), N, W, sms, st));
   notify("conv1/weights", "conv3_1/weights");
   BMARK();
 #undef BMARK

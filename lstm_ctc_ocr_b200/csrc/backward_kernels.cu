@@ -113,7 +113,8 @@ __global__ void __launch_bounds__(256) colsum_bf16_kernel(const __nv_bfloat16* _
 // pass 2 re-derives it from the same two inputs, which saves one 268 MB write + one 268 MB read per BN layer):
 //   dy = routed upstream gradient at the pre-BN resolution, masked by ReLU;  sums[c] += dy, sums[C + c] += dy * xhat
 // POOL = true (conv4_2 / pool3): dout is [P, Wp/2.., C] pooled; x_pre is [P*2 positions..]; the max is re-derived from
-// the saved pre-BN tensor (first position wins ties).  POOL = false (conv4_1): dout has the same shape as x_pre.
+// the saved pre-BN tensor (first position wins ties).  POOL = false: dout has the same shape as x_pre (not launched: conv4_1's
+// sums ride in conv4_2's data-gradient epilogue, gemm.cuh EPI_CONV_STORE_BNRED).
 template <bool POOL>
 __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const uint4* __restrict__ dout, const uint4* __restrict__ x_pre,
                                                             uint4* __restrict__ dy, const float* __restrict__ bn /*scale,shift,mean,invstd*/,
@@ -262,18 +263,6 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const uint4* dout, co
   }
 }
 
-// ---- ReLU backward in place: d *= (a > 0)       (conv3_1)
-__global__ void __launch_bounds__(256) relu_bwd_kernel(uint4* __restrict__ d, const uint4* __restrict__ a, size_t nvec) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= nvec) return;
-  float g[8], y[8];
-  unpack8(d[i], g);
-  unpack8(__ldg(a + i), y);
-#pragma unroll
-  for (int k = 0; k < 8; ++k) g[k] = (y[k] > 0.f) ? g[k] : 0.f;
-  d[i] = pack8(g);
-}
-
 // ---- un-pool + ReLU backward.  WIN = 2 (1x2 over the Wd axis, conv3_2) or 4 (2x2, conv2).
 // dpool/pooled/argmax: [Npos_out..., C]; dpre: pre-pool resolution.  Geometry: pooled [N, Hp, Wp, C];
 // pre-pool [N, Hp*(WIN==4?2:1), Wp*2, C].
@@ -308,143 +297,6 @@ __global__ void __launch_bounds__(256) unpool_relu_bwd_kernel(const uint4* __res
   }
 }
 
-// ---- conv1 weight/bias gradient (Cin = 1, K = 9: SIMT), pool1 + ReLU backward folded in.
-// d_a1 [N,H1,16,64] pooled gradient, a1 pooled activation (ReLU mask), am1 window index (0..3 = dy*2+dx); data [N,W,32].
-//   dW1[r][s][co] += data[2ho+dy+r-1][2wo+dx+s-1] * g     db1[co] += g        (g = d_a1 where a1 > 0)
-// Same tiling as the forward conv1 kernel: tile = one image x 8 pooled rows x 16 pooled cols, input tile in shared memory,
-// thread = 8 channels x 4 pooled positions.  The window index differs per channel, so instead of indexing the patch
-// dynamically every window position k gets the masked gradient (g if idx == k else 0): 36 FMAs per channel, no branches.
-constexpr int C1W_ROWS = 8;
-__global__ void __launch_bounds__(256) conv1_wgrad_kernel(const __nv_bfloat16* __restrict__ d_a1, const __nv_bfloat16* __restrict__ a1,
-                                                          const uint8_t* __restrict__ am1, const float* __restrict__ data,
-                                                          float* __restrict__ dW, float* __restrict__ db, int N, int W) {
-  __shared__ float s_in[2 * C1W_ROWS + 2][36];
-  __shared__ float s_red[8][8][80];
-  const int H1 = W >> 1;
-  const int tiles_per_img = (H1 + C1W_ROWS - 1) / C1W_ROWS;
-  const int num_tiles = N * tiles_per_img;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int cg = lane & 7;
-  const int slot = warp * 4 + (lane >> 3);
-  // accumulators as f32x2 pairs of adjacent channels: the 288 FMAs per pooled position issue as 144 FFMA2 (the 3-register scalar
-  // FFMA issues every other cycle per scheduler -- the same ceiling the SIMT forward conv1 hits)
-  uint64_t acc2[9][4];
-  float accb[8];
-#pragma unroll
-  for (int k = 0; k < 9; ++k)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc2[k][j] = 0ull;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) accb[j] = 0.f;
-
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-    const int n = tile / tiles_per_img;
-    const int ho0 = (tile - n * tiles_per_img) * C1W_ROWS;
-    __syncthreads();
-    for (int i = threadIdx.x; i < (2 * C1W_ROWS + 2) * 34; i += 256) {
-      const int r = i / 34, c = i - r * 34;
-      const int gr = 2 * ho0 - 1 + r, gc = c - 1;
-      s_in[r][c] = (gr >= 0 && gr < W && gc >= 0 && gc < 32) ? __ldg(data + ((size_t)n * W + gr) * 32 + gc) : 0.f;
-    }
-    // this thread's 4 pooled positions: gradient, activation and window index for 8 channels each (loads issued together)
-    uint4 gq[4], yq[4];
-    uint2 iq[4];
-#pragma unroll
-    for (int pp = 0; pp < 4; ++pp) {
-      const int pidx = slot + 32 * pp;
-      const int hol = pidx >> 4, wo = pidx & 15;
-      const int ho = ho0 + hol;
-      if (ho < H1) {
-        const size_t oo = (((size_t)n * H1 + ho) * 16 + wo) * 64 + cg * 8;
-        gq[pp] = __ldg(reinterpret_cast<const uint4*>(d_a1 + oo));
-        yq[pp] = __ldg(reinterpret_cast<const uint4*>(a1 + oo));
-        iq[pp] = __ldg(reinterpret_cast<const uint2*>(am1 + oo));
-      } else {
-        gq[pp] = make_uint4(0u, 0u, 0u, 0u); yq[pp] = gq[pp]; iq[pp] = make_uint2(0u, 0u);
-      }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int pp = 0; pp < 4; ++pp) {
-      const int pidx = slot + 32 * pp;
-      const int hol = pidx >> 4, wo = pidx & 15;
-      float g[8], y[8];
-      unpack8(gq[pp], g);
-      unpack8(yq[pp], y);
-      const uint32_t idx[8] = {iq[pp].x & 255u, (iq[pp].x >> 8) & 255u, (iq[pp].x >> 16) & 255u, iq[pp].x >> 24,
-                               iq[pp].y & 255u, (iq[pp].y >> 8) & 255u, (iq[pp].y >> 16) & 255u, iq[pp].y >> 24};
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { g[j] = (y[j] > 0.f) ? g[j] : 0.f; accb[j] += g[j]; }
-      float patch[4][4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 p0 = *reinterpret_cast<const float2*>(&s_in[2 * hol + i][2 * wo]);
-        const float2 p1 = *reinterpret_cast<const float2*>(&s_in[2 * hol + i][2 * wo + 2]);
-        patch[i][0] = p0.x; patch[i][1] = p0.y; patch[i][2] = p1.x; patch[i][3] = p1.y;
-      }
-#pragma unroll
-      for (int dy = 0; dy < 2; ++dy)
-#pragma unroll
-        for (int dx = 0; dx < 2; ++dx) {
-          uint64_t gs2[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            gs2[j] = ptx::pack_f32x2((idx[2 * j] == (uint32_t)(dy * 2 + dx)) ? g[2 * j] : 0.f,
-                                     (idx[2 * j + 1] == (uint32_t)(dy * 2 + dx)) ? g[2 * j + 1] : 0.f);
-#pragma unroll
-          for (int r = 0; r < 3; ++r)
-#pragma unroll
-            for (int s2 = 0; s2 < 3; ++s2) {
-              const float x = patch[dy + r][dx + s2];
-              const uint64_t x2 = ptx::pack_f32x2(x, x);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) acc2[r * 3 + s2][j] = ptx::ffma2(x2, gs2[j], acc2[r * 3 + s2][j]);
-            }
-        }
-    }
-  }
-  // block reduction: lanes sharing a channel group (lane ^ 8, ^ 16), then the 8 warps through shared memory
-  float acc[9][8];
-#pragma unroll
-  for (int k = 0; k < 9; ++k)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) ptx::unpack_f32x2(acc2[k][j], acc[k][2 * j], acc[k][2 * j + 1]);
-#pragma unroll
-  for (int k = 0; k < 9; ++k)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float v = acc[k][j];
-      v += __shfl_xor_sync(0xffffffffu, v, 8);
-      v += __shfl_xor_sync(0xffffffffu, v, 16);
-      acc[k][j] = v;
-    }
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    float v = accb[j];
-    v += __shfl_xor_sync(0xffffffffu, v, 8);
-    v += __shfl_xor_sync(0xffffffffu, v, 16);
-    accb[j] = v;
-  }
-  __syncthreads();
-  if (lane < 8) {
-#pragma unroll
-    for (int k = 0; k < 9; ++k)
-#pragma unroll
-      for (int j = 0; j < 8; ++j) s_red[warp][cg][k * 8 + j] = acc[k][j];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) s_red[warp][cg][72 + j] = accb[j];
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < 8 * 80; i += 256) {
-    const int g8 = i / 80, e = i - g8 * 80;
-    float v = 0.f;
-#pragma unroll
-    for (int w8 = 0; w8 < 8; ++w8) v += s_red[w8][g8][e];
-    if (e < 72) atomicAdd(dW + (e >> 3) * 64 + g8 * 8 + (e & 7), v);
-    else atomicAdd(db + g8 * 8 + (e - 72), v);
-  }
-}
-
 // ---- weight re-layouts for the backward GEMMs (bf16, K-major B operands) ---------------------------------------
 // data-gradient of a 3x3 SAME conv == 3x3 SAME conv of dY with the spatially flipped, in/out-swapped kernel:
 //   Bd[ci][(r',s',co)] = W[2-r'][2-s'][ci][co]       (W is HWIO)
@@ -469,7 +321,7 @@ __global__ void conv5_dgrad_weight_kernel(const float* __restrict__ w, __nv_bflo
     bd[i] = __float2bfloat16_rn(w[((size_t)r * 1024 + wc) * 512 + co]);
   }
 }
-// LSTM: rows of the TF matrix [768,1024] with gate columns permuted (upc), both directions.
+// LSTM: rows of the TF matrix [768,1024] with gate columns permuted (upc = LSTM_GATE_UNITS), both directions.
 //   bxb[x][dir*1024 + p] (x < 512, dx GEMM)      bhb[dir*256 + u][p] (recurrent backward GEMM)
 __global__ void lstm_bwd_weight_kernel(const float* __restrict__ w_fw, const float* __restrict__ w_bw,
                                        __nv_bfloat16* __restrict__ bxb, __nv_bfloat16* __restrict__ bhb, int upc) {
@@ -605,9 +457,9 @@ int launch_dlogits_rows(const float* dlogits, __nv_bfloat16* rows, float* dbias,
   dlogits_rows_kernel<<<4 * device_sms(), 256, 0, st>>>(dlogits, rows, dbias, T, N, H);
   LAUNCH_CHECK();
 }
-int launch_colsum_bf16(const __nv_bfloat16* src, long long R, int C, float* out, int perm_upc, long long dir_stride, cudaStream_t st) {
+int launch_colsum_bf16(const __nv_bfloat16* src, long long R, int C, float* out, bool lstm_gates, long long dir_stride, cudaStream_t st) {
   dim3 grid(2 * device_sms(), (C + 255) / 256);
-  colsum_bf16_kernel<<<grid, 256, 0, st>>>(src, nullptr, R, C, 0, out, perm_upc, dir_stride);
+  colsum_bf16_kernel<<<grid, 256, 0, st>>>(src, nullptr, R, C, 0, out, lstm_gates ? LSTM_GATE_UNITS : 0, dir_stride);
   LAUNCH_CHECK();
 }
 // out[c] += sum over rows of src[r][c] where mask[r][c] > 0.  Narrow tensors (C = 128) are read as a [R/2, 256] view so that
@@ -620,10 +472,9 @@ int launch_colsum_masked_bf16(const __nv_bfloat16* src, const __nv_bfloat16* mas
   colsum_bf16_kernel<<<grid, 256, 0, st>>>(src, mask, Rv, Cv, Cmod, out, 0, 0);
   LAUNCH_CHECK();
 }
-int launch_bn_bwd_reduce(bool pool, const __nv_bfloat16* dout, const __nv_bfloat16* x_pre, const float* bn, double* sums,
-                         size_t out_positions, int C, cudaStream_t st) {
-  if (pool) bn_bwd_reduce_kernel<true><<<4 * device_sms(), 256, 0, st>>>((const uint4*)dout, (const uint4*)x_pre, nullptr, bn, sums, out_positions, C);
-  else bn_bwd_reduce_kernel<false><<<4 * device_sms(), 256, 0, st>>>((const uint4*)dout, (const uint4*)x_pre, nullptr, bn, sums, out_positions, C);
+int launch_bn_bwd_reduce(const __nv_bfloat16* dout, const __nv_bfloat16* x_pre, const float* bn, double* sums, size_t out_positions, int C,
+                         cudaStream_t st) {
+  bn_bwd_reduce_kernel<true><<<4 * device_sms(), 256, 0, st>>>((const uint4*)dout, (const uint4*)x_pre, nullptr, bn, sums, out_positions, C);
   LAUNCH_CHECK();
 }
 // dx = BN/ReLU(/pool) backward of dout; out_positions = positions of dout (pooled positions when pool); dx may alias dout when !pool
@@ -637,23 +488,12 @@ int launch_bn_bwd_apply(bool pool, const __nv_bfloat16* dout, const __nv_bfloat1
   else bn_bwd_apply_kernel<false><<<(unsigned)((nvec + 255) / 256), 256, 0, st>>>((const uint4*)dout, (const uint4*)x_pre, bn, coef, (uint4*)dx, nvec, C);
   LAUNCH_CHECK();
 }
-int launch_relu_bwd(__nv_bfloat16* d, const __nv_bfloat16* a, size_t n, cudaStream_t st) {
-  const size_t nvec = n / 8;
-  relu_bwd_kernel<<<(unsigned)((nvec + 255) / 256), 256, 0, st>>>((uint4*)d, (const uint4*)a, nvec);
-  LAUNCH_CHECK();
-}
 int launch_unpool_relu_bwd(int win, const __nv_bfloat16* dpool, const __nv_bfloat16* pooled, const uint8_t* argmax,
                            __nv_bfloat16* dpre, size_t out_positions, int Hp, int Wp, int C, cudaStream_t st) {
   const size_t nvec = out_positions * C / 8;
   const unsigned grid = (unsigned)((nvec + 255) / 256);
   if (win == 2) unpool_relu_bwd_kernel<2><<<grid, 256, 0, st>>>((const uint4*)dpool, (const uint4*)pooled, (const uint2*)argmax, (uint4*)dpre, nvec, Hp, Wp, C);
   else unpool_relu_bwd_kernel<4><<<grid, 256, 0, st>>>((const uint4*)dpool, (const uint4*)pooled, (const uint2*)argmax, (uint4*)dpre, nvec, Hp, Wp, C);
-  LAUNCH_CHECK();
-}
-int launch_conv1_wgrad(const __nv_bfloat16* d_a1, const __nv_bfloat16* a1, const uint8_t* am1, const float* data, float* dW, float* db,
-                       int N, int W, cudaStream_t st) {
-  const int tiles = N * (((W >> 1) + C1W_ROWS - 1) / C1W_ROWS);
-  conv1_wgrad_kernel<<<tiles < 2 * device_sms() ? tiles : 2 * device_sms(), 256, 0, st>>>(d_a1, a1, am1, data, dW, db, N, W);
   LAUNCH_CHECK();
 }
 int launch_dgrad_weight(const float* w, __nv_bfloat16* bd, int Cin, int Cout, cudaStream_t st) {
@@ -664,8 +504,8 @@ int launch_conv5_dgrad_weight(const float* w, __nv_bfloat16* bd, cudaStream_t st
   conv5_dgrad_weight_kernel<<<4 * device_sms(), 256, 0, st>>>(w, bd);
   LAUNCH_CHECK();
 }
-int launch_lstm_bwd_weight(const float* w_fw, const float* w_bw, __nv_bfloat16* bxb, __nv_bfloat16* bhb, int upc, cudaStream_t st) {
-  lstm_bwd_weight_kernel<<<4 * device_sms(), 256, 0, st>>>(w_fw, w_bw, bxb, bhb, upc);
+int launch_lstm_bwd_weight(const float* w_fw, const float* w_bw, __nv_bfloat16* bxb, __nv_bfloat16* bhb, cudaStream_t st) {
+  lstm_bwd_weight_kernel<<<4 * device_sms(), 256, 0, st>>>(w_fw, w_bw, bxb, bhb, LSTM_GATE_UNITS);
   LAUNCH_CHECK();
 }
 int launch_cast_bf16(const float* src, __nv_bfloat16* dst, size_t n, cudaStream_t st) {

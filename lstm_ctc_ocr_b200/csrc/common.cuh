@@ -23,6 +23,10 @@ int crnn_fail(int status, const char* fmt, ...);   // records crnn_last_error(),
     if (_s != CRNN_OK) return _s; \
   } while (0)
 
+// hidden units per [i|j|f|o] gate tile of the permuted LSTM weight columns: one CTA of the 8-CTA recurrence clusters owns 32
+// units (lstm.cuh), so gate column j = g*256 + u sits at (u/32)*128 + g*32 + u%32
+constexpr int LSTM_GATE_UNITS = 32;
+
 // ---- saved LSTM state (training): written by the forward recurrence kernels, read by the BPTT kernels.  Both access it with
 // lane = sample row of a 128-row batch tile, so the layout keeps the 128 rows of a tile adjacent: a warp's 32 lanes store / load
 // 32 consecutive 16-byte vectors (one 512-byte segment) instead of 32 sectors that are T*2 KB apart.

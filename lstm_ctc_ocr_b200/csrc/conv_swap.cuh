@@ -208,7 +208,7 @@ conv2_swap_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
             const float x10 = __uint_as_float(v[16 + 2 * pw]), x11 = __uint_as_float(v[16 + 2 * pw + 1]);
             {
               // key = (bf16 bits of relu(x + b) << 2) | (3 - window index): the largest value wins, ties go to the FIRST
-              // window position in (dy, dx) row-major order (same rule as gemm.cuh EPI_RELU_POOL22_T)
+              // window position in (dy, dx) row-major order (the rule of gemm.cuh EPI_RELU_POOL12_T over a 2x2 window)
               const uint32_t p0 = ptx::pack_bf16x2(fmaxf(x00 + bias, 0.f), fmaxf(x01 + bias, 0.f));
               const uint32_t p1 = ptx::pack_bf16x2(fmaxf(x10 + bias, 0.f), fmaxf(x11 + bias, 0.f));
               const uint32_t k0 = ((p0 & 0xFFFFu) << 2) | 3u, k1 = ((p0 >> 16) << 2) | 2u;

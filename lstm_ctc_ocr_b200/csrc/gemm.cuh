@@ -9,7 +9,7 @@
 // every epilogue thread owns one accumulator ROW: 8 warps, accumulator quadrant q = warp % 4 (32 rows), two warps per
 // quadrant each draining half of the staged columns.  At BLOCK_N = 256 the tile goes through one 128 x 64 f32 buffer (32 KB)
 // a 64-column slice at a time, not as a whole (128 KB): that leaves room for a 4-stage ring, where the full tile would leave 2.
-// Narrower tiles, EPI_LSTM and EPI_CONV_STORE_BNRED stage the whole tile (slice_cols).  The MMA warpgroups run with 240
+// Narrower tiles and EPI_CONV_STORE_BNRED stage the whole tile (slice_cols).  The MMA warpgroups run with 240
 // registers (the producer keeps 24): the first slices drain while the later slices' accumulators are still in registers.
 // The bf16-output epilogues at BLOCK_N = 256 (frag_epi) do not stage f32 at all: they finish the values in the fragment registers,
 // write bf16 into the staging region (the whole 64 KB tile, 3 stages) in the layout of the output tensor map and leave through asynchronous TMA stores
@@ -44,15 +44,12 @@ enum Epi {
   EPI_F32 = 0,          // D f32 row-major [M, Nc] (tests)
   EPI_BIAS_BF16 = 1,    // + bias -> bf16 row-major [M, ldo]            (conv5, LSTM input projection)
   EPI_RELU = 2,         // conv: + bias, ReLU -> bf16 NHWC              (conv3_1)
-  EPI_RELU_POOL22 = 3,  // conv: + bias, ReLU, 2x2/2 max-pool           (conv2 + pool2), needs Wd=16
   EPI_RELU_POOL12 = 4,  // conv: + bias, ReLU, max over Wd pairs        (conv3_2 + pool), needs Wd=8
   EPI_STATS = 5,        // conv: + bias -> bf16 pre-BN, per-channel sum / sum^2 (f64 atomics) (conv4_x)
-  EPI_LSTM = 6,         // recurrent step: gates = acc + xproj; LSTM cell; writes h, c, output
   EPI_LOGITS = 7,       // + bias -> f32 time-major [T, N, 64]
   EPI_XPROJ = 8,        // + bias -> bf16 [N*H, 2048]; columns >= 1024 (backward direction) stored reversed-by-length
   EPI_CONV_STORE = 9,   // conv: plain bf16 NHWC store (data-gradient convolutions)
-  EPI_RELU_POOL22_T = 10,  // training variants of the pooled epilogues: also emit the arg-max window index (uint8)
-  EPI_RELU_POOL12_T = 11,
+  EPI_RELU_POOL12_T = 11,  // training variant of EPI_RELU_POOL12: also emits the arg-max window index (uint8)
   EPI_CONV_STORE_MASK = 13,  // EPI_CONV_STORE with the ReLU backward of the PRODUCING layer folded in: zero where p.mask (its bf16 output, same NHWC layout) is 0
   EPI_CONV_STORE_BNRED = 14, // EPI_CONV_STORE + pass 1 of the BatchNorm/ReLU backward of the PRODUCING layer: per-channel f64 sums of the
                              // ReLU-masked gradient and of gradient * xhat (p.mask = its pre-BN bf16 output, p.bnp = scale|shift|mean|invstd)
@@ -85,14 +82,10 @@ struct Params {
   double* stats;         // [2][Nc] (EPI_STATS)
   const __nv_bfloat16* mask;   // EPI_CONV_STORE_MASK: post-ReLU activation of the layer whose pre-activation gradient is being written
   const float* bnp;      // EPI_CONV_STORE_BNRED: [4][Nc] scale, shift, mean, invstd of the producing layer's BatchNorm
-  uint8_t* argmax;       // pooled-epilogue training variants: window index of the max, same shape as `out`
-  // EPI_LSTM
-  const __nv_bfloat16* xproj;   // [Nimg*H, 2048] gate pre-activations (x part + bias), permuted columns
-  float* c_state;               // [2][Npad][256]
-  __nv_bfloat16* h_next;        // [2][Npad][256]
-  __nv_bfloat16* lstm_out;      // [Nimg*H, 512]
-  const int* seq_len;           // [Nimg]
-  int step, Npad, m_tiles_per_dir, T;
+  uint8_t* argmax;       // EPI_RELU_POOL12_T: window index of the max, same shape as `out`
+  // EPI_XPROJ (backward-direction rows reversed by length), EPI_LOGITS (time-major rows)
+  const int* seq_len;    // [Nimg]
+  int T;
   // LINES instantiations (packed evaluation, crnn_forward_lines): [Nimg] clamped line widths in input columns; conv rows at
   // h >= line_w[n] / 4 (every LINES layer runs at H = W/4) are stored as zero, and EPI_STATS sums go to slot n of `stats` [Nimg][2][Nc]
   const int* line_w;
@@ -136,13 +129,13 @@ __device__ __forceinline__ float warp_colsum32(const float (&v)[32], int lane) {
 
 // Accumulator columns staged in shared memory at a time (see the header).  While a slice drains, the accumulators of the
 // later slices stay live in registers (96 at BLOCK_N = 256).  EPI_CONV_STORE_BNRED's epilogue does not fit in the registers
-// left beside them (it spills), so, like EPI_LSTM, it stages the whole tile; it only serves the training backward pass.
+// left beside them (it spills), so it stages the whole tile; it only serves the training backward pass.
 // BLOCK_N = 128 measured slower in 64-column slices (6 stages) than whole (5 stages), so it stays whole.  The register-side
 // bf16 epilogues (frag_epi) stage the whole bf16 tile in the bytes of 128 f32 columns: with 3 stages that measured faster than
 // two 32 KB halves through one buffer with 4 stages (the halves wait on each other's stores).  EPI_RELU_POOL12's pooled tile
 // needs only 32 KB.
 constexpr int slice_cols(int block_n, int epi) {
-  return (block_n < 256 || epi == EPI_LSTM || epi == EPI_CONV_STORE_BNRED) ? block_n
+  return (block_n < 256 || epi == EPI_CONV_STORE_BNRED) ? block_n
        : (epi == EPI_RELU || epi == EPI_STATS || epi == EPI_BIAS_BF16 || epi == EPI_XPROJ || epi == EPI_CONV_STORE) ? 128 : 64;
 }
 
@@ -377,9 +370,8 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
   // ---- conv row geometry (one sub-box of 32 positions per warp)
   int n_img = 0, h = 0, w = 0;
   bool valid = true;
-  if (EPI == EPI_RELU || EPI == EPI_RELU_POOL22 || EPI == EPI_RELU_POOL12 || EPI == EPI_STATS || EPI == EPI_CONV_STORE ||
-      EPI == EPI_RELU_POOL22_T || EPI == EPI_RELU_POOL12_T || EPI == EPI_CONV_F32 || EPI == EPI_CONV_STORE_MASK ||
-      EPI == EPI_CONV_STORE_BNRED) {
+  if (EPI == EPI_RELU || EPI == EPI_RELU_POOL12 || EPI == EPI_STATS || EPI == EPI_RELU_POOL12_T || EPI == EPI_CONV_F32 ||
+      EPI == EPI_CONV_STORE_MASK || EPI == EPI_CONV_STORE_BNRED) {
     const int g = m_blk * 4 + q;
     n_img = g / p.sb_per_img;
     const int hb = g - n_img * p.sb_per_img;
@@ -448,11 +440,10 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
         }
       }
     }
-  } else if (EPI == EPI_RELU || EPI == EPI_RELU_POOL22 || EPI == EPI_RELU_POOL12) {
+  } else if (EPI == EPI_RELU || EPI == EPI_RELU_POOL12) {
     __nv_bfloat16* outb = reinterpret_cast<__nv_bfloat16*>(p.out);
     size_t off;
     if (EPI == EPI_RELU) off = (((size_t)n_img * p.H + h) * p.Wd + w) * p.Nc;
-    else if (EPI == EPI_RELU_POOL22) off = (((size_t)n_img * (p.H >> 1) + (h >> 1)) * (p.Wd >> 1) + (w >> 1)) * p.Nc;
     else off = (((size_t)n_img * p.H + h) * (p.Wd >> 1) + (w >> 1)) * p.Nc;
     __nv_bfloat16* out = outb + off + col0;
 #pragma unroll 1
@@ -472,22 +463,8 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
           for (int i = 0; i < 16; i += 8)
             ptx::st_global_v8(out + c0 + 2 * i, pk[i], pk[i + 1], pk[i + 2], pk[i + 3], pk[i + 4], pk[i + 5], pk[i + 6], pk[i + 7]);
         }
-      } else if (EPI == EPI_RELU_POOL22) {
-        // lane = hl*16 + w : partners lane^1 (w pair) and lane^16 (h pair); rounding to bf16 is monotonic,
-        // so max after packing == packing after max
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          pk[i] = ptx::hmax2_bf16(pk[i], __shfl_xor_sync(0xffffffffu, pk[i], 1));
-          pk[i] = ptx::hmax2_bf16(pk[i], __shfl_xor_sync(0xffffffffu, pk[i], 16));
-        }
-        const int sub = (lane & 1) | ((lane >> 3) & 2);     // which quarter of the 32 columns this lane stores
-        uint4 o;
-        o.x = sub == 0 ? pk[0] : sub == 1 ? pk[4] : sub == 2 ? pk[8] : pk[12];
-        o.y = sub == 0 ? pk[1] : sub == 1 ? pk[5] : sub == 2 ? pk[9] : pk[13];
-        o.z = sub == 0 ? pk[2] : sub == 1 ? pk[6] : sub == 2 ? pk[10] : pk[14];
-        o.w = sub == 0 ? pk[3] : sub == 1 ? pk[7] : sub == 2 ? pk[11] : pk[15];
-        if (valid) *reinterpret_cast<uint4*>(out + c0 + 8 * sub) = o;
       } else {
+        // lane = hl*8 + w: partner lane^1 (w pair); rounding to bf16 is monotonic, so max after packing == packing after max
 #pragma unroll
         for (int i = 0; i < 16; ++i) pk[i] = ptx::hmax2_bf16(pk[i], __shfl_xor_sync(0xffffffffu, pk[i], 1));
         const int sub = lane & 1;
@@ -498,26 +475,6 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
           *reinterpret_cast<uint4*>(out + c0 + 16 * sub) = o0;
           *reinterpret_cast<uint4*>(out + c0 + 16 * sub + 8) = o1;
         }
-      }
-    }
-  } else if (EPI == EPI_CONV_STORE) {
-    __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out) + (((size_t)n_img * p.H + h) * p.Wd + w) * p.Nc + col0;
-#pragma unroll 1
-    for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
-      uint32_t v[32];
-      ptx::acc_ld<NC, 32>(acc, row, c0 - c_acc, v);
-      if (valid) {
-#pragma unroll
-        for (int i = 0; i < 32; i += 16)
-          ptx::st_global_v8(out + c0 + i,
-                            ptx::pack_bf16x2(__uint_as_float(v[i]), __uint_as_float(v[i + 1])),
-                            ptx::pack_bf16x2(__uint_as_float(v[i + 2]), __uint_as_float(v[i + 3])),
-                            ptx::pack_bf16x2(__uint_as_float(v[i + 4]), __uint_as_float(v[i + 5])),
-                            ptx::pack_bf16x2(__uint_as_float(v[i + 6]), __uint_as_float(v[i + 7])),
-                            ptx::pack_bf16x2(__uint_as_float(v[i + 8]), __uint_as_float(v[i + 9])),
-                            ptx::pack_bf16x2(__uint_as_float(v[i + 10]), __uint_as_float(v[i + 11])),
-                            ptx::pack_bf16x2(__uint_as_float(v[i + 12]), __uint_as_float(v[i + 13])),
-                            ptx::pack_bf16x2(__uint_as_float(v[i + 14]), __uint_as_float(v[i + 15])));
       }
     }
   } else if (EPI == EPI_CONV_STORE_MASK) {
@@ -601,19 +558,16 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
           *reinterpret_cast<uint4*>(out + c0 + i) = make_uint4(v[i], v[i + 1], v[i + 2], v[i + 3]);
       }
     }
-  } else if (EPI == EPI_RELU_POOL22_T || EPI == EPI_RELU_POOL12_T) {
-    // Training variants: max over the pooling window carried as an integer key
-    //   key = (bf16 bits of relu(x) << 2) | (3 - window_index)
+  } else if (EPI == EPI_RELU_POOL12_T) {
+    // Training variant: max over the pooling window carried as an integer key
+    //   key = (bf16 bits of relu(x) << 2) | (1 - window_index)
     // post-ReLU bf16 bit patterns are monotone as unsigned integers, so max(key) picks the largest value and, among
-    // equal values, the FIRST window position (row-major (dy,dx), the tie-break of TF/torch max-pool gradients).
-    constexpr bool P22 = (EPI == EPI_RELU_POOL22_T);
-    size_t off;
-    if (P22) off = (((size_t)n_img * (p.H >> 1) + (h >> 1)) * (p.Wd >> 1) + (w >> 1)) * p.Nc;
-    else off = (((size_t)n_img * p.H + h) * (p.Wd >> 1) + (w >> 1)) * p.Nc;
+    // equal values, the FIRST window position (the tie-break of TF/torch max-pool gradients).
+    const size_t off = (((size_t)n_img * p.H + h) * (p.Wd >> 1) + (w >> 1)) * p.Nc;
     __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.out) + off + col0;
     uint8_t* amx = p.argmax + off + col0;
-    const uint32_t kidx = P22 ? (uint32_t)((((lane >> 4) & 1) << 1) | (lane & 1)) : (uint32_t)(lane & 1);
-    const uint32_t kinv = (P22 ? 3u : 1u) - kidx;
+    const uint32_t kidx = (uint32_t)(lane & 1);
+    const uint32_t kinv = 1u - kidx;
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
       uint32_t v[32];
@@ -629,13 +583,10 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
         v[i + 3] = ((p1 >> 16) << 2) | kinv;
       }
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        v[i] = max(v[i], __shfl_xor_sync(0xffffffffu, v[i], 1));
-        if (P22) v[i] = max(v[i], __shfl_xor_sync(0xffffffffu, v[i], 16));
-      }
-      // each lane of the window stores its share of the 32 columns: 8 (2x2 window) or 16 (1x2 window)
-      constexpr int NS = P22 ? 4 : 2, PER = 32 / NS;
-      const int sub = P22 ? ((lane & 1) | ((lane >> 3) & 2)) : (lane & 1);
+      for (int i = 0; i < 32; ++i) v[i] = max(v[i], __shfl_xor_sync(0xffffffffu, v[i], 1));
+      // each lane of the window stores its 16 of the 32 columns
+      constexpr int NS = 2, PER = 32 / NS;
+      const int sub = lane & 1;
       uint32_t sel[PER];
 #pragma unroll
       for (int i = 0; i < PER; ++i) {
@@ -653,7 +604,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
           o.z = ((sel[i + 4] >> 2) & 0xFFFFu) | ((sel[i + 5] >> 2) << 16);
           o.w = ((sel[i + 6] >> 2) & 0xFFFFu) | ((sel[i + 7] >> 2) << 16);
           *reinterpret_cast<uint4*>(out + c0 + sub * PER + i) = o;
-          const uint32_t km = P22 ? 3u : 1u;
+          const uint32_t km = 1u;
           uint2 a;
           a.x = (km - (sel[i] & km)) | ((km - (sel[i + 1] & km)) << 8) | ((km - (sel[i + 2] & km)) << 16) | ((km - (sel[i + 3] & km)) << 24);
           a.y = (km - (sel[i + 4] & km)) | ((km - (sel[i + 5] & km)) << 8) | ((km - (sel[i + 6] & km)) << 16) | ((km - (sel[i + 7] & km)) << 24);
@@ -696,75 +647,7 @@ __device__ __forceinline__ void run_epilogue(const Params& p, float* acc, const 
       atomicAdd(p.stats + col0 + c0 + lane, (double)s1);
       atomicAdd(p.stats + p.Nc + col0 + c0 + lane, (double)s2);
     }
-  } else if (EPI == EPI_LSTM) {
-    // row = sample within the direction-stacked batch; tile columns = [i(64) j(64) f(64) o(64)] of 64 units
-    // (the whole tile is staged: NC == BLOCK_N, c_acc == 0)
-    const int grow = m_blk * BLOCK_M + row;
-    const int dir = (m_blk >= p.m_tiles_per_dir) ? 1 : 0;
-    const int n = grow - dir * p.Npad;
-    const bool okn = n < p.Nimg;
-    const int len = okn ? min(max(__ldg(p.seq_len + n), 0), p.T) : 0;
-    const bool active = p.step < len;
-    const int t = active ? (dir ? (len - 1 - p.step) : p.step) : p.step;
-    const size_t rt = (size_t)n * p.H + t;
-    const __nv_bfloat16* xp = p.xproj + rt * 2048 + dir * 1024 + n_blk * 256;
-    float* cst = p.c_state + ((size_t)dir * p.Npad + n) * 256 + n_blk * 64;
-    __nv_bfloat16* hn = p.h_next + ((size_t)dir * p.Npad + n) * 256 + n_blk * 64;
-    __nv_bfloat16* lo = p.lstm_out + rt * 512 + dir * 256 + n_blk * 64;
-#pragma unroll 1
-    for (int u0 = (c_lo >> 2); u0 < (c_hi >> 2); u0 += 16) {
-      uint32_t gi[16], gj[16], gf[16], go[16];
-      ptx::acc_ld<NC, 16>(acc, row, u0, gi);
-      ptx::acc_ld<NC, 16>(acc, row, 64 + u0, gj);
-      ptx::acc_ld<NC, 16>(acc, row, 128 + u0, gf);
-      ptx::acc_ld<NC, 16>(acc, row, 192 + u0, go);
-      uint32_t hp[8];
-      if (active) {
-        uint4 xi[2], xj[2], xf[2], xo[2];
-        float4 cp[4];
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          xi[i] = __ldg(reinterpret_cast<const uint4*>(xp + u0) + i);
-          xj[i] = __ldg(reinterpret_cast<const uint4*>(xp + 64 + u0) + i);
-          xf[i] = __ldg(reinterpret_cast<const uint4*>(xp + 128 + u0) + i);
-          xo[i] = __ldg(reinterpret_cast<const uint4*>(xp + 192 + u0) + i);
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) cp[i] = *(reinterpret_cast<const float4*>(cst + u0) + i);
-        const uint32_t* xiw = reinterpret_cast<const uint32_t*>(xi);
-        const uint32_t* xjw = reinterpret_cast<const uint32_t*>(xj);
-        const uint32_t* xfw = reinterpret_cast<const uint32_t*>(xf);
-        const uint32_t* xow = reinterpret_cast<const uint32_t*>(xo);
-        float* cpf = reinterpret_cast<float*>(cp);
-        float hv[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float zi = __uint_as_float(gi[i]) + ((i & 1) ? ptx::bf16_hi(xiw[i >> 1]) : ptx::bf16_lo(xiw[i >> 1]));
-          const float zj = __uint_as_float(gj[i]) + ((i & 1) ? ptx::bf16_hi(xjw[i >> 1]) : ptx::bf16_lo(xjw[i >> 1]));
-          const float zf = __uint_as_float(gf[i]) + ((i & 1) ? ptx::bf16_hi(xfw[i >> 1]) : ptx::bf16_lo(xfw[i >> 1]));
-          const float zo = __uint_as_float(go[i]) + ((i & 1) ? ptx::bf16_hi(xow[i >> 1]) : ptx::bf16_lo(xow[i >> 1]));
-          // forget_bias (+1.0) is folded into the projected bias at weight-prep time
-          const float c = ptx::fast_sigmoid(zf) * cpf[i] + ptx::fast_sigmoid(zi) * ptx::fast_tanh(zj);
-          cpf[i] = c;
-          hv[i] = ptx::fast_sigmoid(zo) * ptx::fast_tanh(c);
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) *(reinterpret_cast<float4*>(cst + u0) + i) = cp[i];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) hp[i] = ptx::pack_bf16x2(hv[2 * i], hv[2 * i + 1]);
-      } else {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) hp[i] = 0u;    // zero output past sequence_length; state no longer used
-      }
-      if (okn) {
-        *reinterpret_cast<uint4*>(hn + u0) = make_uint4(hp[0], hp[1], hp[2], hp[3]);
-        *reinterpret_cast<uint4*>(hn + u0 + 8) = make_uint4(hp[4], hp[5], hp[6], hp[7]);
-        *reinterpret_cast<uint4*>(lo + u0) = make_uint4(hp[0], hp[1], hp[2], hp[3]);
-        *reinterpret_cast<uint4*>(lo + u0 + 8) = make_uint4(hp[4], hp[5], hp[6], hp[7]);
-      }
-    }
   }
-
 }
 
 // KIND 0: bf16 operands, 64 elements per 128 B K-block.  KIND 1: f32 words read as tf32, 32 elements per K-block
@@ -823,8 +706,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m_blk = p.m_tile0 + tile / p.num_n_tiles, n_blk = tile % p.num_n_tiles;
-        int b_row = n_blk * BLOCK_N;
-        if (EPI == EPI_LSTM) b_row += (m_blk >= p.m_tiles_per_dir) ? 1024 : 0;
+        const int b_row = n_blk * BLOCK_N;
         // per-tile coordinates of this lane's A box (conv): image n, first H row h0
         int cn = 0, ch0 = 0;
         if (AMODE == A_CONV3 && lane < nA) {

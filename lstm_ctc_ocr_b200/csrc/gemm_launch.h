@@ -2,8 +2,6 @@
 #pragma once
 #include "gemm.cuh"
 #include "gemm_tn.cuh"
-#include <cstdlib>
-#include <string>
 
 // `out` is the tensor map the register-side epilogues (gemm::frag_epi) store through: NHWC box [64, Wd, bh (x4 merged), 1] for
 // conv outputs, [64, 128] over [M, ldo] for plain ones.  The other epilogues take no map.
@@ -26,16 +24,10 @@ static int launch_gemm(const CUtensorMap& a, const CUtensorMap& b, const gemm::P
 }
 
 // Split-K factor of a weight-gradient GEMM.  Work items (output tile x K chunk) all cost the same and the persistent CTAs take them
-// round-robin, so the launch lasts  ceil(items / workers) rounds x (K blocks per chunk + epilogue).  The first-generation rule
-// ("about 3 items per worker") can leave a mostly idle last round.  Pick the factor that minimises the modelled time (ties: fewer chunks =
-// fewer f32 reduction atomics).  CRNN_KSPLIT=old restores the old rule.
+// round-robin, so the launch lasts  ceil(items / workers) rounds x (K blocks per chunk + epilogue).  A fixed "about 3 items per
+// worker" can leave a mostly idle last round.  Pick the factor that minimises the modelled time (ties: fewer chunks = fewer f32
+// reduction atomics).
 static inline int pick_k_splits(int tiles, int k_blocks_total, int workers) {
-  static const bool old_rule = [] { const char* e = getenv("CRNN_KSPLIT"); return e && std::string(e) == "old"; }();
-  if (old_rule) {
-    int s = (3 * workers + tiles - 1) / tiles;
-    if (s > k_blocks_total) s = k_blocks_total;
-    return s < 1 ? 1 : s;
-  }
   const int kEpi = 6;                            // epilogue + pipeline refill of one item, in K-block units
   int best = 1;
   long long best_cost = -1;

@@ -39,8 +39,7 @@ struct Params {
   // TN_CONV geometry
   int sb_per_img, bh, Wd, H, Nimg, Cin;
   int merged, kb_per_img;                    // TN_CONV: 64-position boxes (2*bh rows) when H % (2*bh) == 0
-  int tap_pack;                              // TN_CONV with Cin == 64: an M tile packs TWO taps (rows = (tap, ci)) -> 5 tiles, not 9 half-empty ones
-  int tap_pack_n;                            // TN_CONV with Cin == 64, operands SWAPPED (r2, conv2 weight gradient): A = the output gradient
+  int tap_pack_n;                            // TN_CONV with Cin == 64, operands SWAPPED (conv2 weight gradient): A = the output gradient
                                              // (M = Cout), B = the activation with FOUR tap-shifted 64-channel boxes per 256-column N tile
                                              // (columns = (tap, ci)); N = 256 restores the MMA rate the Cout = 128 N tile halves.  The
                                              // accumulator is written transposed: out[(tap*64 + ci) * ldo + co]
@@ -128,10 +127,6 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         int r = tap / 3, s = tap - 3 * r;
         int ccol = isA ? (m_blk * BLOCK_M + 64 * j) : (n_blk * BLOCK_N + 64 * j);
         bool shifted = isA;                                 // which operand's boxes carry the (r-1, s-1) tap shift
-        if (AMODE == TN_CONV && p.tap_pack && isA) {       // A block j of tile m_blk is tap 2*m_blk + j, channels 0..63
-          const int tp = min(2 * m_blk + j, 8);             // the 10th (non-existent) tap re-reads tap 8; its rows are masked
-          r = tp / 3; s = tp - 3 * r; ccol = 0;
-        }
         if (AMODE == TN_CONV && p.tap_pack_n) {            // B block j of tile n_blk is tap 4*n_blk + j (taps >= 9: columns masked)
           shifted = !isA;
           if (!isA) { const int tp = min(4 * n_blk + j, 8); r = tp / 3; s = tp - 3 * r; ccol = 0; }

@@ -1,141 +1,8 @@
-// HBM-bound / SIMT kernels of the forward path: conv1+pool1 (K = 9, no tensor cores), BatchNorm
-// finalize/apply, weight re-layout (f32 TF layouts -> bf16 K-major GEMM operands), L2 term, loss reduce.
+// HBM-bound / SIMT kernels of the forward path: BatchNorm finalize/apply, weight re-layout (f32 TF layouts -> bf16 K-major GEMM
+// operands), L2 term, loss reduce.
 #include "kernels.cuh"
 
 namespace {
-
-// ------------------------------------------------------------------------------------------------
-// conv1 (3x3 SAME, 1 -> 64, bias, ReLU) fused with pool1 (2x2/2).   lib/networks/LSTM_train.py:24-25
-// data [N, W, 32] f32 (axis1 = image width/time, axis2 = image height)  ->  out [N, W/2, 16, 64] bf16 NHWC.
-// Tile = one image x 8 pooled rows x 16 pooled cols; thread = 8 output channels x 4 pooled positions,
-// 72 filter taps held in registers; input tile (18 x 34 f32, zero halo) staged in shared memory.
-// ------------------------------------------------------------------------------------------------
-constexpr int C1_ROWS = 8;                         // pooled rows per tile
-constexpr int C1_TILE_ELEMS = (2 * C1_ROWS + 2) * 34;
-
-__device__ __forceinline__ float conv1_fetch(const float* __restrict__ data, int n, int ho0, int W, int i) {
-  // element i of the staged tile: rows 2*ho0-1 .. 2*ho0+16 (18 rows) x cols -1..32 (34), zero outside the image
-  const int r = i / 34, c = i - r * 34;
-  const int gr = 2 * ho0 - 1 + r, gc = c - 1;
-  return (gr >= 0 && gr < W && gc >= 0 && gc < 32) ? __ldg(data + ((size_t)n * W + gr) * 32 + gc) : 0.f;
-}
-
-// TRAIN additionally records the arg-max window index of pool1 (needed by the backward pass).
-template <bool TRAIN>
-__global__ void __launch_bounds__(256) conv1_pool_kernel(const float* __restrict__ data,
-                                                         const float* __restrict__ wgt,   // HWIO [3,3,1,64]
-                                                         const float* __restrict__ bias, __nv_bfloat16* __restrict__ out,
-                                                         uint8_t* __restrict__ argmax, int N, int W) {
-  __shared__ __align__(16) float s_in[2][2 * C1_ROWS + 2][36];      // double buffered: next tile is prefetched during compute
-  const int H1 = W >> 1;
-  const int tiles_per_img = (H1 + C1_ROWS - 1) / C1_ROWS;
-  const int num_tiles = N * tiles_per_img;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int cg = lane & 7;                          // channel group: channels cg*8 .. cg*8+7
-  const int slot = warp * 4 + (lane >> 3);          // 0..31
-
-  // taps as f32x2 pairs of adjacent channels: the 288 FMAs per pooled position issue as 144 FFMA2 (the 3-register FFMA
-  // issues every other cycle per scheduler, which caps the scalar loop)
-  uint64_t wr[9][4];
-  float br[8];
-#pragma unroll
-  for (int k = 0; k < 9; ++k)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) wr[k][j] = ptx::pack_f32x2(__ldg(wgt + k * 64 + cg * 8 + 2 * j), __ldg(wgt + k * 64 + cg * 8 + 2 * j + 1));
-#pragma unroll
-  for (int j = 0; j < 8; ++j) br[j] = __ldg(bias + cg * 8 + j);
-
-  int tile = blockIdx.x;
-  if (tile < num_tiles) {
-    const int n = tile / tiles_per_img, ho0 = (tile - n * tiles_per_img) * C1_ROWS;
-    for (int i = threadIdx.x; i < C1_TILE_ELEMS; i += 256) s_in[0][i / 34][i % 34] = conv1_fetch(data, n, ho0, W, i);
-  }
-  __syncthreads();
-  int buf = 0;
-  for (; tile < num_tiles; tile += gridDim.x) {
-    const int n = tile / tiles_per_img;
-    const int ho0 = (tile - n * tiles_per_img) * C1_ROWS;
-    // prefetch the next tile into registers (<= 3 elements per thread); stored to the other buffer after the compute
-    const int nxt = tile + gridDim.x;
-    float pre[3];
-    if (nxt < num_tiles) {
-      const int nn = nxt / tiles_per_img, nho0 = (nxt - nn * tiles_per_img) * C1_ROWS;
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        const int i = threadIdx.x + 256 * k;
-        pre[k] = (i < C1_TILE_ELEMS) ? conv1_fetch(data, nn, nho0, W, i) : 0.f;
-      }
-    }
-#pragma unroll 1
-    for (int pp = 0; pp < 4; ++pp) {
-      const int pidx = slot + 32 * pp;              // 0..127
-      const int hol = pidx >> 4, wo = pidx & 15;
-      const int ho = ho0 + hol;
-      float patch[4][4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 a = *reinterpret_cast<const float2*>(&s_in[buf][2 * hol + i][2 * wo]);
-        const float2 c = *reinterpret_cast<const float2*>(&s_in[buf][2 * hol + i][2 * wo + 2]);
-        patch[i][0] = a.x; patch[i][1] = a.y; patch[i][2] = c.x; patch[i][3] = c.y;
-      }
-      float best[8];
-      uint32_t bidx[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { best[j] = -INFINITY; bidx[j] = 0; }
-#pragma unroll
-      for (int dy = 0; dy < 2; ++dy)
-#pragma unroll
-        for (int dx = 0; dx < 2; ++dx) {
-          uint64_t acc2[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) acc2[j] = 0ull;
-#pragma unroll
-          for (int r = 0; r < 3; ++r)
-#pragma unroll
-            for (int s = 0; s < 3; ++s) {
-              const uint64_t x2 = ptx::pack_f32x2(patch[dy + r][dx + s], patch[dy + r][dx + s]);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) acc2[j] = ptx::ffma2(x2, wr[r * 3 + s][j], acc2[j]);
-            }
-          float acc[8];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) ptx::unpack_f32x2(acc2[j], acc[2 * j], acc[2 * j + 1]);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            if (TRAIN) {
-              if (acc[j] > best[j]) { best[j] = acc[j]; bidx[j] = dy * 2 + dx; }     // strict '>' keeps the first max
-            } else {
-              best[j] = fmaxf(best[j], acc[j]);
-            }
-          }
-        }
-      if (ho < H1) {
-        uint4 o;
-        o.x = ptx::pack_bf16x2(fmaxf(best[0] + br[0], 0.f), fmaxf(best[1] + br[1], 0.f));
-        o.y = ptx::pack_bf16x2(fmaxf(best[2] + br[2], 0.f), fmaxf(best[3] + br[3], 0.f));
-        o.z = ptx::pack_bf16x2(fmaxf(best[4] + br[4], 0.f), fmaxf(best[5] + br[5], 0.f));
-        o.w = ptx::pack_bf16x2(fmaxf(best[6] + br[6], 0.f), fmaxf(best[7] + br[7], 0.f));
-        const size_t oo = (((size_t)n * H1 + ho) * 16 + wo) * 64 + cg * 8;
-        *reinterpret_cast<uint4*>(out + oo) = o;
-        if (TRAIN) {
-          uint2 a;
-          a.x = bidx[0] | (bidx[1] << 8) | (bidx[2] << 16) | (bidx[3] << 24);
-          a.y = bidx[4] | (bidx[5] << 8) | (bidx[6] << 16) | (bidx[7] << 24);
-          *reinterpret_cast<uint2*>(argmax + oo) = a;
-        }
-      }
-    }
-    if (nxt < num_tiles) {
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        const int i = threadIdx.x + 256 * k;
-        if (i < C1_TILE_ELEMS) s_in[buf ^ 1][i / 34][i % 34] = pre[k];
-      }
-    }
-    __syncthreads();
-    buf ^= 1;
-  }
-}
 
 // ------------------------------------------------------------------------------------------------
 // BatchNorm with batch statistics (tf.contrib.layers.batch_norm(is_training=True), network.py:177-178)
@@ -283,7 +150,7 @@ __global__ void clamp_line_width_kernel(const int* __restrict__ in, int* __restr
 
 // ------------------------------------------------------------------------------------------------
 // weight re-layout: dst[perm(c)][r] (bf16, K-major GEMM B operand) = src[r][c] (f32, TF layout)
-// perm_mode 0: identity; upc > 0: LSTM gate permutation  j = g*256+u  ->  (u/upc)*4*upc + g*upc + u%upc
+// perm_mode 0: identity; upc > 0 (= LSTM_GATE_UNITS): LSTM gate permutation  j = g*256+u  ->  (u/upc)*4*upc + g*upc + u%upc
 // (a tile of 4*upc consecutive rows then holds [i|j|f|o] of upc hidden units)
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ int lstm_perm(int j, int upc) {
@@ -371,15 +238,6 @@ __global__ void bf16_to_f32_kernel(const __nv_bfloat16* __restrict__ in, float* 
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------ launchers
-int launch_conv1_pool(const float* data, const float* w, const float* b, __nv_bfloat16* out, uint8_t* argmax, int N, int W,
-                      int num_sms, cudaStream_t st) {
-  const int tiles = N * (((W >> 1) + C1_ROWS - 1) / C1_ROWS);
-  const int grid = tiles < num_sms * 2 ? tiles : num_sms * 2;
-  if (argmax != nullptr) conv1_pool_kernel<true><<<grid, 256, 0, st>>>(data, w, b, out, argmax, N, W);
-  else conv1_pool_kernel<false><<<grid, 256, 0, st>>>(data, w, b, out, argmax, N, W);
-  CUDA_TRY(cudaGetLastError());
-  return CRNN_OK;
-}
 int launch_bn_finalize(const double* stats, double count, const float* gamma, const float* beta, float eps, float* scale,
                        float* shift, float* save_mean, float* save_invstd, int C, cudaStream_t st) {
   bn_finalize_kernel<<<(C + 127) / 128, 128, 0, st>>>(stats, count, gamma, beta, eps, scale, shift, save_mean, save_invstd, C);
@@ -429,15 +287,15 @@ int launch_bn_apply_relu_pool12_lines(const __nv_bfloat16* in, __nv_bfloat16* ou
   CUDA_TRY(cudaGetLastError());
   return CRNN_OK;
 }
-int launch_transpose_cast(const float* src, int R, int Cc, int ld_src, __nv_bfloat16* dst, int ld_dst, int perm_mode,
+int launch_transpose_cast(const float* src, int R, int Cc, int ld_src, __nv_bfloat16* dst, int ld_dst, bool lstm_gates,
                           cudaStream_t st) {
   dim3 grid((Cc + 31) / 32, (R + 31) / 32);
-  transpose_cast_kernel<<<grid, 256, 0, st>>>(src, R, Cc, ld_src, dst, ld_dst, perm_mode);
+  transpose_cast_kernel<<<grid, 256, 0, st>>>(src, R, Cc, ld_src, dst, ld_dst, lstm_gates ? LSTM_GATE_UNITS : 0);
   CUDA_TRY(cudaGetLastError());
   return CRNN_OK;
 }
-int launch_lstm_bias_prep(const float* b_fw, const float* b_bw, float* xbias, int upc, cudaStream_t st) {
-  lstm_bias_prep_kernel<<<8, 256, 0, st>>>(b_fw, b_bw, xbias, upc);
+int launch_lstm_bias_prep(const float* b_fw, const float* b_bw, float* xbias, cudaStream_t st) {
+  lstm_bias_prep_kernel<<<8, 256, 0, st>>>(b_fw, b_bw, xbias, LSTM_GATE_UNITS);
   CUDA_TRY(cudaGetLastError());
   return CRNN_OK;
 }

@@ -8,8 +8,6 @@ struct SumsqSegs {
   long long cnt[8];
 };
 
-int launch_conv1_pool(const float* data, const float* w, const float* b, __nv_bfloat16* out, uint8_t* argmax, int N, int W,
-                      int num_sms, cudaStream_t st);
 int launch_bn_finalize(const double* stats, double count, const float* gamma, const float* beta, float eps, float* scale,
                        float* shift, float* save_mean, float* save_invstd, int C, cudaStream_t st);
 int launch_bn_apply_relu(const __nv_bfloat16* in, __nv_bfloat16* out, const float* scale, const float* shift, size_t rows,
@@ -25,9 +23,10 @@ int launch_bn_apply_relu_lines(const __nv_bfloat16* in, __nv_bfloat16* out, cons
                                int C, cudaStream_t st);
 int launch_bn_apply_relu_pool12_lines(const __nv_bfloat16* in, __nv_bfloat16* out, const float* bn, const int* line_w, int N, int H,
                                       int Wo, int C, cudaStream_t st);
-int launch_transpose_cast(const float* src, int R, int Cc, int ld_src, __nv_bfloat16* dst, int ld_dst, int perm_mode,
+// lstm_gates: the columns are LSTM gate columns, stored permuted (LSTM_GATE_UNITS units per [i|j|f|o] tile)
+int launch_transpose_cast(const float* src, int R, int Cc, int ld_src, __nv_bfloat16* dst, int ld_dst, bool lstm_gates,
                           cudaStream_t st);
-int launch_lstm_bias_prep(const float* b_fw, const float* b_bw, float* xbias, int upc, cudaStream_t st);
+int launch_lstm_bias_prep(const float* b_fw, const float* b_bw, float* xbias, cudaStream_t st);
 int launch_sumsq(const float* params, const SumsqSegs& segs, double* out, cudaStream_t st);
 int launch_total_loss(const float* costs, int N, const double* sumsq, float wd, float* loss, cudaStream_t st);
 int launch_bf16_to_f32(const __nv_bfloat16* in, float* out, size_t n, cudaStream_t st);

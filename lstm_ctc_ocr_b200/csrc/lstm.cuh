@@ -4,24 +4,9 @@
 // (lib/networks/network.py:104-107): per step  z = x_t W_x + b (precomputed, `xproj`) + h_{t-1} W_h ;
 // i,j,f,o = split(z); c = sigma(f+1) c + sigma(i) tanh(j); h = sigma(o) tanh(c); zero output past sequence_length.
 //
-// Two generations live in this file:
-//   lstm_mc_kernel<CS, MODE, EW>   (further down; the default, MODE 2 = "ms") -- two independent 64-row half pipelines per CTA;
-//                                  the cell runs on the wgmma accumulator fragments, h is exchanged as 4 KB half slices that
-//                                  land directly in every CTA's no-swizzle A operand, signalled through mbarriers; no cluster
-//                                  barrier per step
-//   lstm_persistent_kernel<CS>     (first, below; CRNN_LSTM_IMPL=persistent) -- h through global memory, a 64 KB TMA fetch per CTA,
-//                                  fence.proxy.async and one barrier.cluster per step; those per-step costs are the
-//                                  reason the second generation exists (see the comment above lstm_mc_kernel)
-//
-// First generation:
-// Cluster of CS CTAs; CTA `rank` owns UPC = 256/CS hidden units (4*UPC gate columns, ordered [i|j|f|o]):
-//   * its W_h slice [4*UPC x 256] bf16 stays resident in shared memory for all T steps (loaded once by TMA)
-//   * per step: TMA loads h_{t-1} [128 x 256] (written to global/L2 by the whole cluster in the previous step),
-//     two MMA warpgroups issue 16 wgmma (64 x 4*UPC x 16 each), the accumulators are staged in shared memory, 4 epilogue
-//     warps (thread = sample row) add the precomputed input projection (prefetched before the MMA), run the cell with the
-//     f32 cell state held in REGISTERS for the whole sequence, write h (bf16) for the next step and the output row
-//   * one barrier.cluster per step orders the h exchange (generic-proxy global stores -> fence.proxy.async ->
-//     release/acquire cluster barrier -> TMA loads of the next step)
+// lstm_mc_kernel<CS>: two independent 64-row half pipelines per CTA; the cell runs on the wgmma accumulator fragments, h is
+// exchanged as 4 KB half slices that land directly in every CTA's no-swizzle A operand, signalled through mbarriers; no cluster
+// barrier per step (details above the kernel).
 // Clusters are independent (no grid-wide sync), so partial residency cannot deadlock.
 // The backward direction reads xproj rows that the projection GEMM already stored reversed-by-length, so both
 // directions index step s uniformly; outputs are written back at t = len-1-s.
@@ -33,8 +18,8 @@
 
 namespace lstm {
 
-constexpr int NUM_THREADS = 384;     // warpgroup 0: TMA, warpgroups 1..2: MMA (rows 0..63 / 64..127); warps 4..7 epilogue
 constexpr int BLOCK_M = 128;
+constexpr int MC_THREADS = 128 + 8 * 32;   // warpgroup 0 setup, warps 4.. MMA + cell (two warpgroups, one per half)
 
 struct Params {
   const __nv_bfloat16* xproj;   // [Nimg*H, 2048]: [fw 1024 | bw 1024 (rows reversed by length)], permuted columns
@@ -45,7 +30,6 @@ struct Params {
   // training only (nullptr for inference): activations the backward recurrence needs
   __nv_bfloat16* gates;         // post-activation gates i,j,f,o, coalesced per batch tile: layout in common.cuh (lstm_gate_off)
   float* csave;                 // cell state after the step (lstm_c_off)
-  int swap_ls;                  // debug (CRNN_LSTM_SWAPLS=1): exchange the LBO/SBO fields of the no-swizzle A descriptor
   long long* trace;             // debug (CRNN_LSTM_TRACE=1): clock64 stamps [CTA 0 / 5][warpgroup slot 0 / 1][steps 8..11][16 events]
 };
 
@@ -55,7 +39,6 @@ struct Params {
     if (p.trace != nullptr && lane == 0 && s >= 8 && s < 12 && (blockIdx.x == 0 || blockIdx.x == 5))    \
       p.trace[((((blockIdx.x ? 1 : 0) * 2 + (wg)) * 4 + (s - 8)) * 16) + (ev)] = clock64();             \
   } while (0)
-#define LSTM_TRACE(ev) LSTM_TRACE_WG(0, ev)
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
@@ -64,201 +47,10 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 }
 __device__ __forceinline__ void cluster_arrive_release() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait_acquire() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-
-template <int CS>
-struct Cfg {
-  static constexpr int UPC = 256 / CS;          // hidden units per CTA
-  static constexpr int NCOLS = 4 * UPC;         // gate columns per CTA
-  static constexpr int B_BYTES = 4 * NCOLS * 128;   // 4 K-blocks x [NCOLS rows x 128 B]
-  static constexpr int A_BYTES = 4 * BLOCK_M * 128; // 4 K-blocks x [128 rows x 128 B]
-  static constexpr int ACC_OFFSET = A_BYTES + B_BYTES;    // staged accumulators [128 rows][NCOLS] f32
-  static constexpr int BAR_OFFSET = ACC_OFFSET + BLOCK_M * NCOLS * 4;
-  static constexpr int SMEM_BYTES = BAR_OFFSET + 128 + 1024;
-};
-
-template <int CS>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-lstm_persistent_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmW, const Params p) {
-  static_assert(CS == 8, "register budget of the epilogue is sized for 32 units per CTA");
-  using C = Cfg<CS>;
-  constexpr int UPC = C::UPC, NCOLS = C::NCOLS;
-  constexpr int HALF = UPC / 2;                 // units processed per epilogue pass (register budget)
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + C::A_BYTES;
-  uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + C::BAR_OFFSET);   // [4] one per K-block
-  uint64_t* b_full = a_full + 4;
-  float* acc_tile = reinterpret_cast<float*>(smem + C::ACC_OFFSET);
-
-  const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int rank = (int)cluster_ctarank();
-  const int unit = blockIdx.x / CS;                   // (dir, batch tile)
-  const int dir = unit / p.tiles_per_dir;
-  const int tile = unit - dir * p.tiles_per_dir;
-
-  if (warp_idx == 0 && lane == 0) {
-    ptx::prefetch_tmap(&tmH);
-    ptx::prefetch_tmap(&tmW);
-    for (int i = 0; i < 4; ++i) ptx::mbar_init(&a_full[i], 1);
-    ptx::mbar_init(b_full, 1);
-    ptx::fence_barrier_init();
-  }
-  __syncthreads();
-
-  // resident recurrent weights: rows [dir*1024 + rank*NCOLS, +NCOLS) of Bh [2048, 256]
-  if (warp_idx == 0 && lane == 0) {
-    ptx::mbar_arrive_expect_tx(b_full, C::B_BYTES);
-    for (int kb = 0; kb < 4; ++kb)
-      ptx::tma_load_2d(&tmW, b_full, smem_b + kb * NCOLS * 128, kb * 64, dir * 1024 + rank * NCOLS);
-  }
-
-  // ---- per-thread epilogue state (warps 4..7): one sample row, UPC units, cell state in registers
-  const int q = warp_idx & 3;
-  const int row = q * 32 + lane;
-  const int n = tile * BLOCK_M + row;
-  const bool is_epi = warp_idx >= 4 && warp_idx < 8;
-  const bool okn = is_epi && (n < p.Nimg);
-  const int len = okn ? min(max(__ldg(p.seq_len + n), 0), p.T) : 0;
-  float cst[UPC];
-#pragma unroll
-  for (int i = 0; i < UPC; ++i) cst[i] = 0.f;
-
-  if (warp_idx < 4) ptx::setmaxnreg_dec<40>();
-  else ptx::setmaxnreg_inc<232>();
-  if (warp_idx >= 4) ptx::mbar_wait(b_full, 0);      // W_h slice resident before the first MMA / exit
-
-  for (int s = 0; s < p.T; ++s) {
-    if (warp_idx < 4) {
-      LSTM_TRACE(0);
-      if (warp_idx == 0 && lane < 4 && s > 0) {        // one lane per K-block: the four TMA issues overlap instead of serialising
-        fence_proxy_async_all();
-        const int hrow = ((s & 1) * 2 + dir) * p.Npad + tile * BLOCK_M;
-        ptx::mbar_arrive_expect_tx(&a_full[lane], BLOCK_M * 128);
-        ptx::tma_load_2d(&tmH, &a_full[lane], smem_a + lane * BLOCK_M * 128, lane * 64, hrow);
-      }
-      LSTM_TRACE(1);
-      __syncwarp();
-    } else {
-      const bool active = s < len;
-      const int t = active ? (dir ? (len - 1 - s) : s) : s;
-      // prefetch this step's input projection (row n, step s; bw rows were stored reversed by the projection GEMM)
-      uint4 xp[UPC / 2];                                   // 4 gates x UPC bf16 = UPC/2 x 16 B
-      if (active) {
-        const uint4* src = reinterpret_cast<const uint4*>(p.xproj + ((size_t)n * p.H + s) * 2048 + dir * 1024 + rank * NCOLS);
-#pragma unroll
-        for (int i = 0; i < UPC / 2; ++i) xp[i] = __ldg(src + i);
-      }
-      if (warp_idx == 4) LSTM_TRACE(5);
-      if (s > 0) {
-        // ===================== MMA: both warpgroups, rows wgi*64 .. =====================
-        const int wgi = (warp_idx >> 2) - 1;
-        const uint32_t ph = (s - 1) & 1;
-        float d[NCOLS / 2];
-        for (int kb = 0; kb < 4; ++kb) {
-          ptx::mbar_wait(&a_full[kb], ph);
-          if (kb == 0 && warp_idx == 4) LSTM_TRACE(2);
-          if (kb == 3 && warp_idx == 4) LSTM_TRACE(3);
-          const uint64_t a_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_a + kb * BLOCK_M * 128 + wgi * 64 * 128));
-          const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_b + kb * NCOLS * 128));
-          wg::fence();
-#pragma unroll
-          for (int k = 0; k < 4; ++k) wg::mma_bf16<NCOLS>(d, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
-          wg::commit();
-        }
-        wg::wait<0>();
-        wg::fence_operand(d);
-        if (warp_idx == 4) LSTM_TRACE(4);
-        ptx::acc_store<NCOLS, NCOLS>(acc_tile, d, wgi * 64);
-        ptx::bar_sync(1, 256);
-      }
-      if (warp_idx == 4) LSTM_TRACE(6);
-      __nv_bfloat16* hn = p.h_state + ((size_t)(((s + 1) & 1) * 2 + dir) * p.Npad + n) * 256 + rank * UPC;
-      __nv_bfloat16* lo = p.lstm_out + ((size_t)n * p.H + t) * 512 + dir * 256 + rank * UPC;
-      const uint32_t* xw = reinterpret_cast<const uint32_t*>(xp);    // gate g, unit u -> bf16 index g*UPC + u
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int u0 = hh * HALF;
-        uint32_t gi[HALF], gj[HALF], gf[HALF], go[HALF];
-        if (s > 0 && is_epi) {
-          ptx::acc_ld<NCOLS, HALF>(acc_tile, row, 0 * UPC + u0, gi);
-          ptx::acc_ld<NCOLS, HALF>(acc_tile, row, 1 * UPC + u0, gj);
-          ptx::acc_ld<NCOLS, HALF>(acc_tile, row, 2 * UPC + u0, gf);
-          ptx::acc_ld<NCOLS, HALF>(acc_tile, row, 3 * UPC + u0, go);
-          if (warp_idx == 4 && hh == 0) LSTM_TRACE(7);
-        } else {
-#pragma unroll
-          for (int i = 0; i < HALF; ++i) { gi[i] = 0u; gj[i] = 0u; gf[i] = 0u; go[i] = 0u; }
-        }
-        uint32_t hp[HALF / 2];
-        if (active) {
-          float hv[HALF];
-#pragma unroll
-          for (int i = 0; i < HALF; ++i) {
-            const int u = u0 + i;
-            const uint32_t wi = xw[(0 * UPC + u) >> 1], wj = xw[(1 * UPC + u) >> 1], wf = xw[(2 * UPC + u) >> 1], wo = xw[(3 * UPC + u) >> 1];
-            const float zi = __uint_as_float(gi[i]) + ((u & 1) ? ptx::bf16_hi(wi) : ptx::bf16_lo(wi));
-            const float zj = __uint_as_float(gj[i]) + ((u & 1) ? ptx::bf16_hi(wj) : ptx::bf16_lo(wj));
-            const float zf = __uint_as_float(gf[i]) + ((u & 1) ? ptx::bf16_hi(wf) : ptx::bf16_lo(wf));
-            const float zo = __uint_as_float(go[i]) + ((u & 1) ? ptx::bf16_hi(wo) : ptx::bf16_lo(wo));
-            const float ai = ptx::fast_sigmoid(zi), aj = ptx::fast_tanh(zj), af = ptx::fast_sigmoid(zf), ao = ptx::fast_sigmoid(zo);
-            const float c = af * cst[u] + ai * aj;                 // forget_bias (+1.0) is folded into the projected bias
-            cst[u] = c;
-            hv[i] = ao * ptx::fast_tanh(c);
-            if (p.gates != nullptr) {                              // reuse the (now dead) accumulator registers as staging
-              gi[i] = __float_as_uint(ai); gj[i] = __float_as_uint(aj); gf[i] = __float_as_uint(af); go[i] = __float_as_uint(ao);
-            }
-          }
-          if (p.gates != nullptr) {
-            const size_t dts = (size_t)unit * p.T + s;                  // coalesced saved-state layout, common.cuh
-            __nv_bfloat16* gs = p.gates + lstm_gate_off(dts, 0, rank * UPC + u0, row);
-            float* cs = p.csave + lstm_c_off(dts, rank * UPC + u0, row);
-#pragma unroll
-            for (int i = 0; i < HALF; i += 8) {
-              *reinterpret_cast<uint4*>(gs + 0 * LSTM_GATE_STRIDE + (i >> 3) * LSTM_GCHUNK_STRIDE) = make_uint4(ptx::pack_bf16x2(__uint_as_float(gi[i]), __uint_as_float(gi[i + 1])), ptx::pack_bf16x2(__uint_as_float(gi[i + 2]), __uint_as_float(gi[i + 3])), ptx::pack_bf16x2(__uint_as_float(gi[i + 4]), __uint_as_float(gi[i + 5])), ptx::pack_bf16x2(__uint_as_float(gi[i + 6]), __uint_as_float(gi[i + 7])));
-              *reinterpret_cast<uint4*>(gs + 1 * LSTM_GATE_STRIDE + (i >> 3) * LSTM_GCHUNK_STRIDE) = make_uint4(ptx::pack_bf16x2(__uint_as_float(gj[i]), __uint_as_float(gj[i + 1])), ptx::pack_bf16x2(__uint_as_float(gj[i + 2]), __uint_as_float(gj[i + 3])), ptx::pack_bf16x2(__uint_as_float(gj[i + 4]), __uint_as_float(gj[i + 5])), ptx::pack_bf16x2(__uint_as_float(gj[i + 6]), __uint_as_float(gj[i + 7])));
-              *reinterpret_cast<uint4*>(gs + 2 * LSTM_GATE_STRIDE + (i >> 3) * LSTM_GCHUNK_STRIDE) = make_uint4(ptx::pack_bf16x2(__uint_as_float(gf[i]), __uint_as_float(gf[i + 1])), ptx::pack_bf16x2(__uint_as_float(gf[i + 2]), __uint_as_float(gf[i + 3])), ptx::pack_bf16x2(__uint_as_float(gf[i + 4]), __uint_as_float(gf[i + 5])), ptx::pack_bf16x2(__uint_as_float(gf[i + 6]), __uint_as_float(gf[i + 7])));
-              *reinterpret_cast<uint4*>(gs + 3 * LSTM_GATE_STRIDE + (i >> 3) * LSTM_GCHUNK_STRIDE) = make_uint4(ptx::pack_bf16x2(__uint_as_float(go[i]), __uint_as_float(go[i + 1])), ptx::pack_bf16x2(__uint_as_float(go[i + 2]), __uint_as_float(go[i + 3])), ptx::pack_bf16x2(__uint_as_float(go[i + 4]), __uint_as_float(go[i + 5])), ptx::pack_bf16x2(__uint_as_float(go[i + 6]), __uint_as_float(go[i + 7])));
-            }
-#pragma unroll
-            for (int i = 0; i < HALF; i += 4)
-              *reinterpret_cast<float4*>(cs + (i >> 2) * LSTM_CCHUNK_STRIDE) = make_float4(cst[u0 + i], cst[u0 + i + 1], cst[u0 + i + 2], cst[u0 + i + 3]);
-          }
-#pragma unroll
-          for (int i = 0; i < HALF / 2; ++i) hp[i] = ptx::pack_bf16x2(hv[2 * i], hv[2 * i + 1]);
-        } else {
-#pragma unroll
-          for (int i = 0; i < HALF / 2; ++i) hp[i] = 0u;     // zero output past sequence_length
-        }
-        if (okn) {
-#pragma unroll
-          for (int i = 0; i < HALF / 2; i += 4) {
-            const uint4 v = make_uint4(hp[i], hp[i + 1], hp[i + 2], hp[i + 3]);
-            *reinterpret_cast<uint4*>(hn + u0 + 2 * i) = v;
-            *reinterpret_cast<uint4*>(lo + u0 + 2 * i) = v;
-          }
-        }
-      }
-      // make this thread's h stores visible to the async proxy (TMA loads of the next step) of the whole cluster
-      if (warp_idx == 4) LSTM_TRACE(8);
-      fence_proxy_async_all();
-      if (warp_idx == 4) LSTM_TRACE(9);
-    }
-    cluster_arrive_release();
-    if (warp_idx == 4) LSTM_TRACE(10);
-    cluster_wait_acquire();
-    if (warp_idx == 4) LSTM_TRACE(11);
-  }
-}
-
 
 // ---------------------------------------------------------------------------------------------------------------------------
-// v2: the same recurrence WITHOUT a cluster barrier (and without fence.proxy.async + a 64 KB TMA fetch per CTA) on the
-// per-step critical path.  A step of the v1 kernel above serialises a producer-side fence.proxy.async, a 64 KB TMA fetch, the
-// MMA, the cell epilogue, an epilogue-side fence.proxy.async and a barrier.cluster arrive(release)+wait (CRNN_LSTM_TRACE=1 prints
-// the clock64 timeline).
+// The recurrence without a cluster barrier (and without fence.proxy.async + a 64 KB TMA fetch of h per CTA) on the per-step
+// critical path (CRNN_LSTM_TRACE=1 prints the clock64 timeline of a few steps):
 //
 //   * rows of a batch tile never interact, so the two MMA warpgroups run two INDEPENDENT recurrences, warpgroup `wgi` over rows
 //     64*wgi .. 64*wgi+63 (a "half"): each half has its own A buffers, mbarriers, named barrier and exchange, and never waits
@@ -269,23 +61,14 @@ lstm_persistent_kernel(const __grid_constant__ CUtensorMap tmH, const __grid_con
 //   * the cell runs on the wgmma accumulator fragment itself (wgmma.cuh): with the columns of Bh ordered [i|j|f|o] x 32 units,
 //     a thread's m64n128 fragment holds all four gates of units 8k + 2(l%4) + {0,1} (k = 0..3) for rows 16w + l/4 and +8;
 //     the cell state of those 16 cells stays in registers for all T steps.  No accumulator staging, no barrier before the cell.
-//   * each thread stores its h_t words (bf16 pairs) into the half's slice, then
-//       MODE ds: straight into this CTA's own copy of the next A buffer (st.shared), then 7 bulk copies
-//                shared::cta -> shared::cluster push the slice into the peers' A buffers and credit THEIR mbarriers
-//       MODE mc: into a private 4 KB global buffer, then one bulk copy global -> shared::cluster with cluster MULTICAST
-//                lands it in all 8 CTAs (L2 is read once per slice instead of 8 times)
-//       MODE ms / gx: below
+//   * each thread stores its h_t words (bf16 pairs) straight into this CTA's own copy of the next A buffer (st.shared); one
+//     lane then bulk-stores the slice to global memory (L2) and, once written, multicasts it from there into the 7 peers' A
+//     buffers, crediting THEIR mbarriers: no generic-proxy global stores, hence no full fence.proxy.async on the critical path
 //   * the MMA warpgroup of each half waits on its own mbarrier (8 slices) and goes; nobody waits for a cluster barrier
 //   * A is double buffered: a slice of h_t can only be sent after its sender saw h_{t-1} from every CTA, i.e. after every CTA's
 //     MMA of step t-1 of the same half (the last reader of that buffer) has completed -- causality replaces a "buffer free"
 //     handshake.  A half runs and exchanges all T steps even when none of its rows is valid: its peers wait for its slices.
-// Global exchange buffer (modes mc, ms, gx): p.h_state viewed as [2 bufs][2*tiles_per_dir units][2 halves][8 ranks][4 KB].
-// EW = 8 epilogue warps = the two MMA warpgroups.
-template <int EW>
-struct McThreads {
-  static constexpr int EPI = EW * 32;
-  static constexpr int ALL = 128 + EPI;      // warpgroup 0 setup, warps 4.. MMA + cell (two warpgroups, one per half)
-};
+// Global exchange buffer: p.h_state viewed as [2 bufs][2*tiles_per_dir units][2 halves][8 ranks][4 KB].
 
 template <int CS>
 struct CfgMc {
@@ -300,27 +83,14 @@ struct CfgMc {
   static constexpr int SMEM_BYTES = BAR_OFFSET + 128 + 1024;
 };
 
-__device__ __forceinline__ void bulk_copy_s2s_cluster(uint32_t dst_cluster_addr, const void* src_smem, uint32_t bytes,
-                                                      uint32_t bar_cluster_addr) {
-  asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_cluster_addr),
-               "r"(ptx::smem_u32(src_smem)), "r"(bytes), "r"(bar_cluster_addr)
-               : "memory");
-}
-
-// MODE: 0 = global slice + multicast ("mc"), 1 = smem -> peer smem pushes ("ds"), 2 = smem slice -> bulk store to global ->
-// multicast to the 7 peers ("ms": no generic-proxy global stores, hence no full fence.proxy.async on the critical path),
-// 3 = generic proxy only ("gx"): st.global slice -> release.cluster arrive on every peer's mbarrier -> acquire.cluster wait ->
-// the half's 4 warps copy its 32 KB h image L2 -> smem with ld.global.cg / st.shared (the exchange the K-split BPTT uses)
-template <int CS, int MODE, int EW>
-__global__ void __launch_bounds__(McThreads<EW>::ALL, 1)
+template <int CS>
+__global__ void __launch_bounds__(MC_THREADS, 1)
 lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
   static_assert(CS == 8, "8 CTAs x 32 units");
   using C = CfgMc<CS>;
   constexpr int UPC = C::UPC, NCOLS = C::NCOLS;
-  static_assert(EW == 8, "epilogue warps = the two MMA warpgroups");
   static_assert(NCOLS == 128, "fragment column group j = gate j/4, units 8(j%4) ..: one m64n128 product per half and step");
-  constexpr bool DS = (MODE == 1), MS = (MODE == 2), GX = (MODE == 3), LOCAL = DS || MS;   // LOCAL: own slice written in place
-  constexpr uint32_t FILL_TX = LOCAL ? (CS - 1) * C::SLICE_BYTES : C::HALF_A_BYTES;
+  constexpr uint32_t FILL_TX = (CS - 1) * C::SLICE_BYTES;     // the 7 peers' slices; the own slice is written in place
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);   // offset arithmetic keeps the shared address space (STS)
@@ -328,7 +98,6 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
   uint8_t* smem_b = smem + 2 * C::A_BYTES;
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + C::BAR_OFFSET);   // [2 halves][2 bufs]
   uint64_t* b_full = a_full + 4;
-  uint64_t* part_ready = b_full + 1;                      // [2 halves][2 bufs] GX: the 8 CTAs' slices of one half's h buffer are in L2
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rank = (int)cluster_ctarank();
@@ -338,17 +107,14 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
 
   if (warp_idx == 0 && lane == 0) {
     ptx::prefetch_tmap(&tmW);
-    // DS / MS: one arrival arms the byte count (MMA warpgroup), the other says "the local slice is in place" (exchange lane)
-    for (int i = 0; i < 4; ++i) {
-      ptx::mbar_init(&part_ready[i], CS);
-      ptx::mbar_init(&a_full[i], GX ? 128 : LOCAL ? 2 : 1);     // GX: every thread of the half copied its part of the image
-    }
+    // one arrival arms the byte count (MMA warpgroup), the other says "the local slice is in place" (exchange lane)
+    for (int i = 0; i < 4; ++i) ptx::mbar_init(&a_full[i], 2);
     ptx::mbar_init(b_full, 1);
     ptx::fence_barrier_init();
     // first fills of each half: buffer 1 receives h_0 (consumed at step 1), buffer 0 receives h_1 (consumed at step 2)
     for (int hf = 0; hf < 2; ++hf) {
-      if (!GX && p.T > 1) ptx::mbar_arrive_expect_tx(&a_full[2 * hf + 1], FILL_TX);
-      if (!GX && p.T > 2) ptx::mbar_arrive_expect_tx(&a_full[2 * hf + 0], FILL_TX);
+      if (p.T > 1) ptx::mbar_arrive_expect_tx(&a_full[2 * hf + 1], FILL_TX);
+      if (p.T > 2) ptx::mbar_arrive_expect_tx(&a_full[2 * hf + 0], FILL_TX);
     }
     ptx::mbar_arrive_expect_tx(b_full, C::B_BYTES);
     for (int kb = 0; kb < 4; ++kb)
@@ -381,7 +147,6 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
 #pragma unroll
       for (int k = 0; k < 4; ++k) { cst[rh][k][0] = 0.f; cst[rh][k][1] = 0.f; }
     uint64_t* my_full = a_full + 2 * wgi;
-    uint64_t* my_ready = part_ready + 2 * wgi;
     ptx::mbar_wait(b_full, 0);
     // this thread's 4-byte h words inside a half slice: K-chunk k (units 8k ..) at k*1024, row at 16 B per row, + 4 B per lane pair
     const uint32_t word_off = rr0 * 16 + q4 * 4;
@@ -426,12 +191,12 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
         ptx::mbar_wait(&my_full[b], ((s - 1) >> 1) & 1);
         if (w == 0) LSTM_TRACE_WG(wgi, 3);
         // next fill of this buffer is h_{s+1}, consumed at step s+2; its senders are all behind this wait (see header)
-        if (!GX && s + 2 < p.T && (threadIdx.x & 127) == 0) ptx::mbar_arrive_expect_tx(&my_full[b], FILL_TX);
+        if (s + 2 < p.T && (threadIdx.x & 127) == 0) ptx::mbar_arrive_expect_tx(&my_full[b], FILL_TX);
         const uint32_t a_base = ptx::smem_u32(smem_a + b * C::A_BYTES + wgi * C::HALF_A_BYTES);
         wg::fence();
 #pragma unroll
         for (int k = 0; k < 16; ++k) {
-          const uint64_t a_desc = p.swap_ls ? ptx::make_desc_k_nosw(a_base + k * 2048, 128, 1024) : ptx::make_desc_k_nosw(a_base + k * 2048, 1024, 128);
+          const uint64_t a_desc = ptx::make_desc_k_nosw(a_base + k * 2048, 1024, 128);
           const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_b + (k >> 2) * NCOLS * 128)) + 2 * (k & 3);
           wg::mma_bf16<NCOLS>(d, a_desc, b_desc, k != 0);
         }
@@ -475,58 +240,26 @@ lstm_mc_kernel(const __grid_constant__ CUtensorMap tmW, const Params p) {
         const int nb = (s + 1) & 1;
         uint8_t* my_slice = smem_a + nb * C::A_BYTES + wgi * C::HALF_A_BYTES + rank * C::SLICE_BYTES;
         uint8_t* hx_slice = hx_half + (size_t)nb * hx_buf_stride + rank * C::SLICE_BYTES;
-        // a warp's 4-byte stores cover 8 rows x 16 B of one K-chunk: conflict-free in shared memory, 128 B contiguous in global
-        uint8_t* dst = (LOCAL ? my_slice : hx_slice) + word_off;
+        // a warp's 4-byte stores cover 8 rows x 16 B of one K-chunk: conflict-free in shared memory
+        uint8_t* dst = my_slice + word_off;
 #pragma unroll
         for (int rh = 0; rh < 2; ++rh)
 #pragma unroll
           for (int k = 0; k < 4; ++k) *reinterpret_cast<uint32_t*>(dst + k * 1024 + rh * 128) = hw[rh][k];
-        if (LOCAL) ptx::fence_proxy_async_smem();           // generic-proxy smem writes -> async proxy (bulk copies, wgmma)
-        else if (!GX) fence_proxy_async_all();              // generic-proxy global writes -> async proxy (bulk copy)
+        ptx::fence_proxy_async_smem();                      // generic-proxy smem writes -> async proxy (bulk copies, wgmma)
         if (w == 0) LSTM_TRACE_WG(wgi, 8);
         if (wgi == 0) ptx::bar_sync(1, 128);                // the half's slice is complete (named barrier 1 / 2 per half)
         else ptx::bar_sync(2, 128);
         if (w == 0) {
-          if (DS) {
-            if (lane < CS) {
-              if (lane == rank) {
-                ptx::mbar_arrive(&my_full[nb]);
-              } else {
-                const uint32_t dst_peer = ptx::mapa(ptx::smem_u32(my_slice), (uint32_t)lane);
-                const uint32_t bar = ptx::mapa(ptx::smem_u32(&my_full[nb]), (uint32_t)lane);
-                bulk_copy_s2s_cluster(dst_peer, my_slice, C::SLICE_BYTES, bar);
-              }
-            }
-          } else if (MS) {
-            if (lane == 0) {
-              ptx::bulk_store_1d(hx_slice, my_slice, C::SLICE_BYTES);          // async proxy: smem -> global (L2)
-              ptx::bulk_commit();
-              asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");       // writes performed, not just the smem reads
-              ptx::bulk_load_1d_mc(my_slice, hx_slice, C::SLICE_BYTES, &my_full[nb], (uint16_t)(((1u << CS) - 1) & ~(1u << rank)));
-              ptx::mbar_arrive(&my_full[nb]);                                 // the local slice is already in place
-            }
-          } else if (GX) {
-            // cumulative over the barrier above: the release covers every thread's slice stores of this half
-            if (lane < CS) ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&my_ready[nb]), (uint32_t)lane));
-          } else if (lane == 0) {
-            ptx::bulk_load_1d_mc(my_slice, hx_slice, C::SLICE_BYTES, &my_full[nb], (uint16_t)((1u << CS) - 1));
+          if (lane == 0) {
+            ptx::bulk_store_1d(hx_slice, my_slice, C::SLICE_BYTES);          // async proxy: smem -> global (L2)
+            ptx::bulk_commit();
+            asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");       // writes performed, not just the smem reads
+            ptx::bulk_load_1d_mc(my_slice, hx_slice, C::SLICE_BYTES, &my_full[nb], (uint16_t)(((1u << CS) - 1) & ~(1u << rank)));
+            ptx::mbar_arrive(&my_full[nb]);                                 // the local slice is already in place
           }
           __syncwarp();
           LSTM_TRACE_WG(wgi, 9);
-        }
-        if (GX) {
-          // h_t of the half = the cluster's 8 contiguous slices = exactly the half's A operand image: 32 KB, 16 B per thread per pass
-          ptx::mbar_wait_cluster(&my_ready[nb], (uint32_t)(s >> 1) & 1u);
-          const uint8_t* g = hx_half + (size_t)nb * hx_buf_stride;
-          uint8_t* a = smem_a + nb * C::A_BYTES + wgi * C::HALF_A_BYTES;
-          const int et = threadIdx.x & 127;
-          uint4 v[C::HALF_A_BYTES / 16 / 128];
-#pragma unroll
-          for (int k = 0; k < C::HALF_A_BYTES / 16 / 128; ++k) v[k] = __ldcg(reinterpret_cast<const uint4*>(g) + k * 128 + et);
-#pragma unroll
-          for (int k = 0; k < C::HALF_A_BYTES / 16 / 128; ++k) *(reinterpret_cast<uint4*>(a) + k * 128 + et) = v[k];
-          ptx::fence_proxy_async_smem();
-          ptx::mbar_arrive(&my_full[nb]);
         }
       }
 #pragma unroll

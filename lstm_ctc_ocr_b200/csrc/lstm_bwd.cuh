@@ -6,12 +6,8 @@
 //   dh = d_out[t] + dz_{s+1} W_h^T          dc = dc_{s+1->s} + dh * o * (1 - tanh(c_s)^2)
 //   do = dh * tanh(c_s) * o(1-o)   di = dc * j * i(1-i)   dj = dc * i * (1-j^2)   df = dc * c_{s-1} * f(1-f)
 //   dc_{s->s-1} = dc * f
-// Cluster of 8 CTAs per (direction, 128-sample tile); CTA `rank` owns 32 hidden units: it keeps dc for them in
-// registers, holds W_h[units, all 1024 gate columns] (64 KB bf16, K-major over gates) resident in shared memory, and per
-// step computes dh_rec[128 x 32] = dz_{s+1}[128 x 1024] * W_h^T on tensor cores (one warpgroup, 2 x 64 wgmma 64x32x16), streaming
-// dz_{s+1} (written to global/L2 by the whole cluster one step earlier) through a 6-stage TMA ring.  The tile is identical
-// for the 8 CTAs of a cluster, so each K-block is read from L2 ONCE and TMA-multicast into all 8 shared memories.
-// (The step is bound by its serial latency chain, not by MMA count or exchange volume.)
+// Cluster of 8 CTAs per (direction, 128-sample tile); CTA `rank` owns 32 hidden units and keeps dc for them in registers.
+// The recurrent product is split along K and NOTHING but generic-proxy traffic passes between CTAs (details above the kernel).
 // Outputs: dz for every (sample, frame) in FRAME order (`dz_all`, consumed by the dW_x / dW_h / dx GEMMs).
 #pragma once
 #include <cuda.h>
@@ -22,22 +18,14 @@
 
 namespace lstm_bwd {
 
-constexpr int NUM_THREADS = 256;               // warpgroup 0: TMA (warp 0), warpgroup 1: MMA + epilogue
 constexpr int BLOCK_M = 128;
 constexpr int CS = 8;
 constexpr int UPC = 32;
-constexpr int STAGES = 6;
-constexpr int B_BYTES = 16 * UPC * 128;          // 16 K-blocks x [32 rows x 128 B] = 64 KB
-constexpr int A_STAGE = BLOCK_M * 128;           // 16 KB
-constexpr int ACC_OFFSET = B_BYTES + STAGES * A_STAGE;   // staged accumulators [128 rows][32] f32
-constexpr int BAR_OFFSET = ACC_OFFSET + BLOCK_M * UPC * 4;
-constexpr int SMEM_BYTES = BAR_OFFSET + 256 + 1024;
 
 struct Params {
   const __nv_bfloat16* gates;     // saved by the forward kernel, coalesced per batch tile (common.cuh: lstm_gate_off)
   const float* csave;             // (common.cuh: lstm_c_off)
   const __nv_bfloat16* d_out;     // [Nimg*H, 512] gradient w.r.t. the LSTM output (frame order)
-  __nv_bfloat16* dz_state;        // [2 bufs][2 dirs][Npad][1024] step-order exchange buffer
   __nv_bfloat16* dz_all;          // [Nimg*H, 2048] frame order, permuted gate columns, [fw | bw]
   const int* seq_len;
   int Nimg, Npad, H, T, tiles_per_dir;
@@ -52,194 +40,10 @@ __device__ __forceinline__ void unpack8(const uint4 q, float* v) {
   v[4] = ptx::bf16_lo(q.z); v[5] = ptx::bf16_hi(q.z); v[6] = ptx::bf16_lo(q.w); v[7] = ptx::bf16_hi(q.w);
 }
 
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constant__ CUtensorMap tmW, const Params p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_b = smem;
-  uint8_t* smem_a = smem + B_BYTES;
-  uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + BAR_OFFSET);
-  uint64_t* a_empty = a_full + STAGES;
-  uint64_t* b_full = a_empty + STAGES;
-  float* acc_tile = reinterpret_cast<float*>(smem + ACC_OFFSET);
-
-  const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int rank = (int)lstm::cluster_ctarank();
-  const int unit = blockIdx.x / CS;
-  const int dir = unit / p.tiles_per_dir;
-  const int tile = unit - dir * p.tiles_per_dir;
-
-  if (warp_idx == 0 && lane == 0) {
-    ptx::prefetch_tmap(&tmDz);
-    ptx::prefetch_tmap(&tmW);
-    for (int i = 0; i < STAGES; ++i) { ptx::mbar_init(&a_full[i], 1); ptx::mbar_init(&a_empty[i], CS); }   // slot free = all 8 CTAs consumed it
-    ptx::mbar_init(b_full, 1);
-    ptx::fence_barrier_init();
-  }
-  __syncthreads();
-
-  if (warp_idx == 0 && lane == 0) {      // resident W_h rows [dir*256 + rank*32, +32) x 1024 gate columns
-    ptx::mbar_arrive_expect_tx(b_full, B_BYTES);
-    for (int kb = 0; kb < 16; ++kb) ptx::tma_load_2d(&tmW, b_full, smem_b + kb * UPC * 128, kb * 64, dir * 256 + rank * UPC);
-  }
-
-  const int q = warp_idx & 3;
-  const int row = q * 32 + lane;
-  const int n = tile * BLOCK_M + row;
-  const bool is_epi = warp_idx >= 4;
-  const bool okn = is_epi && (n < p.Nimg);
-  const int len = okn ? min(max(__ldg(p.seq_len + n), 0), p.T) : 0;
-  float dcr[UPC];
-#pragma unroll
-  for (int i = 0; i < UPC; ++i) dcr[i] = 0.f;
-
-  if (is_epi) ptx::mbar_wait(b_full, 0);
-
-  uint32_t prod_parity = 0;  // producer lane l: parity of ring slot l (flips on every use of that slot)
-  uint32_t mma_parity = 0;   // MMA threads: bit s = parity of ring slot s
-
-  for (int s = p.T - 1; s >= 0; --s) {
-    const bool has_rec = (s < p.T - 1);
-    if (warp_idx < 4) {
-      // K-block kb of every step lives in ring slot kb % STAGES.  Lanes 0..STAGES-1 own one slot each and issue their
-      // K-blocks in lock-step (one SIMD cp.async.bulk.tensor per round instead of 16 serial single-thread issues).
-      if (warp_idx == 0 && lane < STAGES && has_rec) {
-        lstm::fence_proxy_async_all();
-        const int zrow = ((((s + 1) & 1) * 2 + dir) * p.Npad) + tile * BLOCK_M;
-        for (int kb = lane; kb < 16; kb += STAGES) {
-          // all 8 CTAs of the cluster need the SAME dz tile: CTA (kb % 8) loads K-block kb once and multicasts it; every
-          // CTA arms its own barrier.  a_empty[slot] counts the MMA commits of all 8 CTAs (multicast commit below).
-          ptx::mbar_wait(&a_empty[lane], prod_parity ^ 1);
-          ptx::mbar_arrive_expect_tx(&a_full[lane], A_STAGE);
-          if ((kb & (CS - 1)) == rank)
-            ptx::tma_load_2d_mc(&tmDz, &a_full[lane], smem_a + lane * A_STAGE, kb * 64, zrow, (uint16_t)0xFF);
-          prod_parity ^= 1;
-        }
-      }
-      __syncwarp();
-    } else {
-      const bool active = s < len;
-      const int t = active ? (dir ? (len - 1 - s) : s) : s;
-      const size_t dts = (size_t)unit * p.T + s;                    // coalesced saved-state layout, common.cuh
-      // The saved forward state of step s-1 (gates, c, c_prev, d_out: ~0.7 KB per thread, long evicted from L2) is pulled
-      // into L2 one step ahead so the dependent loads of the next iteration do not pay HBM latency on the serial chain.
-      if (s >= 1 && (s - 1) < len) {
-        const int tp = dir ? (len - s) : (s - 1);
-#pragma unroll
-        for (int g = 0; g < 4; ++g) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.gates + lstm_gate_off(dts - 1, g, rank * UPC, row)));
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(p.csave + lstm_c_off(dts - 1, rank * UPC, row)));
-        if (s >= 2) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.csave + lstm_c_off(dts - 2, rank * UPC, row)));
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(p.d_out + ((size_t)n * p.H + tp) * 512 + dir * 256 + rank * UPC));
-      }
-      if (has_rec) {
-        // dh_rec = dz_{s+1} * W_h^T: rows 0..63 and 64..127 as two accumulator sets of this warpgroup
-        float d0[UPC / 2], d1[UPC / 2];
-        int prev = -1;
-        for (int kb = 0; kb < 16; ++kb) {
-          const int slot = kb % STAGES;
-          ptx::mbar_wait(&a_full[slot], (mma_parity >> slot) & 1u);
-          mma_parity ^= (1u << slot);
-          const uint64_t a_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_a + slot * A_STAGE));
-          const uint64_t b_desc = ptx::make_desc_k_sw128(ptx::smem_u32(smem_b + kb * UPC * 128));
-          wg::fence();
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            wg::mma_bf16<UPC>(d0, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
-            wg::mma_bf16<UPC>(d1, a_desc + (64 * 128 >> 4) + 2 * k, b_desc + 2 * k, (kb | k) != 0);
-          }
-          wg::commit();
-          wg::wait<1>();
-          // the slot is free once every CTA of the cluster has consumed it: one release arrive on each CTA's a_empty
-          if (prev >= 0 && threadIdx.x == 128 + 0)
-            for (int r = 0; r < CS; ++r) ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&a_empty[prev]), (uint32_t)r));
-          prev = slot;
-        }
-        wg::wait<0>();
-        wg::fence_operand(d0);
-        wg::fence_operand(d1);
-        if (threadIdx.x == 128)
-          for (int r = 0; r < CS; ++r) ptx::mbar_arrive_cluster(ptx::mapa(ptx::smem_u32(&a_empty[prev]), (uint32_t)r));
-        ptx::acc_store<UPC, UPC>(acc_tile, d0, 0);
-        ptx::acc_store<UPC, UPC>(acc_tile, d1, 64);
-        ptx::bar_sync(1, 128);
-      }
-      __nv_bfloat16* zs = p.dz_state + ((size_t)(((s & 1) * 2 + dir) * p.Npad) + n) * 1024 + rank * 128;
-      __nv_bfloat16* za = p.dz_all + ((size_t)n * p.H + t) * 2048 + dir * 1024 + rank * 128;
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int u0 = hh * 16;
-        uint32_t acc[16];
-        if (has_rec) {
-          ptx::acc_ld<UPC, 16>(acc_tile, row, u0, acc);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) acc[i] = 0u;
-        }
-        float dzi[16], dzj[16], dzf[16], dzo[16];
-        if (active) {
-          const __nv_bfloat16* gs = p.gates + lstm_gate_off(dts, 0, rank * UPC + u0, row);
-          const float* cs = p.csave + lstm_c_off(dts, rank * UPC + u0, row);
-          const __nv_bfloat16* dout = p.d_out + ((size_t)n * p.H + t) * 512 + dir * 256 + rank * UPC + u0;
-          float gi[16], gj[16], gf[16], go[16], cc[16], cp[16], dh[16];
-#pragma unroll
-          for (int v = 0; v < 2; ++v) {
-            unpack8(__ldg(reinterpret_cast<const uint4*>(gs + 0 * LSTM_GATE_STRIDE + v * LSTM_GCHUNK_STRIDE)), gi + 8 * v);
-            unpack8(__ldg(reinterpret_cast<const uint4*>(gs + 1 * LSTM_GATE_STRIDE + v * LSTM_GCHUNK_STRIDE)), gj + 8 * v);
-            unpack8(__ldg(reinterpret_cast<const uint4*>(gs + 2 * LSTM_GATE_STRIDE + v * LSTM_GCHUNK_STRIDE)), gf + 8 * v);
-            unpack8(__ldg(reinterpret_cast<const uint4*>(gs + 3 * LSTM_GATE_STRIDE + v * LSTM_GCHUNK_STRIDE)), go + 8 * v);
-            unpack8(__ldg(reinterpret_cast<const uint4*>(dout) + v), dh + 8 * v);
-          }
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            const float4 a = __ldg(reinterpret_cast<const float4*>(cs + v * LSTM_CCHUNK_STRIDE));
-            cc[4 * v] = a.x; cc[4 * v + 1] = a.y; cc[4 * v + 2] = a.z; cc[4 * v + 3] = a.w;
-            const float4 b = (s > 0) ? __ldg(reinterpret_cast<const float4*>(cs - LSTM_CSTEP_STRIDE + v * LSTM_CCHUNK_STRIDE)) : make_float4(0.f, 0.f, 0.f, 0.f);
-            cp[4 * v] = b.x; cp[4 * v + 1] = b.y; cp[4 * v + 2] = b.z; cp[4 * v + 3] = b.w;
-          }
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float dht = dh[i] + __uint_as_float(acc[i]);
-            const float tc = ptx::fast_tanh(cc[i]);
-            const float dc = dcr[u0 + i] + dht * go[i] * (1.f - tc * tc);
-            dzo[i] = dht * tc * go[i] * (1.f - go[i]);
-            dzi[i] = dc * gj[i] * gi[i] * (1.f - gi[i]);
-            dzj[i] = dc * gi[i] * (1.f - gj[i] * gj[i]);
-            dzf[i] = dc * cp[i] * gf[i] * (1.f - gf[i]);
-            dcr[u0 + i] = dc * gf[i];
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) { dzi[i] = 0.f; dzj[i] = 0.f; dzf[i] = 0.f; dzo[i] = 0.f; }
-        }
-        if (okn) {
-#pragma unroll
-          for (int v = 0; v < 2; ++v) {
-            const uint4 qi = pack8(dzi + 8 * v), qj = pack8(dzj + 8 * v), qf = pack8(dzf + 8 * v), qo = pack8(dzo + 8 * v);
-            *(reinterpret_cast<uint4*>(zs + 0 * 32 + u0) + v) = qi;
-            *(reinterpret_cast<uint4*>(zs + 1 * 32 + u0) + v) = qj;
-            *(reinterpret_cast<uint4*>(zs + 2 * 32 + u0) + v) = qf;
-            *(reinterpret_cast<uint4*>(zs + 3 * 32 + u0) + v) = qo;
-            *(reinterpret_cast<uint4*>(za + 0 * 32 + u0) + v) = qi;
-            *(reinterpret_cast<uint4*>(za + 1 * 32 + u0) + v) = qj;
-            *(reinterpret_cast<uint4*>(za + 2 * 32 + u0) + v) = qf;
-            *(reinterpret_cast<uint4*>(za + 3 * 32 + u0) + v) = qo;
-          }
-        }
-      }
-      lstm::fence_proxy_async_all();
-    }
-    lstm::cluster_arrive_release();
-    lstm::cluster_wait_acquire();
-  }
-}
-
-
 // ---------------------------------------------------------------------------------------------------------------------------
-// v2 ("ks"): the same recurrence with the product split along K and NOTHING but generic-proxy traffic between CTAs.
-//
-// v1 above moves the whole dz_{s+1} tile (128 x 1024, 256 KB) into every CTA each step (multicast ring with cluster-wide slot
-// hand-shakes), issues MMAs of N = 32 only and pays two
-// fence.proxy.async and a cluster barrier per step.  Here CTA `rank` multiplies ONLY ITS OWN dz slice
+// The recurrence with the product split along K ("ks").  Moving the whole dz_{s+1} tile (128 x 1024, 256 KB) into every CTA
+// each step would mean MMAs of N = 32, a multicast ring with cluster-wide slot hand-shakes, two fence.proxy.async and a
+// cluster barrier per step.  Instead CTA `rank` multiplies ONLY ITS OWN dz slice
 // (128 x 128 gate columns, written by its own epilogue straight into shared memory as the no-swizzle A operand) with the
 // resident W_h[all 256 units, its 128 gate columns]: 8 wgmma of 64 x 256 x 16 per warpgroup give its partial dh for ALL units.  The
 // partials are exchanged all-to-all through L2 as bf16 (8 KB per (source, destination) pair): plain st.global, one

@@ -208,18 +208,6 @@ extern "C" int crnn_model_create(const crnn_config* cfg, crnn_model** out) {
     return crnn_fail(CRNN_UNSUPPORTED, "model_create: needs sm_90 (found sm_%d%d)", prop.major, prop.minor);
   }
   m->num_sms = prop.multiProcessorCount;
-  if (const char* e = getenv("CRNN_BPTT")) m->bptt_ks = std::string(e) != "ring";        // debug A/B switch
-  if (const char* e = getenv("CRNN_CONV1")) m->conv1_tc = std::string(e) != "simt";    // debug A/B switch
-  if (const char* e = getenv("CRNN_BN_FUSE")) m->bn_red_fused = std::string(e) != "0";            // debug A/B switch
-  if (const char* e = getenv("CRNN_RELU_FUSE")) m->relu_mask_fused = std::string(e) != "0";       // debug A/B switch
-  if (const char* e = getenv("CRNN_CONV1_WGRAD")) m->conv1_wgrad_tc = std::string(e) != "simt";  // debug A/B switch
-  if (const char* e = getenv("CRNN_CONV2_DGRAD")) m->conv2_dgrad_swap = std::string(e) != "old";   // debug A/B switch
-  if (const char* e = getenv("CRNN_CONV2_WGRAD")) m->conv2_wgrad_swap = std::string(e) != "old";   // debug A/B switch
-  if (const char* e = getenv("CRNN_CONV2")) m->conv2_swap = std::string(e) != "pos";    // debug A/B switch: "pos" = position-major gemm.cuh kernel
-  if (const char* e = getenv("CRNN_LSTM_IMPL")) {                                                      // debug A/B switch
-    m->lstm_upc = (std::string(e) == "step") ? 64 : 32;
-    m->lstm_mc = std::string(e) == "ds" ? 2 : std::string(e) == "mc" ? 1 : std::string(e) == "gx" ? 4 : (std::string(e) == "persistent" || std::string(e) == "step") ? 0 : 3;
-  }
 
   // one allocation for all derived operand copies
   const size_t nB[9] = {128 * 576, 256 * 1152, 256 * 2304, 512 * 2304, 512 * 4608, 512 * 2048, 2048 * 512, 2048 * 256, 64 * 512};
@@ -240,7 +228,6 @@ extern "C" int crnn_model_create(const crnn_config* cfg, crnn_model** out) {
   if (st == CRNN_OK) st = make_tmap_2d(&m->tB_c42, m->Bc42, 512, 4608, 4608, 256);
   if (st == CRNN_OK) st = make_tmap_2d(&m->tB_c5, m->Bc5, 512, 2048, 2048, 256);
   if (st == CRNN_OK) st = make_tmap_2d(&m->tB_x, m->Bx, 2048, 512, 512, 256);
-  if (st == CRNN_OK) st = make_tmap_2d(&m->tB_h, m->Bh, 2048, 256, 256, 256);
   if (st == CRNN_OK) st = make_tmap_2d(&m->tB_h128, m->Bh, 2048, 256, 256, 128);
   if (st == CRNN_OK) st = make_tmap_2d(&m->tB_l, m->Bl, 64, 512, 512, 64);
   if (st == CRNN_OK && cfg->compute_dtype == 4) st = fp8_create(m);
@@ -297,15 +284,15 @@ int prepare_weights(crnn_model* m, cudaStream_t st) {
   struct { const char* n; __nv_bfloat16* d; int R, C; } cv[6] = {
       {"conv2/weights", m->Bc2, 576, 128},    {"conv3_1/weights", m->Bc31, 1152, 256}, {"conv3_2/weights", m->Bc32, 2304, 256},
       {"conv4_1/weights", m->Bc41, 2304, 512}, {"conv4_2/weights", m->Bc42, 4608, 512}, {"conv5/weights", m->Bc5, 2048, 512}};
-  for (auto& c : cv) CRNN_TRY(launch_transpose_cast(m->P(c.n), c.R, c.C, c.C, c.d, c.R, 0, st));
+  for (auto& c : cv) CRNN_TRY(launch_transpose_cast(m->P(c.n), c.R, c.C, c.C, c.d, c.R, false, st));
   const char* dirs[2] = {"logits/bidirectional_rnn/fw/lstm_cell", "logits/bidirectional_rnn/bw/lstm_cell"};
   for (int d = 0; d < 2; ++d) {
     const float* w = m->P(std::string(dirs[d]) + "/weights");                 // [768,1024], rows [x(512); h(256)]
-    CRNN_TRY(launch_transpose_cast(w, 512, 1024, 1024, m->Bx + (size_t)d * 1024 * 512, 512, m->lstm_upc, st));
-    CRNN_TRY(launch_transpose_cast(w + 512 * 1024, 256, 1024, 1024, m->Bh + (size_t)d * 1024 * 256, 256, m->lstm_upc, st));
+    CRNN_TRY(launch_transpose_cast(w, 512, 1024, 1024, m->Bx + (size_t)d * 1024 * 512, 512, true, st));
+    CRNN_TRY(launch_transpose_cast(w + 512 * 1024, 256, 1024, 1024, m->Bh + (size_t)d * 1024 * 256, 256, true, st));
   }
-  CRNN_TRY(launch_lstm_bias_prep(m->P(std::string(dirs[0]) + "/biases"), m->P(std::string(dirs[1]) + "/biases"), m->xbias, m->lstm_upc, st));
-  CRNN_TRY(launch_transpose_cast(m->P("logits/weights"), 512, 64, 64, m->Bl, 512, 0, st));
+  CRNN_TRY(launch_lstm_bias_prep(m->P(std::string(dirs[0]) + "/biases"), m->P(std::string(dirs[1]) + "/biases"), m->xbias, st));
+  CRNN_TRY(launch_transpose_cast(m->P("logits/weights"), 512, 64, 64, m->Bl, 512, false, st));
   // L2 term depends only on the parameters: computed here, consumed by crnn_total_loss
   SumsqSegs segs;
   segs.n = 0;
@@ -341,7 +328,6 @@ size_t layout_plan(Plan& pl, int N, int W, uint8_t* base, bool train) {
   pl.xproj = (__nv_bfloat16*)take(n * h2 * 2048 * 2);
   pl.lstm_out = (__nv_bfloat16*)take(n * h2 * 512 * 2);
   pl.h_state = (__nv_bfloat16*)take((size_t)2 * 2 * pl.Npad * 256 * 2);
-  pl.c_state = (float*)take((size_t)2 * pl.Npad * 256 * 4);
   pl.stats = (double*)take(2 * 2 * 512 * 8);
   pl.bn = (float*)take(2 * 4 * 512 * 4);
   pl.train = train;
@@ -355,7 +341,6 @@ size_t layout_plan(Plan& pl, int N, int W, uint8_t* base, bool train) {
     pl.dl_rows = (__nv_bfloat16*)take(n * h2 * 64 * 2);
     pl.d_lstm_out = (__nv_bfloat16*)take(n * h2 * 512 * 2);
     pl.dz_all = (__nv_bfloat16*)take(n * h2 * 2048 * 2);
-    pl.dz_state = (__nv_bfloat16*)take((size_t)2 * 2 * pl.Npad * 1024 * 2);
     pl.bptt_x = (uint8_t*)take((size_t)2 * (2 * pl.Npad / 128) * 64 * 8192);
     pl.d_a5 = (__nv_bfloat16*)take(n * h2 * 512 * 2);
     pl.d_a4b = (__nv_bfloat16*)take(n * h2 * 2 * 512 * 2);
@@ -393,7 +378,6 @@ static int build_plan(crnn_model* m, int N, int W, void* ws, cudaStream_t st) {
   pl.ws = ws;
   pl.mg2 = (pl.H1 % 8) == 0; pl.mg3 = (pl.H2 % 16) == 0; pl.mg4 = (pl.H2 % 32) == 0;
   pl.wm2 = (pl.H1 % 4) == 0; pl.wm3 = (pl.H2 % 8) == 0; pl.wm4 = (pl.H2 % 16) == 0;
-  CRNN_TRY(make_tmap_nhwc(&pl.tA_c2, pl.a1, N, pl.H1, 16, 64, pl.mg2 ? 8 : 2));
   CRNN_TRY(make_tmap_nhwc(&pl.tA_c2s, pl.a1, N, pl.H1, 16, 64, 8));
   CRNN_TRY(make_tmap_nhwc(&pl.tA_c31, pl.a2, N, pl.H2, 8, 128, pl.mg3 ? 16 : 4));
   CRNN_TRY(make_tmap_nhwc(&pl.tA_c32, pl.a3, N, pl.H2, 8, 256, pl.mg3 ? 16 : 4));
@@ -402,9 +386,6 @@ static int build_plan(crnn_model* m, int N, int W, void* ws, cudaStream_t st) {
   // conv5 (2x2 VALID over [N,H2,2,512]): output (n,t) = rows n*H2+t and n*H2+t+1 of the [N*H2, 1024] view
   CRNN_TRY(make_tmap_2d(&pl.tA_c5, pl.a4b, (uint64_t)N * pl.H2, 1024, 1024, 128));
   CRNN_TRY(make_tmap_2d(&pl.tA_x, pl.a5, (uint64_t)N * pl.H2, 512, 512, 128));
-  for (int b = 0; b < 2; ++b)
-    CRNN_TRY(make_tmap_2d(&pl.tA_h[b], pl.h_state + (size_t)b * 2 * pl.Npad * 256, (uint64_t)2 * pl.Npad, 256, 256, 128));
-  CRNN_TRY(make_tmap_2d(&pl.tA_hall, pl.h_state, (uint64_t)4 * pl.Npad, 256, 256, 128));
   CRNN_TRY(make_tmap_2d(&pl.tA_l, pl.lstm_out, (uint64_t)N * pl.H2, 512, 512, 128));
   CRNN_TRY(make_tmap_nhwc(&pl.tO_c1, pl.a1, N, pl.H1, 16, 64, 4));               // conv1_tc_kernel's pooled warpgroup tile: 4 pooled rows
   CRNN_TRY(make_tmap_nhwc(&pl.tO_c2s, pl.a2, N, pl.H2, 8, 128, 8));             // conv2_swap_kernel's pooled tile: 8 pooled rows
@@ -421,12 +402,9 @@ static int build_plan(crnn_model* m, int N, int W, void* ws, cudaStream_t st) {
     CRNN_TRY(make_tmap_2d(&pl.tG_dl, pl.dl_rows, R, 64, 64, 128));
     CRNN_TRY(make_tmap_2d(&pl.tG_dz, pl.dz_all, R, 2048, 2048, 128));
     CRNN_TRY(make_tmap_2d(&pl.tG_da5, pl.d_a5, R, 512, 512, 128));
-    CRNN_TRY(make_tmap_2d(&pl.tG_dzstate, pl.dz_state, (uint64_t)4 * pl.Npad, 1024, 1024, 128));
     CRNN_TRY(make_tmap_nhwc(&pl.tG_p4b, pl.d_pre4b, N, pl.H2, 4, 512, pl.mg4 ? 32 : 8));
     CRNN_TRY(make_tmap_nhwc(&pl.tG_p4a, pl.d_pre4a, N, pl.H2, 4, 512, pl.mg4 ? 32 : 8));
     CRNN_TRY(make_tmap_nhwc(&pl.tG_p32, pl.d_pre32, N, pl.H2, 8, 256, pl.mg3 ? 16 : 4));
-    CRNN_TRY(make_tmap_nhwc(&pl.tG_p31, pl.d_pre31, N, pl.H2, 8, 256, pl.mg3 ? 16 : 4));
-    CRNN_TRY(make_tmap_nhwc(&pl.tG_p2, pl.d_pre2, N, pl.H1, 16, 128, pl.mg2 ? 8 : 2));
     CRNN_TRY(make_tmap_nhwc(&pl.tG_p2s, pl.d_pre2, N, pl.H1, 16, 128, 8));
     CRNN_TRY(make_tmap_nhwc(&pl.tG_p31s, pl.d_pre31, N, pl.H2, 8, 256, 16));
     CRNN_TRY(make_tmap_2d(&pl.tO_dlo, pl.d_lstm_out, R, 512, 512, 128));
@@ -555,7 +533,6 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     if (fp8 && !fp8_calibrated(m))
       return crnn_fail(CRNN_INVALID_VALUE, "forward: the fp8 model (compute_dtype 4) has no activation scales: calibration is missing "
                                            "(crnn_model_calibrate_fp8 or crnn_model_set_fp8_scales after the last parameter change)");
-    if (!m->conv2_swap) return crnn_fail(CRNN_UNSUPPORTED, "forward: the fp8 path writes a2 from conv2_swap_kernel (unset CRNN_CONV2)");
     if (m->dp_world > 1) return crnn_fail(CRNN_UNSUPPORTED, "forward: the fp8 path runs on one device (no data parallelism)");
     if (host_data != nullptr) {
       // copy-then-compute, as the f32-class paths do
@@ -597,7 +574,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
 
   // ---- front end, per image range [n0, n0 + nc): conv1+pool1, conv2+pool2, conv3_1, conv3_2+pool (all batch-independent)
   const int sb3 = (H2 + 3) / 4;                      // 32-position sub-boxes per image of the conv3 layers (Wd = 8 -> 4 H rows)
-  const int sb2 = (H1 + 1) / 2;                      // conv2 through gemm.cuh (Wd = 16 -> 2 H rows)
+  const int sb2 = (H1 + 1) / 2;                      // the same at conv2's input resolution (Wd = 16 -> 2 H rows)
   if (chunks < 1) chunks = 1;
   if (chunks > kMaxChunks) chunks = kMaxChunks;
   int nc = (N + chunks - 1) / chunks;
@@ -630,19 +607,15 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
       CUDA_TRY(cudaEventRecord(m->chunk_events[c], copy_st));
     }
     if (host_data != nullptr) CUDA_TRY(cudaStreamWaitEvent(st, m->chunk_events[c], 0));
-    // conv1 + pool1 (SIMT: K = 9)
+    // conv1 + pool1 (tensor cores, split-bf16 operands: conv1_tc.cuh)
     {
       const size_t o1 = (size_t)n0 * H1 * 16 * 64;
-      if (m->conv1_tc)
-        CRNN_TRY(launch_conv1_tc(pl.tO_c1, data + (size_t)n0 * W * 32, m->P("conv1/weights"), m->P("conv1/biases"), n0,
-                                 pl.train ? pl.am1 + o1 : nullptr, cn, W, sms, st, pl.line_w));
-      else
-        CRNN_TRY(launch_conv1_pool(data + (size_t)n0 * W * 32, m->P("conv1/weights"), m->P("conv1/biases"), pl.a1 + o1,
-                                   pl.train ? pl.am1 + o1 : nullptr, cn, W, sms, st));
+      CRNN_TRY(launch_conv1_tc(pl.tO_c1, data + (size_t)n0 * W * 32, m->P("conv1/weights"), m->P("conv1/biases"), n0,
+                               pl.train ? pl.am1 + o1 : nullptr, cn, W, sms, st, pl.line_w));
     }
     if (mark) STAGE_MARK();
     // conv2 + ReLU + pool2
-    if (m->conv2_swap) {
+    {
       convsw::Params p;
       p.Nimg = cn; p.img0 = n0; p.H = H1; p.tiles_per_img = (H1 + 15) / 16; p.bias = m->P("conv2/biases"); p.out = pl.a2;
       p.argmax = pl.train ? pl.am2 : nullptr;
@@ -651,15 +624,6 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
       else if (pl.train) CRNN_TRY(launch_conv2_swap<true>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st));
       else if (lines) CRNN_TRY((launch_conv2_swap<false, true>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st)));
       else CRNN_TRY(launch_conv2_swap<false>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st));
-    } else {
-      gemm::Params p = conv_params(N, H1, 16, 64, 128, 128, m->P("conv2/biases"), pl.a2, pl.mg2);
-      if (chunks > 1) { p.m_tile0 = n0 * sb2 / 4; p.num_m_tiles = cn * sb2 / 4; }
-      if (pl.train) {
-        p.argmax = pl.am2;
-        CRNN_TRY((launch_gemm<128, gemm::A_CONV3, gemm::EPI_RELU_POOL22_T, 6>(pl.tA_c2, m->tB_c2, p, sms, st)));
-      } else {
-        CRNN_TRY((launch_gemm<128, gemm::A_CONV3, gemm::EPI_RELU_POOL22, 6>(pl.tA_c2, m->tB_c2, p, sms, st)));
-      }
     }
     if (mark) STAGE_MARK();
     // conv3_1 + ReLU
@@ -774,11 +738,10 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     p.num_m_tiles = (p.M + 127) / 128; p.num_n_tiles = 8; p.num_k_blocks = 8; p.kb_per_shift = 8;
     p.Nc = 2048; p.bias = m->xbias; p.out = pl.xproj; p.ldo = 2048;
     p.H = H2; p.T = T; p.seq_len = time_step_len;
-    if (m->lstm_upc == 32) CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_XPROJ, 4>(pl.tA_x, m->tB_x, p, sms, st, &pl.tO_x)));
-    else CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_BIAS_BF16, 4>(pl.tA_x, m->tB_x, p, sms, st, &pl.tO_x)));
+    CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_XPROJ, 4>(pl.tA_x, m->tB_x, p, sms, st, &pl.tO_x)));
   }
   STAGE_MARK();
-  if (m->lstm_upc == 32) {
+  {
     // recurrence: ONE persistent launch; a cluster of 8 CTAs per (direction, 128-sample tile) -- csrc/lstm.cuh
     constexpr int CS = 8;
     lstm::Params lp;
@@ -790,36 +753,23 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     if (want_trace && d_trace == nullptr) CUDA_TRY(cudaMalloc(&d_trace, 2 * 2 * 4 * 16 * sizeof(long long)));
     if (want_trace) CUDA_TRY(cudaMemsetAsync(d_trace, 0, 2 * 2 * 4 * 16 * sizeof(long long), st));
     lp.trace = want_trace ? d_trace : nullptr;
-    lp.swap_ls = getenv("CRNN_LSTM_SWAPLS") != nullptr;
-    auto kern = lstm::lstm_persistent_kernel<CS>;
-    auto kern_mc = lstm::lstm_mc_kernel<CS, 0, 8>;
-    auto kern_ds = lstm::lstm_mc_kernel<CS, 1, 8>;
-    auto kern_ms = lstm::lstm_mc_kernel<CS, 2, 8>;
-    auto kern_gx = lstm::lstm_mc_kernel<CS, 3, 8>;
+    auto kern = lstm::lstm_mc_kernel<CS>;
     static bool attr = false;
     if (!attr) {
-      CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lstm::Cfg<CS>::SMEM_BYTES));
-      CUDA_TRY(cudaFuncSetAttribute(kern_mc, cudaFuncAttributeMaxDynamicSharedMemorySize, lstm::CfgMc<CS>::SMEM_BYTES));
-      CUDA_TRY(cudaFuncSetAttribute(kern_ds, cudaFuncAttributeMaxDynamicSharedMemorySize, lstm::CfgMc<CS>::SMEM_BYTES));
-      CUDA_TRY(cudaFuncSetAttribute(kern_ms, cudaFuncAttributeMaxDynamicSharedMemorySize, lstm::CfgMc<CS>::SMEM_BYTES));
-      CUDA_TRY(cudaFuncSetAttribute(kern_gx, cudaFuncAttributeMaxDynamicSharedMemorySize, lstm::CfgMc<CS>::SMEM_BYTES));
+      CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lstm::CfgMc<CS>::SMEM_BYTES));
       attr = true;
     }
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(CS * 2 * lp.tiles_per_dir);
-    cfg.blockDim = dim3(m->lstm_mc ? lstm::McThreads<8>::ALL : lstm::NUM_THREADS);
-    cfg.dynamicSmemBytes = m->lstm_mc ? lstm::CfgMc<CS>::SMEM_BYTES : lstm::Cfg<CS>::SMEM_BYTES;
+    cfg.blockDim = dim3(lstm::MC_THREADS);
+    cfg.dynamicSmemBytes = lstm::CfgMc<CS>::SMEM_BYTES;
     cfg.stream = st;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeClusterDimension;
     at[0].val.clusterDim.x = CS; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
-    if (m->lstm_mc == 4) CUDA_TRY(cudaLaunchKernelEx(&cfg, kern_gx, m->tB_h128, lp));
-    else if (m->lstm_mc == 3) CUDA_TRY(cudaLaunchKernelEx(&cfg, kern_ms, m->tB_h128, lp));
-    else if (m->lstm_mc == 2) CUDA_TRY(cudaLaunchKernelEx(&cfg, kern_ds, m->tB_h128, lp));
-    else if (m->lstm_mc == 1) CUDA_TRY(cudaLaunchKernelEx(&cfg, kern_mc, m->tB_h128, lp));
-    else CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, pl.tA_hall, m->tB_h128, lp));
+    CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, m->tB_h128, lp));
     if (want_trace) {
       long long h[2 * 2 * 4 * 16];            // [CTA 0 / 5][warpgroup slot][step 8..11][event]
       CUDA_TRY(cudaStreamSynchronize(st));
@@ -839,20 +789,6 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
             fprintf(stderr, "\n");
           }
       }
-    }
-  } else {
-    // per-step launches (debug fallback, CRNN_LSTM_IMPL=step): both directions stacked along M
-    CUDA_TRY(cudaMemsetAsync(pl.h_state, 0, (size_t)2 * pl.Npad * 256 * 2, st));
-    CUDA_TRY(cudaMemsetAsync(pl.c_state, 0, (size_t)2 * pl.Npad * 256 * 4, st));
-    for (int s = 0; s < T; ++s) {
-      gemm::Params p;
-      memset(&p, 0, sizeof(p));
-      p.num_m_tiles = 2 * pl.Npad / 128; p.num_n_tiles = 4; p.num_k_blocks = 4; p.kb_per_shift = 4;
-      p.m_tiles_per_dir = pl.Npad / 128;
-      p.Nc = 1024; p.H = H2; p.T = T; p.Nimg = N; p.Npad = pl.Npad; p.step = s;
-      p.xproj = pl.xproj; p.c_state = pl.c_state; p.lstm_out = pl.lstm_out; p.seq_len = time_step_len;
-      p.h_next = pl.h_state + (size_t)((s + 1) & 1) * 2 * pl.Npad * 256;
-      CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_LSTM, 4>(pl.tA_h[s & 1], m->tB_h, p, sms, st)));
     }
   }
   STAGE_MARK();
@@ -928,8 +864,6 @@ extern "C" int crnn_forward_lines(crnn_model* m, const float* data, const int* l
   size_t need = 0;
   CRNN_TRY(crnn_lines_workspace_size(m, N, W, &need));
   if (workspace_bytes < need) return crnn_fail(CRNN_WORKSPACE_TOO_SMALL, "forward_lines: workspace %zu < %zu", workspace_bytes, need);
-  if (!m->conv1_tc || !m->conv2_swap)
-    return crnn_fail(CRNN_UNSUPPORTED, "forward_lines: the line masks live in conv1_tc_kernel and conv2_swap_kernel (unset CRNN_CONV1 / CRNN_CONV2)");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   return forward_impl(m, data, nullptr, time_step_len, N, W, logits_out, workspace, workspace_bytes, 1, st, st, nullptr, 1, line_width,
                       fwd_prec(m));

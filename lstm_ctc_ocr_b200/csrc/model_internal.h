@@ -49,7 +49,6 @@ struct Plan {
   int N = 0, W = 0, H1 = 0, H2 = 0, T = 0, Npad = 0;
   void* ws = nullptr;
   __nv_bfloat16 *a1, *a2, *a3, *a3p, *a4a_pre, *a4a, *a4b_pre, *a4b, *a5, *xproj, *lstm_out, *h_state;
-  float* c_state;
   double* stats;        // [2 layers][2][512]
   float* bn;            // [2 layers][4][512]: scale, shift, mean, invstd
   // packed evaluation (crnn_forward_lines), past the inference layout; line_w == nullptr after any other forward
@@ -57,7 +56,7 @@ struct Plan {
   double* stats_l;            // [2 layers][N][2][512]
   float* bn_l;                // [2 layers][N][4][512]
   CUtensorMap tA_c2s;   // conv2 input through 128-position boxes regardless of H (swapped-operand kernel, conv_swap.cuh)
-  CUtensorMap tA_c2, tA_c31, tA_c32, tA_c41, tA_c42, tA_c5, tA_x, tA_h[2], tA_l, tA_hall;
+  CUtensorMap tA_c31, tA_c32, tA_c41, tA_c42, tA_c5, tA_x, tA_l;
   // output maps of the register-side GEMM epilogues (gemm::frag_epi) where no input map above has the producing layer's tile
   // geometry: conv3_1 stores through tA_c32 and conv5 through tA_x; conv1_tc_kernel stores its pooled tiles through tO_c1
   CUtensorMap tO_c1, tO_c2s, tO_c32, tO_c41, tO_c42, tO_x;
@@ -73,15 +72,15 @@ struct Plan {
   uint8_t *am1, *am2, *am3;                       // arg-max window indices of pool1 / pool2 / the 1x2 pool after conv3_2
   __nv_bfloat16* gates;                           // [2][N][T][4][256] post-activation gates
   float* csave;                                   // [2][N][T][256]
-  __nv_bfloat16 *dl_rows, *d_lstm_out, *dz_all, *dz_state, *d_a5, *d_a4b, *d_pre4b, *d_pre4a, *d_a3p, *d_pre32, *d_pre31, *d_a2,
+  __nv_bfloat16 *dl_rows, *d_lstm_out, *dz_all, *d_a5, *d_a4b, *d_pre4b, *d_pre4a, *d_a3p, *d_pre32, *d_pre31, *d_a2,
       *d_pre2, *d_a1;
   uint8_t* bptt_x;                                // lstm_bwd_ks_kernel exchange buffer [2][units][8 dst][8 src][8 KB]
   double* bn_bwd_sums;                            // [2 layers][2][512]
   float* bn_bwd_coef;                             // [3][512] scratch
   // K-major A maps of gradient buffers (data-gradient GEMMs)
-  CUtensorMap tG_dl, tG_dz, tG_da5, tG_p4b, tG_p4a, tG_p32, tG_p31, tG_p2, tG_dzstate;
+  CUtensorMap tG_dl, tG_dz, tG_da5, tG_p4b, tG_p4a, tG_p32;
   CUtensorMap tG_p2s, tG_p31s;                    // d_pre2 / d_pre31 through 128-position boxes regardless of H (conv_dgrad_swap_kernel)
-  CUtensorMap tO_dlo, tO_da4b, tO_da3p;           // data-gradient GEMM outputs (the others store through tG_da5 / tG_p4a / tG_p31)
+  CUtensorMap tO_dlo, tO_da4b, tO_da3p;           // data-gradient GEMM outputs (the others store through tG_da5 / tG_p4a)
   // MN-major (TN) maps: 2-D [rows, C] with 64x64 boxes, and the NHWC maps above reused for TN_CONV
   CUtensorMap tT_lstm_fw, tT_lstm_bw, tT_lstm_all, tT_dl, tT_a5, tT_dz, tT_dz_fw, tT_dz_bw, tT_a4b, tT_da5;
 };
@@ -98,28 +97,16 @@ struct crnn_model {
   float* xbias = nullptr;    // [2048] permuted LSTM bias with forget_bias folded in
   double* sumsq = nullptr;
   void* wblock = nullptr;
-  CUtensorMap tB_c2, tB_c31, tB_c32, tB_c41, tB_c42, tB_c5, tB_x, tB_h, tB_l, tB_h128;
+  CUtensorMap tB_c2, tB_c31, tB_c32, tB_c41, tB_c42, tB_c5, tB_x, tB_l, tB_h128;
   // training: bf16 operands of the data-gradient GEMMs (allocated by crnn_model_set_training)
   bool training = false;
   bool dirty_bwd = true;
   void* wblock_bwd = nullptr;
   __nv_bfloat16 *Bd_c42 = nullptr, *Bd_c41, *Bd_c32, *Bd_c31, *Bd_c2, *Bd_c5, *Bld, *Bxb, *Bhb;
-  CUtensorMap tD_c42, tD_c41, tD_c32, tD_c31, tD_c2, tD_c5, tD_l, tD_x, tD_h;
+  CUtensorMap tD_c42, tD_c41, tD_c32, tD_c31, tD_c5, tD_l, tD_x;
   CUtensorMap tDs_c2;        // conv2 dgrad weights through a 128-row box (rows 64..127 out of bounds -> zero fill): conv2_dgrad_swap_kernel
-  CUtensorMap tD_h256;       // same W_h^T operand, box = 256 unit rows (K-split BPTT)
-  bool bptt_ks = true;       // BPTT through lstm_bwd::lstm_bwd_ks_kernel (K-split, generic-proxy exchange); CRNN_BPTT=ring -> v1
+  CUtensorMap tD_h256;       // W_h^T operand of the BPTT (Bhb), box = 256 unit rows
   double* grad_sumsq = nullptr;
-  bool conv1_tc = true;      // conv1 + pool1 on the tensor cores (conv1_tc.cuh, split-bf16 operands); CRNN_CONV1=simt -> kernels.cu
-  bool bn_red_fused = true;       // conv4_1's BN-backward sums inside conv4_2's data-gradient epilogue (EPI_CONV_STORE_BNRED); CRNN_BN_FUSE=0 -> separate pass
-  bool relu_mask_fused = true;    // conv3_1's ReLU backward inside conv3_2's data-gradient epilogue (EPI_CONV_STORE_MASK); CRNN_RELU_FUSE=0 -> separate pass
-  bool conv1_wgrad_tc = true;     // conv1 weight gradient on the tensor cores (conv1_wgrad_tc.cuh); CRNN_CONV1_WGRAD=simt -> backward_kernels.cu
-  bool conv2_dgrad_swap = true;   // conv2 / conv3_1 data gradients with swapped operands (conv_swap.cuh); CRNN_CONV2_DGRAD=old -> position-major N = 64 / 128
-  bool conv2_wgrad_swap = true;   // conv2 weight gradient with swapped operands + 4 taps per N tile (gemm_tn.cuh tap_pack_n); CRNN_CONV2_WGRAD=old -> 2 taps per M tile
-  bool conv2_swap = true;    // conv2 with channels on the MMA M side and 256 positions on N (conv_swap.cuh); CRNN_CONV2=pos -> gemm.cuh
-  int lstm_mc = 3;           // recurrence through lstm::lstm_mc_kernel (no per-step cluster barrier): 1 = global slice + multicast bulk copy
-                             // (CRNN_LSTM_IMPL=mc), 2 = slices pushed smem -> peer smem (CRNN_LSTM_IMPL=ds),
-                             // 3 = smem slice -> bulk store -> multicast (default, "ms"); 0 = v1 with a cluster barrier per step (persistent)
-  int lstm_upc = 32;         // hidden units per gate tile: 32 = persistent cluster kernel (default), 64 = per-step launches
   Plan plan;
   void* x3 = nullptr;        // state of the f32-class path (compute_dtype 2, forward_x3.cu)
   void* fp8 = nullptr;       // e4m3 weights and scales of compute_dtype 4 (forward_fp8.cu)

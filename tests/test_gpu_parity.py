@@ -202,16 +202,12 @@ def test_forward_loss_decode_vs_committed_golden():
         assert np.array_equal(logits[int(tsl[n]):, n].cpu().numpy(), np.broadcast_to(b, (T - int(tsl[n]), 64)))
 
 
-@pytest.mark.parametrize("front", ["tc+swap", "simt+pos"])
 @pytest.mark.parametrize("N,W,widths", [(3, 100, None), (5, 24, [24, 20, 9, 24, 16]), (2, 160, [160, 131]), (130, 40, None)])
-def test_forward_layers_vs_oracle(N, W, widths, front, monkeypatch):
-    """Every layer against the fp64 oracle; conv1 and conv2 through both of their kernels: the defaults (conv1_tc.cuh: im2col +
-    split-bf16 wgmma; conv_swap.cuh: channels on the MMA M side) and the first-generation ones (kernels.cu SIMT conv1,
-    CRNN_CONV1=simt; gemm.cuh positions-on-M conv2, CRNN_CONV2=pos)."""
+def test_forward_layers_vs_oracle(N, W, widths):
+    """Every layer against the fp64 oracle (conv1_tc.cuh: im2col + split-bf16 wgmma; conv_swap.cuh: conv2 with channels on the
+    MMA M side)."""
     from lstm_ctc_ocr_b200 import engine
     from oracle import crnn_oracle as O
-    monkeypatch.setenv("CRNN_CONV1", "tc" if front == "tc+swap" else "simt")
-    monkeypatch.setenv("CRNN_CONV2", "swap" if front == "tc+swap" else "pos")
     pn = O.randomize_params(O.init_params(3, dtype=np.float32, logits_scale=10.0))
     data, lab, ll, tsl = O.synth_batch(N, W, seed=5, widths=widths, min_len=1, max_len=3)
     m = engine.CrnnModel(device=DEV)
@@ -335,30 +331,3 @@ def test_full_size_c3_properties():
     out, out_len = engine.ctc_greedy(logits2, t(tsl))
     assert int((out_len > t(tsl)).sum()) == 0
     assert int(out.max()) <= 62 and int(out.min()) >= 0
-
-
-@pytest.mark.parametrize("impl", ["persistent", "mc", "ds", "ms", "gx"])
-def test_cluster_lstm_kernels_match_per_step_kernel(impl):
-    """csrc/lstm.cuh -- v1 (`persistent`: cluster barrier per step), v2 (`mc`: global slice + multicast bulk copy, `ds`: slices
-    pushed smem -> peer smem) -- vs the per-step GEMM+cell launches (CRNN_LSTM_IMPL=step)."""
-    from lstm_ctc_ocr_b200 import engine, synthetic
-    N, W = 200, 100
-    params = synthetic.init_params(3, logits_scale=10.0)
-    widths = np.random.default_rng(2).integers(8, 101, size=N)
-    data, _, _, tsl = synthetic.synth_batch(N, W, seed=12, widths=widths)
-    t = lambda a: torch.tensor(a, device=DEV)
-    outs = []
-    for which in (impl, "step"):
-        os.environ["CRNN_LSTM_IMPL"] = which
-        try:
-            m = engine.CrnnModel(device=DEV)
-        finally:
-            os.environ.pop("CRNN_LSTM_IMPL", None)
-        m.load_params(params)
-        logits = m.forward(t(data), t(tsl)).clone()
-        logits_again = m.forward(t(data), t(tsl)).clone()           # the exchange buffers are reused across launches
-        assert rel(logits_again.cpu().numpy(), logits.cpu().numpy()) < 5e-3
-        outs.append((logits.cpu().numpy(), m.tap("lstm_out", N, W).cpu().numpy()))
-        del m
-    assert np.abs(outs[0][1] - outs[1][1]).max() <= 1e-2        # bf16 h, identical math up to MMA tile order
-    assert rel(outs[0][0], outs[1][0]) < 5e-3

@@ -188,16 +188,3 @@ def test_every_stage_at_batch_scale(N, W, request):
         c.report()
         fail += c.fail
     assert not fail, "\n".join(fail)
-
-
-@pytest.mark.parametrize("env", [p for p in B.ALT_SWITCHES if p.id == "bptt_ring_unfused"])
-def test_bptt_ring_unfused_at_batch_scale(env, monkeypatch, request):
-    """The bptt_ring_unfused switch set of test_gpu_stage_isolation.py (ring BPTT, unfused BatchNorm / ReLU kernels) at
-    512 x 256."""
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
-    torch.cuda.reset_peak_memory_stats()
-    case = "b512_W256/" + request.node.callspec.id
-    _, _, ck = B._run_stage_checks(case, 512, 256, _widths(512, 256), dev=DEV, chunk=CHUNK, ck=_checker(case))
-    _peak(ck)
-    ck.assert_ok()

@@ -49,13 +49,11 @@ def _gpu_grads(m, batch):
     return costs
 
 
-@pytest.mark.parametrize("bptt", ["ks", "ring"])
 @pytest.mark.parametrize("N,W,widths", [(4, 88, [88, 85, 60, 33]), (130, 40, None), (3, 100, [100, 57, 100])])
-def test_gradients_vs_oracle_autograd(N, W, widths, bptt, monkeypatch):
-    """All 24 gradient tensors against fp64 autograd on the oracle graph, through both BPTT kernels (lstm_bwd.cuh: `ks` =
-    K-split with the partial sums exchanged through L2, default; `ring` = first generation, dz streamed through a multicast ring)."""
+def test_gradients_vs_oracle_autograd(N, W, widths):
+    """All 24 gradient tensors against fp64 autograd on the oracle graph (BPTT: lstm_bwd.cuh, K-split with the partial sums
+    exchanged through L2)."""
     from oracle import crnn_oracle as O
-    monkeypatch.setenv("CRNN_BPTT", bptt)
     m, pn, batch = _setup(N, W, widths, wd=0.0)
     out = O.train_step({k: v.astype(np.float64) for k, v in pn.items()}, batch, wd=0.0)
     _gpu_grads(m, batch)

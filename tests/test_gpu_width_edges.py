@@ -112,23 +112,11 @@ def test_every_stage_at_edge_widths(N, W, ctc, request):
     assert not fail, "\n".join(fail)
 
 
-@pytest.mark.parametrize("env", [p for p in B.ALT_SWITCHES if p.id == "bptt_ring_unfused"])
-@pytest.mark.parametrize("N,W", [pytest.param(5, 8, id="T1"), pytest.param(130, 1024, id="W1024")])
-def test_bptt_ring_unfused_at_edge_widths(N, W, env, monkeypatch, request):
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
-    case = request.node.callspec.id
-    torch.cuda.reset_peak_memory_stats()
-    _, _, ck = B._run_stage_checks(case, N, W, _widths(N, W), dev=DEV, chunk=_chunk(W), ck=_checker(case, W // 4 - 1))
-    BB._peak(ck)
-    ck.assert_ok()
-
-
 @pytest.mark.parametrize("W", [8, 12, 16, 1024])
-def test_lstm_exchange_modes_bit_identical_at_edge_widths(W):
-    """All four CRNN_LSTM_IMPL modes, inference and training, two launches each: bit-identical lstm_out, gates and cell
-    state over 130 lines (two row tiles)."""
-    LH.check_modes_bit_identical(130, W)
+def test_lstm_launches_and_training_bit_identical_at_edge_widths(W):
+    """Inference and training, two launches each: bit-identical lstm_out, gates and cell state over 130 lines (two row
+    tiles)."""
+    LH.check_launches_and_training_bit_identical(130, W)
 
 
 # ------------------------------------------------------------------------------------------------------------------- CTC

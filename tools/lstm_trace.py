@@ -1,10 +1,8 @@
 """Timeline of the persistent LSTM kernel (debug): CRNN_LSTM_TRACE=1 makes crnn_forward print clock64 stamps of CTAs 0 and 5
 for steps 8..11 to stderr, one line per (CTA, warpgroup slot, step), in clocks since the CTA's earliest stamp.
-lstm_mc_kernel (default): slot wg0 / wg1 = the MMA warpgroup of row half 0 / 1; events 5 xproj loads issued, 3 h_{s-1} landed
+lstm_mc_kernel: slot wg0 / wg1 = the MMA warpgroup of row half 0 / 1; events 5 xproj loads issued, 3 h_{s-1} landed
 (the half's mbarrier), 4 MMAs done, 7 cell done, 8 h slice stored, 9 exchange issued, 10 output / saved-state stores issued.
-lstm_persistent_kernel (CRNN_LSTM_IMPL=persistent), slot wg0 only: 0 step top, 1 TMA issued, 2 first K-block landed, 3 last
-K-block landed, 4 MMAs committed, 5 xproj loads issued, 6 accumulator ready, 7 first accumulator half loaded, 8 cell + stores
-issued, 9 fence.proxy.async done, 10 cluster arrive, 11 cluster wait done.  Usage: python tools/lstm_trace.py [N] [W]"""
+Usage: python tools/lstm_trace.py [N] [W]"""
 import os
 import sys
 

@@ -149,6 +149,10 @@ int     crnn_param_info(const crnn_model* m, int index, const char** tf_name, in
 int     crnn_model_bind(crnn_model* m, float* params, float* grads, float* adam_m, float* adam_v);
 int     crnn_model_params_changed(crnn_model* m);   /* caller wrote params in place */
 
+/* The workspace is scratch, as in warp-ctc: its contents before a forward (crnn_forward*, crnn_forward_lines,
+ * crnn_model_calibrate_fp8) do not matter, so a caller may use the same memory for anything else between calls, at the same
+ * (N, W, pointer) too.  One exception: between a training forward and its crnn_backward the workspace holds what the
+ * backward reads and must not be touched. */
 int     crnn_model_workspace_size(const crnn_model* m, int N, int W, int train, size_t* bytes);
 
 /* data [N,W,32] f32 (width-major rows, lib/lstm/utils/gen.py:62-64), time_step_len [N] i32

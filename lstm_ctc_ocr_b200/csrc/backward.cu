@@ -126,6 +126,9 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
   }
   BMARK();
   // ------------------------------------------------------------------ BPTT through both directions
+  // dz rows of the padding frames (t = T) are never written by the recurrence, yet dW_x, dW_h, the LSTM bias sums and the conv5
+  // data gradient read them as K rows: zero them in every backward, whatever the workspace held before the forward
+  CUDA_TRY(cudaMemset2DAsync(pl.dz_all + (size_t)T * 2048, (size_t)H2 * 2048 * 2, 0, 2048 * 2, N, st));
   {
     lstm_bwd::Params lp;
     lp.gates = pl.gates; lp.csave = pl.csave; lp.d_out = pl.d_lstm_out; lp.dz_all = pl.dz_all;

@@ -394,8 +394,6 @@ static int build_plan(crnn_model* m, int N, int W, void* ws, cudaStream_t st) {
   CRNN_TRY(make_tmap_nhwc(&pl.tO_c42, pl.a4b_pre, N, pl.H2, 4, 512, pl.mg4 ? 32 : 8));
   CRNN_TRY(make_tmap_2d(&pl.tO_x, pl.xproj, (uint64_t)N * pl.H2, 2048, 2048, 128));
   if (m->cfg.compute_dtype == 4) CRNN_TRY(fp8_plan_maps(pl));
-  // rows t = T (= H2-1) of lstm_out are never produced by a time step: keep them defined (zero)
-  CUDA_TRY(cudaMemsetAsync(pl.lstm_out, 0, (size_t)N * pl.H2 * 512 * 2, st));
   if (pl.train) {
     const uint64_t R = (uint64_t)N * pl.H2;
     // K-major A operands (box = [64 K-elements, 128 rows])
@@ -432,8 +430,6 @@ static int build_plan(crnn_model* m, int N, int W, void* ws, cudaStream_t st) {
     CRNN_TRY(make_tmap_2d_box(&pl.tT_dz_bw, pl.dz_all + 1024, R, 1024, 2048, 64, 64));
     CRNN_TRY(make_tmap_2d_box(&pl.tT_a4b, pl.a4b, R, 1024, 1024, 64, 64));
     CRNN_TRY(make_tmap_2d_box(&pl.tT_da5, pl.d_a5, R, 512, 512, 64, 64));
-    // dz rows of padding frames (t = T) are never written by the backward recurrence: keep them zero
-    CUDA_TRY(cudaMemsetAsync(pl.dz_all, 0, (size_t)R * 2048 * 2, st));
   }
   return CRNN_OK;
 }
@@ -741,6 +737,9 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_XPROJ, 4>(pl.tA_x, m->tB_x, p, sms, st, &pl.tO_x)));
   }
   STAGE_MARK();
+  // rows t = T (= H2-1) of lstm_out are never produced by a time step, yet the logits GEMM and the backward's dW_h GEMMs read
+  // them (dW_h as h_{-1} / h_{T} of the neighbouring image): zero them in every forward, whatever the workspace held before
+  CUDA_TRY(cudaMemset2DAsync(pl.lstm_out + (size_t)T * 512, (size_t)H2 * 512 * 2, 0, 512 * 2, N, st));
   {
     // recurrence: ONE persistent launch; a cluster of 8 CTAs per (direction, 128-sample tile) -- csrc/lstm.cuh
     constexpr int CS = 8;

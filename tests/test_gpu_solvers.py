@@ -1,5 +1,5 @@
-"""The reference's Momentum and RMSProp solvers on the GPU (csrc/backward_kernels.cu clip_momentum_kernel / clip_rmsprop_kernel
-behind crnn_clip_momentum_step / crnn_clip_rmsprop_step), against the fp64 restatements of tests/solver_refs.py, which
+"""The reference's three solvers on the GPU (csrc/backward_kernels.cu clip_adam_kernel / clip_momentum_kernel / clip_rmsprop_kernel
+behind crnn_clip_adam_step / crnn_clip_momentum_step / crnn_clip_rmsprop_step), against the fp64 restatements of tests/solver_refs.py, which
 tests/test_solvers_cpu.py pins to TensorFlow's own known answers.
 
 Per-element check of one update: the reference step is computed in fp64 from the kernel's own inputs (the f32 parameters, slots
@@ -25,7 +25,8 @@ U = 2.0 ** -24
 
 # Largest c (in u of the term magnitudes) per quantity over the three steps of test_update_matches_fp64_per_element, H100 80GB HBM3
 # (SXM).  BOUND = 4.5x.
-MEASURED = {"Momentum": {"params": 1.74, "accum": 1.95}, "RMS": {"params": 2.45, "ms": 0.67, "mom": 4.13}}
+MEASURED = {"Momentum": {"params": 1.74, "accum": 1.95}, "RMS": {"params": 2.45, "ms": 0.67, "mom": 4.13},
+            "Adam": {"params": 4.49, "adam_m": 2.85, "adam_v": 5.33}}
 BOUND = {s: {k: 4.5 * v for k, v in d.items()} for s, d in MEASURED.items()}
 # every run appends what it needed to build/solver_report.jsonl (re-measure from there)
 REPORT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "build", "solver_report.jsonl")
@@ -68,9 +69,10 @@ def _f64(t):
     return t.detach().cpu().numpy().astype(np.float64)
 
 
-def _reference(solver, s, raw, mask, wd, lr, clip, momentum=0.9, decay=0.9, rms_momentum=0.0, eps=1e-10):
+def _reference(solver, s, raw, mask, wd, lr, clip, momentum=0.9, decay=0.9, rms_momentum=0.0, eps=1e-10, step=1):
     """fp64 step from the f32 state `s`, the raw gradients and the f32 hyper-parameters the kernel receives: returns
-    ({quantity: (value, magnitude of the terms that make it up)}, global norm)."""
+    ({quantity: (value, magnitude of the terms that make it up)}, global norm).  Adam: `step` is the 1-based global step, the
+    step size, b1, b2 and eps those crnn_clip_adam_step passes (solver_refs.adam_lr_t, f32 0.9 / 0.999 / 1e-8)."""
     f32 = lambda x: float(np.float32(x))
     wd, lr, clip, momentum, decay, rms_momentum, eps = (f32(x) for x in (wd, lr, clip, momentum, decay, rms_momentum, eps))
     p0 = _f64(s["params"])
@@ -79,6 +81,9 @@ def _reference(solver, s, raw, mask, wd, lr, clip, momentum=0.9, decay=0.9, rms_
     gn = math.sqrt(float((gf * gf).sum()))
     scale = clip / max(gn, clip) if clip > 0 else 1.0
     g, g_mag = gf * scale, (np.abs(raw) + np.abs(wdp)) * scale
+    if solver == "Adam":
+        return R.adam_update(p0, g, _f64(s["adam_m"]), _f64(s["adam_v"]), R.adam_lr_t(lr, step), f32(R.ADAM_B1), f32(R.ADAM_B2),
+                             f32(R.ADAM_EPS), g_mag=g_mag), gn
     if solver == "Momentum":
         a0 = _f64(s["adam_m"]) * momentum
         a = a0 + g
@@ -93,7 +98,7 @@ def _reference(solver, s, raw, mask, wd, lr, clip, momentum=0.9, decay=0.9, rms_
 
 
 def _c_needed(ref, m, solver):
-    got = {"params": m.params, "accum": m.adam_m, "mom": m.adam_m, "ms": m.adam_v}
+    got = {"params": m.params, "accum": m.adam_m, "mom": m.adam_m, "ms": m.adam_v, "adam_m": m.adam_m, "adam_v": m.adam_v}
     out = {}
     for k, (val, mag) in ref.items():
         err = np.abs(_f64(got[k]) - val)
@@ -101,12 +106,15 @@ def _c_needed(ref, m, solver):
     return out
 
 
-def _call(m, solver, lr, clip, grad_mul, wd_mul, hp):
-    """One update: through apply_gradients with the reference's hyper-parameters, or straight through the C entry for `hp`."""
+def _call(m, solver, lr, clip, grad_mul, wd_mul, hp, step=1):
+    """One update: through apply_gradients with the reference's hyper-parameters at global step `step`, or straight through the
+    C entry for `hp` (Adam: {"step": global step})."""
     from lstm_ctc_ocr_b200 import engine
     from lstm_ctc_ocr_b200._lib import check
     if hp is None:
-        m.apply_gradients(lr, 1, clip=clip, grad_mul=grad_mul, wd_mul=wd_mul)
+        m.apply_gradients(lr, step, clip=clip, grad_mul=grad_mul, wd_mul=wd_mul)
+    elif solver == "Adam":
+        check(m.lib.crnn_clip_adam_step(m.handle, lr, clip, hp["step"], grad_mul, wd_mul, engine._stream()))
     elif solver == "Momentum":
         check(m.lib.crnn_clip_momentum_step(m.handle, lr, hp["momentum"], clip, grad_mul, wd_mul, engine._stream()))
     else:
@@ -114,34 +122,39 @@ def _call(m, solver, lr, clip, grad_mul, wd_mul, hp):
                                            engine._stream()))
 
 
-@pytest.mark.parametrize("solver", ["Momentum", "RMS"])
+# the third step of test_update_matches_fp64_per_element: through the C entry with other hyper-parameters (Adam: a global step
+# whose bias correction is near 1)
+THIRD_STEP = {"Adam": {"step": 10000}, "Momentum": {"momentum": 0.5}, "RMS": {"decay": 0.8, "rms_momentum": 0.5, "eps": 1e-3}}
+
+
+@pytest.mark.parametrize("solver", ["Adam", "Momentum", "RMS"])
 def test_update_matches_fp64_per_element(solver):
     """Whole buffer, weight decay on: step 1 clips (raw norm ~ 8e3), step 2 does not (norm ~ 2.7), lr changes between them, and a
-    third step runs the C entry with other hyper-parameters (momentum 0.5 / RMSProp decay 0.8, momentum 0.5, epsilon 1e-3).
-    The simulated data-parallel call -- gradients x2, grad_mul 0.5, wd_mul 2, i.e. a SUM over two equal ranks -- equals the
-    single-device call bit for bit."""
+    third step runs the C entry with other hyper-parameters (Adam at global step 10000, where the bias correction lr_t / lr is
+    0.99998, against 0.316 at step 1 and 0.795 at step 1000 / Momentum 0.5 / RMSProp decay 0.8, momentum 0.5, epsilon 1e-3).  The simulated
+    data-parallel call -- gradients x2, grad_mul 0.5, wd_mul 2, i.e. a SUM over two equal ranks -- equals the single-device
+    call bit for bit."""
     wd, clip = 1e-5, 10.0
     m = _model(wd)
     m.set_solver(solver, momentum=0.9)
     mask = _l2_mask(m)
     rng = np.random.default_rng(7)
-    steps = [(1e-3, 3.0, None), (4e-4, 1e-3, None),
-             (2e-4, 1e-3, {"momentum": 0.5} if solver == "Momentum" else {"decay": 0.8, "rms_momentum": 0.5, "eps": 1e-3})]
+    steps = [(1e-3, 3.0, None), (4e-4, 1e-3, None), (2e-4, 1e-3, THIRD_STEP[solver])]
     worst = {}
     for i, (lr, gscale, hp) in enumerate(steps):
         raw = (rng.standard_normal(m.total) * gscale).astype(np.float32)
         s = _state(m)
         m.grads.copy_(torch.from_numpy(raw).to(DEV))
-        _call(m, solver, lr, clip, 1.0, 1.0, hp)
+        _call(m, solver, lr, clip, 1.0, 1.0, hp, step=i + 1)
         single = _state(m)
         gn_gpu = m.last_grad_norm()
         _load_state(m, s)
         m.grads.copy_(torch.from_numpy(raw * 2).to(DEV))
-        _call(m, solver, lr, clip, 0.5, 2.0, hp)
+        _call(m, solver, lr, clip, 0.5, 2.0, hp, step=i + 1)
         for k in single:
             assert torch.equal(single[k], getattr(m, k)), (solver, i, k)
         assert m.last_grad_norm(0.5) == gn_gpu
-        kw = hp or ({"momentum": 0.9} if solver == "Momentum" else {})
+        kw = hp or ({"momentum": 0.9} if solver == "Momentum" else {"step": i + 1} if solver == "Adam" else {})
         ref, gn = _reference(solver, s, raw.astype(np.float64), mask, wd, lr, clip, **kw)
         assert (gn > clip) == (i == 0), gn
         assert abs(gn_gpu - gn) / gn < 1e-5, (gn_gpu, gn)

@@ -301,15 +301,26 @@ def _backward_checks(ck, F_, grad, dlogits, bnp, inject=None):
 
 
 def _run_stage_checks(case, N, W, widths, dev="cpu", chunk=None, ctc=None, ck=None, max_label=4, seed=5):
-    """The training-mode forward and backward of one batch, every stage checked on its own inputs.  dev: where the fp64
-    references run; chunk: images per reference evaluation (the whole batch by default).  ctc(ck, logits, lab, ll, tsl):
-    returns the backward's d logits (default: a seeded random one).  max_label: label lengths are drawn from 1 ..
-    max_label.  seed: of the synthetic batch.  Returns the model, the operands (_Refs) and the checker (Checker(case) unless
-    given), not yet asserted."""
+    """The training-mode forward and backward of one batch on a fresh model, every stage checked on its own inputs.  dev:
+    where the fp64 references run; chunk: images per reference evaluation (the whole batch by default).  ctc(ck, logits,
+    lab, ll, tsl): returns the backward's d logits (default: a seeded random one).  max_label: label lengths are drawn from
+    1 .. max_label.  seed: of the synthetic batch.  Returns the model, the operands (_Refs) and the checker (Checker(case)
+    unless given), not yet asserted."""
     m, pn, data, lab, ll, tsl = _setup(N, W, widths, seed=seed, max_label=max_label)
+    m.set_training(True)
+    F_, ck = _check_step(m, pn, (data, lab, ll, tsl), case, dev, chunk, ctc, ck)
+    return m, F_, ck
+
+
+def _check_step(m, pn, batch, case, dev="cpu", chunk=None, ctc=None, ck=None):
+    """The training-mode forward and backward of `batch` = (data, lab, ll, tsl) on a model in training mode in whatever state
+    it is in (fresh, or parameters written by a solver step), every stage checked on its own inputs.  pn: the model's current
+    f32 parameters ({name: array}, e.g. m.tensor(k) read back).  dev, chunk, ctc, ck as in _run_stage_checks.  Returns the
+    operands (_Refs) and the checker, not yet asserted."""
+    data, lab, ll, tsl = batch
+    N, W = data.shape[0], data.shape[1]
     T = W // 4 - 1
     t = lambda a: torch.tensor(a, device=DEV)
-    m.set_training(True)
     d_data, d_tsl = t(data), t(tsl)
     logits = m.forward(d_data, d_tsl)
     torch.cuda.synchronize()
@@ -331,7 +342,7 @@ def _run_stage_checks(case, N, W, widths, dev="cpu", chunk=None, ctc=None, ck=No
     grad = {k: m.grad_tensor(k).to(dev, torch.float64) for k in m.table}
     bnp = _forward_checks(ck, F_)
     _backward_checks(ck, F_, grad, dlogits, bnp)
-    return m, F_, ck
+    return F_, ck
 
 
 # SHAPES (shared with other modules) and two 128-row tiles of widths 8 .. 100: the LSTM recurrence's 8-CTA clusters exchange h

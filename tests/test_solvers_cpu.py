@@ -271,3 +271,37 @@ def test_c_entries_refuse_a_null_model_without_touching_the_device():
     assert L.crnn_version() >= 101
     assert L.crnn_clip_momentum_step(None, 1e-3, 0.9, 10.0, 1.0, 1.0, None) == 1
     assert L.crnn_clip_rmsprop_step(None, 1e-3, 0.9, 0.0, 1e-10, 10.0, 1.0, 1.0, None) == 1
+
+
+@pytest.mark.parametrize("steps", [(1, 2, 3), (9998, 9999, 10000)])
+def test_adam_restatement_equals_the_oracle_adam_step(steps):
+    """solver_refs.adam_step (the per-element restatement the GPU Adam checks use) is the oracle's adam_step -- the formula of
+    include/crnn_ctc.h, lr_t = lr*sqrt(1-b2^t)/(1-b1^t), theta -= lr_t*m/(sqrt(v)+1e-8) -- to 1e-12, with the bias correction
+    far from 1 (steps 1 .. 3) and near it (9998 .. 10000), and its magnitudes bound every term."""
+    from oracle import crnn_oracle as O
+    rng = np.random.default_rng(4)
+    shapes = OrderedDict(a=(64,), b=(7, 9))
+    t = lambda a: torch.as_tensor(a, dtype=torch.float64)
+    params = OrderedDict((k, t(rng.standard_normal(s) * 2e-2)) for k, s in shapes.items())
+    p_o = OrderedDict((k, v.clone()) for k, v in params.items())
+    m, v = R.init_slots("Adam", params)["m"], R.init_slots("Adam", params)["v"]
+    m_o = OrderedDict((k, x.clone()) for k, x in m.items())
+    v_o = OrderedDict((k, x.clone()) for k, x in v.items())
+    for step in steps:
+        grads = OrderedDict((k, t(rng.standard_normal(s) * 10.0 ** rng.uniform(-6, 0))) for k, s in shapes.items())
+        params, m, v = R.adam_step(params, grads, m, v, step, 1e-3)
+        p_o, m_o, v_o = O.adam_step(p_o, OrderedDict((k, g.clone()) for k, g in grads.items()), m_o, v_o, step, 1e-3)
+        for k in shapes:
+            for a, b in ((params[k], p_o[k]), (m[k], m_o[k]), (v[k], v_o[k])):
+                assert float((a - b).abs().max()) <= 1e-12 * max(1.0, float(b.abs().max())), (step, k)
+    # the f32 step size crnn_clip_adam_step passes: from the f32 lr, rounded to f32 once (two roundings of 2^-24 at most)
+    for step in (1, 2, 1000, 10000):
+        exact = 1e-3 * math.sqrt(1 - 0.999 ** step) / (1 - 0.9 ** step)
+        assert R.adam_lr_t(1e-3, step, f32=False) == exact
+        assert abs(R.adam_lr_t(1e-3, step) - exact) <= 2.0 ** -23 * exact
+    # magnitudes: each holds |value| (and the f32 step of one element stays within a few units of it)
+    g = np.array([1e-3, -2e-4, 0.0, 5.0])
+    r = R.adam_update(np.array([0.02, -0.01, 0.0, 1.0]), g, np.array([1e-4, 1e-4, 0.0, -1.0]), np.array([1e-8, 0.0, 0.0, 1.0]),
+                      R.adam_lr_t(1e-3, 3))
+    for k, (val, mag) in r.items():
+        assert (np.abs(val) <= mag + 1e-300).all(), k

@@ -213,6 +213,34 @@ int     crnn_model_calibrate_fp8(crnn_model* m, const float* data, const int* ti
 int     crnn_model_get_fp8_scales(crnn_model* m, float* scales_host);
 int     crnn_model_set_fp8_scales(crnn_model* m, const float* scales_host);
 
+/* Moving BatchNorm statistics of conv4_1 / conv4_2 -- the moving_mean / moving_variance that tf.contrib.layers.batch_norm creates
+ * next to gamma / beta (the reference's conv_single, lib/networks/network.py:176-178, trains and evaluates with is_training=True and
+ * never updates them).  `moving` is a caller-owned device buffer f32 [2 layers][mean, variance][512]; TF initialises it to mean 0,
+ * variance 1.  Once bound (NULL unbinds), every crnn_backward updates it once, before anything else, from the f64 sums its training
+ * forward normalised with (over the global batch when data parallel, so every rank computes the same bits), per channel:
+ *   moving -= (moving - batch value) * (1 - decay)      (TF's assign_moving_average without zero-debias)
+ * with the batch mean and the population (biased) variance, every operation in f64 from the stored f32 value, rounded once to f32;
+ * 1 - decay is taken in f64 from the f32 decay (0.999f: 1 - decay is 1.3e-5 below TF's f32 1e-3).
+ * Forwards never update it: training forwards that no crnn_backward follows (validation), evaluation and fp8 calibration.
+ * crnn_model_set_bn_statistics(m, 1) makes evaluation forwards normalise with it:  y = relu(gamma * (conv(x) + b - mean) /
+ * sqrt(var + bn_eps) + beta).  The BatchNorm folds into the conv: s = gamma / sqrt(var + eps) in f64, W' = bf16(W * s) per output
+ * channel and b' = f32((b - mean) * s + beta), each rounded once; conv4_1 then runs as conv3_1's ReLU GEMM and conv4_2 as
+ * conv3_2's ReLU + pool GEMM, with no batch statistics, finalize or apply pass.  Each image's (and, in crnn_forward_lines, each
+ * line's) logits no longer depend on the rest of the batch.  fp8 models fold s into conv4_x's column scales (colscale x s, f64
+ * product rounded once) and the same b'; the e4m3 weights stay.  The folded operands are kept apart from the batch-mode ones and
+ * are re-derived on the next moving-mode forward after a parameter change, a bind, a backward or a mode change; a caller that
+ * writes `moving` in place calls crnn_model_params_changed.  0 (the default, the reference's behaviour) = batch statistics.
+ * Training forwards always use batch statistics.  Errors: set_bn_statistics(m, 1) on a model in training mode
+ * CRNN_INVALID_VALUE; a moving-mode forward with no buffer bound CRNN_NOT_BOUND; compute_dtype 2 or 3 CRNN_UNSUPPORTED (both
+ * calls); decay outside [0, 1] CRNN_INVALID_VALUE.  Binding a buffer and changing the mode invalidate an fp8 model's activation
+ * scales, as a parameter change does: calibrate again in the mode that will be evaluated (crnn_model_calibrate_fp8 runs the
+ * mode's own conv4_x).  After a moving-mode forward the taps "a4a_pre", "a4b_pre", "bn" and "stats" return CRNN_INVALID_VALUE;
+ * crnn_debug_tap_raw adds "moving_w_conv4_1" / "moving_w_conv4_2" (bf16 W' [512][K], K = 2304 / 4608 in (kh, kw, ci) order) and
+ * "moving_bias" (f32 b' [2][512]), and on fp8 models "fp8_colscale_moving" (f32 [2][512]).  crnn_lines_workspace_size depends
+ * on the mode: with moving statistics it holds no per-line statistics. */
+int     crnn_model_bind_bn_moving(crnn_model* m, float* moving, float decay);
+int     crnn_model_set_bn_statistics(crnn_model* m, int moving);   /* 0 = batch statistics (default, the reference), 1 = moving */
+
 /* The host-side copy crnn_forward_pageable uses, on its own: `bytes` from `src` to `dst` (plain host pointers, non-overlapping) split
  * over `threads` threads of the library's persistent pool (the caller's thread included).  No CUDA call is made. */
 int     crnn_host_copy(void* dst, const void* src, size_t bytes, int threads);

@@ -48,6 +48,8 @@ SIGNATURES = {
     "crnn_model_calibrate_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "crnn_model_get_fp8_scales": (c_int, [c_void_p, c_void_p]),
     "crnn_model_set_fp8_scales": (c_int, [c_void_p, c_void_p]),
+    "crnn_model_bind_bn_moving": (c_int, [c_void_p, c_void_p, c_float]),
+    "crnn_model_set_bn_statistics": (c_int, [c_void_p, c_int]),
     "crnn_host_copy": (c_int, [c_void_p, c_void_p, c_size_t, c_int]),
     "crnn_total_loss": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "crnn_debug_tap": (c_int, [c_void_p, c_char_p, c_void_p, c_size_t, c_void_p, c_void_p]),

@@ -109,6 +109,12 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
 #define BMARK() do { if (ev) CUDA_TRY(cudaEventRecord(ev[evi++], st)); } while (0)
   BMARK();
   CUDA_TRY(cudaMemsetAsync(m->grads, 0, (size_t)m->total * sizeof(float), st));
+  // moving statistics: one update per training step, from the sums this step's forward normalised with (pl.stats, over the global
+  // batch when data parallel: both exchanges leave the global sums there)
+  if (m->bn_moving) {
+    CRNN_TRY(launch_bn_moving_update(pl.stats, (double)N * H2 * 4 * m->dp_world, m->bn_moving, m->bn_decay, st));
+    m->bn_fold_dirty = true;
+  }
 
   // ------------------------------------------------------------------ 512 -> 64 projection (network.py:118-128)
   CRNN_TRY(launch_dlogits_rows(dlogits, pl.dl_rows, G("logits/biases"), T, N, H2, st));

@@ -14,7 +14,8 @@
 //                ReLU / pooling as on the bf16 path, and e4m3(y / s_out) where the next consumer is fp8.
 // Producers write e4m3 themselves: conv2_swap_kernel<false, LINES, true> (a2), frag_epilogue EPI_RELU / EPI_RELU_POOL12 with
 // KIND 2 (a3, a3p), bn_apply_e4m3_kernel (a4a, a4b).  conv4_x keep their bf16 pre-BN output and f64 batch statistics, conv5
-// its bf16 output.
+// its bf16 output.  With moving BatchNorm statistics (crnn_model_set_bn_statistics) the BN folds into conv4_x's colscale and bias,
+// and their EPI_RELU / EPI_RELU_POOL12 epilogues write e4m3 a4a / a4b themselves.
 // Calibration (crnn_model_calibrate_fp8) runs the bf16 front end on a caller-supplied batch and reduces the five amaxes on the
 // device (atomicMax on the f32 bits of non-negative values: deterministic); the scales never leave the device.
 #include <cmath>
@@ -88,6 +89,13 @@ __global__ void scale_finalize_kernel(const unsigned* __restrict__ amax, float* 
   if (threadIdx.x < kLayers) scales[threadIdx.x] = pow2_scale(__uint_as_float(amax[threadIdx.x]));
 }
 
+// moving statistics: colscale_m[l][co] = f32(colscale[2 + l][co] * s[l][co]) (f64 product, one rounding), s = the fold's
+// gamma / sqrt(var + eps) of conv4_1 (l = 0) / conv4_2 (l = 1); the e4m3 weights stay as they are
+__global__ void colscale_moving_kernel(const float* __restrict__ colscale, const double* __restrict__ s, float* __restrict__ colscale_m) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < 2 * 512) colscale_m[i] = (float)__dmul_rn((double)colscale[2 * 512 + i], s[i]);
+}
+
 // colscale[l][co] = scales[l] * wscale[l][co]   ([5][512]; conv3_x use 256 columns)
 __global__ void colscale_kernel(const float* __restrict__ scales, const float* __restrict__ wscale, float* __restrict__ colscale) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -153,11 +161,13 @@ struct State {
   float* wscale;        // [5][512]
   float* scales;        // [5] activation scales: a2, a3, a3p, a4a, a4b
   float* colscale;      // [5][512]
+  float* colscale_m;    // [2][512] conv4_x colscale with the moving statistics folded in
   unsigned* amax;       // [5] calibration scratch
   CUtensorMap tB[kLayers];
   bool dirty = true;            // weights changed since the e4m3 copies were made
   bool colscale_dirty = true;   // weight or activation scales changed since colscale was computed
   bool calibrated = false;      // activation scales valid for the current parameters
+  bool colscale_m_dirty = true; // colscale or the moving-statistics fold changed since colscale_m was computed
 };
 
 // allocated once, by crnn_model_create of an fp8 model: calibration and the forward allocate nothing
@@ -166,13 +176,14 @@ static int create_state(crnn_model* m) {
     State* s = new State();
     size_t tot = 0;
     for (int l = 0; l < kLayers; ++l) tot += align_up((size_t)kL[l].K * kL[l].Cout);
-    tot += 3 * align_up(kLayers * 512 * 4) + 1024;
+    tot += 4 * align_up(kLayers * 512 * 4) + 1024;
     if (cudaMalloc(&s->block, tot) != cudaSuccess) { delete s; return crnn_fail(CRNN_CUDA_ERROR, "fp8: cudaMalloc"); }
     if (cudaMemset(s->block, 0, tot) != cudaSuccess) { cudaFree(s->block); delete s; return crnn_fail(CRNN_CUDA_ERROR, "fp8: cudaMemset"); }
     uint8_t* p = reinterpret_cast<uint8_t*>(s->block);
     for (int l = 0; l < kLayers; ++l) { s->Wq[l] = p; p += align_up((size_t)kL[l].K * kL[l].Cout); }
     s->wscale = reinterpret_cast<float*>(p); p += align_up(kLayers * 512 * 4);
     s->colscale = reinterpret_cast<float*>(p); p += align_up(kLayers * 512 * 4);
+    s->colscale_m = reinterpret_cast<float*>(p); p += align_up(kLayers * 512 * 4);
     s->scales = reinterpret_cast<float*>(p); s->amax = reinterpret_cast<unsigned*>(p + 64);
     for (int l = 0; l < kLayers; ++l) {
       const int st = make_tmap_2d_u8(&s->tB[l], s->Wq[l], kL[l].Cout, kL[l].K, kL[l].K, 256);
@@ -226,6 +237,18 @@ int fp8_prepare(crnn_model* m, cudaStream_t st) {
     fp8::colscale_kernel<<<(fp8::kLayers * 512 + 255) / 256, 256, 0, st>>>(s->scales, s->wscale, s->colscale);
     CUDA_TRY(cudaGetLastError());
     s->colscale_dirty = false;
+    s->colscale_m_dirty = true;
+  }
+  return CRNN_OK;
+}
+
+// after fp8_prepare and bn_fold_moving (`refolded`: the fold ran again)
+int fp8_fold_moving(crnn_model* m, bool refolded, cudaStream_t st) {
+  State* s = reinterpret_cast<State*>(m->fp8);
+  if (refolded || s->colscale_m_dirty) {
+    fp8::colscale_moving_kernel<<<4, 256, 0, st>>>(s->colscale, m->bm_scale, s->colscale_m);
+    CUDA_TRY(cudaGetLastError());
+    s->colscale_m_dirty = false;
   }
   return CRNN_OK;
 }
@@ -239,6 +262,7 @@ int fp8_plan_maps(Plan& pl) {
   CRNN_TRY(make_tmap_2d_u8(&pl.q_c5, pl.a4b, (uint64_t)N * pl.H2, 1024, 1024, 128));
   CRNN_TRY(make_tmap_nhwc_u8(&pl.qO_c2s, pl.a2, N, pl.H2, 8, 128, 8));
   CRNN_TRY(make_tmap_nhwc_u8(&pl.qO_c32, pl.a3p, N, pl.H2, 4, 256, pl.mg3 ? 16 : 4));
+  CRNN_TRY(make_tmap_nhwc_u8(&pl.qO_m42, pl.a4b, N, pl.H2, 2, 512, pl.mg4 ? 32 : 8));
   return CRNN_OK;
 }
 
@@ -250,9 +274,10 @@ int fp8_conv2(crnn_model* m, convsw::Params p, bool lines, int sms, cudaStream_t
   return launch_conv2_swap<false, false, true>(pl.tA_c2s, m->tB_c2, pl.qO_c2s, p, sms, st);
 }
 
-// layer 0 conv3_1 (EPI_RELU -> e4m3 a3), 1 conv3_2 (EPI_RELU_POOL12 -> e4m3 a3p), 2 / 3 conv4_1 / conv4_2 (EPI_STATS -> bf16 pre-BN);
+// layer 0 conv3_1 (EPI_RELU -> e4m3 a3), 1 conv3_2 (EPI_RELU_POOL12 -> e4m3 a3p), 2 / 3 conv4_1 / conv4_2 (EPI_STATS -> bf16 pre-BN;
+// `moving`: with the moving statistics folded into colscale_m and p.bias, EPI_RELU -> e4m3 a4a / EPI_RELU_POOL12 -> e4m3 a4b);
 // `p` is the bf16 path's conv_params (output, bias, stats, line widths), re-cut into 128-channel K-blocks here
-int fp8_conv_gemm(crnn_model* m, int layer, gemm::Params p, bool lines, int sms, cudaStream_t st) {
+int fp8_conv_gemm(crnn_model* m, int layer, gemm::Params p, bool lines, int sms, cudaStream_t st, bool moving) {
   State* s = reinterpret_cast<State*>(m->fp8);
   const Plan& pl = m->plan;
   p.cin_blocks = fp8::kL[layer].Cin / 128;
@@ -264,6 +289,15 @@ int fp8_conv_gemm(crnn_model* m, int layer, gemm::Params p, bool lines, int sms,
   const CUtensorMap& a = *tA[layer];
   const CUtensorMap& b = s->tB[layer];
   using namespace gemm;
+  if (moving) {
+    p.colscale = s->colscale_m + (layer - 2) * 512;
+    if (layer == 2) {
+      if (lines) return launch_gemm<256, A_CONV3, EPI_RELU, 4, 2, true>(a, b, p, sms, st, &pl.q_c42);
+      return launch_gemm<256, A_CONV3, EPI_RELU, 4, 2>(a, b, p, sms, st, &pl.q_c42);
+    }
+    if (lines) return launch_gemm<256, A_CONV3, EPI_RELU_POOL12, 4, 2, true>(a, b, p, sms, st, &pl.qO_m42);
+    return launch_gemm<256, A_CONV3, EPI_RELU_POOL12, 4, 2>(a, b, p, sms, st, &pl.qO_m42);
+  }
   switch (layer) {
     case 0:
       if (lines) return launch_gemm<256, A_CONV3, EPI_RELU, 4, 2, true>(a, b, p, sms, st, tO[0]);
@@ -357,7 +391,8 @@ int fp8_dequant_tap(crnn_model* m, int idx, const void* src, float* dst, size_t 
   return CRNN_OK;
 }
 
-// crnn_debug_tap_raw names of the fp8 state: "fp8_scales" f32 [5], "fp8_colscale" f32 [5][512], "fp8_wscale" f32 [5][512],
+// crnn_debug_tap_raw names of the fp8 state: "fp8_scales" f32 [5], "fp8_colscale" f32 [5][512], "fp8_colscale_moving" f32 [2][512],
+// "fp8_wscale" f32 [5][512],
 // "fp8_w_<layer>" u8 [Cout][K].  Returns 1 when `name` is one of them (the copy is issued or has failed with a status in *status).
 int fp8_debug_tap_raw(crnn_model* m, const std::string& name, void* dst, size_t dst_bytes, cudaStream_t st, int* status) {
   State* s = reinterpret_cast<State*>(m->fp8);
@@ -365,6 +400,7 @@ int fp8_debug_tap_raw(crnn_model* m, const std::string& name, void* dst, size_t 
   size_t bytes = 0;
   if (name == "fp8_scales") { bytes = fp8::kLayers * sizeof(float); src = s ? s->scales : nullptr; }
   else if (name == "fp8_colscale") { bytes = fp8::kLayers * 512 * sizeof(float); src = s ? s->colscale : nullptr; }
+  else if (name == "fp8_colscale_moving") { bytes = 2 * 512 * sizeof(float); src = s ? s->colscale_m : nullptr; }
   else if (name == "fp8_wscale") { bytes = fp8::kLayers * 512 * sizeof(float); src = s ? s->wscale : nullptr; }
   else {
     for (int l = 0; l < fp8::kLayers; ++l)

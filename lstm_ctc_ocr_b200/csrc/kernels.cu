@@ -142,6 +142,40 @@ __global__ void __launch_bounds__(256) bn_apply_relu_pool12_lines_kernel(const u
   out[i] = o;
 }
 
+// ---- moving statistics (tf.contrib.layers.batch_norm's moving_mean / moving_variance, non-fused, zero_debias = False).
+// Every operation is an explicitly rounded f64 operation (no fma contraction), so an fp64 restatement predicts every bit.
+// One thread per (layer, channel): stats [2 layers][sum, sum of squares][512] of the training forward, count = positions of the
+// (global) batch; moving [2 layers][mean, variance][512] f32 in place:  moving -= (moving - batch value) * (1 - decay)
+__global__ void bn_moving_update_kernel(const double* __restrict__ stats, double count, float* __restrict__ moving, float decay) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 2 * 512) return;
+  const int l = i >> 9, c = i & 511;
+  const double* st = stats + l * 1024;
+  const double mean = __ddiv_rn(st[c], count);
+  double var = __dsub_rn(__ddiv_rn(st[512 + c], count), __dmul_rn(mean, mean));    // population variance, as the forward's
+  if (var < 0) var = 0;
+  const double f = __dsub_rn(1.0, (double)decay);
+  float* mv = moving + l * 1024;
+  const double m0 = mv[c], v0 = mv[512 + c];
+  mv[c] = (float)__dsub_rn(m0, __dmul_rn(__dsub_rn(m0, mean), f));
+  mv[512 + c] = (float)__dsub_rn(v0, __dmul_rn(__dsub_rn(v0, var), f));
+}
+
+// Fold the moving statistics of one BN layer into its conv: s = gamma / sqrt(var + eps) (f64), B'[co][k] = bf16(W[k][co] * s) (one
+// rounding), b'[co] = f32((b - mean) * s + beta) (one rounding); scale_out keeps s for the fp8 column scales.  One CTA per channel.
+__global__ void __launch_bounds__(256) bn_fold_kernel(const float* __restrict__ w, int K, int Cout, const float* __restrict__ bias,
+                                                      const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                      const float* __restrict__ moving, float eps, __nv_bfloat16* __restrict__ bout,
+                                                      float* __restrict__ bias_out, double* __restrict__ scale_out) {
+  const int co = blockIdx.x;
+  const double s = __ddiv_rn((double)gamma[co], __dsqrt_rn(__dadd_rn((double)moving[Cout + co], (double)eps)));
+  for (int r = threadIdx.x; r < K; r += 256) bout[(size_t)co * K + r] = __double2bfloat16(__dmul_rn((double)__ldg(w + (size_t)r * Cout + co), s));
+  if (threadIdx.x == 0) {
+    bias_out[co] = (float)__dadd_rn(__dmul_rn(__dsub_rn((double)bias[co], (double)moving[co]), s), (double)beta[co]);
+    scale_out[co] = s;
+  }
+}
+
 // line widths as every packed-evaluation kernel reads them: clamped to [8, W] and rounded down to a multiple of 4
 __global__ void clamp_line_width_kernel(const int* __restrict__ in, int* __restrict__ out, int N, int W) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -257,6 +291,17 @@ int launch_bn_apply_relu_pool12(const __nv_bfloat16* in, __nv_bfloat16* out, con
   const size_t nvec = out_positions * C / 8;
   bn_apply_relu_pool12_kernel<<<(unsigned)((nvec + 255) / 256), 256, 0, st>>>(
       reinterpret_cast<const uint4*>(in), reinterpret_cast<uint4*>(out), scale, shift, nvec, C);
+  CUDA_TRY(cudaGetLastError());
+  return CRNN_OK;
+}
+int launch_bn_moving_update(const double* stats, double count, float* moving, float decay, cudaStream_t st) {
+  bn_moving_update_kernel<<<4, 256, 0, st>>>(stats, count, moving, decay);
+  CUDA_TRY(cudaGetLastError());
+  return CRNN_OK;
+}
+int launch_bn_fold(const float* w, int K, int Cout, const float* bias, const float* gamma, const float* beta, const float* moving, float eps,
+                   __nv_bfloat16* bout, float* bias_out, double* scale_out, cudaStream_t st) {
+  bn_fold_kernel<<<Cout, 256, 0, st>>>(w, K, Cout, bias, gamma, beta, moving, eps, bout, bias_out, scale_out);
   CUDA_TRY(cudaGetLastError());
   return CRNN_OK;
 }

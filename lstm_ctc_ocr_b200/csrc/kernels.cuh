@@ -23,6 +23,11 @@ int launch_bn_apply_relu_lines(const __nv_bfloat16* in, __nv_bfloat16* out, cons
                                int C, cudaStream_t st);
 int launch_bn_apply_relu_pool12_lines(const __nv_bfloat16* in, __nv_bfloat16* out, const float* bn, const int* line_w, int N, int H,
                                       int Wo, int C, cudaStream_t st);
+// moving BatchNorm statistics of conv4_1 / conv4_2: the per-step update from the training forward's f64 sums, and the fold of one
+// layer's statistics into its conv (bf16 B operand [Cout][K], f32 bias, f64 per-channel scale)
+int launch_bn_moving_update(const double* stats, double count, float* moving, float decay, cudaStream_t st);
+int launch_bn_fold(const float* w, int K, int Cout, const float* bias, const float* gamma, const float* beta, const float* moving, float eps,
+                   __nv_bfloat16* bout, float* bias_out, double* scale_out, cudaStream_t st);
 // lstm_gates: the columns are LSTM gate columns, stored permuted (LSTM_GATE_UNITS units per [i|j|f|o] tile)
 int launch_transpose_cast(const float* src, int R, int Cc, int ld_src, __nv_bfloat16* dst, int ld_dst, bool lstm_gates,
                           cudaStream_t st);

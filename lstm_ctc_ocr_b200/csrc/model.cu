@@ -27,7 +27,7 @@ int crnn_fail(int status, const char* fmt, ...) {
   return status;
 }
 extern "C" const char* crnn_last_error(void) { return g_err; }
-extern "C" int crnn_version(void) { return 103; }
+extern "C" int crnn_version(void) { return 104; }
 extern "C" const char* crnn_status_string(int s) {
   switch (s) {
     case CRNN_OK: return "CRNN_OK";
@@ -242,6 +242,7 @@ extern "C" int crnn_model_destroy(crnn_model* m) {
   fp8_destroy(m);
   if (m->wblock) cudaFree(m->wblock);
   if (m->wblock_bwd) cudaFree(m->wblock_bwd);
+  if (m->wblock_bnm) cudaFree(m->wblock_bnm);
   if (m->d_peers) cudaFree(m->d_peers);
   for (auto e : m->prof_events) cudaEventDestroy(e);
   for (auto e : m->prof_events_bwd) cudaEventDestroy(e);
@@ -266,6 +267,7 @@ extern "C" int crnn_model_bind(crnn_model* m, float* params, float* grads, float
   m->params = params; m->grads = grads; m->adam_m = adam_m; m->adam_v = adam_v;
   m->dirty = true;
   m->dirty_bwd = true;
+  m->bn_fold_dirty = true;
   x3_params_changed(m);
   fp8_params_changed(m);
   return CRNN_OK;
@@ -274,8 +276,64 @@ extern "C" int crnn_model_params_changed(crnn_model* m) {
   if (!m) return crnn_fail(CRNN_INVALID_VALUE, "null model");
   m->dirty = true;
   m->dirty_bwd = true;
+  m->bn_fold_dirty = true;
   x3_params_changed(m);
   fp8_params_changed(m);
+  return CRNN_OK;
+}
+
+// ---- moving BatchNorm statistics of conv4_1 / conv4_2
+extern "C" int crnn_model_bind_bn_moving(crnn_model* m, float* moving, float decay) {
+  if (!m) return crnn_fail(CRNN_INVALID_VALUE, "bind_bn_moving: null model");
+  if (!(decay >= 0.f && decay <= 1.f)) return crnn_fail(CRNN_INVALID_VALUE, "bind_bn_moving: decay %g outside [0, 1]", (double)decay);
+  if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3)
+    return crnn_fail(CRNN_UNSUPPORTED, "bind_bn_moving: moving statistics run on the bf16 and fp8 paths (compute_dtype 1, 4)");
+  if (moving && !m->wblock_bnm) {
+    const size_t b41 = align_up((size_t)512 * 2304 * 2), b42 = align_up((size_t)512 * 4608 * 2);
+    CUDA_TRY(cudaMalloc(&m->wblock_bnm, b41 + b42 + align_up(2 * 512 * 4) + 2 * 512 * 8));
+    uint8_t* p = reinterpret_cast<uint8_t*>(m->wblock_bnm);
+    m->Bm41 = reinterpret_cast<__nv_bfloat16*>(p); p += b41;
+    m->Bm42 = reinterpret_cast<__nv_bfloat16*>(p); p += b42;
+    m->bm_bias = reinterpret_cast<float*>(p); p += align_up(2 * 512 * 4);
+    m->bm_scale = reinterpret_cast<double*>(p);
+    CRNN_TRY(make_tmap_2d(&m->tB_m41, m->Bm41, 512, 2304, 2304, 256));
+    CRNN_TRY(make_tmap_2d(&m->tB_m42, m->Bm42, 512, 4608, 4608, 256));
+  }
+  m->bn_moving = moving;
+  m->bn_decay = decay;
+  m->bn_fold_dirty = true;
+  fp8_params_changed(m);      // fp8 scales calibrated on the old statistics are stale
+  return CRNN_OK;
+}
+
+extern "C" int crnn_model_set_bn_statistics(crnn_model* m, int moving) {
+  if (!m) return crnn_fail(CRNN_INVALID_VALUE, "set_bn_statistics: null model");
+  if (moving != 0 && moving != 1) return crnn_fail(CRNN_INVALID_VALUE, "set_bn_statistics: 0 (batch) or 1 (moving), got %d", moving);
+  if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3)
+    return crnn_fail(CRNN_UNSUPPORTED, "set_bn_statistics: moving statistics run on the bf16 and fp8 paths (compute_dtype 1, 4)");
+  if (moving && m->training)
+    return crnn_fail(CRNN_INVALID_VALUE, "set_bn_statistics: a model in training mode normalises with batch statistics");
+  if (m->bn_use_moving != (moving != 0)) {
+    m->bn_use_moving = moving != 0;
+    m->bn_fold_dirty = true;
+    fp8_params_changed(m);    // the fp8 scales of a4a / a4b belong to one mode
+  }
+  return CRNN_OK;
+}
+
+// the folded conv4_x operands for the bound moving statistics, re-derived when params, the buffer or the mode changed
+int bn_fold_moving(crnn_model* m, bool* refolded, cudaStream_t st) {
+  *refolded = false;
+  if (!m->bn_fold_dirty) return CRNN_OK;
+  const struct { const char* n; int K; __nv_bfloat16* d; } L[2] = {{"conv4_1", 2304, m->Bm41}, {"conv4_2", 4608, m->Bm42}};
+  for (int l = 0; l < 2; ++l) {
+    const std::string nm(L[l].n);
+    CRNN_TRY(launch_bn_fold(m->P(nm + "/weights"), L[l].K, 512, m->P(nm + "/biases"), m->P(nm + "/" + nm + "/gamma"),
+                            m->P(nm + "/" + nm + "/beta"), m->bn_moving + l * 1024, m->cfg.bn_eps, L[l].d, m->bm_bias + l * 512,
+                            m->bm_scale + l * 512, st));
+  }
+  m->bn_fold_dirty = false;
+  *refolded = true;
   return CRNN_OK;
 }
 
@@ -392,6 +450,7 @@ static int build_plan(crnn_model* m, int N, int W, void* ws, cudaStream_t st) {
   CRNN_TRY(make_tmap_nhwc(&pl.tO_c32, pl.a3p, N, pl.H2, 4, 256, pl.mg3 ? 16 : 4));     // conv3_2's pooled tile: 64 positions
   CRNN_TRY(make_tmap_nhwc(&pl.tO_c41, pl.a4a_pre, N, pl.H2, 4, 512, pl.mg4 ? 32 : 8));
   CRNN_TRY(make_tmap_nhwc(&pl.tO_c42, pl.a4b_pre, N, pl.H2, 4, 512, pl.mg4 ? 32 : 8));
+  CRNN_TRY(make_tmap_nhwc(&pl.tO_m42, pl.a4b, N, pl.H2, 2, 512, pl.mg4 ? 32 : 8));     // moving statistics: conv4_2's pooled tile
   CRNN_TRY(make_tmap_2d(&pl.tO_x, pl.xproj, (uint64_t)N * pl.H2, 2048, 2048, 128));
   if (m->cfg.compute_dtype == 4) CRNN_TRY(fp8_plan_maps(pl));
   if (pl.train) {
@@ -520,6 +579,9 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
   const bool fp8 = prec == FWD_FP8, calib = prec == FWD_CALIB;
   if (!m || !data || !time_step_len || (!logits_out && !calib) || !workspace) return crnn_fail(CRNN_INVALID_VALUE, "forward: null pointer");
   if (!m->params) return crnn_fail(CRNN_NOT_BOUND, "forward: call crnn_model_bind first");
+  const bool moving = m->bn_use_moving && !m->training;     // training forwards always normalise with batch statistics
+  if (moving && !m->bn_moving)
+    return crnn_fail(CRNN_NOT_BOUND, "forward: moving BatchNorm statistics selected but no buffer bound (crnn_model_bind_bn_moving)");
   if (N <= 0 || W < 8 || (W % 4) != 0) return crnn_fail(CRNN_INVALID_VALUE, "forward: need N>0, W>=8, W%%4==0");
   size_t need = 0;
   CRNN_TRY(crnn_model_workspace_size(m, N, W, m->training ? 1 : 0, &need));
@@ -549,8 +611,14 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
   }
   if (m->dirty) CRNN_TRY(prepare_weights(m, st));
   if (fp8) CRNN_TRY(fp8_prepare(m, st));
+  if (moving) {
+    bool refolded = false;
+    CRNN_TRY(bn_fold_moving(m, &refolded, st));
+    if (fp8) CRNN_TRY(fp8_fold_moving(m, refolded, st));
+  }
   Plan& pl = m->plan;
   CRNN_TRY(ensure_plan(m, N, W, workspace, st));
+  pl.moving = moving;
   const int H1 = pl.H1, H2 = pl.H2, T = pl.T, sms = m->num_sms;
   const bool lines = line_width != nullptr;
   pl.line_w = nullptr;
@@ -652,7 +720,24 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     if (mark) STAGE_MARK();
   }
   if (chunks > 1) for (int i = 0; i < 4; ++i) STAGE_MARK();     // keep the event layout (front-end stages read as ~0)
-  if (lines) {
+  if (moving) {
+    // conv4_x with the moving statistics folded into the weights and bias: conv4_1 + BN + ReLU is conv3_1's EPI_RELU GEMM, conv4_2
+    // + BN + ReLU + pool3 conv3_2's EPI_RELU_POOL12 GEMM; line masks zero the rows past each line, nothing else is per line.  The
+    // BN apply stages do not run (their events read ~0).
+    const struct { const char* name; int cin; const CUtensorMap* tA; const CUtensorMap* tB; __nv_bfloat16* out; } L[2] = {
+        {"conv4_1", 256, &pl.tA_c41, &m->tB_m41, pl.a4a}, {"conv4_2", 512, &pl.tA_c42, &m->tB_m42, pl.a4b}};
+    for (int l = 0; l < 2; ++l) {
+      gemm::Params p = conv_params(N, H2, 4, L[l].cin, 512, 256, m->bm_bias + l * 512, L[l].out, pl.mg4);
+      p.line_w = pl.line_w;
+      if (fp8) CRNN_TRY(fp8_conv_gemm(m, 2 + l, p, lines, sms, st, true));
+      else if (l == 0 && lines) CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4, 0, true>(*L[0].tA, *L[0].tB, p, sms, st, &pl.tA_c42)));
+      else if (l == 0) CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4>(*L[0].tA, *L[0].tB, p, sms, st, &pl.tA_c42)));
+      else if (lines) CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12, 4, 0, true>(*L[1].tA, *L[1].tB, p, sms, st, &pl.tO_m42)));
+      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12, 4>(*L[1].tA, *L[1].tB, p, sms, st, &pl.tO_m42)));
+      STAGE_MARK();
+      STAGE_MARK();
+    }
+  } else if (lines) {
     // conv4_x with per-line statistics: each line's own sums, scale and shift; zero at h >= W_i/4
     CUDA_TRY(cudaMemsetAsync(pl.stats_l, 0, (size_t)2 * N * 2 * 512 * sizeof(double), st));
     const struct { const char* name; const CUtensorMap* tA; const CUtensorMap* tB; const CUtensorMap* tO; int cin; __nv_bfloat16* pre; } L[2] = {
@@ -841,15 +926,16 @@ extern "C" int crnn_model_set_fp8_scales(crnn_model* m, const float* scales_host
   return fp8_set_scales(m, scales_host);
 }
 
-// packed evaluation: the inference plan, then line widths [N] i32, per-line statistics [2][N][2][512] f64, coefficients [2][N][4][512] f32
+// packed evaluation: the inference plan, then line widths [N] i32, per-line statistics [2][N][2][512] f64, coefficients [2][N][4][512] f32;
+// with moving statistics no per-line statistics or coefficients exist
 extern "C" int crnn_lines_workspace_size(const crnn_model* m, int N, int W, size_t* bytes) {
   if (!m || !bytes) return crnn_fail(CRNN_INVALID_VALUE, "lines_workspace_size: null");
   if (N <= 0 || W < 8 || (W % 4) != 0) return crnn_fail(CRNN_INVALID_VALUE, "lines_workspace_size: need N>0, W>=8, W%%4==0");
   if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3)
     return crnn_fail(CRNN_UNSUPPORTED, "lines_workspace_size: packed evaluation runs on the bf16 and fp8 paths (compute_dtype 1, 4)");
   Plan pl;
-  *bytes = layout_plan(pl, N, W, nullptr, false) + align_up((size_t)N * 4) + align_up((size_t)2 * N * 2 * 512 * 8) +
-           align_up((size_t)2 * N * 4 * 512 * 4);
+  *bytes = layout_plan(pl, N, W, nullptr, false) + align_up((size_t)N * 4);
+  if (!m->bn_use_moving) *bytes += align_up((size_t)2 * N * 2 * 512 * 8) + align_up((size_t)2 * N * 4 * 512 * 4);
   return CRNN_OK;
 }
 
@@ -944,8 +1030,11 @@ extern "C" int crnn_debug_tap(crnn_model* m, const char* name, float* dst, size_
   else if (s == "conv5") { src = pl.a5; cnt = n * h2 * 512; }
   else if (s == "lstm_out") { src = pl.lstm_out; cnt = n * h2 * 512; }
   else if (s == "xproj") { src = pl.xproj; cnt = n * h2 * 2048; }
-  else if (s == "a4a_pre") { src = pl.a4a_pre; cnt = n * h2 * 4 * 512; }
-  else if (s == "a4b_pre") { src = pl.a4b_pre; cnt = n * h2 * 4 * 512; }
+  else if (s == "a4a_pre" || s == "a4b_pre") {
+    if (pl.moving) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap: %s: the last forward used moving statistics (no pre-BN output)", name);
+    src = s == "a4a_pre" ? pl.a4a_pre : pl.a4b_pre;
+    cnt = n * h2 * 4 * 512;
+  }
   else {
     // saved state and backward buffers: only a training-mode plan holds them
     const struct { const char* name; const __nv_bfloat16* p; size_t cnt; } train_taps[] = {
@@ -984,8 +1073,20 @@ extern "C" int crnn_debug_tap_raw(crnn_model* m, const char* name, void* dst, si
     int status = CRNN_OK;
     if (fp8_debug_tap_raw(m, s, dst, dst_bytes, reinterpret_cast<cudaStream_t>(stream), &status)) return status;
   }
+  // the folded operands of the moving statistics (model state, not workspace): bf16 [Cout][K] and f32 [2][512]
+  if (s == "moving_w_conv4_1" || s == "moving_w_conv4_2" || s == "moving_bias") {
+    if (!m->wblock_bnm || m->bn_fold_dirty)
+      return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: %s: no forward with the current moving statistics ran yet", name);
+    const void* src = s == "moving_bias" ? (const void*)m->bm_bias : s == "moving_w_conv4_1" ? (const void*)m->Bm41 : (const void*)m->Bm42;
+    const size_t bytes = s == "moving_bias" ? 2 * 512 * sizeof(float) : (size_t)512 * (s == "moving_w_conv4_1" ? 2304 : 4608) * 2;
+    if (dst_bytes < bytes) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: dst too small (%zu < %zu bytes)", dst_bytes, bytes);
+    CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, reinterpret_cast<cudaStream_t>(stream)));
+    return CRNN_OK;
+  }
   Plan& pl = m->plan;
   if (pl.ws == nullptr || pl.ws != workspace) return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: no forward ran on this workspace");
+  if (pl.moving && (s == "bn" || s == "stats"))
+    return crnn_fail(CRNN_INVALID_VALUE, "debug_tap_raw: %s: the last forward used moving statistics (no batch statistics)", name);
   const size_t n = pl.N, h1 = pl.H1, h2 = pl.H2;
   const void* src = nullptr;
   size_t bytes = 0;

@@ -53,6 +53,7 @@ struct Plan {
   float* bn;            // [2 layers][4][512]: scale, shift, mean, invstd
   // packed evaluation (crnn_forward_lines), past the inference layout; line_w == nullptr after any other forward
   int* line_w = nullptr;      // [N] clamped line widths
+  bool moving = false;        // the last forward normalised conv4_x with the moving statistics (no a4x_pre, bn or stats written)
   double* stats_l;            // [2 layers][N][2][512]
   float* bn_l;                // [2 layers][N][4][512]
   CUtensorMap tA_c2s;   // conv2 input through 128-position boxes regardless of H (swapped-operand kernel, conv_swap.cuh)
@@ -67,6 +68,8 @@ struct Plan {
   // compute_dtype 4: UINT8 views of the e4m3 activations, which live in the first half of the bf16 buffers a2, a3, a3p, a4a, a4b
   // (forward_fp8.cu): A operands of conv3_1 .. conv5, conv3_1 stores through q_c32, conv2 / conv3_2 through qO_c2s / qO_c32
   CUtensorMap q_c31, q_c32, q_c41, q_c42, q_c5, qO_c2s, qO_c32;
+  // moving statistics: conv4_2's pooled output a4b as a conv output (Wd = 2), bf16 and e4m3
+  CUtensorMap tO_m42, qO_m42;
   // ---- training only -------------------------------------------------------------------------------------------
   bool train = false;
   uint8_t *am1, *am2, *am3;                       // arg-max window indices of pool1 / pool2 / the 1x2 pool after conv3_2
@@ -107,6 +110,16 @@ struct crnn_model {
   CUtensorMap tDs_c2;        // conv2 dgrad weights through a 128-row box (rows 64..127 out of bounds -> zero fill): conv2_dgrad_swap_kernel
   CUtensorMap tD_h256;       // W_h^T operand of the BPTT (Bhb), box = 256 unit rows
   double* grad_sumsq = nullptr;
+  // ---- moving BatchNorm statistics of conv4_1 / conv4_2 (crnn_model_bind_bn_moving / crnn_model_set_bn_statistics)
+  float* bn_moving = nullptr;            // caller-owned [2 layers][mean, variance][512] f32; updated by every crnn_backward
+  float bn_decay = 0.999f;
+  bool bn_use_moving = false;            // evaluation forwards normalise conv4_x with bn_moving (training forwards never do)
+  bool bn_fold_dirty = true;             // params, bn_moving or the mode changed since the folded operands were derived
+  void* wblock_bnm = nullptr;            // folded operands, allocated by the first crnn_model_bind_bn_moving
+  __nv_bfloat16 *Bm41 = nullptr, *Bm42 = nullptr;   // bf16(W * s) [Cout][K]
+  float* bm_bias = nullptr;              // [2][512] (b - mean) * s + beta
+  double* bm_scale = nullptr;            // [2][512] s = gamma / sqrt(var + eps)
+  CUtensorMap tB_m41, tB_m42;
   Plan plan;
   void* x3 = nullptr;        // state of the f32-class path (compute_dtype 2, forward_x3.cu)
   void* fp8 = nullptr;       // e4m3 weights and scales of compute_dtype 4 (forward_fp8.cu)
@@ -153,7 +166,9 @@ bool fp8_calibrated(const crnn_model* m);
 int fp8_prepare(crnn_model* m, cudaStream_t st);
 int fp8_plan_maps(Plan& pl);
 int fp8_conv2(crnn_model* m, convsw::Params p, bool lines, int sms, cudaStream_t st);
-int fp8_conv_gemm(crnn_model* m, int layer, gemm::Params p, bool lines, int sms, cudaStream_t st);
+// moving = true (layers 2, 3): conv4_x with the folded BatchNorm, e4m3 a4a (EPI_RELU) / pooled a4b (EPI_RELU_POOL12) out
+int fp8_conv_gemm(crnn_model* m, int layer, gemm::Params p, bool lines, int sms, cudaStream_t st, bool moving = false);
+int fp8_fold_moving(crnn_model* m, bool refolded, cudaStream_t st);   // colscale of conv4_x times the moving-statistics scale
 int fp8_bn_apply(crnn_model* m, int layer, const float* bn, bool lines, cudaStream_t st);
 int fp8_conv5(crnn_model* m, gemm::Params p, int sms, cudaStream_t st);
 int fp8_finish_calibration(crnn_model* m, cudaStream_t st);
@@ -170,6 +185,7 @@ int dp_allreduce_bn_finalize(crnn_model* m, double* stats, double count_global, 
 size_t layout_plan(Plan& pl, int N, int W, uint8_t* base, bool train);
 int prepare_weights(crnn_model* m, cudaStream_t st);
 int ensure_plan(crnn_model* m, int N, int W, void* ws, cudaStream_t st);
+int bn_fold_moving(crnn_model* m, bool* refolded, cudaStream_t st);
 
 static inline gemm::Params conv_params(int N, int H, int Wd, int Cin, int Cout, int block_n, const float* bias, void* out,
                                        int merged = 0) {

@@ -19,6 +19,11 @@ SOLVER_SLOTS = {"Adam": (("adam_m", "adam_m"), ("adam_v", "adam_v")),
 # tf.train.RMSPropOptimizer defaults: the reference constructs it with the learning rate alone (lib/lstm/train.py:75)
 RMS_DECAY, RMS_MOMENTUM, RMS_EPSILON = 0.9, 0.0, 1e-10
 # the five e4m3 GEMMs of compute_dtype "fp8": layer -> (K, Cout) of its [Cout][K] weight operand
+# moving BatchNorm statistics of conv4_1 / conv4_2 under their TF names (buffer [layer][mean, variance][512]), tracked with
+# tf.contrib.layers.batch_norm's default decay
+BN_MOVING_KEYS = ("conv4_1/conv4_1/moving_mean", "conv4_1/conv4_1/moving_variance",
+                  "conv4_2/conv4_2/moving_mean", "conv4_2/conv4_2/moving_variance")
+BN_MOVING_DECAY = 0.999
 FP8_WEIGHTS = OrderedDict([("conv3_1", (1152, 256)), ("conv3_2", (2304, 256)), ("conv4_1", (2304, 512)), ("conv4_2", (4608, 512)),
                            ("conv5", (2048, 512))])
 
@@ -62,6 +67,15 @@ class CrnnModel:
         self.solver = "Adam"
         self.momentum = 0.9
         self._bind()
+        # moving statistics (bf16 and fp8 models): always bound, so every training step tracks them; evaluation uses them after
+        # set_bn_statistics("moving")
+        self.bn_statistics = "batch"
+        self.bn_moving = None
+        if self.compute_dtype in (1, 4):
+            self.bn_moving = torch.empty((2, 2, 512), dtype=torch.float32, device=self.device)
+            self.bn_moving[:, 0].zero_()
+            self.bn_moving[:, 1].fill_(1.0)
+            check(self.lib.crnn_model_bind_bn_moving(h, self.bn_moving.data_ptr(), BN_MOVING_DECAY))
         self._ws = None
         self._ws_key = None
         self._ws_lines = False
@@ -162,10 +176,49 @@ class CrnnModel:
     def state_dict(self):
         return OrderedDict((k, self.tensor(k).detach().cpu().numpy().copy()) for k in self.table)
 
+    # ---- moving BatchNorm statistics ----------------------------------------------------------
+    def _moving_buffer(self):
+        if self.bn_moving is None:
+            raise CrnnError("moving BatchNorm statistics exist on the bf16 and fp8 models only")
+        return self.bn_moving
+
+    def bn_moving_state(self):
+        """{TF name (BN_MOVING_KEYS): float32 [512]} of the moving statistics; synchronises the device."""
+        b = self._moving_buffer().detach().cpu().numpy()
+        return OrderedDict((k, b[i // 2, i % 2].copy()) for i, k in enumerate(BN_MOVING_KEYS))
+
+    def load_bn_moving(self, state=None):
+        """Set the moving statistics from {TF name: [512]} (all four BN_MOVING_KEYS), or, with None, to TF's initial values
+        (mean 0, variance 1).  Invalidates fp8 scales, as a parameter change does."""
+        b = self._moving_buffer()
+        if state is None:
+            b[:, 0].zero_()
+            b[:, 1].fill_(1.0)
+        else:
+            missing = [k for k in BN_MOVING_KEYS if k not in state]
+            if missing:
+                raise KeyError(f"moving statistics missing: {missing}")
+            for i, k in enumerate(BN_MOVING_KEYS):
+                b[i // 2, i % 2].copy_(torch.as_tensor(np.asarray(state[k], dtype=np.float32).reshape(512)).to(self.device))
+        check(self.lib.crnn_model_params_changed(self.handle))
+        self.fp8_calibrated = False
+
+    def set_bn_statistics(self, mode):
+        """"batch" (default, the reference): conv4_1 / conv4_2 normalise with the statistics of the evaluated batch (each line's
+        own in forward_lines).  "moving": evaluation forwards normalise with the moving statistics training tracked, folded into
+        the conv weights and bias; training forwards always use batch statistics.  A change invalidates fp8 scales."""
+        if mode not in ("batch", "moving"):
+            raise CrnnError(f"BN statistics must be 'batch' or 'moving', got {mode!r}")
+        check(self.lib.crnn_model_set_bn_statistics(self.handle, 1 if mode == "moving" else 0))
+        if mode != self.bn_statistics:
+            self.fp8_calibrated = False
+            self._ws_key = None            # a packed-evaluation workspace has a mode-dependent size
+        self.bn_statistics = mode
+
     # ---- forward ----------------------------------------------------------------------------
     def _workspace(self, N, W, lines=False):
         # a packed-evaluation workspace holds the inference plan too, so it serves both forwards (and the taps after either)
-        key = (N, W, self.training)
+        key = (N, W, self.training, self.bn_statistics)
         if self._ws_key != key or (lines and not self._ws_lines):
             nbytes = _lib.c_size_t()
             if lines:
@@ -317,6 +370,9 @@ class CrnnModel:
         shapes = {"bn": ((2, 4, 512), torch.float32), "stats": ((2, 2, 512), torch.float64)}
         if lines:
             shapes = {"bn": ((2, N, 4, 512), torch.float32), "stats": ((2, N, 2, 512), torch.float64)}
+        # folded operands of the moving statistics (bf16 and fp8 models): W' [Cout][K] bf16, b' [2][512] f32
+        shapes.update({"moving_w_conv4_1": ((512, 2304), torch.bfloat16), "moving_w_conv4_2": ((512, 4608), torch.bfloat16),
+                       "moving_bias": ((2, 512), torch.float32), "fp8_colscale_moving": ((2, 512), torch.float32)})
         if self.compute_dtype == 1:
             shapes.update({"am1": ((N, H1, 16, 64), torch.uint8), "am2": ((N, H2, 8, 128), torch.uint8),
                            "am3": ((N, H2, 4, 256), torch.uint8), "csave": ((2 * Npad // 128, T, 64, 128, 4), torch.float32)})

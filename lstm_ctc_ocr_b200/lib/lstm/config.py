@@ -51,7 +51,10 @@ _DEFAULTS = {
     "TEST": {"BATCH_SIZE": 64,
              # not in the reference: "fp8" evaluates LSTM_test networks with e4m3 operands in conv3_1 .. conv5 (compute_dtype 4),
              # calibrated on a fixed rendered set when the weights are assigned
-             "COMPUTE_DTYPE": "bf16"},
+             "COMPUTE_DTYPE": "bf16",
+             # not in the reference (it evaluates with is_training=True): "moving" normalises conv4_1 / conv4_2 of LSTM_test networks
+             # with the moving mean / variance training tracks (TF's is_training=False); "batch" with the evaluated batch's statistics
+             "BN_STATS": "batch"},
 }
 
 

@@ -14,6 +14,7 @@ import re
 
 import numpy as np
 
+from ... import engine
 from ...session import Session
 from ..networks.network import Fetch
 from .config import cfg
@@ -80,6 +81,8 @@ class SolverWrapper(object):
         path = os.path.join(self.output_dir, filename)
         eng = sess.engine_for(self.net)
         blob = dict(eng.state_dict())
+        if getattr(eng, "bn_moving", None) is not None:
+            blob.update(eng.bn_moving_state())          # moving_mean / moving_variance of conv4_1, conv4_2 under TF's names
         if eng.adam_m is not None:
             blob.update(slot_arrays(eng))
         blob["global_step"] = np.array(getattr(self, "_global_step", Variable(0)).eval())
@@ -101,6 +104,8 @@ class SolverWrapper(object):
         blob = np.load(path + ".npz")
         eng = sess.engine_for(self.net)
         eng.load_params({k: blob[k] for k in eng.table})
+        if getattr(eng, "bn_moving", None) is not None:
+            restore_bn_moving(eng, blob)
         loaded = getattr(sess, "params_loaded", None)     # Session: an fp8 evaluation engine recalibrates for the restored weights
         if loaded is not None:
             loaded(self.net)
@@ -217,6 +222,19 @@ def slot_arrays(eng):
             n = int(np.prod(shp))
             out[prefix + "/" + k] = buf[off:off + n].view(*shp).cpu().numpy()
     return out
+
+
+def restore_bn_moving(eng, blob):
+    """Moving statistics from a checkpoint that holds them; an older one leaves TF's initial values (mean 0, variance 1), so it
+    still resumes -- but an engine that evaluates with moving statistics refuses it: untrained statistics are a mistake."""
+    files = set(getattr(blob, "files", blob))
+    if all(k in files for k in engine.BN_MOVING_KEYS):
+        eng.load_bn_moving({k: blob[k] for k in engine.BN_MOVING_KEYS})
+        return
+    if eng.bn_statistics == "moving":
+        raise KeyError("cfg.TEST.BN_STATS is 'moving' but the checkpoint holds no moving statistics ({})".format(
+            ", ".join(engine.BN_MOVING_KEYS)))
+    eng.load_bn_moving(None)
 
 
 def restore_slots(eng, blob):

@@ -235,12 +235,18 @@ class Session(object):
         eng = self._engines.get(id(net))
         if eng is None:
             from .lib.lstm.config import cfg
-            # evaluation networks run in cfg.TEST.COMPUTE_DTYPE ("bf16" or "fp8"); training networks ignore the key
-            dt = str(cfg.TEST.get("COMPUTE_DTYPE", "bf16")) if type(net).__name__ == "LSTM_test" else "bf16"
+            # evaluation networks run in cfg.TEST.COMPUTE_DTYPE ("bf16" or "fp8") and normalise conv4_x with cfg.TEST.BN_STATS
+            # ("batch" or "moving"); training networks ignore both keys
+            test = type(net).__name__ == "LSTM_test"
+            dt = str(cfg.TEST.get("COMPUTE_DTYPE", "bf16")) if test else "bf16"
             if dt not in ("bf16", "fp8"):
                 raise ValueError(f"cfg.TEST.COMPUTE_DTYPE must be 'bf16' or 'fp8', got {dt!r}")
+            bn = str(cfg.TEST.get("BN_STATS", "batch")) if test else "batch"
+            if bn not in ("batch", "moving"):
+                raise ValueError(f"cfg.TEST.BN_STATS must be 'batch' or 'moving', got {bn!r}")
             eng = engine.CrnnModel(weight_decay=float(getattr(net, "_wd", cfg.TRAIN.WEIGHT_DECAY)), device=self.device,
                                    compute_dtype=dt)
+            eng.set_bn_statistics(bn)
             self._engines[id(net)] = eng
         return eng
 
@@ -253,6 +259,11 @@ class Session(object):
             elif not ignore_missing:
                 raise KeyError(k)
         eng.load_params(full)
+        # moving statistics under their TF names (engine.BN_MOVING_KEYS) when given; required by an engine that evaluates with them
+        if all(k in state_dict for k in engine.BN_MOVING_KEYS):
+            eng.load_bn_moving(state_dict)
+        elif eng.bn_statistics == "moving" and not ignore_missing:
+            raise KeyError("cfg.TEST.BN_STATS is 'moving' but no moving statistics were given ({})".format(", ".join(engine.BN_MOVING_KEYS)))
         self.params_loaded(net)
 
     def params_loaded(self, net):

@@ -62,7 +62,8 @@ def ulp_tf32(x):
     return 2.0 ** (np.floor(np.log2(a)) - 10)
 
 
-_COUNTS = ("mismatches", "out_of_range", "wrong_clear", "wrong_near_tie", "live")
+_COUNTS = ("mismatches", "out_of_range", "wrong_clear", "wrong_near_tie", "live", "carry_recovered", "carry_fallbacks",
+           "near_midpoint_partials")
 
 
 def _larger(new, old):
@@ -168,6 +169,36 @@ class Checker:
             kv.update(rel_l2=en / max(rn, 1e-30), l2_limit=self.l2_limit.get(key or stage, 1e-4), _err_sq=en * en,
                       _ref_sq=rn * rn)
         self._record(stage, float(ratio.max()), **kv)
+
+    def close_allow(self, stage, gpu, ref, acc, allow, mask, key=None, axes=None, origin=None, **counts):
+        """A stored output whose reference leaves some of the kernel's roundings to a per-element allowance `allow`
+        (stage_refs.bptt_steps_isolated): bound ulps * ulp(|ref| + allow) + allow + c * acc on the elements where `mask`
+        holds (the ulp of the largest value the kernel's result may take before it is stored).
+        c_needed is the part of the error neither the ulps nor the allowance cover, over acc.  Torch tensors of one shape
+        (acc, allow, mask broadcast to it).  axes names the dimensions for the worst element's coordinates (worst_at), and
+        origin is added to them (the first image of a chunk).  counts: extra totals for the row (_COUNTS)."""
+        ulps, c = self.bounds[key or stage]
+        r = ref.to(torch.float64)
+        g = gpu.to(r.device, torch.float64)
+        a = acc.to(r.device, torch.float64).expand(r.shape)
+        al = allow.to(r.device, torch.float64).expand(r.shape)
+        m = mask.to(r.device).expand(r.shape)
+        if not bool(m.any()):
+            return
+        zero = r.new_zeros(())
+        err = torch.where(m, (g - r).abs(), zero)
+        share = ulps * self.ulp(r.abs() + al) + al          # the allowance may carry the stored value up a binade
+        ratio = torch.where(m, err / (share + c * a + 1e-30), zero)
+        ratio = torch.where(torch.isnan(ratio), float("inf"), ratio)                 # a NaN from the GPU is the worst
+        i = int(ratio.reshape(-1).argmax())
+        at = [int(v) for v in np.unravel_index(i, tuple(r.shape))]
+        at = [v + int(o) for v, o in zip(at, origin or [0] * len(at))]
+        kv = dict(max_abs_err=float(err.max()), worst_gpu=float(g.reshape(-1)[i]), worst_ref=float(r.reshape(-1)[i]),
+                  worst_acc=float(a.reshape(-1)[i]), worst_allow=float(al.reshape(-1)[i]),
+                  worst_at=dict(zip(axes or [f"dim{k}" for k in range(len(at))], at)), ulps=ulps, c=c,
+                  c_needed=float(torch.where(m, (err - share).clamp_min(0.0) / a.clamp_min(1e-300), zero).max()),
+                  **counts)
+        self._record(stage, float(ratio.reshape(-1)[i]), **kv)
 
     def close_scaled(self, stage, gpu, ref, mask=None, key=None):
         """Recurrence / BPTT: bound ulps * ulp(|ref|) + c * max|ref|."""

@@ -467,10 +467,12 @@ def bptt_stage(d_out, gates, c_steps, wh_fw, wh_bw, lens, T, dz_in=None, rnd=bf1
     """Backward recurrence of both directions.  gates [2, N, T, 4, 256] / c_steps [2, N, T, 256] are the saved per-step
     values, d_out [N, H2, 512] the gradient w.r.t. lstm_out.  dz of step s+1 enters step s through W_h^T: taken from
     `dz_in` (the workspace's dz_all: the bf16 values the kernel exchanged) when given, else rnd(own result).
-    Returns dz_all [N, H2, 2048] in frame order with permuted gate columns (zero for frames >= len)."""
+    Returns dz_all [N, H2, 2048] in frame order with permuted gate columns (zero for frames >= len), and the cell gradient
+    dc of every step [2, N, T, 256] (zero for steps >= len)."""
     N, H2, _ = d_out.shape
     L = torch.as_tensor(clamp_lens(lens, T), device=d_out.device)
     dz_all = d_out.new_zeros((N, H2, 2048))
+    dcs = d_out.new_zeros((2, N, T, HID))
     ar = torch.arange(N, device=d_out.device)
     for d, wh in enumerate((wh_fw, wh_bw)):
         dz_next = d_out.new_zeros((N, 1024))
@@ -495,7 +497,141 @@ def bptt_stage(d_out, gates, c_steps, wh_fw, wh_bw, lens, T, dz_in=None, rnd=bf1
             else:
                 dz_next = rnd(dz)
             dc_next, f_next = torch.where(m, dc, zero), torch.where(m, f, zero)
-    return dict(dz=dz_all)
+            dcs[d, :, s] = dc_next
+    return dict(dz=dz_all, dc=dcs)
+
+
+# tanh.approx.f32 (ptx.cuh: fast_tanh): the PTX ISA states a maximum relative error of 2^-10.987 for the .f32 type
+D_TANH = 2.0 ** -10.987
+# The f32 accumulation of one 128-deep partial product of the BPTT exchange: 8 wgmma k-steps, each losing at most one f32
+# ulp of the partial sum (2^-23 of acc, test_gpu_stage_isolation_batch.py), so at most 2^-20 of acc.  A partial whose fp64
+# value lies within 4x that (2^-18 of acc) of a bf16 rounding midpoint is allowed to round either way.
+MMA_WINDOW = 2.0 ** -18
+# relative error of a value recovered from its bf16 round-to-nearest-even q: |x - q| <= 2^-8 |x| <= 2^-8 / (1 - 2^-8) |q|
+R_BF16 = 2.0 ** -8 / (1.0 - 2.0 ** -8)
+
+
+def ulp_bf16(x):
+    """One bf16 ulp of |x| (2^(floor(log2 |x|) - 7), |x| at least 2^-126), fp64 on x's device."""
+    return torch.ldexp(torch.ones_like(x), torch.frexp(x.abs().clamp_min(2.0 ** -126)).exponent - 8)
+
+
+def _shift_next(x):
+    """x of step s+1 at step s along axis 1 (zero at the last step)."""
+    out = torch.zeros_like(x)
+    out[:, :-1] = x[:, 1:]
+    return out
+
+
+def bptt_steps_isolated(d_out, gates, c_steps, wh_fw, wh_bw, dz_all, lens, T, rnd=bf16):
+    """Every BPTT step on its own operands, the GPU's dz_all [N, H2, 2048] among them: nothing carries from step to step,
+    so a wrong step fails at that step.  Step s of direction d (frame s forward, len-1-s backward; active while s < len):
+      exchange  dh = d_out[frame] + sum_r rnd(p_r): p_r = the GPU's dz of step s+1 (zero when s+1 >= len) restricted to the
+                permuted gate columns r*128 .. r*128+127 (rank r of the cluster) times to_perm(W_h) over those columns,
+                rounded to bf16 by the rank before the f32 sum (lstm_bwd.cuh);
+      o         dz_o = dh tanh(c_s) o(1-o) on the saved gates / cell state;
+      carry     dc_s = dc_{s+1} f_{s+1} + dh o (1 - tanh(c_s)^2), dc_{s+1} recovered from the GPU's stored dz of step s+1
+                as dz_j / (i(1-j^2)) or dz_i / (j i(1-i)), whichever factor is larger (zero at s = len-1).  Where both
+                factors are zero the reference's own dc_{s+1} is carried instead, with its allowance (`fallback`);
+      i, j, f   dz_i = dc j i(1-i), dz_j = dc i(1-j^2), dz_f = dc c_{s-1} f(1-f) (c_{-1} = 0).
+    gates [2, N, T, 4, 256], c_steps [2, N, T, 256]: the saved per-step values; d_out [N, H2, 512].  Returns per step
+    [2, N, T, 4, 256] (TF gate order i, j, f, o): dz (the reference), gpu (the GPU's dz of that step), allow (what the
+    kernel's roundings the reference does not restate can move: a partial within MMA_WINDOW of a bf16 rounding midpoint
+    (one ulp of it), the bf16-stored dz the carry is recovered from (R_BF16), tanh.approx (D_TANH)), acc (the same
+    expressions on absolute values, the scale of the f32 arithmetic); active [2, N, T]; dc / dc_hat [2, N, T, 256] (the
+    reference's dc and the dc recovered from the GPU's dz of each step), recovered / fallback [2, N, T, 256] (where the
+    carry INTO a step was recovered / carried), near_midpoint [2, N, T, 256] (partials with a one-ulp allowance).
+    rnd = ident: the partials are not rounded (the fp64 chain of tests/test_stage_refs_cpu.py)."""
+    N = d_out.shape[0]
+    dev = d_out.device
+    L = torch.as_tensor(clamp_lens(lens, T), device=dev)
+    s = torch.arange(T, device=dev)
+    act = s[None, :] < L[:, None]                                             # [N, T]
+    has_next = _shift_next(act)
+    keys = ("dz", "gpu", "allow", "acc", "dc", "dc_hat", "recovered", "fallback", "near_midpoint")
+    out = {k: [] for k in keys}
+    a3 = act[..., None]
+    for d, wh in enumerate((wh_fw, wh_bw)):
+        t_of = _step_frames(L[:, None], s[None, :], d)                       # [N, T]
+        zp = torch.gather(dz_all[:, :, d * 1024:(d + 1) * 1024], 1, t_of[..., None].expand(N, T, 1024))
+        zp = torch.where(a3, zp, zp.new_zeros(()))                           # the GPU's dz per step, permuted columns
+        # ---- exchange: the 8 ranks' partial products of dz_{s+1}, each rounded to bf16, summed
+        znr = _shift_next(zp).reshape(N, T, 8, 128)
+        whp = to_perm(wh).reshape(HID, 8, 128)
+        p = torch.einsum("ntrk,urk->ntru", znr, whp)                          # [N, T, 8 ranks, 256 units]
+        window = MMA_WINDOW * torch.einsum("ntrk,urk->ntru", znr.abs(), whp.abs())
+        del znr
+        near = (bf16(p - window) != bf16(p + window)) if rnd is not ident else torch.zeros_like(p, dtype=torch.bool)
+        allow_x = torch.where(near, ulp_bf16(p.abs() + window), p.new_zeros(())).sum(2)
+        del window
+        q = rnd(p)
+        del p
+        rec, rec_acc = q.sum(2), q.abs().sum(2)
+        del q
+        dh = torch.gather(d_out[..., d * HID:(d + 1) * HID], 1, t_of[..., None].expand(N, T, HID))
+        zero = dh.new_zeros(())
+        dht = torch.where(a3, dh + rec, zero)
+        dht_acc = torch.where(a3, dh.abs() + rec_acc, zero)
+        allow_x = torch.where(a3, allow_x, zero)
+        i, j, f, o = (torch.where(a3, g, zero) for g in gates[d].unbind(-2))
+        c = torch.where(a3, c_steps[d], zero)
+        cp = torch.zeros_like(c)
+        cp[:, 1:] = c[:, :-1]
+        tc = torch.tanh(c)
+        # ---- o column: nothing carried
+        so = o * (1 - o)
+        ref_o = dht * tc * so
+        allow_o = allow_x * (tc * so).abs() + D_TANH * ref_o.abs()
+        acc_o = dht_acc * (tc * so).abs()
+        # ---- carry: dc of step s+1 recovered from the GPU's stored dz_j / dz_i of that step
+        zs = from_perm(zp)
+        fi, fj = j * i * (1 - i), i * (1 - j * j)
+        use_j = fj.abs() >= fi.abs()
+        fac = torch.where(use_j, fj, fi)
+        ok = fac != 0
+        dc_hat = torch.where(ok, torch.where(use_j, zs[..., HID:2 * HID], zs[..., :HID]) / torch.where(ok, fac, 1.0), zero)
+        dch_n, f_n, ok_n = _shift_next(dc_hat), _shift_next(f), _shift_next(ok)
+        hn = has_next[..., None]
+        rec_ok, fb = hn & ok_n, hn & ~ok_n
+        carry_r = torch.where(rec_ok, dch_n * f_n, zero)
+        allow_cr = R_BF16 * carry_r.abs()
+        acc_cr = carry_r.abs()
+        sd = 1 - tc * tc
+        d_own = dht * o * sd
+        allow_own = allow_x * (o * sd).abs() + 2 * D_TANH * (1 + D_TANH) * (dht * o).abs() * tc * tc
+        acc_own = dht_acc * o.abs() * (1 + tc * tc)
+        dc, a_dc, acc_dc = carry_r + d_own, allow_cr + allow_own, acc_cr + acc_own
+        if bool(fb.any()):
+            # carried where nothing can be recovered: the reference's own dc_{s+1}, its allowance times f_{s+1}; a run of k
+            # such steps settles after k + 1 passes
+            for _ in range(T + 1):
+                nxt = (torch.where(fb, _shift_next(dc) * f_n, carry_r) + d_own,
+                       torch.where(fb, _shift_next(a_dc) * f_n.abs(), allow_cr) + allow_own,
+                       torch.where(fb, _shift_next(acc_dc) * f_n.abs(), acc_cr) + acc_own)
+                done = all(torch.equal(x, y) for x, y in zip(nxt, (dc, a_dc, acc_dc)))
+                dc, a_dc, acc_dc = nxt
+                if done:
+                    break
+        ref, allow, acc = [], [], []
+        for fc in (fi, fj, cp * f * (1 - f)):
+            ref.append(dc * fc)
+            allow.append(a_dc * fc.abs())
+            acc.append(acc_dc * fc.abs())
+        ref.append(ref_o)
+        allow.append(allow_o)
+        acc.append(acc_o)
+        out["dz"].append(torch.stack(ref, -2))
+        out["allow"].append(torch.stack(allow, -2))
+        out["acc"].append(torch.stack(acc, -2))
+        out["gpu"].append(zs.reshape(N, T, 4, HID))
+        out["dc"].append(torch.where(a3, dc, zero))
+        out["dc_hat"].append(dc_hat)
+        out["recovered"].append(rec_ok)
+        out["fallback"].append(fb)
+        out["near_midpoint"].append(near.sum(2) if rnd is not ident else torch.zeros_like(rec, dtype=torch.long))
+    r = {k: torch.stack(v) for k, v in out.items()}
+    r["active"] = act[None].expand(2, N, T)
+    return r
 
 
 def lstm_grads_stage(dz_all, a5, lstm_out, wx_fw, wx_bw, wh_fw, wh_bw):

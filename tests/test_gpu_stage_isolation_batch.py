@@ -135,6 +135,11 @@ def _ref_self_check(ck, F_):
         dz = S.bptt_stage(g("d_lstm_out"), steps("gates_steps"), steps("csave_steps"), wh[0], wh[1], lens, T,
                           dz_in=g("dz_all"))["dz"]
         r["dz_all"] = dict(out=dz, acc=dz.abs().max())
+        bs = S.bptt_steps_isolated(g("d_lstm_out"), steps("gates_steps"), steps("csave_steps"), wh[0], wh[1], g("dz_all"),
+                                   lens, T)
+        r["bptt_steps"] = dict(out=bs["dz"], acc=bs["acc"])
+        r["bptt_steps_allow"] = dict(out=bs["allow"], acc=bs["allow"])
+        del bs
         c = S.conv_bwd(g("d_pre2"), g("conv1"), Wb["conv2/weights"])
         r["d_a1"] = dict(out=c["dx"], acc=c["dx_acc"])
         r["conv2/weights"] = dict(out=c["dw"], acc=c["dw_acc"])

@@ -12,7 +12,8 @@ of at least MIN_SHARE of every weight tensor (else a stale bf16 operand cache wo
 checked per element against fp64 on the kernel's own inputs (test_gpu_solvers.py's convention, MEASURED below), the
 simulated data-parallel call bit for bit against the single-device one, total_loss against mean(costs) + wd * 1/2 sum w^2 of
 the parameters that step's forward ran with, and last_grad_norm against the fp64 norm of the finished gradient.  A control
-shows the check sees a stale cache: parameters rewritten in place without crnn_model_params_changed fail it.
+shows the check sees a stale cache: parameters rewritten in place without crnn_model_params_changed fail it, and so does
+W_h alone 1 % off, through the recurrence's and the BPTT's per-step checks.
 
 NaN-filled buffers: a buffer filled with 0xFF bytes holds NaN as bf16, f32 and f64.  Before first use the engine's
 workspace and every caller-owned output (logits, CTC costs / gradient / workspace, greedy and beam outputs, the beam arena)
@@ -220,42 +221,59 @@ def test_training_run_checks_every_stage_and_update(solver):
     assert not fail, "\n".join(fail)
 
 
-def _perturb_in_place(m, rel=0.05, seed=3):
+def _perturb_in_place(m, rel=0.05, seed=3, names=None):
     """New f32 parameters written into m.params in place, without crnn_model_params_changed (the misuse include/crnn_ctc.h
-    documents): every weight scaled by 1 + rel * U(-1, 1)."""
+    documents): every weight (or the tensors `names`, name -> row slice) scaled by 1 + rel * U(-1, 1)."""
     gen = torch.Generator(device=DEV).manual_seed(seed)
-    m.params.mul_(1.0 + rel * (2.0 * torch.rand(m.params.shape, generator=gen, device=DEV) - 1.0))
+    for w in [m.params] if names is None else [m.tensor(k)[rows] for k, rows in names.items()]:
+        w.mul_(1.0 + rel * (2.0 * torch.rand(w.shape, generator=gen, device=DEV) - 1.0))
     torch.cuda.synchronize()
 
 
 # the stages that read a bf16 weight cache: the forward's (prepare_weights) and the backward's data gradients
-# (prepare_weights_bwd).  conv1 reads the f32 weights and each bias is read as f32, so they follow the new values.
+# (prepare_weights_bwd), the recurrence's W_h (step_gates, step_c: each step on its own saved inputs) and the BPTT's
+# (bptt_step_o, bptt_step_ijf).  conv1 reads the f32 weights and each bias is read as f32, so they follow the new values.
 STALE_STAGES = ("conv2", "conv3_1", "conv3_2", "a4a_pre", "a4b_pre", "conv5", "xproj", "logits",
-                "d_lstm_out", "d_a5", "d_a4b", "d_pre4a", "d_a3p", "d_pre31", "d_a2", "d_a1")
+                "d_lstm_out", "d_a5", "d_a4b", "d_pre4a", "d_a3p", "d_pre31", "d_a2", "d_a1",
+                "step_gates", "step_c", "bptt_step_o", "bptt_step_ijf")
+# only the recurrent weights W_h of both directions, 1 % off: the forward's and the backward's per-step checks see it
+STALE_WH = {B.FW + "/weights": slice(512, 768), B.BW + "/weights": slice(512, 768)}
+STALE_WH_STAGES = ("step_c", "bptt_step_o")
 
 
-def test_stage_check_sees_a_stale_weight_cache():
-    """Control: after a forward and backward, parameters rewritten in place without crnn_model_params_changed leave the bf16
-    caches of both passes stale; the same stage check must then fail on every conv stage that reads a cache, xproj, logits and
-    the data gradients.  After params_changed it passes."""
+def _stale_cache_control(tag, must_fail, rel, names=None):
+    """After a forward and backward, parameters rewritten in place without crnn_model_params_changed leave the bf16 caches
+    stale: the stage check must fail on every stage of `must_fail`, and pass again after params_changed."""
     from lstm_ctc_ocr_b200._lib import check
     m, pn = _model("Adam")
     N, W, widths = RUN[1]
     batch = _batch(N, W, widths)
-    ck = _checker("stale/fresh")
+    ck = _checker(f"{tag}/fresh")
     B._check_step(m, _params_now(m), batch, ck.case, dev=DEV, ck=ck)
     ck.assert_ok()
-    _perturb_in_place(m)
-    ck = _checker("stale/in_place")
+    _perturb_in_place(m, rel, names=names)
+    ck = _checker(f"{tag}/in_place")
     B._check_step(m, _params_now(m), batch, ck.case, dev=DEV, ck=ck)
     ck.report()
     rows = {r["stage"]: r for r in ck.rows}
-    passed = [s for s in STALE_STAGES if rows[s]["max_ratio"] <= 1.0]
+    passed = [s for s in must_fail if rows[s]["max_ratio"] <= 1.0]
     assert not passed, f"a stale bf16 cache went unnoticed in {passed}"
     check(m.lib.crnn_model_params_changed(m.handle))
-    ck = _checker("stale/params_changed")
+    ck = _checker(f"{tag}/params_changed")
     B._check_step(m, _params_now(m), batch, ck.case, dev=DEV, ck=ck)
     ck.assert_ok()
+
+
+def test_stage_check_sees_a_stale_weight_cache():
+    """Control: every parameter 5 % off in place.  The check must fail on every conv stage that reads a cache, xproj,
+    logits, the data gradients, and the recurrence's and the BPTT's per-step checks."""
+    _stale_cache_control("stale", STALE_STAGES, 0.05)
+
+
+def test_stage_check_sees_stale_recurrent_weights():
+    """Control: only W_h of both LSTM directions 1 % off in place.  The recurrence's step_c and the BPTT's bptt_step_o must
+    fail; the report's dz_all row shows how far the free-running BPTT check stays from noticing."""
+    _stale_cache_control("stale_wh", STALE_WH_STAGES, 0.01, STALE_WH)
 
 
 def test_training_run_at_batch_scale():

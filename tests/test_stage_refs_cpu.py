@@ -199,6 +199,34 @@ def _check_backward_chain(c):
     assert len(got) == len(G) - 2
 
 
+def test_bptt_steps_reproduce_the_chain(chain):
+    _check_bptt_steps(chain)
+
+
+def test_bptt_steps_at_edge_widths(edge_chain):
+    _check_bptt_steps(edge_chain)
+
+
+def _check_bptt_steps(c):
+    """Fed the fp64 chain's own values (no rounding; dz from bptt_stage itself), every isolated BPTT step reproduces
+    bptt_stage, and the dc recovered from each step's dz equals the chain's dc wherever a successor recovers it."""
+    r = _forward_chain(c)
+    P, T, H2, tsl = c["P"], c["T"], c["H2"], c["tsl"]
+    wh = (P[f"{FW}/weights"][512:], P[f"{BW}/weights"][512:])
+    d_out = S.logits_bwd(r["rec"]["out"], S.dl_rows_stage(c["dlogits"], H2)["dl_rows"], P["logits/weights"])["d_lstm_out"]
+    bp = S.bptt_stage(d_out, r["rec"]["gates"], r["rec"]["c"], wh[0], wh[1], tsl, T, rnd=S.ident)
+    bs = S.bptt_steps_isolated(d_out, r["rec"]["gates"], r["rec"]["c"], wh[0], wh[1], bp["dz"], tsl, T, rnd=S.ident)
+    act = bs["active"]
+    assert rel(bs["dz"][act], bs["gpu"][act]) < 1e-12
+    assert rel(bs["dc"][act], bp["dc"][act]) < 1e-12
+    rec = bs["recovered"][:, :, :-1]                   # the carry into step s recovered from step s+1
+    assert int(bs["fallback"].sum()) == 0
+    assert int(rec.sum()) == int(act[:, :, 1:].sum()) * S.HID
+    if T > 1:
+        assert rel(bs["dc_hat"][:, :, 1:][rec], bp["dc"][:, :, 1:][rec]) < 1e-12
+    assert torch.equal(bs["dz"][:, :, 0, 2][act[:, :, 0]], torch.zeros_like(bs["dz"][:, :, 0, 2][act[:, :, 0]]))
+
+
 # ---------------------------------------------------------------------------------------------------------- f32-class path
 def _zero_pair(x):
     return (x, torch.zeros_like(x))

@@ -200,6 +200,15 @@ class Checker:
                   **counts)
         self._record(stage, float(ratio.reshape(-1)[i]), **kv)
 
+    def l2(self, stage, gpu, ref, key=None):
+        """The relative L2 of an f32 output against its reference on its own, limit l2_limit[key or stage] (the
+        per-element bounds are other stages' rows).  Torch tensors."""
+        r = ref.to(torch.float64)
+        g = gpu.to(r.device, torch.float64)
+        en, rn = float(torch.linalg.vector_norm(g - r)), float(torch.linalg.vector_norm(r))
+        self._record(stage, 0.0, rel_l2=en / max(rn, 1e-30), l2_limit=self.l2_limit.get(key or stage, 1e-4), _err_sq=en * en,
+                     _ref_sq=rn * rn)
+
     def close_scaled(self, stage, gpu, ref, mask=None, key=None):
         """Recurrence / BPTT: bound ulps * ulp(|ref|) + c * max|ref|."""
         if isinstance(ref, torch.Tensor):

@@ -35,7 +35,9 @@ def test_tcgen05_gemm(bn, M, Nc, K):
     assert rel(D.cpu(), ref.cpu()) < 2e-5
 
 
-def _ctc_case(T, N, lens, ilens, seed, scale=2.0):
+def _ctc_case(T, N, lens, ilens, seed, scale=2.0, blank=0):
+    """Label ids 1 .. 62, except that a blank other than 0 takes the place of the blank's own id: it becomes 0, and ids
+    2, 3 become a repeated pair of 0."""
     from oracle import crnn_oracle as O
     rng = np.random.default_rng(seed)
     x = (rng.standard_normal((T, N, 64)) * scale).astype(np.float32)
@@ -43,12 +45,16 @@ def _ctc_case(T, N, lens, ilens, seed, scale=2.0):
     lab = rng.integers(1, 63, size=int(ll.sum())).astype(np.int32)
     if lab.size > 1:
         lab[1] = lab[0]                 # a repeated label
-    return x, lab, ll, il, O.ctc_loss_np(x, lab, ll, il)
+    if blank != 0:
+        lab[lab == blank] = 0
+        lab[2:4] = 0
+    return x, lab, ll, il, O.ctc_loss_np(x, lab, ll, il, blank=blank)
 
 
+@pytest.mark.parametrize("blank", [0, 17, 63])
 @pytest.mark.parametrize("kernel", ["fast", "fast-me", "tma", "tma-me", "generic"])
 @pytest.mark.parametrize("case", ["ragged", "edge", "two_warp", "many_frames", "long_ks2", "long_ks4"])
-def test_ctc_loss_and_grad_vs_oracle(case, kernel, monkeypatch):
+def test_ctc_loss_and_grad_vs_oracle(case, kernel, blank, monkeypatch):
     """ctc_fast_kernel (S <= 32, default: per-thread bulk row copies), ctc_tma_kernel (S <= 32: one tensor-map tile load/store per
     utterance) -- each with the log2-space recursion (default) and the mantissa/exponent recursion (`-me`) -- and the generic
     ctc_loss_kernel<KS> against the fp64 oracle; CRNN_CTC_KERNEL / CRNN_CTC_RECUR select them."""
@@ -77,10 +83,10 @@ def test_ctc_loss_and_grad_vs_oracle(case, kernel, monkeypatch):
     else:
         T, N = 130, 3
         lens = [40, 63, 33]; ilens = [130, 130, 100]
-    x, lab, ll, il, (co, go) = _ctc_case(T, N, lens, ilens, seed=1)
+    x, lab, ll, il, (co, go) = _ctc_case(T, N, lens, ilens, seed=1, blank=blank)
     t = lambda a: torch.tensor(a, device=DEV)
-    c, g = engine.ctc_loss(t(x), t(lab), t(ll), t(il), want_grad=True)
-    c2, _ = engine.ctc_loss(t(x), t(lab), t(ll), t(il), want_grad=False)
+    c, g = engine.ctc_loss(t(x), t(lab), t(ll), t(il), blank=blank, want_grad=True)
+    c2, _ = engine.ctc_loss(t(x), t(lab), t(ll), t(il), blank=blank, want_grad=False)
     assert np.allclose(c.cpu().numpy(), co, rtol=1e-4, atol=1e-4)
     assert np.array_equal(c.cpu().numpy(), c2.cpu().numpy())
     # f32 ex2/lg2.approx recursion: error grows with the chain length (T=130 in the KS=4 case)
@@ -90,6 +96,14 @@ def test_ctc_loss_and_grad_vs_oracle(case, kernel, monkeypatch):
         assert not g[int(il[n]):, n].any()
     if case == "edge":
         assert float(c[1]) == 0.0 and not g[:, 1].any()
+    # the blank as a label id: that utterance alone gets cost NaN and a zero gradient
+    n = int(np.flatnonzero(ll > 0)[0])
+    bad = lab.copy()
+    bad[int(ll[:n].sum())] = blank
+    c3, g3 = engine.ctc_loss(t(x), t(bad), t(ll), t(il), blank=blank, want_grad=True)
+    assert bool(torch.isnan(c3[n])) and not g3[:, n].any()
+    keep = torch.arange(N, device=DEV) != n
+    assert torch.equal(c3[keep], c[keep]) and torch.equal(g3[:, keep], g[:, keep])
 
 
 def test_ctc_fast_kernel_extreme_logits_match_generic(monkeypatch):
@@ -299,6 +313,14 @@ def test_warpctc_drop_in_call_shape_and_autograd():
     xt = torch.tensor(x, device=DEV, requires_grad=True)
     c = warpctc.ctc(xt, lab, ll, il)
     (c * torch.arange(1, N + 1, device=DEV)).sum().backward()                                    # dloss[n] = n+1
+    assert np.abs(xt.grad.cpu().numpy() - go * np.arange(1, N + 1)[None, :, None]).max() < 1e-3
+    # blank_label = 63, with id 0 (a repeated pair of it) among the labels
+    lab[2:4] = 0
+    co, go = O.ctc_loss_np(x, lab, ll, il, blank=63)
+    xt = torch.tensor(x, device=DEV, requires_grad=True)
+    c = warpctc.ctc(xt, lab, ll, il, blank_label=63)
+    (c * torch.arange(1, N + 1, device=DEV)).sum().backward()
+    assert np.allclose(c.detach().cpu().numpy(), co, rtol=1e-4)
     assert np.abs(xt.grad.cpu().numpy() - go * np.arange(1, N + 1)[None, :, None]).max() < 1e-3
 
 

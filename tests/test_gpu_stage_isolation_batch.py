@@ -16,10 +16,10 @@ sampled images (tile edges, the shortest and longest lengths) the same reference
 with the GPU's to 1e-12 of acc.
 
 At c3 the backward is driven by the real CTC gradient of the GPU's own logits (engine.ctc_loss with grad_scale 1/N, as
-the training step runs it), checked against torch's fp64 CTC with autograd through log_softmax: costs to 1e-4 relative,
-the gradient to 2e-4 * grad_scale absolute (tests/test_gpu_parity.py), zero past each length.  Utterances whose labels
-do not fit their length have no finite fp64 cost; there the kernel must give cost 0 and a zero gradient, and that
-gradient, unchanged, drives the backward.  The inference plan (bench.py's) of a fresh model is checked stage by stage as well: conv1 .. conv3_2 equal to
+the training step runs it), checked against tests/ctc_refs.py's fp64 CTC: costs to 1e-4 relative, the gradient per element
+(ctc_grad_softmax, ctc_grad_posterior), zero past each length.  Utterances whose labels do not fit their length have no
+finite fp64 cost; there the kernel must give cost 0 and a zero gradient, and that gradient, unchanged, drives the
+backward.  ctc_long_kernel runs once more on the same logits, its gradient and its stored tables checked too.  The inference plan (bench.py's) of a fresh model is checked stage by stage as well: conv1 .. conv3_2 equal to
 the training plan's taps bit for bit, conv4_x within one bf16 ulp.
 
 Rows go to build/stage_isolation_batch_report.jsonl, with the peak GPU memory of each case."""
@@ -29,9 +29,9 @@ import sys
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import ctc_refs as CR  # noqa: E402
 import stage_refs as S  # noqa: E402
 import test_gpu_stage_isolation as B  # noqa: E402
 from stage_check import Checker, ulp_bf16, widths_of  # noqa: E402
@@ -57,11 +57,14 @@ MEASURED_WGRAD = {
     "conv1/weights": (4.74e-6, 7.56e-6),
 }
 WGRAD = {k: (4.5 * c, max(1e-4, 4.5 * l2)) for k, (c, l2) in MEASURED_WGRAD.items() if 4.5 * c > B.STAGE_BOUNDS["wgrad"][1]}
-# plus the GPU references against the CPU ones, and the CTC bounds of test_gpu_parity.py (cost relative to |cost|,
-# gradient absolute in units of grad_scale; its relative L2 measured 2.4e-5)
+# plus the GPU references against the CPU ones, and the CTC stages of tests/ctc_refs.py (the default kernel and, at c3,
+# ctc_long_kernel): the cost of test_gpu_parity.py relative to |cost| (1e-4), the gradient per element, its relative L2
+# (measured 2.4e-5)
+CTC_KINDS = {"fast": 1e-4, "long": 4.5 * 2.80e-6}
 BOUNDS = dict(B.STAGE_BOUNDS, **{f"wgrad/{k}": (0, c) for k, (c, _) in WGRAD.items()}, ref_cpu=(0, 1e-12),
-              ctc_cost=(0, 1e-4), ctc_grad=(0, 2e-4))
-L2_LIMIT = dict(B.L2_LIMIT, **{f"wgrad/{k}": l2 for k, (_, l2) in WGRAD.items()}, ctc_grad=1.1e-4)
+              **{f"ctc_cost/{k}": (0, c) for k, c in CTC_KINDS.items()},
+              **CR.bounds(CTC_KINDS, {k: 4.5 * CR.MEASURED_POSTERIOR[k] for k in CTC_KINDS}))
+L2_LIMIT = dict(B.L2_LIMIT, **{f"wgrad/{k}": l2 for k, (_, l2) in WGRAD.items()}, **{f"ctc_grad/{k}": 1.1e-4 for k in CTC_KINDS})
 
 CASES = [
     pytest.param(1024, 256, id="c3"),
@@ -83,29 +86,34 @@ def _widths(N, W, seed=11):
     return [cyc[i // 2] if i % 2 == 0 else int(rnd[i]) for i in range(N)]
 
 
-def _ctc_grad(ck, logits, lab, ll, tsl):
-    """engine.ctc_loss on the GPU's logits (grad_scale 1/N) against torch's fp64 CTC; returns the backward's d logits."""
+def _ctc_grad(ck, logits, lab, ll, tsl, long_tables=False):
+    """engine.ctc_loss on the GPU's logits (grad_scale 1/N) against ctc_refs.ctc_fp64; returns the backward's d logits.
+    long_tables: also run ctc_long_kernel (CRNN_CTC_KERNEL=long) on the same logits, its gradient and its stored tables
+    checked as well."""
     from lstm_ctc_ocr_b200 import engine
     T, N, _ = logits.shape
     t = lambda a: torch.tensor(a, device=DEV)
-    costs, grad = engine.ctc_loss(logits, t(lab), t(ll), t(tsl), want_grad=True, grad_scale=1.0 / N,
-                                  max_label_len=int(ll.max()))
-    il = torch.tensor(S.clamp_lens(tsl, T), device=DEV)
-    x = logits.double().requires_grad_(True)
-    args = (t(lab).long(), il, t(ll).long())
-    with torch.no_grad():
-        ok = torch.isfinite(F.ctc_loss(torch.log_softmax(x, 2), *args, blank=0, reduction="none"))
-    ref = F.ctc_loss(torch.log_softmax(x, 2), *args, blank=0, reduction="none", zero_infinity=True)
-    (gref,) = torch.autograd.grad(ref.sum(), x)
-    ref = ref.detach()
-    ck.close("ctc_cost", costs[ok], ref[ok], ref[ok].abs())
-    ck.close("ctc_grad", grad[:, ok], gref[:, ok] / N, 1.0 / N)
-    ck.exact("ctc_grad_past_len_zero", grad[torch.arange(T, device=DEV)[:, None] >= il[None, :]], 0.0)
-    # labels that do not fit their length (warp-ctc's convention): cost 0 and a zero gradient, so they add nothing
-    ck.exact("ctc_infeasible_cost_zero", costs[~ok], 0.0)
-    ck.exact("ctc_infeasible_grad_zero", grad[:, ~ok], 0.0)
-    ck._record("ctc_feasible", 0.0, utterances=int(ok.sum()))
+    m = int(ll.max())
+    costs, grad = engine.ctc_loss(logits, t(lab), t(ll), t(tsl), want_grad=True, grad_scale=1.0 / N, max_label_len=m)
+    ref = CR.ctc_fp64(logits, lab, ll, S.clamp_lens(tsl, T), grad_scale=1.0 / N, max_label_len=m)
+    CR.check_grad(ck, "fast", costs, grad, ref, 1.0 / N)
+    if long_tables:
+        os.environ["CRNN_CTC_KERNEL"] = "long"
+        try:
+            ws = torch.empty(engine.ctc_workspace_bytes(T, N, 64, m), dtype=torch.uint8, device=DEV)
+            c_l, g_l = engine.ctc_loss(logits, t(lab), t(ll), t(tsl), want_grad=True, grad_scale=1.0 / N, max_label_len=m,
+                                       workspace=ws)
+        finally:
+            del os.environ["CRNN_CTC_KERNEL"]
+        CR.check_grad(ck, "long", c_l, g_l, ref, 1.0 / N)
+        CR.check_long_workspace(ck, "long", ws, logits, c_l, ref, 0, m)
+        del ws, g_l
+    del ref
     return grad
+
+
+def _ctc_long_too(ck, logits, lab, ll, tsl):
+    return _ctc_grad(ck, logits, lab, ll, tsl, long_tables=True)
 
 
 def _ref_self_check(ck, F_):
@@ -178,7 +186,7 @@ def test_every_stage_at_batch_scale(N, W, request):
     case = request.node.callspec.id
     torch.cuda.reset_peak_memory_stats()
     m, F_, ck = B._run_stage_checks(case, N, W, _widths(N, W), dev=DEV, chunk=CHUNK,
-                                    ctc=_ctc_grad if case == "c3" else None, ck=_checker(case))
+                                    ctc=_ctc_long_too if case == "c3" else None, ck=_checker(case))
     _ref_self_check(ck, F_)
     checkers = [ck]
     if case == "c3":

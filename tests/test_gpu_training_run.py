@@ -59,9 +59,9 @@ LR = {"Adam": 1e-3, "Momentum": 2e-2, "RMS": 3e-2}
 MIN_SHARE = 0.10
 # (N, W, widths): W changes as BucketSampler changes it, N changes at fixed W, and N130_W40 comes back at the end
 RUN = [(130, 40, "cycle"), (5, 80, [80, 4, 8, 57, 33]), (3, 80, [80, 57, 12]), (3, 160, [160, 8, 97]), (130, 40, "cycle")]
-BOUNDS = dict(B.STAGE_BOUNDS, ctc_cost=BB.BOUNDS["ctc_cost"], ctc_grad=BB.BOUNDS["ctc_grad"],
+BOUNDS = dict(B.STAGE_BOUNDS, **{k: v for k, v in BB.BOUNDS.items() if k.startswith("ctc_")},
               total_loss=(0, 64 * U), l2_loss=(0, 64 * U), grad_norm=(0, 1e-6))
-L2_LIMIT = dict(B.L2_LIMIT, ctc_grad=BB.L2_LIMIT["ctc_grad"])
+L2_LIMIT = dict(B.L2_LIMIT, **{k: v for k, v in BB.L2_LIMIT.items() if k.startswith("ctc_")})
 # Largest c (in u = 2^-24 of the term magnitudes, test_gpu_solvers.py's convention) per quantity over every update of
 # test_training_run_checks_every_stage_and_update and test_training_run_at_batch_scale (slots carried over from real steps),
 # H100 80GB HBM3 (SXM, 700 W); the enforced bound is 4.5x.
@@ -123,7 +123,7 @@ def _finite(t):
 
 def _ctc_costs(ck_store):
     """A ctc callback for _check_step: the CTC gradient (grad_scale 1/N) checked against torch's fp64 CTC by
-    test_gpu_stage_isolation_batch._ctc_grad, the costs of the same logits kept for the loss check."""
+    test_gpu_stage_isolation_batch._ctc_grad (tests/ctc_refs.py), the costs of the same logits kept for the loss check."""
     def ctc(ck, logits, lab, ll, tsl):
         from lstm_ctc_ocr_b200 import engine
         t = lambda a: torch.tensor(a, device=DEV)

@@ -251,6 +251,34 @@ int     crnn_total_loss(crnn_model* m, const float* costs, int N, float* loss_ou
                         crnn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * uint8 feed.  Every text line starts as an 8-bit gray image (the reference reads cv2.imread(..., 0) and resizes it with PIL,
+ * still uint8); these twins take those bytes instead of the f32 `data`, a quarter of the host memory traffic, PCIe and device
+ * bytes.  u [N,W,32] uint8 has the layout of the f32 data (width-major rows, lib/lstm/utils/gen.py:62-64), and the input value
+ * of a byte is
+ *     x = (float)u / 255.0f      (IEEE round-to-nearest division; numpy: u.astype(np.float32) / np.float32(255))
+ * -- the value the f32 data tensor holds for that pixel, so conv1 gets the same operands and everything downstream is the same
+ * computation on the same values (a reciprocal multiply would differ on 126 of the 256 bytes).  Each twin takes the arguments
+ * and returns the status codes of its f32 entry point; only data, host_data and the staging buffers are uint8_t (the staging
+ * buffers of _host_u8 / _pageable_u8 hold N*W*32 bytes).  Copies are sized by the byte count; the chunking rule is unchanged.
+ * The device pointer the kernels read (data, data_staging) must be 4-byte aligned: otherwise CRNN_INVALID_VALUE and the
+ * outputs are untouched.  _lines_u8 ignores the bytes past each line's width, as crnn_forward_lines ignores those columns.
+ * ---------------------------------------------------------------------------------------- */
+int     crnn_forward_u8(crnn_model* m, const uint8_t* data, const int* time_step_len, int N, int W, float* logits_out,
+                        void* workspace, size_t workspace_bytes, crnn_stream_t stream);
+int     crnn_forward_host_u8(crnn_model* m, const uint8_t* host_data, uint8_t* data_staging, const int* time_step_len, int N, int W,
+                             float* logits_out, void* workspace, size_t workspace_bytes, int chunks, crnn_stream_t stream,
+                             crnn_stream_t copy_stream);
+int     crnn_forward_pageable_u8(crnn_model* m, const uint8_t* pageable_data, uint8_t* pinned_staging, uint8_t* data_staging,
+                                 const int* time_step_len, int N, int W, float* logits_out, void* workspace, size_t workspace_bytes,
+                                 int chunks, int host_threads, crnn_stream_t stream, crnn_stream_t copy_stream);
+int     crnn_forward_lines_u8(crnn_model* m, const uint8_t* data, const int* line_width, const int* time_step_len, int N, int W,
+                              float* logits_out, void* workspace, size_t workspace_bytes, crnn_stream_t stream);
+int     crnn_model_calibrate_fp8_u8(crnn_model* m, const uint8_t* data, const int* time_step_len, int N, int W, void* workspace,
+                                    size_t workspace_bytes, crnn_stream_t stream);
+int     crnn_backward_u8(crnn_model* m, const uint8_t* data, const int* time_step_len, const float* dlogits, int N, int W,
+                         void* workspace, size_t workspace_bytes, crnn_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Training.  Replaces tf.gradients + tf.clip_by_global_norm(., 10.0) + {Adam, RMSProp, Momentum}Optimizer.apply_gradients
  * (lib/lstm/train.py:73-83).  Protocol per step:
  *   crnn_model_set_training(m, 1) once; crnn_forward (saves what the backward needs in the workspace);

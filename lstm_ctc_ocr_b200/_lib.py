@@ -46,6 +46,15 @@ SIGNATURES = {
     "crnn_lines_workspace_size": (c_int, [c_void_p, c_int, c_int, ctypes.POINTER(c_size_t)]),
     "crnn_forward_lines": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "crnn_model_calibrate_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    # uint8 twins: the same arguments, uint8 pixels in place of the f32 data
+    "crnn_forward_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "crnn_forward_host_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t, c_int,
+                                     c_void_p, c_void_p]),
+    "crnn_forward_pageable_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t,
+                                         c_int, c_int, c_void_p, c_void_p]),
+    "crnn_forward_lines_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "crnn_model_calibrate_fp8_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "crnn_backward_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "crnn_model_get_fp8_scales": (c_int, [c_void_p, c_void_p]),
     "crnn_model_set_fp8_scales": (c_int, [c_void_p, c_void_p]),
     "crnn_model_bind_bn_moving": (c_int, [c_void_p, c_void_p, c_float]),

@@ -81,8 +81,9 @@ static gemm_tn::Params tn_conv(int N, int H, int Wd, int Cin, int Cout, float* o
   return p;
 }
 
-extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_step_len, const float* dlogits, int N, int W,
-                             void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
+// `u8` (crnn_backward_u8): `data` holds uint8 pixels, read only by conv1's weight gradient
+static int backward_impl(crnn_model* m, const void* data, bool u8, const int* time_step_len, const float* dlogits, int N, int W,
+                         void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
   if (!m || !data || !time_step_len || !dlogits || !workspace) return crnn_fail(CRNN_INVALID_VALUE, "backward: null pointer");
   if (!m->params || !m->grads) return crnn_fail(CRNN_NOT_BOUND, "backward: bind params and grads first");
   if (!m->training) return crnn_fail(CRNN_INVALID_VALUE, "backward: call crnn_model_set_training(m, 1) before the forward pass");
@@ -314,11 +315,22 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
   BMARK();
   // ------------------------------------------------------------------ conv1 (Cin = 1): pool1 + ReLU backward folded in; tensor-core
   // kernel with thread-built operands (conv1_wgrad_tc.cuh)
-  CRNN_TRY(launch_conv1_wgrad_tc(pl.d_a1, pl.a1, pl.am1, data, G("conv1/weights"), G("conv1/biases"), N, W, sms, st));
+  CRNN_TRY(launch_conv1_wgrad_tc(pl.d_a1, pl.a1, pl.am1, data, u8, G("conv1/weights"), G("conv1/biases"), N, W, sms, st));
   notify("conv1/weights", "conv3_1/weights");
   BMARK();
 #undef BMARK
   return CRNN_OK;
+}
+
+extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_step_len, const float* dlogits, int N, int W,
+                             void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
+  return backward_impl(m, data, false, time_step_len, dlogits, N, W, workspace, workspace_bytes, stream);
+}
+extern "C" int crnn_backward_u8(crnn_model* m, const uint8_t* data, const int* time_step_len, const float* dlogits, int N, int W,
+                                void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
+  // the uint8 kernel loads each row's pixels as 4-byte words
+  if ((reinterpret_cast<uintptr_t>(data) & 3) != 0) return crnn_fail(CRNN_INVALID_VALUE, "backward_u8: uint8 data must be 4-byte aligned");
+  return backward_impl(m, data, true, time_step_len, dlogits, N, W, workspace, workspace_bytes, stream);
 }
 
 // The half of every solver step that does not depend on the solver: grads <- grads + wd*wd_mul*w on the L2-regularised tensors

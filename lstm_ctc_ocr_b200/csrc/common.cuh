@@ -23,6 +23,36 @@ int crnn_fail(int status, const char* fmt, ...);   // records crnn_last_error(),
     if (_s != CRNN_OK) return _s; \
   } while (0)
 
+// ---- input pixels: the f32 data tensor [N, W, 32] or its uint8 twin (the crnn_*_u8 entry points).  A byte u is the pixel
+// x = (float)u / 255.0f, an IEEE round-to-nearest division (numpy's u.astype(float32) / float32(255)): the value the f32 feed
+// holds, so both feeds give conv1 the same operands.  A reciprocal multiply alone differs from that quotient on 126 of the 256
+// bytes; one FMA correction of it (q0 = u * r, q = q0 + (u - q0 * 255) * r, r = f32(1/255)) is the quotient on all 256 (checked
+// exhaustively in exact arithmetic by tests/test_u8_feed_cpu.py) at a third of the instructions of the division.
+// Pixels4<T> loads 4 consecutive pixels of a row (16 bytes of f32, one 4-byte word of u8) and widens them where they are used.
+__device__ __forceinline__ float u8_pixel(uint32_t u) {
+  constexpr float r = 1.0f / 255.0f;
+  const float x = (float)u;
+  const float q0 = __fmul_rn(x, r);
+  return __fmaf_rn(__fmaf_rn(-q0, 255.0f, x), r, q0);
+}
+template <typename T> struct Pixels4;
+template <> struct Pixels4<float> {
+  using Raw = float4;
+  static __device__ __forceinline__ Raw zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
+  static __device__ __forceinline__ Raw load(const float* row, int c4) { return __ldg(reinterpret_cast<const float4*>(row) + c4); }
+  static __device__ __forceinline__ float4 f32(const Raw& v) { return v; }
+};
+template <> struct Pixels4<uint8_t> {
+  using Raw = uint32_t;
+  static __device__ __forceinline__ Raw zero() { return 0u; }
+  static __device__ __forceinline__ Raw load(const uint8_t* row, int c4) { return __ldg(reinterpret_cast<const unsigned int*>(row) + c4); }
+  static __device__ __forceinline__ float4 f32(const Raw& v) {
+    return make_float4(u8_pixel(v & 255u), u8_pixel((v >> 8) & 255u), u8_pixel((v >> 16) & 255u), u8_pixel(v >> 24));
+  }
+};
+__device__ __forceinline__ float pixel_f32(float x) { return x; }
+__device__ __forceinline__ float pixel_f32(uint8_t u) { return u8_pixel(u); }
+
 // hidden units per [i|j|f|o] gate tile of the permuted LSTM weight columns: one CTA of the 8-CTA recurrence clusters owns 32
 // units (lstm.cuh), so gate column j = g*256 + u sits at (u/32)*128 + g*32 + u%32
 constexpr int LSTM_GATE_UNITS = 32;

@@ -63,7 +63,7 @@ __device__ __forceinline__ uint32_t bf16_bits(float v) { return (uint32_t)__bflo
 __device__ __forceinline__ float bf16_back(uint32_t b) { return __uint_as_float(b << 16); }
 
 struct Params {
-  const float* data;        // images img0 .. img0+N-1: [N, W, 32] f32
+  const void* data;         // images img0 .. img0+N-1: [N, W, 32] f32 or uint8 (the kernel's TIn)
   const float* wgt;         // HWIO [3,3,1,64]
   const float* bias;        // [64]
   uint8_t* argmax;          // TRAIN: window index (dy*2+dx) of the max, [N, W/2, 16, 64] (this launch's images)
@@ -74,8 +74,10 @@ struct Params {
 };
 
 // `tmO`: NHWC map of the whole pooled output [*, W/2, 16, 64] bf16, box [64, 16, 4, 1], SWIZZLE_128B
-template <bool TRAIN, bool LINES = false>
+// TIn: float (the f32 data tensor) or uint8_t (pixel bytes, widened to the same f32 values when they are staged: common.cuh)
+template <bool TRAIN, bool LINES = false, typename TIn = float>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const __grid_constant__ CUtensorMap tmO, const Params p) {
+  using Px = Pixels4<TIn>;
   extern __shared__ uint8_t smem_raw[];
   // aligned by OFFSET (not by casting through an integer): the pointers stay in the shared address space -> LDS/STS, not LD/ST
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -126,7 +128,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const __grid_c
     // staged input of a tile: image rows h0-1 .. h0+16 (zero outside the image) = 144 float4; thread bt owns entries bt and
     // bt+128.  The loads of tile i+1 are issued BEFORE tile i is built and land in shared memory after it, so their
     // L2/HBM latency is off the per-tile critical path (a tile is a short piece of builder work).
-    auto fetch = [&](int tile, float4 (&v)[2]) {
+    auto fetch = [&](int tile, typename Px::Raw (&v)[2]) {
       const int n = tile / p.tiles_per_img;
       const int h0 = (tile - n * p.tiles_per_img) * 16;
       const int wl = LINES ? __ldg(p.line_w + n) : p.W;
@@ -135,23 +137,24 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const __grid_c
         const int e = bt + k * BUILD_THREADS;
         const int r = e >> 3, c4 = e & 7;
         const int gr = h0 - 1 + r;
-        v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (e < IN_ROWS * 8 && gr >= 0 && gr < wl) v[k] = __ldg(reinterpret_cast<const float4*>(p.data + ((size_t)n * p.W + gr) * 32) + c4);
+        v[k] = Px::zero();
+        if (e < IN_ROWS * 8 && gr >= 0 && gr < wl) v[k] = Px::load(static_cast<const TIn*>(p.data) + ((size_t)n * p.W + gr) * 32, c4);
       }
     };
-    auto stash = [&](float* stg, const float4 (&v)[2]) {
+    auto stash = [&](float* stg, const typename Px::Raw (&raw)[2]) {
 #pragma unroll
       for (int k = 0; k < 2; ++k) {
         const int e = bt + k * BUILD_THREADS;
         if (e < IN_ROWS * 8) {
+          const float4 v = Px::f32(raw[k]);
           float* d = stg + (e >> 3) * IN_STRIDE + 1 + (e & 7) * 4;
-          d[0] = v[k].x; d[1] = v[k].y; d[2] = v[k].z; d[3] = v[k].w;
+          d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
         }
       }
     };
     for (int b = 0; b < 2; ++b)                               // zero halo columns of both stages, once
       if (bt < IN_ROWS) { s_in[b * IN_ROWS * IN_STRIDE + bt * IN_STRIDE] = 0.f; s_in[b * IN_ROWS * IN_STRIDE + bt * IN_STRIDE + 33] = 0.f; }
-    float4 pre[2];
+    typename Px::Raw pre[2];
     if (blockIdx.x < num_tiles) {
       fetch(blockIdx.x, pre);
       stash(s_in, pre);
@@ -298,24 +301,30 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_tc_kernel(const __grid_c
 }  // namespace conv1tc
 
 // `out`: NHWC map of the pooled output [*, W/2, 16, 64] bf16 with box [64, 16, 4, 1]; this launch writes images
-// img0 .. img0+N-1 of it (`data` and `argmax` point at image img0).  `line_w` != nullptr: packed evaluation lines (inference only)
-static int launch_conv1_tc(const CUtensorMap& out, const float* data, const float* w, const float* b, int img0, uint8_t* argmax,
+// img0 .. img0+N-1 of it (`data` and `argmax` point at image img0).  `line_w` != nullptr: packed evaluation lines (inference only).
+// `u8`: `data` holds uint8 pixels (crnn_*_u8), else f32.
+template <typename TIn>
+static int launch_conv1_tc_t(const CUtensorMap& out, const conv1tc::Params& p, int num_sms, cudaStream_t st) {
+  static bool attr = false;
+  if (!attr) {
+    CUDA_TRY(cudaFuncSetAttribute(conv1tc::conv1_tc_kernel<true, false, TIn>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv1tc::SMEM_BYTES));
+    CUDA_TRY(cudaFuncSetAttribute(conv1tc::conv1_tc_kernel<false, false, TIn>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv1tc::SMEM_BYTES));
+    CUDA_TRY(cudaFuncSetAttribute(conv1tc::conv1_tc_kernel<false, true, TIn>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv1tc::SMEM_BYTES));
+    attr = true;
+  }
+  const int tiles = p.N * p.tiles_per_img;
+  const int grid = tiles < num_sms ? tiles : num_sms;
+  if (p.line_w != nullptr) conv1tc::conv1_tc_kernel<false, true, TIn><<<grid, conv1tc::NUM_THREADS, conv1tc::SMEM_BYTES, st>>>(out, p);
+  else if (p.argmax != nullptr) conv1tc::conv1_tc_kernel<true, false, TIn><<<grid, conv1tc::NUM_THREADS, conv1tc::SMEM_BYTES, st>>>(out, p);
+  else conv1tc::conv1_tc_kernel<false, false, TIn><<<grid, conv1tc::NUM_THREADS, conv1tc::SMEM_BYTES, st>>>(out, p);
+  CUDA_TRY(cudaGetLastError());
+  return CRNN_OK;
+}
+
+static int launch_conv1_tc(const CUtensorMap& out, const void* data, bool u8, const float* w, const float* b, int img0, uint8_t* argmax,
                            int N, int W, int num_sms, cudaStream_t st, const int* line_w = nullptr) {
   conv1tc::Params p;
   p.data = data; p.wgt = w; p.bias = b; p.argmax = argmax; p.N = N; p.W = W; p.tiles_per_img = (W + 15) / 16; p.img0 = img0;
   p.line_w = line_w;
-  static bool attr = false;
-  if (!attr) {
-    CUDA_TRY(cudaFuncSetAttribute(conv1tc::conv1_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv1tc::SMEM_BYTES));
-    CUDA_TRY(cudaFuncSetAttribute(conv1tc::conv1_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv1tc::SMEM_BYTES));
-    CUDA_TRY(cudaFuncSetAttribute(conv1tc::conv1_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv1tc::SMEM_BYTES));
-    attr = true;
-  }
-  const int tiles = N * p.tiles_per_img;
-  const int grid = tiles < num_sms ? tiles : num_sms;
-  if (line_w != nullptr) conv1tc::conv1_tc_kernel<false, true><<<grid, conv1tc::NUM_THREADS, conv1tc::SMEM_BYTES, st>>>(out, p);
-  else if (argmax != nullptr) conv1tc::conv1_tc_kernel<true><<<grid, conv1tc::NUM_THREADS, conv1tc::SMEM_BYTES, st>>>(out, p);
-  else conv1tc::conv1_tc_kernel<false><<<grid, conv1tc::NUM_THREADS, conv1tc::SMEM_BYTES, st>>>(out, p);
-  CUDA_TRY(cudaGetLastError());
-  return CRNN_OK;
+  return u8 ? launch_conv1_tc_t<uint8_t>(out, p, num_sms, st) : launch_conv1_tc_t<float>(out, p, num_sms, st);
 }

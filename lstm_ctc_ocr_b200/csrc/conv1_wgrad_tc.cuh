@@ -49,7 +49,7 @@ struct Params {
   const __nv_bfloat16* d_a1;   // [N, W/2, 16, 64] gradient of the pooled activation
   const __nv_bfloat16* a1;     // same shape, pooled activation (ReLU mask)
   const uint8_t* am1;          // same shape, window index dy*2+dx of the maximum
-  const float* data;           // [N, W, 32]
+  const void* data;            // [N, W, 32] f32 or uint8 (the kernel's TIn)
   float* dW;                   // [9][64], accumulated with atomics
   float* db;                   // [64]
   int N, W, tiles_per_img;     // tiles_per_img = ceil((W/2) / 4)
@@ -62,7 +62,10 @@ __device__ __forceinline__ void quad_words(uint32_t gbits, uint32_t idx, uint32_
   w23 = (idx & 2u) ? v : 0u;
 }
 
+// TIn: float (the f32 data tensor) or uint8_t (pixel bytes, widened to the same f32 values when they are staged: common.cuh)
+template <typename TIn = float>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_wgrad_tc_kernel(const Params p) {
+  using Px = Pixels4<TIn>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* smem_a = smem;
@@ -137,16 +140,17 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_wgrad_tc_kernel(const Pa
     const int r = bt % 3, cs = bt / 3;
     const int set = cs & 1, chunk = cs >> 1;
     const int hol = set * 2 + (chunk >> 3), pw = chunk & 7;  // pooled row within the stage, pair of pooled columns
-    auto fetch = [&](int tile, float4& v) {
+    auto fetch = [&](int tile, typename Px::Raw& v) {
       const int n = tile / p.tiles_per_img;
       const int ho0 = (tile - n * p.tiles_per_img) * 4;
       const int rr = bt >> 3, c4 = bt & 7;
       const int gr = 2 * ho0 - 1 + rr;
-      v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (bt < IN_ROWS * 8 && gr >= 0 && gr < p.W) v = __ldg(reinterpret_cast<const float4*>(p.data + ((size_t)n * p.W + gr) * 32) + c4);
+      v = Px::zero();
+      if (bt < IN_ROWS * 8 && gr >= 0 && gr < p.W) v = Px::load(static_cast<const TIn*>(p.data) + ((size_t)n * p.W + gr) * 32, c4);
     };
-    auto stash = [&](float* stg, const float4& v) {
+    auto stash = [&](float* stg, const typename Px::Raw& raw) {
       if (bt < IN_ROWS * 8) {
+        const float4 v = Px::f32(raw);
         float* d = stg + (bt >> 3) * IN_STRIDE + 1 + (bt & 7) * 4;    // image column c lives at index c + 1
         d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
       }
@@ -159,7 +163,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_wgrad_tc_kernel(const Pa
     // input rows are prefetched TWO tiles ahead in registers (a tile is about one HBM round trip of work: one tile ahead
     // left the load latency exposed every iteration) and parked in the other s_in buffer one tile ahead
     const int G = gridDim.x;
-    float4 pre[2];
+    typename Px::Raw pre[2];
     if ((int)blockIdx.x < num_tiles) {
       fetch(blockIdx.x, pre[0]);
       stash(s_in, pre[0]);
@@ -273,19 +277,22 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv1_wgrad_tc_kernel(const Pa
 
 }  // namespace conv1wg
 
-static int launch_conv1_wgrad_tc(const __nv_bfloat16* d_a1, const __nv_bfloat16* a1, const uint8_t* am1, const float* data, float* dW,
+// `u8`: `data` holds uint8 pixels (crnn_backward_u8), else f32
+static int launch_conv1_wgrad_tc(const __nv_bfloat16* d_a1, const __nv_bfloat16* a1, const uint8_t* am1, const void* data, bool u8, float* dW,
                                  float* db, int N, int W, int num_sms, cudaStream_t st) {
   conv1wg::Params p;
   p.d_a1 = d_a1; p.a1 = a1; p.am1 = am1; p.data = data; p.dW = dW; p.db = db; p.N = N; p.W = W;
   p.tiles_per_img = ((W >> 1) + 3) / 4;
   static bool attr = false;
   if (!attr) {
-    CUDA_TRY(cudaFuncSetAttribute(conv1wg::conv1_wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, conv1wg::SMEM_BYTES));
+    CUDA_TRY(cudaFuncSetAttribute(conv1wg::conv1_wgrad_tc_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv1wg::SMEM_BYTES));
+    CUDA_TRY(cudaFuncSetAttribute(conv1wg::conv1_wgrad_tc_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv1wg::SMEM_BYTES));
     attr = true;
   }
   const int tiles = N * p.tiles_per_img;
   const int grid = tiles < num_sms ? tiles : num_sms;
-  conv1wg::conv1_wgrad_tc_kernel<<<grid, conv1wg::NUM_THREADS, conv1wg::SMEM_BYTES, st>>>(p);
+  if (u8) conv1wg::conv1_wgrad_tc_kernel<uint8_t><<<grid, conv1wg::NUM_THREADS, conv1wg::SMEM_BYTES, st>>>(p);
+  else conv1wg::conv1_wgrad_tc_kernel<float><<<grid, conv1wg::NUM_THREADS, conv1wg::SMEM_BYTES, st>>>(p);
   CUDA_TRY(cudaGetLastError());
   return CRNN_OK;
 }

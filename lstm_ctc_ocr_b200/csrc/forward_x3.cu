@@ -83,9 +83,10 @@ __device__ __forceinline__ void store_quad(void* base, size_t off, size_t lo_off
 }
 
 // ---- conv1 (3x3 SAME, 1 -> 64) + bias + ReLU + pool1 (2x2/2), f32 FMAs, hi/lo output [N, W/2, 16, 128]
-//      (lib/networks/LSTM_train.py:24-25).  One thread per (pooled position, 4 channels).
-template <bool TF>
-__global__ void __launch_bounds__(256) conv1_kernel(const float* __restrict__ data, const float* __restrict__ wgt,
+//      (lib/networks/LSTM_train.py:24-25).  One thread per (pooled position, 4 channels).  TIn: float (the f32 data tensor) or
+//      uint8_t (pixel bytes, widened at the load to the same f32 values: common.cuh)
+template <bool TF, typename TIn = float>
+__global__ void __launch_bounds__(256) conv1_kernel(const TIn* __restrict__ data, const float* __restrict__ wgt,
                                                     const float* __restrict__ bias, void* __restrict__ out, int N, int W) {
   const int H1 = W >> 1;
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -102,7 +103,7 @@ __global__ void __launch_bounds__(256) conv1_kernel(const float* __restrict__ da
 #pragma unroll
     for (int b = 0; b < 4; ++b) {
       const int gr = 2 * ho - 1 + a, gc = 2 * wo - 1 + b;
-      patch[a][b] = (gr >= 0 && gr < W && gc >= 0 && gc < 32) ? __ldg(data + ((size_t)n * W + gr) * 32 + gc) : 0.f;
+      patch[a][b] = (gr >= 0 && gr < W && gc >= 0 && gc < 32) ? pixel_f32(__ldg(data + ((size_t)n * W + gr) * 32 + gc)) : 0.f;
     }
   float best[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
 #pragma unroll
@@ -431,7 +432,7 @@ void x3_params_changed(crnn_model* m) {
   if (m->x3) reinterpret_cast<x3::State*>(m->x3)->dirty = true;
 }
 
-int x3_forward(crnn_model* m, const float* data, const int* time_step_len, int N, int W, float* logits_out, void* workspace,
+int x3_forward(crnn_model* m, const void* data, bool u8, const int* time_step_len, int N, int W, float* logits_out, void* workspace,
                size_t workspace_bytes, cudaStream_t st) {
   using namespace x3;
   if (!m->x3) {
@@ -454,8 +455,14 @@ int x3_forward(crnn_model* m, const float* data, const int* time_step_len, int N
   {
     const size_t total = (size_t)N * H1 * 16 * 16;
     const unsigned grid = (unsigned)((total + 255) / 256);
-    if (tf) conv1_kernel<true><<<grid, 256, 0, st>>>(data, m->P("conv1/weights"), m->P("conv1/biases"), pl.s1, N, W);
-    else conv1_kernel<false><<<grid, 256, 0, st>>>(data, m->P("conv1/weights"), m->P("conv1/biases"), pl.s1, N, W);
+    const float* wc = m->P("conv1/weights");
+    const float* bc = m->P("conv1/biases");
+    const float* df = static_cast<const float*>(data);
+    const uint8_t* du = static_cast<const uint8_t*>(data);
+    if (tf && u8) conv1_kernel<true, uint8_t><<<grid, 256, 0, st>>>(du, wc, bc, pl.s1, N, W);
+    else if (tf) conv1_kernel<true><<<grid, 256, 0, st>>>(df, wc, bc, pl.s1, N, W);
+    else if (u8) conv1_kernel<false, uint8_t><<<grid, 256, 0, st>>>(du, wc, bc, pl.s1, N, W);
+    else conv1_kernel<false><<<grid, 256, 0, st>>>(df, wc, bc, pl.s1, N, W);
     CUDA_TRY(cudaGetLastError());
   }
   auto conv = [&](const CUtensorMap& ta, const CUtensorMap& tb, int H, int Wd, int Cin, int Cout, int merged, bool n128) -> int {

@@ -572,12 +572,18 @@ class CopyPool {
 // epilogues zero each activation past the line's width and conv4_x use per-line batch statistics.
 // compute_dtype 4: FWD_FP8 runs conv3_1 .. conv5 on e4m3 operands (forward_fp8.cu); from host memory it copies, then computes.
 // FWD_CALIB (crnn_model_calibrate_fp8) runs the bf16 front end up to conv4_2's BatchNorm (a4b), then reduces the fp8 scales.
+// `u8` (the crnn_*_u8 twins): `data`, `host_data` and `pageable_src` hold uint8 pixels, one byte per element instead of four; every
+// copy is sized by that element size and conv1 widens the bytes when it loads them.
 enum FwdPrec { FWD_BF16 = 0, FWD_FP8 = 1, FWD_CALIB = 2 };
-static int forward_impl(crnn_model* m, const float* data, const float* host_data, const int* time_step_len, int N, int W,
+static int forward_impl(crnn_model* m, const void* data, const void* host_data, const int* time_step_len, int N, int W,
                         float* logits_out, void* workspace, size_t workspace_bytes, int chunks, cudaStream_t st, cudaStream_t copy_st,
-                        const float* pageable_src = nullptr, int host_threads = 1, const int* line_width = nullptr, int prec = FWD_BF16) {
+                        const void* pageable_src = nullptr, int host_threads = 1, const int* line_width = nullptr, int prec = FWD_BF16,
+                        bool u8 = false) {
   const bool fp8 = prec == FWD_FP8, calib = prec == FWD_CALIB;
   if (!m || !data || !time_step_len || (!logits_out && !calib) || !workspace) return crnn_fail(CRNN_INVALID_VALUE, "forward: null pointer");
+  const size_t es = u8 ? 1 : sizeof(float);                 // bytes per element of the batch
+  // image n of a batch pointer, in bytes
+  auto at = [&](const void* base, size_t n) { return const_cast<uint8_t*>(static_cast<const uint8_t*>(base)) + n * W * 32 * es; };
   if (!m->params) return crnn_fail(CRNN_NOT_BOUND, "forward: call crnn_model_bind first");
   const bool moving = m->bn_use_moving && !m->training;     // training forwards always normalise with batch statistics
   if (moving && !m->bn_moving)
@@ -594,8 +600,8 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     if (m->dp_world > 1) return crnn_fail(CRNN_UNSUPPORTED, "forward: the fp8 path runs on one device (no data parallelism)");
     if (host_data != nullptr) {
       // copy-then-compute, as the f32-class paths do
-      if (pageable_src != nullptr) CopyPool::get().copy(const_cast<float*>(host_data), pageable_src, (size_t)N * W * 32 * sizeof(float), host_threads);
-      CUDA_TRY(cudaMemcpyAsync(const_cast<float*>(data), host_data, (size_t)N * W * 32 * sizeof(float), cudaMemcpyHostToDevice, st));
+      if (pageable_src != nullptr) CopyPool::get().copy(at(host_data, 0), pageable_src, (size_t)N * W * 32 * es, host_threads);
+      CUDA_TRY(cudaMemcpyAsync(at(data, 0), host_data, (size_t)N * W * 32 * es, cudaMemcpyHostToDevice, st));
       host_data = nullptr;
       pageable_src = nullptr;
     }
@@ -604,10 +610,10 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
   if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3) {
     // f32-class paths (forward_x3.cu): copy-then-compute when fed from host memory
     if (host_data != nullptr) {
-      if (pageable_src != nullptr) CopyPool::get().copy(const_cast<float*>(host_data), pageable_src, (size_t)N * W * 32 * sizeof(float), host_threads);
-      CUDA_TRY(cudaMemcpyAsync(const_cast<float*>(data), host_data, (size_t)N * W * 32 * sizeof(float), cudaMemcpyHostToDevice, st));
+      if (pageable_src != nullptr) CopyPool::get().copy(at(host_data, 0), pageable_src, (size_t)N * W * 32 * es, host_threads);
+      CUDA_TRY(cudaMemcpyAsync(at(data, 0), host_data, (size_t)N * W * 32 * es, cudaMemcpyHostToDevice, st));
     }
-    return x3_forward(m, data, time_step_len, N, W, logits_out, workspace, workspace_bytes, st);
+    return x3_forward(m, data, u8, time_step_len, N, W, logits_out, workspace, workspace_bytes, st);
   }
   if (m->dirty) CRNN_TRY(prepare_weights(m, st));
   if (fp8) CRNN_TRY(fp8_prepare(m, st));
@@ -654,9 +660,7 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     CUDA_TRY(cudaStreamWaitEvent(copy_st, m->chunk_events[kMaxChunks], 0));
     for (int c = 0; pageable_src == nullptr && c * nc < N; ++c) {
       const int n0 = c * nc, n1 = (n0 + nc < N) ? n0 + nc : N;
-      const size_t off = (size_t)n0 * W * 32;
-      CUDA_TRY(cudaMemcpyAsync(const_cast<float*>(data) + off, host_data + off, (size_t)(n1 - n0) * W * 32 * sizeof(float),
-                               cudaMemcpyHostToDevice, copy_st));
+      CUDA_TRY(cudaMemcpyAsync(at(data, n0), at(host_data, n0), (size_t)(n1 - n0) * W * 32 * es, cudaMemcpyHostToDevice, copy_st));
       CUDA_TRY(cudaEventRecord(m->chunk_events[c], copy_st));
     }
   }
@@ -665,16 +669,16 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
     const bool mark = (n1 == N) && chunks == 1;      // per-stage events only make sense for an unchunked front end
     if (pageable_src != nullptr) {
       // pageable source: move this range into the page-locked staging now (the GPU is busy with the previous range), then issue its DMA
-      const size_t off = (size_t)n0 * W * 32, bytes = (size_t)cn * W * 32 * sizeof(float);
-      CopyPool::get().copy(const_cast<float*>(host_data) + off, pageable_src + off, bytes, host_threads);
-      CUDA_TRY(cudaMemcpyAsync(const_cast<float*>(data) + off, host_data + off, bytes, cudaMemcpyHostToDevice, copy_st));
+      const size_t bytes = (size_t)cn * W * 32 * es;
+      CopyPool::get().copy(at(host_data, n0), at(pageable_src, n0), bytes, host_threads);
+      CUDA_TRY(cudaMemcpyAsync(at(data, n0), at(host_data, n0), bytes, cudaMemcpyHostToDevice, copy_st));
       CUDA_TRY(cudaEventRecord(m->chunk_events[c], copy_st));
     }
     if (host_data != nullptr) CUDA_TRY(cudaStreamWaitEvent(st, m->chunk_events[c], 0));
     // conv1 + pool1 (tensor cores, split-bf16 operands: conv1_tc.cuh)
     {
       const size_t o1 = (size_t)n0 * H1 * 16 * 64;
-      CRNN_TRY(launch_conv1_tc(pl.tO_c1, data + (size_t)n0 * W * 32, m->P("conv1/weights"), m->P("conv1/biases"), n0,
+      CRNN_TRY(launch_conv1_tc(pl.tO_c1, at(data, n0), u8, m->P("conv1/weights"), m->P("conv1/biases"), n0,
                                pl.train ? pl.am1 + o1 : nullptr, cn, W, sms, st, pl.line_w));
     }
     if (mark) STAGE_MARK();
@@ -892,28 +896,67 @@ static int forward_impl(crnn_model* m, const float* data, const float* host_data
 
 static int fwd_prec(const crnn_model* m) { return (m && m->cfg.compute_dtype == 4) ? FWD_FP8 : FWD_BF16; }
 
-extern "C" int crnn_forward(crnn_model* m, const float* data, const int* time_step_len, int N, int W, float* logits_out,
-                            void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return forward_impl(m, data, nullptr, time_step_len, N, W, logits_out, workspace, workspace_bytes, 1, st, st, nullptr, 1, nullptr,
-                      fwd_prec(m));
+// the uint8 kernels load each row's pixels as 4-byte words
+static int check_u8_aligned(const void* p, const char* fn) {
+  if ((reinterpret_cast<uintptr_t>(p) & 3) != 0) return crnn_fail(CRNN_INVALID_VALUE, "%s: uint8 data must be 4-byte aligned", fn);
+  return CRNN_OK;
 }
 
+static int forward_dev(crnn_model* m, const void* data, bool u8, const int* time_step_len, int N, int W, float* logits_out,
+                       void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return forward_impl(m, data, nullptr, time_step_len, N, W, logits_out, workspace, workspace_bytes, 1, st, st, nullptr, 1, nullptr,
+                      fwd_prec(m), u8);
+}
+extern "C" int crnn_forward(crnn_model* m, const float* data, const int* time_step_len, int N, int W, float* logits_out,
+                            void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
+  return forward_dev(m, data, false, time_step_len, N, W, logits_out, workspace, workspace_bytes, stream);
+}
+extern "C" int crnn_forward_u8(crnn_model* m, const uint8_t* data, const int* time_step_len, int N, int W, float* logits_out,
+                               void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
+  CRNN_TRY(check_u8_aligned(data, "forward_u8"));
+  return forward_dev(m, data, true, time_step_len, N, W, logits_out, workspace, workspace_bytes, stream);
+}
+
+static int forward_host(crnn_model* m, const void* host_data, void* data_staging, bool u8, const int* time_step_len, int N, int W,
+                        float* logits_out, void* workspace, size_t workspace_bytes, int chunks, crnn_stream_t stream,
+                        crnn_stream_t copy_stream) {
+  if (!host_data || !data_staging) return crnn_fail(CRNN_INVALID_VALUE, "forward_host: null pointer");
+  return forward_impl(m, data_staging, host_data, time_step_len, N, W, logits_out, workspace, workspace_bytes, chunks,
+                      reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<cudaStream_t>(copy_stream), nullptr, 1, nullptr, fwd_prec(m),
+                      u8);
+}
 extern "C" int crnn_forward_host(crnn_model* m, const float* host_data, float* data_staging, const int* time_step_len, int N, int W,
                                  float* logits_out, void* workspace, size_t workspace_bytes, int chunks, crnn_stream_t stream,
                                  crnn_stream_t copy_stream) {
-  if (!host_data || !data_staging) return crnn_fail(CRNN_INVALID_VALUE, "forward_host: null pointer");
-  return forward_impl(m, data_staging, host_data, time_step_len, N, W, logits_out, workspace, workspace_bytes, chunks,
-                      reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<cudaStream_t>(copy_stream), nullptr, 1, nullptr, fwd_prec(m));
+  return forward_host(m, host_data, data_staging, false, time_step_len, N, W, logits_out, workspace, workspace_bytes, chunks, stream,
+                      copy_stream);
+}
+extern "C" int crnn_forward_host_u8(crnn_model* m, const uint8_t* host_data, uint8_t* data_staging, const int* time_step_len, int N,
+                                    int W, float* logits_out, void* workspace, size_t workspace_bytes, int chunks, crnn_stream_t stream,
+                                    crnn_stream_t copy_stream) {
+  CRNN_TRY(check_u8_aligned(data_staging, "forward_host_u8"));
+  return forward_host(m, host_data, data_staging, true, time_step_len, N, W, logits_out, workspace, workspace_bytes, chunks, stream,
+                      copy_stream);
 }
 
 // ---- fp8 (compute_dtype 4) scales
-extern "C" int crnn_model_calibrate_fp8(crnn_model* m, const float* data, const int* time_step_len, int N, int W, void* workspace,
-                                        size_t workspace_bytes, crnn_stream_t stream) {
+static int calibrate_fp8(crnn_model* m, const void* data, bool u8, const int* time_step_len, int N, int W, void* workspace,
+                         size_t workspace_bytes, crnn_stream_t stream) {
   if (!m) return crnn_fail(CRNN_INVALID_VALUE, "calibrate_fp8: null model");
   if (m->cfg.compute_dtype != 4) return crnn_fail(CRNN_UNSUPPORTED, "calibrate_fp8: the model is not an fp8 model (compute_dtype 4)");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return forward_impl(m, data, nullptr, time_step_len, N, W, nullptr, workspace, workspace_bytes, 1, st, st, nullptr, 1, nullptr, FWD_CALIB);
+  return forward_impl(m, data, nullptr, time_step_len, N, W, nullptr, workspace, workspace_bytes, 1, st, st, nullptr, 1, nullptr, FWD_CALIB,
+                      u8);
+}
+extern "C" int crnn_model_calibrate_fp8(crnn_model* m, const float* data, const int* time_step_len, int N, int W, void* workspace,
+                                        size_t workspace_bytes, crnn_stream_t stream) {
+  return calibrate_fp8(m, data, false, time_step_len, N, W, workspace, workspace_bytes, stream);
+}
+extern "C" int crnn_model_calibrate_fp8_u8(crnn_model* m, const uint8_t* data, const int* time_step_len, int N, int W, void* workspace,
+                                           size_t workspace_bytes, crnn_stream_t stream) {
+  CRNN_TRY(check_u8_aligned(data, "calibrate_fp8_u8"));
+  return calibrate_fp8(m, data, true, time_step_len, N, W, workspace, workspace_bytes, stream);
 }
 extern "C" int crnn_model_get_fp8_scales(crnn_model* m, float* scales_host) {
   if (!m || !scales_host) return crnn_fail(CRNN_INVALID_VALUE, "get_fp8_scales: null");
@@ -939,8 +982,8 @@ extern "C" int crnn_lines_workspace_size(const crnn_model* m, int N, int W, size
   return CRNN_OK;
 }
 
-extern "C" int crnn_forward_lines(crnn_model* m, const float* data, const int* line_width, const int* time_step_len, int N, int W,
-                                  float* logits_out, void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
+static int forward_lines(crnn_model* m, const void* data, bool u8, const int* line_width, const int* time_step_len, int N, int W,
+                         float* logits_out, void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
   if (!m || !data || !line_width || !time_step_len || !logits_out || !workspace) return crnn_fail(CRNN_INVALID_VALUE, "forward_lines: null pointer");
   if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3)
     return crnn_fail(CRNN_UNSUPPORTED, "forward_lines: packed evaluation runs on the bf16 and fp8 paths (compute_dtype 1, 4)");
@@ -951,7 +994,16 @@ extern "C" int crnn_forward_lines(crnn_model* m, const float* data, const int* l
   if (workspace_bytes < need) return crnn_fail(CRNN_WORKSPACE_TOO_SMALL, "forward_lines: workspace %zu < %zu", workspace_bytes, need);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   return forward_impl(m, data, nullptr, time_step_len, N, W, logits_out, workspace, workspace_bytes, 1, st, st, nullptr, 1, line_width,
-                      fwd_prec(m));
+                      fwd_prec(m), u8);
+}
+extern "C" int crnn_forward_lines(crnn_model* m, const float* data, const int* line_width, const int* time_step_len, int N, int W,
+                                  float* logits_out, void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
+  return forward_lines(m, data, false, line_width, time_step_len, N, W, logits_out, workspace, workspace_bytes, stream);
+}
+extern "C" int crnn_forward_lines_u8(crnn_model* m, const uint8_t* data, const int* line_width, const int* time_step_len, int N, int W,
+                                     float* logits_out, void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
+  CRNN_TRY(check_u8_aligned(data, "forward_lines_u8"));
+  return forward_lines(m, data, true, line_width, time_step_len, N, W, logits_out, workspace, workspace_bytes, stream);
 }
 
 extern "C" int crnn_host_copy(void* dst, const void* src, size_t bytes, int threads) {
@@ -960,13 +1012,26 @@ extern "C" int crnn_host_copy(void* dst, const void* src, size_t bytes, int thre
   return CRNN_OK;
 }
 
-extern "C" int crnn_forward_pageable(crnn_model* m, const float* pageable_data, float* pinned_staging, float* data_staging,
-                                     const int* time_step_len, int N, int W, float* logits_out, void* workspace, size_t workspace_bytes,
-                                     int chunks, int host_threads, crnn_stream_t stream, crnn_stream_t copy_stream) {
+static int forward_pageable(crnn_model* m, const void* pageable_data, void* pinned_staging, void* data_staging, bool u8,
+                            const int* time_step_len, int N, int W, float* logits_out, void* workspace, size_t workspace_bytes, int chunks,
+                            int host_threads, crnn_stream_t stream, crnn_stream_t copy_stream) {
   if (!pageable_data || !pinned_staging || !data_staging) return crnn_fail(CRNN_INVALID_VALUE, "forward_pageable: null pointer");
   return forward_impl(m, data_staging, pinned_staging, time_step_len, N, W, logits_out, workspace, workspace_bytes, chunks,
                       reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<cudaStream_t>(copy_stream), pageable_data,
-                      host_threads < 1 ? 1 : host_threads, nullptr, fwd_prec(m));
+                      host_threads < 1 ? 1 : host_threads, nullptr, fwd_prec(m), u8);
+}
+extern "C" int crnn_forward_pageable(crnn_model* m, const float* pageable_data, float* pinned_staging, float* data_staging,
+                                     const int* time_step_len, int N, int W, float* logits_out, void* workspace, size_t workspace_bytes,
+                                     int chunks, int host_threads, crnn_stream_t stream, crnn_stream_t copy_stream) {
+  return forward_pageable(m, pageable_data, pinned_staging, data_staging, false, time_step_len, N, W, logits_out, workspace,
+                          workspace_bytes, chunks, host_threads, stream, copy_stream);
+}
+extern "C" int crnn_forward_pageable_u8(crnn_model* m, const uint8_t* pageable_data, uint8_t* pinned_staging, uint8_t* data_staging,
+                                        const int* time_step_len, int N, int W, float* logits_out, void* workspace, size_t workspace_bytes,
+                                        int chunks, int host_threads, crnn_stream_t stream, crnn_stream_t copy_stream) {
+  CRNN_TRY(check_u8_aligned(data_staging, "forward_pageable_u8"));
+  return forward_pageable(m, pageable_data, pinned_staging, data_staging, true, time_step_len, N, W, logits_out, workspace,
+                          workspace_bytes, chunks, host_threads, stream, copy_stream);
 }
 
 // ------------------------------------------------------------------------------------------------ profiling

@@ -150,7 +150,7 @@ struct crnn_model {
 
 // f32-class ("3xbf16") forward path, forward_x3.cu
 size_t x3_workspace_size(int N, int W);
-int x3_forward(crnn_model* m, const float* data, const int* time_step_len, int N, int W, float* logits_out, void* workspace,
+int x3_forward(crnn_model* m, const void* data, bool u8, const int* time_step_len, int N, int W, float* logits_out, void* workspace,
                size_t workspace_bytes, cudaStream_t st);
 int x3_debug_tap(crnn_model* m, const char* name, float* dst, size_t dst_elems, void* workspace, cudaStream_t st);
 int x3_debug_tap_raw(crnn_model* m, const char* name, void* dst, size_t dst_bytes, void* workspace, cudaStream_t st);

@@ -36,6 +36,15 @@ def _ptr(t):
     return 0 if t is None else t.data_ptr()
 
 
+def _feed_suffix(dtype):
+    """Entry-point suffix of a batch's element type: f32 data -> "", uint8 pixels (x = u / 255, include/crnn_ctc.h) -> "_u8"."""
+    if dtype in (torch.float32, np.float32):
+        return ""
+    if dtype in (torch.uint8, np.uint8):
+        return "_u8"
+    raise CrnnError(f"data must be float32 or uint8 pixels, got {dtype}")
+
+
 class CrnnModel:
     """Owns the flat f32 parameter buffer (TF variable names/layouts) and the C model handle."""
 
@@ -132,10 +141,12 @@ class CrnnModel:
         return self.grads[off:off + int(np.prod(shp))].view(*shp)
 
     def backward(self, data, time_step_len, dlogits):
-        """dlogits [T,N,64] f32 = d loss / d logits (e.g. the CTC gradient scaled by 1/N) -> fills self.grads."""
+        """dlogits [T,N,64] f32 = d loss / d logits (e.g. the CTC gradient scaled by 1/N) -> fills self.grads.  `data` is the
+        batch the training forward read: f32, or uint8 pixels (crnn_backward_u8)."""
         N, W, _ = data.shape
         ws, nbytes = self._workspace(N, W)
-        check(self.lib.crnn_backward(self.handle, data.data_ptr(), time_step_len.data_ptr(), dlogits.data_ptr(), N, W, ws, nbytes,
+        fn = getattr(self.lib, "crnn_backward" + _feed_suffix(data.dtype))
+        check(fn(self.handle, data.data_ptr(), time_step_len.data_ptr(), dlogits.data_ptr(), N, W, ws, nbytes,
                                      _stream()))
 
     def clip_adam_step(self, lr, step, clip=10.0, grad_mul=1.0, wd_mul=1.0):
@@ -234,8 +245,10 @@ class CrnnModel:
         return aligned, self._ws.numel() - (aligned - base)
 
     def forward(self, data, time_step_len, out=None):
-        """data [N,W,32] f32 cuda, time_step_len [N] i32 cuda -> logits [T,N,64] f32 (time-major)."""
-        assert data.is_cuda and data.dtype == torch.float32 and data.is_contiguous()
+        """data [N,W,32] f32 cuda, or uint8 pixels (crnn_forward_u8: x = u / 255), time_step_len [N] i32 cuda -> logits [T,N,64]
+        f32 (time-major)."""
+        fn = getattr(self.lib, "crnn_forward" + _feed_suffix(data.dtype))
+        assert data.is_cuda and data.is_contiguous()
         assert time_step_len.is_cuda and time_step_len.dtype == torch.int32
         N, W, Hh = data.shape
         if Hh != 32:
@@ -244,21 +257,23 @@ class CrnnModel:
         if out is None:
             out = torch.empty((T, N, NCLASSES), dtype=torch.float32, device=self.device)
         ws, nbytes = self._workspace(N, W)
-        check(self.lib.crnn_forward(self.handle, data.data_ptr(), time_step_len.data_ptr(), N, W, out.data_ptr(), ws,
+        check(fn(self.handle, data.data_ptr(), time_step_len.data_ptr(), N, W, out.data_ptr(), ws,
                                     nbytes, _stream()))
         return out
 
     # ---- fp8 scales (compute_dtype "fp8") -----------------------------------------------------
     def calibrate_fp8(self, data, time_step_len):
         """Set the five activation scales of an fp8 model from a calibration batch (data [N,W,32] f32 cuda, time_step_len [N]
-        i32 cuda): the bf16 front end runs on it and each scale becomes 2^ceil(log2(amax / 448)).  Asynchronous, on the device."""
-        assert data.is_cuda and data.dtype == torch.float32 and data.is_contiguous()
+        i32 cuda; or uint8 pixels): the bf16 front end runs on it and each scale becomes 2^ceil(log2(amax / 448)).  Asynchronous,
+        on the device."""
+        fn = getattr(self.lib, "crnn_model_calibrate_fp8" + _feed_suffix(data.dtype))
+        assert data.is_cuda and data.is_contiguous()
         assert time_step_len.is_cuda and time_step_len.dtype == torch.int32
         N, W, Hh = data.shape
         if Hh != 32:
             raise CrnnError("data must be [N, W, 32] (cfg.NUM_FEATURES = 32)")
         ws, nbytes = self._workspace(N, W)
-        check(self.lib.crnn_model_calibrate_fp8(self.handle, data.data_ptr(), time_step_len.data_ptr(), N, W, ws, nbytes, _stream()))
+        check(fn(self.handle, data.data_ptr(), time_step_len.data_ptr(), N, W, ws, nbytes, _stream()))
         self.fp8_calibrated = True
 
     def fp8_scales(self):
@@ -277,8 +292,9 @@ class CrnnModel:
         """Packed evaluation: data [N,W,32] f32 cuda holding line i in columns [0, W_i), line_width [N] i32 cuda (W_i, a multiple
         of 4 in [8, W]), time_step_len [N] i32 cuda (<= W_i/4 - 1) -> logits [W/4-1,N,64] f32, each line's frames t < W_i/4 - 1
         as forward() computes them for that line fed alone as [1, W_i, 32] (per-line BatchNorm statistics and width boundaries).
-        Evaluation only: a model in training mode is refused."""
-        assert data.is_cuda and data.dtype == torch.float32 and data.is_contiguous()
+        Evaluation only: a model in training mode is refused.  uint8 pixels (crnn_forward_lines_u8) are accepted as data."""
+        fn = getattr(self.lib, "crnn_forward_lines" + _feed_suffix(data.dtype))
+        assert data.is_cuda and data.is_contiguous()
         assert line_width.is_cuda and line_width.dtype == torch.int32 and time_step_len.is_cuda and time_step_len.dtype == torch.int32
         N, W, Hh = data.shape
         if Hh != 32:
@@ -289,53 +305,66 @@ class CrnnModel:
         if out is None:
             out = torch.empty((T, N, NCLASSES), dtype=torch.float32, device=self.device)
         ws, nbytes = self._workspace(N, W, lines=True)
-        check(self.lib.crnn_forward_lines(self.handle, data.data_ptr(), line_width.data_ptr(), time_step_len.data_ptr(), N, W,
+        check(fn(self.handle, data.data_ptr(), line_width.data_ptr(), time_step_len.data_ptr(), N, W,
                                           out.data_ptr(), ws, nbytes, _stream()))
         return out
 
     def forward_host(self, host_data, time_step_len, chunks=4, out=None, wait_copy=True):
-        """host_data: C-contiguous f32 numpy array [N,W,32] in PAGE-LOCKED memory.  The H2D copy is cut into `chunks` image
-        ranges on a side stream and overlapped with the conv front end (crnn_forward_host).  Returns (logits, device data)."""
+        """host_data: C-contiguous f32 (or uint8 pixel) numpy array [N,W,32] in PAGE-LOCKED memory.  The H2D copy is cut into
+        `chunks` image ranges on a side stream and overlapped with the conv front end (crnn_forward_host / _u8).  Returns
+        (logits, device data): the device staging of the batch's dtype."""
         N, W, Hh = host_data.shape
         if Hh != 32:
             raise CrnnError("data must be [N, W, 32] (cfg.NUM_FEATURES = 32)")
-        assert host_data.dtype == np.float32 and host_data.flags.c_contiguous
+        fn = getattr(self.lib, "crnn_forward_host" + _feed_suffix(host_data.dtype))
+        assert host_data.flags.c_contiguous
         T = W // 4 - 1
         if out is None:
             out = torch.empty((T, N, NCLASSES), dtype=torch.float32, device=self.device)
-        if getattr(self, "_stage", None) is None or self._stage.shape != (N, W, 32):
-            self._stage = torch.empty((N, W, 32), dtype=torch.float32, device=self.device)
+        stage = self._staging(N, W, host_data.dtype)
         if getattr(self, "_copy_stream", None) is None:
             self._copy_stream = torch.cuda.Stream(device=self.device)
         ws, nbytes = self._workspace(N, W)
-        check(self.lib.crnn_forward_host(self.handle, host_data.ctypes.data, self._stage.data_ptr(), time_step_len.data_ptr(), N, W,
+        check(fn(self.handle, host_data.ctypes.data, stage.data_ptr(), time_step_len.data_ptr(), N, W,
                                          out.data_ptr(), ws, nbytes, int(chunks), _stream(), self._copy_stream.cuda_stream))
         if wait_copy:
             # the caller may rewrite `host_data` as soon as this returns (a feeder recycling its ring slot): wait for the DMA --
             # not for the compute, which keeps running on the main stream
             self._copy_stream.synchronize()
-        return out, self._stage
+        return out, stage
+
+    def _staging(self, N, W, dtype):
+        """Device staging [N,W,32] of the host feeds, one per element type (f32, uint8)."""
+        dt = torch.uint8 if _feed_suffix(dtype) else torch.float32
+        if getattr(self, "_stage", None) is None:
+            self._stage = {}
+        st = self._stage.get(dt)
+        if st is None or st.shape != (N, W, 32):
+            st = self._stage[dt] = torch.empty((N, W, 32), dtype=dt, device=self.device)
+        return st
 
     def forward_pageable(self, host_data, pinned, time_step_len, chunks=4, host_threads=8, out=None):
-        """host_data: C-contiguous f32 numpy array [N,W,32] in ORDINARY memory (the reference's np.array(...) per step); `pinned`: a
-        page-locked f32 torch tensor with at least N*W*32 elements.  Range by range the library's host threads move the batch into
-        `pinned`, DMA it and run the conv front end (crnn_forward_pageable).  Returns (logits, device data, copy stream)."""
+        """host_data: C-contiguous f32 (or uint8 pixel) numpy array [N,W,32] in ORDINARY memory (the reference's np.array(...) per
+        step); `pinned`: a page-locked torch tensor with at least N*W*32 elements of the same element size.  Range by range the
+        library's host threads move the batch into `pinned`, DMA it and run the conv front end (crnn_forward_pageable / _u8).
+        Returns (logits, device data, copy stream)."""
         N, W, Hh = host_data.shape
         if Hh != 32:
             raise CrnnError("data must be [N, W, 32] (cfg.NUM_FEATURES = 32)")
-        assert host_data.dtype == np.float32 and host_data.flags.c_contiguous and pinned.is_pinned() and pinned.numel() >= host_data.size
+        fn = getattr(self.lib, "crnn_forward_pageable" + _feed_suffix(host_data.dtype))
+        assert (host_data.flags.c_contiguous and pinned.is_pinned() and pinned.element_size() == host_data.itemsize
+                and pinned.numel() >= host_data.size)
         T = W // 4 - 1
         if out is None:
             out = torch.empty((T, N, NCLASSES), dtype=torch.float32, device=self.device)
-        if getattr(self, "_stage", None) is None or self._stage.shape != (N, W, 32):
-            self._stage = torch.empty((N, W, 32), dtype=torch.float32, device=self.device)
+        stage = self._staging(N, W, host_data.dtype)
         if getattr(self, "_copy_stream", None) is None:
             self._copy_stream = torch.cuda.Stream(device=self.device)
         ws, nbytes = self._workspace(N, W)
-        check(self.lib.crnn_forward_pageable(self.handle, host_data.ctypes.data, pinned.data_ptr(), self._stage.data_ptr(),
+        check(fn(self.handle, host_data.ctypes.data, pinned.data_ptr(), stage.data_ptr(),
                                              time_step_len.data_ptr(), N, W, out.data_ptr(), ws, nbytes, int(chunks), int(host_threads),
                                              _stream(), self._copy_stream.cuda_stream))
-        return out, self._stage, self._copy_stream
+        return out, stage, self._copy_stream
 
     def tap(self, name, N, W):
         """Intermediate of the last forward (or, for the backward buffers, the last backward) as f32 NHWC (tests only)."""

@@ -36,6 +36,10 @@ _DEFAULTS = {
     # not in the reference: which decoder `dense_decoded` runs -- "greedy" (GPU kernel, the hot path) or "beam" (the reference's
     # ctc_beam_search_decoder semantics, network.py:656; decoded on the GPU, width BEAM_WIDTH <= 128)
     "DECODER": "greedy", "BEAM_WIDTH": 100,
+    # not in the reference (it widens every line to f32 on the host): "uint8" builds training, validation and evaluation batches
+    # as 8-bit pixels and feeds them through the networks' data_u8 placeholder -- a quarter of the host and PCIe bytes, the same
+    # values on the device (x = u / 255 in f32); "float32" feeds data as the reference does
+    "FEED_DTYPE": "float32",
     "NET_NAME": "lstm", "EXP_DIR": "default", "LOG_DIR": "default", "RNG_SEED": 3,
     "TRAIN": {
         "SOLVER": "Adam", "TXT": "annotation_train.txt",

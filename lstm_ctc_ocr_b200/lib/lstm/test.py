@@ -17,6 +17,7 @@ import numpy as np
 
 from ...session import Session
 from .config import cfg, get_encode_decode_dict
+from .utils.gen import feed_dtype
 from .utils.timer import Timer
 
 
@@ -33,28 +34,37 @@ def load_line_image(path):
     return np.asarray(Image.open(path).convert("L"), dtype=np.uint8)
 
 
-def prepare_line(img):
-    """[H=32, W] uint8 -> ([1, Wpad, 32] f32, time_step_len) exactly as test.py:65-70 lays the tensor out."""
+def prepare_line(img, dtype=np.float32):
+    """[H=32, W] uint8 -> ([1, Wpad, 32] f32, time_step_len) exactly as test.py:65-70 lays the tensor out.  ``dtype=np.uint8``:
+    the same tensor as the 8-bit pixels, without the division (its f32 quotient by 255 is the f32 tensor bit for bit)."""
     if img.shape[0] != cfg.IMG_HEIGHT:
         from PIL import Image
         nw = max(1, int(cfg.IMG_HEIGHT / img.shape[0] * img.shape[1]))
         img = np.asarray(Image.fromarray(img).resize((nw, cfg.IMG_HEIGHT), Image.BILINEAR), dtype=np.uint8)
     w = img.shape[1]
     width = max(8, int(math.ceil(w / cfg.POOL_SCALE) * cfg.POOL_SCALE))
-    pad = np.zeros((cfg.IMG_HEIGHT, width), np.float32)
-    pad[:, :w] = img.astype(np.float32) / 255.0
+    if np.dtype(dtype) == np.uint8:
+        pad = np.zeros((cfg.IMG_HEIGHT, width), np.uint8)
+        pad[:, :w] = img
+    else:
+        pad = np.zeros((cfg.IMG_HEIGHT, width), np.float32)
+        pad[:, :w] = img.astype(np.float32) / 255.0
     data = np.ascontiguousarray(pad.swapaxes(0, 1)).reshape(1, width, cfg.NUM_FEATURES)
     return data, np.array([max(w // cfg.POOL_SCALE + cfg.OFFSET_TIME_STEP, 0)], np.int32)
 
 
 def pack_lines(lines):
     """[(data [1, W_i, 32] f32, time_step_len [1] i32) as prepare_line returns them] -> (data [N, W, 32] f32 with line i in columns
-    [0, W_i) of slot i and zero beyond, line_width [N] i32 = W_i, time_step_len [N] i32), W = max W_i: the feed of a packed run."""
+    [0, W_i) of slot i and zero beyond, line_width [N] i32 = W_i, time_step_len [N] i32), W = max W_i: the feed of a packed run.
+    Lines prepared as uint8 pack into a uint8 batch (the lines' dtype; all lines must share it)."""
     if not lines:
         raise ValueError("pack_lines: no lines")
     widths = []
+    dtype = np.asarray(lines[0][0]).dtype
     for d, t in lines:
         d, t = np.asarray(d), np.asarray(t)
+        if d.dtype != dtype:
+            raise ValueError(f"pack_lines: lines of dtypes {dtype} and {d.dtype}")
         if d.ndim != 3 or d.shape[0] != 1 or d.shape[2] != cfg.NUM_FEATURES:
             raise ValueError(f"pack_lines: each line must be [1, W_i, {cfg.NUM_FEATURES}], got {d.shape}")
         w = d.shape[1]
@@ -63,7 +73,7 @@ def pack_lines(lines):
         if t.shape != (1,) or t[0] < 0 or t[0] > w // cfg.POOL_SCALE - 1:
             raise ValueError(f"pack_lines: time_step_len {t} must lie in [0, {w // cfg.POOL_SCALE - 1}] for a line {w} wide")
         widths.append(w)
-    data = np.zeros((len(lines), max(widths), cfg.NUM_FEATURES), np.float32)
+    data = np.zeros((len(lines), max(widths), cfg.NUM_FEATURES), dtype)
     for i, (d, _) in enumerate(lines):
         data[i, :widths[i]] = d[0]
     tsl = np.array([int(np.asarray(t)[0]) for _, t in lines], np.int32)
@@ -100,7 +110,8 @@ class SolverWrapper(object):
             except Exception:
                 raise Exception("Check your pretrained {:s}".format(str(path)))
         files = sorted(os.listdir(testDir))
-        lines = [prepare_line(load_line_image(os.path.join(testDir, f))) for f in files]
+        dtype = feed_dtype(cfg.FEED_DTYPE)       # "uint8": lines stay 8-bit pixels and are fed through data_u8
+        lines = [prepare_line(load_line_image(os.path.join(testDir, f)), dtype=dtype) for f in files]
         # batches of lines of similar width (stable sort: ties keep name order), so little of a batch is padding
         order = sorted(range(len(files)), key=lambda i: lines[i][0].shape[1])
         bs = max(1, int(cfg.TEST.BATCH_SIZE))
@@ -110,7 +121,7 @@ class SolverWrapper(object):
             idx = order[b0:b0 + bs]
             timer.tic()
             data, lw, tsl = pack_lines([lines[i] for i in idx])
-            feed_dict = {self.net.data: data, self.net.line_width: lw, self.net.time_step_len: tsl, self.net.keep_prob: 1.0}
+            feed_dict = {(self.net.data_u8 if dtype == np.uint8 else self.net.data): data, self.net.line_width: lw, self.net.time_step_len: tsl, self.net.keep_prob: 1.0}
             dense = sess.run(fetches=dense_decoded, feed_dict=feed_dict)
             dt = timer.toc(average=False) / len(idx)
             for r, i in enumerate(idx):

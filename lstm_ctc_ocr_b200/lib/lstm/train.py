@@ -18,7 +18,7 @@ from ... import engine
 from ...session import Session
 from ..networks.network import Fetch
 from .config import cfg
-from .utils.gen import get_batch
+from .utils.gen import feed_dtype, get_batch
 from .utils.timer import Timer
 from .utils.training import accuracy_calculation
 
@@ -122,12 +122,12 @@ class SolverWrapper(object):
 
     # ---- the loop (train.py:63-162) -----------------------------------------------------------------------------
     def _feed(self, batch, keep_prob):
-        """feed_dict for one data-layer tuple (train.py:119-127)."""
+        """feed_dict for one data-layer tuple (train.py:119-127); uint8 batches (cfg.FEED_DTYPE "uint8") go to data_u8."""
         imgs, flat_labels, label_len, time_steps = batch
         net = self.net
         # a PrefetchFeeder hands out an ndarray view of a page-locked ring slot: keep it (np.array would copy it to pageable memory)
         data = imgs if isinstance(imgs, np.ndarray) and imgs.ndim == 3 else np.array(imgs)
-        return {net.data: data, net.labels: np.array(flat_labels), net.time_step_len: np.array(time_steps),
+        return {(net.data_u8 if data.dtype == np.uint8 else net.data): data, net.labels: np.array(flat_labels), net.time_step_len: np.array(time_steps),
                 net.labels_len: np.array(label_len), net.keep_prob: keep_prob}
 
     def _prepare(self, sess, restore, lr, global_step):
@@ -172,8 +172,9 @@ class SolverWrapper(object):
 
     def train_model(self, sess, max_iters, restore=False, train_gen=None, val_gen=None):
         from ... import parallel
-        train_gen = train_gen or get_batch(num_workers=12, batch_size=cfg.TRAIN.BATCH_SIZE, vis=False)
-        val_gen = val_gen or get_batch(num_workers=1, batch_size=cfg.VAL.BATCH_SIZE, vis=False)
+        dtype = feed_dtype(cfg.FEED_DTYPE)
+        train_gen = train_gen or get_batch(num_workers=12, batch_size=cfg.TRAIN.BATCH_SIZE, vis=False, dtype=dtype)
+        val_gen = val_gen or get_batch(num_workers=1, batch_size=cfg.VAL.BATCH_SIZE, vis=False, dtype=dtype)
         loss, dense_decoded = self.net.build_loss()
         lr, global_step = Variable(cfg.TRAIN.LEARNING_RATE), Variable(0)
         self._lr, self._global_step = lr, global_step

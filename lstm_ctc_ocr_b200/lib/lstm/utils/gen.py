@@ -185,10 +185,21 @@ def generateImg(rng=random):
     return render_line(theChars, rng=rng), theChars
 
 
-def groupBatch(imgs, labels, pad_to=None):
+def feed_dtype(name):
+    """cfg.FEED_DTYPE ("float32" or "uint8") -> the numpy dtype of the batches the data layer builds."""
+    if str(name) not in ("float32", "uint8"):
+        raise ValueError(f"FEED_DTYPE must be 'float32' or 'uint8', got {name!r}")
+    return np.dtype(str(name))
+
+
+def groupBatch(imgs, labels, pad_to=None, dtype=np.float32):
     """Resize to height 32 keeping aspect, time_step = nw//4 - 1, right-pad with 0 to a multiple of 4 (or to ``pad_to``), /255,
-    transpose to [W, 32] (gen.py:41-67)."""
+    transpose to [W, 32] (gen.py:41-67).  ``dtype=np.uint8``: the same lines as the resized 8-bit pixels, without the division
+    (uint8 images only); ``groupBatch(..., dtype=np.uint8)`` / 255 in f32 equals the default f32 batch bit for bit."""
     from PIL import Image
+    dtype = np.dtype(dtype)
+    if dtype not in (np.float32, np.uint8):
+        raise ValueError(f"groupBatch builds float32 or uint8 batches, not {dtype}")
     nh = cfg.IMG_HEIGHT
     resized, time_steps, label_len, label_vec = [], [], [], []
     max_w = 0
@@ -196,7 +207,9 @@ def groupBatch(imgs, labels, pad_to=None):
         h, w = img.shape[:2]
         nw = int(nh / h * w)
         max_w = max(max_w, nw)
-        resized.append(np.asarray(Image.fromarray(img).resize((nw, nh), Image.BILINEAR), dtype=np.float32))
+        if dtype == np.uint8 and np.asarray(img).dtype != np.uint8:
+            raise ValueError("uint8 batches are built from 8-bit images")
+        resized.append(np.asarray(Image.fromarray(img).resize((nw, nh), Image.BILINEAR), dtype=dtype))
         time_steps.append(nw // cfg.POOL_SCALE + cfg.OFFSET_TIME_STEP)
         label_vec.extend(encode_maps[c] for c in lab)
         label_len.append(len(lab))
@@ -206,9 +219,12 @@ def groupBatch(imgs, labels, pad_to=None):
             raise ValueError(f"line of width {max_w} does not fit the bucket width {pad_to}")
         max_w = int(pad_to)
     # one zero-filled [N, W, 32] block, every line written transposed into its rows; the list holds its N contiguous [W, 32] views
-    block = np.zeros((len(resized), max_w, nh), np.float32)
+    block = np.zeros((len(resized), max_w, nh), dtype)
     for i, im in enumerate(resized):
-        np.divide(im.T, np.float32(255.0), out=block[i, :im.shape[1], :])
+        if dtype == np.uint8:
+            block[i, :im.shape[1], :] = im.T
+        else:
+            np.divide(im.T, np.float32(255.0), out=block[i, :im.shape[1], :])
     return list(block), label_vec, label_len, time_steps
 
 
@@ -218,25 +234,31 @@ def batch_seed(k, seed=None, rank=0, world=1):
     return int(cfg.RNG_SEED if seed is None else seed) + k * int(world) + int(rank)
 
 
-def make_batch(k, batch_size=32, render=True, seed=None, rank=0, world=1, bucket=None, width=None, lens=None):
+def _synth_pixels(data, dtype):
+    """Synthetic f32 pixels in [0, 1) as the batch dtype: uint8 rounds them to bytes (the synthetic stream has no 8-bit source)."""
+    return data if np.dtype(dtype) == np.float32 else np.rint(data * np.float32(255)).astype(np.uint8)
+
+
+def make_batch(k, batch_size=32, render=True, seed=None, rank=0, world=1, bucket=None, width=None, lens=None, dtype=np.float32):
     """Batch k of a deterministic stream (picklable entry point of the feeder's worker processes).
     ``bucket`` = None: the reference's 4-6 character lines padded to the batch max width; else one of BUCKETS.
     ``lens`` = (min, max) characters per line of the bucket-less stream, cfg.MIN_LEN / cfg.MAX_LEN when None (worker
-    processes start from the default configuration, so the feeder passes the parent's values)."""
+    processes start from the default configuration, so the feeder passes the parent's values).  ``dtype``: float32 or uint8
+    pixels (groupBatch)."""
     s = batch_seed(k, seed, rank, world)
     if not render:
         if width is not None:                  # full-width synthetic lines (the throughput workloads)
             data, lab, ll, tsl = synthetic.synth_batch(batch_size, int(width), seed=s)
-            return data, lab.tolist(), ll.tolist(), tsl.tolist()
+            return _synth_pixels(data, dtype), lab.tolist(), ll.tolist(), tsl.tolist()
         if bucket is None:
             data, lab, ll, tsl = synthetic.synth_batch(batch_size, 88, seed=s, widths=[85] * batch_size)
         else:
             data, lab, ll, tsl = synthetic.synth_bucket_batch(batch_size, bucket, seed=s, buckets=BUCKETS)
-        return list(data), lab.tolist(), ll.tolist(), tsl.tolist()
+        return list(_synth_pixels(data, dtype)), lab.tolist(), ll.tolist(), tsl.tolist()
     rng = random.Random(s)
     if bucket is None:
         labels = [gen_rand(rng, *(lens or (None, None))) for _ in range(batch_size)]
-        return groupBatch([render_line(l, rng=rng) for l in labels], labels)
+        return groupBatch([render_line(l, rng=rng) for l in labels], labels, dtype=dtype)
     lo = max([b for b in BUCKETS if b < bucket] or [0])
     cmin, cmax = BUCKET_CHARS[bucket]
     imgs, labels = [], []
@@ -246,7 +268,7 @@ def make_batch(k, batch_size=32, render=True, seed=None, rank=0, world=1, bucket
         nw = int(cfg.IMG_HEIGHT / im.shape[0] * im.shape[1])
         if lo < nw <= bucket:                      # rejection: the resized width must fall into (previous bucket, bucket]
             imgs.append(im); labels.append(text)
-    return groupBatch(imgs, labels, pad_to=bucket)
+    return groupBatch(imgs, labels, pad_to=bucket, dtype=dtype)
 
 
 def generator(batch_size=32, vis=False, render=None, seed=None, rank=None, world=None):
@@ -264,8 +286,9 @@ class BucketSampler(object):
     """Width-bucketed batch stream (BASELINE configs[3]): batch k comes from bucket ``order[k % len(order)]`` and is padded to
     that bucket's width.  Iterating yields data-layer tuples; ``.bucket_of(k)`` tells which width batch k has."""
 
-    def __init__(self, batch_size=512, buckets=BUCKETS, render=None, seed=None, rank=None, world=None, order=None):
+    def __init__(self, batch_size=512, buckets=BUCKETS, render=None, seed=None, rank=None, world=None, order=None, dtype=np.float32):
         self.batch_size, self.buckets = batch_size, tuple(buckets)
+        self.dtype = np.dtype(dtype)
         self.render = can_render() if render is None else render
         self.seed = seed
         if rank is None or world is None:
@@ -278,7 +301,7 @@ class BucketSampler(object):
 
     def args(self, k):
         return dict(k=k, batch_size=self.batch_size, render=self.render, seed=self.seed, rank=self.rank, world=self.world,
-                    bucket=self.bucket_of(k))
+                    bucket=self.bucket_of(k), dtype=self.dtype)
 
     def batch(self, k):
         return make_batch(**self.args(k))
@@ -314,21 +337,24 @@ def _attach(name):
 
 
 def _fill(buf, kwargs):
-    """Produce batch `kwargs` and write it into `buf` as [N, W, 32] f32; returns (N, W, labels, label_len, time_steps)."""
+    """Produce batch `kwargs` and write it into `buf` as [N, W, 32] of its dtype (f32 or uint8); returns (N, W, labels, label_len,
+    time_steps)."""
     cache = kwargs.pop("cache", 0)
     if cache and not kwargs.get("render", True):
         # synthetic stream for throughput runs: `cache` distinct batches per producer, generated once, then re-written into the
         # slot every time (the per-step work that remains is the copy into page-locked memory a real decoder would do)
-        key = (kwargs["batch_size"], kwargs.get("width"), kwargs.get("seed"), kwargs.get("rank"), kwargs["k"] % cache)
+        key = (kwargs["batch_size"], kwargs.get("width"), kwargs.get("seed"), kwargs.get("rank"), kwargs["k"] % cache,
+               np.dtype(kwargs.get("dtype", np.float32)).str)
         if key not in _SYNTH_CACHE:
             _SYNTH_CACHE[key] = make_batch(**dict(kwargs, k=kwargs["k"] % cache))
         imgs, lab, ll, tsl = _SYNTH_CACHE[key]
     else:
         imgs, lab, ll, tsl = make_batch(**kwargs)
     N, W = len(imgs), imgs[0].shape[0]
-    if N * W * cfg.NUM_FEATURES * 4 > len(buf):
+    dt = np.dtype(kwargs.get("dtype", np.float32))
+    if N * W * cfg.NUM_FEATURES * dt.itemsize > len(buf):
         raise ValueError(f"batch [{N},{W}] does not fit the feeder's ring slot")
-    view = np.ndarray((N, W, cfg.NUM_FEATURES), np.float32, buffer=buf)
+    view = np.ndarray((N, W, cfg.NUM_FEATURES), dt, buffer=buf)
     if isinstance(imgs, np.ndarray):
         np.copyto(view, imgs)
     else:
@@ -349,7 +375,8 @@ def _warm_synth_cache(kwargs_list):
     for kw in kwargs_list:
         kw = dict(kw)
         cache = kw.pop("cache", 0)
-        key = (kw["batch_size"], kw.get("width"), kw.get("seed"), kw.get("rank"), kw["k"] % max(cache, 1))
+        key = (kw["batch_size"], kw.get("width"), kw.get("seed"), kw.get("rank"), kw["k"] % max(cache, 1),
+               np.dtype(kw.get("dtype", np.float32)).str)
         if cache and key not in _SYNTH_CACHE:
             _SYNTH_CACHE[key] = make_batch(**dict(kw, k=kw["k"] % cache))
 
@@ -363,15 +390,17 @@ class PrefetchFeeder(object):
     batches are in flight / ready ahead of the consumer, delivered in order as ``(ndarray view [N,W,32], labels, label_len,
     time_steps)`` (the three integer feeds as int32 arrays).  ``Session.run`` recognises the view as page-locked (crnn_host_is_pinned) and DMAs straight from it (chunked
     crnn_forward_host).  The ring has ``depth + keep`` slots: the views of the last ``keep`` delivered batches are never
-    rewritten, so the consumer may still be DMA-ing from batch j while batches j+1 .. j+depth are produced."""
+    rewritten, so the consumer may still be DMA-ing from batch j while batches j+1 .. j+depth are produced.  The batches' dtype
+    (float32 or uint8 pixels) is the ``dtype`` of ``arg_fn``'s kwargs; slots are sized by its item size."""
 
     def __init__(self, arg_fn, num_workers=4, depth=3, max_width=256, batch_size=None, pinned=True, keep=3, warm=None):
         from multiprocessing import shared_memory
         self.arg_fn, self.depth, self.keep = arg_fn, max(1, int(depth)), max(1, int(keep))
         self.num_workers = int(num_workers)
         self.batch_size = batch_size if batch_size is not None else arg_fn(0)["batch_size"]
+        self.dtype = np.dtype(arg_fn(0).get("dtype", np.float32))
         self.max_width = int(max_width)
-        self.slot_bytes = self.batch_size * self.max_width * cfg.NUM_FEATURES * 4
+        self.slot_bytes = self.batch_size * self.max_width * cfg.NUM_FEATURES * self.dtype.itemsize
         self._shm, self._registered = [], []
         self._rt = None
         if pinned:
@@ -437,7 +466,7 @@ class PrefetchFeeder(object):
             self._submit()
         else:
             N, W, lab, ll, tsl = _fill(self._slot(k).buf, self.arg_fn(k))
-        view = np.ndarray((N, W, cfg.NUM_FEATURES), np.float32, buffer=self._slot(k).buf)
+        view = np.ndarray((N, W, cfg.NUM_FEATURES), self.dtype, buffer=self._slot(k).buf)
         return view, lab, ll, tsl
 
     def close(self):
@@ -482,11 +511,12 @@ def get_batch(num_workers, **kwargs):
     if rank is None or world is None:
         rank, world = _dist_rank_world()
     bucket = kwargs.pop("bucket", None)
+    dtype = np.dtype(kwargs.pop("dtype", np.float32))         # float32 or uint8 pixels (groupBatch)
 
     lens = (cfg.MIN_LEN, cfg.MAX_LEN)          # this process's configuration (e.g. --set MIN_LEN 30 MAX_LEN 70), for the workers
 
     def arg_fn(k):
-        return dict(k=k, batch_size=batch_size, render=render, seed=seed, rank=rank, world=world, bucket=bucket, lens=lens)
+        return dict(k=k, batch_size=batch_size, render=render, seed=seed, rank=rank, world=world, bucket=bucket, lens=lens, dtype=dtype)
     if num_workers is None or num_workers <= 1 or not render:
         return (make_batch(**arg_fn(k)) for k in _count())
     # ring slots hold the widest batch the configured line lengths can render (cfg.MAX_LEN 70 lines are about 1 000 px wide);

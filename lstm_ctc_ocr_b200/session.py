@@ -11,7 +11,7 @@ from . import engine
 from ._lib import CrnnError
 from .lib.networks.network import Fetch, Placeholder
 
-_NP2T = {np.dtype("float32"): torch.float32, np.dtype("int32"): torch.int32}
+_NP2T = {np.dtype("float32"): torch.float32, np.dtype("int32"): torch.int32, np.dtype("uint8"): torch.uint8}
 
 
 class _Pinned(object):
@@ -90,12 +90,13 @@ class _Pinned(object):
         ev.record()
         return {k: d[offs[k]:offs[k] + a.size].view(a.shape) for k, a in arrays.items()}
 
-    def staging_for(self, name, numel):
-        """Page-locked f32 staging buffer `name` with room for `numel` elements, safe to overwrite (the previous DMA out of it has
-        completed), and the event the caller must record after issuing the next DMA out of it."""
+    def staging_for(self, name, numel, dtype=torch.float32):
+        """Page-locked staging buffer `name` of `dtype` (f32, or uint8 for pixel batches) with room for `numel` elements, safe to
+        overwrite (the previous DMA out of it has completed), and the event the caller must record after issuing the next DMA out
+        of it."""
         t = self.bufs.get(name)
-        if t is None or t.numel() < numel or t.dtype != torch.float32:
-            t = self.bufs[name] = torch.empty(max(numel, 1), dtype=torch.float32).pin_memory()
+        if t is None or t.numel() < numel or t.dtype != dtype:
+            t = self.bufs[name] = torch.empty(max(numel, 1), dtype=dtype).pin_memory()
             self.events.pop(name, None)
         ev = self.events.get(name)
         if ev is not None:
@@ -186,13 +187,13 @@ class Session(object):
         except StopIteration:
             return
         data = nxt[0]
-        if not (isinstance(data, np.ndarray) and data.dtype == np.float32 and data.flags.c_contiguous and data.ndim == 3
+        if not (isinstance(data, np.ndarray) and data.dtype in (np.float32, np.uint8) and data.flags.c_contiguous and data.ndim == 3
                 and self._pinned.is_page_locked(data)):
             return
         i = self._ahead_idx
         buf = self._ahead_bufs[i]
-        if buf is None or tuple(buf.shape) != tuple(data.shape):
-            buf = self._ahead_bufs[i] = torch.empty(data.shape, dtype=torch.float32, device=self.device)
+        if buf is None or tuple(buf.shape) != tuple(data.shape) or buf.dtype != _NP2T[data.dtype]:
+            buf = self._ahead_bufs[i] = torch.empty(data.shape, dtype=_NP2T[data.dtype], device=self.device)
             self._ahead_free[i] = None
         if self._ahead_stream is None:
             self._ahead_stream = torch.cuda.Stream(device=self.device)
@@ -224,7 +225,8 @@ class Session(object):
             return None
         self._ahead = None
         seq, ptr, nbytes, buf, ev, i, ints = a
-        if seq != f.delivered - 1 or ptr != data.ctypes.data or nbytes != data.nbytes or tuple(buf.shape) != tuple(data.shape):
+        if (seq != f.delivered - 1 or ptr != data.ctypes.data or nbytes != data.nbytes or tuple(buf.shape) != tuple(data.shape)
+                or buf.dtype != _NP2T[data.dtype]):
             return None
         torch.cuda.current_stream(self.device).wait_event(ev)
         self._pinned.pending.append(ev)        # the ring slot must not be recycled before this DMA is done (it is, long before)
@@ -328,6 +330,16 @@ class Session(object):
             if (tsl > line_width // 4 - 1).any():
                 raise ValueError("time_step_len[i] must be <= line_width[i]/4 - 1 (frames past a line are not defined)")
 
+    @staticmethod
+    def _data_feed(feeds):
+        """The fed batch: `data` widened to f32 as a TF float placeholder casts it, or `data_u8` kept as uint8 pixels (the engine's
+        u8 entry points divide by 255 on the device).  Feeding both is ambiguous and refused."""
+        if "data_u8" in feeds:
+            if "data" in feeds:
+                raise ValueError("feed either data or data_u8, not both")
+            return np.asarray(feeds["data_u8"], dtype=np.uint8)
+        return np.asarray(feeds["data"], dtype=np.float32)
+
     def run(self, fetches, feed_dict=None):
         single = not isinstance(fetches, (list, tuple))
         flist = [fetches] if single else list(fetches)
@@ -345,7 +357,7 @@ class Session(object):
             feeds[k.name] = v
         kinds = [f.kind for f in flist]
         need_labels = any(k in ("loss", "ctc_costs", "train_op", "ctc_grad") for k in kinds)
-        data = np.asarray(feeds["data"], dtype=np.float32)
+        data = self._data_feed(feeds)
         tsl = np.asarray(feeds["time_step_len"], dtype=np.int32)
         labels = np.asarray(feeds["labels"], dtype=np.int32) if need_labels else None
         llen = np.asarray(feeds["labels_len"], dtype=np.int32) if need_labels else None
@@ -389,12 +401,12 @@ class Session(object):
         elif self.pageable_pool and self.h2d_chunks > 1 and data.nbytes >= self._pinned.REGISTER_MIN_BYTES:
             # large batch in ordinary memory (the reference's np.array(...) per step): the library's host threads move it into
             # page-locked staging range by range while the GPU copies / computes the previous range (crnn_forward_pageable)
-            pin, ev = self._pinned.staging_for("data", data.size)
+            pin, ev = self._pinned.staging_for("data" + engine._feed_suffix(data.dtype), data.size, _NP2T[data.dtype])
             logits, d_data, cst = eng.forward_pageable(data, pin, d_tsl, chunks=self.h2d_chunks, host_threads=self.host_copy_threads)
             ev.record(cst)
             self.last_feed_path = "staged"
         else:
-            d_data = self._pinned.stage("data", data, dev)
+            d_data = self._pinned.stage("data" + engine._feed_suffix(data.dtype), data, dev)
             logits = eng.forward(d_data, d_tsl)
             self.last_feed_path = "staged"
         costs = grad = loss = None
@@ -460,7 +472,7 @@ class Session(object):
             ints["labels"], ints["llen"] = labels, llen
         d_ints = self._pinned.stage_ints(ints, self.device)
         d_tsl = d_ints["tsl"]
-        d_data = self._pinned.stage("data", data, self.device)
+        d_data = self._pinned.stage("data" + engine._feed_suffix(data.dtype), data, self.device)
         self.h2d_bytes = data.nbytes + tsl.nbytes + line_width.nbytes + (labels.nbytes + llen.nbytes if labels is not None else 0)
         self.last_feed_path = "staged"
         logits = eng.forward_lines(d_data, d_ints["lw"], d_tsl)

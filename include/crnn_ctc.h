@@ -76,6 +76,38 @@ int crnn_ctc_loss(const float* logits, float* grad, const int* flat_labels, cons
                   float grad_scale, float* costs, void* workspace, size_t workspace_bytes,
                   crnn_stream_t stream);
 
+/* CTC forced alignment: the best path (Viterbi, max-plus form of the alpha recursion above) of a GIVEN labelling, where each
+ * label sits in it and how sure the model is of each label.  Per utterance n, with y_t = softmax(logits[t,n,:]) (max
+ * subtracted), the extended labelling l' = (blank, l_1, blank, ..., l_L, blank) of S = 2L+1 states and e_t(s) = log y_t(l'_s):
+ *   v_0(0) = e_0(0), v_0(1) = e_0(1), every other state -inf;  v_t(s) = e_t(s) + max over P(s) of v_{t-1},
+ *   P(s) = {s, s-1}, plus s-2 when l'_s != blank and l'_s != l'_{s-2} (the transitions of crnn_ctc_loss).
+ * Ties: among predecessors s beats s-1, which beats s-2; at the end state S-1 beats S-2.  Natural log, f32 arithmetic
+ * (lse_t = m + log(sum exp(x - m)) per frame, e = x - lse_t).
+ *   logits        [T,N,C] f32, unnormalised, time-major; 4-byte alignment is enough
+ *   labels        label_stride == 0: flat [sum(label_len)] i32, utterance n at offset sum(label_len[0..n)) (crnn_ctc_loss's layout);
+ *                 label_stride > 0: dense rows [N, label_stride] i32 (the decoders' layout), row n holds its label_len[n] ids
+ *   label_len [N], input_len [N] i32 (input_len clamped to [0,T] = T_n); blank in [0,C) (class 0 is what warp-ctc trains as blank)
+ *   start, end    i32 and peak f32, indexed like `labels`: the best path is in label k's state 2k+1 during frames
+ *                 [start[k], end[k]) -- at least one frame, spans ordered and disjoint, a blank frame between equal neighbours;
+ *                 peak[k] = max over the span of y_t(l_k), the per-label confidence.  Dense rows are written in full: entries
+ *                 past label_len[n] get -1 / -1 / 0.
+ *   path_logprob  [N] f32: sum over t < T_n of e_t(pi_t) along the best path (log p of the best alignment, not of the labelling).
+ * Edge cases: L = 0 -> the all-blank path, no spans (path_logprob 0 when T_n = 0).  Infeasible labelling (T_n < L + number of
+ * adjacent equal pairs) -> path_logprob -inf, spans -1, peaks 0.  Invalid utterance, as in crnn_ctc_loss (an id outside [0,C)
+ * or equal to `blank`, label_len negative, above max_label_len or, dense, above label_stride) -> path_logprob NaN, spans -1,
+ * peaks 0; no invalid id is used as an index.
+ * Frames to pixels: frame t is conv5 output t, which reads pooled columns t and t+1, so the span [s, e) covers input columns
+ * [4s, 4e+4) of the line (3x3 halos aside).
+ * Supported: C = 64 and max_label_len <= 639 (S <= 1279), any T; otherwise CRNN_UNSUPPORTED.  The workspace (any alignment; size
+ * from crnn_ctc_align_workspace_size, no CUDA call) holds T * (8 + S_pad) bytes per utterance (S_pad = 2*max_label_len+1 rounded
+ * up to 4) plus 256.  Every pointer is a device pointer; the call is asynchronous on `stream` and allocates nothing.  A short
+ * workspace returns CRNN_WORKSPACE_TOO_SMALL, a null pointer CRNN_INVALID_VALUE; the outputs are then untouched.  The outputs do
+ * not depend on what the outputs or the workspace held before, and a run gives the same bits every time (no float atomics). */
+int crnn_ctc_align_workspace_size(int T, int N, int C, int max_label_len, size_t* bytes);
+int crnn_ctc_align(const float* logits, const int* labels, int label_stride, const int* label_len, const int* input_len, int T, int N,
+                   int C, int blank, int max_label_len, int* start, int* end, float* peak, float* path_logprob, void* workspace,
+                   size_t workspace_bytes, crnn_stream_t stream);
+
 /* Greedy decode.  Replaces tf.nn.ctc_*_decoder(merge_repeated=True) + sparse_tensor_to_dense
  * at lib/networks/network.py:656-657 and the zero stripping of lib/lstm/utils/training.py:32:
  * per frame argmax (lowest index on ties) for t < input_len; emit iff != tf_blank and != the

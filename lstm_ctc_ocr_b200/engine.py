@@ -501,6 +501,81 @@ def ctc_loss(logits, flat_labels, label_len, input_len, blank=0, want_grad=False
     return costs, (grad if want_grad else None)
 
 
+_align_ws = {}                # device -> workspace tensor of crnn_ctc_align, the largest size asked for so far
+
+
+def ctc_align_workspace_bytes(T, N, C, max_label_len):
+    """Bytes of device workspace crnn_ctc_align needs for this shape.  CrnnError (CRNN_UNSUPPORTED) for C != 64 or max_label_len
+    above 639.  No CUDA call."""
+    nbytes = _lib.c_size_t()
+    check(_lib.load().crnn_ctc_align_workspace_size(int(T), int(N), int(C), int(max_label_len), nbytes))
+    return int(nbytes.value)
+
+
+def ctc_align(logits, labels, label_len, input_len, blank=0, max_label_len=None, workspace="auto"):
+    """CTC forced alignment (crnn_ctc_align): the best path of each utterance's GIVEN labelling.  logits [T,N,64] f32 cuda;
+    labels i32 cuda, 2-D [N, M] dense rows (the decoders' layout: row n holds label_len[n] ids) or 1-D flat (crnn_ctc_loss's
+    layout); label_len, input_len [N] i32 cuda.  Returns device (start, end, peak, path_logprob): start / end i32 and peak f32
+    shaped like `labels` -- label k occupies frames [start, end) of the best path (input columns [4*start, 4*end + 4)), peak is
+    its largest posterior over them; dense entries past label_len[n] are -1 / -1 / 0 -- and path_logprob [N] f32 (natural log).
+    Infeasible labellings give -inf and spans -1, invalid ones (ids outside [0,64) or equal to the blank, label_len negative or
+    above max_label_len) NaN and spans -1.  max_label_len: None takes the row width for dense labels and label_len.max() for
+    flat ones (one host sync).  workspace: "auto" reuses a per-device buffer; a contiguous uint8 cuda tensor is passed as given.
+    No host fallback: CPU tensors raise CrnnError."""
+    tensors = (logits, labels, label_len, input_len)
+    if not all(torch.is_tensor(t) and t.is_cuda for t in tensors):
+        raise CrnnError("ctc_align needs CUDA tensors (sm_90a); there is no CPU fallback")
+    if logits.dtype != torch.float32 or logits.dim() != 3 or any(t.dtype != torch.int32 for t in tensors[1:]):
+        raise CrnnError("ctc_align: logits must be [T,N,64] f32 and labels, label_len, input_len i32")
+    if labels.dim() not in (1, 2):
+        raise CrnnError("ctc_align: labels must be 1-D (flat) or 2-D (dense rows)")
+    lib = _lib.load()
+    logits, labels = logits.contiguous(), labels.contiguous()
+    label_len, input_len = label_len.contiguous(), input_len.contiguous()
+    T, N, C = logits.shape
+    if label_len.numel() != N or input_len.numel() != N or (labels.dim() == 2 and labels.shape[0] != N):
+        raise CrnnError("ctc_align: labels (dense), label_len and input_len must hold one entry / row per utterance")
+    dense = labels.dim() == 2
+    if max_label_len is None:
+        max_label_len = labels.shape[1] if dense else (int(label_len.max().item()) if N else 0)
+    dev = logits.device
+    start = torch.empty(labels.shape, dtype=torch.int32, device=dev)
+    end = torch.empty(labels.shape, dtype=torch.int32, device=dev)
+    peak = torch.empty(labels.shape, dtype=torch.float32, device=dev)
+    lp = torch.empty(N, dtype=torch.float32, device=dev)
+    # a labelling with no ids at all (every L = 0) still passes non-null pointers; dense rows of width 0 are the flat layout
+    stride = labels.shape[1] if dense else 0
+    if labels.numel() == 0:
+        labels = torch.zeros(1, dtype=torch.int32, device=dev)
+        bufs = [torch.empty(1, dtype=t.dtype, device=dev) for t in (start, end, peak)]
+    else:
+        bufs = [start, end, peak]
+    nbytes = ctc_align_workspace_bytes(T, N, C, max_label_len)
+    if isinstance(workspace, str):
+        if workspace != "auto":
+            raise CrnnError(f"ctc_align: workspace must be 'auto' or a cuda tensor, got {workspace!r}")
+        workspace = _align_ws.get(dev)
+        if workspace is None or workspace.numel() < nbytes:
+            _align_ws.pop(dev, None)
+            workspace = _align_ws[dev] = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    if not (torch.is_tensor(workspace) and workspace.is_cuda and workspace.is_contiguous()):
+        raise CrnnError("ctc_align: workspace must be a contiguous cuda tensor")
+    check(lib.crnn_ctc_align(logits.data_ptr(), labels.data_ptr(), stride, label_len.data_ptr(), input_len.data_ptr(), T, N, C,
+                             int(blank), int(max_label_len), bufs[0].data_ptr(), bufs[1].data_ptr(), bufs[2].data_ptr(), lp.data_ptr(),
+                             workspace.data_ptr(), workspace.numel() * workspace.element_size(), _stream()))
+    return start, end, peak, lp
+
+
+def alignment_dict(labels, start, end, peak, path_logprob):
+    """Host arrays of one alignment, dense [N, M] (entries past each length: label 0, span -1, peak 0), as Session.run returns
+    them for "read_alignment" / "label_alignment": labels, start, end, x0 / x1 (the input columns [4*start, 4*end + 4) the span
+    covers: frame t is conv5 output t, which reads pooled columns t and t+1), peak and path_logprob [N]."""
+    start, end = np.asarray(start, np.int32), np.asarray(end, np.int32)
+    return dict(labels=np.asarray(labels, np.int32), start=start, end=end,
+                x0=np.where(start >= 0, 4 * start, -1).astype(np.int32), x1=np.where(end >= 0, 4 * end + 4, -1).astype(np.int32),
+                peak=np.asarray(peak, np.float32), path_logprob=np.asarray(path_logprob, np.float32))
+
+
 def ctc_greedy(logits, input_len, tf_blank=TF_BLANK, strip=0):
     """Returns (out [N,T] i32 zero padded, out_len [N] i32) on device."""
     lib = _lib.load()

@@ -58,7 +58,10 @@ _DEFAULTS = {
              "COMPUTE_DTYPE": "bf16",
              # not in the reference (it evaluates with is_training=True): "moving" normalises conv4_1 / conv4_2 of LSTM_test networks
              # with the moving mean / variance training tracks (TF's is_training=False); "batch" with the evaluated batch's statistics
-             "BN_STATS": "batch"},
+             "BN_STATS": "batch",
+             # not in the reference: True adds to each file's line of test_model the read's confidence exp(path_logprob) (the
+             # probability of its best CTC alignment) and each character's peak posterior (Session.run's "read_alignment")
+             "CONFIDENCE": False},
 }
 
 

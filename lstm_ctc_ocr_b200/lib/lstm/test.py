@@ -97,6 +97,9 @@ class SolverWrapper(object):
         dense_decoded = self.net.get_output("logits").net  # noqa: F841  (handle kept for symmetry with the reference)
         from ..networks.network import Fetch
         dense_decoded = Fetch(self.net, "dense_decoded")
+        confidence = bool(cfg.TEST.get("CONFIDENCE", False))
+        if confidence:      # the alignment's labels are dense_decoded's
+            dense_decoded = Fetch(self.net, "read_alignment")
         if restore:
             from .train import SolverWrapper as TrainSolver
             ts = TrainSolver.__new__(TrainSolver)
@@ -116,7 +119,7 @@ class SolverWrapper(object):
         order = sorted(range(len(files)), key=lambda i: lines[i][0].shape[1])
         bs = max(1, int(cfg.TEST.BATCH_SIZE))
         timer = Timer()
-        res_of, time_of = {}, {}
+        res_of, time_of, conf_of = {}, {}, {}
         for b0 in range(0, len(order), bs):
             idx = order[b0:b0 + bs]
             timer.tic()
@@ -124,9 +127,15 @@ class SolverWrapper(object):
             feed_dict = {(self.net.data_u8 if dtype == np.uint8 else self.net.data): data, self.net.line_width: lw, self.net.time_step_len: tsl, self.net.keep_prob: 1.0}
             dense = sess.run(fetches=dense_decoded, feed_dict=feed_dict)
             dt = timer.toc(average=False) / len(idx)
+            if confidence:
+                al, dense = dense, dense["labels"]
             for r, i in enumerate(idx):
                 res_of[i] = "".join(decodeRes(dense[r]))
                 time_of[i] = dt
+                if confidence:
+                    k = int((dense[r] != 0).sum())
+                    conf_of[i] = ", conf: {:.4f}, peaks: [{}]".format(float(np.exp(np.float64(al["path_logprob"][r]))),
+                                                                     " ".join("{:.3f}".format(float(p)) for p in al["peak"][r, :k]))
         total = correct = 0
         for i, file in enumerate(files):
             total += 1
@@ -134,7 +143,7 @@ class SolverWrapper(object):
             if org == res_of[i]:
                 correct += 1
             print(file, end=" ")
-            print("cost time: {:.3f},\n    res: {}".format(time_of[i], res_of[i]))
+            print("cost time: {:.3f},\n    res: {}{}".format(time_of[i], res_of[i], conf_of.get(i, "")))
         print("total acc:{}/{}={:.4f}".format(correct, total, correct / max(total, 1)))
         return correct, total
 

@@ -12,6 +12,7 @@ from ._lib import CrnnError
 from .lib.networks.network import Fetch, Placeholder
 
 _NP2T = {np.dtype("float32"): torch.float32, np.dtype("int32"): torch.int32, np.dtype("uint8"): torch.uint8}
+LOSS_KINDS = ("loss", "ctc_costs", "train_op", "ctc_grad")
 
 
 class _Pinned(object):
@@ -356,7 +357,8 @@ class Session(object):
                 raise TypeError("feed_dict keys must be the network's placeholders")
             feeds[k.name] = v
         kinds = [f.kind for f in flist]
-        need_labels = any(k in ("loss", "ctc_costs", "train_op", "ctc_grad") for k in kinds)
+        need_loss = any(k in LOSS_KINDS for k in kinds)
+        need_labels = need_loss or "label_alignment" in kinds
         data = self._data_feed(feeds)
         tsl = np.asarray(feeds["time_step_len"], dtype=np.int32)
         labels = np.asarray(feeds["labels"], dtype=np.int32) if need_labels else None
@@ -409,10 +411,11 @@ class Session(object):
             d_data = self._pinned.stage("data" + engine._feed_suffix(data.dtype), data, dev)
             logits = eng.forward(d_data, d_tsl)
             self.last_feed_path = "staged"
-        costs = grad = loss = None
+        costs = grad = loss = d_lab = d_ll = None
         if need_labels:
             d_lab, d_ll = d_ints["labels"], d_ints["llen"]
             self.h2d_bytes += labels.nbytes + llen.nbytes
+        if need_loss:
             N = data.shape[0]
             # warp-ctc computes the gradient inside its forward op; so does this kernel (one launch)
             costs, grad = engine.ctc_loss(logits, d_lab, d_ll, d_tsl, want_grad=True, grad_scale=1.0 / N,
@@ -435,6 +438,10 @@ class Session(object):
                 v = logits.cpu().numpy()
             elif k == "dense_decoded":
                 v = self._decode(logits, d_tsl)
+            elif k == "read_alignment":
+                v = self._read_alignment(logits, d_tsl)
+            elif k == "label_alignment":
+                v = self._label_alignment(logits, d_tsl, d_lab, d_ll, llen)
             elif k == "train_op":
                 v = f.step_fn(eng, logits, grad, d_data, d_tsl)
                 self._stage_ahead()
@@ -446,6 +453,8 @@ class Session(object):
                 raise ValueError(f"unknown fetch {f}")
             if isinstance(v, np.ndarray):
                 self.d2h_bytes += v.nbytes
+            elif isinstance(v, dict):
+                self.d2h_bytes += sum(a.nbytes for a in v.values())
             elif isinstance(v, (np.floating, float)):
                 self.d2h_bytes += 4
             out.append(v)
@@ -477,7 +486,7 @@ class Session(object):
         self.last_feed_path = "staged"
         logits = eng.forward_lines(d_data, d_ints["lw"], d_tsl)
         costs = grad = loss = None
-        if labels is not None:
+        if any(k in LOSS_KINDS for k in kinds):
             costs, grad = engine.ctc_loss(logits, d_ints["labels"], d_ints["llen"], d_tsl, want_grad="ctc_grad" in kinds,
                                           grad_scale=1.0 / data.shape[0], max_label_len=int(llen.max()) if llen.size else 0,
                                           workspace="auto")
@@ -494,6 +503,10 @@ class Session(object):
                 v = logits.cpu().numpy()
             elif k == "dense_decoded":
                 v = self._decode(logits, d_tsl)
+            elif k == "read_alignment":
+                v = self._read_alignment(logits, d_tsl)
+            elif k == "label_alignment":
+                v = self._label_alignment(logits, d_tsl, d_ints["labels"], d_ints["llen"], llen)
             elif k.startswith("layer:"):
                 name = k.split(":", 1)[1]
                 tapname = {"pool1": "conv1", "pool2": "conv3_2", "pool3": "conv4_2", "reshaped_layer": "conv5"}.get(name, name)
@@ -501,17 +514,47 @@ class Session(object):
             else:
                 raise ValueError(f"unknown fetch kind {k!r}")
             out.append(v)
-        self.d2h_bytes = sum(v.nbytes if isinstance(v, np.ndarray) else 4 for v in out)
+        self.d2h_bytes = sum(v.nbytes if isinstance(v, np.ndarray) else sum(a.nbytes for a in v.values()) if isinstance(v, dict) else 4
+                             for v in out)
         self._pinned.wait_pending()
         return out[0] if single else out
 
     @staticmethod
-    def _decode(logits, d_tsl):
-        """dense_decoded of device logits with cfg.DECODER (greedy, or the reference's beam search on the device)."""
+    def _decode_device(logits, d_tsl):
+        """(out [N,T], out_len [N]) on the device, decoded with cfg.DECODER (greedy, or the reference's beam search)."""
         from .lib.lstm.config import cfg
         if str(cfg.get("DECODER", "greedy")) == "beam":
             # the reference's own decoder (network.py:656): prefix beam search, width 100, blank 63, on the device
             o, ol, _ = engine.ctc_beam_search_device(logits, d_tsl, beam_width=int(cfg.get("BEAM_WIDTH", 100)), merge_repeated=True)
         else:
             o, ol = engine.ctc_greedy(logits, d_tsl)
-        return engine.dense_decoded(o, ol).cpu().numpy()
+        return o, ol
+
+    @staticmethod
+    def _decode(logits, d_tsl):
+        """dense_decoded of device logits with cfg.DECODER (greedy, or the reference's beam search on the device)."""
+        return engine.dense_decoded(*Session._decode_device(logits, d_tsl)).cpu().numpy()
+
+    @staticmethod
+    def _read_alignment(logits, d_tsl):
+        """"read_alignment": the best alignment (blank 0) of the read dense_decoded returns, as engine.alignment_dict."""
+        o, ol = Session._decode_device(logits, d_tsl)
+        dense = engine.dense_decoded(o, ol)
+        r = engine.ctc_align(logits, dense, ol, d_tsl, blank=0, max_label_len=dense.shape[1])
+        return engine.alignment_dict(dense.cpu().numpy(), *(a.cpu().numpy() for a in r))
+
+    @staticmethod
+    def _label_alignment(logits, d_tsl, d_lab, d_ll, llen):
+        """"label_alignment": the best alignment (blank 0) of the fed flat labels, laid out [N, max(labels_len)] as
+        engine.alignment_dict (label 0, span -1 and peak 0 past each length)."""
+        N = llen.size
+        M = int(llen.max()) if N else 0
+        r = [a.cpu().numpy() for a in engine.ctc_align(logits, d_lab, d_ll, d_tsl, blank=0, max_label_len=M)]
+        rows = np.repeat(np.arange(N), llen)
+        cols = np.arange(llen.sum()) - np.repeat(np.cumsum(llen) - llen, llen)
+        out = []
+        for flat, fill, dt in ((d_lab.cpu().numpy(), 0, np.int32), (r[0], -1, np.int32), (r[1], -1, np.int32), (r[2], 0, np.float32)):
+            a = np.full((N, M), fill, dt)
+            a[rows, cols] = flat
+            out.append(a)
+        return engine.alignment_dict(out[0], out[1], out[2], out[3], r[3])

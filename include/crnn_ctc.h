@@ -108,6 +108,47 @@ int crnn_ctc_align(const float* logits, const int* labels, int label_stride, con
                    int C, int blank, int max_label_len, int* start, int* end, float* peak, float* path_logprob, void* workspace,
                    size_t workspace_bytes, crnn_stream_t stream);
 
+/* Lexicon-based reading (CRNN's lexicon transcription, Shi, Bai & Yao, §2.3.2): for each line the lexicon entry l* that
+ * maximises p(l | y), searched among the entries within edit distance max_edit of the lexicon-free read.  Two calls: the
+ * candidates by edit distance, then their CTC scores.  The lexicon is caller-owned device CSR:
+ *   lex_ids  i32, the entries' class ids concatenated;  lex_off [K+1] i32, entry k is lex_ids[lex_off[k] .. lex_off[k+1])
+ *   max_entry_len  a host-side bound on every entry's length, at most 63 (else CRNN_UNSUPPORTED).  An entry longer than it (or
+ *                  with lex_off decreasing) is never a candidate, and scores NaN.
+ *
+ * crnn_lexicon_candidates: reads [N, read_stride] i32 and read_len [N] i32 in the decoders' dense layout (engine.dense_decoded;
+ * read_len clamped to [0, read_stride]).  d = the Levenshtein distance (unit insert, delete, substitute) between the read and an
+ * entry, compared id for id; an id outside [0,64), in a read or an entry, matches nothing (not even itself) and is never used as
+ * an index.  The candidates are the entries with d <= max_edit (max_edit < 0: no threshold), ordered by (d, lexicon index); the
+ * first max_candidates (1 .. 256) are kept:
+ *   cand [N, max_candidates] i32       the lexicon index, -1 past the count
+ *   cand_dist [N, max_candidates] i32  d, -1 past the count
+ *   cand_total [N] i32                 how many entries have d <= max_edit (all well-formed entries when max_edit < 0), so a
+ *                                      truncated list is visible
+ * Ties at the last kept distance go to the lower lexicon indices.  The outputs are the same bits run to run and do not depend
+ * on what they held before (integer arithmetic, a fixed order; no workspace).  Supported: read_stride <= 1024 (the read is the
+ * pattern of a bit-parallel Levenshtein kernel, 16 words of 64 rows), else CRNN_UNSUPPORTED.
+ *
+ * crnn_ctc_lexicon_score: score[n, j] = ln p(lex[cand[n, j]] | y_n), the sum over the CTC lattice of crnn_ctc_loss (same
+ * transitions and `blank`; mathematically -cost of crnn_ctc_loss on that labelling), f32 in log2 arithmetic as crnn_ctc_loss
+ * computes it (log2-softmax with the row maximum subtracted), returned in natural log.
+ *   logits [T,N,C] f32, input_len [N] i32 (clamped to [0,T] = T_n); blank in [0,C) (0 is the blank warp-ctc trains);
+ *   cand [N, max_candidates] i32 as crnn_lexicon_candidates writes it (any value below 0 is an empty slot; an index must be < K).
+ *   score [N, max_candidates] f32;  best [N] i32: the lexicon index of the highest finite score, ties to the lowest slot (the
+ *   nearer distance, then the lower index), -1 when no slot has a finite score;  best_score [N] f32: its score, or -inf.
+ * Special values: an empty slot -> -inf; an infeasible labelling (T_n < L + number of adjacent equal pairs) -> -inf; L = 0 is the
+ * all-blank path (0 when T_n = 0); an invalid entry (an id outside [0,C) or equal to `blank`, or longer than max_entry_len) ->
+ * NaN.  No float atomics: the same bits run to run.
+ * Supported: C = 64 and T <= 768 (the line's log2-softmax, 256 B per frame, is kept in shared memory and shared by all of its
+ * candidates), otherwise CRNN_UNSUPPORTED with crnn_last_error() naming T or the entry length.
+ * Both calls: every pointer a device pointer, asynchronous on `stream`, no allocation; a null pointer returns
+ * CRNN_INVALID_VALUE and every status other than CRNN_OK leaves the outputs untouched. */
+int crnn_lexicon_candidates(const int* reads, int read_stride, const int* read_len, int N, const int* lex_ids, const int* lex_off,
+                            int K, int max_entry_len, int max_edit, int max_candidates, int* cand, int* cand_dist, int* cand_total,
+                            crnn_stream_t stream);
+int crnn_ctc_lexicon_score(const float* logits, const int* input_len, int T, int N, int C, int blank, const int* lex_ids,
+                           const int* lex_off, int max_entry_len, const int* cand, int max_candidates, float* score, int* best,
+                           float* best_score, crnn_stream_t stream);
+
 /* Greedy decode.  Replaces tf.nn.ctc_*_decoder(merge_repeated=True) + sparse_tensor_to_dense
  * at lib/networks/network.py:656-657 and the zero stripping of lib/lstm/utils/training.py:32:
  * per frame argmax (lowest index on ties) for t < input_len; emit iff != tf_blank and != the

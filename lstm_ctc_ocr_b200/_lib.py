@@ -26,6 +26,10 @@ SIGNATURES = {
     "crnn_ctc_align_workspace_size": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
     "crnn_ctc_align": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "crnn_lexicon_candidates": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
+                                        c_void_p, c_void_p, c_void_p]),
+    "crnn_ctc_lexicon_score": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int,
+                                       c_void_p, c_void_p, c_void_p, c_void_p]),
     "crnn_ctc_greedy": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "crnn_ctc_beam_search": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int]),
     "crnn_ctc_beam_workspace_size": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),

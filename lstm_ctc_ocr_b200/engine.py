@@ -576,6 +576,132 @@ def alignment_dict(labels, start, end, peak, path_logprob):
                 peak=np.asarray(peak, np.float32), path_logprob=np.asarray(path_logprob, np.float32))
 
 
+LEXICON_MAX_ENTRY = 63
+
+
+class Lexicon(object):
+    """A device-resident word list for lexicon-based reading (crnn_lexicon_candidates / crnn_ctc_lexicon_score): CSR `ids` i32
+    (the entries' class ids concatenated) and `off` [K+1] i32 on `device`.  `entries` are id sequences over the charset's ids
+    [1, nclasses-2] (0 is the CTC blank, nclasses-1 the decoders' blank), 1 .. 63 ids each; anything else raises ValueError.
+    Exact duplicates are kept at their first occurrence only (`index_of` maps each kept entry back to its position in
+    `entries`), so a tie between two slots is a tie between different words."""
+
+    def __init__(self, entries, device="cuda", nclasses=64):
+        kept, seen, index_of = [], set(), []
+        for i, e in enumerate(entries):
+            e = tuple(int(v) for v in e)
+            if not e or len(e) > LEXICON_MAX_ENTRY:
+                raise ValueError(f"Lexicon: entry {i} has {len(e)} ids; entries hold 1 .. {LEXICON_MAX_ENTRY}")
+            bad = [v for v in e if not 1 <= v <= nclasses - 2]
+            if bad:
+                raise ValueError(f"Lexicon: entry {i} holds id {bad[0]} outside the charset's ids [1, {nclasses - 2}]")
+            if e not in seen:
+                seen.add(e)
+                kept.append(e)
+                index_of.append(i)
+        if not kept:
+            raise ValueError("Lexicon: no entries")
+        self.entries = kept
+        self.index_of = np.asarray(index_of, np.int64)
+        lens = np.array([len(e) for e in kept], np.int32)
+        off = np.zeros(len(kept) + 1, np.int32)
+        np.cumsum(lens, out=off[1:])
+        self.max_entry_len = int(lens.max())
+        self.ids = torch.tensor(np.fromiter((v for e in kept for v in e), np.int32, int(off[-1])), device=device)
+        self.off = torch.tensor(off, device=device)
+        self.lens = lens
+
+    def __len__(self):
+        return len(self.entries)
+
+    def padded(self, width=None):
+        """[K, width] i32 host array of the entries, zero-padded (width: the longest entry by default)."""
+        width = self.max_entry_len if width is None else int(width)
+        out = np.zeros((len(self.entries), width), np.int32)
+        for k, e in enumerate(self.entries):
+            out[k, :len(e)] = e
+        return out
+
+
+def _cuda_i32(name, *tensors):
+    if not all(torch.is_tensor(t) and t.is_cuda for t in tensors):
+        raise CrnnError(f"{name} needs CUDA tensors (sm_90a); there is no CPU fallback")
+    if any(t.dtype != torch.int32 for t in tensors):
+        raise CrnnError(f"{name}: index tensors must be i32")
+
+
+def lexicon_candidates(reads, read_len, lexicon, max_edit=3, max_candidates=64):
+    """The lexicon entries nearest each read by edit distance (crnn_lexicon_candidates): reads [N, M] i32 cuda in the decoders'
+    dense layout (dense_decoded), read_len [N] i32 cuda.  Returns device (cand, cand_dist) [N, max_candidates] i32 ordered by
+    (distance, lexicon index), -1 past the count, and cand_total [N] i32 (the entries within max_edit; max_edit < 0: no
+    threshold)."""
+    _cuda_i32("lexicon_candidates", reads, read_len)
+    if reads.dim() != 2 or read_len.numel() != reads.shape[0]:
+        raise CrnnError("lexicon_candidates: reads must be [N, M] and read_len [N]")
+    reads, read_len = reads.contiguous(), read_len.contiguous()
+    N, M = reads.shape
+    dev = reads.device
+    cand = torch.empty((N, max_candidates), dtype=torch.int32, device=dev)
+    dist = torch.empty((N, max_candidates), dtype=torch.int32, device=dev)
+    total = torch.empty(N, dtype=torch.int32, device=dev)
+    if N == 0:
+        return cand, dist, total
+    src = reads if reads.numel() else torch.zeros(1, dtype=torch.int32, device=dev)   # rows of width 0 still pass a pointer
+    check(_lib.load().crnn_lexicon_candidates(src.data_ptr(), M, read_len.data_ptr(), N, lexicon.ids.data_ptr(), lexicon.off.data_ptr(),
+                                              len(lexicon), lexicon.max_entry_len, int(max_edit), int(max_candidates), cand.data_ptr(),
+                                              dist.data_ptr(), total.data_ptr(), _stream()))
+    return cand, dist, total
+
+
+def ctc_lexicon_score(logits, input_len, lexicon, cand, blank=0):
+    """CTC scores of the candidates (crnn_ctc_lexicon_score): logits [T,N,64] f32 cuda, input_len [N] i32, cand [N, J] i32 as
+    lexicon_candidates returns it.  Returns device score [N, J] f32 (ln p(entry | line); -inf for empty slots and infeasible
+    entries, NaN for invalid ones), best [N] i32 (lexicon index of the highest finite score, lowest slot on ties, -1 if none) and
+    best_score [N] f32."""
+    _cuda_i32("ctc_lexicon_score", input_len, cand)
+    if not (torch.is_tensor(logits) and logits.is_cuda and logits.dtype == torch.float32 and logits.dim() == 3):
+        raise CrnnError("ctc_lexicon_score: logits must be a [T,N,64] f32 cuda tensor")
+    logits, input_len, cand = logits.contiguous(), input_len.contiguous(), cand.contiguous()
+    T, N, C = logits.shape
+    if input_len.numel() != N or cand.dim() != 2 or cand.shape[0] != N:
+        raise CrnnError("ctc_lexicon_score: input_len [N] and cand [N, J] must hold one entry / row per line")
+    dev = logits.device
+    J = cand.shape[1]
+    score = torch.empty((N, J), dtype=torch.float32, device=dev)
+    best = torch.empty(N, dtype=torch.int32, device=dev)
+    best_score = torch.empty(N, dtype=torch.float32, device=dev)
+    check(_lib.load().crnn_ctc_lexicon_score(logits.data_ptr(), input_len.data_ptr(), T, N, C, int(blank), lexicon.ids.data_ptr(),
+                                             lexicon.off.data_ptr(), lexicon.max_entry_len, cand.data_ptr(), J, score.data_ptr(),
+                                             best.data_ptr(), best_score.data_ptr(), _stream()))
+    return score, best, best_score
+
+
+def lexicon_decode(logits, input_len, reads, read_len, lexicon, max_edit=3, max_candidates=64):
+    """Lexicon-based reading of a batch: the candidates of each read within max_edit, scored by CTC (blank 0, the blank warp-ctc
+    trains), and the most probable one.  logits [T,N,64] f32, input_len [N], reads [N, M] and read_len [N] i32, all cuda.
+    Returns host arrays: labels [N, max(M, longest entry)] i32 (the chosen entry's ids zero-padded; the read itself when no
+    candidate has a finite score), index [N] (lexicon index, -1 when none), score [N] f32 (ln p of the chosen entry, -inf when
+    none), distance [N] (edit distance of the chosen entry, -1 when none), candidates [N] (entries within max_edit)."""
+    cand, dist, total = lexicon_candidates(reads, read_len, lexicon, max_edit, max_candidates)
+    _, best, best_score = ctc_lexicon_score(logits, input_len, lexicon, cand, blank=0)
+    cand, dist, total, best, best_score = (a.cpu().numpy() for a in (cand, dist, total, best, best_score))
+    rd, rl = reads.cpu().numpy(), read_len.cpu().numpy()
+    N = rd.shape[0]
+    labels = np.zeros((N, max(rd.shape[1], lexicon.max_entry_len)), np.int32)
+    distance = np.full(N, -1, np.int32)
+    for n in range(N):
+        k = int(best[n])
+        if k >= 0:
+            e = lexicon.entries[k]
+            labels[n, :len(e)] = e
+            distance[n] = dist[n][np.flatnonzero(cand[n] == k)[0]]
+        else:
+            L = min(max(int(rl[n]), 0), rd.shape[1])
+            labels[n, :L] = rd[n, :L]
+    return dict(labels=labels, index=best.astype(np.int32), score=best_score.astype(np.float32), distance=distance,
+                candidates=total.astype(np.int32))
+
+
 def ctc_greedy(logits, input_len, tf_blank=TF_BLANK, strip=0):
     """Returns (out [N,T] i32 zero padded, out_len [N] i32) on device."""
     lib = _lib.load()

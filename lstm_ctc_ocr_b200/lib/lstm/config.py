@@ -61,7 +61,11 @@ _DEFAULTS = {
              "BN_STATS": "batch",
              # not in the reference: True adds to each file's line of test_model the read's confidence exp(path_logprob) (the
              # probability of its best CTC alignment) and each character's peak posterior (Session.run's "read_alignment")
-             "CONFIDENCE": False},
+             "CONFIDENCE": False,
+             # not in the reference (CRNN's lexicon-based transcription): a word-list file (one word per line) makes test_model read
+             # each line as the most probable word (CTC score) among the LEXICON_CANDIDATES nearest words within edit distance
+             # LEXICON_MAX_EDIT of the plain read (CRNN's delta = 3; < 0: no threshold); "" reads without a lexicon
+             "LEXICON": "", "LEXICON_MAX_EDIT": 3, "LEXICON_CANDIDATES": 64},
 }
 
 

@@ -100,6 +100,9 @@ class SolverWrapper(object):
         confidence = bool(cfg.TEST.get("CONFIDENCE", False))
         if confidence:      # the alignment's labels are dense_decoded's
             dense_decoded = Fetch(self.net, "read_alignment")
+        lexicon = bool(cfg.TEST.get("LEXICON", ""))
+        if lexicon:         # the lexicon read of each line next to its plain read
+            dense_decoded = [dense_decoded, Fetch(self.net, "lexicon_decoded")]
         if restore:
             from .train import SolverWrapper as TrainSolver
             ts = TrainSolver.__new__(TrainSolver)
@@ -127,14 +130,20 @@ class SolverWrapper(object):
             feed_dict = {(self.net.data_u8 if dtype == np.uint8 else self.net.data): data, self.net.line_width: lw, self.net.time_step_len: tsl, self.net.keep_prob: 1.0}
             dense = sess.run(fetches=dense_decoded, feed_dict=feed_dict)
             dt = timer.toc(average=False) / len(idx)
+            if lexicon:
+                dense, lex = dense
             if confidence:
                 al, dense = dense, dense["labels"]
             for r, i in enumerate(idx):
                 res_of[i] = "".join(decodeRes(dense[r]))
                 time_of[i] = dt
+                if lexicon:
+                    plain, res_of[i] = res_of[i], "".join(decodeRes(lex["labels"][r]))
+                    if plain != res_of[i]:
+                        conf_of[i] = ", read: {}".format(plain)
                 if confidence:
                     k = int((dense[r] != 0).sum())
-                    conf_of[i] = ", conf: {:.4f}, peaks: [{}]".format(float(np.exp(np.float64(al["path_logprob"][r]))),
+                    conf_of[i] = conf_of.get(i, "") + ", conf: {:.4f}, peaks: [{}]".format(float(np.exp(np.float64(al["path_logprob"][r]))),
                                                                      " ".join("{:.3f}".format(float(p)) for p in al["peak"][r, :k]))
         total = correct = 0
         for i, file in enumerate(files):

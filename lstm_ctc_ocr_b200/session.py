@@ -442,6 +442,8 @@ class Session(object):
                 v = self._read_alignment(logits, d_tsl)
             elif k == "label_alignment":
                 v = self._label_alignment(logits, d_tsl, d_lab, d_ll, llen)
+            elif k == "lexicon_decoded":
+                v = self._lexicon_decoded(logits, d_tsl)
             elif k == "train_op":
                 v = f.step_fn(eng, logits, grad, d_data, d_tsl)
                 self._stage_ahead()
@@ -507,6 +509,8 @@ class Session(object):
                 v = self._read_alignment(logits, d_tsl)
             elif k == "label_alignment":
                 v = self._label_alignment(logits, d_tsl, d_ints["labels"], d_ints["llen"], llen)
+            elif k == "lexicon_decoded":
+                v = self._lexicon_decoded(logits, d_tsl)
             elif k.startswith("layer:"):
                 name = k.split(":", 1)[1]
                 tapname = {"pool1": "conv1", "pool2": "conv3_2", "pool3": "conv4_2", "reshaped_layer": "conv5"}.get(name, name)
@@ -542,6 +546,23 @@ class Session(object):
         dense = engine.dense_decoded(o, ol)
         r = engine.ctc_align(logits, dense, ol, d_tsl, blank=0, max_label_len=dense.shape[1])
         return engine.alignment_dict(dense.cpu().numpy(), *(a.cpu().numpy() for a in r))
+
+    def _lexicon_decoded(self, logits, d_tsl):
+        """"lexicon_decoded": each line read against cfg.TEST.LEXICON (engine.lexicon_decode, blank 0) from the read dense_decoded
+        returns (cfg.DECODER applies).  The word list is loaded once per path and device and stays on the device."""
+        from .lib.lstm.config import cfg
+        path = str(cfg.TEST.get("LEXICON", ""))
+        if not path:
+            raise ValueError('the "lexicon_decoded" fetch needs cfg.TEST.LEXICON (a word-list file)')
+        cache = self.__dict__.setdefault("_lexicons", {})
+        key = (path, str(logits.device))
+        if key not in cache:
+            from .lib.lstm.lexicon import load_lexicon
+            cache[key] = engine.Lexicon(load_lexicon(path), device=logits.device)
+        o, ol = Session._decode_device(logits, d_tsl)
+        return engine.lexicon_decode(logits, d_tsl, engine.dense_decoded(o, ol), ol, cache[key],
+                                     max_edit=int(cfg.TEST.get("LEXICON_MAX_EDIT", 3)),
+                                     max_candidates=int(cfg.TEST.get("LEXICON_CANDIDATES", 64)))
 
     @staticmethod
     def _label_alignment(logits, d_tsl, d_lab, d_ll, llen):

@@ -9,6 +9,11 @@
  * workspace (size queried first), every call asynchronous on the caller's stream, no
  * hidden host synchronisation.  All pointers are DEVICE pointers unless marked host.
  * One host thread per handle (thread-compatible, not thread-safe).
+ * These calls can be captured into a CUDA graph once the same call has run at the same shape, on a single-device model:
+ * crnn_forward / _u8, crnn_forward_lines, crnn_forward_host (every compute_dtype; copy_stream joins the capture through the
+ * events of its copy handshake), crnn_forward + crnn_backward in training mode, the three crnn_clip_*_step solvers (the step
+ * number is baked into the graph), crnn_ctc_loss (shared-memory and workspace kernels), crnn_ctc_greedy, crnn_ctc_align,
+ * crnn_lexicon_candidates and crnn_ctc_lexicon_score.
  */
 #ifndef CRNN_CTC_H_
 #define CRNN_CTC_H_
@@ -207,6 +212,8 @@ typedef struct crnn_config {
                          *     crnn_model_calibrate_fp8 or crnn_model_set_fp8_scales provides (see below) */
 } crnn_config;
 
+/* Not on the hot path: an fp8 model's creation synchronises the device after zeroing its e4m3 weight and scale block, so that
+ * work on any stream afterwards (a non-blocking one included) sees the block zeroed before it writes it. */
 int     crnn_model_create(const crnn_config* cfg, crnn_model** out);
 int     crnn_model_destroy(crnn_model* m);
 
@@ -239,7 +246,9 @@ int     crnn_forward(crnn_model* m, const float* data, const int* time_step_len,
  * tensor `data_staging` [N,W,32] while the batch-independent front end (conv1 .. conv3_2) of the previous range runs on
  * `stream`; from the first batch-statistics BatchNorm on the batch is processed whole.  chunks <= 1 (or a batch that does not
  * split on tile boundaries) degenerates to copy-then-compute.  `data_staging` holds the whole batch on return order of
- * `stream` (crnn_backward reads it). */
+ * `stream` (crnn_backward reads it).  Whatever the compute_dtype, every copy out of `host_data` runs on `copy_stream`
+ * (after the work queued earlier on `stream`): the caller may rewrite `host_data` once the work queued on `copy_stream`
+ * has completed. */
 int     crnn_forward_host(crnn_model* m, const float* host_data, float* data_staging, const int* time_step_len,
                           int N, int W, float* logits_out, void* workspace, size_t workspace_bytes, int chunks,
                           crnn_stream_t stream, crnn_stream_t copy_stream);
@@ -248,7 +257,8 @@ int     crnn_forward_host(crnn_model* m, const float* host_data, float* data_sta
  * iteration (lib/lstm/train.py:119-125).  Every image range is first moved into the caller's page-locked `pinned_staging`
  * [N,W,32] by `host_threads` host threads (a persistent pool inside the library), then DMA'd and processed as in
  * crnn_forward_host; the host moves range c+1 while the GPU copies / computes range c.  The caller must not touch
- * `pinned_staging` until the copies issued on `copy_stream` have completed. */
+ * `pinned_staging` until the copies issued on `copy_stream` have completed; whatever the compute_dtype, every copy out of it
+ * runs there, so `pinned_staging` may be reused once the work queued on `copy_stream` has completed. */
 int     crnn_forward_pageable(crnn_model* m, const float* pageable_data, float* pinned_staging, float* data_staging,
                               const int* time_step_len, int N, int W, float* logits_out, void* workspace,
                               size_t workspace_bytes, int chunks, int host_threads, crnn_stream_t stream,
@@ -277,8 +287,9 @@ int     crnn_forward_lines(crnn_model* m, const float* data, const int* line_wid
  * asynchronous, no host sync, no allocation (an fp8 model allocates its e4m3 weights and scales in crnn_model_create),
  * deterministic.  Any parameter change (crnn_model_bind, crnn_model_params_changed)
  * invalidates the scales; an fp8 forward without valid scales returns CRNN_INVALID_VALUE ("calibration is missing") and leaves
- * its outputs untouched.  get (syncs the device) and set (host arrays of 5 floats; set refuses anything but powers of two in
- * [2^-126, 2^127] with CRNN_INVALID_VALUE) restate them.  On a model of another compute_dtype all three return CRNN_UNSUPPORTED.
+ * its outputs untouched.  get and set (host arrays of 5 floats; set refuses anything but powers of two in [2^-126, 2^127] with
+ * CRNN_INVALID_VALUE) restate them; both synchronise the device, set before and after its write, so that a forward on any
+ * stream afterwards reads the new scales.  On a model of another compute_dtype all three return CRNN_UNSUPPORTED.
  * crnn_forward, _host and _pageable (copy, then compute) and crnn_forward_lines run the fp8 path on an fp8 model;
  * crnn_model_set_training(m, 1) and a training workspace return CRNN_UNSUPPORTED. */
 int     crnn_model_calibrate_fp8(crnn_model* m, const float* data, const int* time_step_len, int N, int W, void* workspace,
@@ -406,7 +417,9 @@ int     crnn_model_set_grad_ready_callback(crnn_model* m, crnn_grad_ready_fn fn,
  * kernels the caller launches from the grad-ready callback find free SMs instead of delaying the tail of a full-GPU grid. */
 int     crnn_model_set_backward_sm_reserve(crnn_model* m, int sms);
 /* Peer-memory inboxes (cudaMalloc + CUDA IPC): create one per rank, exchange the 64-byte handles through the host language
- * (e.g. torch.distributed.all_gather_object), open the peers', hand all `world` pointers (own at [rank]) to the model. */
+ * (e.g. torch.distributed.all_gather_object), open the peers', hand all `world` pointers (own at [rank]) to the model.
+ * crnn_peer_inbox_create and crnn_model_set_peers synchronise the device after writing device memory (the zeroed inbox, the
+ * peer table), so that exchanges on any stream afterwards read what they wrote.  Neither is on the hot path. */
 size_t  crnn_peer_inbox_bytes(void);
 int     crnn_peer_inbox_create(void** dev_ptr, unsigned char handle[64]);
 int     crnn_peer_inbox_open(const unsigned char handle[64], void** dev_ptr);

@@ -178,7 +178,11 @@ static int create_state(crnn_model* m) {
     for (int l = 0; l < kLayers; ++l) tot += align_up((size_t)kL[l].K * kL[l].Cout);
     tot += 4 * align_up(kLayers * 512 * 4) + 1024;
     if (cudaMalloc(&s->block, tot) != cudaSuccess) { delete s; return crnn_fail(CRNN_CUDA_ERROR, "fp8: cudaMalloc"); }
-    if (cudaMemset(s->block, 0, tot) != cudaSuccess) { cudaFree(s->block); delete s; return crnn_fail(CRNN_CUDA_ERROR, "fp8: cudaMemset"); }
+    // cudaMemset is ordered on the legacy stream only: wait for it, or a busy legacy stream lets it land after the first forward
+    // or calibration on a non-blocking stream has written this block
+    if (cudaMemset(s->block, 0, tot) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) {
+      cudaFree(s->block); delete s; return crnn_fail(CRNN_CUDA_ERROR, "fp8: cudaMemset");
+    }
     uint8_t* p = reinterpret_cast<uint8_t*>(s->block);
     for (int l = 0; l < kLayers; ++l) { s->Wq[l] = p; p += align_up((size_t)kL[l].K * kL[l].Cout); }
     s->wscale = reinterpret_cast<float*>(p); p += align_up(kLayers * 512 * 4);
@@ -378,6 +382,8 @@ int fp8_set_scales(crnn_model* m, const float* host) {
   State* s = reinterpret_cast<State*>(m->fp8);
   CUDA_TRY(cudaDeviceSynchronize());     // a calibration still queued on some stream must not overwrite these afterwards
   CUDA_TRY(cudaMemcpy(s->scales, host, fp8::kLayers * sizeof(float), cudaMemcpyHostToDevice));
+  // a copy from pageable memory may return before its DMA lands, and the next forward may run on a non-blocking stream
+  CUDA_TRY(cudaDeviceSynchronize());
   s->calibrated = true;
   s->colscale_dirty = true;
   return CRNN_OK;

@@ -562,6 +562,31 @@ class CopyPool {
 };
 }  // namespace
 
+// The events of the host-fed forwards' copy handshake, created on first use: [c] = image range c copied (recorded on the copy
+// stream), [kMaxChunks] = the work queued on the compute stream before the copies (it may still read the staging tensor).
+static int ensure_chunk_events(crnn_model* m) {
+  if (m->chunk_events.empty()) {
+    m->chunk_events.resize(kMaxChunks + 1);
+    for (auto& e : m->chunk_events) CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  }
+  return CRNN_OK;
+}
+
+// Copy-then-compute from host memory (the fp8 and f32-class paths): the whole batch goes to `data` on `copy_st`, after the work
+// queued earlier on `st` and before anything `st` runs next -- the bf16 path's handshake with one range.  So on every path the
+// host buffers may be reused once the work queued on `copy_st` has completed, and a graph captured on `st` takes the copy in.
+static int host_copy_whole(crnn_model* m, void* data, void* host_data, const void* pageable_src, size_t bytes, int host_threads,
+                           cudaStream_t st, cudaStream_t copy_st) {
+  CRNN_TRY(ensure_chunk_events(m));
+  CUDA_TRY(cudaEventRecord(m->chunk_events[kMaxChunks], st));
+  CUDA_TRY(cudaStreamWaitEvent(copy_st, m->chunk_events[kMaxChunks], 0));
+  if (pageable_src != nullptr) CopyPool::get().copy(host_data, pageable_src, bytes, host_threads);
+  CUDA_TRY(cudaMemcpyAsync(data, host_data, bytes, cudaMemcpyHostToDevice, copy_st));
+  CUDA_TRY(cudaEventRecord(m->chunk_events[0], copy_st));
+  CUDA_TRY(cudaStreamWaitEvent(st, m->chunk_events[0], 0));
+  return CRNN_OK;
+}
+
 // Forward pass.  `host_data` != nullptr (crnn_forward_host): the batch is still in page-locked HOST memory; it is cut into
 // `chunks` image ranges whose H2D copies run on `copy_st` while the batch-independent front end (conv1 .. conv3_2 + pools) of
 // the previous range runs on `st` -- the copy (33.6 MB at batch 1024 x 32x256) hides behind that compute instead of preceding it.  From conv4_1 on (batch-statistics BatchNorm) the batch is processed whole.
@@ -600,8 +625,7 @@ static int forward_impl(crnn_model* m, const void* data, const void* host_data, 
     if (m->dp_world > 1) return crnn_fail(CRNN_UNSUPPORTED, "forward: the fp8 path runs on one device (no data parallelism)");
     if (host_data != nullptr) {
       // copy-then-compute, as the f32-class paths do
-      if (pageable_src != nullptr) CopyPool::get().copy(at(host_data, 0), pageable_src, (size_t)N * W * 32 * es, host_threads);
-      CUDA_TRY(cudaMemcpyAsync(at(data, 0), host_data, (size_t)N * W * 32 * es, cudaMemcpyHostToDevice, st));
+      CRNN_TRY(host_copy_whole(m, at(data, 0), at(host_data, 0), pageable_src, (size_t)N * W * 32 * es, host_threads, st, copy_st));
       host_data = nullptr;
       pageable_src = nullptr;
     }
@@ -609,10 +633,8 @@ static int forward_impl(crnn_model* m, const void* data, const void* host_data, 
   }
   if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3) {
     // f32-class paths (forward_x3.cu): copy-then-compute when fed from host memory
-    if (host_data != nullptr) {
-      if (pageable_src != nullptr) CopyPool::get().copy(at(host_data, 0), pageable_src, (size_t)N * W * 32 * es, host_threads);
-      CUDA_TRY(cudaMemcpyAsync(at(data, 0), host_data, (size_t)N * W * 32 * es, cudaMemcpyHostToDevice, st));
-    }
+    if (host_data != nullptr)
+      CRNN_TRY(host_copy_whole(m, at(data, 0), at(host_data, 0), pageable_src, (size_t)N * W * 32 * es, host_threads, st, copy_st));
     return x3_forward(m, data, u8, time_step_len, N, W, logits_out, workspace, workspace_bytes, st);
   }
   if (m->dirty) CRNN_TRY(prepare_weights(m, st));
@@ -651,10 +673,7 @@ static int forward_impl(crnn_model* m, const void* data, const void* host_data, 
   // a range must start on a tile-PAIR boundary of every layer (128-position tiles = 4 sub-boxes, pairs = 8)
   if (chunks > 1 && ((nc * sb3) % 8 != 0 || (nc * sb2) % 8 != 0)) { chunks = 1; nc = N; }
   if (host_data != nullptr) {
-    if (m->chunk_events.empty()) {
-      m->chunk_events.resize(kMaxChunks + 1);
-      for (auto& e : m->chunk_events) CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    }
+    CRNN_TRY(ensure_chunk_events(m));
     // the staging tensor may still be read by work queued earlier on `st` (previous forward / backward)
     CUDA_TRY(cudaEventRecord(m->chunk_events[kMaxChunks], st));
     CUDA_TRY(cudaStreamWaitEvent(copy_st, m->chunk_events[kMaxChunks], 0));

@@ -105,6 +105,7 @@ extern "C" int crnn_peer_inbox_create(void** dev_ptr, unsigned char handle[64]) 
   void* p = nullptr;
   CUDA_TRY(cudaMalloc(&p, sizeof(Inbox)));
   CUDA_TRY(cudaMemset(p, 0, sizeof(Inbox)));
+  CUDA_TRY(cudaDeviceSynchronize());     // the memset is ordered on the legacy stream only: done before any stream's exchange
   cudaIpcMemHandle_t h;
   cudaError_t e = cudaIpcGetMemHandle(&h, p);
   if (e != cudaSuccess) { cudaFree(p); return crnn_fail(CRNN_CUDA_ERROR, "cudaIpcGetMemHandle: %s", cudaGetErrorString(e)); }
@@ -155,6 +156,8 @@ extern "C" int crnn_model_set_peers(crnn_model* m, int rank, int world, void* co
   CUDA_TRY(cudaMalloc(&m->d_peers, sizeof(void*) * MAX_WORLD + sizeof(int)));
   CUDA_TRY(cudaMemset(m->d_peers, 0, sizeof(void*) * MAX_WORLD + sizeof(int)));
   CUDA_TRY(cudaMemcpy(m->d_peers, inbox_ptrs_host, sizeof(void*) * world, cudaMemcpyHostToDevice));
+  // a copy from pageable memory may return before its DMA lands, and the next exchange may run on a non-blocking stream
+  CUDA_TRY(cudaDeviceSynchronize());
   m->d_peer_err = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(m->d_peers) + sizeof(void*) * MAX_WORLD);
   m->dp_rank = rank; m->dp_world = world;
   m->peer_epoch = 0;

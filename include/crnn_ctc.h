@@ -154,6 +154,27 @@ int crnn_ctc_lexicon_score(const float* logits, const int* input_len, int T, int
                            const int* lex_off, int max_entry_len, const int* cand, int max_candidates, float* score, int* best,
                            float* best_score, crnn_stream_t stream);
 
+/* Resize native-size 8-bit gray text lines to the network's 32 rows and pack them into the batch crnn_forward_lines_u8 takes.
+ * Replaces the host step of lib/lstm/test.py (Image.resize((nw, 32), BILINEAR) per line, then pad and transpose): the result
+ * is byte for byte Pillow's 8-bit BILINEAR on mode "L" -- the horizontal pass (src_w -> out_w) first, then the vertical pass
+ * (src_h -> 32) on its u8 result, each skipped when its size is unchanged, integer taps of 22 fractional bits; a source more
+ * than 100 times taller than wide takes the vertical pass first, as Pillow (12.2) does.
+ *   src         u8; line i is src_h[i] x src_w[i] bytes, row-major, at src + src_offset[i] (any alignment)
+ *   src_offset  [N] i64;  src_h, src_w, out_w [N] i32
+ *   out         [N, W, 32] u8, 4-byte aligned: out[i, x, y] = resized line i at row y, column x for x < out_w[i]; every column
+ *               from out_w[i] to W is written as zero, so `out` needs no clearing.
+ * max_h is a host-side bound on every src_h[i] and sizes the launch: at most 1024 (CRNN_INVALID_VALUE outside [1, 1024]).
+ * The per-line values are preconditions the call cannot check without a host sync: 1 <= src_h[i] <= max_h, src_w[i] >= 1,
+ * 1 <= out_w[i] <= W, src_w[i] / out_w[i] <= max_h / 16 + 1 (the size rule below keeps it under src_h[i] / 16), and the bytes
+ * of line i inside `src`.  A line whose height, widths or ratio break them gets an all-zero slot and is not read.
+ * The size rule of the evaluation path (lib/lstm/test.py line_size): out_w = src_w if src_h == 32 else
+ * max(1, (int)(32.0 / src_h * src_w)) in double arithmetic, computed on the host; the line's padded width is
+ * max(8, ceil(out_w / 4) * 4) and its time_step_len max(out_w / 4 - 1, 0).
+ * CRNN_INVALID_VALUE for a null pointer, N <= 0, W < 8, W % 4 != 0 or a misaligned `out`; CRNN_UNSUPPORTED for W above
+ * 2 097 120.  Every pointer is a device pointer; asynchronous on `stream`, no allocation, the same bits on every run. */
+int crnn_resize_lines_u8(const uint8_t* src, const int64_t* src_offset, const int* src_h, const int* src_w, const int* out_w, int N,
+                         int W, int max_h, uint8_t* out, crnn_stream_t stream);
+
 /* Greedy decode.  Replaces tf.nn.ctc_*_decoder(merge_repeated=True) + sparse_tensor_to_dense
  * at lib/networks/network.py:656-657 and the zero stripping of lib/lstm/utils/training.py:32:
  * per frame argmax (lowest index on ties) for t < input_len; emit iff != tf_blank and != the

@@ -702,6 +702,35 @@ def lexicon_decode(logits, input_len, reads, read_len, lexicon, max_edit=3, max_
                 candidates=total.astype(np.int32))
 
 
+RESIZE_MAX_HEIGHT = 1024      # the tallest source line crnn_resize_lines_u8 takes
+
+
+def resize_lines_u8(src, src_offset, src_h, src_w, out_w, W, max_h, out=None):
+    """Native-size 8-bit gray lines -> the packed [N, W, 32] uint8 batch of forward_lines (crnn_resize_lines_u8): line i is
+    src_h[i] x src_w[i] bytes, row-major, at src[src_offset[i]:], resized to 32 rows and out_w[i] columns with Pillow's 8-bit
+    BILINEAR, byte for byte, and written width-major into slot i; columns out_w[i] .. W-1 are zero.  src uint8, src_offset [N]
+    int64, src_h / src_w / out_w [N] int32, all cuda; max_h (host int) bounds every src_h[i], at most RESIZE_MAX_HEIGHT.  The
+    per-line values are preconditions (include/crnn_ctc.h); out_w and W come from lib.lstm.test.line_size.  out: a contiguous
+    [N, W, 32] uint8 cuda tensor, or None to allocate one.  No host fallback: CPU tensors raise CrnnError."""
+    idx = (src_h, src_w, out_w)
+    if not all(torch.is_tensor(t) and t.is_cuda for t in (src, src_offset) + idx):
+        raise CrnnError("resize_lines_u8 needs CUDA tensors (sm_90a); there is no CPU fallback")
+    if src.dtype != torch.uint8 or src_offset.dtype != torch.int64 or any(t.dtype != torch.int32 for t in idx):
+        raise CrnnError("resize_lines_u8: src must be uint8, src_offset int64 and src_h, src_w, out_w int32")
+    N = src_h.numel()
+    if src_offset.numel() != N or src_w.numel() != N or out_w.numel() != N:
+        raise CrnnError("resize_lines_u8: src_offset, src_h, src_w and out_w must hold one entry per line")
+    src, src_offset, src_h, src_w, out_w = (t.contiguous() for t in (src, src_offset, src_h, src_w, out_w))
+    if out is None:
+        out = torch.empty((N, int(W), 32), dtype=torch.uint8, device=src.device)
+    elif not (torch.is_tensor(out) and out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous()
+              and tuple(out.shape) == (N, int(W), 32)):
+        raise CrnnError(f"resize_lines_u8: out must be a contiguous [{N}, {int(W)}, 32] uint8 cuda tensor")
+    check(_lib.load().crnn_resize_lines_u8(src.data_ptr(), src_offset.data_ptr(), src_h.data_ptr(), src_w.data_ptr(), out_w.data_ptr(),
+                                           N, int(W), int(max_h), out.data_ptr(), _stream()))
+    return out
+
+
 def ctc_greedy(logits, input_len, tf_blank=TF_BLANK, strip=0):
     """Returns (out [N,T] i32 zero padded, out_len [N] i32) on device."""
     lib = _lib.load()

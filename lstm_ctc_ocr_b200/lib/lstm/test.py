@@ -6,10 +6,12 @@ Per file (test.py:57-88): read as gray, right-pad the width to a multiple of POO
 Deviation from the reference, per SURVEY §3.4: ``time_step_len`` is fed as W//4 - 1 (the data layer's convention,
 gen.py:54), not the off-by-one W//4 of test.py:74 which exceeds the number of conv frames.
 
-Lines are evaluated in packed batches of ``cfg.TEST.BATCH_SIZE`` (``pack_lines`` + the ``line_width`` feed): every line is still
-computed as if it were run alone, as the reference runs it -- its own BatchNorm statistics, zero padding at its own right edge --
-so the decodes are those of one line per run.  Files are grouped by width to cut padding; the report keeps the reference's
-order (sorted names) and charges each file its batch's time divided by the batch's lines."""
+Lines are evaluated in packed batches of ``cfg.TEST.BATCH_SIZE`` (the ``images`` feed: each batch's lines travel at their native
+size and crnn_resize_lines_u8 resizes and packs them on the device, byte for byte what ``prepare_line`` + ``pack_lines`` build on
+the host): every line is still computed as if it were run alone, as the reference runs it -- its own BatchNorm statistics, zero
+padding at its own right edge -- so the decodes are those of one line per run.  Files are grouped by padded width to cut padding;
+the report keeps the reference's order (sorted names) and charges each file its batch's time (the resize included) divided by the
+batch's lines.  ``cfg.FEED_DTYPE`` does not apply: the lines are fed as 8-bit pixels, which give the f32 feed's bits."""
 import math
 import os
 
@@ -17,7 +19,6 @@ import numpy as np
 
 from ...session import Session
 from .config import cfg, get_encode_decode_dict
-from .utils.gen import feed_dtype
 from .utils.timer import Timer
 
 
@@ -34,15 +35,26 @@ def load_line_image(path):
     return np.asarray(Image.open(path).convert("L"), dtype=np.uint8)
 
 
+def line_size(h, w):
+    """The size rule of an evaluation line h rows x w columns: (nw, line_width, time_step_len) -- nw its width once resized to
+    cfg.IMG_HEIGHT rows (the reference's int(32 / h * w) in Python's double arithmetic, at least 1; w itself when h is already 32),
+    line_width its padded width (nw rounded up to a multiple of POOL_SCALE, at least 8) and time_step_len its conv frames
+    (nw // 4 - 1, at least 0).  prepare_line and the `images` feed (crnn_resize_lines_u8) both take their sizes from here."""
+    h, w = int(h), int(w)
+    nw = w if h == cfg.IMG_HEIGHT else max(1, int(cfg.IMG_HEIGHT / h * w))
+    width = max(8, int(math.ceil(nw / cfg.POOL_SCALE) * cfg.POOL_SCALE))
+    return nw, width, max(nw // cfg.POOL_SCALE + cfg.OFFSET_TIME_STEP, 0)
+
+
 def prepare_line(img, dtype=np.float32):
-    """[H=32, W] uint8 -> ([1, Wpad, 32] f32, time_step_len) exactly as test.py:65-70 lays the tensor out.  ``dtype=np.uint8``:
-    the same tensor as the 8-bit pixels, without the division (its f32 quotient by 255 is the f32 tensor bit for bit)."""
+    """[H, W] uint8 -> ([1, Wpad, 32] f32, time_step_len) exactly as test.py:65-70 lays the tensor out, after Pillow's BILINEAR
+    resize to 32 rows when H is not 32 (sizes from line_size).  ``dtype=np.uint8``: the same tensor as the 8-bit pixels, without
+    the division (its f32 quotient by 255 is the f32 tensor bit for bit)."""
+    nw, width, tsl = line_size(img.shape[0], img.shape[1])
     if img.shape[0] != cfg.IMG_HEIGHT:
         from PIL import Image
-        nw = max(1, int(cfg.IMG_HEIGHT / img.shape[0] * img.shape[1]))
         img = np.asarray(Image.fromarray(img).resize((nw, cfg.IMG_HEIGHT), Image.BILINEAR), dtype=np.uint8)
     w = img.shape[1]
-    width = max(8, int(math.ceil(w / cfg.POOL_SCALE) * cfg.POOL_SCALE))
     if np.dtype(dtype) == np.uint8:
         pad = np.zeros((cfg.IMG_HEIGHT, width), np.uint8)
         pad[:, :w] = img
@@ -50,7 +62,7 @@ def prepare_line(img, dtype=np.float32):
         pad = np.zeros((cfg.IMG_HEIGHT, width), np.float32)
         pad[:, :w] = img.astype(np.float32) / 255.0
     data = np.ascontiguousarray(pad.swapaxes(0, 1)).reshape(1, width, cfg.NUM_FEATURES)
-    return data, np.array([max(w // cfg.POOL_SCALE + cfg.OFFSET_TIME_STEP, 0)], np.int32)
+    return data, np.array([tsl], np.int32)
 
 
 def pack_lines(lines):
@@ -116,18 +128,18 @@ class SolverWrapper(object):
             except Exception:
                 raise Exception("Check your pretrained {:s}".format(str(path)))
         files = sorted(os.listdir(testDir))
-        dtype = feed_dtype(cfg.FEED_DTYPE)       # "uint8": lines stay 8-bit pixels and are fed through data_u8
-        lines = [prepare_line(load_line_image(os.path.join(testDir, f)), dtype=dtype) for f in files]
-        # batches of lines of similar width (stable sort: ties keep name order), so little of a batch is padding
-        order = sorted(range(len(files)), key=lambda i: lines[i][0].shape[1])
+        # each line goes to the device at its native size and is resized there (the `images` feed), whatever cfg.FEED_DTYPE says
+        images = [load_line_image(os.path.join(testDir, f)) for f in files]
+        # batches of lines of similar padded width (stable sort: ties keep name order), so little of a batch is padding
+        widths = [line_size(im.shape[0], im.shape[1])[1] for im in images]
+        order = sorted(range(len(files)), key=lambda i: widths[i])
         bs = max(1, int(cfg.TEST.BATCH_SIZE))
         timer = Timer()
         res_of, time_of, conf_of = {}, {}, {}
         for b0 in range(0, len(order), bs):
             idx = order[b0:b0 + bs]
             timer.tic()
-            data, lw, tsl = pack_lines([lines[i] for i in idx])
-            feed_dict = {(self.net.data_u8 if dtype == np.uint8 else self.net.data): data, self.net.line_width: lw, self.net.time_step_len: tsl, self.net.keep_prob: 1.0}
+            feed_dict = {self.net.images: [images[i] for i in idx], self.net.keep_prob: 1.0}
             dense = sess.run(fetches=dense_decoded, feed_dict=feed_dict)
             dt = timer.toc(average=False) / len(idx)
             if lexicon:

@@ -123,6 +123,18 @@ class Network(object):
             ph = self.__dict__["_data_u8"] = Placeholder("data_u8", "uint8", [None, None, cfg.NUM_FEATURES])
         return ph
 
+    @property
+    def images(self):
+        """Optional placeholder, not in the reference: a batch of text lines at their native size, a sequence of 2-D uint8 gray
+        arrays (H_i x W_i, 1 <= H_i <= 1024).  Each line travels to the device as it is and is resized there to 32 rows with
+        Pillow's BILINEAR, byte for byte (crnn_resize_lines_u8), then evaluated packed as with `line_width`: the batch, widths and
+        time_step_len that prepare_line + pack_lines would build on the host.  Evaluation fetches only; feed it instead of data,
+        data_u8, line_width and time_step_len.  Shared by every network built on this class."""
+        ph = self.__dict__.get("_images")
+        if ph is None:
+            ph = self.__dict__["_images"] = Placeholder("images", "uint8", [None, None])
+        return ph
+
     def get_output(self, layer):
         try:
             return self.layers[layer]

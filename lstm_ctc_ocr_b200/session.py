@@ -359,13 +359,20 @@ class Session(object):
         kinds = [f.kind for f in flist]
         need_loss = any(k in LOSS_KINDS for k in kinds)
         need_labels = need_loss or "label_alignment" in kinds
-        data = self._data_feed(feeds)
-        tsl = np.asarray(feeds["time_step_len"], dtype=np.int32)
+        if "images" in feeds:
+            clash = [k for k in ("data", "data_u8", "line_width", "time_step_len") if k in feeds]
+            if clash:
+                raise ValueError(f"images carries the lines, their widths and time_step_len: do not feed it with {', '.join(clash)}")
+            images = self._images_feed(feeds["images"])
+        data = self._data_feed(feeds) if "images" not in feeds else None
+        tsl = np.asarray(feeds["time_step_len"], dtype=np.int32) if "images" not in feeds else None
         labels = np.asarray(feeds["labels"], dtype=np.int32) if need_labels else None
         llen = np.asarray(feeds["labels_len"], dtype=np.int32) if need_labels else None
         eng = self.engine_for(net)
         if eng.compute_dtype == 4 and not eng.fp8_calibrated:
             self._calibrate_fp8(eng)        # parameters loaded straight into the engine (not through assign / a restore)
+        if "images" in feeds:
+            return self._run_images(flist, single, eng, images, labels, llen)
         dev = self.device
         if feeds.get("line_width") is not None:
             return self._run_lines(flist, single, net, eng, data, tsl, labels, llen, np.asarray(feeds["line_width"], dtype=np.int32))
@@ -468,29 +475,91 @@ class Session(object):
         self._pinned.wait_pending()
         return out[0] if single else out
 
+    @staticmethod
+    def _check_lines(kinds, eng, what):
+        if "train_op" in kinds:
+            raise ValueError(f"{what} (packed evaluation) cannot be fed with train_op: training uses whole-batch statistics")
+        if eng.training:
+            raise ValueError(f"{what} (packed evaluation) needs a model that has not been switched to training")
+
     def _run_lines(self, flist, single, net, eng, data, tsl, labels, llen, line_width):
         """Packed evaluation (``line_width`` fed): the batch is staged to the device and every line is evaluated as if it were run
         alone (engine.CrnnModel.forward_lines).  Evaluation fetches only."""
-        kinds = [f.kind for f in flist]
-        if "train_op" in kinds:
-            raise ValueError("line_width (packed evaluation) cannot be fed with train_op: training uses whole-batch statistics")
-        if eng.training:
-            raise ValueError("line_width (packed evaluation) needs a model that has not been switched to training")
+        self._check_lines([f.kind for f in flist], eng, "line_width")
         data = np.ascontiguousarray(data)
         self.validate_feed(data, tsl, labels, llen, line_width)
         ints = {"tsl": tsl, "lw": line_width}
         if labels is not None:
             ints["labels"], ints["llen"] = labels, llen
         d_ints = self._pinned.stage_ints(ints, self.device)
-        d_tsl = d_ints["tsl"]
         d_data = self._pinned.stage("data" + engine._feed_suffix(data.dtype), data, self.device)
         self.h2d_bytes = data.nbytes + tsl.nbytes + line_width.nbytes + (labels.nbytes + llen.nbytes if labels is not None else 0)
         self.last_feed_path = "staged"
+        return self._eval_lines(flist, single, eng, d_data, d_ints, llen)
+
+    @staticmethod
+    def _images_feed(images):
+        """The `images` feed checked on the host: a non-empty sequence of 2-D uint8 arrays of 1 .. engine.RESIZE_MAX_HEIGHT rows and
+        at least one column.  Nothing is converted: a line of another dtype is refused rather than cast."""
+        if isinstance(images, np.ndarray) and images.dtype != object:
+            raise ValueError("images must be a sequence of 2-D uint8 arrays (one per line), not one array")
+        images = list(images)
+        if not images:
+            raise ValueError("images: no lines")
+        for i, im in enumerate(images):
+            if not isinstance(im, np.ndarray) or im.ndim != 2 or im.dtype != np.uint8:
+                raise ValueError(f"images[{i}] must be a 2-D uint8 array (a gray line), got "
+                                 f"{getattr(im, 'dtype', type(im).__name__)} {getattr(im, 'shape', '')}")
+            h, w = im.shape
+            if not 1 <= h <= engine.RESIZE_MAX_HEIGHT or w < 1:
+                raise ValueError(f"images[{i}] is {h} x {w}: lines need 1 .. {engine.RESIZE_MAX_HEIGHT} rows and at least one column")
+        return images
+
+    def _run_images(self, flist, single, eng, images, labels, llen):
+        """Packed evaluation of native-size lines (``images`` fed, checked by _images_feed): the raw bytes go to the device in one
+        copy, crnn_resize_lines_u8 resizes and packs them into the uint8 batch that prepare_line + pack_lines build on the host, and
+        from forward_lines on the run is _run_lines'.  Evaluation fetches only."""
+        from .lib.lstm.test import line_size
+        self._check_lines([f.kind for f in flist], eng, "images")
+        N = len(images)
+        src_h = np.array([im.shape[0] for im in images], np.int32)
+        src_w = np.array([im.shape[1] for im in images], np.int32)
+        size = np.array([line_size(h, w) for h, w in zip(src_h, src_w)], np.int32).reshape(N, 3)
+        out_w, lw, tsl = (np.ascontiguousarray(size[:, k]) for k in range(3))
+        W = int(lw.max())
+        nbytes = src_h.astype(np.int64) * src_w
+        offs = np.zeros(N, np.int64)
+        np.cumsum(nbytes[:-1], out=offs[1:])
+        tot = int(nbytes.sum())
+        # labels checked as for any packed batch (a zero-stride stand-in has the batch's shape and no memory)
+        self.validate_feed(np.broadcast_to(np.uint8(0), (N, W, 32)), tsl, labels, llen, lw)
+        pin, ev = self._pinned.staging_for("images", tot, torch.uint8)
+        pn = pin.numpy()
+        for im, o in zip(images, offs):
+            pn[o:o + im.size].reshape(im.shape)[...] = im
+        d_src = pin[:tot].to(self.device, non_blocking=True)
+        ev.record()
+        ints = {"off": offs.view(np.int32), "h": src_h, "w": src_w, "ow": out_w, "tsl": tsl, "lw": lw}
+        if labels is not None:
+            ints["labels"], ints["llen"] = labels, llen
+        d_ints = self._pinned.stage_ints(ints, self.device)
+        d_data = engine.resize_lines_u8(d_src, d_ints["off"].view(torch.int64), d_ints["h"], d_ints["w"], d_ints["ow"], W,
+                                        int(src_h.max()))
+        self.h2d_bytes = tot + sum(a.nbytes for a in ints.values())
+        self.last_feed_path = "native-size lines, resized on the device"
+        return self._eval_lines(flist, single, eng, d_data, d_ints, llen)
+
+    def _eval_lines(self, flist, single, eng, d_data, d_ints, llen):
+        """The fetches of a packed batch already on the device: d_data [N, W, 32], d_ints["lw"] / ["tsl"] (and ["labels"] /
+        ["llen"] with labels)."""
+        kinds = [f.kind for f in flist]
+        N, W = d_data.shape[0], d_data.shape[1]
+        d_tsl = d_ints["tsl"]
         logits = eng.forward_lines(d_data, d_ints["lw"], d_tsl)
         costs = grad = loss = None
         if any(k in LOSS_KINDS for k in kinds):
             costs, grad = engine.ctc_loss(logits, d_ints["labels"], d_ints["llen"], d_tsl, want_grad="ctc_grad" in kinds,
-                                          grad_scale=1.0 / data.shape[0], max_label_len=int(llen.max()) if llen.size else 0,
+                                          grad_scale=1.0 / N, max_label_len=int(llen.max()) if llen.size else 0,
                                           workspace="auto")
             loss = eng.total_loss(costs)
         out = []
@@ -514,7 +583,7 @@ class Session(object):
             elif k.startswith("layer:"):
                 name = k.split(":", 1)[1]
                 tapname = {"pool1": "conv1", "pool2": "conv3_2", "pool3": "conv4_2", "reshaped_layer": "conv5"}.get(name, name)
-                v = eng.tap(tapname, data.shape[0], data.shape[1]).cpu().numpy()
+                v = eng.tap(tapname, N, W).cpu().numpy()
             else:
                 raise ValueError(f"unknown fetch kind {k!r}")
             out.append(v)

@@ -145,17 +145,8 @@ static int backward_impl(crnn_model* m, const void* data, bool u8, const int* ti
       CUDA_TRY(cudaFuncSetAttribute(lstm_bwd::lstm_bwd_ks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lstm_bwd::ks::SMEM_BYTES));
       attr = true;
     }
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(lstm_bwd::CS * 2 * lp.tiles_per_dir);
-    cfg.blockDim = dim3(lstm_bwd::ks::NUM_THREADS);
-    cfg.dynamicSmemBytes = lstm_bwd::ks::SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = lstm_bwd::CS; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    CUDA_TRY(cudaLaunchKernelEx(&cfg, lstm_bwd::lstm_bwd_ks_kernel, m->tD_h256, lp, pl.bptt_x));
+    CRNN_TRY(launch_cluster(lstm_bwd::lstm_bwd_ks_kernel, lstm_bwd::CS, lstm_bwd::CS * 2 * lp.tiles_per_dir, lstm_bwd::ks::NUM_THREADS,
+                            lstm_bwd::ks::SMEM_BYTES, st, m->tD_h256, lp, pl.bptt_x));
   }
   BMARK();
   {

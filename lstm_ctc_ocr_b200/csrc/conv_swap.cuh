@@ -363,6 +363,14 @@ static int launch_conv2_swap(const CUtensorMap& x, const CUtensorMap& w, const C
   return CRNN_OK;
 }
 
+// the inference launch with LINES picked at run time: `lines` = a packed evaluation batch (crnn_forward_lines)
+template <bool FP8 = false>
+static int launch_conv2_swap_lines(bool lines, const CUtensorMap& x, const CUtensorMap& w, const CUtensorMap& out, const convsw::Params& p,
+                                   int num_sms, cudaStream_t st) {
+  if (lines) return launch_conv2_swap<false, true, FP8>(x, w, out, p, num_sms, st);
+  return launch_conv2_swap<false, false, FP8>(x, w, out, p, num_sms, st);
+}
+
 template <int WD, int CB, int MVALID>
 static int launch_conv_dgrad_swap(const CUtensorMap& x, const CUtensorMap& w, const convsw::DgradParams& p, int num_sms, cudaStream_t st) {
   auto kern = convsw::conv_dgrad_swap_kernel<WD, CB, MVALID>;

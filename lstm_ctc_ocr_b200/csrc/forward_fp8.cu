@@ -274,8 +274,7 @@ int fp8_conv2(crnn_model* m, convsw::Params p, bool lines, int sms, cudaStream_t
   State* s = reinterpret_cast<State*>(m->fp8);
   const Plan& pl = m->plan;
   p.oscale = s->scales + 0;
-  if (lines) return launch_conv2_swap<false, true, true>(pl.tA_c2s, m->tB_c2, pl.qO_c2s, p, sms, st);
-  return launch_conv2_swap<false, false, true>(pl.tA_c2s, m->tB_c2, pl.qO_c2s, p, sms, st);
+  return launch_conv2_swap_lines<true>(lines, pl.tA_c2s, m->tB_c2, pl.qO_c2s, p, sms, st);
 }
 
 // layer 0 conv3_1 (EPI_RELU -> e4m3 a3), 1 conv3_2 (EPI_RELU_POOL12 -> e4m3 a3p), 2 / 3 conv4_1 / conv4_2 (EPI_STATS -> bf16 pre-BN;
@@ -295,23 +294,13 @@ int fp8_conv_gemm(crnn_model* m, int layer, gemm::Params p, bool lines, int sms,
   using namespace gemm;
   if (moving) {
     p.colscale = s->colscale_m + (layer - 2) * 512;
-    if (layer == 2) {
-      if (lines) return launch_gemm<256, A_CONV3, EPI_RELU, 4, 2, true>(a, b, p, sms, st, &pl.q_c42);
-      return launch_gemm<256, A_CONV3, EPI_RELU, 4, 2>(a, b, p, sms, st, &pl.q_c42);
-    }
-    if (lines) return launch_gemm<256, A_CONV3, EPI_RELU_POOL12, 4, 2, true>(a, b, p, sms, st, &pl.qO_m42);
-    return launch_gemm<256, A_CONV3, EPI_RELU_POOL12, 4, 2>(a, b, p, sms, st, &pl.qO_m42);
+    if (layer == 2) return launch_gemm_lines<256, A_CONV3, EPI_RELU, 4, 2>(lines, a, b, p, sms, st, &pl.q_c42);
+    return launch_gemm_lines<256, A_CONV3, EPI_RELU_POOL12, 4, 2>(lines, a, b, p, sms, st, &pl.qO_m42);
   }
   switch (layer) {
-    case 0:
-      if (lines) return launch_gemm<256, A_CONV3, EPI_RELU, 4, 2, true>(a, b, p, sms, st, tO[0]);
-      return launch_gemm<256, A_CONV3, EPI_RELU, 4, 2>(a, b, p, sms, st, tO[0]);
-    case 1:
-      if (lines) return launch_gemm<256, A_CONV3, EPI_RELU_POOL12, 4, 2, true>(a, b, p, sms, st, tO[1]);
-      return launch_gemm<256, A_CONV3, EPI_RELU_POOL12, 4, 2>(a, b, p, sms, st, tO[1]);
-    default:
-      if (lines) return launch_gemm<256, A_CONV3, EPI_STATS, 4, 2, true>(a, b, p, sms, st, tO[layer]);
-      return launch_gemm<256, A_CONV3, EPI_STATS, 4, 2>(a, b, p, sms, st, tO[layer]);
+    case 0: return launch_gemm_lines<256, A_CONV3, EPI_RELU, 4, 2>(lines, a, b, p, sms, st, tO[0]);
+    case 1: return launch_gemm_lines<256, A_CONV3, EPI_RELU_POOL12, 4, 2>(lines, a, b, p, sms, st, tO[1]);
+    default: return launch_gemm_lines<256, A_CONV3, EPI_STATS, 4, 2>(lines, a, b, p, sms, st, tO[layer]);
   }
 }
 
@@ -325,10 +314,10 @@ int fp8_bn_apply(crnn_model* m, int layer, const float* bn, bool lines, cudaStre
   const uint4* in = reinterpret_cast<const uint4*>(layer ? pl.a4b_pre : pl.a4a_pre);
   uint2* out = reinterpret_cast<uint2*>(layer ? pl.a4b : pl.a4a);
   const float* os = s->scales + 3 + layer;
-  if (layer == 0 && lines) fp8::bn_apply_e4m3_kernel<false, true><<<grid, 256, 0, st>>>(in, out, bn, pl.line_w, os, nvec, pl.H2, Wo, 512);
-  else if (layer == 0) fp8::bn_apply_e4m3_kernel<false, false><<<grid, 256, 0, st>>>(in, out, bn, nullptr, os, nvec, pl.H2, Wo, 512);
-  else if (lines) fp8::bn_apply_e4m3_kernel<true, true><<<grid, 256, 0, st>>>(in, out, bn, pl.line_w, os, nvec, pl.H2, Wo, 512);
-  else fp8::bn_apply_e4m3_kernel<true, false><<<grid, 256, 0, st>>>(in, out, bn, nullptr, os, nvec, pl.H2, Wo, 512);
+  using fp8::bn_apply_e4m3_kernel;
+  const auto kern = layer ? (lines ? bn_apply_e4m3_kernel<true, true> : bn_apply_e4m3_kernel<true, false>)
+                          : (lines ? bn_apply_e4m3_kernel<false, true> : bn_apply_e4m3_kernel<false, false>);
+  kern<<<grid, 256, 0, st>>>(in, out, bn, lines ? pl.line_w : nullptr, os, nvec, pl.H2, Wo, 512);
   CUDA_TRY(cudaGetLastError());
   return CRNN_OK;
 }

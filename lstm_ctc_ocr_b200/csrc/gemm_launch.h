@@ -23,6 +23,31 @@ static int launch_gemm(const CUtensorMap& a, const CUtensorMap& b, const gemm::P
   return CRNN_OK;
 }
 
+// launch_gemm with LINES picked at run time: `lines` = a packed evaluation batch (crnn_forward_lines)
+template <int BN, int AM, int EPI, int ST, int KIND = 0>
+static int launch_gemm_lines(bool lines, const CUtensorMap& a, const CUtensorMap& b, const gemm::Params& p, int num_sms, cudaStream_t st,
+                             const CUtensorMap* out = nullptr) {
+  if (lines) return launch_gemm<BN, AM, EPI, ST, KIND, true>(a, b, p, num_sms, st, out);
+  return launch_gemm<BN, AM, EPI, ST, KIND, false>(a, b, p, num_sms, st, out);
+}
+
+// Launch of a kernel in clusters of `cluster` CTAs along x (the LSTM recurrence and its BPTT)
+template <class... KArgs, class... Args>
+static int launch_cluster(void (*kern)(KArgs...), int cluster, int grid, int threads, size_t smem, cudaStream_t st, Args... args) {
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(threads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+  cfg.attrs = at; cfg.numAttrs = 1;
+  CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, args...));
+  return CRNN_OK;
+}
+
 // Split-K factor of a weight-gradient GEMM.  Work items (output tile x K chunk) all cost the same and the persistent CTAs take them
 // round-robin, so the launch lasts  ceil(items / workers) rounds x (K blocks per chunk + epilogue).  A fixed "about 3 items per
 // worker" can leave a mostly idle last round.  Pick the factor that minimises the modelled time (ties: fewer chunks = fewer f32

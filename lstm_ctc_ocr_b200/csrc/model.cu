@@ -368,7 +368,9 @@ int prepare_weights(crnn_model* m, cudaStream_t st) {
 // ------------------------------------------------------------------------------------------------ workspace
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-size_t layout_plan(Plan& pl, int N, int W, uint8_t* base, bool train) {
+// `lines` (crnn_forward_lines, inference only): the packed-line region past the inference layout -- line widths [N] i32, then, unless
+// conv4_x normalise with the `moving` statistics, per-line statistics [2][N][2][512] f64 and coefficients [2][N][4][512] f32
+size_t layout_plan(Plan& pl, int N, int W, uint8_t* base, bool train, bool lines, bool moving) {
   pl.N = N; pl.W = W; pl.H1 = W / 2; pl.H2 = W / 4; pl.T = W / 4 - 1;
   pl.Npad = (N + 127) / 128 * 128;
   size_t off = 0;
@@ -388,6 +390,9 @@ size_t layout_plan(Plan& pl, int N, int W, uint8_t* base, bool train) {
   pl.h_state = (__nv_bfloat16*)take((size_t)2 * 2 * pl.Npad * 256 * 2);
   pl.stats = (double*)take(2 * 2 * 512 * 8);
   pl.bn = (float*)take(2 * 4 * 512 * 4);
+  pl.line_w = lines ? (int*)take(n * 4) : nullptr;
+  pl.stats_l = lines && !moving ? (double*)take(2 * n * 2 * 512 * 8) : nullptr;
+  pl.bn_l = lines && !moving ? (float*)take(2 * n * 4 * 512 * 4) : nullptr;
   pl.train = train;
   if (train) {
     const size_t T = pl.T;
@@ -572,43 +577,116 @@ static int ensure_chunk_events(crnn_model* m) {
   return CRNN_OK;
 }
 
-// Copy-then-compute from host memory (the fp8 and f32-class paths): the whole batch goes to `data` on `copy_st`, after the work
-// queued earlier on `st` and before anything `st` runs next -- the bf16 path's handshake with one range.  So on every path the
-// host buffers may be reused once the work queued on `copy_st` has completed, and a graph captured on `st` takes the copy in.
-static int host_copy_whole(crnn_model* m, void* data, void* host_data, const void* pageable_src, size_t bytes, int host_threads,
-                           cudaStream_t st, cudaStream_t copy_st) {
-  CRNN_TRY(ensure_chunk_events(m));
-  CUDA_TRY(cudaEventRecord(m->chunk_events[kMaxChunks], st));
-  CUDA_TRY(cudaStreamWaitEvent(copy_st, m->chunk_events[kMaxChunks], 0));
-  if (pageable_src != nullptr) CopyPool::get().copy(host_data, pageable_src, bytes, host_threads);
-  CUDA_TRY(cudaMemcpyAsync(data, host_data, bytes, cudaMemcpyHostToDevice, copy_st));
-  CUDA_TRY(cudaEventRecord(m->chunk_events[0], copy_st));
-  CUDA_TRY(cudaStreamWaitEvent(st, m->chunk_events[0], 0));
+// One forward call: where its batch lies and how it is computed.
+//   host == nullptr (crnn_forward, crnn_forward_lines, calibration): `data` is the batch on the device.
+//   host != nullptr, pageable == nullptr (crnn_forward_host): the batch is in page-locked host memory; it is copied to `data` on
+//     `copy_st` in `chunks` image ranges, each range's front end starting once its copy has landed.
+//   pageable != nullptr (crnn_forward_pageable): the batch is in ordinary host memory; the copy pool (`host_threads`) moves each range
+//     into the page-locked staging `host` first.
+//   line_width != nullptr (crnn_forward_lines): every image is a line evaluated as if alone.
+//   u8 (the crnn_*_u8 twins): the batch holds uint8 pixels, one byte per element instead of four.
+// The precision is the model's (bf16 or, compute_dtype 4, e4m3); `calib` (crnn_model_calibrate_fp8) runs the bf16 front end up to
+// conv4_2's BatchNorm, then reduces the fp8 scales.
+struct FwdCall {
+  const void* data = nullptr;
+  const void* host = nullptr;
+  const void* pageable = nullptr;
+  int host_threads = 1, chunks = 1;
+  bool u8 = false;
+  cudaStream_t copy_st = nullptr;
+  const int* line_width = nullptr;
+  bool calib = false;
+  // bytes of n images of width W, and image n of one of the batch pointers
+  size_t bytes(size_t n, int W) const { return n * W * 32 * (u8 ? 1 : sizeof(float)); }
+  uint8_t* at(const void* base, size_t n, int W) const {
+    return const_cast<uint8_t*>(static_cast<const uint8_t*>(base)) + bytes(n, W);
+  }
+};
+
+// The batch in image ranges of `nc`: `compute(n0, n1)` queues range [n0, n1)'s work on `st`.  A host-fed batch reaches the device on
+// `copy_st`: the copies wait for the work queued earlier on `st` (it may still read the staging tensor), and `st` waits for range c's
+// copy before range c's work.  From page-locked memory every range's DMA is queued before the first range's work; from pageable memory
+// the host copy of range c + 1 overlaps the GPU work on range c.  So the host buffers may be reused once the work queued on `copy_st`
+// has completed, and a graph captured on `st` takes the copies in.
+template <class F>
+static int for_each_range(crnn_model* m, const FwdCall& a, int N, int W, int nc, cudaStream_t st, F&& compute) {
+  const bool fed = a.host != nullptr;
+  auto copy = [&](int c) -> int {
+    const int n0 = c * nc, n = (n0 + nc < N) ? nc : N - n0;
+    if (a.pageable != nullptr) CopyPool::get().copy(a.at(a.host, n0, W), a.at(a.pageable, n0, W), a.bytes(n, W), a.host_threads);
+    CUDA_TRY(cudaMemcpyAsync(a.at(a.data, n0, W), a.at(a.host, n0, W), a.bytes(n, W), cudaMemcpyHostToDevice, a.copy_st));
+    CUDA_TRY(cudaEventRecord(m->chunk_events[c], a.copy_st));
+    return CRNN_OK;
+  };
+  if (fed) {
+    CRNN_TRY(ensure_chunk_events(m));
+    CUDA_TRY(cudaEventRecord(m->chunk_events[kMaxChunks], st));
+    CUDA_TRY(cudaStreamWaitEvent(a.copy_st, m->chunk_events[kMaxChunks], 0));
+  }
+  for (int c = 0; fed && a.pageable == nullptr && c * nc < N; ++c) CRNN_TRY(copy(c));
+  for (int c = 0; c * nc < N; ++c) {
+    if (fed && a.pageable != nullptr) CRNN_TRY(copy(c));
+    if (fed) CUDA_TRY(cudaStreamWaitEvent(st, m->chunk_events[c], 0));
+    const int n0 = c * nc;
+    CRNN_TRY(compute(n0, (n0 + nc < N) ? n0 + nc : N));
+  }
   return CRNN_OK;
 }
 
-// Forward pass.  `host_data` != nullptr (crnn_forward_host): the batch is still in page-locked HOST memory; it is cut into
-// `chunks` image ranges whose H2D copies run on `copy_st` while the batch-independent front end (conv1 .. conv3_2 + pools) of
-// the previous range runs on `st` -- the copy (33.6 MB at batch 1024 x 32x256) hides behind that compute instead of preceding it.  From conv4_1 on (batch-statistics BatchNorm) the batch is processed whole.
-// `pageable_src` != nullptr (crnn_forward_pageable): the batch is in ordinary host memory; every range is first moved into the
-// page-locked `host_data` staging by the copy pool, its DMA is issued, its front end is launched -- and the host moves the next
-// range while the GPU works on this one.
-// `line_width` != nullptr (crnn_forward_lines, device-fed, inference plan): every image is a line evaluated as if alone -- the conv
-// epilogues zero each activation past the line's width and conv4_x use per-line batch statistics.
-// compute_dtype 4: FWD_FP8 runs conv3_1 .. conv5 on e4m3 operands (forward_fp8.cu); from host memory it copies, then computes.
-// FWD_CALIB (crnn_model_calibrate_fp8) runs the bf16 front end up to conv4_2's BatchNorm (a4b), then reduces the fp8 scales.
-// `u8` (the crnn_*_u8 twins): `data`, `host_data` and `pageable_src` hold uint8 pixels, one byte per element instead of four; every
-// copy is sized by that element size and conv1 widens the bytes when it loads them.
-enum FwdPrec { FWD_BF16 = 0, FWD_FP8 = 1, FWD_CALIB = 2 };
-static int forward_impl(crnn_model* m, const void* data, const void* host_data, const int* time_step_len, int N, int W,
-                        float* logits_out, void* workspace, size_t workspace_bytes, int chunks, cudaStream_t st, cudaStream_t copy_st,
-                        const void* pageable_src = nullptr, int host_threads = 1, const int* line_width = nullptr, int prec = FWD_BF16,
-                        bool u8 = false) {
-  const bool fp8 = prec == FWD_FP8, calib = prec == FWD_CALIB;
-  if (!m || !data || !time_step_len || (!logits_out && !calib) || !workspace) return crnn_fail(CRNN_INVALID_VALUE, "forward: null pointer");
-  const size_t es = u8 ? 1 : sizeof(float);                 // bytes per element of the batch
-  // image n of a batch pointer, in bytes
-  auto at = [&](const void* base, size_t n) { return const_cast<uint8_t*>(static_cast<const uint8_t*>(base)) + n * W * 32 * es; };
+// The BiLSTM recurrence: ONE persistent launch, a cluster of 8 CTAs per (direction, 128-sample tile) -- csrc/lstm.cuh.
+// CRNN_LSTM_TRACE=1 records a debug timeline and prints it to stderr after every launch (tools/lstm_trace.py reads it).
+static int launch_lstm_forward(crnn_model* m, const int* time_step_len, cudaStream_t st) {
+  constexpr int CS = 8;
+  const Plan& pl = m->plan;
+  lstm::Params lp;
+  lp.xproj = pl.xproj; lp.h_state = pl.h_state; lp.lstm_out = pl.lstm_out; lp.seq_len = time_step_len;
+  lp.Nimg = pl.N; lp.Npad = pl.Npad; lp.H = pl.H2; lp.T = pl.T; lp.tiles_per_dir = pl.Npad / 128;
+  lp.gates = pl.train ? pl.gates : nullptr; lp.csave = pl.train ? pl.csave : nullptr;
+  static long long* d_trace = nullptr;
+  const bool want_trace = getenv("CRNN_LSTM_TRACE") != nullptr;
+  if (want_trace && d_trace == nullptr) CUDA_TRY(cudaMalloc(&d_trace, 2 * 2 * 4 * 16 * sizeof(long long)));
+  if (want_trace) CUDA_TRY(cudaMemsetAsync(d_trace, 0, 2 * 2 * 4 * 16 * sizeof(long long), st));
+  lp.trace = want_trace ? d_trace : nullptr;
+  auto kern = lstm::lstm_mc_kernel<CS>;
+  static bool attr = false;
+  if (!attr) {
+    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lstm::CfgMc<CS>::SMEM_BYTES));
+    attr = true;
+  }
+  CRNN_TRY(launch_cluster(kern, CS, CS * 2 * lp.tiles_per_dir, lstm::MC_THREADS, lstm::CfgMc<CS>::SMEM_BYTES, st, m->tB_h128, lp));
+  if (want_trace) {
+    long long h[2 * 2 * 4 * 16];            // [CTA 0 / 5][warpgroup slot][step 8..11][event]
+    CUDA_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaMemcpy(h, d_trace, sizeof(h), cudaMemcpyDeviceToHost));
+    for (int c = 0; c < 2; ++c) {
+      long long t0 = 0;                       // earliest stamp of the CTA: both warpgroups on one time axis
+      for (int i = c * 128; i < (c + 1) * 128; ++i)
+        if (h[i] && (!t0 || h[i] < t0)) t0 = h[i];
+      for (int wg = 0; wg < 2; ++wg)
+        for (int s = 0; s < 4; ++s) {
+          const long long* r = h + ((c * 2 + wg) * 4 + s) * 16;
+          bool any = false;
+          for (int e = 0; e < 16; ++e) any = any || r[e];
+          if (!any) continue;
+          fprintf(stderr, "lstm_trace cta%d wg%d step%d:", c ? 5 : 0, wg, 8 + s);
+          for (int e = 0; e < 12; ++e) fprintf(stderr, " %lld", r[e] ? r[e] - t0 : -1);
+          fprintf(stderr, "\n");
+        }
+    }
+  }
+  return CRNN_OK;
+}
+
+// The forward pass of every entry point (FwdCall).  A chunked front end (crnn_forward_host / _pageable) runs the batch-independent
+// conv1 .. conv3_2 + pools per image range, so the copy (33.6 MB at batch 1024 x 32x256) hides behind that compute instead of
+// preceding it; from conv4_1 on (batch-statistics BatchNorm) the batch is processed whole.  Packed lines: the conv epilogues zero each
+// activation past the line's width and conv4_x use per-line batch statistics.  compute_dtype 4 runs conv3_1 .. conv5 on e4m3 operands
+// (forward_fp8.cu); it and the f32-class paths (forward_x3.cu) copy a host-fed batch whole, then compute.
+static int forward(crnn_model* m, FwdCall a, const int* time_step_len, int N, int W, float* logits_out, void* workspace,
+                   size_t workspace_bytes, crnn_stream_t stream) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const bool calib = a.calib, fp8 = m && m->cfg.compute_dtype == 4 && !calib;
+  if (!m || !a.data || !time_step_len || (!logits_out && !calib) || !workspace) return crnn_fail(CRNN_INVALID_VALUE, "forward: null pointer");
   if (!m->params) return crnn_fail(CRNN_NOT_BOUND, "forward: call crnn_model_bind first");
   const bool moving = m->bn_use_moving && !m->training;     // training forwards always normalise with batch statistics
   if (moving && !m->bn_moving)
@@ -623,20 +701,15 @@ static int forward_impl(crnn_model* m, const void* data, const void* host_data, 
       return crnn_fail(CRNN_INVALID_VALUE, "forward: the fp8 model (compute_dtype 4) has no activation scales: calibration is missing "
                                            "(crnn_model_calibrate_fp8 or crnn_model_set_fp8_scales after the last parameter change)");
     if (m->dp_world > 1) return crnn_fail(CRNN_UNSUPPORTED, "forward: the fp8 path runs on one device (no data parallelism)");
-    if (host_data != nullptr) {
-      // copy-then-compute, as the f32-class paths do
-      CRNN_TRY(host_copy_whole(m, at(data, 0), at(host_data, 0), pageable_src, (size_t)N * W * 32 * es, host_threads, st, copy_st));
-      host_data = nullptr;
-      pageable_src = nullptr;
-    }
-    chunks = 1;
   }
-  if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3) {
-    // f32-class paths (forward_x3.cu): copy-then-compute when fed from host memory
-    if (host_data != nullptr)
-      CRNN_TRY(host_copy_whole(m, at(data, 0), at(host_data, 0), pageable_src, (size_t)N * W * 32 * es, host_threads, st, copy_st));
-    return x3_forward(m, data, u8, time_step_len, N, W, logits_out, workspace, workspace_bytes, st);
+  const bool x3 = m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3;
+  if (fp8 || calib || x3) {
+    // copy-then-compute: the whole batch as one range, no work in it
+    CRNN_TRY(for_each_range(m, a, N, W, N, st, [](int, int) -> int { return CRNN_OK; }));
+    a.host = a.pageable = nullptr;
+    a.chunks = 1;
   }
+  if (x3) return x3_forward(m, a.data, a.u8, time_step_len, N, W, logits_out, workspace, workspace_bytes, st);
   if (m->dirty) CRNN_TRY(prepare_weights(m, st));
   if (fp8) CRNN_TRY(fp8_prepare(m, st));
   if (moving) {
@@ -646,58 +719,31 @@ static int forward_impl(crnn_model* m, const void* data, const void* host_data, 
   }
   Plan& pl = m->plan;
   CRNN_TRY(ensure_plan(m, N, W, workspace, st));
+  const bool lines = a.line_width != nullptr;
+  layout_plan(pl, N, W, reinterpret_cast<uint8_t*>(workspace), pl.train, lines, moving);    // this call's packed-line region, or none
   pl.moving = moving;
-  const int H1 = pl.H1, H2 = pl.H2, T = pl.T, sms = m->num_sms;
-  const bool lines = line_width != nullptr;
-  pl.line_w = nullptr;
-  if (lines) {
-    Plan tmp;
-    uint8_t* x = reinterpret_cast<uint8_t*>(workspace) + layout_plan(tmp, N, W, nullptr, false);
-    pl.line_w = reinterpret_cast<int*>(x); x += align_up((size_t)N * 4);
-    pl.stats_l = reinterpret_cast<double*>(x); x += align_up((size_t)2 * N * 2 * 512 * 8);
-    pl.bn_l = reinterpret_cast<float*>(x);
-    CRNN_TRY(launch_clamp_line_width(line_width, pl.line_w, N, W, st));
-  }
+  const int H1 = pl.H1, H2 = pl.H2, sms = m->num_sms;
+  if (lines) CRNN_TRY(launch_clamp_line_width(a.line_width, pl.line_w, N, W, st));
   cudaEvent_t* ev = nullptr;
   if (!calib && m->prof_on && m->prof_used < m->prof_slots) ev = &m->prof_events[(size_t)(m->prof_used++) * (kNumStages + 1)];
   int evi = 0;
 #define STAGE_MARK() do { if (ev) CUDA_TRY(cudaEventRecord(ev[evi++], st)); } while (0)
   STAGE_MARK();
 
-  // ---- front end, per image range [n0, n0 + nc): conv1+pool1, conv2+pool2, conv3_1, conv3_2+pool (all batch-independent)
+  // ---- front end, per image range [n0, n1): conv1+pool1, conv2+pool2, conv3_1, conv3_2+pool (all batch-independent)
   const int sb3 = (H2 + 3) / 4;                      // 32-position sub-boxes per image of the conv3 layers (Wd = 8 -> 4 H rows)
   const int sb2 = (H1 + 1) / 2;                      // the same at conv2's input resolution (Wd = 16 -> 2 H rows)
-  if (chunks < 1) chunks = 1;
-  if (chunks > kMaxChunks) chunks = kMaxChunks;
+  int chunks = a.chunks < 1 ? 1 : a.chunks > kMaxChunks ? kMaxChunks : a.chunks;
   int nc = (N + chunks - 1) / chunks;
   // a range must start on a tile-PAIR boundary of every layer (128-position tiles = 4 sub-boxes, pairs = 8)
   if (chunks > 1 && ((nc * sb3) % 8 != 0 || (nc * sb2) % 8 != 0)) { chunks = 1; nc = N; }
-  if (host_data != nullptr) {
-    CRNN_TRY(ensure_chunk_events(m));
-    // the staging tensor may still be read by work queued earlier on `st` (previous forward / backward)
-    CUDA_TRY(cudaEventRecord(m->chunk_events[kMaxChunks], st));
-    CUDA_TRY(cudaStreamWaitEvent(copy_st, m->chunk_events[kMaxChunks], 0));
-    for (int c = 0; pageable_src == nullptr && c * nc < N; ++c) {
-      const int n0 = c * nc, n1 = (n0 + nc < N) ? n0 + nc : N;
-      CUDA_TRY(cudaMemcpyAsync(at(data, n0), at(host_data, n0), (size_t)(n1 - n0) * W * 32 * es, cudaMemcpyHostToDevice, copy_st));
-      CUDA_TRY(cudaEventRecord(m->chunk_events[c], copy_st));
-    }
-  }
-  for (int c = 0; c * nc < N; ++c) {
-    const int n0 = c * nc, n1 = (n0 + nc < N) ? n0 + nc : N, cn = n1 - n0;
+  CRNN_TRY(for_each_range(m, a, N, W, nc, st, [&](int n0, int n1) -> int {
+    const int cn = n1 - n0;
     const bool mark = (n1 == N) && chunks == 1;      // per-stage events only make sense for an unchunked front end
-    if (pageable_src != nullptr) {
-      // pageable source: move this range into the page-locked staging now (the GPU is busy with the previous range), then issue its DMA
-      const size_t bytes = (size_t)cn * W * 32 * es;
-      CopyPool::get().copy(at(host_data, n0), at(pageable_src, n0), bytes, host_threads);
-      CUDA_TRY(cudaMemcpyAsync(at(data, n0), at(host_data, n0), bytes, cudaMemcpyHostToDevice, copy_st));
-      CUDA_TRY(cudaEventRecord(m->chunk_events[c], copy_st));
-    }
-    if (host_data != nullptr) CUDA_TRY(cudaStreamWaitEvent(st, m->chunk_events[c], 0));
     // conv1 + pool1 (tensor cores, split-bf16 operands: conv1_tc.cuh)
     {
       const size_t o1 = (size_t)n0 * H1 * 16 * 64;
-      CRNN_TRY(launch_conv1_tc(pl.tO_c1, at(data, n0), u8, m->P("conv1/weights"), m->P("conv1/biases"), n0,
+      CRNN_TRY(launch_conv1_tc(pl.tO_c1, a.at(a.data, n0, W), a.u8, m->P("conv1/weights"), m->P("conv1/biases"), n0,
                                pl.train ? pl.am1 + o1 : nullptr, cn, W, sms, st, pl.line_w));
     }
     if (mark) STAGE_MARK();
@@ -709,8 +755,7 @@ static int forward_impl(crnn_model* m, const void* data, const void* host_data, 
       p.line_w = pl.line_w;
       if (fp8) CRNN_TRY(fp8_conv2(m, p, lines, sms, st));
       else if (pl.train) CRNN_TRY(launch_conv2_swap<true>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st));
-      else if (lines) CRNN_TRY((launch_conv2_swap<false, true>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st)));
-      else CRNN_TRY(launch_conv2_swap<false>(pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st));
+      else CRNN_TRY(launch_conv2_swap_lines(lines, pl.tA_c2s, m->tB_c2, pl.tO_c2s, p, sms, st));
     }
     if (mark) STAGE_MARK();
     // conv3_1 + ReLU
@@ -719,105 +764,60 @@ static int forward_impl(crnn_model* m, const void* data, const void* host_data, 
       if (chunks > 1) { p.m_tile0 = n0 * sb3 / 4; p.num_m_tiles = cn * sb3 / 4; }
       p.line_w = pl.line_w;
       if (fp8) CRNN_TRY(fp8_conv_gemm(m, 0, p, lines, sms, st));
-      else if (lines) CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4, 0, true>(pl.tA_c31, m->tB_c31, p, sms, st, &pl.tA_c32)));
-      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4>(pl.tA_c31, m->tB_c31, p, sms, st, &pl.tA_c32)));
+      else CRNN_TRY((launch_gemm_lines<256, gemm::A_CONV3, gemm::EPI_RELU, 4>(lines, pl.tA_c31, m->tB_c31, p, sms, st, &pl.tA_c32)));
     }
     if (mark) STAGE_MARK();
     // conv3_2 + ReLU + height pool
     {
       gemm::Params p = conv_params(N, H2, 8, 256, 256, 256, m->P("conv3_2/biases"), pl.a3p, pl.mg3);
       if (chunks > 1) { p.m_tile0 = n0 * sb3 / 4; p.num_m_tiles = cn * sb3 / 4; }
-      if (fp8) {
-        p.line_w = pl.line_w;
-        CRNN_TRY(fp8_conv_gemm(m, 1, p, lines, sms, st));
-      } else if (pl.train) {
+      if (pl.train) {
         p.argmax = pl.am3;
         CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12_T, 4>(pl.tA_c32, m->tB_c32, p, sms, st)));
-      } else if (lines) {
-        p.line_w = pl.line_w;
-        CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12, 4, 0, true>(pl.tA_c32, m->tB_c32, p, sms, st, &pl.tO_c32)));
       } else {
-        CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12, 4>(pl.tA_c32, m->tB_c32, p, sms, st, &pl.tO_c32)));
+        p.line_w = pl.line_w;
+        if (fp8) CRNN_TRY(fp8_conv_gemm(m, 1, p, lines, sms, st));
+        else CRNN_TRY((launch_gemm_lines<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12, 4>(lines, pl.tA_c32, m->tB_c32, p, sms, st, &pl.tO_c32)));
       }
     }
     if (mark) STAGE_MARK();
-  }
+    return CRNN_OK;
+  }));
   if (chunks > 1) for (int i = 0; i < 4; ++i) STAGE_MARK();     // keep the event layout (front-end stages read as ~0)
-  if (moving) {
-    // conv4_x with the moving statistics folded into the weights and bias: conv4_1 + BN + ReLU is conv3_1's EPI_RELU GEMM, conv4_2
-    // + BN + ReLU + pool3 conv3_2's EPI_RELU_POOL12 GEMM; line masks zero the rows past each line, nothing else is per line.  The
-    // BN apply stages do not run (their events read ~0).
-    const struct { const char* name; int cin; const CUtensorMap* tA; const CUtensorMap* tB; __nv_bfloat16* out; } L[2] = {
-        {"conv4_1", 256, &pl.tA_c41, &m->tB_m41, pl.a4a}, {"conv4_2", 512, &pl.tA_c42, &m->tB_m42, pl.a4b}};
-    for (int l = 0; l < 2; ++l) {
-      gemm::Params p = conv_params(N, H2, 4, L[l].cin, 512, 256, m->bm_bias + l * 512, L[l].out, pl.mg4);
-      p.line_w = pl.line_w;
-      if (fp8) CRNN_TRY(fp8_conv_gemm(m, 2 + l, p, lines, sms, st, true));
-      else if (l == 0 && lines) CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4, 0, true>(*L[0].tA, *L[0].tB, p, sms, st, &pl.tA_c42)));
-      else if (l == 0) CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU, 4>(*L[0].tA, *L[0].tB, p, sms, st, &pl.tA_c42)));
-      else if (lines) CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12, 4, 0, true>(*L[1].tA, *L[1].tB, p, sms, st, &pl.tO_m42)));
-      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12, 4>(*L[1].tA, *L[1].tB, p, sms, st, &pl.tO_m42)));
-      STAGE_MARK();
-      STAGE_MARK();
-    }
-  } else if (lines) {
-    // conv4_x with per-line statistics: each line's own sums, scale and shift; zero at h >= W_i/4
-    CUDA_TRY(cudaMemsetAsync(pl.stats_l, 0, (size_t)2 * N * 2 * 512 * sizeof(double), st));
-    const struct { const char* name; const CUtensorMap* tA; const CUtensorMap* tB; const CUtensorMap* tO; int cin; __nv_bfloat16* pre; } L[2] = {
-        {"conv4_1", &pl.tA_c41, &m->tB_c41, &pl.tO_c41, 256, pl.a4a_pre}, {"conv4_2", &pl.tA_c42, &m->tB_c42, &pl.tO_c42, 512, pl.a4b_pre}};
-    for (int l = 0; l < 2; ++l) {
-      const std::string nm(L[l].name);
-      gemm::Params p = conv_params(N, H2, 4, L[l].cin, 512, 256, m->P(nm + "/biases"), L[l].pre, pl.mg4);
-      p.stats = pl.stats_l + (size_t)l * N * 2 * 512;
-      p.line_w = pl.line_w;
-      if (fp8) CRNN_TRY(fp8_conv_gemm(m, 2 + l, p, true, sms, st));
-      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4, 0, true>(*L[l].tA, *L[l].tB, p, sms, st, L[l].tO)));
-      STAGE_MARK();
-      float* bn = pl.bn_l + (size_t)l * N * 4 * 512;
-      CRNN_TRY(launch_bn_finalize_lines(p.stats, pl.line_w, m->P(nm + "/" + nm + "/gamma"), m->P(nm + "/" + nm + "/beta"), m->cfg.bn_eps,
-                                        bn, N, 512, st));
-      if (fp8) CRNN_TRY(fp8_bn_apply(m, l, bn, true, st));
-      else if (l == 0) CRNN_TRY(launch_bn_apply_relu_lines(pl.a4a_pre, pl.a4a, bn, pl.line_w, N, H2, 4, 512, st));
-      else CRNN_TRY(launch_bn_apply_relu_pool12_lines(pl.a4b_pre, pl.a4b, bn, pl.line_w, N, H2, 2, 512, st));
-      STAGE_MARK();
-    }
-  } else {
-    CUDA_TRY(cudaMemsetAsync(pl.stats, 0, 2 * 2 * 512 * sizeof(double), st));
-    const double bn_count = (double)N * H2 * 4;
-    // conv4_1 + bias -> batch statistics -> BN + ReLU
-    {
-      gemm::Params p = conv_params(N, H2, 4, 256, 512, 256, m->P("conv4_1/biases"), pl.a4a_pre, pl.mg4);
-      p.stats = pl.stats;
-      if (fp8) CRNN_TRY(fp8_conv_gemm(m, 2, p, false, sms, st));
-      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c41, m->tB_c41, p, sms, st, &pl.tO_c41)));
-      STAGE_MARK();
-      float* bn = pl.bn;
-      // batch statistics over the GLOBAL batch when the batch is sharded over ranks: the exchange is fused into the finalize kernel
-      if (m->dp_world > 1)
-        CRNN_TRY(dp_allreduce_bn_finalize(m, pl.stats, bn_count * m->dp_world, m->P("conv4_1/conv4_1/gamma"), m->P("conv4_1/conv4_1/beta"),
-                                          m->cfg.bn_eps, bn, st));
-      else
-      CRNN_TRY(launch_bn_finalize(pl.stats, bn_count, m->P("conv4_1/conv4_1/gamma"), m->P("conv4_1/conv4_1/beta"),
-                                  m->cfg.bn_eps, bn, bn + 512, bn + 1024, bn + 1536, 512, st));
-      if (fp8) CRNN_TRY(fp8_bn_apply(m, 0, bn, false, st));
-      else CRNN_TRY(launch_bn_apply_relu(pl.a4a_pre, pl.a4a, bn, bn + 512, (size_t)N * H2 * 4, 512, st));
-    }
+
+  // ---- conv4_1 + BN + ReLU, conv4_2 + BN + ReLU + pool3, each a GEMM, a BatchNorm finalize and an apply.  The statistics are the
+  // batch's (over the GLOBAL batch when it is sharded over ranks: the exchange is fused into the finalize kernel) or each line's own.
+  // With the moving statistics the BatchNorm is folded into the weights and bias: conv4_1 + BN + ReLU is conv3_1's EPI_RELU GEMM,
+  // conv4_2 + BN + ReLU + pool3 conv3_2's EPI_RELU_POOL12 GEMM, and the finalize and apply do not run (their events read ~0).
+  const struct { const char* name; int cin; const CUtensorMap *tA, *tB, *tO, *tB_m, *tO_m; __nv_bfloat16 *pre, *out; } L[2] = {
+      {"conv4_1", 256, &pl.tA_c41, &m->tB_c41, &pl.tO_c41, &m->tB_m41, &pl.tA_c42, pl.a4a_pre, pl.a4a},
+      {"conv4_2", 512, &pl.tA_c42, &m->tB_c42, &pl.tO_c42, &m->tB_m42, &pl.tO_m42, pl.a4b_pre, pl.a4b}};
+  double* const stats = lines ? pl.stats_l : pl.stats;              // [2 layers][N or 1][2][512]
+  float* const bn_all = lines ? pl.bn_l : pl.bn;                    // [2 layers][N or 1][4][512]
+  const size_t per_layer = lines ? (size_t)N * 512 : 512;
+  if (!moving) CUDA_TRY(cudaMemsetAsync(stats, 0, 2 * per_layer * 2 * sizeof(double), st));
+  for (int l = 0; l < 2; ++l) {
+    const std::string nm(L[l].name);
+    gemm::Params p = conv_params(N, H2, 4, L[l].cin, 512, 256, moving ? m->bm_bias + l * 512 : m->P(nm + "/biases"),
+                                 moving ? L[l].out : L[l].pre, pl.mg4);
+    p.line_w = pl.line_w;
+    if (!moving) p.stats = stats + l * per_layer * 2;
+    if (fp8) CRNN_TRY(fp8_conv_gemm(m, 2 + l, p, lines, sms, st, moving));
+    else if (moving && l == 0) CRNN_TRY((launch_gemm_lines<256, gemm::A_CONV3, gemm::EPI_RELU, 4>(lines, *L[0].tA, *L[0].tB_m, p, sms, st, L[0].tO_m)));
+    else if (moving) CRNN_TRY((launch_gemm_lines<256, gemm::A_CONV3, gemm::EPI_RELU_POOL12, 4>(lines, *L[1].tA, *L[1].tB_m, p, sms, st, L[1].tO_m)));
+    else CRNN_TRY((launch_gemm_lines<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(lines, *L[l].tA, *L[l].tB, p, sms, st, L[l].tO)));
     STAGE_MARK();
-    // conv4_2 + bias -> batch statistics -> BN + ReLU + height pool (pool3)
-    {
-      gemm::Params p = conv_params(N, H2, 4, 512, 512, 256, m->P("conv4_2/biases"), pl.a4b_pre, pl.mg4);
-      p.stats = pl.stats + 1024;
-      if (fp8) CRNN_TRY(fp8_conv_gemm(m, 3, p, false, sms, st));
-      else CRNN_TRY((launch_gemm<256, gemm::A_CONV3, gemm::EPI_STATS, 4>(pl.tA_c42, m->tB_c42, p, sms, st, &pl.tO_c42)));
-      STAGE_MARK();
-      float* bn = pl.bn + 2048;
-      if (m->dp_world > 1)
-        CRNN_TRY(dp_allreduce_bn_finalize(m, pl.stats + 1024, bn_count * m->dp_world, m->P("conv4_2/conv4_2/gamma"),
-                                          m->P("conv4_2/conv4_2/beta"), m->cfg.bn_eps, bn, st));
-      else
-      CRNN_TRY(launch_bn_finalize(pl.stats + 1024, bn_count, m->P("conv4_2/conv4_2/gamma"), m->P("conv4_2/conv4_2/beta"),
-                                  m->cfg.bn_eps, bn, bn + 512, bn + 1024, bn + 1536, 512, st));
-      if (fp8) CRNN_TRY(fp8_bn_apply(m, 1, bn, false, st));
+    if (!moving) {
+      float* bn = bn_all + l * per_layer * 4;
+      const float *gamma = m->P(nm + "/" + nm + "/gamma"), *beta = m->P(nm + "/" + nm + "/beta");
+      const double bn_count = (double)N * H2 * 4;
+      if (lines) CRNN_TRY(launch_bn_finalize_lines(p.stats, pl.line_w, gamma, beta, m->cfg.bn_eps, bn, N, 512, st));
+      else if (m->dp_world > 1) CRNN_TRY(dp_allreduce_bn_finalize(m, p.stats, bn_count * m->dp_world, gamma, beta, m->cfg.bn_eps, bn, st));
+      else CRNN_TRY(launch_bn_finalize(p.stats, bn_count, gamma, beta, m->cfg.bn_eps, bn, bn + 512, bn + 1024, bn + 1536, 512, st));
+      if (fp8) CRNN_TRY(fp8_bn_apply(m, l, bn, lines, st));
+      else if (lines && l == 0) CRNN_TRY(launch_bn_apply_relu_lines(pl.a4a_pre, pl.a4a, bn, pl.line_w, N, H2, 4, 512, st));
+      else if (lines) CRNN_TRY(launch_bn_apply_relu_pool12_lines(pl.a4b_pre, pl.a4b, bn, pl.line_w, N, H2, 2, 512, st));
+      else if (l == 0) CRNN_TRY(launch_bn_apply_relu(pl.a4a_pre, pl.a4a, bn, bn + 512, (size_t)N * H2 * 4, 512, st));
       else CRNN_TRY(launch_bn_apply_relu_pool12(pl.a4b_pre, pl.a4b, bn, bn + 512, (size_t)N * H2 * 2, 512, st));
     }
     STAGE_MARK();
@@ -841,63 +841,14 @@ static int forward_impl(crnn_model* m, const void* data, const void* host_data, 
     p.M = N * H2;
     p.num_m_tiles = (p.M + 127) / 128; p.num_n_tiles = 8; p.num_k_blocks = 8; p.kb_per_shift = 8;
     p.Nc = 2048; p.bias = m->xbias; p.out = pl.xproj; p.ldo = 2048;
-    p.H = H2; p.T = T; p.seq_len = time_step_len;
+    p.H = H2; p.T = pl.T; p.seq_len = time_step_len;
     CRNN_TRY((launch_gemm<256, gemm::A_PLAIN, gemm::EPI_XPROJ, 4>(pl.tA_x, m->tB_x, p, sms, st, &pl.tO_x)));
   }
   STAGE_MARK();
   // rows t = T (= H2-1) of lstm_out are never produced by a time step, yet the logits GEMM and the backward's dW_h GEMMs read
   // them (dW_h as h_{-1} / h_{T} of the neighbouring image): zero them in every forward, whatever the workspace held before
-  CUDA_TRY(cudaMemset2DAsync(pl.lstm_out + (size_t)T * 512, (size_t)H2 * 512 * 2, 0, 512 * 2, N, st));
-  {
-    // recurrence: ONE persistent launch; a cluster of 8 CTAs per (direction, 128-sample tile) -- csrc/lstm.cuh
-    constexpr int CS = 8;
-    lstm::Params lp;
-    lp.xproj = pl.xproj; lp.h_state = pl.h_state; lp.lstm_out = pl.lstm_out; lp.seq_len = time_step_len;
-    lp.Nimg = N; lp.Npad = pl.Npad; lp.H = H2; lp.T = T; lp.tiles_per_dir = pl.Npad / 128;
-    lp.gates = pl.train ? pl.gates : nullptr; lp.csave = pl.train ? pl.csave : nullptr;
-    static long long* d_trace = nullptr;          // debug timeline (CRNN_LSTM_TRACE=1), printed to stderr after every launch
-    const bool want_trace = getenv("CRNN_LSTM_TRACE") != nullptr;
-    if (want_trace && d_trace == nullptr) CUDA_TRY(cudaMalloc(&d_trace, 2 * 2 * 4 * 16 * sizeof(long long)));
-    if (want_trace) CUDA_TRY(cudaMemsetAsync(d_trace, 0, 2 * 2 * 4 * 16 * sizeof(long long), st));
-    lp.trace = want_trace ? d_trace : nullptr;
-    auto kern = lstm::lstm_mc_kernel<CS>;
-    static bool attr = false;
-    if (!attr) {
-      CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lstm::CfgMc<CS>::SMEM_BYTES));
-      attr = true;
-    }
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(CS * 2 * lp.tiles_per_dir);
-    cfg.blockDim = dim3(lstm::MC_THREADS);
-    cfg.dynamicSmemBytes = lstm::CfgMc<CS>::SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = CS; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, m->tB_h128, lp));
-    if (want_trace) {
-      long long h[2 * 2 * 4 * 16];            // [CTA 0 / 5][warpgroup slot][step 8..11][event]
-      CUDA_TRY(cudaStreamSynchronize(st));
-      CUDA_TRY(cudaMemcpy(h, d_trace, sizeof(h), cudaMemcpyDeviceToHost));
-      for (int c = 0; c < 2; ++c) {
-        long long t0 = 0;                       // earliest stamp of the CTA: both warpgroups on one time axis
-        for (int i = c * 128; i < (c + 1) * 128; ++i)
-          if (h[i] && (!t0 || h[i] < t0)) t0 = h[i];
-        for (int wg = 0; wg < 2; ++wg)
-          for (int s = 0; s < 4; ++s) {
-            const long long* r = h + ((c * 2 + wg) * 4 + s) * 16;
-            bool any = false;
-            for (int e = 0; e < 16; ++e) any = any || r[e];
-            if (!any) continue;
-            fprintf(stderr, "lstm_trace cta%d wg%d step%d:", c ? 5 : 0, wg, 8 + s);
-            for (int e = 0; e < 12; ++e) fprintf(stderr, " %lld", r[e] ? r[e] - t0 : -1);
-            fprintf(stderr, "\n");
-          }
-      }
-    }
-  }
+  CUDA_TRY(cudaMemset2DAsync(pl.lstm_out + (size_t)pl.T * 512, (size_t)H2 * 512 * 2, 0, 512 * 2, N, st));
+  CRNN_TRY(launch_lstm_forward(m, time_step_len, st));
   STAGE_MARK();
   // 512 -> 64 projection, written time-major [T, N, 64] (network.py:126-128)
   {
@@ -905,7 +856,7 @@ static int forward_impl(crnn_model* m, const void* data, const void* host_data, 
     memset(&p, 0, sizeof(p));
     p.M = N * H2;
     p.num_m_tiles = (p.M + 127) / 128; p.num_n_tiles = 1; p.num_k_blocks = 8; p.kb_per_shift = 8;
-    p.Nc = 64; p.bias = m->P("logits/biases"); p.out = logits_out; p.H = H2; p.T = T; p.Nimg = N;
+    p.Nc = 64; p.bias = m->P("logits/biases"); p.out = logits_out; p.H = H2; p.T = pl.T; p.Nimg = N;
     CRNN_TRY((launch_gemm<64, gemm::A_PLAIN, gemm::EPI_LOGITS, 8>(pl.tA_l, m->tB_l, p, sms, st)));
   }
   STAGE_MARK();
@@ -913,69 +864,95 @@ static int forward_impl(crnn_model* m, const void* data, const void* host_data, 
   return CRNN_OK;
 }
 
-static int fwd_prec(const crnn_model* m) { return (m && m->cfg.compute_dtype == 4) ? FWD_FP8 : FWD_BF16; }
-
 // the uint8 kernels load each row's pixels as 4-byte words
 static int check_u8_aligned(const void* p, const char* fn) {
   if ((reinterpret_cast<uintptr_t>(p) & 3) != 0) return crnn_fail(CRNN_INVALID_VALUE, "%s: uint8 data must be 4-byte aligned", fn);
   return CRNN_OK;
 }
 
-static int forward_dev(crnn_model* m, const void* data, bool u8, const int* time_step_len, int N, int W, float* logits_out,
-                       void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return forward_impl(m, data, nullptr, time_step_len, N, W, logits_out, workspace, workspace_bytes, 1, st, st, nullptr, 1, nullptr,
-                      fwd_prec(m), u8);
+// a device-fed batch of floats or (u8) uint8 pixels
+static FwdCall device_batch(const void* data, bool u8) {
+  FwdCall a;
+  a.data = data; a.u8 = u8;
+  return a;
 }
+// a batch in page-locked (pageable == nullptr) or ordinary host memory, copied to `data` on `copy_stream`
+static FwdCall host_batch(const void* host, const void* pageable, const void* data, bool u8, int chunks, int host_threads,
+                          crnn_stream_t copy_stream) {
+  FwdCall a = device_batch(data, u8);
+  a.host = host; a.pageable = pageable; a.chunks = chunks; a.host_threads = host_threads < 1 ? 1 : host_threads;
+  a.copy_st = reinterpret_cast<cudaStream_t>(copy_stream);
+  return a;
+}
+
 extern "C" int crnn_forward(crnn_model* m, const float* data, const int* time_step_len, int N, int W, float* logits_out,
                             void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
-  return forward_dev(m, data, false, time_step_len, N, W, logits_out, workspace, workspace_bytes, stream);
+  return forward(m, device_batch(data, false), time_step_len, N, W, logits_out, workspace, workspace_bytes, stream);
 }
 extern "C" int crnn_forward_u8(crnn_model* m, const uint8_t* data, const int* time_step_len, int N, int W, float* logits_out,
                                void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
   CRNN_TRY(check_u8_aligned(data, "forward_u8"));
-  return forward_dev(m, data, true, time_step_len, N, W, logits_out, workspace, workspace_bytes, stream);
+  return forward(m, device_batch(data, true), time_step_len, N, W, logits_out, workspace, workspace_bytes, stream);
 }
 
-static int forward_host(crnn_model* m, const void* host_data, void* data_staging, bool u8, const int* time_step_len, int N, int W,
-                        float* logits_out, void* workspace, size_t workspace_bytes, int chunks, crnn_stream_t stream,
-                        crnn_stream_t copy_stream) {
-  if (!host_data || !data_staging) return crnn_fail(CRNN_INVALID_VALUE, "forward_host: null pointer");
-  return forward_impl(m, data_staging, host_data, time_step_len, N, W, logits_out, workspace, workspace_bytes, chunks,
-                      reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<cudaStream_t>(copy_stream), nullptr, 1, nullptr, fwd_prec(m),
-                      u8);
-}
 extern "C" int crnn_forward_host(crnn_model* m, const float* host_data, float* data_staging, const int* time_step_len, int N, int W,
                                  float* logits_out, void* workspace, size_t workspace_bytes, int chunks, crnn_stream_t stream,
                                  crnn_stream_t copy_stream) {
-  return forward_host(m, host_data, data_staging, false, time_step_len, N, W, logits_out, workspace, workspace_bytes, chunks, stream,
-                      copy_stream);
+  if (!host_data || !data_staging) return crnn_fail(CRNN_INVALID_VALUE, "forward_host: null pointer");
+  return forward(m, host_batch(host_data, nullptr, data_staging, false, chunks, 1, copy_stream), time_step_len, N, W, logits_out, workspace,
+                 workspace_bytes, stream);
 }
 extern "C" int crnn_forward_host_u8(crnn_model* m, const uint8_t* host_data, uint8_t* data_staging, const int* time_step_len, int N,
                                     int W, float* logits_out, void* workspace, size_t workspace_bytes, int chunks, crnn_stream_t stream,
                                     crnn_stream_t copy_stream) {
   CRNN_TRY(check_u8_aligned(data_staging, "forward_host_u8"));
-  return forward_host(m, host_data, data_staging, true, time_step_len, N, W, logits_out, workspace, workspace_bytes, chunks, stream,
-                      copy_stream);
+  if (!host_data || !data_staging) return crnn_fail(CRNN_INVALID_VALUE, "forward_host: null pointer");
+  return forward(m, host_batch(host_data, nullptr, data_staging, true, chunks, 1, copy_stream), time_step_len, N, W, logits_out, workspace,
+                 workspace_bytes, stream);
+}
+
+extern "C" int crnn_forward_pageable(crnn_model* m, const float* pageable_data, float* pinned_staging, float* data_staging,
+                                     const int* time_step_len, int N, int W, float* logits_out, void* workspace, size_t workspace_bytes,
+                                     int chunks, int host_threads, crnn_stream_t stream, crnn_stream_t copy_stream) {
+  if (!pageable_data || !pinned_staging || !data_staging) return crnn_fail(CRNN_INVALID_VALUE, "forward_pageable: null pointer");
+  return forward(m, host_batch(pinned_staging, pageable_data, data_staging, false, chunks, host_threads, copy_stream), time_step_len, N, W,
+                 logits_out, workspace, workspace_bytes, stream);
+}
+extern "C" int crnn_forward_pageable_u8(crnn_model* m, const uint8_t* pageable_data, uint8_t* pinned_staging, uint8_t* data_staging,
+                                        const int* time_step_len, int N, int W, float* logits_out, void* workspace, size_t workspace_bytes,
+                                        int chunks, int host_threads, crnn_stream_t stream, crnn_stream_t copy_stream) {
+  CRNN_TRY(check_u8_aligned(data_staging, "forward_pageable_u8"));
+  if (!pageable_data || !pinned_staging || !data_staging) return crnn_fail(CRNN_INVALID_VALUE, "forward_pageable: null pointer");
+  return forward(m, host_batch(pinned_staging, pageable_data, data_staging, true, chunks, host_threads, copy_stream), time_step_len, N, W,
+                 logits_out, workspace, workspace_bytes, stream);
+}
+
+extern "C" int crnn_host_copy(void* dst, const void* src, size_t bytes, int threads) {
+  if ((!dst || !src) && bytes) return crnn_fail(CRNN_INVALID_VALUE, "host_copy: null pointer");
+  CopyPool::get().copy(dst, src, bytes, threads < 1 ? 1 : threads);
+  return CRNN_OK;
 }
 
 // ---- fp8 (compute_dtype 4) scales
-static int calibrate_fp8(crnn_model* m, const void* data, bool u8, const int* time_step_len, int N, int W, void* workspace,
-                         size_t workspace_bytes, crnn_stream_t stream) {
+static int check_calibrate(const crnn_model* m) {
   if (!m) return crnn_fail(CRNN_INVALID_VALUE, "calibrate_fp8: null model");
   if (m->cfg.compute_dtype != 4) return crnn_fail(CRNN_UNSUPPORTED, "calibrate_fp8: the model is not an fp8 model (compute_dtype 4)");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return forward_impl(m, data, nullptr, time_step_len, N, W, nullptr, workspace, workspace_bytes, 1, st, st, nullptr, 1, nullptr, FWD_CALIB,
-                      u8);
+  return CRNN_OK;
 }
 extern "C" int crnn_model_calibrate_fp8(crnn_model* m, const float* data, const int* time_step_len, int N, int W, void* workspace,
                                         size_t workspace_bytes, crnn_stream_t stream) {
-  return calibrate_fp8(m, data, false, time_step_len, N, W, workspace, workspace_bytes, stream);
+  CRNN_TRY(check_calibrate(m));
+  FwdCall a = device_batch(data, false);
+  a.calib = true;
+  return forward(m, a, time_step_len, N, W, nullptr, workspace, workspace_bytes, stream);
 }
 extern "C" int crnn_model_calibrate_fp8_u8(crnn_model* m, const uint8_t* data, const int* time_step_len, int N, int W, void* workspace,
                                            size_t workspace_bytes, crnn_stream_t stream) {
   CRNN_TRY(check_u8_aligned(data, "calibrate_fp8_u8"));
-  return calibrate_fp8(m, data, true, time_step_len, N, W, workspace, workspace_bytes, stream);
+  CRNN_TRY(check_calibrate(m));
+  FwdCall a = device_batch(data, true);
+  a.calib = true;
+  return forward(m, a, time_step_len, N, W, nullptr, workspace, workspace_bytes, stream);
 }
 extern "C" int crnn_model_get_fp8_scales(crnn_model* m, float* scales_host) {
   if (!m || !scales_host) return crnn_fail(CRNN_INVALID_VALUE, "get_fp8_scales: null");
@@ -988,21 +965,20 @@ extern "C" int crnn_model_set_fp8_scales(crnn_model* m, const float* scales_host
   return fp8_set_scales(m, scales_host);
 }
 
-// packed evaluation: the inference plan, then line widths [N] i32, per-line statistics [2][N][2][512] f64, coefficients [2][N][4][512] f32;
-// with moving statistics no per-line statistics or coefficients exist
+// packed evaluation: the inference plan with its packed-line region (layout_plan)
 extern "C" int crnn_lines_workspace_size(const crnn_model* m, int N, int W, size_t* bytes) {
   if (!m || !bytes) return crnn_fail(CRNN_INVALID_VALUE, "lines_workspace_size: null");
   if (N <= 0 || W < 8 || (W % 4) != 0) return crnn_fail(CRNN_INVALID_VALUE, "lines_workspace_size: need N>0, W>=8, W%%4==0");
   if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3)
     return crnn_fail(CRNN_UNSUPPORTED, "lines_workspace_size: packed evaluation runs on the bf16 and fp8 paths (compute_dtype 1, 4)");
   Plan pl;
-  *bytes = layout_plan(pl, N, W, nullptr, false) + align_up((size_t)N * 4);
-  if (!m->bn_use_moving) *bytes += align_up((size_t)2 * N * 2 * 512 * 8) + align_up((size_t)2 * N * 4 * 512 * 4);
+  *bytes = layout_plan(pl, N, W, nullptr, false, true, m->bn_use_moving);
   return CRNN_OK;
 }
 
-static int forward_lines(crnn_model* m, const void* data, bool u8, const int* line_width, const int* time_step_len, int N, int W,
-                         float* logits_out, void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
+// the checks of a packed batch, before the forward's own
+static int check_lines(crnn_model* m, const void* data, const int* line_width, const int* time_step_len, int N, int W, const float* logits_out,
+                       const void* workspace, size_t workspace_bytes) {
   if (!m || !data || !line_width || !time_step_len || !logits_out || !workspace) return crnn_fail(CRNN_INVALID_VALUE, "forward_lines: null pointer");
   if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3)
     return crnn_fail(CRNN_UNSUPPORTED, "forward_lines: packed evaluation runs on the bf16 and fp8 paths (compute_dtype 1, 4)");
@@ -1011,46 +987,22 @@ static int forward_lines(crnn_model* m, const void* data, bool u8, const int* li
   size_t need = 0;
   CRNN_TRY(crnn_lines_workspace_size(m, N, W, &need));
   if (workspace_bytes < need) return crnn_fail(CRNN_WORKSPACE_TOO_SMALL, "forward_lines: workspace %zu < %zu", workspace_bytes, need);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return forward_impl(m, data, nullptr, time_step_len, N, W, logits_out, workspace, workspace_bytes, 1, st, st, nullptr, 1, line_width,
-                      fwd_prec(m), u8);
+  return CRNN_OK;
 }
 extern "C" int crnn_forward_lines(crnn_model* m, const float* data, const int* line_width, const int* time_step_len, int N, int W,
                                   float* logits_out, void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
-  return forward_lines(m, data, false, line_width, time_step_len, N, W, logits_out, workspace, workspace_bytes, stream);
+  CRNN_TRY(check_lines(m, data, line_width, time_step_len, N, W, logits_out, workspace, workspace_bytes));
+  FwdCall a = device_batch(data, false);
+  a.line_width = line_width;
+  return forward(m, a, time_step_len, N, W, logits_out, workspace, workspace_bytes, stream);
 }
 extern "C" int crnn_forward_lines_u8(crnn_model* m, const uint8_t* data, const int* line_width, const int* time_step_len, int N, int W,
                                      float* logits_out, void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
   CRNN_TRY(check_u8_aligned(data, "forward_lines_u8"));
-  return forward_lines(m, data, true, line_width, time_step_len, N, W, logits_out, workspace, workspace_bytes, stream);
-}
-
-extern "C" int crnn_host_copy(void* dst, const void* src, size_t bytes, int threads) {
-  if ((!dst || !src) && bytes) return crnn_fail(CRNN_INVALID_VALUE, "host_copy: null pointer");
-  CopyPool::get().copy(dst, src, bytes, threads < 1 ? 1 : threads);
-  return CRNN_OK;
-}
-
-static int forward_pageable(crnn_model* m, const void* pageable_data, void* pinned_staging, void* data_staging, bool u8,
-                            const int* time_step_len, int N, int W, float* logits_out, void* workspace, size_t workspace_bytes, int chunks,
-                            int host_threads, crnn_stream_t stream, crnn_stream_t copy_stream) {
-  if (!pageable_data || !pinned_staging || !data_staging) return crnn_fail(CRNN_INVALID_VALUE, "forward_pageable: null pointer");
-  return forward_impl(m, data_staging, pinned_staging, time_step_len, N, W, logits_out, workspace, workspace_bytes, chunks,
-                      reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<cudaStream_t>(copy_stream), pageable_data,
-                      host_threads < 1 ? 1 : host_threads, nullptr, fwd_prec(m), u8);
-}
-extern "C" int crnn_forward_pageable(crnn_model* m, const float* pageable_data, float* pinned_staging, float* data_staging,
-                                     const int* time_step_len, int N, int W, float* logits_out, void* workspace, size_t workspace_bytes,
-                                     int chunks, int host_threads, crnn_stream_t stream, crnn_stream_t copy_stream) {
-  return forward_pageable(m, pageable_data, pinned_staging, data_staging, false, time_step_len, N, W, logits_out, workspace,
-                          workspace_bytes, chunks, host_threads, stream, copy_stream);
-}
-extern "C" int crnn_forward_pageable_u8(crnn_model* m, const uint8_t* pageable_data, uint8_t* pinned_staging, uint8_t* data_staging,
-                                        const int* time_step_len, int N, int W, float* logits_out, void* workspace, size_t workspace_bytes,
-                                        int chunks, int host_threads, crnn_stream_t stream, crnn_stream_t copy_stream) {
-  CRNN_TRY(check_u8_aligned(data_staging, "forward_pageable_u8"));
-  return forward_pageable(m, pageable_data, pinned_staging, data_staging, true, time_step_len, N, W, logits_out, workspace,
-                          workspace_bytes, chunks, host_threads, stream, copy_stream);
+  CRNN_TRY(check_lines(m, data, line_width, time_step_len, N, W, logits_out, workspace, workspace_bytes));
+  FwdCall a = device_batch(data, true);
+  a.line_width = line_width;
+  return forward(m, a, time_step_len, N, W, logits_out, workspace, workspace_bytes, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ profiling

@@ -51,11 +51,12 @@ struct Plan {
   __nv_bfloat16 *a1, *a2, *a3, *a3p, *a4a_pre, *a4a, *a4b_pre, *a4b, *a5, *xproj, *lstm_out, *h_state;
   double* stats;        // [2 layers][2][512]
   float* bn;            // [2 layers][4][512]: scale, shift, mean, invstd
-  // packed evaluation (crnn_forward_lines), past the inference layout; line_w == nullptr after any other forward
+  // packed evaluation (crnn_forward_lines), past the inference layout; line_w == nullptr after any other forward, stats_l / bn_l ==
+  // nullptr also under moving statistics
   int* line_w = nullptr;      // [N] clamped line widths
   bool moving = false;        // the last forward normalised conv4_x with the moving statistics (no a4x_pre, bn or stats written)
-  double* stats_l;            // [2 layers][N][2][512]
-  float* bn_l;                // [2 layers][N][4][512]
+  double* stats_l = nullptr;  // [2 layers][N][2][512]
+  float* bn_l = nullptr;      // [2 layers][N][4][512]
   CUtensorMap tA_c2s;   // conv2 input through 128-position boxes regardless of H (swapped-operand kernel, conv_swap.cuh)
   CUtensorMap tA_c31, tA_c32, tA_c41, tA_c42, tA_c5, tA_x, tA_l;
   // output maps of the register-side GEMM epilogues (gemm::frag_epi) where no input map above has the producing layer's tile
@@ -182,7 +183,7 @@ int dp_allreduce_1024(crnn_model* m, const double* in, double* out, cudaStream_t
 int dp_allreduce_bn_finalize(crnn_model* m, double* stats, double count_global, const float* gamma, const float* beta, float eps,
                              float* bn /*scale, shift, mean, invstd: [4][512]*/, cudaStream_t st);
 
-size_t layout_plan(Plan& pl, int N, int W, uint8_t* base, bool train);
+size_t layout_plan(Plan& pl, int N, int W, uint8_t* base, bool train, bool lines = false, bool moving = false);
 int prepare_weights(crnn_model* m, cudaStream_t st);
 int ensure_plan(crnn_model* m, int N, int W, void* ws, cudaStream_t st);
 int bn_fold_moving(crnn_model* m, bool* refolded, cudaStream_t st);

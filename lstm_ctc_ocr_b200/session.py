@@ -431,42 +431,8 @@ class Session(object):
         has_train = any(k == "train_op" for k in kinds)
         if not has_train:
             self._stage_ahead()                # everything of this step is enqueued: start the next batch's copy before waiting for results
-        out = []
-        self.d2h_bytes = 0
-        for f in flist:
-            k = f.kind
-            if k == "loss":
-                v = loss.cpu().numpy()[0]
-            elif k == "ctc_costs":
-                v = costs.cpu().numpy()
-            elif k == "ctc_grad":
-                v = grad.cpu().numpy()
-            elif k == "logits":
-                v = logits.cpu().numpy()
-            elif k == "dense_decoded":
-                v = self._decode(logits, d_tsl)
-            elif k == "read_alignment":
-                v = self._read_alignment(logits, d_tsl)
-            elif k == "label_alignment":
-                v = self._label_alignment(logits, d_tsl, d_lab, d_ll, llen)
-            elif k == "lexicon_decoded":
-                v = self._lexicon_decoded(logits, d_tsl)
-            elif k == "train_op":
-                v = f.step_fn(eng, logits, grad, d_data, d_tsl)
-                self._stage_ahead()
-            elif k.startswith("layer:"):
-                name = k.split(":", 1)[1]
-                tapname = {"pool1": "conv1", "pool2": "conv3_2", "pool3": "conv4_2", "reshaped_layer": "conv5"}.get(name, name)
-                v = eng.tap(tapname, data.shape[0], data.shape[1]).cpu().numpy()
-            else:
-                raise ValueError(f"unknown fetch {f}")
-            if isinstance(v, np.ndarray):
-                self.d2h_bytes += v.nbytes
-            elif isinstance(v, dict):
-                self.d2h_bytes += sum(a.nbytes for a in v.values())
-            elif isinstance(v, (np.floating, float)):
-                self.d2h_bytes += 4
-            out.append(v)
+        out = self._fetch(flist, eng, logits, d_tsl, data.shape[0], data.shape[1], loss, costs, grad, d_lab, d_ll, llen,
+                          train=lambda f: f.step_fn(eng, logits, grad, d_data, d_tsl))
         if used_ahead is not None:
             ev = self._ahead_free[used_ahead]
             if ev is None:
@@ -562,8 +528,17 @@ class Session(object):
                                           grad_scale=1.0 / N, max_label_len=int(llen.max()) if llen.size else 0,
                                           workspace="auto")
             loss = eng.total_loss(costs)
+        out = self._fetch(flist, eng, logits, d_tsl, N, W, loss, costs, grad, d_ints.get("labels"), d_ints.get("llen"), llen)
+        self._pinned.wait_pending()
+        return out[0] if single else out
+
+    def _fetch(self, flist, eng, logits, d_tsl, N, W, loss, costs, grad, d_lab, d_ll, llen, train=None):
+        """The values of the fetches, counting the bytes they bring to the host in d2h_bytes.  `train(f)` runs a train_op fetch (the
+        whole-batch path only: packed feeds refuse it)."""
         out = []
-        for k in kinds:
+        self.d2h_bytes = 0
+        for f in flist:
+            k = f.kind
             if k == "loss":
                 v = loss.cpu().numpy()[0]
             elif k == "ctc_costs":
@@ -577,20 +552,26 @@ class Session(object):
             elif k == "read_alignment":
                 v = self._read_alignment(logits, d_tsl)
             elif k == "label_alignment":
-                v = self._label_alignment(logits, d_tsl, d_ints["labels"], d_ints["llen"], llen)
+                v = self._label_alignment(logits, d_tsl, d_lab, d_ll, llen)
             elif k == "lexicon_decoded":
                 v = self._lexicon_decoded(logits, d_tsl)
+            elif k == "train_op" and train is not None:
+                v = train(f)
+                self._stage_ahead()
             elif k.startswith("layer:"):
                 name = k.split(":", 1)[1]
                 tapname = {"pool1": "conv1", "pool2": "conv3_2", "pool3": "conv4_2", "reshaped_layer": "conv5"}.get(name, name)
                 v = eng.tap(tapname, N, W).cpu().numpy()
             else:
-                raise ValueError(f"unknown fetch kind {k!r}")
+                raise ValueError(f"unknown fetch {f}")
+            if isinstance(v, np.ndarray):
+                self.d2h_bytes += v.nbytes
+            elif isinstance(v, dict):
+                self.d2h_bytes += sum(a.nbytes for a in v.values())
+            elif isinstance(v, (np.floating, float)):
+                self.d2h_bytes += 4
             out.append(v)
-        self.d2h_bytes = sum(v.nbytes if isinstance(v, np.ndarray) else sum(a.nbytes for a in v.values()) if isinstance(v, dict) else 4
-                             for v in out)
-        self._pinned.wait_pending()
-        return out[0] if single else out
+        return out
 
     @staticmethod
     def _decode_device(logits, d_tsl):

@@ -175,6 +175,47 @@ int crnn_ctc_lexicon_score(const float* logits, const int* input_len, int T, int
 int crnn_resize_lines_u8(const uint8_t* src, const int64_t* src_offset, const int* src_h, const int* src_w, const int* out_w, int N,
                          int W, int max_h, uint8_t* out, crnn_stream_t stream);
 
+/* Training lines rendered on the device.  Replaces the host generator (lib/lstm/utils/gen.py render_line + groupBatch, the
+ * reference's gen.py:31-110): a batch's random layout, its glyphs composited with Pillow's blend arithmetic into 60-row
+ * canvases, and the Pillow BILINEAR resize of crnn_resize_lines_u8 into the [N, W, 32] uint8 batch groupBatch(..., uint8)
+ * builds.  Every pixel equals what Pillow draws (ImageDraw's draw_bitmap of each glyph mask) and resizes for the layout the
+ * call reports.
+ *
+ * Glyph atlas (built on the host from one PIL font, lstm_ctc_ocr_b200.engine.GlyphAtlas): glyphs [nglyphs][8] i32 rows
+ *   (advance int(getlength), mask width w, mask height h, offset ox, offset oy, byte offset of the mask in `masks`, 0, 0);
+ *   masks: each glyph's w x h anti-aliased mask (getmask2(ch, "L", anchor="la")), row-major.  Charset index c is label id c + 1.
+ *
+ * crnn_render_layout: the layouts of lines 0 .. N-1 of the stream `seed`, from Philox4x64-10 with key (seed, 0x43524e4e52454e44)
+ * and counter (line, attempt, block, 0).  An integer in [a, b] is a + ((u * (b - a + 1)) >> 64) of one 64-bit word u; its bias
+ * is below 2^-57.  Words: block 0 gives the length U[min_len, max_len] (w0), the background U[180, 255] (w1) and x0 U[2, 12]
+ * (w2); block 1 + j gives glyph j's charset index U[0, nglyphs-1] (w0), y U[0, 10] (w1), fill U[0, 90] (w2) and advance
+ * jitter dx U[-2, 3] (w3).  Glyph j is drawn at x_j (x_0 = x0, x_{j+1} = x_j + advance_j + dx_j), y_j on a canvas of 60 rows and
+ * sum(advance) + 28 columns; nw = (int)(32.0 / 60 * canvas_w) in double, time_step = nw / 4 - 1.  nw_hi > 0 makes the stream
+ * bucketed: line i is redrawn with attempt + 1 until nw_lo < nw <= nw_hi, at most 256 attempts; nw_hi = 0: no bucket.
+ *   layout  [N][8 + 4 * max_len] i32: length, background, x0, canvas width, nw, time_step, flat label offset, attempt, then
+ *           label ids [max_len], x [max_len], y [max_len], fill [max_len] (entries past the length are unspecified)
+ *   feeds   [4 + 2N + N * max_len] i32: [0] lines that found no width in the bucket within 256 attempts (0 = every line fits),
+ *           [1] max nw, [2] labels in total, [3] padded width (nw_hi, else max(8, max nw rounded up to 4)), then label_len [N],
+ *           time_step [N] and the flat labels (label ids 1 .. nglyphs).  One copy of it gives every integer feed of the batch.
+ * CRNN_INVALID_VALUE for a null pointer, N <= 0, min_len < 1 or max_len < min_len, nglyphs outside [1, 62], or a bucket with
+ * nw_hi < 8, nw_hi % 4 != 0 or nw_lo outside [0, nw_hi); CRNN_UNSUPPORTED for max_len > 256.
+ *
+ * crnn_render_lines_u8: the batch of `layout` (crnn_render_layout's output for N lines of max_len): each canvas filled with its
+ * background, then glyph j's mask blended in draw order at (x_j + ox, y_j + oy), clipped to the canvas on every side, as Pillow's
+ * fill_mask_L does: out = DIV255(out * (255 - m) + fill * m), DIV255(v) = (((v + 128) >> 8) + v + 128) >> 8.  The canvases are
+ * then resized to nw x 32 and written to out [N, W, 32] u8 (4-byte aligned) exactly as crnn_resize_lines_u8 writes, columns nw
+ * .. W-1 zero.  W: the padded width (feeds[3]), a multiple of 4 and >= 8.  max_adv bounds every advance of the atlas and sizes
+ * the canvases: workspace (256-byte aligned) of crnn_render_workspace_size(N, max_len, max_adv) bytes.  A record whose canvas
+ * does not fit that bound gets an all-zero slot.
+ * CRNN_INVALID_VALUE for a null pointer, N <= 0, max_len < 1, max_adv < 1, a bad W or a misaligned out / workspace;
+ * CRNN_UNSUPPORTED for max_len > 256 or widths beyond the launch grid; CRNN_WORKSPACE_TOO_SMALL.  Every pointer is a device
+ * pointer; asynchronous on `stream`, no allocation, the same bits on every run; a failing call leaves the outputs untouched. */
+int crnn_render_layout(int64_t seed, int N, int min_len, int max_len, int nw_lo, int nw_hi, const int* glyphs, int nglyphs,
+                       int* layout, int* feeds, crnn_stream_t stream);
+int crnn_render_workspace_size(int N, int max_len, int max_adv, size_t* bytes);
+int crnn_render_lines_u8(const int* layout, int N, int max_len, const int* glyphs, const uint8_t* masks, int max_adv, int W,
+                         void* workspace, size_t workspace_bytes, uint8_t* out, crnn_stream_t stream);
+
 /* Greedy decode.  Replaces tf.nn.ctc_*_decoder(merge_repeated=True) + sparse_tensor_to_dense
  * at lib/networks/network.py:656-657 and the zero stripping of lib/lstm/utils/training.py:32:
  * per frame argmax (lowest index on ties) for t < input_len; emit iff != tf_blank and != the

@@ -22,6 +22,7 @@
 //    from it in the store loop)
 // Columns from out_w[i] to W are written as zero, so the batch needs no memset.
 #include "common.cuh"
+#include "resize.h"
 #include <stdint.h>
 
 namespace {
@@ -177,6 +178,17 @@ resize_lines_u8_kernel(const uint8_t* __restrict__ src, const int64_t* __restric
 
 }  // namespace
 
+int resize_lines_u8_launch(const uint8_t* src, const int64_t* src_offset, const int* src_h, const int* src_w, const int* out_w,
+                           int N, int W, int max_h, uint8_t* out, cudaStream_t stream) {
+  const int tiles = (W + RS_TILE - 1) / RS_TILE;
+  const size_t smem = rs_smem_bytes(max_h);
+  if (smem > 48 * 1024)
+    CUDA_TRY(cudaFuncSetAttribute(resize_lines_u8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  resize_lines_u8_kernel<<<dim3(N, tiles), RS_THREADS, smem, stream>>>(src, src_offset, src_h, src_w, out_w, W, max_h, out);
+  CUDA_TRY(cudaGetLastError());
+  return CRNN_OK;
+}
+
 extern "C" int crnn_resize_lines_u8(const uint8_t* src, const int64_t* src_offset, const int* src_h, const int* src_w,
                                     const int* out_w, int N, int W, int max_h, uint8_t* out, crnn_stream_t stream) {
   if (!src || !src_offset || !src_h || !src_w || !out_w || !out) return crnn_fail(CRNN_INVALID_VALUE, "resize_lines_u8: null pointer");
@@ -184,13 +196,7 @@ extern "C" int crnn_resize_lines_u8(const uint8_t* src, const int64_t* src_offse
   if (max_h < 1 || max_h > RS_MAX_H)
     return crnn_fail(CRNN_INVALID_VALUE, "resize_lines_u8: max_h = %d outside [1, %d]", max_h, RS_MAX_H);
   if (reinterpret_cast<uintptr_t>(out) & 3) return crnn_fail(CRNN_INVALID_VALUE, "resize_lines_u8: out must be 4-byte aligned");
-  const int tiles = (W + RS_TILE - 1) / RS_TILE;
-  if (tiles > 65535) return crnn_fail(CRNN_UNSUPPORTED, "resize_lines_u8: W = %d is beyond the kernel (<= %d)", W, 65535 * RS_TILE);
-  const size_t smem = rs_smem_bytes(max_h);
-  if (smem > 48 * 1024)
-    CUDA_TRY(cudaFuncSetAttribute(resize_lines_u8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  resize_lines_u8_kernel<<<dim3(N, tiles), RS_THREADS, smem, reinterpret_cast<cudaStream_t>(stream)>>>(src, src_offset, src_h, src_w,
-                                                                                                    out_w, W, max_h, out);
-  CUDA_TRY(cudaGetLastError());
-  return CRNN_OK;
+  if ((W + RS_TILE - 1) / RS_TILE > 65535)
+    return crnn_fail(CRNN_UNSUPPORTED, "resize_lines_u8: W = %d is beyond the kernel (<= %d)", W, 65535 * RS_TILE);
+  return resize_lines_u8_launch(src, src_offset, src_h, src_w, out_w, N, W, max_h, out, reinterpret_cast<cudaStream_t>(stream));
 }

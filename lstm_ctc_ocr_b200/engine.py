@@ -731,6 +731,96 @@ def resize_lines_u8(src, src_offset, src_h, src_w, out_w, W, max_h, out=None):
     return out
 
 
+class GlyphAtlas(object):
+    """A PIL font's glyphs on the device for crnn_render_lines_u8: ``glyphs`` [n, 8] i32 (advance, mask w, h, offset ox, oy, mask
+    byte offset) and ``masks`` u8, from gen.glyph_atlas (which refuses a font whose cached glyph path does not reproduce
+    ImageDraw.text).  ``charset``: cfg.CHARSET by default; charset index c is label id c + 1."""
+
+    def __init__(self, font, charset=None, device="cuda"):
+        from .lib.lstm.utils import gen
+        glyphs, masks = gen.glyph_atlas(font, charset)
+        self.nglyphs = glyphs.shape[0]
+        self.max_adv = int(glyphs[:, 0].max())
+        self.glyphs = torch.tensor(glyphs, device=device)
+        self.masks = torch.tensor(masks, device=device)
+
+
+def render_record_ints(max_len):
+    """i32 entries of one line's layout record (include/crnn_ctc.h crnn_render_layout)."""
+    return 8 + 4 * int(max_len)
+
+
+def render_feed_ints(N, max_len):
+    """i32 entries of crnn_render_layout's `feeds` for N lines of at most max_len characters."""
+    return 4 + 2 * int(N) + int(N) * int(max_len)
+
+
+def render_workspace_bytes(N, max_len, max_adv):
+    """Bytes of device workspace crnn_render_lines_u8 needs for N lines of at most max_len glyphs of advance <= max_adv."""
+    nbytes = _lib.c_size_t()
+    check(_lib.load().crnn_render_workspace_size(int(N), int(max_len), int(max_adv), nbytes))
+    return int(nbytes.value)
+
+
+def _render_buf(t, shape, dtype, what):
+    if not (torch.is_tensor(t) and t.is_cuda and t.dtype == dtype and t.is_contiguous() and tuple(t.shape) == tuple(shape)):
+        raise CrnnError(f"{what} must be a contiguous {list(shape)} {dtype} cuda tensor")
+
+
+def render_layout(seed, min_len, max_len, nw_lo, nw_hi, atlas, layout=None, feeds=None, N=None):
+    """Layouts of one batch of the device line stream (crnn_render_layout) on the current stream: lines of min_len .. max_len
+    characters of ``atlas``'s charset, seed ``seed`` (gen.batch_seed), bucket nw_lo < nw <= nw_hi (nw_hi 0: none).  Returns the
+    device (layout [N, render_record_ints(max_len)], feeds [render_feed_ints(N, max_len)]) i32, written into the given tensors
+    when they are passed (N from layout)."""
+    if layout is None:
+        layout = torch.empty((int(N), render_record_ints(max_len)), dtype=torch.int32, device=atlas.glyphs.device)
+    N = layout.shape[0]
+    if feeds is None:
+        feeds = torch.empty(render_feed_ints(N, max_len), dtype=torch.int32, device=layout.device)
+    _render_buf(layout, (N, render_record_ints(max_len)), torch.int32, "render_layout: layout")
+    _render_buf(feeds, (render_feed_ints(N, max_len),), torch.int32, "render_layout: feeds")
+    s = int(seed) & (2 ** 64 - 1)
+    s = s - 2 ** 64 if s >= 2 ** 63 else s                  # the seed's 64 bits as the ABI's int64_t
+    check(_lib.load().crnn_render_layout(s, N, int(min_len), int(max_len), int(nw_lo), int(nw_hi), atlas.glyphs.data_ptr(),
+                                         atlas.nglyphs, layout.data_ptr(), feeds.data_ptr(), _stream()))
+    return layout, feeds
+
+
+def render_lines_u8(layout, max_len, atlas, W, workspace=None, out=None):
+    """The [N, W, 32] uint8 batch of a device layout (crnn_render_lines_u8) on the current stream: glyphs of ``atlas``
+    composited as Pillow's draw_bitmap blends them, then Pillow's BILINEAR resize, byte for byte.  W: the padded width (feeds[3]
+    of render_layout).  workspace: u8 cuda tensor of render_workspace_bytes(N, max_len, atlas.max_adv) bytes, or None."""
+    N = layout.shape[0]
+    _render_buf(layout, (N, render_record_ints(max_len)), torch.int32, "render_lines_u8: layout")
+    need = render_workspace_bytes(N, max_len, atlas.max_adv)
+    if workspace is None:
+        workspace = torch.empty(need, dtype=torch.uint8, device=layout.device)
+    if out is None:
+        out = torch.empty((N, int(W), 32), dtype=torch.uint8, device=layout.device)
+    _render_buf(out, (N, int(W), 32), torch.uint8, "render_lines_u8: out")
+    if not (torch.is_tensor(workspace) and workspace.is_cuda):
+        raise CrnnError("render_lines_u8: workspace must be a cuda tensor")
+    check(_lib.load().crnn_render_lines_u8(layout.data_ptr(), N, int(max_len), atlas.glyphs.data_ptr(), atlas.masks.data_ptr(),
+                                           atlas.max_adv, int(W), workspace.data_ptr(), workspace.numel() * workspace.element_size(),
+                                           out.data_ptr(), _stream()))
+    return out
+
+
+def render_layout_dict(layout, feeds):
+    """A device layout and its feeds as host arrays laid out like gen.philox_layout's dict (chars, x, y, fill past each length
+    zeroed; dx is not recorded)."""
+    lay, f = layout.cpu().numpy().astype(np.int64), feeds.cpu().numpy()
+    N, L = lay.shape[0], (lay.shape[1] - 8) // 4
+    ln = lay[:, 0]
+    live = np.arange(L)[None, :] < ln[:, None]
+    d = {k: lay[:, c] for c, k in enumerate(("len", "bg", "x0", "canvas_w", "nw", "tsl", "label_off", "attempt"))}
+    for j, k in enumerate(("chars", "x", "y", "fill")):
+        d[k] = np.where(live, lay[:, 8 + j * L:8 + (j + 1) * L], 0)
+    d.update(status=int(f[0]), max_nw=int(f[1]), W=int(f[3]), label_len=f[4:4 + N].copy(), time_steps=f[4 + N:4 + 2 * N].copy(),
+             labels=f[4 + 2 * N:4 + 2 * N + int(f[2])].copy(), max_len=L)
+    return d
+
+
 def ctc_greedy(logits, input_len, tf_blank=TF_BLANK, strip=0):
     """Returns (out [N,T] i32 zero padded, out_len [N] i32) on device."""
     lib = _lib.load()

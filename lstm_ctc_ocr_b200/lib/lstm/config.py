@@ -40,6 +40,10 @@ _DEFAULTS = {
     # as 8-bit pixels and feeds them through the networks' data_u8 placeholder -- a quarter of the host and PCIe bytes, the same
     # values on the device (x = u / 255 in f32); "float32" feeds data as the reference does
     "FEED_DTYPE": "float32",
+    # not in the reference: where train_model's default training and validation batches are rendered -- "host" (PIL in producer
+    # processes, gen.get_batch) or "device" (gen.DeviceLineRenderer: the same layouts drawn and resized on the GPU, byte for byte
+    # what PIL draws for them, fed as uint8 whatever FEED_DTYPE says)
+    "RENDER": "host",
     "NET_NAME": "lstm", "EXP_DIR": "default", "LOG_DIR": "default", "RNG_SEED": 3,
     "TRAIN": {
         "SOLVER": "Adam", "TXT": "annotation_train.txt",

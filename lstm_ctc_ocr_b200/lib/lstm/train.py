@@ -55,6 +55,19 @@ class TrainOp(Fetch):
         return None
 
 
+def render_on_device(name):
+    """cfg.RENDER ("host" or "device") -> True when train_model renders its default batches on the GPU."""
+    if str(name) not in ("host", "device"):
+        raise ValueError(f"RENDER must be 'host' or 'device', got {name!r}")
+    return str(name) == "device"
+
+
+def is_device_batch(imgs):
+    """True for the pixels of a batch already on the GPU (a DeviceLineRenderer's uint8 cuda tensor)."""
+    import torch
+    return torch.is_tensor(imgs) and imgs.is_cuda
+
+
 def solver_from_cfg(train_cfg):
     """cfg.TRAIN -> (engine solver name, momentum), chosen as the reference chooses its optimizer (train.py:74-76): SOLVER 'Adam'
     -> "Adam", 'RMS' -> "RMS" (TF defaults, no config key), every other value -> "Momentum" with TRAIN.MOMENTUM.  The momentum is
@@ -125,6 +138,9 @@ class SolverWrapper(object):
         """feed_dict for one data-layer tuple (train.py:119-127); uint8 batches (cfg.FEED_DTYPE "uint8") go to data_u8."""
         imgs, flat_labels, label_len, time_steps = batch
         net = self.net
+        if is_device_batch(imgs):                         # a DeviceLineRenderer batch: uint8 on the device, fed in place
+            return {net.data_u8: imgs, net.labels: np.array(flat_labels), net.time_step_len: np.array(time_steps),
+                    net.labels_len: np.array(label_len), net.keep_prob: keep_prob}
         # a PrefetchFeeder hands out an ndarray view of a page-locked ring slot: keep it (np.array would copy it to pageable memory)
         data = imgs if isinstance(imgs, np.ndarray) and imgs.ndim == 3 else np.array(imgs)
         return {(net.data_u8 if data.dtype == np.uint8 else net.data): data, net.labels: np.array(flat_labels), net.time_step_len: np.array(time_steps),
@@ -173,6 +189,12 @@ class SolverWrapper(object):
     def train_model(self, sess, max_iters, restore=False, train_gen=None, val_gen=None):
         from ... import parallel
         dtype = feed_dtype(cfg.FEED_DTYPE)
+        on_device = render_on_device(cfg.RENDER)
+        if on_device:
+            # batches rendered on the session's GPU: the host streams' seeds and rank handling, no producer processes
+            dev = getattr(sess, "device", None)
+            train_gen = train_gen or get_batch(num_workers=0, batch_size=cfg.TRAIN.BATCH_SIZE, on_device=True, device=dev)
+            val_gen = val_gen or get_batch(num_workers=0, batch_size=cfg.VAL.BATCH_SIZE, on_device=True, device=dev)
         train_gen = train_gen or get_batch(num_workers=12, batch_size=cfg.TRAIN.BATCH_SIZE, vis=False, dtype=dtype)
         val_gen = val_gen or get_batch(num_workers=1, batch_size=cfg.VAL.BATCH_SIZE, vis=False, dtype=dtype)
         loss, dense_decoded = self.net.build_loss()

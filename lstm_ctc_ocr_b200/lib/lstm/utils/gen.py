@@ -498,22 +498,250 @@ class PrefetchFeeder(object):
             pass
 
 
+# ---- the device renderer's stream, restated on the host ------------------------------------------------------------------------
+# csrc/render.cu draws each line's layout from Philox4x64-10 with key (batch seed, RENDER_KEY1) and counter (line, attempt, block,
+# 0); the functions below are the same stream in numpy, and PIL drawing of any layout, so every device batch can be rebuilt here.
+
+RENDER_KEY1 = 0x43524E4E52454E44               # "CRNNREND"
+RENDER_MAX_ATTEMPTS = 256                      # redraws of a bucketed line before the bucket counts as unreachable
+_M32 = np.uint64(0xFFFFFFFF)
+
+
+def _mulhi64(a, b):
+    """High 64 bits of the 128-bit products of uint64 arrays a * b."""
+    a_lo, a_hi, b_lo, b_hi = a & _M32, a >> np.uint64(32), b & _M32, b >> np.uint64(32)
+    lh, hl = a_lo * b_hi, a_hi * b_lo
+    mid = ((a_lo * b_lo) >> np.uint64(32)) + (lh & _M32) + (hl & _M32)
+    return a_hi * b_hi + (lh >> np.uint64(32)) + (hl >> np.uint64(32)) + (mid >> np.uint64(32))
+
+
+def philox4x64(counter, key):
+    """Philox4x64-10 (Salmon et al., SC'11) of uint64 counters [..., 4] under key (k0, k1): the [..., 4] words of each block."""
+    c = [np.array(counter, dtype=np.uint64)[..., k] for k in range(4)]
+    k0, k1 = np.uint64(int(key[0]) & (2 ** 64 - 1)), np.uint64(int(key[1]) & (2 ** 64 - 1))
+    m0, m1 = np.uint64(0xD2E7470EE14C6C93), np.uint64(0xCA5A826395121157)
+    w0, w1 = np.uint64(0x9E3779B97F4A7C15), np.uint64(0xBB67AE8584CAA73B)
+    with np.errstate(over="ignore"):
+        for r in range(10):
+            if r:
+                k0, k1 = k0 + w0, k1 + w1
+            hi0, lo0 = _mulhi64(m0, c[0]), m0 * c[0]
+            hi1, lo1 = _mulhi64(m1, c[2]), m1 * c[2]
+            c = [hi1 ^ c[1] ^ k0, lo1, hi0 ^ c[3] ^ k1, lo0]
+    return np.stack(c, axis=-1)
+
+
+def _draw(u, a, b):
+    """a + ((u * (b - a + 1)) >> 64): integers in [a, b] from uint64 words, as the device draws them."""
+    return int(a) + _mulhi64(u, np.uint64(int(b) - int(a) + 1)).astype(np.int64)
+
+
+def _glyph_adv(font, charset):
+    g = _glyphs(font)
+    for ch in charset:
+        if ch not in g["adv"]:
+            g["adv"][ch] = int(font.getlength(ch))
+    return np.array([g["adv"][ch] for ch in charset], np.int64)
+
+
+def _render_range(bucket=None, lens=None):
+    """(min_len, max_len, nw_lo, nw_hi) of a stream: the bucket's BUCKET_CHARS and resized-width interval, else ``lens`` (or
+    cfg.MIN_LEN / cfg.MAX_LEN) and no width interval (nw_hi 0)."""
+    if bucket is not None:
+        if bucket not in BUCKET_CHARS:
+            raise ValueError(f"bucket must be one of {BUCKETS}, got {bucket!r}")
+        return BUCKET_CHARS[bucket] + (max([b for b in BUCKETS if b < bucket] or [0]), int(bucket))
+    lo, hi = lens if lens is not None else (cfg.MIN_LEN, cfg.MAX_LEN)
+    return int(lo), int(hi), 0, 0
+
+
+def philox_layout(N, seed, bucket=None, lens=None, font=None):
+    """The layouts csrc/render.cu draws for lines 0 .. N-1 of batch seed ``seed`` (batch_seed(k, seed, rank, world)), in numpy:
+    a dict of int64 arrays len, bg, x0, canvas_w, nw, tsl, attempt [N] and chars (label ids 1..62, 0 past the length), x, y,
+    fill, dx [N, max_len], plus ``status`` (lines that found no width in the bucket) and ``max_len``.  Word order and ranges as
+    include/crnn_ctc.h states them (render_line's ranges); advances from ``font`` (_font(42) by default)."""
+    font = _font(42) if font is None else font
+    adv = _glyph_adv(font, cfg.CHARSET)
+    min_len, max_len, nw_lo, nw_hi = _render_range(bucket, lens)
+    nglyphs = len(cfg.CHARSET)
+    key = (int(seed), RENDER_KEY1)
+    out = {k: np.zeros(N, np.int64) for k in ("len", "bg", "x0", "canvas_w", "nw", "tsl", "attempt")}
+    for k in ("chars", "x", "y", "fill", "dx"):
+        out[k] = np.zeros((N, max_len), np.int64)
+    pending = np.arange(N)
+    failed = np.zeros(N, bool)
+    for attempt in range(RENDER_MAX_ATTEMPTS):
+        n = pending.size
+        ctr = np.zeros((n, max_len + 1, 4), np.uint64)
+        ctr[:, :, 0] = pending[:, None]
+        ctr[:, :, 1] = attempt
+        ctr[:, :, 2] = np.arange(max_len + 1)[None, :]
+        w = philox4x64(ctr, key)
+        ln = _draw(w[:, 0, 0], min_len, max_len)
+        live = np.arange(max_len)[None, :] < ln[:, None]
+        c = _draw(w[:, 1:, 0], 0, nglyphs - 1)
+        dx = _draw(w[:, 1:, 3], -2, 3)
+        a = adv[c]
+        x0 = _draw(w[:, 0, 2], 2, 12)
+        step = np.where(live, a + dx, 0)
+        x = x0[:, None] + np.concatenate([np.zeros((n, 1), np.int64), np.cumsum(step, axis=1)[:, :-1]], axis=1)
+        cw = np.where(live, a, 0).sum(axis=1) + 28
+        nw = (cfg.IMG_HEIGHT / 60 * cw.astype(np.float64)).astype(np.int64)
+        ok = np.ones(n, bool) if nw_hi == 0 else (nw > nw_lo) & (nw <= nw_hi)
+        done = ok | (attempt + 1 == RENDER_MAX_ATTEMPTS)
+        idx = pending[done]
+        failed[idx] = ~ok[done]
+        for k, v in (("len", ln), ("bg", _draw(w[:, 0, 1], 180, 255)), ("x0", x0), ("canvas_w", cw), ("nw", nw),
+                     ("tsl", nw // cfg.POOL_SCALE + cfg.OFFSET_TIME_STEP), ("attempt", np.full(n, attempt))):
+            out[k][idx] = v[done]
+        lv = live[done]
+        for k, v in (("chars", c + 1), ("x", x), ("y", _draw(w[:, 1:, 1], 0, 10)), ("fill", _draw(w[:, 1:, 2], 0, 90)), ("dx", dx)):
+            out[k][idx] = np.where(lv, v[done], 0)
+        pending = pending[~done]
+        if pending.size == 0:
+            break
+    out["status"] = int(failed.sum())
+    out["max_len"] = max_len
+    return out
+
+
+def glyph_atlas(font, charset=None):
+    """Host side of the device glyph atlas (engine.GlyphAtlas): (glyphs [n, 8] int32 rows of advance int(getlength), mask w, h,
+    offset ox, oy, byte offset of the mask, 0, 0; masks uint8, each glyph's getmask2(ch, "L", anchor="la") bytes row-major).
+    Refused (ValueError) for a font whose cached glyph path is off (_glyphs(font)["fast"] False): then draw_bitmap of these masks
+    is not what ImageDraw.text draws, and device lines would not be the host's."""
+    g = _glyphs(font)
+    if not g["fast"]:
+        raise ValueError("this font's glyph masks do not reproduce ImageDraw.text (the cached glyph path is off): "
+                         "no device glyph atlas can be built from it")
+    charset = cfg.CHARSET if charset is None else charset
+    adv = _glyph_adv(font, charset)
+    rows, chunks, off = [], [], 0
+    for ch, a in zip(charset, adv):
+        m = g["mask"].get(ch)
+        if m is None:
+            m = g["mask"][ch] = font.getmask2(ch, "L", anchor="la", start=(0.0, 0.0))
+        mask, (ox, oy) = m
+        w, h = mask.size
+        b = np.asarray(mask, dtype=np.uint8).reshape(-1)[:w * h]
+        rows.append((int(a), w, h, int(ox), int(oy), off, 0, 0))
+        chunks.append(b)
+        off += b.size
+    return np.array(rows, np.int32), np.concatenate(chunks + [np.zeros(4, np.uint8)])
+
+
+def draw_layout_line(layout, i, font=None):
+    """Line i of a layout (philox_layout's dict, or the device's record as engine.render_layout returns it) drawn with PIL:
+    the 60-row gray canvas, each glyph through _draw_glyph (ImageDraw's draw_bitmap) in order."""
+    from PIL import Image, ImageDraw
+    font = _font(42) if font is None else font
+    g = _glyphs(font)
+    img = Image.new("L", (int(layout["canvas_w"][i]), 60), color=int(layout["bg"][i]))
+    d = ImageDraw.Draw(img)
+    for j in range(int(layout["len"][i])):
+        ch = cfg.CHARSET[int(layout["chars"][i, j]) - 1]
+        _draw_glyph(d, g, font, ch, int(layout["x"][i, j]), int(layout["y"][i, j]), int(layout["fill"][i, j]))
+    return np.asarray(img, dtype=np.uint8)
+
+
+def layout_labels(layout):
+    """The text of each line of a layout."""
+    return ["".join(cfg.CHARSET[int(c) - 1] for c in layout["chars"][i, :int(layout["len"][i])]) for i in range(len(layout["len"]))]
+
+
+def render_layout(layout, font=None, pad_to=None):
+    """A layout's batch on the host: every line drawn by draw_layout_line, then groupBatch(..., dtype=uint8, pad_to) -- what
+    the device renderer hands out for the same layout, byte for byte."""
+    imgs = [draw_layout_line(layout, i, font) for i in range(len(layout["len"]))]
+    return groupBatch(imgs, layout_labels(layout), pad_to=pad_to, dtype=np.uint8)
+
+
+class DeviceLineRenderer(object):
+    """Training batches rendered on the GPU (csrc/render.cu): iterates like get_batch and yields (uint8 cuda tensor [N, W, 32],
+    labels, label_len, time_steps), the three integer feeds as int32 numpy arrays.  Batch k is the stream
+    batch_seed(k, seed, rank, world) of philox_layout, drawn with _font(42); ``bucket`` pads to a bucket width, else lines of
+    ``lens`` = (min, max) characters (cfg.MIN_LEN / cfg.MAX_LEN) are padded to the batch max, as groupBatch pads.
+
+    The layout of batch k+1 is drawn on the renderer's own stream while batch k trains, and its integer feeds copied into
+    page-locked memory behind an event; ``next()`` waits for that event on the host (the only host sync), composites and resizes
+    batch k+1 at its width, makes the current stream wait for it on the GPU, starts the layout of batch k+2 and returns batch k+1.
+    Each handed-out tensor is recorded on the consumer's stream, so its memory is not reused while a step still reads it."""
+
+    def __init__(self, batch_size, seed=None, rank=0, world=1, bucket=None, lens=None, device=None):
+        import torch
+        from .... import engine
+        self.batch_size, self.seed, self.rank, self.world, self.bucket = int(batch_size), seed, int(rank), int(world), bucket
+        self.min_len, self.max_len, self.nw_lo, self.nw_hi = _render_range(bucket, lens)
+        self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
+        self.atlas = engine.GlyphAtlas(_font(42), device=self.device)
+        self.stream = torch.cuda.Stream(device=self.device)
+        N = self.batch_size
+        with torch.cuda.stream(self.stream):
+            self.layout = torch.empty((N, engine.render_record_ints(self.max_len)), dtype=torch.int32, device=self.device)
+            self.feeds = torch.empty(engine.render_feed_ints(N, self.max_len), dtype=torch.int32, device=self.device)
+            self.workspace = torch.empty(engine.render_workspace_bytes(N, self.max_len, self.atlas.max_adv), dtype=torch.uint8,
+                                         device=self.device)
+        self.host_feeds = torch.empty(self.feeds.numel(), dtype=torch.int32).pin_memory()
+        self.ready = torch.cuda.Event()
+        self.k = 0
+        self._launch_layout(0)
+
+    def _launch_layout(self, k):
+        import torch
+        from .... import engine
+        with torch.cuda.stream(self.stream):
+            engine.render_layout(batch_seed(k, self.seed, self.rank, self.world), self.min_len, self.max_len, self.nw_lo, self.nw_hi,
+                                 self.atlas, self.layout, self.feeds)
+            self.host_feeds.copy_(self.feeds, non_blocking=True)
+            self.ready.record(self.stream)
+
+    def __iter__(self):
+        return self
+
+    def __next__(self):
+        import torch
+        from .... import engine
+        self.ready.synchronize()                            # the layout of batch k and its integer feeds are on the host
+        f = self.host_feeds.numpy()
+        N = self.batch_size
+        if f[0]:
+            raise ValueError(f"{int(f[0])} line(s) of batch {self.k} found no width in bucket {self.bucket} "
+                             f"({self.nw_lo}, {self.nw_hi}] within {RENDER_MAX_ATTEMPTS} draws of {self.min_len} .. {self.max_len} "
+                             "characters")
+        W = int(f[3])
+        ll = f[4:4 + N].copy()
+        tsl = f[4 + N:4 + 2 * N].copy()
+        labels = f[4 + 2 * N:4 + 2 * N + int(f[2])].copy()
+        consumer = torch.cuda.current_stream(self.device)
+        with torch.cuda.stream(self.stream):
+            out = torch.empty((N, W, cfg.NUM_FEATURES), dtype=torch.uint8, device=self.device)
+            engine.render_lines_u8(self.layout, self.max_len, self.atlas, W, self.workspace, out)
+        consumer.wait_stream(self.stream)
+        out.record_stream(consumer)
+        self.k += 1
+        self._launch_layout(self.k)
+        return out, labels, ll, tsl
+
+
 def get_batch(num_workers, **kwargs):
     """Reference entry point (gen.py:112-128): ``get_batch(num_workers=12, batch_size=64, vis=False)``.  ``num_workers`` render
-    processes feed a page-locked ring (PrefetchFeeder); ``num_workers <= 1`` renders in-process."""
+    processes feed a page-locked ring (PrefetchFeeder); ``num_workers <= 1`` renders in-process.  ``on_device=True``: the lines
+    are rendered on the GPU instead (DeviceLineRenderer, uint8 cuda batches; ``num_workers``, ``render`` and ``dtype`` do not
+    apply)."""
     kwargs.pop("vis", None)
     batch_size = kwargs.pop("batch_size", 32)
     render = kwargs.pop("render", None)
-    if render is None:
-        render = can_render()
     seed = kwargs.pop("seed", None)
     rank, world = kwargs.pop("rank", None), kwargs.pop("world", None)
     if rank is None or world is None:
         rank, world = _dist_rank_world()
     bucket = kwargs.pop("bucket", None)
-    dtype = np.dtype(kwargs.pop("dtype", np.float32))         # float32 or uint8 pixels (groupBatch)
-
     lens = (cfg.MIN_LEN, cfg.MAX_LEN)          # this process's configuration (e.g. --set MIN_LEN 30 MAX_LEN 70), for the workers
+    if kwargs.pop("on_device", False):
+        return DeviceLineRenderer(batch_size, seed=seed, rank=rank, world=world, bucket=bucket, lens=lens, device=kwargs.pop("device", None))
+    if render is None:
+        render = can_render()
+    dtype = np.dtype(kwargs.pop("dtype", np.float32))         # float32 or uint8 pixels (groupBatch)
 
     def arg_fn(k):
         return dict(k=k, batch_size=batch_size, render=render, seed=seed, rank=rank, world=world, bucket=bucket, lens=lens, dtype=dtype)

@@ -334,11 +334,19 @@ class Session(object):
     @staticmethod
     def _data_feed(feeds):
         """The fed batch: `data` widened to f32 as a TF float placeholder casts it, or `data_u8` kept as uint8 pixels (the engine's
-        u8 entry points divide by 255 on the device).  Feeding both is ambiguous and refused."""
+        u8 entry points divide by 255 on the device).  Feeding both is ambiguous and refused.  `data_u8` may also be a batch
+        already on the device (gen.DeviceLineRenderer): a contiguous [N, W, 32] uint8 CUDA tensor, used in place (run checks
+        that it is on the session's device)."""
         if "data_u8" in feeds:
             if "data" in feeds:
                 raise ValueError("feed either data or data_u8, not both")
-            return np.asarray(feeds["data_u8"], dtype=np.uint8)
+            d = feeds["data_u8"]
+            if torch.is_tensor(d):
+                if not (d.is_cuda and d.dtype == torch.uint8 and d.dim() == 3 and d.is_contiguous()):
+                    raise ValueError(f"a tensor fed as data_u8 must be a contiguous [N, W, 32] uint8 CUDA tensor, got "
+                                     f"{d.dtype} {tuple(d.shape)} on {d.device}")
+                return d
+            return np.asarray(d, dtype=np.uint8)
         return np.asarray(feeds["data"], dtype=np.float32)
 
     def run(self, fetches, feed_dict=None):
@@ -375,13 +383,19 @@ class Session(object):
             return self._run_images(flist, single, eng, images, labels, llen)
         dev = self.device
         if feeds.get("line_width") is not None:
+            if torch.is_tensor(data):
+                raise ValueError("line_width (packed evaluation) takes host batches: feed data_u8 as a numpy array")
             return self._run_lines(flist, single, net, eng, data, tsl, labels, llen, np.asarray(feeds["line_width"], dtype=np.int32))
         # training mode is sticky: its forward is a superset (it also saves what the backward needs), and switching back
         # and forth would re-plan the multi-GB workspace
         if any(k == "train_op" for k in kinds) and not eng.training:
             eng.set_training(True)
-        data = np.ascontiguousarray(data)
-        ahead = self._take_ahead(data)
+        on_device = torch.is_tensor(data)
+        if on_device and data.device != dev:
+            raise ValueError(f"data_u8 is on {data.device}, the session runs on {dev}")
+        if not on_device:
+            data = np.ascontiguousarray(data)
+        ahead = self._take_ahead(data) if not on_device else None
         d_ints = None
         if ahead is not None and ahead[2] is not None:
             h, dv = ahead[2]
@@ -394,9 +408,13 @@ class Session(object):
                 ints["labels"], ints["llen"] = labels, llen
             d_ints = self._pinned.stage_ints(ints, dev)
         d_tsl = d_ints["tsl"]
-        self.h2d_bytes = data.nbytes + tsl.nbytes
+        self.h2d_bytes = (0 if on_device else data.nbytes) + tsl.nbytes
         used_ahead = None
-        if ahead is not None:
+        if on_device:
+            d_data = data
+            logits = eng.forward(d_data, d_tsl)
+            self.last_feed_path = "device-resident"
+        elif ahead is not None:
             d_data, used_ahead = ahead[0], ahead[1]
             logits = eng.forward(d_data, d_tsl)
             self.last_feed_path = "page-locked in place, copied during the previous step (device prefetch)"

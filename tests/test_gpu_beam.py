@@ -98,13 +98,18 @@ def test_device_beam_matches_host_and_oracle(kind, seed):
             assert np.isfinite(nlp).all() and nlp[1] == 0.0
 
 
-@pytest.mark.parametrize("seed", range(36))
+EDGE_C = (2, 32, 33, 34, 63)                   # the second lane slot (c = lane + 32) partly used, class masks of 31 ... 62 bits
+EDGE_WIDTHS = (31, 32, 33, 63, 64, 65, 127)     # heap depth boundaries
+
+
+@pytest.mark.parametrize("seed", range(36 + 2 * len(EDGE_C)))
 def test_device_beam_ties_and_narrow_beams(seed):
-    """Quantised logits with exact ties, all-equal frames, C in {3, 6, 17}, widths that evict constantly, both merge modes:
-    the inputs on which the visit order and the tie rules decide the result."""
+    """Quantised logits with exact ties, all-equal frames, C in {3, 6, 17} and (seeds 36 on) the edge class counts EDGE_C,
+    widths that evict constantly and the heap-depth widths EDGE_WIDTHS, both merge modes: the inputs on which the visit
+    order and the tie rules decide the result.  The oracle is compared at the narrow widths and 100."""
     from oracle import crnn_oracle as O
     rng = np.random.default_rng(100 + seed)
-    C = int(rng.choice([3, 6, 17]))
+    C = int(rng.choice([3, 6, 17])) if seed < 36 else EDGE_C[seed % len(EDGE_C)]
     T, N = int(rng.integers(4, 15)), 8
     kind = seed % 3
     if kind == 0:
@@ -117,10 +122,11 @@ def test_device_beam_ties_and_narrow_beams(seed):
     x = x.astype(np.float32)
     il = rng.integers(0, T + 1, size=N).astype(np.int32)
     il[0] = T
-    for bw in (1, 2, 3, 5, 7, 100):
+    for bw in (1, 2, 3, 5, 7, 100) + EDGE_WIDTHS:
         for merge in (True, False):
             got, _ = _both(x, il, beam_width=bw, merge_repeated=merge, strip=-1)
-            assert got == O.beam_search_decode(x, il, beam_width=bw, merge_repeated=merge, strip=-1), (C, T, bw, merge)
+            if bw not in EDGE_WIDTHS:
+                assert got == O.beam_search_decode(x, il, beam_width=bw, merge_repeated=merge, strip=-1), (C, T, bw, merge)
 
 
 def test_device_beam_reproduces_tensorflows_own_known_answer():

@@ -149,6 +149,21 @@ def test_candidates_across_the_word_boundaries():
     check_candidates("word_boundary", reads, rl, lex, (0, 1, 3, 8, -1), (1, 64, 256))
     lone = _Raw([ents[0]])
     check_candidates("one_entry", reads[2:3], rl[2:3], lone, (0, 3, -1), (1, 64))
+    # Session.run's lexicon_decoded passes dense_decoded with stride T: strides 257 ... 512 run the 8-word kernel, 513 ... 1024
+    # the 16-word one; with delta = -1 the histogram has 1025 bins at stride 1024
+    for stride in (300, 512, 513, 1024):
+        lens = [L for L in (0, 1, 64, 256, 257, 511, 512, 513, 1023, 1024) if L <= stride]
+        rows = []
+        for i in range(4 * len(lens)):
+            L = lens[i % len(lens)]
+            base = []
+            while len(base) < L:
+                base += list(ents[int(rng.integers(0, 1000))])
+            rows.append(_edit(rng, base[:L], int(rng.integers(0, 3)))[:stride] if L else [])
+        reads, rl = _dense(rows, stride)
+        rl = np.minimum(rl, stride)
+        wt = 8 if stride <= 512 else 16
+        check_candidates(f"stride{stride}_wt{wt}", reads, rl, lex, (0, 3, 8, -1), (1, 64, 256))
 
 
 def test_out_of_range_ids_match_nothing():

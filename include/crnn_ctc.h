@@ -247,6 +247,24 @@ int crnn_ctc_beam_search_device(const float* logits, const int* input_len, int T
                                 int merge_repeated, int strip, int* out, int* out_len, float* neg_log_prob,
                                 void* workspace, size_t workspace_bytes, crnn_stream_t stream);
 
+/* The n best labellings of each utterance: tf.nn.ctc_beam_search_decoder's top_paths, on the host (crnn_ctc_beam_search's
+ * pointers and threads) and on the device (crnn_ctc_beam_search_device's pointers, limits, workspace and stream rules).  The
+ * beam runs exactly as in the single-best decoders; after the last frame the entries it lists (at most beam_width, the empty
+ * prefix and entries of total -inf included) are ranked by total, highest first, exact ties broken by insertion order,
+ * earliest first (TensorFlow leaves the order of exact ties undefined).  Path 0 is therefore the single-best decoders' output,
+ * bit for bit.  Path i is entry i's labels, consecutive equal labels merged when merge_repeated is set, `strip` dropped, zero
+ * padded to T: two different prefixes can give the same labels ("a a" and "a" with merge_repeated), and both are returned.
+ * out [N, top_paths, T] i32; out_len [N, top_paths] i32; log_prob [N, top_paths] f32 or NULL: the entry's total, log P <= 0
+ * (TensorFlow's log_probability; note the sign is that of neither neg_log_prob above); num_paths [N] i32 or NULL: the paths
+ * that are real, min(top_paths, listed entries).  Paths past num_paths have length 0 and log_prob -inf (where TensorFlow fails
+ * the op).  1 <= top_paths <= beam_width, else CRNN_INVALID_VALUE. */
+int crnn_ctc_beam_search_topk(const float* logits_host, const int* input_len_host, int T, int N, int C, int beam_width,
+                              int top_paths, int merge_repeated, int strip, int* out_host, int* out_len_host,
+                              float* log_prob_host, int* num_paths_host, int num_threads);
+int crnn_ctc_beam_search_topk_device(const float* logits, const int* input_len, int T, int N, int C, int beam_width,
+                                     int top_paths, int merge_repeated, int strip, int* out, int* out_len, float* log_prob,
+                                     int* num_paths, void* workspace, size_t workspace_bytes, crnn_stream_t stream);
+
 /* 1 when `host_ptr` lies in page-locked (cudaHostAlloc / cudaHostRegister) memory, else 0.  The Python feed path uses it to
  * decide whether a fed numpy batch can be DMA'd in place (crnn_forward_host) or has to be staged. */
 int crnn_host_is_pinned(const void* host_ptr);

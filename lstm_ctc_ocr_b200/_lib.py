@@ -39,6 +39,10 @@ SIGNATURES = {
     "crnn_ctc_beam_workspace_size": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
     "crnn_ctc_beam_search_device": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                             c_void_p, c_size_t, c_void_p]),
+    "crnn_ctc_beam_search_topk": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                          c_void_p, c_void_p, c_int]),
+    "crnn_ctc_beam_search_topk_device": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                                 c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "crnn_host_is_pinned": (c_int, [c_void_p]),
     "crnn_model_create": (c_int, [ctypes.POINTER(CrnnConfig), ctypes.POINTER(c_void_p)]),
     "crnn_model_destroy": (c_int, [c_void_p]),

@@ -12,7 +12,8 @@
 // current frame; per frame (1) every entry of the beam is re-scored in place, (2) entries are expanded in descending order of
 // their previous total against the running bottom of a beam_width-bounded list, a full list evicting its bottom.  The result is
 // the label sequence of the best entry, with consecutive equal labels collapsed when merge_repeated is set (TF applies that to
-// the decoded sequence, so "a, blank, a" also comes out as one "a").
+// the decoded sequence, so "a, blank, a" also comes out as one "a").  crnn_ctc_beam_search_topk returns TopPaths' n best: the
+// listed entries by total, highest first, exact ties in insertion order.
 #include <algorithm>
 #include <atomic>
 #include <cmath>
@@ -126,8 +127,10 @@ struct Scratch {
   }
 };
 
-void decode_one(Scratch& S, const float* logits, int stride_t, int len, int C, int beam_width, int merge_repeated, int strip, int* out,
-                int max_out, int* out_len, float* log_prob) {
+// out [top_paths, max_out], out_len / score [top_paths]; `score` gets newp.total (negated when `negate`), `num_paths` the count
+// of real paths
+void decode_one(Scratch& S, const float* logits, int stride_t, int len, int C, int beam_width, int top_paths, int merge_repeated,
+                int strip, int* out, int max_out, int* out_len, float* score, int negate, int* num_paths) {
   const int blank = C - 1, nlab = C - 1;
   S.reset(C);
   std::vector<int>& kid_pool = S.kid_pool;
@@ -240,30 +243,42 @@ void decode_one(Scratch& S, const float* logits, int stride_t, int len, int C, i
       }
     }
   }
+  // TopPaths: the listed entries by total, highest first, exact ties in insertion order (the order drain leaves them in)
   leaves.drain(branches);
-  Entry* best = branches[0];
-  for (Entry* e : branches) if (e->newp.total > best->newp.total) best = e;
+  std::stable_sort(branches.begin(), branches.end(), [](const Entry* a, const Entry* b) { return a->newp.total > b->newp.total; });
+  const int paths = (int)std::min<size_t>(branches.size(), (size_t)top_paths);
   std::vector<int> seq;
-  for (Entry* e = best; e->parent != nullptr; e = e->parent) seq.push_back(e->label);
-  int n = 0, prev = -1;
-  for (auto it = seq.rbegin(); it != seq.rend(); ++it) {
-    const int l = *it;
-    const bool keep = !(merge_repeated && l == prev);
-    prev = l;
-    if (keep && l != strip && n < max_out) out[n++] = l;
+  for (int p = 0; p < top_paths; ++p) {
+    int* o = out + (size_t)p * max_out;
+    int n = 0;
+    double total = kLogZero;
+    if (p < paths) {
+      total = branches[p]->newp.total;
+      seq.clear();
+      for (Entry* e = branches[p]; e->parent != nullptr; e = e->parent) seq.push_back(e->label);
+      int prev = -1;
+      for (auto it = seq.rbegin(); it != seq.rend(); ++it) {
+        const int l = *it;
+        const bool keep = !(merge_repeated && l == prev);
+        prev = l;
+        if (keep && l != strip && n < max_out) o[n++] = l;
+      }
+    }
+    for (int i = n; i < max_out; ++i) o[i] = 0;
+    out_len[p] = n;
+    if (score) score[p] = (float)(negate ? -total : total);
   }
-  for (int i = n; i < max_out; ++i) out[i] = 0;
-  *out_len = n;
-  if (log_prob) *log_prob = (float)(-best->newp.total);
+  if (num_paths) *num_paths = paths;
 }
 
-}  // namespace
-
-extern "C" int crnn_ctc_beam_search(const float* logits_host, const int* input_len_host, int T, int N, int C, int beam_width,
-                                    int merge_repeated, int strip, int* out_host, int* out_len_host, float* neg_log_prob_host,
-                                    int num_threads) {
+// both host entry points: out [N, top_paths, T], out_len / score [N, top_paths], num_paths [N]
+int beam_search_host(const float* logits_host, const int* input_len_host, int T, int N, int C, int beam_width, int top_paths,
+                     int merge_repeated, int strip, int* out_host, int* out_len_host, float* score_host, int negate,
+                     int* num_paths_host, int num_threads) {
   if (!logits_host || !input_len_host || !out_host || !out_len_host) return crnn_fail(CRNN_INVALID_VALUE, "beam_search: null pointer");
   if (T <= 0 || N <= 0 || C < 2 || beam_width < 1) return crnn_fail(CRNN_INVALID_VALUE, "beam_search: bad shape");
+  if (top_paths < 1 || top_paths > beam_width)
+    return crnn_fail(CRNN_INVALID_VALUE, "beam_search: top_paths %d outside [1, beam_width = %d]", top_paths, beam_width);
   for (int n = 0; n < N; ++n)
     if (input_len_host[n] < 0 || input_len_host[n] > T) return crnn_fail(CRNN_INVALID_VALUE, "beam_search: input_len[%d] outside [0, T]", n);
   int nt = num_threads > 0 ? num_threads : (int)std::thread::hardware_concurrency();
@@ -274,9 +289,12 @@ extern "C" int crnn_ctc_beam_search(const float* logits_host, const int* input_l
   auto work = [&]() {
     try {
       Scratch S;
-      for (int n = next.fetch_add(1); n < N && !failed.load(std::memory_order_relaxed); n = next.fetch_add(1))
-        decode_one(S, logits_host + (size_t)n * C, N * C, input_len_host[n], C, beam_width, merge_repeated, strip,
-                   out_host + (size_t)n * T, T, out_len_host + n, neg_log_prob_host ? neg_log_prob_host + n : nullptr);
+      for (int n = next.fetch_add(1); n < N && !failed.load(std::memory_order_relaxed); n = next.fetch_add(1)) {
+        const size_t row = (size_t)n * top_paths;
+        decode_one(S, logits_host + (size_t)n * C, N * C, input_len_host[n], C, beam_width, top_paths, merge_repeated, strip,
+                   out_host + row * T, T, out_len_host + row, score_host ? score_host + row : nullptr, negate,
+                   num_paths_host ? num_paths_host + n : nullptr);
+      }
     } catch (...) {
       failed.store(true);
     }
@@ -293,4 +311,20 @@ extern "C" int crnn_ctc_beam_search(const float* logits_host, const int* input_l
   }
   if (failed.load()) return crnn_fail(CRNN_INVALID_VALUE, "beam_search: out of host memory");
   return CRNN_OK;
+}
+
+}  // namespace
+
+extern "C" int crnn_ctc_beam_search(const float* logits_host, const int* input_len_host, int T, int N, int C, int beam_width,
+                                    int merge_repeated, int strip, int* out_host, int* out_len_host, float* neg_log_prob_host,
+                                    int num_threads) {
+  return beam_search_host(logits_host, input_len_host, T, N, C, beam_width, 1, merge_repeated, strip, out_host, out_len_host,
+                          neg_log_prob_host, 1, nullptr, num_threads);
+}
+
+extern "C" int crnn_ctc_beam_search_topk(const float* logits_host, const int* input_len_host, int T, int N, int C, int beam_width,
+                                         int top_paths, int merge_repeated, int strip, int* out_host, int* out_len_host,
+                                         float* log_prob_host, int* num_paths_host, int num_threads) {
+  return beam_search_host(logits_host, input_len_host, T, N, C, beam_width, top_paths, merge_repeated, strip, out_host, out_len_host,
+                          log_prob_host, 0, num_paths_host, num_threads);
 }

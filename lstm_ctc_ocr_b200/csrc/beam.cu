@@ -1,6 +1,7 @@
 // CTC prefix beam search on the device (SURVEY §8(f)4): the algorithm of beam.cpp -- TensorFlow's CTCBeamSearchDecoder
-// (network.py:656, test.py:30: width 100, top_paths 1, blank = C-1, merge_repeated) -- for logits that are already on the
-// GPU, so that cfg.DECODER = "beam" needs no copy of the [T,N,C] logits and no host decode.
+// (network.py:656, test.py:30: width 100, top_paths 1, blank = C-1, merge_repeated; any top_paths up to the width through
+// crnn_ctc_beam_search_topk_device) -- for logits that are already on the GPU, so that cfg.DECODER = "beam" needs no copy of
+// the [T,N,C] logits and no host decode.
 //
 // One CTA of one warp per utterance.  Per frame the warp computes the log-softmax row (exp in parallel, the normaliser's sum
 // sequentially in class order, as the host does: on exactly tied frames the decode depends on its last bit) and ranks the
@@ -9,7 +10,8 @@
 //   that order (a parent sorted earlier has already been re-scored: its newp decides whether it is active); re-push them;
 //   expand them in that order, classes in ascending index, against the bottom of the width-bounded list -- the FIRST of the
 //   smallest totals in insertion order, kept in a (total, insertion number) min-heap -- evicting the bottom when full.
-// The beam (heap, branch list, lp row) lives in shared memory, the prefix tree in the workspace.
+// The beam (heap, branch list, lp row) lives in shared memory, the prefix tree in the workspace.  After the last frame the
+// whole warp ranks the listed entries and writes the top_paths best, one lane per path (finish_paths).
 //
 // Prefix identity.  A prefix that is evicted and later re-admitted must be the entry its listed children point at, so
 // entries live in a tree keyed by (parent, label).  Only listed entries, their ancestors and the entries of the current frame
@@ -252,34 +254,6 @@ struct Decoder {
     rescore(lp);
     expand(lp, lp_desc, by_lp);
   }
-
-  // best = first maximum of newp.total in insertion order; its labels (merged, `strip` dropped) zero-padded to T
-  BEAM_HD void finish(int T, int merge_repeated, int strip, int* out, int* out_len, float* neg_log_prob) {
-    int best = -1, best_seq = 0;
-    double best_total = 0.0;
-    for (int i = 0; i < hsize; ++i) {
-      const Item& it = heap[i];
-      if (nd[it.node].leaf_seq != it.seq) continue;
-      const double v = nd[it.node].nt;
-      if (best < 0 || v > best_total || (v == best_total && it.seq < best_seq)) {
-        best = it.node; best_seq = it.seq; best_total = v;
-      }
-    }
-    int depth = 0;
-    for (int e = best; nd[e].parent >= 0; e = nd[e].parent) ++depth;
-    int i = depth;
-    for (int e = best; nd[e].parent >= 0; e = nd[e].parent) out[--i] = nd[e].label;
-    int n = 0, prev = -1;
-    for (i = 0; i < depth; ++i) {
-      const int l = out[i];
-      const bool keep = !(merge_repeated && l == prev);
-      prev = l;
-      if (keep && l != strip) out[n++] = l;
-    }
-    for (i = n; i < T; ++i) out[i] = 0;
-    *out_len = n;
-    if (neg_log_prob) *neg_log_prob = (float)(-best_total);
-  }
 };
 
 // entries one utterance can hold at once (see the header comment); 0 when it does not fit an int index
@@ -288,14 +262,71 @@ size_t beam_node_cap(int T, int C, int beam_width) {
   return cap > (size_t)0x7fffffff ? 0 : cap;
 }
 
+// The warp's end of one utterance: the listed entries (the valid items of the heap's first `hsize`) ranked by (newp.total
+// descending, insertion number ascending) -- beam.cpp's drain + stable sort, so path 0 is the entry the single-best decode
+// returns -- and path p written by lane p % 32: its labels (merged, `strip` dropped) zero-padded to T in out[p], its length,
+// and newp.total as a float (negated when `negate`).  Paths past the listed entries: length 0 and a -inf total.  `key` is
+// scratch for hsize items.
+__device__ void finish_paths(const Node* nd, const Item* heap, int hsize, Item* key, int* path_node, int T, int top_paths,
+                             int merge_repeated, int strip, int* out, int* out_len, float* score, int negate, int* num_paths) {
+  const int lane = threadIdx.x;
+  for (int i = lane; i < hsize; i += kThreads) {
+    const Item it = heap[i];
+    key[i] = Item{nd[it.node].nt, nd[it.node].leaf_seq == it.seq ? it.seq : -1, it.node};    // seq -1: a stale item
+  }
+  __syncwarp();
+  int listed = 0;
+  for (int i0 = 0; i0 < hsize; i0 += kThreads) {
+    const int i = i0 + lane;
+    const bool valid = i < hsize && key[i].seq >= 0;
+    if (valid) {
+      const Item v = key[i];
+      int r = 0;
+      for (int k = 0; k < hsize; ++k) {
+        const Item o = key[k];
+        r += o.seq >= 0 && (o.total > v.total || (o.total == v.total && o.seq < v.seq));
+      }
+      if (r < top_paths) path_node[r] = v.node;
+    }
+    listed += __popc(__ballot_sync(0xffffffffu, valid));
+  }
+  __syncwarp();
+  const int paths = min(listed, top_paths);
+  for (int p = lane; p < top_paths; p += kThreads) {
+    int* o = out + (size_t)p * T;
+    int n = 0;
+    double total = neg_inf();
+    if (p < paths) {
+      const int e0 = path_node[p];
+      total = nd[e0].nt;
+      int depth = 0;
+      for (int e = e0; nd[e].parent >= 0; e = nd[e].parent) ++depth;
+      int i = depth;
+      for (int e = e0; nd[e].parent >= 0; e = nd[e].parent) o[--i] = nd[e].label;
+      int prev = -1;
+      for (i = 0; i < depth; ++i) {
+        const int l = o[i];
+        const bool keep = !(merge_repeated && l == prev);
+        prev = l;
+        if (keep && l != strip) o[n++] = l;
+      }
+    }
+    for (int i = n; i < T; ++i) o[i] = 0;
+    out_len[p] = n;
+    if (score) score[p] = (float)(negate ? -total : total);
+  }
+  if (num_paths && lane == 0) *num_paths = paths;
+}
+
 __global__ void __launch_bounds__(kThreads) ctc_beam_kernel(const float* __restrict__ logits, const int* __restrict__ input_len,
-                                                            int T, int N, int C, int beam_width, int merge_repeated, int strip,
-                                                            int* __restrict__ out, int* __restrict__ out_len,
-                                                            float* __restrict__ neg_log_prob, Node* __restrict__ arena,
-                                                            size_t node_cap) {
+                                                            int T, int N, int C, int beam_width, int top_paths, int merge_repeated,
+                                                            int strip, int* __restrict__ out, int* __restrict__ out_len,
+                                                            float* __restrict__ score, int negate, int* __restrict__ num_paths,
+                                                            Node* __restrict__ arena, size_t node_cap) {
   __shared__ Item s_heap[kMaxWidth], s_br[kMaxWidth];
   __shared__ double s_lp[kMaxClasses], s_lp_desc[kMaxClasses], s_ex[kMaxClasses];
   __shared__ int s_by_lp[kMaxClasses];
+  __shared__ int s_path[kMaxWidth];
   __shared__ double s_norm;
   const int n = blockIdx.x, lane = threadIdx.x;
   const int nlab = C - 1;
@@ -357,7 +388,11 @@ __global__ void __launch_bounds__(kThreads) ctc_beam_kernel(const float* __restr
     if (lane == 0) D.step(s_lp, s_lp_desc, s_by_lp);
     __syncwarp();
   }
-  if (lane == 0) D.finish(T, merge_repeated, strip, out + (size_t)n * T, out_len + n, neg_log_prob ? neg_log_prob + n : nullptr);
+  __syncwarp();                                                   // lane 0's init when len == 0
+  const int hsize = __shfl_sync(0xffffffffu, lane == 0 ? D.hsize : 0, 0);
+  const size_t row = (size_t)n * top_paths;
+  finish_paths(arena + (size_t)n * node_cap, s_heap, hsize, s_br, s_path, T, top_paths, merge_repeated, strip, out + row * T,
+               out_len + row, score ? score + row : nullptr, negate, num_paths ? num_paths + n : nullptr);
 }
 
 int beam_check_shape(int T, int N, int C, int beam_width, size_t* node_cap) {
@@ -382,21 +417,42 @@ extern "C" int crnn_ctc_beam_workspace_size(int T, int N, int C, int beam_width,
   return CRNN_OK;
 }
 
-extern "C" int crnn_ctc_beam_search_device(const float* logits, const int* input_len, int T, int N, int C, int beam_width,
-                                           int merge_repeated, int strip, int* out, int* out_len, float* neg_log_prob,
-                                           void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
+namespace {
+
+// both device entry points: the argument checks and the launch
+int beam_search_device(const float* logits, const int* input_len, int T, int N, int C, int beam_width, int top_paths,
+                       int merge_repeated, int strip, int* out, int* out_len, float* score, int negate, int* num_paths,
+                       void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
   if (!logits || !input_len || !out || !out_len) return crnn_fail(CRNN_INVALID_VALUE, "beam_search_device: null pointer");
   size_t cap = 0;
   const int st = beam_check_shape(T, N, C, beam_width, &cap);
   if (st != CRNN_OK) return st;
+  if (top_paths < 1 || top_paths > beam_width)
+    return crnn_fail(CRNN_INVALID_VALUE, "beam_search_device: top_paths %d outside [1, beam_width = %d]", top_paths, beam_width);
   if (workspace_bytes < (size_t)N * cap * sizeof(Node))
     return crnn_fail(CRNN_WORKSPACE_TOO_SMALL, "beam_search_device: workspace %zu bytes, needs %zu", workspace_bytes,
                      (size_t)N * cap * sizeof(Node));
   if (!workspace || reinterpret_cast<uintptr_t>(workspace) % 16 != 0)
     return crnn_fail(CRNN_INVALID_VALUE, "beam_search_device: workspace must be a 16-byte aligned device pointer");
   ctc_beam_kernel<<<N, kThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      logits, input_len, T, N, C, beam_width, merge_repeated ? 1 : 0, strip, out, out_len, neg_log_prob,
+      logits, input_len, T, N, C, beam_width, top_paths, merge_repeated ? 1 : 0, strip, out, out_len, score, negate, num_paths,
       reinterpret_cast<Node*>(workspace), cap);
   CUDA_TRY(cudaGetLastError());
   return CRNN_OK;
+}
+
+}  // namespace
+
+extern "C" int crnn_ctc_beam_search_device(const float* logits, const int* input_len, int T, int N, int C, int beam_width,
+                                           int merge_repeated, int strip, int* out, int* out_len, float* neg_log_prob,
+                                           void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
+  return beam_search_device(logits, input_len, T, N, C, beam_width, 1, merge_repeated, strip, out, out_len, neg_log_prob, 1, nullptr,
+                            workspace, workspace_bytes, stream);
+}
+
+extern "C" int crnn_ctc_beam_search_topk_device(const float* logits, const int* input_len, int T, int N, int C, int beam_width,
+                                                int top_paths, int merge_repeated, int strip, int* out, int* out_len, float* log_prob,
+                                                int* num_paths, void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
+  return beam_search_device(logits, input_len, T, N, C, beam_width, top_paths, merge_repeated, strip, out, out_len, log_prob, 0,
+                            num_paths, workspace, workspace_bytes, stream);
 }

@@ -832,20 +832,41 @@ def ctc_greedy(logits, input_len, tf_blank=TF_BLANK, strip=0):
     return out, out_len
 
 
+def _host_beam_inputs(logits, input_len):
+    x = logits.detach().float().cpu().numpy() if torch.is_tensor(logits) else np.asarray(logits, dtype=np.float32)
+    x = np.ascontiguousarray(x)
+    il = input_len.detach().cpu().numpy() if torch.is_tensor(input_len) else np.asarray(input_len)
+    return x, np.ascontiguousarray(il, dtype=np.int32)
+
+
 def ctc_beam_search(logits, input_len, beam_width=100, merge_repeated=True, strip=0, num_threads=0):
     """The reference's decoder (network.py:656: ctc_beam_search_decoder, width 100, blank C-1, merge_repeated) on the HOST, as
     the TF op is.  logits: [T,N,C] f32 (cuda tensor -> copied back once, or numpy); returns (out [N,T] i32, out_len [N] i32,
     neg_log_prob [N] f32) as numpy arrays."""
     lib = _lib.load()
-    x = logits.detach().float().cpu().numpy() if torch.is_tensor(logits) else np.asarray(logits, dtype=np.float32)
-    x = np.ascontiguousarray(x)
-    il = input_len.detach().cpu().numpy() if torch.is_tensor(input_len) else np.asarray(input_len)
-    il = np.ascontiguousarray(il, dtype=np.int32)
+    x, il = _host_beam_inputs(logits, input_len)
     T, N, C = x.shape
     out = np.zeros((N, T), np.int32); out_len = np.zeros(N, np.int32); nlp = np.zeros(N, np.float32)
     check(lib.crnn_ctc_beam_search(x.ctypes.data, il.ctypes.data, T, N, C, int(beam_width), 1 if merge_repeated else 0, int(strip),
                                    out.ctypes.data, out_len.ctypes.data, nlp.ctypes.data, int(num_threads)))
     return out, out_len, nlp
+
+
+def ctc_beam_search_topk(logits, input_len, beam_width=100, top_paths=1, merge_repeated=True, strip=0, num_threads=0):
+    """ctc_beam_search_decoder's top_paths on the HOST: the `top_paths` best entries of ctc_beam_search's beam, by total (exact
+    ties in insertion order; path 0 is ctc_beam_search's read).  1 <= top_paths <= beam_width.  Returns numpy (out [N,K,T] i32
+    zero padded, out_len [N,K] i32, log_prob [N,K] f32 = TF's log_probability (<= 0), num_paths [N] i32); paths past
+    num_paths have length 0 and log_prob -inf.  Equal labellings from different prefixes are all returned."""
+    lib = _lib.load()
+    x, il = _host_beam_inputs(logits, input_len)
+    T, N, C = x.shape
+    K = int(top_paths)
+    out = np.zeros((N, max(K, 0), T), np.int32); out_len = np.zeros((N, max(K, 0)), np.int32)
+    lp = np.zeros((N, max(K, 0)), np.float32); npaths = np.zeros(N, np.int32)
+    check(lib.crnn_ctc_beam_search_topk(x.ctypes.data, il.ctypes.data, T, N, C, int(beam_width), K, 1 if merge_repeated else 0,
+                                        int(strip), out.ctypes.data, out_len.ctypes.data, lp.ctypes.data, npaths.ctypes.data,
+                                        int(num_threads)))
+    return out, out_len, lp, npaths
 
 
 _beam_ws = {}        # device -> ((T, N, C, beam_width), workspace tensor): the last shape's workspace, reused call to call
@@ -858,21 +879,17 @@ def beam_workspace_bytes(T, N, C, beam_width):
     return int(nbytes.value)
 
 
-def ctc_beam_search_device(logits, input_len, beam_width=100, merge_repeated=True, strip=0):
-    """The same decoder as ctc_beam_search (labellings identical to the host's), run on the GPU from device logits: one warp
-    per utterance, asynchronous on the current stream, no host sync.  logits [T,N,C] f32 cuda (2 <= C <= 64), input_len [N]
-    i32 cuda (clamped to [0, T]), 1 <= beam_width <= 128.  Returns device (out [N,T] i32 zero padded, out_len [N] i32,
-    neg_log_prob [N] f32).  There is no host fallback: CPU tensors or an unsupported shape raise CrnnError."""
+def _device_beam_inputs(name, logits, input_len, beam_width):
+    """Checked contiguous (logits, input_len) and the device's cached workspace for their shape."""
     if not (torch.is_tensor(logits) and logits.is_cuda and torch.is_tensor(input_len) and input_len.is_cuda):
-        raise CrnnError("ctc_beam_search_device needs CUDA tensors; ctc_beam_search is the host decoder")
+        raise CrnnError(f"{name} needs CUDA tensors; {name.replace('_device', '')} is the host decoder")
     if logits.dtype != torch.float32 or logits.dim() != 3 or input_len.dtype != torch.int32:
-        raise CrnnError("ctc_beam_search_device: logits must be [T,N,C] f32 and input_len i32")
-    lib = _lib.load()
+        raise CrnnError(f"{name}: logits must be [T,N,C] f32 and input_len i32")
     logits = logits.contiguous()
     input_len = input_len.contiguous()
     T, N, C = logits.shape
     if input_len.numel() != N:
-        raise CrnnError("ctc_beam_search_device: input_len must hold one entry per utterance")
+        raise CrnnError(f"{name}: input_len must hold one entry per utterance")
     key = (T, N, C, int(beam_width))
     dev = logits.device
     cached = _beam_ws.get(dev)
@@ -880,7 +897,18 @@ def ctc_beam_search_device(logits, input_len, beam_width=100, merge_repeated=Tru
         _beam_ws.pop(dev, None)
         nbytes = beam_workspace_bytes(T, N, C, beam_width)
         cached = _beam_ws[dev] = (key, torch.empty(nbytes, dtype=torch.uint8, device=dev))
-    ws = cached[1]
+    return logits, input_len, cached[1]
+
+
+def ctc_beam_search_device(logits, input_len, beam_width=100, merge_repeated=True, strip=0):
+    """The same decoder as ctc_beam_search (labellings identical to the host's), run on the GPU from device logits: one warp
+    per utterance, asynchronous on the current stream, no host sync.  logits [T,N,C] f32 cuda (2 <= C <= 64), input_len [N]
+    i32 cuda (clamped to [0, T]), 1 <= beam_width <= 128.  Returns device (out [N,T] i32 zero padded, out_len [N] i32,
+    neg_log_prob [N] f32).  There is no host fallback: CPU tensors or an unsupported shape raise CrnnError."""
+    lib = _lib.load()
+    logits, input_len, ws = _device_beam_inputs("ctc_beam_search_device", logits, input_len, beam_width)
+    T, N, C = logits.shape
+    dev = logits.device
     out = torch.empty((N, T), dtype=torch.int32, device=dev)
     out_len = torch.empty(N, dtype=torch.int32, device=dev)
     nlp = torch.empty(N, dtype=torch.float32, device=dev)
@@ -890,10 +918,42 @@ def ctc_beam_search_device(logits, input_len, beam_width=100, merge_repeated=Tru
     return out, out_len, nlp
 
 
+def ctc_beam_search_topk_device(logits, input_len, beam_width=100, top_paths=1, merge_repeated=True, strip=0):
+    """ctc_beam_search_topk on the GPU: ctc_beam_search_device's beam, inputs, workspace and stream rules, and
+    ctc_beam_search_topk's outputs (identical labels, lengths and num_paths) as device tensors (out [N,K,T], out_len [N,K],
+    log_prob [N,K], num_paths [N]).  Asynchronous, no host sync; no host fallback."""
+    lib = _lib.load()
+    logits, input_len, ws = _device_beam_inputs("ctc_beam_search_topk_device", logits, input_len, beam_width)
+    T, N, C = logits.shape
+    dev = logits.device
+    K = int(top_paths)
+    out = torch.empty((N, max(K, 0), T), dtype=torch.int32, device=dev)
+    out_len = torch.empty((N, max(K, 0)), dtype=torch.int32, device=dev)
+    lp = torch.empty((N, max(K, 0)), dtype=torch.float32, device=dev)
+    npaths = torch.empty(N, dtype=torch.int32, device=dev)
+    check(lib.crnn_ctc_beam_search_topk_device(logits.data_ptr(), input_len.data_ptr(), T, N, C, int(beam_width), K,
+                                               1 if merge_repeated else 0, int(strip), out.data_ptr(), out_len.data_ptr(),
+                                               lp.data_ptr(), npaths.data_ptr(), ws.data_ptr(), ws.numel(), _stream()))
+    return out, out_len, lp, npaths
+
+
 def dense_decoded(out, out_len):
     """sparse_tensor_to_dense(default 0) shape [N, max_len] (network.py:657); one D2H sync."""
     m = int(out_len.max().item()) if out_len.numel() else 0
     return out[:, :m].contiguous()
+
+
+def dense_decoded_topk(out, out_len):
+    """The K decodings of ctc_beam_search_topk(_device) (out [N,K,T], out_len [N,K]) as K [N, max_len] arrays, each what
+    sparse_tensor_to_dense(decoded[k], default 0) gives: max_len is that path's longest read.  numpy or torch in, the same out
+    (a torch input costs one D2H sync)."""
+    K = out.shape[1]
+    if torch.is_tensor(out_len):
+        m = out_len.max(0).values.cpu().tolist() if out_len.numel() else [0] * K
+    else:
+        m = out_len.max(0).tolist() if out_len.size else [0] * K
+    return [out[:, k, :int(m[k])].contiguous() if torch.is_tensor(out) else np.ascontiguousarray(out[:, k, :int(m[k])])
+            for k in range(K)]
 
 
 def test_gemm_tn_bf16(A, B, block_n, k_splits=0):

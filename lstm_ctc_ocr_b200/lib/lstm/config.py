@@ -69,7 +69,11 @@ _DEFAULTS = {
              # not in the reference (CRNN's lexicon-based transcription): a word-list file (one word per line) makes test_model read
              # each line as the most probable word (CTC score) among the LEXICON_CANDIDATES nearest words within edit distance
              # LEXICON_MAX_EDIT of the plain read (CRNN's delta = 3; < 0: no threshold); "" reads without a lexicon
-             "LEXICON": "", "LEXICON_MAX_EDIT": 3, "LEXICON_CANDIDATES": 64},
+             "LEXICON": "", "LEXICON_MAX_EDIT": 3, "LEXICON_CANDIDATES": 64,
+             # not in the reference (ctc_beam_search_decoder's top_paths, which it leaves at 1): K > 1 adds to each file's line of
+             # test_model the K best beam reads (width BEAM_WIDTH) with their probabilities and the log-probability margin of the
+             # first over the second (Session.run's "beam_decoded"); 1 prints what the reference prints
+             "TOP_PATHS": 1},
 }
 
 

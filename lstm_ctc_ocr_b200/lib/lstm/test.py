@@ -97,6 +97,19 @@ def decodeRes(nums, ignore=0):
     return [decode_maps[int(i)] for i in nums if i != ignore]
 
 
+def nbest_text(nbest, r):
+    """test_model's addition for line r of a "beam_decoded" fetch: ", n-best: <read> (<p>), ..." over its real paths, p =
+    exp(log_prob), then ", margin: <log P1 - log P2>" when a second path exists."""
+    k = int(nbest["num_paths"][r])
+    lp = nbest["log_prob"][r].astype(np.float64)
+    reads = ("{} ({:.4f})".format("".join(decodeRes(nbest["labels"][r, j, :nbest["len"][r, j]])), float(np.exp(lp[j])))
+             for j in range(k))
+    text = ", n-best: " + ", ".join(reads)
+    if k > 1:
+        text += ", margin: {:.4f}".format(float(lp[0] - lp[1]))
+    return text
+
+
 class SolverWrapper(object):
     def __init__(self, sess, network, imgdb, output_dir, logdir, pretrained_model=None):
         self.net = network
@@ -115,6 +128,9 @@ class SolverWrapper(object):
         lexicon = bool(cfg.TEST.get("LEXICON", ""))
         if lexicon:         # the lexicon read of each line next to its plain read
             dense_decoded = [dense_decoded, Fetch(self.net, "lexicon_decoded")]
+        top_paths = int(cfg.TEST.get("TOP_PATHS", 1))
+        if top_paths > 1:   # the n best beam reads after the read
+            dense_decoded = (dense_decoded if lexicon else [dense_decoded]) + [Fetch(self.net, "beam_decoded")]
         if restore:
             from .train import SolverWrapper as TrainSolver
             ts = TrainSolver.__new__(TrainSolver)
@@ -142,6 +158,9 @@ class SolverWrapper(object):
             feed_dict = {self.net.images: [images[i] for i in idx], self.net.keep_prob: 1.0}
             dense = sess.run(fetches=dense_decoded, feed_dict=feed_dict)
             dt = timer.toc(average=False) / len(idx)
+            if top_paths > 1:
+                *dense, nbest = dense
+                dense = dense if lexicon else dense[0]
             if lexicon:
                 dense, lex = dense
             if confidence:
@@ -157,6 +176,8 @@ class SolverWrapper(object):
                     k = int((dense[r] != 0).sum())
                     conf_of[i] = conf_of.get(i, "") + ", conf: {:.4f}, peaks: [{}]".format(float(np.exp(np.float64(al["path_logprob"][r]))),
                                                                      " ".join("{:.3f}".format(float(p)) for p in al["peak"][r, :k]))
+                if top_paths > 1:
+                    conf_of[i] = conf_of.get(i, "") + nbest_text(nbest, r)
         total = correct = 0
         for i, file in enumerate(files):
             total += 1

@@ -573,6 +573,8 @@ class Session(object):
                 v = self._label_alignment(logits, d_tsl, d_lab, d_ll, llen)
             elif k == "lexicon_decoded":
                 v = self._lexicon_decoded(logits, d_tsl)
+            elif k == "beam_decoded":
+                v = self._beam_decoded(logits, d_tsl)
             elif k == "train_op" and train is not None:
                 v = train(f)
                 self._stage_ahead()
@@ -631,6 +633,18 @@ class Session(object):
         return engine.lexicon_decode(logits, d_tsl, engine.dense_decoded(o, ol), ol, cache[key],
                                      max_edit=int(cfg.TEST.get("LEXICON_MAX_EDIT", 3)),
                                      max_candidates=int(cfg.TEST.get("LEXICON_CANDIDATES", 64)))
+
+    @staticmethod
+    def _beam_decoded(logits, d_tsl):
+        """"beam_decoded": the cfg.TEST.TOP_PATHS best reads of the beam search (width cfg.BEAM_WIDTH, on the device, whatever
+        cfg.DECODER says), engine.ctc_beam_search_topk_device: {"labels" [N,K,L] (L the longest read, zero padded), "len" [N,K],
+        "log_prob" [N,K], "num_paths" [N]}."""
+        from .lib.lstm.config import cfg
+        o, ol, lp, npaths = engine.ctc_beam_search_topk_device(logits, d_tsl, beam_width=int(cfg.get("BEAM_WIDTH", 100)),
+                                                               top_paths=int(cfg.TEST.get("TOP_PATHS", 1)), merge_repeated=True)
+        ol = ol.cpu().numpy()
+        L = int(ol.max()) if ol.size else 0
+        return {"labels": o[:, :, :L].cpu().numpy(), "len": ol, "log_prob": lp.cpu().numpy(), "num_paths": npaths.cpu().numpy()}
 
     @staticmethod
     def _label_alignment(logits, d_tsl, d_lab, d_ll, llen):

@@ -305,7 +305,8 @@ int64_t crnn_param_count(const crnn_model* m);
 int     crnn_param_info(const crnn_model* m, int index, const char** tf_name, int64_t* offset,
                         int64_t shape[4], int* ndim);
 /* Bind caller-owned flat buffers (each crnn_param_count() f32).  grads/adam_* may be NULL
- * for inference.  Marks the derived bf16 operand copies dirty. */
+ * for inference.  Marks the derived bf16 operand copies dirty.  Each non-null pointer must be 16-byte aligned (bias rows and the
+ * solver steps read them as float4): otherwise CRNN_INVALID_VALUE and the previous binding stays. */
 int     crnn_model_bind(crnn_model* m, float* params, float* grads, float* adam_m, float* adam_v);
 int     crnn_model_params_changed(crnn_model* m);   /* caller wrote params in place */
 
@@ -316,7 +317,11 @@ int     crnn_model_params_changed(crnn_model* m);   /* caller wrote params in pl
 int     crnn_model_workspace_size(const crnn_model* m, int N, int W, int train, size_t* bytes);
 
 /* data [N,W,32] f32 (width-major rows, lib/lstm/utils/gen.py:62-64), time_step_len [N] i32
- * (nw//4-1, gen.py:54) -> logits_out [T=W/4-1, N, 64] f32. */
+ * (nw//4-1, gen.py:54) -> logits_out [T=W/4-1, N, 64] f32.  workspace 1024-byte aligned.
+ * Alignment (every forward entry point, crnn_model_calibrate_fp8 and crnn_backward): the f32 `data` / `data_staging` the kernels
+ * read and `logits_out` must be 16-byte aligned (float4 loads and stores); otherwise CRNN_INVALID_VALUE, checked on the host
+ * before anything is enqueued, and the outputs are untouched.  Host pointers (host_data, pageable_data, pinned_staging) may
+ * have any alignment. */
 int     crnn_forward(crnn_model* m, const float* data, const int* time_step_len, int N, int W,
                      float* logits_out, void* workspace, size_t workspace_bytes,
                      crnn_stream_t stream);
@@ -401,7 +406,8 @@ int     crnn_model_set_fp8_scales(crnn_model* m, const float* scales_host);
  * mode's own conv4_x).  After a moving-mode forward the taps "a4a_pre", "a4b_pre", "bn" and "stats" return CRNN_INVALID_VALUE;
  * crnn_debug_tap_raw adds "moving_w_conv4_1" / "moving_w_conv4_2" (bf16 W' [512][K], K = 2304 / 4608 in (kh, kw, ci) order) and
  * "moving_bias" (f32 b' [2][512]), and on fp8 models "fp8_colscale_moving" (f32 [2][512]).  crnn_lines_workspace_size depends
- * on the mode: with moving statistics it holds no per-line statistics. */
+ * on the mode: with moving statistics it holds no per-line statistics.  `moving` must be 4-byte aligned (CRNN_INVALID_VALUE
+ * otherwise, the previous binding stays). */
 int     crnn_model_bind_bn_moving(crnn_model* m, float* moving, float decay);
 int     crnn_model_set_bn_statistics(crnn_model* m, int moving);   /* 0 = batch statistics (default, the reference), 1 = moving */
 
@@ -450,6 +456,8 @@ int     crnn_backward_u8(crnn_model* m, const uint8_t* data, const int* time_ste
  *   [data parallel: all-reduce(SUM) `grads` across ranks];  crnn_clip_adam_step (or _momentum_step / _rmsprop_step).
  * ---------------------------------------------------------------------------------------- */
 int     crnn_model_set_training(crnn_model* m, int flag);
+/* dlogits [T,N,64] f32, 16-byte aligned (read as float4); f32 data 16-byte aligned as in crnn_forward: otherwise
+ * CRNN_INVALID_VALUE and `grads` is untouched. */
 int     crnn_backward(crnn_model* m, const float* data, const int* time_step_len, const float* dlogits,
                       int N, int W, void* workspace, size_t workspace_bytes, crnn_stream_t stream);
 /* grads += weight_decay*wd_mul*w on the L2-regularised tensors (network.py:660-662); g *= grad_mul;

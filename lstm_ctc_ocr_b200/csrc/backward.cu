@@ -85,6 +85,9 @@ static gemm_tn::Params tn_conv(int N, int H, int Wd, int Cin, int Cout, float* o
 static int backward_impl(crnn_model* m, const void* data, bool u8, const int* time_step_len, const float* dlogits, int N, int W,
                          void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
   if (!m || !data || !time_step_len || !dlogits || !workspace) return crnn_fail(CRNN_INVALID_VALUE, "backward: null pointer");
+  // conv1's weight gradient loads f32 pixels as float4, the dlogits rows are read as float4
+  if (!u8) CRNN_TRY(check_aligned(data, 16, "backward", "data"));
+  CRNN_TRY(check_aligned(dlogits, 16, "backward", "dlogits"));
   if (!m->params || !m->grads) return crnn_fail(CRNN_NOT_BOUND, "backward: bind params and grads first");
   if (!m->training) return crnn_fail(CRNN_INVALID_VALUE, "backward: call crnn_model_set_training(m, 1) before the forward pass");
   Plan& pl = m->plan;
@@ -320,7 +323,7 @@ extern "C" int crnn_backward(crnn_model* m, const float* data, const int* time_s
 extern "C" int crnn_backward_u8(crnn_model* m, const uint8_t* data, const int* time_step_len, const float* dlogits, int N, int W,
                                 void* workspace, size_t workspace_bytes, crnn_stream_t stream) {
   // the uint8 kernel loads each row's pixels as 4-byte words
-  if ((reinterpret_cast<uintptr_t>(data) & 3) != 0) return crnn_fail(CRNN_INVALID_VALUE, "backward_u8: uint8 data must be 4-byte aligned");
+  CRNN_TRY(check_aligned(data, 4, "backward_u8", "uint8 data"));
   return backward_impl(m, data, true, time_step_len, dlogits, N, W, workspace, workspace_bytes, stream);
 }
 

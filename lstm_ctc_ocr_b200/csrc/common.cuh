@@ -23,6 +23,15 @@ int crnn_fail(int status, const char* fmt, ...);   // records crnn_last_error(),
     if (_s != CRNN_OK) return _s; \
   } while (0)
 
+// A caller's pointer that the kernels access in units wider than its element type (f32 rows as float4, uint8 pixels as 4-byte
+// words) must be `align`-byte aligned; a misaligned one would fault on the device and poison the caller's CUDA context, so the
+// entry points refuse it on the host before anything is enqueued.  A null pointer passes (the null checks are the callers').
+inline int check_aligned(const void* p, unsigned align, const char* fn, const char* arg) {
+  if ((reinterpret_cast<uintptr_t>(p) & (align - 1)) != 0)
+    return crnn_fail(CRNN_INVALID_VALUE, "%s: %s must be %u-byte aligned", fn, arg, align);
+  return CRNN_OK;
+}
+
 // ---- input pixels: the f32 data tensor [N, W, 32] or its uint8 twin (the crnn_*_u8 entry points).  A byte u is the pixel
 // x = (float)u / 255.0f, an IEEE round-to-nearest division (numpy's u.astype(float32) / float32(255)): the value the f32 feed
 // holds, so both feeds give conv1 the same operands.  A reciprocal multiply alone differs from that quotient on 126 of the 256

@@ -264,6 +264,11 @@ extern "C" int crnn_param_info(const crnn_model* m, int index, const char** tf_n
 }
 extern "C" int crnn_model_bind(crnn_model* m, float* params, float* grads, float* adam_m, float* adam_v) {
   if (!m || !params) return crnn_fail(CRNN_INVALID_VALUE, "model_bind: null params");
+  // bias rows, the L2 sums and every solver step read and write the four buffers as float4
+  CRNN_TRY(check_aligned(params, 16, "model_bind", "params"));
+  CRNN_TRY(check_aligned(grads, 16, "model_bind", "grads"));
+  CRNN_TRY(check_aligned(adam_m, 16, "model_bind", "adam_m"));
+  CRNN_TRY(check_aligned(adam_v, 16, "model_bind", "adam_v"));
   m->params = params; m->grads = grads; m->adam_m = adam_m; m->adam_v = adam_v;
   m->dirty = true;
   m->dirty_bwd = true;
@@ -286,6 +291,7 @@ extern "C" int crnn_model_params_changed(crnn_model* m) {
 extern "C" int crnn_model_bind_bn_moving(crnn_model* m, float* moving, float decay) {
   if (!m) return crnn_fail(CRNN_INVALID_VALUE, "bind_bn_moving: null model");
   if (!(decay >= 0.f && decay <= 1.f)) return crnn_fail(CRNN_INVALID_VALUE, "bind_bn_moving: decay %g outside [0, 1]", (double)decay);
+  CRNN_TRY(check_aligned(moving, 4, "bind_bn_moving", "moving"));
   if (m->cfg.compute_dtype == 2 || m->cfg.compute_dtype == 3)
     return crnn_fail(CRNN_UNSUPPORTED, "bind_bn_moving: moving statistics run on the bf16 and fp8 paths (compute_dtype 1, 4)");
   if (moving && !m->wblock_bnm) {
@@ -687,6 +693,9 @@ static int forward(crnn_model* m, FwdCall a, const int* time_step_len, int N, in
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const bool calib = a.calib, fp8 = m && m->cfg.compute_dtype == 4 && !calib;
   if (!m || !a.data || !time_step_len || (!logits_out && !calib) || !workspace) return crnn_fail(CRNN_INVALID_VALUE, "forward: null pointer");
+  // conv1 loads f32 pixels as float4 and the logits epilogues store float4 (the uint8 twins check their 4-byte rule first)
+  if (!a.u8) CRNN_TRY(check_aligned(a.data, 16, "forward", a.host ? "data_staging" : "data"));
+  CRNN_TRY(check_aligned(logits_out, 16, "forward", "logits_out"));
   if (!m->params) return crnn_fail(CRNN_NOT_BOUND, "forward: call crnn_model_bind first");
   const bool moving = m->bn_use_moving && !m->training;     // training forwards always normalise with batch statistics
   if (moving && !m->bn_moving)
@@ -865,10 +874,7 @@ static int forward(crnn_model* m, FwdCall a, const int* time_step_len, int N, in
 }
 
 // the uint8 kernels load each row's pixels as 4-byte words
-static int check_u8_aligned(const void* p, const char* fn) {
-  if ((reinterpret_cast<uintptr_t>(p) & 3) != 0) return crnn_fail(CRNN_INVALID_VALUE, "%s: uint8 data must be 4-byte aligned", fn);
-  return CRNN_OK;
-}
+static int check_u8_aligned(const void* p, const char* fn) { return check_aligned(p, 4, fn, "uint8 data"); }
 
 // a device-fed batch of floats or (u8) uint8 pixels
 static FwdCall device_batch(const void* data, bool u8) {

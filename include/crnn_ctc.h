@@ -175,6 +175,65 @@ int crnn_ctc_lexicon_score(const float* logits, const int* input_len, int T, int
 int crnn_resize_lines_u8(const uint8_t* src, const int64_t* src_offset, const int* src_h, const int* src_w, const int* out_w, int N,
                          int W, int max_h, uint8_t* out, crnn_stream_t stream);
 
+/* PNG files decoded to 8-bit gray on the device, byte for byte what the host reader of lib/lstm/test.py load_line_image gives:
+ *   rule 0  cv2.imread(path, 0) (OpenCV 4.13 on libpng 1.6): colour (9797 R + 19234 G + 3737 B) >> 15 at 8 bits,
+ *           ((9797 R + 19234 G + 3737 B + 16384) >> 15) >> 8 at 16 bits; 16-bit gray the high byte
+ *   rule 1  Pillow 12.2 Image.convert("L"): colour (19595 R + 38470 G + 7471 B + 0x8000) >> 16 on the high bytes; 16-bit gray
+ *           clipped to 255
+ * Under both, alpha is dropped, gray below 8 bits is scaled by 255 / (2^d - 1), palette entries go through the colour formula
+ * and 16-bit gray+alpha gives its high byte.  Every colour type, bit depth, Adam7 and DEFLATE block kind is read.
+ *
+ * The decoder is at least as strict as both readers: a file it accepts reads the same on the host.  Any irregularity, and any
+ * chunk that makes a host reader compute something else, gives the file a non-zero status and an all-zero slot:
+ *   CRNN_PNG_BAD_HEADER     no PNG signature, IHDR missing, invalid or unlike h[i] x w[i], more than 1024 rows, more than
+ *                           1 000 000 columns or 178 956 970 pixels (beyond Pillow's decompression-bomb limit)
+ *   CRNN_PNG_BAD_CHUNK      truncated chunk, bad length or type, unknown critical chunk, PLTE missing / misplaced / invalid,
+ *                           IDAT not consecutive, IEND missing or bytes after it, an ancillary chunk of the wrong size or place
+ *   CRNN_PNG_BAD_CRC        a chunk CRC (ancillary or critical)
+ *   CRNN_PNG_BAD_ZLIB       zlib header (method, window, check bits, preset dictionary), Adler-32, bytes after the stream
+ *   CRNN_PNG_BAD_DEFLATE    block type 3, a bad stored length, over-subscribed or incomplete codes, a code or distance out of
+ *                           range, a distance past the window or the output, the stream ending early
+ *   CRNN_PNG_BAD_SIZE       more or less image data than IHDR implies
+ *   CRNN_PNG_BAD_DATA       a filter type above 4, a palette index at or beyond the PLTE length
+ *   CRNN_PNG_HOST_DIFFERS   a chunk a host reader acts on: any ancillary chunk but cHRM, pHYs, tIME, sBIT, tRNS, bKGD, tEXt,
+ *                           zTXt, iTXt, gAMA, sRGB and iCCP (so acTL / APNG and eXIf orientation among them); under rule 0
+ *                           gAMA, sRGB or iCCP on a colour or palette file (libpng then gamma-corrects its gray conversion,
+ *                           palette entries included); under rule 1 a zTXt, compressed iTXt or iCCP payload above 1016 bytes
+ *                           (it may inflate past the 1 MiB Pillow refuses) or text chunks that may hold more than Pillow's
+ *                           64 MiB in all
+ *   CRNN_PNG_WORKSPACE      the file's workspace region is smaller than its plan or lies beyond `bytes`
+ *
+ * crnn_png_plan (host only) lays out the workspace: file i owns bytes [ws_offset[i], ws_offset[i+1]) of it, first its zlib
+ * stream (the IDAT payloads gathered in order; file_len[i] rounded up to 16 bytes of room) and then its inflated scanlines (a
+ * filter byte and the packed samples of every row of every non-empty Adam7 pass, in pass order; room rounded up to 16), whose
+ * rows the call unfilters in place: after a successful call each row holds its samples, its filter byte unchanged.  A file whose 13 IHDR bytes are invalid gets an empty region.  ihdr is [N][13] (bytes 16 .. 28 of each
+ * file), file_len [N], ws_offset [N + 1]; *workspace_bytes = ws_offset[N].  CRNN_INVALID_VALUE for a null pointer or N <= 0.
+ *
+ * crnn_png_decode_gray_u8: file i is file_len[i] bytes at files + file_offset[i]; its gray image, h[i] x w[i] bytes row-major,
+ * goes to out + out_offset[i] (the src / src_offset / src_h / src_w layout crnn_resize_lines_u8 reads) and its status to
+ * status[i].  ws_offset [N + 1] is crnn_png_plan's, on the device; `bytes` is the workspace's size.  One warp per file: chunk
+ * walk with warp-wide CRC-32, inflate with warp-wide copies and Adler-32, unfilter, expand, convert and the Adam7 scatter.
+ * file_offset, file_len, out_offset and ws_offset must be 8-byte aligned, h, w and status 4-byte aligned; files, out and the
+ * workspace take any alignment.  CRNN_INVALID_VALUE for a null pointer, N <= 0, rule outside {0, 1} or a misaligned pointer,
+ * and then nothing is written.  Every pointer but the host-side plan's is a device pointer; asynchronous on `stream`, no
+ * allocation, the same bits on every run. */
+enum crnn_png_status {
+  CRNN_PNG_OK = 0,
+  CRNN_PNG_BAD_HEADER = 1,
+  CRNN_PNG_BAD_CHUNK = 2,
+  CRNN_PNG_BAD_CRC = 3,
+  CRNN_PNG_BAD_ZLIB = 4,
+  CRNN_PNG_BAD_DEFLATE = 5,
+  CRNN_PNG_BAD_SIZE = 6,
+  CRNN_PNG_BAD_DATA = 7,
+  CRNN_PNG_HOST_DIFFERS = 8,
+  CRNN_PNG_WORKSPACE = 9
+};
+int crnn_png_plan(const uint8_t* ihdr, const int64_t* file_len, int N, int64_t* ws_offset, size_t* workspace_bytes);
+int crnn_png_decode_gray_u8(const uint8_t* files, const int64_t* file_offset, const int64_t* file_len, int N, const int* h,
+                            const int* w, const int64_t* out_offset, int rule, uint8_t* out, int* status, void* workspace,
+                            const int64_t* ws_offset, size_t bytes, crnn_stream_t stream);
+
 /* Training lines rendered on the device.  Replaces the host generator (lib/lstm/utils/gen.py render_line + groupBatch, the
  * reference's gen.py:31-110): a batch's random layout, its glyphs composited with Pillow's blend arithmetic into 60-row
  * canvases, and the Pillow BILINEAR resize of crnn_resize_lines_u8 into the [N, W, 32] uint8 batch groupBatch(..., uint8)

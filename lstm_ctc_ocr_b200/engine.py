@@ -1,6 +1,7 @@
 """Device-side engine behind the reference-facing API.  PyTorch tensors are used purely as
 device-memory containers and for the current CUDA stream; every kernel on this path lives in
 libcrnnctc.so (hand-written sm_90a CUDA, see csrc/)."""
+import ctypes
 from collections import OrderedDict
 
 import numpy as np
@@ -729,6 +730,79 @@ def resize_lines_u8(src, src_offset, src_h, src_w, out_w, W, max_h, out=None):
     check(_lib.load().crnn_resize_lines_u8(src.data_ptr(), src_offset.data_ptr(), src_h.data_ptr(), src_w.data_ptr(), out_w.data_ptr(),
                                            N, int(W), int(max_h), out.data_ptr(), _stream()))
     return out
+
+
+PNG_SIGNATURE = b"\x89PNG\r\n\x1a\n"
+PNG_MAX_WIDTH = 1000000       # the widest PNG crnn_png_decode_gray_u8 reads (libpng's default limit)
+PNG_STATUS = {0: "ok", 1: "bad header", 2: "bad chunk", 3: "bad CRC", 4: "bad zlib stream", 5: "bad DEFLATE data",
+              6: "wrong amount of image data", 7: "bad filter type or palette index", 8: "a chunk the host reader acts on",
+              9: "workspace too small"}
+
+
+class PngDecodeError(CrnnError):
+    """Files of an `images` feed the device decoder refused: ``entries`` their indices in the feed, ``status`` their codes."""
+
+    def __init__(self, entries, status):
+        self.entries, self.status = list(entries), list(status)
+        super().__init__("images: entries {} are PNG files the device decoder refused ({})".format(
+            self.entries, ", ".join(PNG_STATUS.get(s, str(s)) for s in self.status)))
+
+
+def png_size(data):
+    """(h, w) from a PNG file's signature and IHDR (bytes-like), or None when `data` does not start with them.  Only the fields
+    are read: the rest of the header is the device decoder's to check."""
+    b = bytes(data[:33])
+    if len(b) < 33 or b[:8] != PNG_SIGNATURE or b[8:16] != b"\x00\x00\x00\x0dIHDR":
+        return None
+    return int.from_bytes(b[20:24], "big"), int.from_bytes(b[16:20], "big")
+
+
+def png_plan(ihdr, file_len):
+    """crnn_png_plan: ihdr [N, 13] uint8 (bytes 16 .. 28 of each file), file_len [N] int64 (host arrays) -> (ws_offset [N + 1]
+    int64, workspace bytes).  File i's zlib stream and inflated scanlines lie in workspace[ws_offset[i]:ws_offset[i + 1]]."""
+    ihdr = np.ascontiguousarray(ihdr, np.uint8)
+    file_len = np.ascontiguousarray(file_len, np.int64)
+    N = file_len.size
+    if ihdr.shape != (N, 13):
+        raise CrnnError(f"png_plan: ihdr must be [{N}, 13] uint8")
+    off = np.zeros(N + 1, np.int64)
+    nbytes = _lib.c_size_t()
+    check(_lib.load().crnn_png_plan(ihdr.ctypes.data, file_len.ctypes.data, N, off.ctypes.data, ctypes.byref(nbytes)))
+    return off, int(nbytes.value)
+
+
+def decode_png_gray(files, file_offset, file_len, h, w, out_offset, ws_offset, rule, out=None, workspace=None, status=None):
+    """PNG files -> 8-bit gray lines on the device (crnn_png_decode_gray_u8), byte for byte the host reader's: rule 0
+    cv2.imread(path, 0), rule 1 Pillow's convert("L").  File i is files[file_offset[i]:][:file_len[i]]; its h[i] x w[i] image goes
+    row-major to out[out_offset[i]:], the layout resize_lines_u8 reads.  files / out uint8, file_offset / file_len / out_offset
+    [N] int64, h / w [N] int32, ws_offset [N + 1] int64 (png_plan's), all cuda.  out: None allocates sum(h * w) bytes;
+    workspace: None allocates ws_offset's last entry (read back from the device when needed: pass it to stay asynchronous);
+    status: a [N] int32 cuda tensor, or None.  Returns (out, status); a file with a non-zero status (PNG_STATUS) has an
+    all-zero slot.  No host fallback: CPU tensors raise CrnnError."""
+    ints64, ints32 = (file_offset, file_len, out_offset, ws_offset), (h, w)
+    if not all(torch.is_tensor(t) and t.is_cuda for t in (files,) + ints64 + ints32):
+        raise CrnnError("decode_png_gray needs CUDA tensors (sm_90a); there is no CPU fallback")
+    if files.dtype != torch.uint8 or any(t.dtype != torch.int64 for t in ints64) or any(t.dtype != torch.int32 for t in ints32):
+        raise CrnnError("decode_png_gray: files must be uint8, file_offset, file_len, out_offset and ws_offset int64, h and w int32")
+    N = h.numel()
+    if any(t.numel() != N for t in (file_offset, file_len, out_offset, w)) or ws_offset.numel() != N + 1:
+        raise CrnnError("decode_png_gray: one file_offset, file_len, out_offset, h and w per file and N + 1 ws_offset entries")
+    files, file_offset, file_len, out_offset, ws_offset, h, w = (t.contiguous() for t in (files,) + ints64 + ints32)
+    dev = files.device
+    if out is None:
+        out = torch.empty(max(int((h.long() * w.long()).sum().item()), 1), dtype=torch.uint8, device=dev)
+    elif not (torch.is_tensor(out) and out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous()):
+        raise CrnnError("decode_png_gray: out must be a contiguous uint8 cuda tensor")
+    if workspace is None:
+        workspace = torch.empty(max(int(ws_offset[-1].item()), 1), dtype=torch.uint8, device=dev)
+    if status is None:
+        status = torch.empty(N, dtype=torch.int32, device=dev)
+    elif not (torch.is_tensor(status) and status.is_cuda and status.dtype == torch.int32 and status.numel() == N):
+        raise CrnnError(f"decode_png_gray: status must be a [{N}] int32 cuda tensor")
+    check(_lib.load().crnn_png_decode_gray_u8(files.data_ptr(), file_offset.data_ptr(), file_len.data_ptr(), N, h.data_ptr(),
+                                              w.data_ptr(), out_offset.data_ptr(), int(rule), out.data_ptr(), status.data_ptr(),
+                                              workspace.data_ptr(), ws_offset.data_ptr(), workspace.numel(), _stream()))
+    return out, status
 
 
 class GlyphAtlas(object):

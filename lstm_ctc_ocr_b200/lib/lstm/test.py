@@ -17,20 +17,33 @@ import os
 
 import numpy as np
 
+from ... import engine
 from ...session import Session
 from .config import cfg, get_encode_decode_dict
 from .utils.timer import Timer
 
 
+def gray_rule():
+    """How a file becomes gray here: 0 when OpenCV imports (cv2.imread(path, 0), as the reference reads), 1 otherwise (Pillow's
+    convert("L")).  load_line_image reads with it, and the device PNG decoder of the `images` feed follows it, so both give the
+    same bytes."""
+    try:
+        import cv2  # noqa: F401
+        return 0
+    except Exception:
+        return 1
+
+
 def load_line_image(path):
     """uint8 gray HxW (cv2.imread(path, 0) in the reference; PIL here when cv2 is unavailable)."""
-    try:
-        import cv2
-        img = cv2.imread(path, 0)
-        if img is not None:
-            return img
-    except Exception:
-        pass
+    if gray_rule() == 0:
+        try:
+            import cv2
+            img = cv2.imread(path, 0)
+            if img is not None:
+                return img
+        except Exception:
+            pass
     from PIL import Image
     return np.asarray(Image.open(path).convert("L"), dtype=np.uint8)
 
@@ -44,6 +57,24 @@ def line_size(h, w):
     nw = w if h == cfg.IMG_HEIGHT else max(1, int(cfg.IMG_HEIGHT / h * w))
     width = max(8, int(math.ceil(nw / cfg.POOL_SCALE) * cfg.POOL_SCALE))
     return nw, width, max(nw // cfg.POOL_SCALE + cfg.OFFSET_TIME_STEP, 0)
+
+
+def _line_entry(path):
+    """A file's entry of the `images` feed: its bytes when they are a PNG of 1 .. engine.RESIZE_MAX_HEIGHT rows and 1 ..
+    engine.PNG_MAX_WIDTH columns (read once, decoded on the device), otherwise load_line_image(path)."""
+    try:
+        with open(path, "rb") as f:
+            data = f.read()
+    except OSError:
+        return load_line_image(path)
+    size = engine.png_size(data)
+    if size is not None and 1 <= size[0] <= engine.RESIZE_MAX_HEIGHT and 1 <= size[1] <= engine.PNG_MAX_WIDTH:
+        return data
+    return load_line_image(path)
+
+
+def _entry_size(entry):
+    return engine.png_size(entry) if isinstance(entry, bytes) else entry.shape
 
 
 def prepare_line(img, dtype=np.float32):
@@ -144,10 +175,11 @@ class SolverWrapper(object):
             except Exception:
                 raise Exception("Check your pretrained {:s}".format(str(path)))
         files = sorted(os.listdir(testDir))
-        # each line goes to the device at its native size and is resized there (the `images` feed), whatever cfg.FEED_DTYPE says
-        images = [load_line_image(os.path.join(testDir, f)) for f in files]
+        # each line goes to the device at its native size and is resized there (the `images` feed), whatever cfg.FEED_DTYPE says:
+        # a PNG file as its bytes, decoded on the device, any other file as load_line_image's array
+        images = [_line_entry(os.path.join(testDir, f)) for f in files]
         # batches of lines of similar padded width (stable sort: ties keep name order), so little of a batch is padding
-        widths = [line_size(im.shape[0], im.shape[1])[1] for im in images]
+        widths = [line_size(*_entry_size(im))[1] for im in images]
         order = sorted(range(len(files)), key=lambda i: widths[i])
         bs = max(1, int(cfg.TEST.BATCH_SIZE))
         timer = Timer()
@@ -156,7 +188,13 @@ class SolverWrapper(object):
             idx = order[b0:b0 + bs]
             timer.tic()
             feed_dict = {self.net.images: [images[i] for i in idx], self.net.keep_prob: 1.0}
-            dense = sess.run(fetches=dense_decoded, feed_dict=feed_dict)
+            try:
+                dense = sess.run(fetches=dense_decoded, feed_dict=feed_dict)
+            except engine.PngDecodeError as e:     # files the device refused are read on the host, and the batch runs again
+                for r in e.entries:
+                    images[idx[r]] = load_line_image(os.path.join(testDir, files[idx[r]]))
+                feed_dict[self.net.images] = [images[i] for i in idx]
+                dense = sess.run(fetches=dense_decoded, feed_dict=feed_dict)
             dt = timer.toc(average=False) / len(idx)
             if top_paths > 1:
                 *dense, nbest = dense

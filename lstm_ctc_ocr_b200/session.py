@@ -483,18 +483,27 @@ class Session(object):
 
     @staticmethod
     def _images_feed(images):
-        """The `images` feed checked on the host: a non-empty sequence of 2-D uint8 arrays of 1 .. engine.RESIZE_MAX_HEIGHT rows and
-        at least one column.  Nothing is converted: a line of another dtype is refused rather than cast."""
+        """The `images` feed checked on the host: a non-empty sequence of lines, each a 2-D uint8 array or the bytes of a PNG file,
+        of 1 .. engine.RESIZE_MAX_HEIGHT rows and at least one column (a PNG's size read from its IHDR, at most
+        engine.PNG_MAX_WIDTH columns).  Nothing is converted: a line of another dtype is refused rather than cast."""
         if isinstance(images, np.ndarray) and images.dtype != object:
-            raise ValueError("images must be a sequence of 2-D uint8 arrays (one per line), not one array")
+            raise ValueError("images must be a sequence of 2-D uint8 arrays or PNG file bytes (one per line), not one array")
         images = list(images)
         if not images:
             raise ValueError("images: no lines")
         for i, im in enumerate(images):
-            if not isinstance(im, np.ndarray) or im.ndim != 2 or im.dtype != np.uint8:
-                raise ValueError(f"images[{i}] must be a 2-D uint8 array (a gray line), got "
+            if isinstance(im, (bytes, bytearray)):
+                size = engine.png_size(im)
+                if size is None:
+                    raise ValueError(f"images[{i}] is {len(im)} bytes that do not start with a PNG signature and IHDR")
+                h, w = size
+                if w > engine.PNG_MAX_WIDTH:
+                    raise ValueError(f"images[{i}] is a PNG {w} columns wide: the device decoder reads at most {engine.PNG_MAX_WIDTH}")
+            elif not isinstance(im, np.ndarray) or im.ndim != 2 or im.dtype != np.uint8:
+                raise ValueError(f"images[{i}] must be a 2-D uint8 array (a gray line) or PNG file bytes, got "
                                  f"{getattr(im, 'dtype', type(im).__name__)} {getattr(im, 'shape', '')}")
-            h, w = im.shape
+            else:
+                h, w = im.shape
             if not 1 <= h <= engine.RESIZE_MAX_HEIGHT or w < 1:
                 raise ValueError(f"images[{i}] is {h} x {w}: lines need 1 .. {engine.RESIZE_MAX_HEIGHT} rows and at least one column")
         return images
@@ -502,16 +511,21 @@ class Session(object):
     def _run_images(self, flist, single, eng, images, labels, llen):
         """Packed evaluation of native-size lines (``images`` fed, checked by _images_feed): the raw bytes go to the device in one
         copy, crnn_resize_lines_u8 resizes and packs them into the uint8 batch that prepare_line + pack_lines build on the host, and
-        from forward_lines on the run is _run_lines'.  Evaluation fetches only."""
-        from .lib.lstm.test import line_size
+        from forward_lines on the run is _run_lines'.  Evaluation fetches only.  PNG entries travel encoded and
+        crnn_png_decode_gray_u8 decodes them in front of the resize with lib/lstm/test.py gray_rule(); a file it refuses raises
+        engine.PngDecodeError naming the entries, and the run returns nothing."""
+        from .lib.lstm.test import gray_rule, line_size
         self._check_lines([f.kind for f in flist], eng, "images")
         N = len(images)
-        src_h = np.array([im.shape[0] for im in images], np.int32)
-        src_w = np.array([im.shape[1] for im in images], np.int32)
+        png = [i for i, im in enumerate(images) if not isinstance(im, np.ndarray)]
+        hw = [engine.png_size(im) if not isinstance(im, np.ndarray) else im.shape for im in images]
+        src_h = np.array([s[0] for s in hw], np.int32)
+        src_w = np.array([s[1] for s in hw], np.int32)
         size = np.array([line_size(h, w) for h, w in zip(src_h, src_w)], np.int32).reshape(N, 3)
         out_w, lw, tsl = (np.ascontiguousarray(size[:, k]) for k in range(3))
         W = int(lw.max())
-        nbytes = src_h.astype(np.int64) * src_w
+        # what travels: the arrays' pixels and the PNG files' bytes; the decoded PNG lines follow them in the same device buffer
+        nbytes = np.array([len(im) if not isinstance(im, np.ndarray) else im.size for im in images], np.int64)
         offs = np.zeros(N, np.int64)
         np.cumsum(nbytes[:-1], out=offs[1:])
         tot = int(nbytes.sum())
@@ -520,18 +534,53 @@ class Session(object):
         pin, ev = self._pinned.staging_for("images", tot, torch.uint8)
         pn = pin.numpy()
         for im, o in zip(images, offs):
-            pn[o:o + im.size].reshape(im.shape)[...] = im
-        d_src = pin[:tot].to(self.device, non_blocking=True)
+            if isinstance(im, np.ndarray):
+                pn[o:o + im.size].reshape(im.shape)[...] = im
+            else:
+                pn[o:o + len(im)] = np.frombuffer(im, np.uint8)
+        src_offset = offs
+        if png:
+            dec = src_h[png].astype(np.int64) * src_w[png]
+            dec_off = np.zeros(len(png), np.int64)
+            np.cumsum(dec[:-1], out=dec_off[1:])
+            dec_off += tot
+            src_offset = offs.copy()
+            src_offset[png] = dec_off
+            d_src = torch.empty(tot + int(dec.sum()), dtype=torch.uint8, device=self.device)
+            d_src[:tot].copy_(pin[:tot], non_blocking=True)
+        else:
+            d_src = pin[:tot].to(self.device, non_blocking=True)
         ev.record()
-        ints = {"off": offs.view(np.int32), "h": src_h, "w": src_w, "ow": out_w, "tsl": tsl, "lw": lw}
+        ints = {"off": src_offset.view(np.int32), "h": src_h, "w": src_w, "ow": out_w, "tsl": tsl, "lw": lw}
+        if png:
+            ihdr = np.stack([np.frombuffer(images[i], np.uint8, 13, 16) for i in png])
+            ws_offset, ws_bytes = engine.png_plan(ihdr, nbytes[png])
+            ints.update({"foff": offs[png].view(np.int32), "flen": nbytes[png].view(np.int32), "doff": dec_off.view(np.int32),
+                         "ws": ws_offset.view(np.int32), "ph": src_h[png], "pw": src_w[png]})
         if labels is not None:
             ints["labels"], ints["llen"] = labels, llen
         d_ints = self._pinned.stage_ints(ints, self.device)
+        status = None
+        if png:
+            i64 = lambda k: d_ints[k].view(torch.int64)   # noqa: E731
+            _, d_status = engine.decode_png_gray(d_src, i64("foff"), i64("flen"), d_ints["ph"], d_ints["pw"], i64("doff"), i64("ws"),
+                                                 gray_rule(), out=d_src,
+                                                 workspace=torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=self.device))
+            status, sev = self._pinned.staging_for("png_status", len(png), torch.int32)
+            status[:len(png)].copy_(d_status, non_blocking=True)
+            sev.record()
         d_data = engine.resize_lines_u8(d_src, d_ints["off"].view(torch.int64), d_ints["h"], d_ints["w"], d_ints["ow"], W,
                                         int(src_h.max()))
         self.h2d_bytes = tot + sum(a.nbytes for a in ints.values())
         self.last_feed_path = "native-size lines, resized on the device"
-        return self._eval_lines(flist, single, eng, d_data, d_ints, llen)
+        out = self._eval_lines(flist, single, eng, d_data, d_ints, llen)
+        if status is not None:
+            sev.synchronize()
+            st = status[:len(png)].numpy()
+            if st.any():
+                bad = np.flatnonzero(st)
+                raise engine.PngDecodeError([png[k] for k in bad], st[bad].tolist())
+        return out
 
     def _eval_lines(self, flist, single, eng, d_data, d_ints, llen):
         """The fetches of a packed batch already on the device: d_data [N, W, 32], d_ints["lw"] / ["tsl"] (and ["labels"] /

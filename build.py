@@ -7,7 +7,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(ROOT, "lstm_ctc_ocr_b200", "csrc")
 OUT = os.path.join(ROOT, "lstm_ctc_ocr_b200", "libcrnnctc.so")
 SOURCES = ["ctc.cu", "align.cu", "lexicon.cu", "kernels.cu", "model.cu", "backward_kernels.cu", "backward.cu", "forward_x3.cu", "forward_fp8.cu", "peer.cu", "beam.cpp",
-           "beam.cu", "resize.cu", "render.cu", "png.cu"]
+           "beam.cu", "resize.cu", "render.cu", "png.cu", "jpeg.cu"]
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-I/usr/local/cuda/include"]
 

@@ -234,6 +234,73 @@ int crnn_png_decode_gray_u8(const uint8_t* files, const int64_t* file_offset, co
                             const int* w, const int64_t* out_offset, int rule, uint8_t* out, int* status, void* workspace,
                             const int64_t* ws_offset, size_t bytes, crnn_stream_t stream);
 
+/* JPEG files decoded to 8-bit gray on the device, byte for byte what the host reader of lib/lstm/test.py load_line_image gives
+ * (libjpeg-turbo 3.1, ISLOW IDCT):
+ *   rule 0  cv2.imread(path, 0) (OpenCV 4.13): libjpeg's JCS_GRAYSCALE output, the Y plane; the chroma is entropy-decoded only
+ *   rule 1  Pillow 12.2 Image.convert("L"): a 1-component file its Y plane; a colour file libjpeg-turbo's RGB decode (fancy
+ *           upsampling, jdcolor.c's table-driven YCbCr -> RGB), then (19595 R + 38470 G + 7471 B + 0x8000) >> 16
+ * Read: baseline and extended-sequential Huffman files (SOF0, SOF1), 8-bit, one scan holding every component, 1 component or 3
+ * taken as YCbCr (a JFIF APP0, an Adobe APP14 with transform 1, or neither with component ids other than 'R', 'G', 'B'),
+ * 1 .. 1024 rows, 1 .. 65535 columns, any restart interval, fill bytes, bytes after EOI (ignored).  Under rule 0 every sampling
+ * is read whose Y carries the largest factors; under rule 1 every component's factors must divide the largest by 1 or 2.
+ *
+ * The decoder is at least as strict as both readers: a file it accepts reads the same on the host.  libjpeg-turbo warns and
+ * goes on over much of what is refused here.  A refused file gets a non-zero status and an all-zero slot:
+ *   CRNN_JPEG_BAD_HEADER    no SOI, SOS before SOF, an invalid SOF (length, sampling factors, component ids, quantisation table
+ *                           index, more than 10 blocks per MCU), a size unlike h[i] x w[i] or beyond 1024 rows
+ *   CRNN_JPEG_UNSUPPORTED   progressive, lossless, hierarchical or arithmetic-coded frames, precision other than 8, 2 or 4
+ *                           components, RGB colour (Adobe transform 0, any other Adobe transform, or ids 'R', 'G', 'B'), the
+ *                           components in several scans, a second scan, DNL or a zero height
+ *   CRNN_JPEG_BAD_MARKER    a bad marker or segment length, a truncated or malformed DQT, DHT, DRI or SOS (spectral selection
+ *                           and approximation other than 0, 63, 0), a table the scan needs missing, RSTn before the scan, a
+ *                           marker after the scan other than RSTn and EOI, no EOI
+ *   CRNN_JPEG_BAD_HUFFMAN   a DHT class above 1 or index above 3, more than 256 symbols, an over-subscribed code or an all-ones
+ *                           code (libjpeg's jpeg_make_d_derived_tbl checks), a DC symbol above 15
+ *   CRNN_JPEG_BAD_DATA      an invalid code, a coefficient index past 63, a DC category above 11 or an AC category above 10, a
+ *                           segment that ends before its MCUs or holds bytes after them
+ *   CRNN_JPEG_BAD_RESTART   an RSTn out of order, missing or beyond the last interval
+ *   CRNN_JPEG_HOST_DIFFERS  rule 0: an Exif APP1 whose IFD0 orientation is not 1 or cannot be read (OpenCV turns the image), a
+ *                           colour file whose Y lacks the largest sampling factors; rule 1: a sampling ratio other than 1 or 2;
+ *                           both: a block outside the range where jidctint.c and libjpeg-turbo's SIMD IDCT (which the host
+ *                           readers run) agree -- a dequantised coefficient or first-pass output beyond +-16383, or an output sum
+ *                           outside [-512, 511], where jidctint.c's range-limit table wraps and the SIMD code saturates
+ *   CRNN_JPEG_WORKSPACE     the file's workspace region is smaller than its plan, lies beyond `bytes` or starts off a 16-byte
+ *                           boundary
+ *
+ * crnn_jpeg_plan (host only) lays out the workspace: file i owns bytes [ws_offset[i], ws_offset[i+1]) of it: a 512-byte record
+ * (what the IDCT reads: block grids, quantisation tables), the restart segment table (8 bytes per MCU, plus 8), the int16
+ * coefficients of each stored component (Y, or under rule 1 all three of a colour file; 64 per block in natural order, the block
+ * grid padded to whole MCUs, a 1-component file's grid ceil(w / 8) x ceil(h / 8)), then under rule 1 a colour file's three
+ * component planes (8 x 8 bytes per block).  Every size is a multiple of 16.  sof is [N][16]: each file's SOF payload after its
+ * length field (precision, height, width, Nf, then id, sampling factors and table index per component), zero-filled to 16
+ * bytes; a record the decoder cannot lay out gets an empty region.  file_len [N], ws_offset [N + 1]; *workspace_bytes =
+ * ws_offset[N].  CRNN_INVALID_VALUE for a null pointer, N <= 0 or rule outside {0, 1}.
+ *
+ * crnn_jpeg_decode_gray_u8: file i is file_len[i] bytes at files + file_offset[i]; its gray image, h[i] x w[i] bytes row-major,
+ * goes to out + out_offset[i] (the src / src_offset / src_h / src_w layout crnn_resize_lines_u8 reads) and its status to
+ * status[i].  ws_offset [N + 1] is crnn_jpeg_plan's for the same rule, on the device; `bytes` is the workspace's size.  Three
+ * kernels: jpeg_entropy_kernel (one warp per file: marker walk, Huffman tables, RSTn scan, one restart segment per lane),
+ * jpeg_idct_kernel (ISLOW, 8 threads per block), jpeg_finish_kernel (zero slots of refused files; rule 1 colour conversion).
+ * file_offset, file_len, out_offset and ws_offset must be 8-byte aligned, h, w and status 4-byte aligned, the workspace 16-byte
+ * aligned; files and out take any alignment.  CRNN_INVALID_VALUE for a null pointer, N <= 0, rule outside {0, 1} or a
+ * misaligned pointer, and then nothing is written.  Every pointer but the host-side plan's is a device pointer; asynchronous on
+ * `stream`, no allocation, the same bits on every run. */
+enum crnn_jpeg_status {
+  CRNN_JPEG_OK = 0,
+  CRNN_JPEG_BAD_HEADER = 1,
+  CRNN_JPEG_UNSUPPORTED = 2,
+  CRNN_JPEG_BAD_MARKER = 3,
+  CRNN_JPEG_BAD_HUFFMAN = 4,
+  CRNN_JPEG_BAD_DATA = 5,
+  CRNN_JPEG_BAD_RESTART = 6,
+  CRNN_JPEG_HOST_DIFFERS = 7,
+  CRNN_JPEG_WORKSPACE = 8
+};
+int crnn_jpeg_plan(const uint8_t* sof, const int64_t* file_len, int N, int rule, int64_t* ws_offset, size_t* workspace_bytes);
+int crnn_jpeg_decode_gray_u8(const uint8_t* files, const int64_t* file_offset, const int64_t* file_len, int N, const int* h,
+                             const int* w, const int64_t* out_offset, int rule, uint8_t* out, int* status, void* workspace,
+                             const int64_t* ws_offset, size_t bytes, crnn_stream_t stream);
+
 /* Training lines rendered on the device.  Replaces the host generator (lib/lstm/utils/gen.py render_line + groupBatch, the
  * reference's gen.py:31-110): a batch's random layout, its glyphs composited with Pillow's blend arithmetic into 60-row
  * canvases, and the Pillow BILINEAR resize of crnn_resize_lines_u8 into the [N, W, 32] uint8 batch groupBatch(..., uint8)

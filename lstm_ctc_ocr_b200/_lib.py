@@ -34,6 +34,9 @@ SIGNATURES = {
     "crnn_png_plan": (c_int, [c_void_p, c_void_p, c_int, c_void_p, ctypes.POINTER(c_size_t)]),
     "crnn_png_decode_gray_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                         c_void_p, c_void_p, c_size_t, c_void_p]),
+    "crnn_jpeg_plan": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, ctypes.POINTER(c_size_t)]),
+    "crnn_jpeg_decode_gray_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
+                                         c_void_p, c_void_p, c_size_t, c_void_p]),
     "crnn_render_layout": (c_int, [c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "crnn_render_workspace_size": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
     "crnn_render_lines_u8": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p, c_void_p]),

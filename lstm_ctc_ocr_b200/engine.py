@@ -739,13 +739,44 @@ PNG_STATUS = {0: "ok", 1: "bad header", 2: "bad chunk", 3: "bad CRC", 4: "bad zl
               9: "workspace too small"}
 
 
-class PngDecodeError(CrnnError):
-    """Files of an `images` feed the device decoder refused: ``entries`` their indices in the feed, ``status`` their codes."""
+class ImageDecodeError(CrnnError):
+    """Encoded files of an `images` feed the device decoders refused: ``entries`` their indices in the feed, ``status`` their codes
+    (PNG_STATUS for a PNG entry, JPEG_STATUS for a JPEG one).  Raised as such when both kinds were refused in one feed."""
+
+    def __init__(self, entries, status, message=None):
+        self.entries, self.status = list(entries), list(status)
+        super().__init__(message or "images: entries {} are files the device decoders refused (status {})".format(
+            self.entries, self.status))
+
+
+    @classmethod
+    def mixed(cls, refused):
+        """The error for refused files of both kinds: refused [(entry, code, kind)], kind "PNG" or "JPEG"; entries in feed order."""
+        refused = sorted(refused)
+        names = {"PNG": PNG_STATUS, "JPEG": JPEG_STATUS}
+        entries = [e for e, _, _ in refused]
+        return cls(entries, [c for _, c, _ in refused], "images: entries {} are files the device decoders refused ({})".format(
+            entries, ", ".join("{} {}".format(k, names[k].get(c, str(c))) for _, c, k in refused)))
+
+
+class PngDecodeError(ImageDecodeError):
+    """Files of an `images` feed the device decoder refused, all of them PNG: ``entries`` their indices in the feed, ``status``
+    their codes."""
 
     def __init__(self, entries, status):
-        self.entries, self.status = list(entries), list(status)
-        super().__init__("images: entries {} are PNG files the device decoder refused ({})".format(
-            self.entries, ", ".join(PNG_STATUS.get(s, str(s)) for s in self.status)))
+        entries, status = list(entries), list(status)
+        super().__init__(entries, status, "images: entries {} are PNG files the device decoder refused ({})".format(
+            entries, ", ".join(PNG_STATUS.get(s, str(s)) for s in status)))
+
+
+class JpegDecodeError(ImageDecodeError):
+    """Files of an `images` feed the device decoder refused, all of them JPEG: ``entries`` their indices in the feed, ``status``
+    their codes (JPEG_STATUS)."""
+
+    def __init__(self, entries, status):
+        entries, status = list(entries), list(status)
+        super().__init__(entries, status, "images: entries {} are JPEG files the device decoder refused ({})".format(
+            entries, ", ".join(JPEG_STATUS.get(s, str(s)) for s in status)))
 
 
 def png_size(data):
@@ -779,30 +810,112 @@ def decode_png_gray(files, file_offset, file_len, h, w, out_offset, ws_offset, r
     workspace: None allocates ws_offset's last entry (read back from the device when needed: pass it to stay asynchronous);
     status: a [N] int32 cuda tensor, or None.  Returns (out, status); a file with a non-zero status (PNG_STATUS) has an
     all-zero slot.  No host fallback: CPU tensors raise CrnnError."""
+    return _decode_gray("decode_png_gray", "crnn_png_decode_gray_u8", files, file_offset, file_len, h, w, out_offset, ws_offset,
+                        rule, out, workspace, status)
+
+
+def _decode_gray(name, entry, files, file_offset, file_len, h, w, out_offset, ws_offset, rule, out, workspace, status):
     ints64, ints32 = (file_offset, file_len, out_offset, ws_offset), (h, w)
     if not all(torch.is_tensor(t) and t.is_cuda for t in (files,) + ints64 + ints32):
-        raise CrnnError("decode_png_gray needs CUDA tensors (sm_90a); there is no CPU fallback")
+        raise CrnnError(f"{name} needs CUDA tensors (sm_90a); there is no CPU fallback")
     if files.dtype != torch.uint8 or any(t.dtype != torch.int64 for t in ints64) or any(t.dtype != torch.int32 for t in ints32):
-        raise CrnnError("decode_png_gray: files must be uint8, file_offset, file_len, out_offset and ws_offset int64, h and w int32")
+        raise CrnnError(f"{name}: files must be uint8, file_offset, file_len, out_offset and ws_offset int64, h and w int32")
     N = h.numel()
     if any(t.numel() != N for t in (file_offset, file_len, out_offset, w)) or ws_offset.numel() != N + 1:
-        raise CrnnError("decode_png_gray: one file_offset, file_len, out_offset, h and w per file and N + 1 ws_offset entries")
+        raise CrnnError(f"{name}: one file_offset, file_len, out_offset, h and w per file and N + 1 ws_offset entries")
     files, file_offset, file_len, out_offset, ws_offset, h, w = (t.contiguous() for t in (files,) + ints64 + ints32)
     dev = files.device
     if out is None:
         out = torch.empty(max(int((h.long() * w.long()).sum().item()), 1), dtype=torch.uint8, device=dev)
     elif not (torch.is_tensor(out) and out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous()):
-        raise CrnnError("decode_png_gray: out must be a contiguous uint8 cuda tensor")
+        raise CrnnError(f"{name}: out must be a contiguous uint8 cuda tensor")
     if workspace is None:
         workspace = torch.empty(max(int(ws_offset[-1].item()), 1), dtype=torch.uint8, device=dev)
     if status is None:
         status = torch.empty(N, dtype=torch.int32, device=dev)
     elif not (torch.is_tensor(status) and status.is_cuda and status.dtype == torch.int32 and status.numel() == N):
-        raise CrnnError(f"decode_png_gray: status must be a [{N}] int32 cuda tensor")
-    check(_lib.load().crnn_png_decode_gray_u8(files.data_ptr(), file_offset.data_ptr(), file_len.data_ptr(), N, h.data_ptr(),
-                                              w.data_ptr(), out_offset.data_ptr(), int(rule), out.data_ptr(), status.data_ptr(),
-                                              workspace.data_ptr(), ws_offset.data_ptr(), workspace.numel(), _stream()))
+        raise CrnnError(f"{name}: status must be a [{N}] int32 cuda tensor")
+    check(getattr(_lib.load(), entry)(files.data_ptr(), file_offset.data_ptr(), file_len.data_ptr(), N, h.data_ptr(), w.data_ptr(),
+                                      out_offset.data_ptr(), int(rule), out.data_ptr(), status.data_ptr(), workspace.data_ptr(),
+                                      ws_offset.data_ptr(), workspace.numel(), _stream()))
     return out, status
+
+
+JPEG_STATUS = {0: "ok", 1: "bad header", 2: "unsupported JPEG process", 3: "bad marker segment", 4: "bad Huffman table",
+               5: "bad entropy-coded data", 6: "bad restart marker", 7: "the host reader computes something else",
+               8: "workspace too small"}
+_JPEG_SOF = set(range(0xC0, 0xD0)) - {0xC4, 0xC8, 0xCC}
+
+
+def jpeg_sof(data):
+    """(marker, payload) of a JPEG file's first SOFn segment -- the marker code (0xC0 baseline, 0xC1 extended sequential, ...)
+    and the segment's bytes after its length field -- found by walking the marker segments from SOI (only their headers are read,
+    however long the segments before the frame); None when `data` is not such a prefix (a bad marker or segment length, or SOS /
+    EOI before any SOF)."""
+    b = memoryview(data).cast("B")
+    n = len(b)
+    if n < 2 or b[0] != 0xFF or b[1] != 0xD8:
+        return None
+    pos = 2
+    while True:
+        if pos >= n or b[pos] != 0xFF:
+            return None
+        while pos < n and b[pos] == 0xFF:
+            pos += 1
+        if pos + 3 > n:
+            return None
+        m = b[pos]
+        if m == 0x00 or m == 0x01 or 0xD0 <= m <= 0xDA:        # no segment here, or the scan / EOI before a frame
+            return None
+        length = (b[pos + 1] << 8) | b[pos + 2]
+        if length < 2 or pos + 1 + length > n:
+            return None
+        if m in _JPEG_SOF:
+            payload = bytes(b[pos + 3:pos + 1 + length])
+            return (m, payload) if len(payload) >= 6 else None
+        pos += 1 + length
+
+
+def jpeg_size(data):
+    """(h, w) from a JPEG file's first SOFn segment (bytes-like), or None when `data` does not walk from SOI to one (jpeg_sof).
+    Only the size is read: the rest of the file is the device decoder's to check."""
+    sof = jpeg_sof(data)
+    return None if sof is None else (int.from_bytes(sof[1][1:3], "big"), int.from_bytes(sof[1][3:5], "big"))
+
+
+def jpeg_plan(sof, file_len, rule):
+    """crnn_jpeg_plan: sof [N, 16] uint8 (each file's SOF payload after its length field, zero-filled to 16 bytes), file_len [N]
+    int64 (host arrays), rule 0 / 1 -> (ws_offset [N + 1] int64, workspace bytes).  File i's record, restart segment table,
+    coefficients and (rule 1, colour) planes lie in workspace[ws_offset[i]:ws_offset[i + 1]]."""
+    sof = np.ascontiguousarray(sof, np.uint8)
+    file_len = np.ascontiguousarray(file_len, np.int64)
+    N = file_len.size
+    if sof.shape != (N, 16):
+        raise CrnnError(f"jpeg_plan: sof must be [{N}, 16] uint8")
+    off = np.zeros(N + 1, np.int64)
+    nbytes = _lib.c_size_t()
+    check(_lib.load().crnn_jpeg_plan(sof.ctypes.data, file_len.ctypes.data, N, int(rule), off.ctypes.data, ctypes.byref(nbytes)))
+    return off, int(nbytes.value)
+
+
+def jpeg_sof_records(files):
+    """[N, 16] uint8: each file's SOF payload zero-filled to 16 bytes, the `sof` of jpeg_plan (zeros where jpeg_sof finds none)."""
+    rec = np.zeros((len(files), 16), np.uint8)
+    for i, f in enumerate(files):
+        sof = jpeg_sof(f)
+        if sof is not None:
+            p = sof[1][:16]
+            rec[i, :len(p)] = np.frombuffer(p, np.uint8)
+    return rec
+
+
+def decode_jpeg_gray(files, file_offset, file_len, h, w, out_offset, ws_offset, rule, out=None, workspace=None, status=None):
+    """JPEG files -> 8-bit gray lines on the device (crnn_jpeg_decode_gray_u8), byte for byte the host reader's: rule 0
+    cv2.imread(path, 0), rule 1 Pillow's convert("L").  The arguments are decode_png_gray's; ws_offset is jpeg_plan's for the
+    same rule and the workspace must be 16-byte aligned.  Returns (out, status); a file with a non-zero status (JPEG_STATUS) has
+    an all-zero slot.  No host fallback: CPU tensors raise CrnnError."""
+    return _decode_gray("decode_jpeg_gray", "crnn_jpeg_decode_gray_u8", files, file_offset, file_len, h, w, out_offset, ws_offset,
+                        rule, out, workspace, status)
 
 
 class GlyphAtlas(object):

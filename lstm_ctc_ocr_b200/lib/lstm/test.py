@@ -61,7 +61,8 @@ def line_size(h, w):
 
 def _line_entry(path):
     """A file's entry of the `images` feed: its bytes when they are a PNG of 1 .. engine.RESIZE_MAX_HEIGHT rows and 1 ..
-    engine.PNG_MAX_WIDTH columns (read once, decoded on the device), otherwise load_line_image(path)."""
+    engine.PNG_MAX_WIDTH columns, or a baseline or extended-sequential JPEG (SOF0 / SOF1) of 1 .. engine.RESIZE_MAX_HEIGHT rows
+    (read once, decoded on the device), otherwise load_line_image(path)."""
     try:
         with open(path, "rb") as f:
             data = f.read()
@@ -70,11 +71,16 @@ def _line_entry(path):
     size = engine.png_size(data)
     if size is not None and 1 <= size[0] <= engine.RESIZE_MAX_HEIGHT and 1 <= size[1] <= engine.PNG_MAX_WIDTH:
         return data
+    sof = engine.jpeg_sof(data) if size is None else None
+    if sof is not None and sof[0] in (0xC0, 0xC1):     # progressive and the other processes are read on the host
+        h, w = engine.jpeg_size(data)
+        if 1 <= h <= engine.RESIZE_MAX_HEIGHT and w >= 1:
+            return data
     return load_line_image(path)
 
 
 def _entry_size(entry):
-    return engine.png_size(entry) if isinstance(entry, bytes) else entry.shape
+    return (engine.png_size(entry) or engine.jpeg_size(entry)) if isinstance(entry, bytes) else entry.shape
 
 
 def prepare_line(img, dtype=np.float32):
@@ -176,7 +182,7 @@ class SolverWrapper(object):
                 raise Exception("Check your pretrained {:s}".format(str(path)))
         files = sorted(os.listdir(testDir))
         # each line goes to the device at its native size and is resized there (the `images` feed), whatever cfg.FEED_DTYPE says:
-        # a PNG file as its bytes, decoded on the device, any other file as load_line_image's array
+        # a PNG or JPEG file as its bytes, decoded on the device, any other file as load_line_image's array
         images = [_line_entry(os.path.join(testDir, f)) for f in files]
         # batches of lines of similar padded width (stable sort: ties keep name order), so little of a batch is padding
         widths = [line_size(*_entry_size(im))[1] for im in images]
@@ -190,7 +196,7 @@ class SolverWrapper(object):
             feed_dict = {self.net.images: [images[i] for i in idx], self.net.keep_prob: 1.0}
             try:
                 dense = sess.run(fetches=dense_decoded, feed_dict=feed_dict)
-            except engine.PngDecodeError as e:     # files the device refused are read on the host, and the batch runs again
+            except engine.ImageDecodeError as e:   # files the device refused are read on the host, and the batch runs again
                 for r in e.entries:
                     images[idx[r]] = load_line_image(os.path.join(testDir, files[idx[r]]))
                 feed_dict[self.net.images] = [images[i] for i in idx]

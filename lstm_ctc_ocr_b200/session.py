@@ -483,11 +483,12 @@ class Session(object):
 
     @staticmethod
     def _images_feed(images):
-        """The `images` feed checked on the host: a non-empty sequence of lines, each a 2-D uint8 array or the bytes of a PNG file,
-        of 1 .. engine.RESIZE_MAX_HEIGHT rows and at least one column (a PNG's size read from its IHDR, at most
-        engine.PNG_MAX_WIDTH columns).  Nothing is converted: a line of another dtype is refused rather than cast."""
+        """The `images` feed checked on the host: a non-empty sequence of lines, each a 2-D uint8 array or the bytes of a PNG or JPEG
+        file, of 1 .. engine.RESIZE_MAX_HEIGHT rows and at least one column (a PNG's size read from its IHDR, at most
+        engine.PNG_MAX_WIDTH columns; a JPEG's from its first SOF segment).  Nothing is converted: a line of another dtype is refused
+        rather than cast."""
         if isinstance(images, np.ndarray) and images.dtype != object:
-            raise ValueError("images must be a sequence of 2-D uint8 arrays or PNG file bytes (one per line), not one array")
+            raise ValueError("images must be a sequence of 2-D uint8 arrays or PNG / JPEG file bytes (one per line), not one array")
         images = list(images)
         if not images:
             raise ValueError("images: no lines")
@@ -495,12 +496,15 @@ class Session(object):
             if isinstance(im, (bytes, bytearray)):
                 size = engine.png_size(im)
                 if size is None:
-                    raise ValueError(f"images[{i}] is {len(im)} bytes that do not start with a PNG signature and IHDR")
+                    size = engine.jpeg_size(im)
+                    if size is None:
+                        raise ValueError(f"images[{i}] is {len(im)} bytes that start with neither a PNG signature and IHDR nor "
+                                         "JPEG marker segments up to an SOF")
+                elif size[1] > engine.PNG_MAX_WIDTH:
+                    raise ValueError(f"images[{i}] is a PNG {size[1]} columns wide: the device decoder reads at most {engine.PNG_MAX_WIDTH}")
                 h, w = size
-                if w > engine.PNG_MAX_WIDTH:
-                    raise ValueError(f"images[{i}] is a PNG {w} columns wide: the device decoder reads at most {engine.PNG_MAX_WIDTH}")
             elif not isinstance(im, np.ndarray) or im.ndim != 2 or im.dtype != np.uint8:
-                raise ValueError(f"images[{i}] must be a 2-D uint8 array (a gray line) or PNG file bytes, got "
+                raise ValueError(f"images[{i}] must be a 2-D uint8 array (a gray line) or PNG / JPEG file bytes, got "
                                  f"{getattr(im, 'dtype', type(im).__name__)} {getattr(im, 'shape', '')}")
             else:
                 h, w = im.shape
@@ -511,20 +515,23 @@ class Session(object):
     def _run_images(self, flist, single, eng, images, labels, llen):
         """Packed evaluation of native-size lines (``images`` fed, checked by _images_feed): the raw bytes go to the device in one
         copy, crnn_resize_lines_u8 resizes and packs them into the uint8 batch that prepare_line + pack_lines build on the host, and
-        from forward_lines on the run is _run_lines'.  Evaluation fetches only.  PNG entries travel encoded and
-        crnn_png_decode_gray_u8 decodes them in front of the resize with lib/lstm/test.py gray_rule(); a file it refuses raises
-        engine.PngDecodeError naming the entries, and the run returns nothing."""
+        from forward_lines on the run is _run_lines'.  Evaluation fetches only.  PNG and JPEG entries travel encoded, and
+        crnn_png_decode_gray_u8 / crnn_jpeg_decode_gray_u8 decode them in front of the resize with lib/lstm/test.py gray_rule().
+        Files they refuse raise engine.PngDecodeError (PNG entries only), engine.JpegDecodeError (JPEG entries only) or
+        engine.ImageDecodeError (both) naming the entries, and the run returns nothing."""
         from .lib.lstm.test import gray_rule, line_size
         self._check_lines([f.kind for f in flist], eng, "images")
         N = len(images)
-        png = [i for i, im in enumerate(images) if not isinstance(im, np.ndarray)]
-        hw = [engine.png_size(im) if not isinstance(im, np.ndarray) else im.shape for im in images]
+        coded = [i for i, im in enumerate(images) if not isinstance(im, np.ndarray)]
+        png = [i for i in coded if engine.png_size(images[i]) is not None]
+        jpeg = [i for i in coded if i not in set(png)]
+        hw = [im.shape if isinstance(im, np.ndarray) else engine.png_size(im) or engine.jpeg_size(im) for im in images]
         src_h = np.array([s[0] for s in hw], np.int32)
         src_w = np.array([s[1] for s in hw], np.int32)
         size = np.array([line_size(h, w) for h, w in zip(src_h, src_w)], np.int32).reshape(N, 3)
         out_w, lw, tsl = (np.ascontiguousarray(size[:, k]) for k in range(3))
         W = int(lw.max())
-        # what travels: the arrays' pixels and the PNG files' bytes; the decoded PNG lines follow them in the same device buffer
+        # what travels: the arrays' pixels and the files' bytes; the decoded lines follow them in the same device buffer
         nbytes = np.array([len(im) if not isinstance(im, np.ndarray) else im.size for im in images], np.int64)
         offs = np.zeros(N, np.int64)
         np.cumsum(nbytes[:-1], out=offs[1:])
@@ -539,47 +546,69 @@ class Session(object):
             else:
                 pn[o:o + len(im)] = np.frombuffer(im, np.uint8)
         src_offset = offs
-        if png:
-            dec = src_h[png].astype(np.int64) * src_w[png]
-            dec_off = np.zeros(len(png), np.int64)
+        if coded:
+            dec = src_h[coded].astype(np.int64) * src_w[coded]
+            dec_off = np.zeros(len(coded), np.int64)
             np.cumsum(dec[:-1], out=dec_off[1:])
             dec_off += tot
             src_offset = offs.copy()
-            src_offset[png] = dec_off
+            src_offset[coded] = dec_off
             d_src = torch.empty(tot + int(dec.sum()), dtype=torch.uint8, device=self.device)
             d_src[:tot].copy_(pin[:tot], non_blocking=True)
         else:
             d_src = pin[:tot].to(self.device, non_blocking=True)
         ev.record()
         ints = {"off": src_offset.view(np.int32), "h": src_h, "w": src_w, "ow": out_w, "tsl": tsl, "lw": lw}
+        rule = gray_rule()
         if png:
             ihdr = np.stack([np.frombuffer(images[i], np.uint8, 13, 16) for i in png])
             ws_offset, ws_bytes = engine.png_plan(ihdr, nbytes[png])
-            ints.update({"foff": offs[png].view(np.int32), "flen": nbytes[png].view(np.int32), "doff": dec_off.view(np.int32),
+            ints.update({"foff": offs[png].view(np.int32), "flen": nbytes[png].view(np.int32), "doff": src_offset[png].view(np.int32),
                          "ws": ws_offset.view(np.int32), "ph": src_h[png], "pw": src_w[png]})
+        if jpeg:
+            jws_offset, jws_bytes = engine.jpeg_plan(engine.jpeg_sof_records([images[i] for i in jpeg]), nbytes[jpeg], rule)
+            ints.update({"jfoff": offs[jpeg].view(np.int32), "jflen": nbytes[jpeg].view(np.int32),
+                         "jdoff": src_offset[jpeg].view(np.int32), "jws": jws_offset.view(np.int32), "jh": src_h[jpeg],
+                         "jw": src_w[jpeg]})
         if labels is not None:
             ints["labels"], ints["llen"] = labels, llen
         d_ints = self._pinned.stage_ints(ints, self.device)
-        status = None
+        i64 = lambda k: d_ints[k].view(torch.int64)   # noqa: E731
+        statuses = []                                  # (feed entries, pinned status, event, error class)
         if png:
-            i64 = lambda k: d_ints[k].view(torch.int64)   # noqa: E731
             _, d_status = engine.decode_png_gray(d_src, i64("foff"), i64("flen"), d_ints["ph"], d_ints["pw"], i64("doff"), i64("ws"),
-                                                 gray_rule(), out=d_src,
+                                                 rule, out=d_src,
                                                  workspace=torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=self.device))
             status, sev = self._pinned.staging_for("png_status", len(png), torch.int32)
             status[:len(png)].copy_(d_status, non_blocking=True)
             sev.record()
+            statuses.append((png, status, sev, engine.PngDecodeError))
+        if jpeg:
+            _, d_status = engine.decode_jpeg_gray(d_src, i64("jfoff"), i64("jflen"), d_ints["jh"], d_ints["jw"], i64("jdoff"),
+                                                  i64("jws"), rule, out=d_src,
+                                                  workspace=torch.empty(max(jws_bytes, 1), dtype=torch.uint8, device=self.device))
+            status, sev = self._pinned.staging_for("jpeg_status", len(jpeg), torch.int32)
+            status[:len(jpeg)].copy_(d_status, non_blocking=True)
+            sev.record()
+            statuses.append((jpeg, status, sev, engine.JpegDecodeError))
         d_data = engine.resize_lines_u8(d_src, d_ints["off"].view(torch.int64), d_ints["h"], d_ints["w"], d_ints["ow"], W,
                                         int(src_h.max()))
         self.h2d_bytes = tot + sum(a.nbytes for a in ints.values())
         self.last_feed_path = "native-size lines, resized on the device"
         out = self._eval_lines(flist, single, eng, d_data, d_ints, llen)
-        if status is not None:
+        refused = []                                   # (error class, entries, codes) per codec with refused files
+        for entries, status, sev, err in statuses:
             sev.synchronize()
-            st = status[:len(png)].numpy()
-            if st.any():
-                bad = np.flatnonzero(st)
-                raise engine.PngDecodeError([png[k] for k in bad], st[bad].tolist())
+            st = status[:len(entries)].numpy()
+            bad = np.flatnonzero(st)
+            if bad.size:
+                refused.append((err, [entries[k] for k in bad], st[bad].tolist()))
+        if len(refused) == 1:
+            err, entries, codes = refused[0]
+            raise err(entries, codes)
+        if refused:
+            raise engine.ImageDecodeError.mixed([(e, c, "PNG" if err is engine.PngDecodeError else "JPEG")
+                                                 for err, es, cs in refused for e, c in zip(es, cs)])
         return out
 
     def _eval_lines(self, flist, single, eng, d_data, d_ints, llen):
